@@ -1,8 +1,9 @@
 #!/usr/bin/env python
-"""Benchmark of the TrajNet++ hot path on B200 (driver contract: see the task statement).
+"""Benchmark of the TrajNet++ hot path on one or more H100 GPUs.
 
     python bench.py --gpus N --steps K --warmup W            # CUDA arm
-    python bench.py --impl reference --gpus N --steps K --warmup W   # CPU arm: the unmodified reference (baseline/_ref)
+    python bench.py --impl reference --gpus N --steps K --warmup W   # CPU arm: the unmodified reference (oracle/_ref)
+    python bench.py ... --dump-outputs DIR    # also write the last timed step's outputs as DIR/<name>.npy
 
 A "step" is one pass of the hot path over one batch of synthetic scenes: one call of
 LSTM.forward = (obs-1) + (pred-1) = 19 recurrence steps for every track of the batch.
@@ -35,10 +36,6 @@ STATE_BYTES_PER_PED_STEP = 2092                   # SURVEY.md 8d: xy 16 + h,c in
 DENSE_FLOP_PER_PED_STEP = {                       # SURVEY.md 8d, dense-equivalent forward FLOPs
     "sparse_layer1": 2 * 4096 * 1024,             # first Linear of the grid embedding (4096 -> 1024)
     "sparse_layer1_mma": 2 * 4096 * 1024,
-    "sparse_layer1_tc": 2 * 4096 * 1024,
-    "sparse_layer1_pair": 2 * 4096 * 1024,
-    "sparse_layer1_pair_ts": 2 * 4096 * 1024,
-    "sparse_layer1_solo": 2 * 4096 * 1024,
     "dense_layer": 2 * 1024 * 256,
     "dense_layer_tc": 2 * 1024 * 256,
     "lstm_gates": 2 * (64 + 256 + 128) * 512 + 2 * 128 * 5,
@@ -51,7 +48,7 @@ def peaks():
     if os.path.exists(path):
         d = json.load(open(path))
         return d["hbm_gbs"], d["bf16_tflops"], d.get("bf16_tflops_sustained", d["bf16_tflops"]), "measured"
-    return 6650.0, 1590.0, 1400.0, "fallback"
+    return 3350.0, 989.0, 989.0, "H100 SXM data sheet (dense bf16)"
 
 
 class ClockSampler(threading.Thread):
@@ -132,7 +129,7 @@ def cpu_oracle_run(scenes):
 
 
 class ReferenceCpu:
-    """The UNMODIFIED reference (baseline/_ref, see baseline/install_ref.sh) on the host cores: its own
+    """The UNMODIFIED reference (oracle/_ref, see oracle/build_ref.py) on the host cores: its own
     `trajnetbaselines.lstm.LSTM` + `GridBasedPooling`, torch CPU, same seeded weights and synthetic scenes as the
     CUDA arm, `LSTM.forward(observed, goals, batch_split, n_predict=12)` under torch.no_grad()."""
 
@@ -185,7 +182,7 @@ def run_reference(args):
     try:
         ref = ReferenceCpu()
         kind = "reference"
-    except Exception as exc:                      # no baseline/_ref on this box: the numpy restatement, labelled as such
+    except Exception as exc:                      # reference not importable: the numpy restatement, labelled as such
         ref, kind = None, "port"
         note = "reference install not importable (%s: %s); numpy fp32 oracle port instead" % (type(exc).__name__, exc)
     cores = os.cpu_count()
@@ -228,7 +225,7 @@ def run_reference(args):
     print(json.dumps(line))
 
 
-def train_record(torch, dist, device, world, rank, steps=10, warmup=3):
+def train_record(torch, dist, device, world, rank, steps, warmup=3):
     """BASELINE configs[3] under the same launch: D-LSTM `Trainer.train_batch` work (teacher-forced forward,
     PredictionLoss x batch, CUDA BPTT, Adam) on 256 scenes per GPU, plus ONE flat-bucket all-reduce of the
     gradients per step when world > 1.  Device-timed, max over ranks (reference lstm/trainer.py:229-269)."""
@@ -305,6 +302,8 @@ def main():
     ap.add_argument("--scenes", type=int, default=SCENES_PER_GPU, help="scenes per GPU")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-train", action="store_true", help="skip the D-LSTM training sub-record")
+    ap.add_argument("--dump-outputs", metavar="DIR",
+                    help="write the (rel, pred) arrays of the last timed inference step as DIR/<name>.npy (float32)")
     args = ap.parse_args()
     if args.impl == "reference":
         return run_reference(args)
@@ -343,7 +342,7 @@ def main():
     observed_dev = observed_host.to(device)
     goals = torch.zeros(M, 2)
     bs_t = torch.from_numpy(bs)
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=device)     # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=device)     # > 50 MB L2
 
     def step_resident():
         with torch.no_grad():
@@ -365,16 +364,31 @@ def main():
     stops = [torch.cuda.Event(enable_timing=True) for _ in range(args.steps)]
     barrier()
     t_wall0 = time.perf_counter()
+    last = None
     for i in range(args.steps):
         flush.zero_()                       # L2 flush between timed iterations (untimed)
         starts[i].record()
-        step_resident()
+        last = step_resident()
         stops[i].record()
     barrier()
     t_wall = time.perf_counter() - t_wall0
     launches = int(lib.tb2_launch_count()) - launches0
     ms = sum(s.elapsed_time(e) for s, e in zip(starts, stops))
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        # inputs and weights are seeded, so two builds can be compared output for output (5120 tracks: ~2.7 MB).
+        # Above 64 MB in all, a fixed seeded sample of tracks (axis 1) is written, with its indices as track_index.npy.
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        arrs = {name: arr.detach().cpu().numpy().astype(np.float32) for name, arr in zip(("rel", "pred"), last)}
+        per_track = sum(a.nbytes // a.shape[1] for a in arrs.values())
+        if per_track * M > (64 << 20):
+            keep = (64 << 20) // (per_track + 8)          # + 8 bytes per track for its float64 index
+            idx = np.sort(np.random.RandomState(0).choice(M, keep, replace=False))
+            arrs = {name: np.ascontiguousarray(a[:, idx]) for name, a in arrs.items()}
+            arrs["track_index"] = idx.astype(np.float64)
+        for name, a in arrs.items():
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), a)
+    last = None
 
     # ---- end-to-end arm (host buffers, copies inside the timed region) -----------------------
     keep = None
@@ -414,7 +428,7 @@ def main():
     # ---- training sub-record: the one workload with a collective (BASELINE configs[3]) ------------------
     train = None
     if not args.no_train:
-        train = train_record(torch, dist, device, world, rank)
+        train = train_record(torch, dist, device, world, rank, args.steps)
 
     if rank == 0:
         ped_steps = M * STEPS_PER_FORWARD * world          # every rank runs the same shape
@@ -429,19 +443,11 @@ def main():
             avg = v["total_ms"] / v["launches"]
             kern[name] = {"avg_us": 1e3 * avg, "launches_per_forward": v["launches"] / prof_iters,
                           "share": v["total_ms"] / total_ms}
-        traffic = None
-        for tname in ("round2_traffic.json", "round1_traffic.json"):
-            tpath = os.path.join(ROOT, "profiles", tname)
-            if os.path.exists(tpath):      # dram bytes per launch from the committed ncu --set full capture
-                per_launch = json.load(open(tpath))["bytes_per_launch"]
-                traffic = per_launch.get(dom, per_launch.get(dom[:-3]) if dom.endswith("_ts") else None)
-                if traffic is not None:
-                    break
         if dom in DENSE_FLOP_PER_PED_STEP:
             flops = DENSE_FLOP_PER_PED_STEP[dom] * M
             achieved = flops / (dom_avg_ms * 1e-3) / 1e12
             roofline = {"kernel": dom, "bound": "tensor", "achieved": achieved, "peak": tf_sust,
-                        "unit": "TFLOP/s", "frac": achieved / tf_sust, "traffic": traffic,
+                        "unit": "TFLOP/s", "frac": achieved / tf_sust,
                         "peak_source": how + " bf16 sustained (kernel timed inside a long step)",
                         "note": "achieved = dense algorithmic FLOPs of the 4096->1024 grid Linear (SURVEY 8d: "
                                 "2*4096*1024 per ped-step) / CUDA-event time; the kernel issues 3 bf16 passes "
@@ -450,7 +456,7 @@ def main():
             bytes_ = STATE_BYTES_PER_PED_STEP * M
             achieved = bytes_ / (dom_avg_ms * 1e-3) / 1e9
             roofline = {"kernel": dom, "bound": "hbm", "achieved": achieved, "peak": hbm, "unit": "GB/s",
-                        "frac": achieved / hbm, "traffic": traffic, "peak_source": how}
+                        "frac": achieved / hbm, "peak_source": how}
         # state-streaming view of the whole step (all kernels of one recurrence step)
         step_ms = total_ms / prof_iters / STEPS_PER_FORWARD
         roofline["step_hbm"] = {"achieved": STATE_BYTES_PER_PED_STEP * M / (step_ms * 1e-3) / 1e9,

@@ -1,5 +1,5 @@
 /*
- * trajnet_b200.h -- C ABI of the B200-native TrajNet++ hot path (libtrajnet_b200.so).
+ * trajnet_b200.h -- C ABI of the H100-native TrajNet++ hot path (libtrajnet_b200.so).
  *
  * The reference (vita-epfl/trajnetplusplusbaselines) is pure Python and has no FFI; this
  * header is the boundary a maintainer binds with ctypes (see INTEGRATION.md).  Every entry

@@ -1,4 +1,4 @@
-"""Per-parameter gradient comparison: CUDA backward vs the unmodified reference (baseline/_ref) autograd."""
+"""Per-parameter gradient comparison: CUDA backward vs the unmodified reference (oracle/_ref) autograd."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, torch

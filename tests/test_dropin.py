@@ -8,7 +8,7 @@ drives this package's classes.
   * `trajnetbaselines.lstm.trajnet_evaluator.predict_scene` (reference lstm/trajnet_evaluator.py:15-19) calls
     this package's `LSTMPredictor` and is compared with the reference's predictor.
 
-The reference comes from baseline/_ref (baseline/install_ref.sh; git-ignored, travels to the GPU box) or
+The reference comes from oracle/_ref (oracle/build_ref.py, run by build(); git-ignored bytecode) or
 /root/reference, through the stub shim in oracle/ref_shim.py.  No reference code is modified or copied.
 """
 import argparse

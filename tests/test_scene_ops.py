@@ -60,26 +60,23 @@ def test_scene_frames_match_center_scene():
     assert table[2, 2] == math.cos(rotation[2]) and table[2, 3] == math.sin(rotation[2])
 
 
-@pytest.mark.needs_reference
 def test_host_functions_match_reference():
-    from oracle.ref_shim import import_reference
-    import_reference()
-    from trajnetbaselines import augmentation
-    from trajnetbaselines.lstm import lstm as ref_lstm
-    from trajnetbaselines.lstm import utils as ref_utils
+    """Bit for bit against the reference's own functions on the same scenes (oracle/make_scene_ops_golden.py)."""
+    import os
     import warnings
-    for xy in _scenes([1, 4, 9, 33], seed=5):
+    g = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "scene_ops_golden.npz"))
+    for i, xy in enumerate(_scenes([1, 4, 9, 33], seed=5)):
+        assert np.array_equal(xy, g["xy%d" % i], equal_nan=True)
         with warnings.catch_warnings():
             warnings.simplefilter("ignore")
             a, ma = drop_distant(xy)
-            b, mb = ref_lstm.drop_distant(xy)
-        assert np.array_equal(ma, mb) and np.array_equal(a, b, equal_nan=True)
+        assert np.array_equal(ma, g["mask%d" % i]) and np.array_equal(a, g["drop%d" % i], equal_nan=True)
         c, rot, cen = center_scene(xy, 9)
-        d, rot_r, cen_r = ref_utils.center_scene(xy, 9)
-        assert rot == rot_r and np.array_equal(cen, cen_r) and np.array_equal(c, d, equal_nan=True)
-        assert np.array_equal(theta_rotation(xy, 1.234), ref_utils.theta_rotation(xy, 1.234), equal_nan=True)
+        assert rot == g["rot%d" % i] and np.array_equal(cen, g["cen%d" % i])
+        assert np.array_equal(c, g["center%d" % i], equal_nan=True)
+        assert np.array_equal(theta_rotation(xy, 1.234), g["theta%d" % i], equal_nan=True)
         pred = c.astype(np.float32)
-        assert np.array_equal(inverse_scene(pred, rot, cen), augmentation.inverse_scene(pred, rot_r, cen_r), equal_nan=True)
+        assert np.array_equal(inverse_scene(pred, rot, cen), g["inverse%d" % i], equal_nan=True)
 
 
 CASES = [

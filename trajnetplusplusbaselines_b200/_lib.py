@@ -194,4 +194,4 @@ def check(rc):
 def require_cuda():
     import torch
     if not torch.cuda.is_available():
-        raise RuntimeError("trajnetplusplusbaselines_b200 needs a CUDA device (sm_100a); there is no CPU path")
+        raise RuntimeError("trajnetplusplusbaselines_b200 needs a CUDA device (sm_90a); there is no CPU path")

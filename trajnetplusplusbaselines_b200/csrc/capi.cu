@@ -60,8 +60,6 @@ size_t carve_workspace(const tb2_lstm* m, const tb2_layout* l, void* base, Works
     w.win_val = (float*)take(M * nm1 * 2 * sizeof(float));
     w.pair_cell = (int*)take(M * nm1 * sizeof(int));
     w.pair_flag = (uint8_t*)take(M * nm1);
-    w.cell_row = nullptr;
-    if (m->Wt1_sw_hi != nullptr && m->cells <= 256) w.cell_row = (uint8_t*)take(M * (size_t)m->cells);
     size_t wmax = 1;
     for (int i = 1; i <= m->n_mlp; ++i) wmax = std::max(wmax, (size_t)m->mlp_dims[i]);
     w.act[0] = (float*)take(M * wmax * sizeof(float));
@@ -214,8 +212,7 @@ int tb2_lstm_create(const tb2_lstm_config* cfg, tb2_lstm** out) {
     m->weights_set = false;
     m->C = 0; m->cells = 0; m->n_mlp = 0; m->P = 0; m->pool_out = 0;
     m->We = m->be = m->Wn = m->bn = m->WencT = m->benc = m->Wt1 = m->base1 = nullptr;
-    m->Wt1_hi = m->Wt1_lo = m->Wt1_nat_hi = m->Wt1_nat_lo = m->Wt1_sw_hi = m->Wt1_sw_lo = nullptr;
-    m->W2_sw = nullptr;
+    m->Wt1_hi = m->Wt1_lo = nullptr;
     for (int i = 0; i < 2; ++i) { m->WgT[i] = m->bg[i] = nullptr; m->Wg_hi[i] = m->Wg_lo[i] = nullptr; }
     for (int i = 0; i < kMaxMlpLayers; ++i) { m->WT[i] = m->bl[i] = nullptr; m->W_hi[i] = m->W_lo[i] = nullptr; }
     m->mp_Ws = m->mp_bs = m->mp_Wv = m->mp_bv = m->mp_WhT = m->mp_bh = m->mp_WoT = m->mp_bo = nullptr;
@@ -368,25 +365,10 @@ int tb2_lstm_create(const tb2_lstm_config* cfg, tb2_lstm** out) {
                 ALLOC(lo, 4);
                 m->Wt1_hi = hi;
                 m->Wt1_lo = lo;
-                float *nh, *nl;
-                ALLOC(nh, half);
-                ALLOC(nl, half);
-                m->Wt1_nat_hi = nh;
-                m->Wt1_nat_lo = nl;
-                float *sh, *sl;
-                ALLOC(sh, 2 * half);      // hi and lo interleaved by 8-row group (one bulk copy per slab)
-                ALLOC(sl, 4);
-                m->Wt1_sw_hi = sh;
-                m->Wt1_sw_lo = sl;
-                if (m->n_mlp == 2 && m->mlp_dims[2] == 256 && m->mlp_dims[1] % 32 == 0) {
-                    float* w2;
-                    ALLOC(w2, (size_t)m->mlp_dims[1] * 256);      // bf16 hi + lo of [256, d1]
-                    m->W2_sw = w2;
-                }
             }
         }
         {
-            // occupancy / directional: first Linear as a dense 3-pass tcgen05 GEMM over an explicit (sparse, zero-padded)
+            // occupancy / directional: first Linear as a dense 3-pass wgmma GEMM over an explicit (sparse, zero-padded)
             // grid row per pedestrian: weights [d1][K padded to 64] in (cell, channel) order as bf16 (hi, lo)
             const char* no_tc = getenv("TB2_DISABLE_TC");
             const int k0p = (m->C * m->cells + 63) / 64 * 64;
@@ -403,7 +385,7 @@ int tb2_lstm_create(const tb2_lstm_config* cfg, tb2_lstm** out) {
         for (int layer = 1; layer < m->n_mlp; ++layer) {
             ALLOC(m->WT[layer], (size_t)m->mlp_dims[layer] * m->mlp_dims[layer + 1]);
             ALLOC(m->bl[layer], m->mlp_dims[layer + 1]);
-            // TB2_DISABLE_TC=1: debug knob for A/B parity runs (fp32 FFMA layer instead of tcgen05)
+            // TB2_DISABLE_TC=1: debug knob for A/B parity runs (fp32 FFMA layer instead of wgmma)
             const char* no_tc = getenv("TB2_DISABLE_TC");
             if (layer == 1 && !(no_tc && no_tc[0] == '1') && dense_tc_supported(m->mlp_dims[1], m->mlp_dims[2])) {
                 const size_t half = ((size_t)m->mlp_dims[1] * m->mlp_dims[2] + 1) / 2;   // bf16 pairs in float units

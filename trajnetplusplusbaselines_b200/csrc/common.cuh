@@ -1,10 +1,9 @@
-// Shared host/device declarations of libtrajnet_b200 (sm_100a only).
+// Shared host/device declarations of libtrajnet_b200 (sm_90a only).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stddef.h>
 #include <atomic>
-#include <list>
 #include <string>
 #include <vector>
 
@@ -40,7 +39,7 @@ extern std::atomic<uint64_t> g_launch_count;
 
 // Programmatic dependent launch: the kernels of a recurrence step are launched with
 // cudaLaunchAttributeProgrammaticStreamSerialization, so the next kernel's CTAs become resident
-// and run their prologue (barrier init, TMEM allocation, tensor-map prefetch) while the previous
+// and run their prologue (barrier init, tensor-map prefetch) while the previous
 // kernel drains.  Every thread executes grid_dep_wait() before its first access to global memory
 // (it returns once the preceding grid has completed and its writes are visible), then
 // grid_dep_launch() lets the following kernel start its own prologue.  TB2_PDL=0 switches the
@@ -126,14 +125,9 @@ struct tb2_lstm {
     float* base1;          // [d1] = b1 + constant * rowsum(W1)
     void* Wt1_hi;          // social, C == 16: bf16 [cells, d1, 16] (hi, lo) slabs for sparse_layer1_mma
     void* Wt1_lo;
-    void* Wt1_nat_hi;      // social, C == 16: bf16 [cells, d1, 16] natural k order (TMA source of sparse_layer1_tc)
-    void* Wt1_nat_lo;
-    void* Wt1_sw_hi;       // social, C == 16: the same slabs as a SWIZZLE_32B shared-memory image (bulk-copy source of
-    void* Wt1_sw_lo;       // sparse_layer1_pair)
-    void* W2_sw;           // social two_layer with 256 outputs: pool.embedding.2.weight as k-step bulk-copy images (fused layer 2)
     float* WT[tb2::kMaxMlpLayers];   // layers >= 2: [K, N] transposed
     float* bl[tb2::kMaxMlpLayers];   // biases of layers >= 2
-    void* W_hi[tb2::kMaxMlpLayers];  // bf16 [N, K] (hi, lo) split for the tcgen05 path (null: FFMA path)
+    void* W_hi[tb2::kMaxMlpLayers];  // bf16 [N, K] (hi, lo) split for the wgmma path (null: FFMA path)
     void* W_lo[tb2::kMaxMlpLayers];
     std::vector<cudaEvent_t> step_events;     // tb2_lstm_forward_sequence_host: one event per recurrence step
     // HiddenStateMLPPooling (TB2_POOL_HIDDEN_MLP)
@@ -159,9 +153,6 @@ struct tb2_layout {
     int group_cap[2];
     int num_groups[2];
     int* group_off[2];     // [G+1] scene indices, device
-    // round tables of sparse_layer1_pair (one per (layer width, unit count, CTAs per unit)), built on first use
-    struct PairPlan { int OUT, units_max, nC, units, rounds_per_unit, max_slots, R; void* dev; int* tile_slots; float* partials; };
-    std::list<PairPlan> pair_plans;           // (list: entries are handed out by pointer)
     std::vector<void*> owned;
 };
 
@@ -176,8 +167,6 @@ struct Workspace {
     float* win_val;        // [M, nm1, 2]
     int* pair_cell;        // [M, nm1]
     uint8_t* pair_flag;    // [M, nm1]
-    uint8_t* cell_row;     // [M, cells] social, cells <= 256: per-row cell map (scene-local winner index, 0xFF none,
-                           // 0xFE NaN-padded slot) read by sparse_layer1_pair; null otherwise
     float* act[2];         // ping-pong MLP activations [M, max width]
     float* act2;           // third scratch (three_layer with a tensor-core second layer)
     float* pooled;         // [M, pool_out]
@@ -228,17 +217,6 @@ int launch_gates(const tb2_lstm* m, const tb2_layout* l, int phase, const float*
                  float* h_out, float* c_out, float* normal_out, float* pos_out, cudaStream_t st);
 int launch_repack(tb2_lstm* m, const tb2_lstm_weights* w, cudaStream_t st);
 int launch_repack_layer1_mma(const float* W1, void* hi, void* lo, int OUT, int cells, cudaStream_t st);
-int launch_repack_layer1_nat(const float* W1, void* hi, void* lo, int OUT, int cells, cudaStream_t st);
-bool sparse_tc_supported(const tb2_lstm* m, const tb2_layout* l, int gsel);
-int launch_sparse_tc(const tb2_lstm* m, const tb2_layout* l, int gsel, Workspace* ws, float* out, void* out_hi,
-                     void* out_lo, cudaStream_t st);
-// round-2 kernel of the same layer (pedestrians on the M side; mode 1 = one CTA, 2 = CTA pair with cta_group::2)
-bool sparse_pair_supported(const tb2_lstm* m, const tb2_layout* l);
-int launch_sparse_pair(const tb2_lstm* m, const tb2_layout* l, int mode, Workspace* ws, float* out, void* out_hi,
-                       void* out_lo, bool fuse2, cudaStream_t st);
-bool sparse_pair_can_fuse(const tb2_lstm* m);
-int launch_repack_layer2_sw(const float* W2, void* dst, int N2, int K, cudaStream_t st);
-int launch_repack_layer1_sw(const float* W1, void* hi, void* lo, int OUT, int cells, cudaStream_t st);
 int launch_hidden_mlp_pool(const tb2_lstm* m, const tb2_layout* l, const float* hidden, const float* obs1,
                            const float* obs2, float* out, cudaStream_t st);
 int launch_attn_mlp_pool(const tb2_lstm* m, const tb2_layout* l, const float* hidden, const float* obs1, const float* obs2,

@@ -1,5 +1,5 @@
-// Fused recurrence step on the tensor cores: LSTMCell gate GEMM (tcgen05 + TMEM + TMA) with the
-// cell update, the Gaussian head and the position feedback in the epilogue.
+// Fused recurrence step on the Hopper tensor cores: LSTMCell gate GEMM (wgmma + TMA + mbarrier)
+// with the cell update, the Gaussian head and the position feedback in the epilogue.
 //
 // Same contract as lstm_gates_kernel (csrc/lstm_step.cu; reference LSTM.step lstm.py:118-168,
 // torch.nn.LSTMCell, Hidden2Normal modules.py:56-64), specialised for E = 64, H = 128,
@@ -7,15 +7,17 @@
 //
 // All three K segments arrive as bf16 (hi, lo) pairs written by their producers (embed_split,
 // the grid-embedding layer's epilogue, the previous step's epilogue) and the product is the
-// 3-pass split  A_hi.W_hi + A_hi.W_lo + A_lo.W_hi  accumulated in fp32 in TMEM.
+// 3-pass split  A_hi.W_hi + A_hi.W_lo + A_lo.W_hi  accumulated in fp32 registers.
 //
 // Grid: (2, ceil(M / 128)) with __cluster_dims__(2, 1, 1).  The two CTAs of a cluster share a
-// 128-row tile and each owns 64 hidden units x 4 gates (256 TMEM columns; W rows are permuted at
-// repack so a CTA's tile holds complete i/f/g/o quadruples).  Warp roles as in gemm_tc.cu.  The
-// epilogue thread of a row reads its gates from TMEM, updates c / h (fp32 state + bf16 split for
-// the next step) and accumulates its half of the 5-wide Hidden2Normal dot products; rank 1 ships
-// its partial sums to rank 0 through distributed shared memory and rank 0 finishes mu / sigma /
-// rho and the fed-back position.
+// 128-row tile and each owns 64 hidden units x 4 gates (N = 256; W rows are permuted at repack so
+// a CTA's tile holds complete i/f/g/o quadruples).  Warpgroup 2 is the TMA producer; warpgroups 0
+// and 1 each run wgmma.m64n256k16 on 64 rows.  In the accumulator fragment (wgmma.cuh) the four
+// gates of a unit sit in the same thread (columns u, 64 + u, 128 + u, 192 + u), so the epilogue
+// updates c / h (fp32 state + bf16 split for the next step) straight from registers and
+// accumulates its share of the 5-wide Hidden2Normal dot products; the four threads of a row add
+// theirs with shuffles, rank 1 ships its partial sums to rank 0 through distributed shared memory
+// and rank 0 finishes mu / sigma / rho and the fed-back position.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <math_constants.h>
@@ -24,6 +26,7 @@
 #include <vector>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace tb2 {
 
@@ -31,64 +34,13 @@ constexpr int kGtBM = 128;
 constexpr int kGtBN = 256;          // 64 units x 4 gates
 constexpr int kGtBK = 64;
 constexpr int kGtStages = 2;
-constexpr int kGtThreads = 576;        // TMA warp, MMA warp, 16 epilogue warps (4 per TMEM lane quarter)
-constexpr int kGtEpiThreads = 512;
+constexpr int kGtThreads = 384;     // two MMA + epilogue warpgroups, one producer warpgroup
+constexpr int kGtConsumerWarps = 8;
 constexpr int kGtH = 128;
 constexpr uint32_t kGtABytes = kGtBM * kGtBK * 2;      // 16 KB
 constexpr uint32_t kGtBBytes = kGtBN * kGtBK * 2;      // 32 KB
 constexpr uint32_t kGtStageBytes = 2 * kGtABytes + 2 * kGtBBytes;   // 96 KB
-constexpr uint32_t kGtTmemCols = 256;
 
-__device__ __forceinline__ uint32_t g_smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void g_mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void g_mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void g_mbar_wait(uint32_t bar, uint32_t parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "G_WAIT_LOOP:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra G_WAIT_DONE;\n"
-        "bra G_WAIT_LOOP;\n"
-        "G_WAIT_DONE:\n"
-        "}\n" ::"r"(bar), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void g_tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ uint64_t g_umma_desc(uint32_t smem_addr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-__device__ __forceinline__ void g_umma(uint32_t tmem_d, uint64_t a, uint64_t b, uint32_t idesc, uint32_t acc) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d), "l"(a), "l"(b), "r"(idesc), "r"(acc) : "memory");
-}
-__device__ __forceinline__ void g_umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void g_tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr));
-}
 // Gate non-linearities on the SFU (ex2.approx, ~2 ulp) -- the epilogue was bound by the ~200
 // instructions per hidden unit of the libm-accurate expf / tanhf.  Absolute error ~1e-7 per
 // activation, the same order as fp32 summation-order noise; parity is re-measured in the tests.
@@ -102,8 +54,6 @@ struct GateTcParams {
     const float* c_in;
     float* h_out;
     float* c_out;
-    const __nv_bfloat16* hs_in_hi;   // split of h_in (read through TMA; here only for masked copy-through)
-    const __nv_bfloat16* hs_in_lo;
     __nv_bfloat16* hs_out_hi;   // [M, 128] split of h_out for the next step
     __nv_bfloat16* hs_out_lo;
     float* normal_out;          // [M, 5]
@@ -112,7 +62,6 @@ struct GateTcParams {
     const float* Wn;            // [5, 128]
     const float* bn;            // [5]
     int M, P;
-    long long* dbg;             // optional [grid, 8] cycle stamps (TB2_GATES_DEBUG=1)
 };
 
 __global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kGtThreads, 1)
@@ -124,250 +73,185 @@ lstm_gates_tc_kernel(const __grid_constant__ CUtensorMap map_emb_hi, const __gri
     extern __shared__ __align__(1024) unsigned char smem_gt[];
     __shared__ __align__(8) uint64_t full_bar[kGtStages];
     __shared__ __align__(8) uint64_t empty_bar[kGtStages];
-    __shared__ __align__(8) uint64_t tmem_full_bar;
-    __shared__ uint32_t tmem_base_slot;
     __shared__ float wn_s[5][64];          // Hidden2Normal weights of this CTA's 64 units
     __shared__ float bg_s[4][64];          // fused gate bias of this CTA's units
     __shared__ float peer_part[kGtBM][5];  // rank 0: partial head sums received from rank 1
-    __shared__ float part_s[4][kGtBM][5];  // per unit-group partial head sums of this CTA
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int rank = blockIdx.x;           // cluster rank == n-tile: units [64 rank, 64 rank + 64)
     const int m0 = blockIdx.y * kGtBM;
     const int kb_pool = p.P / kGtBK;       // k-blocks: [emb | pooled x kb_pool | h x 2]
     const int num_kb = 1 + kb_pool + 2;
-    const uint32_t ring = (g_smem_u32(smem_gt) + 1023u) & ~1023u;
-    long long* dbg = p.dbg ? p.dbg + (size_t)(blockIdx.y * 2 + blockIdx.x) * 8 : nullptr;
-    const long long t_begin = clock64();
+    const uint32_t ring = (smem_u32(smem_gt) + 1023u) & ~1023u;
 
     for (int i = threadIdx.x; i < 5 * 64; i += kGtThreads) wn_s[i / 64][i % 64] = p.Wn[(i / 64) * kGtH + rank * 64 + (i % 64)];
     for (int i = threadIdx.x; i < 4 * 64; i += kGtThreads) bg_s[i / 64][i % 64] = p.bg[(i / 64) * kGtH + rank * 64 + (i % 64)];
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         for (int s = 0; s < kGtStages; ++s) {
-            g_mbar_init(g_smem_u32(&full_bar[s]), 1);
-            g_mbar_init(g_smem_u32(&empty_bar[s]), 1);
+            mbar_init(smem_u32(&full_bar[s]), 1);
+            mbar_init(smem_u32(&empty_bar[s]), kGtConsumerWarps);
         }
-        g_mbar_init(g_smem_u32(&tmem_full_bar), 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                     ::"r"(g_smem_u32(&tmem_base_slot)), "r"(kGtTmemCols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = tmem_base_slot;
     grid_dep_wait();          // embedding / pooled / state operands come from the previous kernels
     grid_dep_launch();
-    if (dbg && threadIdx.x == 0) dbg[0] = clock64() - t_begin;
     // cluster barrier phase 1 (arrive now, wait before the first DSMEM access): a CTA may only
     // touch its peer's shared memory once the peer is known to be resident
     asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
     bool waited_phase1 = false;
 
-    float part[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
-    bool row_valid = false, row_masked = true;
-    int row = 0;
+    // rows (rl, rl + 8) of the tile and their quarter-row share of the head sums (consumer threads)
+    const int rl = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    float part[2][5] = {{0.f, 0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f, 0.f}};
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (wg == 2) {
+        if (threadIdx.x == 256) {
             for (int kb = 0; kb < num_kb; ++kb) {
                 const int s = kb % kGtStages;
                 const uint32_t phase = (kb / kGtStages) & 1;
-                g_mbar_wait(g_smem_u32(&empty_bar[s]), phase ^ 1);
-                const uint32_t bar = g_smem_u32(&full_bar[s]);
+                mbar_wait(smem_u32(&empty_bar[s]), phase ^ 1);
+                const uint32_t bar = smem_u32(&full_bar[s]);
                 const uint32_t base = ring + s * kGtStageBytes;
-                g_mbar_expect_tx(bar, kGtStageBytes);
+                mbar_expect_tx(bar, kGtStageBytes);
                 const CUtensorMap *ahi, *alo;
                 int ka;
                 if (kb == 0) { ahi = &map_emb_hi; alo = &map_emb_lo; ka = 0; }
                 else if (kb <= kb_pool) { ahi = &map_pool_hi; alo = &map_pool_lo; ka = (kb - 1) * kGtBK; }
                 else { ahi = &map_h_hi; alo = &map_h_lo; ka = (kb - 1 - kb_pool) * kGtBK; }
-                g_tma_load_2d(base, ahi, bar, ka, m0);
-                g_tma_load_2d(base + kGtABytes, alo, bar, ka, m0);
-                g_tma_load_2d(base + 2 * kGtABytes, &map_w_hi, bar, kb * kGtBK, rank * kGtBN);
-                g_tma_load_2d(base + 2 * kGtABytes + kGtBBytes, &map_w_lo, bar, kb * kGtBK, rank * kGtBN);
+                tma_load_2d(base, ahi, bar, ka, m0);
+                tma_load_2d(base + kGtABytes, alo, bar, ka, m0);
+                tma_load_2d(base + 2 * kGtABytes, &map_w_hi, bar, kb * kGtBK, rank * kGtBN);
+                tma_load_2d(base + 2 * kGtABytes + kGtBBytes, &map_w_lo, bar, kb * kGtBK, rank * kGtBN);
             }
-        }
-        __syncwarp();
-    } else if (warp == 1) {
-        if (lane == 0) {
-            const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(kGtBN >> 3) << 17) |
-                                   ((uint32_t)(kGtBM >> 4) << 24);
-            long long wait_tma = 0;
-            for (int kb = 0; kb < num_kb; ++kb) {
-                const int s = kb % kGtStages;
-                const uint32_t phase = (kb / kGtStages) & 1;
-                const long long tw = clock64();
-                g_mbar_wait(g_smem_u32(&full_bar[s]), phase);
-                wait_tma += clock64() - tw;
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t base = ring + s * kGtStageBytes;
-                const uint64_t a_hi = g_umma_desc(base);
-                const uint64_t a_lo = g_umma_desc(base + kGtABytes);
-                const uint64_t b_hi = g_umma_desc(base + 2 * kGtABytes);
-                const uint64_t b_lo = g_umma_desc(base + 2 * kGtABytes + kGtBBytes);
-#pragma unroll
-                for (int k = 0; k < kGtBK / 16; ++k) {
-                    const uint64_t adv = (uint64_t)((k * 16 * 2) >> 4);
-                    g_umma(tmem_base, a_hi + adv, b_hi + adv, idesc, (kb | k) != 0);
-                    g_umma(tmem_base, a_hi + adv, b_lo + adv, idesc, 1u);
-                    g_umma(tmem_base, a_lo + adv, b_hi + adv, idesc, 1u);
-                }
-                g_umma_commit(g_smem_u32(&empty_bar[s]));
-            }
-            g_umma_commit(g_smem_u32(&tmem_full_bar));
-            if (dbg) { dbg[1] = clock64() - t_begin; dbg[2] = wait_tma; }
         }
         __syncwarp();
     } else {
-        const int q = warp & 3;              // TMEM lane quarter this warp may read
-        const int ug = (warp - 2) >> 2;      // 16-unit slice of the CTA's 64 hidden units
-        row = m0 + q * 32 + lane;
-        row_valid = row < p.M;
-        float2 o1 = make_float2(CUDART_NAN_F, CUDART_NAN_F), o2 = o1;
-        if (row_valid) { o1 = p.obs1[row]; o2 = p.obs2[row]; }
-        row_masked = isnan(o1.x) || isnan(o2.x);                             // lstm.py:118
-        g_mbar_wait(g_smem_u32(&tmem_full_bar), 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        if (dbg && warp == 2 && lane == 0) dbg[3] = clock64() - t_begin;
-        const uint32_t trow = tmem_base + ((uint32_t)(q * 32) << 16);
-        // All MMAs have retired, so the operand ring is free: each epilogue warp stages its
-        // [32 rows x 16 units] tiles of c and h there, so that global loads / stores run with
-        // lanes along the unit dimension (8 rows x 64 B per instruction) instead of one row per lane.
-        float* tile_h = reinterpret_cast<float*>(smem_gt + (ring - g_smem_u32(smem_gt))) + (size_t)(warp - 2) * (2 * 32 * 17);
-        float* tile_c = tile_h + 32 * 17;
-        const int rsub = lane >> 2, c4 = (lane & 3) * 4;
-        const size_t col0 = (size_t)rank * 64 + ug * 16 + c4;
+        float acc[kGtBN / 2];
 #pragma unroll
-        for (int ps = 0; ps < 4; ++ps) {
-            const int rl = ps * 8 + rsub;
-            const int gr = m0 + q * 32 + rl;
-            float4 v = make_float4(0.f, 0.f, 0.f, 0.f);
-            if (gr < p.M) v = *reinterpret_cast<const float4*>(p.c_in + (size_t)gr * kGtH + col0);
-            float* t = tile_c + rl * 17 + c4;
-            t[0] = v.x; t[1] = v.y; t[2] = v.z; t[3] = v.w;
+        for (int i = 0; i < kGtBN / 2; ++i) acc[i] = 0.f;
+        const uint32_t a_off = (uint32_t)wg * 64 * 128;
+        for (int kb = 0; kb < num_kb; ++kb) {
+            const int s = kb % kGtStages;
+            const uint32_t phase = (kb / kGtStages) & 1;
+            mbar_wait(smem_u32(&full_bar[s]), phase);
+            const uint32_t base = ring + s * kGtStageBytes;
+            const uint64_t a_hi = wgmma_desc(base + a_off);
+            const uint64_t a_lo = wgmma_desc(base + kGtABytes + a_off);
+            const uint64_t b_hi = wgmma_desc(base + 2 * kGtABytes);
+            const uint64_t b_lo = wgmma_desc(base + 2 * kGtABytes + kGtBBytes);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < kGtBK / 16; ++k) {
+                const uint64_t adv = (uint64_t)((k * 16 * 2) >> 4);
+                wgmma_bf16(acc, a_hi + adv, b_hi + adv, (kb | k) != 0);
+                wgmma_bf16(acc, a_hi + adv, b_lo + adv, 1u);
+                wgmma_bf16(acc, a_lo + adv, b_hi + adv, 1u);
+            }
+            wgmma_commit();
+            wgmma_wait_all();
+            if (lane == 0) mbar_arrive(smem_u32(&empty_bar[s]));
         }
-        __syncwarp();
-        {
-            const int u0 = ug * 16;
-            uint32_t gi[16], gf[16], gg[16], go[16];
-            g_tmem_ld16(trow + 0 * 64 + u0, gi);
-            g_tmem_ld16(trow + 1 * 64 + u0, gf);
-            g_tmem_ld16(trow + 2 * 64 + u0, gg);
-            g_tmem_ld16(trow + 3 * 64 + u0, go);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            float* th = tile_h + lane * 17;
-            float* tc = tile_c + lane * 17;
-            if (row_valid && !row_masked) {
+        // gate g of unit u = 8 n8 + 2 (lane % 4) + j, row rl + 8 hr: acc[4 (8 g + n8) + 2 hr + j]
 #pragma unroll
-                for (int v = 0; v < 16; ++v) {
-                    const int u = u0 + v;
-                    const float ig = g_sigmoid(__uint_as_float(gi[v]) + bg_s[0][u]);
-                    const float fg = g_sigmoid(__uint_as_float(gf[v]) + bg_s[1][u]);
-                    const float gt = g_tanh(__uint_as_float(gg[v]) + bg_s[2][u]);
-                    const float og = g_sigmoid(__uint_as_float(go[v]) + bg_s[3][u]);
-                    const float cn = fg * tc[v] + ig * gt;
-                    const float hn = og * g_tanh(cn);
-                    tc[v] = cn;
-                    th[v] = hn;
+        for (int hr = 0; hr < 2; ++hr) {
+            const int row = m0 + rl + 8 * hr;
+            if (row >= p.M) continue;
+            const float2 o1 = p.obs1[row], o2 = p.obs2[row];
+            const bool masked = isnan(o1.x) || isnan(o2.x);                  // lstm.py:118
 #pragma unroll
-                    for (int o = 0; o < 5; ++o) part[o] = fmaf(hn, wn_s[o][u], part[o]);
+            for (int n8 = 0; n8 < 8; ++n8) {
+                const int u = 8 * n8 + 2 * (lane & 3);
+                const size_t o = (size_t)row * kGtH + rank * 64 + u;
+                float2 c = *reinterpret_cast<const float2*>(p.c_in + o);
+                float2 h;
+                if (!masked) {
+                    float cn[2], hn[2];
+                    const float cc[2] = {c.x, c.y};
+#pragma unroll
+                    for (int j = 0; j < 2; ++j) {
+                        const int r = 4 * n8 + 2 * hr + j;
+                        const float ig = g_sigmoid(acc[r] + bg_s[0][u + j]);
+                        const float fg = g_sigmoid(acc[r + 32] + bg_s[1][u + j]);
+                        const float gt = g_tanh(acc[r + 64] + bg_s[2][u + j]);
+                        const float og = g_sigmoid(acc[r + 96] + bg_s[3][u + j]);
+                        cn[j] = fg * cc[j] + ig * gt;
+                        hn[j] = og * g_tanh(cn[j]);
+#pragma unroll
+                        for (int q = 0; q < 5; ++q) part[hr][q] = fmaf(hn[j], wn_s[q][u + j], part[hr][q]);
+                    }
+                    c = make_float2(cn[0], cn[1]);
+                    h = make_float2(hn[0], hn[1]);
+                } else {
+                    // absent track: state copied through unchanged (lstm.py:158-166)
+                    h = *reinterpret_cast<const float2*>(p.h_in + o);
                 }
-            } else if (row_valid) {
-                // absent track: state copied through unchanged (lstm.py:158-166); tile_c already holds c_in
-                const float* hin = p.h_in + (size_t)row * kGtH + rank * 64 + u0;
-#pragma unroll
-                for (int v = 0; v < 16; ++v) th[v] = hin[v];
+                *reinterpret_cast<float2*>(p.h_out + o) = h;
+                *reinterpret_cast<float2*>(p.c_out + o) = c;
+                const __nv_bfloat16 h0 = __float2bfloat16_rn(h.x), h1 = __float2bfloat16_rn(h.y);
+                const __nv_bfloat16 l0 = __float2bfloat16_rn(h.x - __bfloat162float(h0));
+                const __nv_bfloat16 l1 = __float2bfloat16_rn(h.y - __bfloat162float(h1));
+                *reinterpret_cast<uint32_t*>(p.hs_out_hi + o) =
+                    (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
+                *reinterpret_cast<uint32_t*>(p.hs_out_lo + o) =
+                    (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
             }
         }
-        __syncwarp();
+        // the four threads of a row add their shares (fixed order: deterministic)
 #pragma unroll
-        for (int ps = 0; ps < 4; ++ps) {
-            const int rl = ps * 8 + rsub;
-            const int gr = m0 + q * 32 + rl;
-            if (gr < p.M) {
-                const float* sh = tile_h + rl * 17 + c4;
-                const float* sc = tile_c + rl * 17 + c4;
-                const float hv[4] = {sh[0], sh[1], sh[2], sh[3]};
-                const size_t o = (size_t)gr * kGtH + col0;
-                *reinterpret_cast<float4*>(p.h_out + o) = make_float4(hv[0], hv[1], hv[2], hv[3]);
-                *reinterpret_cast<float4*>(p.c_out + o) = make_float4(sc[0], sc[1], sc[2], sc[3]);
-                unsigned short hh[4], hl[4];
+        for (int hr = 0; hr < 2; ++hr)
 #pragma unroll
-                for (int w = 0; w < 4; ++w) {
-                    const __nv_bfloat16 h = __float2bfloat16_rn(hv[w]);
-                    hh[w] = __bfloat16_as_ushort(h);
-                    hl[w] = __bfloat16_as_ushort(__float2bfloat16_rn(hv[w] - __bfloat162float(h)));
-                }
-                *reinterpret_cast<uint2*>(p.hs_out_hi + o) =
-                    make_uint2((uint32_t)hh[0] | ((uint32_t)hh[1] << 16), (uint32_t)hh[2] | ((uint32_t)hh[3] << 16));
-                *reinterpret_cast<uint2*>(p.hs_out_lo + o) =
-                    make_uint2((uint32_t)hl[0] | ((uint32_t)hl[1] << 16), (uint32_t)hl[2] | ((uint32_t)hl[3] << 16));
+            for (int q = 0; q < 5; ++q) {
+                part[hr][q] += __shfl_xor_sync(0xffffffffu, part[hr][q], 1);
+                part[hr][q] += __shfl_xor_sync(0xffffffffu, part[hr][q], 2);
             }
-        }
-        // combine the four unit-groups of a row (fixed order: deterministic)
-        {
-            const int rl = q * 32 + lane;
-#pragma unroll
-            for (int o = 0; o < 5; ++o) part_s[ug][rl][o] = part[o];
-        }
-        asm volatile("bar.sync 1, %0;" ::"n"(kGtEpiThreads) : "memory");
-        if (ug == 0) {
-            const int rl = q * 32 + lane;
-#pragma unroll
-            for (int o = 0; o < 5; ++o) part[o] = ((part_s[0][rl][o] + part_s[1][rl][o]) + part_s[2][rl][o]) + part_s[3][rl][o];
-        }
-        if (rank == 1 && ug == 0) {
+        if (rank == 1) {
             asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");     // phase 1: peer is resident
             waited_phase1 = true;
             // ship this half's head sums to rank 0 through distributed shared memory
-            const int rl = q * 32 + lane;
-            const uint32_t local = g_smem_u32(&peer_part[rl][0]);
-            uint32_t remote;
-            asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(local), "r"(0));
+            if ((lane & 3) == 0) {
 #pragma unroll
-            for (int o = 0; o < 5; ++o)
-                asm volatile("st.shared::cluster.f32 [%0], %1;" ::"r"(remote + 4 * o), "f"(part[o]) : "memory");
+                for (int hr = 0; hr < 2; ++hr) {
+                    const uint32_t local = smem_u32(&peer_part[rl + 8 * hr][0]);
+                    uint32_t remote;
+                    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(local), "r"(0));
+#pragma unroll
+                    for (int q = 0; q < 5; ++q)
+                        asm volatile("st.shared::cluster.f32 [%0], %1;" ::"r"(remote + 4 * q), "f"(part[hr][q]) : "memory");
+                }
+            }
+            __syncwarp();
         }
     }
-    if (dbg && warp == 2 && lane == 0) dbg[4] = clock64() - t_begin;
     // cluster barrier phase 2: rank 1's partial sums are visible in rank 0's shared memory afterwards
     if (!waited_phase1) asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
     asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
     asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-    if (dbg && warp == 2 && lane == 0) dbg[5] = clock64() - t_begin;
-    if (warp >= 2 && warp < 6 && rank == 0 && row_valid) {
-        const int rl = (warp & 3) * 32 + lane;
-        float* no = p.normal_out + (size_t)row * 5;
-        if (row_masked) {
+    if (wg < 2 && rank == 0 && (lane & 3) == 0) {
 #pragma unroll
-            for (int o = 0; o < 5; ++o) no[o] = CUDART_NAN_F;
-            if (p.pos_out) p.pos_out[row] = make_float2(CUDART_NAN_F, CUDART_NAN_F);
-        } else {
-            float s[5];
+        for (int hr = 0; hr < 2; ++hr) {
+            const int row = m0 + rl + 8 * hr;
+            if (row >= p.M) continue;
+            float* no = p.normal_out + (size_t)row * 5;
+            const float2 o1 = p.obs1[row], o2 = p.obs2[row];
+            if (isnan(o1.x) || isnan(o2.x)) {
 #pragma unroll
-            for (int o = 0; o < 5; ++o) s[o] = part[o] + peer_part[rl][o] + p.bn[o];
-            const float n0 = s[0], n1 = s[1];
-            no[0] = n0;
-            no[1] = n1;
-            no[2] = 0.01f + 0.2f * g_sigmoid(s[2]);                           // modules.py:60-62
-            no[3] = 0.01f + 0.2f * g_sigmoid(s[3]);
-            no[4] = 0.7f * g_sigmoid(s[4]);
-            if (p.pos_out) {
-                const float2 o2 = p.obs2[row];
-                p.pos_out[row] = make_float2(o2.x + n0, o2.y + n1);          // lstm.py:232,255
+                for (int q = 0; q < 5; ++q) no[q] = CUDART_NAN_F;
+                if (p.pos_out) p.pos_out[row] = make_float2(CUDART_NAN_F, CUDART_NAN_F);
+            } else {
+                float s[5];
+#pragma unroll
+                for (int q = 0; q < 5; ++q) s[q] = part[hr][q] + peer_part[rl + 8 * hr][q] + p.bn[q];
+                const float n0 = s[0], n1 = s[1];
+                no[0] = n0;
+                no[1] = n1;
+                no[2] = 0.01f + 0.2f * g_sigmoid(s[2]);                           // modules.py:60-62
+                no[3] = 0.01f + 0.2f * g_sigmoid(s[3]);
+                no[4] = 0.7f * g_sigmoid(s[4]);
+                if (p.pos_out) p.pos_out[row] = make_float2(o2.x + n0, o2.y + n1);   // lstm.py:232,255
             }
         }
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (dbg && threadIdx.x == 0) dbg[6] = clock64() - t_begin;
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kGtTmemCols) : "memory");
     }
 }
 
@@ -483,7 +367,6 @@ int launch_gates_tc(const tb2_lstm* m, const tb2_layout* l, int phase, const flo
     p.obs1 = (const float2*)obs1;
     p.obs2 = (const float2*)obs2;
     p.h_in = h_in; p.c_in = c_in; p.h_out = h_out; p.c_out = c_out;
-    p.hs_in_hi = (const __nv_bfloat16*)hs_in_hi; p.hs_in_lo = (const __nv_bfloat16*)hs_in_lo;
     p.hs_out_hi = (__nv_bfloat16*)hs_out_hi; p.hs_out_lo = (__nv_bfloat16*)hs_out_lo;
     p.normal_out = normal_out;
     p.pos_out = (float2*)pos_out;
@@ -492,17 +375,6 @@ int launch_gates_tc(const tb2_lstm* m, const tb2_layout* l, int phase, const flo
     p.bn = m->bn;
     p.M = M;
     p.P = m->P;
-    p.dbg = nullptr;
-    static long long* dbg_buf = nullptr;
-    static int dbg_calls = 0;
-    const int n_cta = 2 * ((M + kGtBM - 1) / kGtBM);
-    {
-        const char* e = getenv("TB2_GATES_DEBUG");
-        if (e && e[0] == '1') {
-            if (!dbg_buf) cudaMalloc(&dbg_buf, (size_t)n_cta * 8 * sizeof(long long));
-            p.dbg = dbg_buf;
-        }
-    }
     const size_t smem = (size_t)kGtStages * kGtStageBytes + 1024;
     static DynSmemConfig configured;
     TB2_CHECK_CUDA(configured.ensure(lstm_gates_tc_kernel, smem));
@@ -513,16 +385,6 @@ int launch_gates_tc(const tb2_lstm* m, const tb2_layout* l, int phase, const flo
                    mw_hi, mw_lo, p);
     }
     TB2_LAUNCH_CHECK();
-    if (p.dbg && ++dbg_calls == 60) {
-        std::vector<long long> h((size_t)n_cta * 8);
-        cudaStreamSynchronize(st);
-        cudaMemcpy(h.data(), dbg_buf, h.size() * sizeof(long long), cudaMemcpyDeviceToHost);
-        double a[7] = {0, 0, 0, 0, 0, 0, 0};
-        for (int c = 0; c < n_cta; ++c) for (int k = 0; k < 7; ++k) a[k] += (double)h[(size_t)c * 8 + k] / n_cta;
-        fprintf(stderr, "[tb2 gates_tc debug] per-CTA cycles since start: setup %.0f | mma issued %.0f (waited on TMA %.0f) | "
-                        "acc ready %.0f | epilogue done %.0f | cluster barrier %.0f | end %.0f\n",
-                a[0], a[1], a[2], a[3], a[4], a[5], a[6]);
-    }
     return TB2_OK;
 }
 

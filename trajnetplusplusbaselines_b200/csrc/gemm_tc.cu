@@ -1,86 +1,37 @@
-// Dense layers of the grid embedding on the 5th-generation tensor cores (tcgen05 + TMEM + TMA).
+// Dense layers of the grid embedding on the Hopper tensor cores (wgmma + TMA + mbarrier).
 //
 //   Y[M, N] = relu(A[M, K] . W[N, K]^T + b)          (reference: the Linear + ReLU pairs of
 //   GridBasedPooling.two_layer / three_layer, trajnetbaselines/lstm/gridbased_pooling.py:316-335)
 //
 // The ADE/FDE gate (1e-4 m) rules out single-pass bf16/tf32 inputs, so the fp32 operands are
-// split into bf16 (hi, lo) pairs and the product is accumulated in fp32 in TMEM from three
+// split into bf16 (hi, lo) pairs and the product is accumulated in fp32 registers from three
 // tensor-core passes:  A.W ~= A_hi.W_hi + A_hi.W_lo + A_lo.W_hi   (dropped terms ~ 2^-17 rel.).
 // A_hi / A_lo are written by the producing kernel (sparse_layer1), W_hi / W_lo at weight repack.
 //
-// Kernel shape (one output tile per CTA, 192 threads):
-//   warp 0      TMA producer: 4 tiles per stage (A_hi, A_lo 128x64, W_hi, W_lo 64x64; bf16,
-//               128B-swizzled, K-major) into a 4-stage shared-memory ring, mbarrier tx-counted
-//   warp 1      allocates 64 TMEM columns, one elected lane issues 12 tcgen05.mma (128x64x16,
-//               kind::f16, cta_group::1) per stage and commits the stage back to the producer
-//   warps 2..5  epilogue: tcgen05.ld 32x32b of the fp32 accumulator (lane = output row),
-//               bias + ReLU, fp32 store
+// Kernel shape (one 128 x BN output tile per CTA, 384 threads):
+//   warpgroup 2   TMA producer (one thread): 4 tiles per stage (A_hi, A_lo 128x64, W_hi, W_lo BNx64;
+//                 bf16, 128B-swizzled, K-major) into a shared-memory ring, mbarrier tx-counted
+//   warpgroups 0, 1  rows [64 wg, 64 wg + 64) of the tile: 12 wgmma.m64nBNk16 per stage into
+//                 fp32 register accumulators, then bias + ReLU and the stores straight from registers
 #include <cuda.h>
 #include <cuda_bf16.h>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace tb2 {
 
 constexpr int kTcBM = 128;
 constexpr int kTcBK = 64;          // 64 bf16 = 128 bytes = one swizzle atom
-constexpr int kTcThreads = 192;
+constexpr int kTcThreads = 384;
+constexpr int kTcConsumerWarps = 8;
 constexpr uint32_t kTcABytes = kTcBM * kTcBK * 2;     // 16 KB
-// BN = 128: 64 KB / stage, 3 stages (M = 5120, N = 256 -> 80 CTAs, one wave on 148 SMs)
-// BN =  64: 48 KB / stage, 4 stages (narrow layers)
+// BN = 128: 64 KB / stage, 3 stages;  BN = 64: 48 KB / stage, 4 stages (narrow layers)
 template <int BN> struct TcCfg {
     static constexpr uint32_t kBBytes = BN * kTcBK * 2;
     static constexpr uint32_t kStageBytes = 2 * kTcABytes + 2 * kBBytes;
     static constexpr int kStages = BN == 128 ? 3 : 4;
-    static constexpr uint32_t kTmemCols = BN;
 };
-
-__device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "WAIT_LOOP:\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n"
-        "@p bra WAIT_DONE;\n"
-        "bra WAIT_LOOP;\n"
-        "WAIT_DONE:\n"
-        "}\n" ::"r"(bar), "r"(parity) : "memory");
-}
-__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, uint32_t bar, int c0, int c1) {
-    asm volatile(
-        "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-        ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ uint64_t umma_smem_desc(uint32_t smem_addr) {
-    // K-major, SWIZZLE_128B: 8-row x 128-byte atoms, SBO = 1024 B between atoms along M/N, LBO unused
-    uint64_t d = 0;
-    d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);          // start address, bits [0,14)
-    d |= (uint64_t)0 << 16;                               // leading byte offset
-    d |= (uint64_t)(1024 >> 4) << 32;                     // stride byte offset, bits [32,46)
-    d |= (uint64_t)1 << 46;                               // descriptor version (Blackwell)
-    d |= (uint64_t)2 << 61;                               // layout type SWIZZLE_128B
-    return d;
-}
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                          uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(tmem_d), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
 
 struct TcParams {
     const float* bias;
@@ -90,6 +41,8 @@ struct TcParams {
     int M, N, K, relu;
 };
 
+__device__ __forceinline__ uint32_t pack_bf16x2(unsigned short a, unsigned short b) { return (uint32_t)a | ((uint32_t)b << 16); }
+
 template <int kTcBN>
 __global__ void __launch_bounds__(kTcThreads, 1)
 dense_layer_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
@@ -98,45 +51,33 @@ dense_layer_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid
     constexpr int kTcStages = TcCfg<kTcBN>::kStages;
     constexpr uint32_t kTcBBytes = TcCfg<kTcBN>::kBBytes;
     constexpr uint32_t kTcStageBytes = TcCfg<kTcBN>::kStageBytes;
-    constexpr uint32_t kTcTmemCols = TcCfg<kTcBN>::kTmemCols;
     extern __shared__ __align__(1024) unsigned char smem_tc[];
     __shared__ __align__(8) uint64_t full_bar[kTcStages];
     __shared__ __align__(8) uint64_t empty_bar[kTcStages];
-    __shared__ __align__(8) uint64_t tmem_full_bar;
-    __shared__ uint32_t tmem_base_slot;
 
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int m0 = blockIdx.y * kTcBM, n0 = blockIdx.x * kTcBN;
     const int num_kb = p.K / kTcBK;
     // 1024-byte aligned tile ring (dynamic smem base alignment is only guaranteed to 16 B)
     const uint32_t ring = (smem_u32(smem_tc) + 1023u) & ~1023u;
 
-    if (warp == 0 && lane == 0) {
+    if (threadIdx.x == 0) {
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a_hi) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a_lo) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b_hi) : "memory");
         asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b_lo) : "memory");
         for (int s = 0; s < kTcStages; ++s) {
             mbar_init(smem_u32(&full_bar[s]), 1);
-            mbar_init(smem_u32(&empty_bar[s]), 1);
+            mbar_init(smem_u32(&empty_bar[s]), kTcConsumerWarps);
         }
-        mbar_init(smem_u32(&tmem_full_bar), 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
-    if (warp == 1) {
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;"
-                     ::"r"(smem_u32(&tmem_base_slot)), "r"(kTcTmemCols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
     __syncthreads();
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-    const uint32_t tmem_base = tmem_base_slot;
     grid_dep_wait();          // the A operand is the previous kernel's output
     grid_dep_launch();
 
-    if (warp == 0) {
-        if (lane == 0) {
+    if (wg == 2) {
+        if (threadIdx.x == 256) {
             for (int kb = 0; kb < num_kb; ++kb) {
                 const int s = kb % kTcStages;
                 const uint32_t phase = (kb / kTcStages) & 1;
@@ -150,99 +91,52 @@ dense_layer_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid
                 tma_load_2d(base + 2 * kTcABytes + kTcBBytes, &map_b_lo, bar, kb * kTcBK, n0);
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            // instruction descriptor: D = F32, A = B = BF16, both K-major, N = 64, M = 128
-            const uint32_t idesc = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(kTcBN >> 3) << 17) |
-                                   ((uint32_t)(kTcBM >> 4) << 24);
-            for (int kb = 0; kb < num_kb; ++kb) {
-                const int s = kb % kTcStages;
-                const uint32_t phase = (kb / kTcStages) & 1;
-                mbar_wait(smem_u32(&full_bar[s]), phase);
-                asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-                const uint32_t base = ring + s * kTcStageBytes;
-                const uint64_t a_hi = umma_smem_desc(base);
-                const uint64_t a_lo = umma_smem_desc(base + kTcABytes);
-                const uint64_t b_hi = umma_smem_desc(base + 2 * kTcABytes);
-                const uint64_t b_lo = umma_smem_desc(base + 2 * kTcABytes + kTcBBytes);
-#pragma unroll
-                for (int k = 0; k < kTcBK / 16; ++k) {
-                    const uint64_t adv = (uint64_t)((k * 16 * 2) >> 4);      // 32 bytes per UMMA_K step
-                    umma_bf16(tmem_base, a_hi + adv, b_hi + adv, idesc, (kb | k) != 0);
-                    umma_bf16(tmem_base, a_hi + adv, b_lo + adv, idesc, 1u);
-                    umma_bf16(tmem_base, a_lo + adv, b_hi + adv, idesc, 1u);
-                }
-                umma_commit(smem_u32(&empty_bar[s]));        // frees the stage when these MMAs retire
-            }
-            umma_commit(smem_u32(&tmem_full_bar));
-        }
-    } else {
-        // epilogue warps 2..5: TMEM lane quarter = warp % 4
-        const int q = warp & 3;
-        mbar_wait(smem_u32(&tmem_full_bar), 0);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const int row = m0 + q * 32 + lane;
-#pragma unroll 1
-        for (int half = 0; half < kTcBN / 32; ++half) {
-            uint32_t r[32];
-            const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(half * 32);
-            asm volatile(
-                "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-                "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-                "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-                : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-                  "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]),
-                  "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]),
-                  "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-                : "r"(taddr));
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-            // stage the warp's [32 rows x 32 cols] chunk (bias + ReLU applied) in the now-free operand
-            // ring and write it out with lanes along the columns: 4 rows x 128 B (fp32) / 64 B (bf16)
-            // per instruction instead of one row per lane
-            float* tile = reinterpret_cast<float*>(smem_tc + (ring - smem_u32(smem_tc))) + (size_t)(warp - 2) * (32 * 33);
-            {
-                const float* brow = p.bias + n0 + half * 32;
-                float* trow_s = tile + lane * 33;
-#pragma unroll
-                for (int c = 0; c < 32; ++c) {
-                    float v = __uint_as_float(r[c]) + brow[c];
-                    if (p.relu) v = fmaxf(v, 0.f);
-                    trow_s[c] = v;
-                }
-            }
-            __syncwarp();
-            const int rsub = lane >> 3, c4 = (lane & 7) * 4;
-#pragma unroll
-            for (int ps = 0; ps < 8; ++ps) {
-                const int rl = ps * 4 + rsub;
-                const int gr = m0 + q * 32 + rl;
-                if (gr < p.M) {
-                    const float* s = tile + rl * 33 + c4;
-                    const float f[4] = {s[0], s[1], s[2], s[3]};
-                    const size_t yoff = (size_t)gr * p.N + n0 + half * 32 + c4;
-                    if (p.Y) *reinterpret_cast<float4*>(p.Y + yoff) = make_float4(f[0], f[1], f[2], f[3]);
-                    if (p.Y_hi) {
-                        unsigned short hh[4], hl[4];
-#pragma unroll
-                        for (int w = 0; w < 4; ++w) {
-                            const __nv_bfloat16 h = __float2bfloat16_rn(f[w]);
-                            hh[w] = __bfloat16_as_ushort(h);
-                            hl[w] = __bfloat16_as_ushort(__float2bfloat16_rn(f[w] - __bfloat162float(h)));
-                        }
-                        *reinterpret_cast<uint2*>(p.Y_hi + yoff) =
-                            make_uint2((uint32_t)hh[0] | ((uint32_t)hh[1] << 16), (uint32_t)hh[2] | ((uint32_t)hh[3] << 16));
-                        *reinterpret_cast<uint2*>(p.Y_lo + yoff) =
-                            make_uint2((uint32_t)hl[0] | ((uint32_t)hl[1] << 16), (uint32_t)hl[2] | ((uint32_t)hl[3] << 16));
-                    }
-                }
-            }
-            __syncwarp();
-        }
+        return;
     }
-    asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-    __syncthreads();
-    if (warp == 1) {
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(kTcTmemCols) : "memory");
+    float acc[kTcBN / 2];
+#pragma unroll
+    for (int i = 0; i < kTcBN / 2; ++i) acc[i] = 0.f;
+    const uint32_t a_off = (uint32_t)wg * 64 * 128;        // this warpgroup's 64 rows of the A tiles
+    for (int kb = 0; kb < num_kb; ++kb) {
+        const int s = kb % kTcStages;
+        const uint32_t phase = (kb / kTcStages) & 1;
+        mbar_wait(smem_u32(&full_bar[s]), phase);
+        const uint32_t base = ring + s * kTcStageBytes;
+        const uint64_t a_hi = wgmma_desc(base + a_off);
+        const uint64_t a_lo = wgmma_desc(base + kTcABytes + a_off);
+        const uint64_t b_hi = wgmma_desc(base + 2 * kTcABytes);
+        const uint64_t b_lo = wgmma_desc(base + 2 * kTcABytes + kTcBBytes);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < kTcBK / 16; ++k) {
+            const uint64_t adv = (uint64_t)((k * 16 * 2) >> 4);      // 32 bytes per K step
+            wgmma_bf16(acc, a_hi + adv, b_hi + adv, (kb | k) != 0);
+            wgmma_bf16(acc, a_hi + adv, b_lo + adv, 1u);
+            wgmma_bf16(acc, a_lo + adv, b_hi + adv, 1u);
+        }
+        wgmma_commit();
+        wgmma_wait_all();
+        if (lane == 0) mbar_arrive(smem_u32(&empty_bar[s]));        // this warp no longer reads the stage
+    }
+    // epilogue from the accumulator fragment: per register pair, one row and two adjacent columns
+    const int row0 = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int col0 = n0 + 2 * (lane & 3);
+#pragma unroll
+    for (int i = 0; i < kTcBN / 2; i += 2) {
+        const int gr = row0 + 8 * ((i >> 1) & 1);
+        const int gc = col0 + 8 * (i >> 2);
+        float v0 = acc[i] + p.bias[gc], v1 = acc[i + 1] + p.bias[gc + 1];
+        if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
+        if (gr >= p.M) continue;
+        const size_t yoff = (size_t)gr * p.N + gc;
+        if (p.Y) *reinterpret_cast<float2*>(p.Y + yoff) = make_float2(v0, v1);
+        if (p.Y_hi) {
+            const __nv_bfloat16 h0 = __float2bfloat16_rn(v0), h1 = __float2bfloat16_rn(v1);
+            *reinterpret_cast<uint32_t*>(p.Y_hi + yoff) = pack_bf16x2(__bfloat16_as_ushort(h0), __bfloat16_as_ushort(h1));
+            *reinterpret_cast<uint32_t*>(p.Y_lo + yoff) =
+                pack_bf16x2(__bfloat16_as_ushort(__float2bfloat16_rn(v0 - __bfloat162float(h0))),
+                            __bfloat16_as_ushort(__float2bfloat16_rn(v1 - __bfloat162float(h1))));
+        }
     }
 }
 

@@ -467,12 +467,6 @@ int launch_repack(tb2_lstm* m, const tb2_lstm_weights* w, cudaStream_t st) {
         if (m->Wt1_hi &&
             (rc = launch_repack_layer1_mma(w->pool_embedding_weight[0], m->Wt1_hi, m->Wt1_lo, m->mlp_dims[1], m->cells, st)))
             return rc;
-        if (m->Wt1_nat_hi &&
-            (rc = launch_repack_layer1_nat(w->pool_embedding_weight[0], m->Wt1_nat_hi, m->Wt1_nat_lo, m->mlp_dims[1], m->cells, st)))
-            return rc;
-        if (m->Wt1_sw_hi &&
-            (rc = launch_repack_layer1_sw(w->pool_embedding_weight[0], m->Wt1_sw_hi, m->Wt1_sw_lo, m->mlp_dims[1], m->cells, st)))
-            return rc;
         if (m->W_hi[0]) {
             const int k0p = (m->C * m->cells + 63) / 64 * 64;
             grid_weight_split_kernel<<<256, 256, 0, st>>>(w->pool_embedding_weight[0], (__nv_bfloat16*)m->W_hi[0],
@@ -485,9 +479,6 @@ int launch_repack(tb2_lstm* m, const tb2_lstm_weights* w, cudaStream_t st) {
                                                   m->mlp_dims[layer + 1], m->mlp_dims[layer]);
             TB2_LAUNCH_CHECK();
             if ((rc = copy_dev(w->pool_embedding_bias[layer], m->bl[layer], (size_t)m->mlp_dims[layer + 1], st))) return rc;
-            if (layer == 1 && m->W2_sw &&
-                (rc = launch_repack_layer2_sw(w->pool_embedding_weight[1], m->W2_sw, m->mlp_dims[2], m->mlp_dims[1], st)))
-                return rc;
             if (m->W_hi[layer] &&
                 (rc = launch_split_bf16(w->pool_embedding_weight[layer], m->W_hi[layer], m->W_lo[layer],
                                         (size_t)m->mlp_dims[layer] * m->mlp_dims[layer + 1], st)))

@@ -77,7 +77,6 @@ struct PrepParams {
     float* win_val;
     int* pair_cell;
     uint8_t* pair_flag;
-    uint8_t* cell_row;        // [M, n * n] per-row cell map for sparse_layer1_pair (or null)
     const float* We;          // input embedding (fused producer of the gate kernel's emb operand)
     const float* be;
     __nv_bfloat16* emb_hi;    // [M, E] bf16 split or null
@@ -228,8 +227,6 @@ __global__ void __launch_bounds__(kPrepMaxThreads, 2) pool_prepare_kernel(PrepPa
     }
     if (nm1 <= 0) {   // single-pedestrian batch: constant grid (gridbased_pooling.py:252-253)
         for (int i = tid; i < n_s; i += kPrepThreads) p.win_count[row0 + i] = 0;
-        if (p.cell_row)
-            for (int idx = tid; idx < n_s * p.n * p.n; idx += kPrepThreads) p.cell_row[(size_t)row0 * p.n * p.n + idx] = 0xffu;
         return;
     }
 
@@ -277,11 +274,6 @@ __global__ void __launch_bounds__(kPrepMaxThreads, 2) pool_prepare_kernel(PrepPa
         // pass 2: winners, compacted in ascending jj
         const bool masked = isnan(vi.x);      // obs2 - obs1 is NaN iff the track is absent at either frame
         int count = 0;
-        uint8_t* crow = p.cell_row ? p.cell_row + (size_t)(row0 + i) * (p.n * p.n) : nullptr;
-        if (crow) {       // all cells empty, winners marked below (same warp: ordered by the __syncwarp)
-            for (int c = lane * 4; c < p.n * p.n; c += 128) *reinterpret_cast<uint32_t*>(crow + c) = 0xffffffffu;
-            __syncwarp();
-        }
         if (!(p.skip_masked && masked)) {
             for (int base = 0; base < nm1; base += 32) {
                 int jj = base + lane;
@@ -305,7 +297,6 @@ __global__ void __launch_bounds__(kPrepMaxThreads, 2) pool_prepare_kernel(PrepPa
                     int j = jj + (jj >= i);
                     // a padded slot can only win in the (discarded) row of an absent pedestrian
                     p.win_ent[gi + slot] = ((uint32_t)cell << 16) | (uint32_t)(j < n_s ? j : 0xffff);
-                    if (crow) crow[cell] = (uint8_t)(j < n_s ? j : 0xfe);
                     if (p.pool_type == TB2_POOL_DIRECTIONAL) {
                         const float2 vj = (j < n_s) ? vel[j] : make_float2(CUDART_NAN_F, CUDART_NAN_F);
                         p.win_val[(gi + slot) * 2 + 0] = nan_to_num_f(vj.x - vi.x);      // :131-140
@@ -341,8 +332,6 @@ int launch_pool_prepare(const tb2_lstm* m, const tb2_layout* l, const float* hid
     p.win_val = ws->win_val;
     p.pair_cell = ws->pair_cell;
     p.pair_flag = ws->pair_flag;
-    // the cell map is written as 32-bit words: n * n must be a multiple of 4 (the pair kernel asks for 16)
-    p.cell_row = (m->cfg.pool_type == TB2_POOL_SOCIAL && (m->cfg.n * m->cfg.n) % 16 == 0 && l->n_max <= 0xFD) ? ws->cell_row : nullptr;
     p.n_max = l->n_max;
     p.H = m->H;
     p.C = m->C;
@@ -617,7 +606,7 @@ __global__ void __launch_bounds__(kL1Threads, 1) sparse_layer1_kernel(L1Params p
 // sparse_layer1_mma: the social grid (C = 16 latent channels) on the tensor cores.
 //   For one cell the pairs binned there form A [pairs x 16] (latent vectors of the winning
 //   neighbours) and the cell's weight slab is B [16 x 256]; pairs-per-cell is ~10, far below the
-//   64/128-row minimum of tcgen05.mma, so this irregular piece uses warp-level
+//   64-row minimum of wgmma, so this irregular piece uses warp-level
 //   mma.sync.m16n8k16 (bf16 inputs, fp32 accumulate) with the same 3-pass (hi, lo) split as the
 //   dense layers.  Warp w owns output columns [32w, 32w+32) of the chunk for ALL pedestrians of
 //   the scene group, so accumulator rows are never shared between warps: no atomics, no
@@ -1063,7 +1052,7 @@ __global__ void __launch_bounds__(kRowsThreads, 1) pool_rows_kernel(RowsParams p
     }
 }
 
-// Dense grid row of every pedestrian for the tcgen05 first Linear (occupancy / directional): [M][Kp] bf16 (hi, lo),
+// Dense grid row of every pedestrian for the wgmma first Linear (occupancy / directional): [M][Kp] bf16 (hi, lo),
 // (value - constant) at the winners' (cell, channel) columns, zero elsewhere (the bias carries constant * sum W).
 // One warp per row.
 __global__ void __launch_bounds__(256) grid_rows_split_kernel(const int* __restrict__ win_count, const uint32_t* __restrict__ win_ent,
@@ -1203,24 +1192,17 @@ int launch_pool_mlp(const tb2_lstm* m, const tb2_layout* l, Workspace* ws, float
         p.out_lo = reinterpret_cast<__nv_bfloat16*>(pool_lo);
     }
     int rc;
-    const char* sp_env = getenv("TB2_SPARSE");       // debug knob: "mma" forces the warp-level MMA kernel,
-    const bool allow_tc = !(sp_env && sp_env[0] == 'm');     // "bucket" the per-cell bucket kernel, "tc" round 1's
-    const bool allow_rows = !(sp_env && sp_env[0] == 'b');   // tcgen05 kernel
-    int pair_mode = 3;                                       // default: the round-2 CTA-pair kernel with the A operand in tensor
-    if (sp_env && sp_env[0] == 'p') pair_mode = 2;           // memory; "pair": A in shared memory; "solo": one CTA per unit;
-    if (sp_env && sp_env[0] == 's' && sp_env[1] == 'o') pair_mode = 1;       // "tc" / "mma" / "bucket": the round-1 kernels
-    if (sp_env && (sp_env[0] == 't' || sp_env[0] == 'm' || sp_env[0] == 'b')) pair_mode = 0;
-    if (sp_env && sp_env[0] == 't' && sp_env[1] == 's') pair_mode = 3;
-    // TB2_GRID_TC=1 (opt-in): built and parity-green, but at the BASELINE batch two launches (grid rows 7-9 us + dense GEMM)
-    // only tie with pool_rows (17-21 us) in inference and cost the launch-bound D-LSTM training step 0.5 ms of host time
-    // (tensor-map encodes per call): profiles/round2_grid_tc_experiment.txt
+    const char* sp_env = getenv("TB2_SPARSE");       // debug knob: "bucket" sends occupancy / directional to the
+    const bool allow_rows = !(sp_env && sp_env[0] == 'b');   // per-cell bucket kernel instead of pool_rows
+    // TB2_GRID_TC=1 (opt-in): explicit grid rows + the dense wgmma GEMM; two launches and tensor-map encodes per call
+    // instead of pool_rows' one launch, so it is not the default
     const char* gtc = getenv("TB2_GRID_TC");
     const int k0p = (m->C * m->cells + 63) / 64 * 64;
     size_t wmax_floats = 1;
     for (int i = 1; i <= m->n_mlp; ++i) wmax_floats = std::max(wmax_floats, (size_t)m->mlp_dims[i]);
     if (!social && m->W_hi[0] != nullptr && gtc && gtc[0] == '1' && (size_t)k0p * 2 <= wmax_floats * sizeof(float) &&
         m->n_mlp == 1) {     // deeper embeddings keep their layer-1 output in the same scratch
-        // occupancy / directional: explicit grid rows (bf16 hi | lo, in the activation scratch) -> dense 3-pass tcgen05 GEMM
+        // occupancy / directional: explicit grid rows (bf16 hi | lo, in the activation scratch) -> dense 3-pass wgmma GEMM
         __nv_bfloat16* a_hi = reinterpret_cast<__nv_bfloat16*>(ws->act[0]);
         __nv_bfloat16* a_lo = reinterpret_cast<__nv_bfloat16*>(ws->act[1]);
         {
@@ -1235,19 +1217,6 @@ int launch_pool_mlp(const tb2_lstm* m, const tb2_layout* l, Workspace* ws, float
     } else
     if (allow_rows && pool_rows_chunk(m, d1) > 0) {   // occupancy / directional: weights resident in smem
         rc = launch_pool_rows(m, l, ws, d1, nm1, p.out, p.out_hi, p.out_lo, st);
-    } else
-    if (pair_mode && ws->cell_row && sparse_pair_supported(m, l)) {   // social, 16 latent channels: CTA-pair tcgen05 kernel
-        // TB2_FUSE2=1: also run the 1024 -> 256 Linear inside the kernel (hidden1 never leaves the SM).  Built, parity-
-        // green (2.9e-7 vs the separate layer) and measured: it LOSES 1.3 % per forward at the BASELINE shape and the
-        // per-piece partial sums make results depend on the batch decomposition -- off by default
-        // (profiles/round2_fuse2_experiment.txt).
-        const char* f2 = getenv("TB2_FUSE2");
-        if (!keep_hidden && sparse_pair_can_fuse(m) && f2 && f2[0] == '1')
-            return launch_sparse_pair(m, l, pair_mode, ws, pooled_out, pool_hi, pool_lo, true, st);
-        rc = launch_sparse_pair(m, l, pair_mode, ws, p.out, p.out_hi, p.out_lo, false, st);
-    } else
-    if (allow_tc && sparse_tc_supported(m, l, 0)) {  // social, 16 latent channels: tcgen05 path
-        rc = launch_sparse_tc(m, l, 0, ws, p.out, p.out_hi, p.out_lo, st);
     } else
     if (m->Wt1_hi != nullptr) {      // social, 16 latent channels: warp-level tensor-core path
         int gm = 0;

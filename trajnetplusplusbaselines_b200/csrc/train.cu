@@ -1321,7 +1321,7 @@ struct SocBuffers {
     uint8_t* pflag;
     uint32_t* wine;
     __nv_bfloat16 *Wt1_hi, *Wt1_lo;                       // bf16 split of the cell-major first-layer weights (dgrid on mma.sync)
-    // 3-pass tcgen05 versions of the row GEMMs (dense_layer_tc_kernel): bf16 (hi, lo) operands
+    // 3-pass wgmma versions of the row GEMMs (dense_layer_tc_kernel): bf16 (hi, lo) operands
     __nv_bfloat16 *X_hi, *X_lo;                           // [S][M][K]
     __nv_bfloat16 *DG_hi[2], *DG_lo[2];                   // [M][512], steps s and s + 1
     __nv_bfloat16 *DZ2_hi, *DZ2_lo;                       // [M][P]
@@ -1504,7 +1504,7 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
         }
         TB2_LAUNCH_CHECK();
     }
-    // The row GEMMs (rows = all tracks) run on the 3-pass tcgen05 kernel of the forward (dense_layer_tc_kernel:
+    // The row GEMMs (rows = all tracks) run on the 3-pass wgmma kernel of the forward (dense_layer_tc_kernel:
     // Y = A . W^T + bias, bf16 (hi, lo) operands, fp32 accumulation) when the shapes allow it: A and the (transposed)
     // weights are split once, the outputs stay fp32.  TB2_BWD_TC=0: cuBLAS / FFMA GEMMs (A/B).
     const char* notc = getenv("TB2_BWD_TC");

@@ -128,7 +128,7 @@ class GridBasedPooling(torch.nn.Module):
             elif not params:      # nothing to .cuda(): parameter-free grid on host inputs
                 device = torch.device('cuda', torch.cuda.current_device())
             else:
-                raise RuntimeError("GridBasedPooling runs on CUDA only: move the module (or inputs) to a B200")
+                raise RuntimeError("GridBasedPooling runs on CUDA only: move the module (or inputs) to the GPU")
         if self._handle is None or self._handle.device != device:
             cfg = _lib.LstmConfig()
             cfg.hidden_dim = 128            # the stand-alone plug does not touch the LSTM cell

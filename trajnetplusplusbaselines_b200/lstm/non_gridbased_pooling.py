@@ -82,7 +82,7 @@ class HiddenStateMLPPooling(torch.nn.Module):
         batch_size, num_tracks = obs2.size(0), obs2.size(1)
         device = self.out_projection.weight.device
         if device.type != 'cuda':
-            raise RuntimeError("HiddenStateMLPPooling runs on CUDA only: move the module to a B200 (module.cuda())")
+            raise RuntimeError("HiddenStateMLPPooling runs on CUDA only: move the module to the GPU (module.cuda())")
         if hidden_states.size(-1) != self.hidden_dim:
             raise ValueError("hidden_states width != hidden_dim")
         if self._handle is None or self._handle.device != device:
@@ -184,7 +184,7 @@ class NearestNeighborMLP(torch.nn.Module, _StandalonePlug):
         batch_size, num_tracks = obs2.size(0), obs2.size(1)
         device = self.embedding[0].weight.device
         if device.type != 'cuda':
-            raise RuntimeError("NearestNeighborMLP runs on CUDA only: move the module to a B200 (module.cuda())")
+            raise RuntimeError("NearestNeighborMLP runs on CUDA only: move the module to the GPU (module.cuda())")
         handle = self._plug_handle(device)
         layout = self._layouts.get(range(0, batch_size * num_tracks + 1, num_tracks), device=device)
         f32 = dict(device=device, dtype=torch.float32)
@@ -258,7 +258,7 @@ class AttentionMLPPooling(torch.nn.Module, _StandalonePlug):
         batch_size, num_tracks = obs2.size(0), obs2.size(1)
         device = self.out_projection.weight.device
         if device.type != 'cuda':
-            raise RuntimeError("AttentionMLPPooling runs on CUDA only: move the module to a B200 (module.cuda())")
+            raise RuntimeError("AttentionMLPPooling runs on CUDA only: move the module to the GPU (module.cuda())")
         if hidden_states.size(-1) != self.hidden_dim:
             raise ValueError("hidden_states width != hidden_dim")
         handle = self._plug_handle(device)
@@ -320,7 +320,7 @@ class NearestNeighborLSTM(torch.nn.Module, _StandalonePlug):
         batch_size, num_tracks = obs2.size(0), obs2.size(1)
         device = self.hidden2pool.weight.device
         if device.type != 'cuda':
-            raise RuntimeError("NearestNeighborLSTM runs on CUDA only: move the module to a B200 (module.cuda())")
+            raise RuntimeError("NearestNeighborLSTM runs on CUDA only: move the module to the GPU (module.cuda())")
         handle = self._plug_handle(device)
         layout = self._layouts.get(range(0, batch_size * num_tracks + 1, num_tracks), device=device)
         if self._reset_pending:
