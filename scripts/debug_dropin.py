@@ -32,7 +32,7 @@ def grads(kind, B, N, seed, ragged, nan_tracks, wseed=11):
         if rel > 1e-4:
             print("    %-40s rel err %.3e  (max |g| %.3e)" % (k, rel, np.abs(g).max()))
 
-print("env TB2_DISABLE_TC=%s TB2_SPARSE=%s" % (os.environ.get("TB2_DISABLE_TC"), os.environ.get("TB2_SPARSE")))
+print("env TB2_DISABLE_TC=%s" % os.environ.get("TB2_DISABLE_TC"))
 grads("social", 10, 7, 17, False, False)
 grads("social", 5, 7, 17, False, False)
 grads("social", 10, 7, 18, False, False)

@@ -42,6 +42,13 @@ static int dev_alloc(std::vector<void*>& owned, void** out, size_t bytes) {
 
 static size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
+// TB2_DISABLE_TC=1: models created from now on run the fp32 FFMA kernels even where the tensor-core kernels
+// apply (A/B parity runs against the bf16 3-pass split)
+static bool tensor_cores_disabled() {
+    const char* e = getenv("TB2_DISABLE_TC");
+    return e && e[0] == '1';
+}
+
 size_t carve_workspace(const tb2_lstm* m, const tb2_layout* l, void* base, Workspace* ws) {
     const size_t M = (size_t)l->M;
     const size_t nm1 = (size_t)(l->n_max > 1 ? l->n_max - 1 : 1);
@@ -300,17 +307,15 @@ int tb2_lstm_create(const tb2_lstm_config* cfg, tb2_lstm** out) {
         ALLOC(m->WgT[ph], (size_t)m->K_gate_pad * 4 * m->H);
         ALLOC(m->bg[ph], 4 * m->H);
     }
-    {
-        const char* no_tc = getenv("TB2_DISABLE_TC");
-        if (!(no_tc && no_tc[0] == '1') && gates_tc_supported(m)) {
-            const size_t half = ((size_t)4 * m->H * m->K_gate + 1) / 2;
-            for (int ph = 0; ph < 2; ++ph) {
-                float *hi, *lo;
-                ALLOC(hi, half);
-                ALLOC(lo, half);
-                m->Wg_hi[ph] = hi;
-                m->Wg_lo[ph] = lo;
-            }
+    const bool no_tc = tensor_cores_disabled();
+    if (!no_tc && gates_tc_supported(m)) {
+        const size_t half = ((size_t)4 * m->H * m->K_gate + 1) / 2;
+        for (int ph = 0; ph < 2; ++ph) {
+            float *hi, *lo;
+            ALLOC(hi, half);
+            ALLOC(lo, half);
+            m->Wg_hi[ph] = hi;
+            m->Wg_lo[ph] = lo;
         }
     }
     if (cfg->pool_type == TB2_POOL_SOCIAL) {
@@ -356,38 +361,18 @@ int tb2_lstm_create(const tb2_lstm_config* cfg, tb2_lstm** out) {
     if (m->n_mlp >= 1) {
         ALLOC(m->Wt1, (size_t)m->cells * m->C * m->mlp_dims[1]);
         ALLOC(m->base1, m->mlp_dims[1]);
-        {
-            const char* no_tc = getenv("TB2_DISABLE_TC");
-            if (cfg->pool_type == TB2_POOL_SOCIAL && m->C == 16 && !(no_tc && no_tc[0] == '1')) {
-                const size_t half = ((size_t)m->cells * 16 * m->mlp_dims[1] + 1) / 2;
-                float *hi, *lo;
-                ALLOC(hi, 2 * half);      // interleaved (hi | lo) slabs
-                ALLOC(lo, 4);
-                m->Wt1_hi = hi;
-                m->Wt1_lo = lo;
-            }
-        }
-        {
-            // occupancy / directional: first Linear as a dense 3-pass wgmma GEMM over an explicit (sparse, zero-padded)
-            // grid row per pedestrian: weights [d1][K padded to 64] in (cell, channel) order as bf16 (hi, lo)
-            const char* no_tc = getenv("TB2_DISABLE_TC");
-            const int k0p = (m->C * m->cells + 63) / 64 * 64;
-            if (cfg->pool_type != TB2_POOL_SOCIAL && m->n_mlp >= 1 && !(no_tc && no_tc[0] == '1') &&
-                dense_tc_supported(k0p, m->mlp_dims[1])) {
-                const size_t half = ((size_t)k0p * m->mlp_dims[1] + 1) / 2;
-                float *hi, *lo;
-                ALLOC(hi, half);
-                ALLOC(lo, half);
-                m->W_hi[0] = hi;
-                m->W_lo[0] = lo;
-            }
+        if (cfg->pool_type == TB2_POOL_SOCIAL && m->C == 16 && !no_tc) {
+            const size_t half = ((size_t)m->cells * 16 * m->mlp_dims[1] + 1) / 2;
+            float *hi, *lo;
+            ALLOC(hi, 2 * half);      // interleaved (hi | lo) slabs
+            ALLOC(lo, 4);
+            m->Wt1_hi = hi;
+            m->Wt1_lo = lo;
         }
         for (int layer = 1; layer < m->n_mlp; ++layer) {
             ALLOC(m->WT[layer], (size_t)m->mlp_dims[layer] * m->mlp_dims[layer + 1]);
             ALLOC(m->bl[layer], m->mlp_dims[layer + 1]);
-            // TB2_DISABLE_TC=1: debug knob for A/B parity runs (fp32 FFMA layer instead of wgmma)
-            const char* no_tc = getenv("TB2_DISABLE_TC");
-            if (layer == 1 && !(no_tc && no_tc[0] == '1') && dense_tc_supported(m->mlp_dims[1], m->mlp_dims[2])) {
+            if (layer == 1 && !no_tc && dense_tc_supported(m->mlp_dims[1], m->mlp_dims[2])) {
                 const size_t half = ((size_t)m->mlp_dims[1] * m->mlp_dims[2] + 1) / 2;   // bf16 pairs in float units
                 float *hi, *lo;
                 ALLOC(hi, half);
@@ -570,7 +555,7 @@ static int step_impl(const tb2_lstm* m, const tb2_layout* l, int phase, const fl
         else if (m->cfg.pool_type == TB2_POOL_ATTN_MLP) rc = launch_attn_mlp_pool(m, l, h_in, obs1, obs2, ws->pooled, st);
         else rc = launch_hidden_mlp_pool(m, l, h_in, obs1, obs2, ws->pooled, st);
         if (rc) return rc;
-        if (tc && (rc = launch_split_rows(ws->pooled, ws->pool_hi, ws->pool_lo, (size_t)l->M * m->P, st))) return rc;
+        if (tc && (rc = launch_split_bf16(ws->pooled, ws->pool_hi, ws->pool_lo, (size_t)l->M * m->P, st))) return rc;
         pooled = ws->pooled;
     } else
     if (m->cfg.pool_type != TB2_POOL_NONE) {
@@ -603,7 +588,7 @@ int tb2_lstm_step_forward(const tb2_lstm* m, const tb2_layout* l, int32_t phase,
     carve_workspace(m, l, workspace, &ws);
     cudaStream_t st = (cudaStream_t)stream;
     if (m->Wg_hi[0] &&
-        (rc = launch_split_rows(h_in, ws.hs_hi[0], ws.hs_lo[0], (size_t)l->M * m->H, st)))
+        (rc = launch_split_bf16(h_in, ws.hs_hi[0], ws.hs_lo[0], (size_t)l->M * m->H, st)))
         return rc;
     return step_impl(m, l, phase, obs1, obs2, h_in, c_in, h_out, c_out, normal_out, pos_out, &ws, 0, st);
 }
@@ -647,7 +632,7 @@ static int forward_steps_impl(const tb2_lstm* m, const tb2_layout* l, const floa
             TB2_CHECK_CUDA(cudaMemsetAsync(ws.hs_lo[0], 0, M * H * 2, st));
         }
     } else if (m->Wg_hi[0]) {      // bf16 split of the incoming state for the tensor-core gate kernel
-        if ((rc = launch_split_rows(h, ws.hs_hi[first_step & 1], ws.hs_lo[first_step & 1], M * H, st))) return rc;
+        if ((rc = launch_split_bf16(h, ws.hs_hi[first_step & 1], ws.hs_lo[first_step & 1], M * H, st))) return rc;
     }
     const float* h_prev = h;
     const float* c_prev = c;

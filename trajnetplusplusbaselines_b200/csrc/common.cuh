@@ -42,15 +42,18 @@ extern std::atomic<uint64_t> g_launch_count;
 // and run their prologue (barrier init, tensor-map prefetch) while the previous
 // kernel drains.  Every thread executes grid_dep_wait() before its first access to global memory
 // (it returns once the preceding grid has completed and its writes are visible), then
-// grid_dep_launch() lets the following kernel start its own prologue.  TB2_PDL=0 switches the
-// launch attribute off (the two instructions are then no-ops).
+// grid_dep_launch() lets the following kernel start its own prologue.
 #ifdef __CUDACC__
 __device__ __forceinline__ void grid_dep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void grid_dep_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 
-inline bool pdl_enabled() {
-    static const bool on = [] { const char* e = getenv("TB2_PDL"); return !(e && e[0] == '0'); }();
-    return on;
+// Warp-level D += A . B, m16n8k16, bf16 inputs, fp32 accumulation (the 3-pass split kernels of pool.cu and train.cu)
+__device__ __forceinline__ void mma_bf16_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
+    asm volatile(
+        "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
+        "{%0, %1, %2, %3};"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
 template <typename... KArgs, typename... Args>
@@ -65,7 +68,7 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = pdl_enabled() ? 1 : 0;
+    cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 #endif
@@ -127,7 +130,7 @@ struct tb2_lstm {
     void* Wt1_lo;
     float* WT[tb2::kMaxMlpLayers];   // layers >= 2: [K, N] transposed
     float* bl[tb2::kMaxMlpLayers];   // biases of layers >= 2
-    void* W_hi[tb2::kMaxMlpLayers];  // bf16 [N, K] (hi, lo) split for the wgmma path (null: FFMA path)
+    void* W_hi[tb2::kMaxMlpLayers];  // [1] only (second Linear): bf16 [N, K] (hi, lo) split for the wgmma path (null: FFMA path)
     void* W_lo[tb2::kMaxMlpLayers];
     std::vector<cudaEvent_t> step_events;     // tb2_lstm_forward_sequence_host: one event per recurrence step
     // HiddenStateMLPPooling (TB2_POOL_HIDDEN_MLP)
@@ -202,16 +205,15 @@ struct TrainCache {
 size_t carve_train_cache(const tb2_lstm* m, const tb2_layout* l, size_t S, void* base, TrainCache* out);
 size_t carve_workspace(const tb2_lstm* m, const tb2_layout* l, void* base, Workspace* ws);
 
-// kernels.cu launchers (all asynchronous on `st`)
+// kernel launchers (all asynchronous on `st`)
 int launch_resolve_obs(const tb2_layout* l, const float* base, const float* pred, float* out,
                        cudaStream_t st);
 int launch_pool_prepare(const tb2_lstm* m, const tb2_layout* l, const float* hidden,
                         const float* obs1, const float* obs2, int skip_masked, int write_pairs,
                         int write_emb, Workspace* ws, cudaStream_t st);
 // pooled_out fp32 and/or (pool_hi, pool_lo) bf16 split (either may be null, not both)
-// keep_hidden: the caller reads hidden1 afterwards (training recompute): the fused layer-1 + layer-2 kernel is not used
 int launch_pool_mlp(const tb2_lstm* m, const tb2_layout* l, Workspace* ws, float* pooled_out,
-                    void* pool_hi, void* pool_lo, cudaStream_t st, bool keep_hidden = false);
+                    void* pool_hi, void* pool_lo, cudaStream_t st);
 int launch_gates(const tb2_lstm* m, const tb2_layout* l, int phase, const float* obs1,
                  const float* obs2, const float* pooled, const float* h_in, const float* c_in,
                  float* h_out, float* c_out, float* normal_out, float* pos_out, cudaStream_t st);
@@ -233,7 +235,6 @@ int launch_dense_tc(const void* a_hi, const void* a_lo, const void* w_hi, const 
 bool gates_tc_supported(const tb2_lstm* m);
 int launch_repack_gates_tc(const float* w_ih, const float* w_hh, void* hi, void* lo, int in_dim, int H, cudaStream_t st);
 int launch_embed_split(const tb2_lstm* m, int M, const float* obs1, const float* obs2, void* hi, void* lo, cudaStream_t st);
-int launch_split_rows(const float* src, void* hi, void* lo, size_t n, cudaStream_t st);
 int launch_gates_tc(const tb2_lstm* m, const tb2_layout* l, int phase, const float* obs1, const float* obs2,
                     const void* emb_hi, const void* emb_lo, const void* pool_hi, const void* pool_lo,
                     const void* hs_in_hi, const void* hs_in_lo, void* hs_out_hi, void* hs_out_lo,

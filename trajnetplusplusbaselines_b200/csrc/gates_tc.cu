@@ -278,16 +278,6 @@ __global__ void embed_split_kernel(const float2* __restrict__ obs1, const float2
     lo[idx] = __float2bfloat16_rn(v - __bfloat162float(h));
 }
 
-__global__ void split_rows_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ hi,
-                                  __nv_bfloat16* __restrict__ lo, size_t n) {
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-        const float v = src[i];
-        const __nv_bfloat16 h = __float2bfloat16_rn(v);
-        hi[i] = h;
-        lo[i] = __float2bfloat16_rn(v - __bfloat162float(h));
-    }
-}
-
 // W_cat[n][k] = [W_ih | W_hh] with rows permuted to (rank, gate, unit) order, as bf16 (hi, lo)
 __global__ void repack_gates_tc_kernel(const float* __restrict__ w_ih, const float* __restrict__ w_hh,
                                        __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo,
@@ -332,12 +322,6 @@ int launch_embed_split(const tb2_lstm* m, int M, const float* obs1, const float*
                    (const float2*)obs2, (const float*)m->We, (const float*)m->be, (__nv_bfloat16*)hi,
                    (__nv_bfloat16*)lo, M, m->E);
     }
-    TB2_LAUNCH_CHECK();
-    return TB2_OK;
-}
-
-int launch_split_rows(const float* src, void* hi, void* lo, size_t n, cudaStream_t st) {
-    split_rows_kernel<<<256, 256, 0, st>>>(src, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo, n);
     TB2_LAUNCH_CHECK();
     return TB2_OK;
 }

@@ -15,6 +15,7 @@
 //                 fp32 register accumulators, then bias + ReLU and the stores straight from registers
 #include <cuda.h>
 #include <cuda_bf16.h>
+#include <algorithm>
 
 #include "common.cuh"
 #include "wgmma.cuh"
@@ -227,7 +228,7 @@ int launch_dense_tc(const void* a_hi, const void* a_lo, const void* w_hi, const 
                      : launch_dense_tc_t<64>(ma_hi, ma_lo, mb_hi, mb_lo, p, st);
 }
 
-// fp32 -> (hi, lo) bf16 split of a weight matrix (repack time)
+// fp32 -> (hi, lo) bf16 split of a flat array: hi = rn(v), lo = rn(v - hi)
 __global__ void split_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ hi,
                                   __nv_bfloat16* __restrict__ lo, size_t n) {
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
@@ -239,7 +240,10 @@ __global__ void split_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* 
 }
 
 int launch_split_bf16(const float* src, void* hi, void* lo, size_t n, cudaStream_t st) {
-    split_bf16_kernel<<<512, 256, 0, st>>>(src, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo, n);
+    if (n == 0) return TB2_OK;
+    // grid-stride over at most 1184 CTAs of 256 threads (about 9 per SM of a 132-SM H100: one resident wave)
+    const unsigned blocks = (unsigned)std::min<size_t>((n + 255) / 256, 1184);
+    split_bf16_kernel<<<blocks, 256, 0, st>>>(src, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo, n);
     TB2_LAUNCH_CHECK();
     return TB2_OK;
 }

@@ -11,9 +11,6 @@
 #include <cuda_bf16.h>
 #include <math_constants.h>
 #include <algorithm>
-#include <cstdio>
-#include <cstdlib>
-#include <vector>
 
 #include "common.cuh"
 
@@ -84,7 +81,6 @@ struct PrepParams {
     int E;
     int n_max, H, C, n, pool_type, front, skip_masked, write_pairs, pad_to_max;
     float side, width;
-    long long* dbg;           // optional [B, 8] clock64 stamps (TB2_PREP_DEBUG=1)
 };
 
 __device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
@@ -131,8 +127,6 @@ __global__ void __launch_bounds__(kPrepMaxThreads, 2) pool_prepare_kernel(PrepPa
     }
     grid_dep_wait();          // obs / hidden state come from the previous kernels of the stream
     grid_dep_launch();
-    long long* dbg = p.dbg ? p.dbg + (size_t)blockIdx.x * 8 : nullptr;
-    const long long t_begin = clock64();
 
     if (fast_lat) {           // raw rows (nan_to_num is applied where they are read), asynchronously
         const float* hsrc = p.hidden + (size_t)row0 * 128;
@@ -157,7 +151,6 @@ __global__ void __launch_bounds__(kPrepMaxThreads, 2) pool_prepare_kernel(PrepPa
     }
     cp_async_wait_all();
     __syncthreads();
-    if (dbg && tid == 0) dbg[0] = clock64() - t_begin;
     if (p.emb_hi != nullptr) {
         // emb = cat(relu(W_e . (4 v) + b_e), 0, 0) (modules.py:24-30) as bf16 (hi, lo) for the gate GEMM
         const int e_shift = (p.E & (p.E - 1)) == 0 ? 31 - __clz(p.E) : -1;       // E = 64: no integer division per element
@@ -172,7 +165,6 @@ __global__ void __launch_bounds__(kPrepMaxThreads, 2) pool_prepare_kernel(PrepPa
             p.emb_lo[(size_t)(row0 + j) * p.E + k] = __float2bfloat16_rn(e - __bfloat162float(h));
         }
     }
-    if (dbg && tid == 0) dbg[1] = clock64() - t_begin;
     if (fast_lat) {
         // lat[j][c] = sum_k nan_to_num(h[j][k]) * WencT[k][c] + benc[c]: one warp per pedestrian, lane = (4 channels,
         // 16-wide k slice); the slice sums are added across the 8 slices by an xor tree (fixed order)
@@ -230,7 +222,6 @@ __global__ void __launch_bounds__(kPrepMaxThreads, 2) pool_prepare_kernel(PrepPa
         return;
     }
 
-    if (dbg && tid == 0) dbg[2] = clock64() - t_begin;
     const float offx = p.width * 0.5f;
     const float offy = p.front ? 0.f : p.width * 0.5f;
     int* myrow = cellrow + warp * nm1;
@@ -270,7 +261,6 @@ __global__ void __launch_bounds__(kPrepMaxThreads, 2) pool_prepare_kernel(PrepPa
             }
         }
         __syncwarp();
-        if (dbg && warp == 0 && lane == 0 && i == 0) dbg[5] = clock64() - t_begin;
         // pass 2: winners, compacted in ascending jj
         const bool masked = isnan(vi.x);      // obs2 - obs1 is NaN iff the track is absent at either frame
         int count = 0;
@@ -310,9 +300,7 @@ __global__ void __launch_bounds__(kPrepMaxThreads, 2) pool_prepare_kernel(PrepPa
         }
         if (lane == 0) p.win_count[row0 + i] = count;
         __syncwarp();
-        if (dbg && warp == 0 && lane == 0 && i == 0) dbg[6] = clock64() - t_begin;
     }
-    if (dbg && lane == 0 && warp == 0) dbg[3] = clock64() - t_begin;
 }
 
 int launch_pool_prepare(const tb2_lstm* m, const tb2_layout* l, const float* hidden,
@@ -346,16 +334,6 @@ int launch_pool_prepare(const tb2_lstm* m, const tb2_layout* l, const float* hid
     p.E = m->E;
     p.emb_hi = write_emb ? (__nv_bfloat16*)ws->emb_hi : nullptr;
     p.emb_lo = write_emb ? (__nv_bfloat16*)ws->emb_lo : nullptr;
-    p.dbg = nullptr;
-    static long long* dbg_buf = nullptr;
-    static int dbg_calls = 0;
-    {
-        const char* e = getenv("TB2_PREP_DEBUG");
-        if (e && e[0] == '1') {
-            if (!dbg_buf) cudaMalloc(&dbg_buf, (size_t)4096 * 8 * sizeof(long long));
-            if (l->B <= 4096 && l->B >= 64) p.dbg = dbg_buf;        // the BASELINE-size batches only
-        }
-    }
     p.side = m->cfg.cell_side;        // pool_size == 1
     p.width = (float)m->cfg.n;
     int nm1 = l->n_max > 1 ? l->n_max - 1 : 1;
@@ -371,16 +349,6 @@ int launch_pool_prepare(const tb2_lstm* m, const tb2_layout* l, const float* hid
         launch_pdl(pool_prepare_kernel, dim3(l->B), dim3(nthreads), smem, st, p);
     }
     TB2_LAUNCH_CHECK();
-    if (p.dbg && ++dbg_calls == 60) {
-        std::vector<long long> h((size_t)l->B * 8);
-        cudaStreamSynchronize(st);
-        cudaMemcpy(h.data(), dbg_buf, h.size() * sizeof(long long), cudaMemcpyDeviceToHost);
-        double a[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-        for (int c = 0; c < l->B; ++c) for (int k = 0; k < 8; ++k) a[k] += (double)h[(size_t)c * 8 + k] / l->B;
-        fprintf(stderr, "[tb2 pool_prepare debug] per-CTA cycles since start (after the dependency wait): staged %.0f | emb %.0f | "
-                        "lat %.0f | winners: row 0 binned %.0f, row 0 done %.0f, warp 0 done %.0f\n",
-                a[0], a[1], a[2], a[5], a[6], a[3]);
-    }
     return TB2_OK;
 }
 
@@ -617,14 +585,6 @@ __global__ void __launch_bounds__(kL1Threads, 1) sparse_layer1_kernel(L1Params p
 // ------------------------------------------------------------------------------------------
 constexpr int kMmaAccStride = kL1Cols + 8;
 
-__device__ __forceinline__ void mma_bf16_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile(
-        "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, "
-        "{%0, %1, %2, %3};"
-        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
-        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-
 __device__ __forceinline__ int kperm16(int k) { return 4 * ((k & 7) >> 1) + 2 * (k >> 3) + (k & 1); }
 
 struct L1MmaParams {
@@ -642,7 +602,6 @@ struct L1MmaParams {
     __nv_bfloat16* out_lo;
     int OUT, cells, nm1, cap, relu;
     float constant;
-    long long* dbg;               // optional [grid, 8] clock64 phase stamps (TB2_L1_DEBUG=1)
 };
 
 constexpr int kMmaThreads = 256;          // 8 warps x 32 output columns
@@ -655,8 +614,6 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
     const int row0 = p.scene_off[s0];
     const int P = p.scene_off[s1] - row0;
     const int chunk0 = blockIdx.y * kL1Cols;
-    long long* dbg = p.dbg ? p.dbg + (size_t)(blockIdx.y * gridDim.x + blockIdx.x) * 8 : nullptr;
-    if (dbg && tid == 0) dbg[0] = clock64();
 
     // acc rows [0, cap) real, [cap, cap + 16) dummies absorbing the padding rows of an MMA tile;
     // lat rows [0, cap) real, cap = NaN-padded slot (b_enc), cap + 1 = zeros (padding rows)
@@ -734,7 +691,6 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
         }
     }
     __syncthreads();
-    if (dbg && tid == 0) dbg[1] = clock64();
 
     // padding rows of a tile: zero latent row, per-lane dummy accumulator rows
     const uint32_t dummy0 = ((uint32_t)(p.cap + 1) << 16) | (uint32_t)(p.cap + g);
@@ -747,13 +703,12 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
 #pragma unroll
     for (int j = 0; j < 4; ++j) okc[j] = ncol0 + 8 * j < p.OUT;
     struct BFrag { uint2 h[4], l[4]; };
-    auto load_b = [&](int cell) -> BFrag {
+    auto load_b = [&](const __nv_bfloat16* w) -> BFrag {      // w: this lane's fragments of one cell
         BFrag f;
-        const size_t o = (size_t)cell * cell_stride;
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             // one 16-byte L2 load per n-tile: (hi.x, hi.y, lo.x, lo.y) fragments of column ncol0 + 8 j
-            const uint4 v = okc[j] ? __ldcg(reinterpret_cast<const uint4*>(wh + o + (size_t)j * 8 * 32))
+            const uint4 v = okc[j] ? __ldcg(reinterpret_cast<const uint4*>(w + (size_t)j * 8 * 32))
                                    : make_uint4(0u, 0u, 0u, 0u);
             f.h[j] = make_uint2(v.x, v.y);
             f.l[j] = make_uint2(v.z, v.w);
@@ -791,34 +746,30 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
     // register ring of 4 fragment sets: the slab of cell c+4 is requested right after cell c is
     // consumed, i.e. three cell-times ahead of its use
     const int nc = p.cells;
-    auto phys = [&](int i) { return i; };
-    BFrag b0 = load_b(phys(0));
-    BFrag b1 = load_b(phys(min(1, nc - 1)));
-    BFrag b2 = load_b(phys(min(2, nc - 1)));
-    BFrag b3 = load_b(phys(min(3, nc - 1)));
+    BFrag b0 = load_b(wh);
+    BFrag b1 = load_b(wh + (size_t)min(1, nc - 1) * cell_stride);
+    BFrag b2 = load_b(wh + (size_t)min(2, nc - 1) * cell_stride);
+    BFrag b3 = load_b(wh + (size_t)min(3, nc - 1) * cell_stride);
+    // the slab requested next (cell + 4) advances by one cell per request: a loop-carried pointer keeps ptxas from
+    // recomputing the addresses from the kernel parameters every cell
+    const __nv_bfloat16* wnext = wh + 4 * cell_stride;
     for (int cell = 0; cell < nc; cell += 4) {
-        int c = phys(cell);
-        process(start[c], start[c + 1], b0);
-        if (cell + 4 < nc) b0 = load_b(phys(cell + 4));
+        process(start[cell], start[cell + 1], b0);
+        if (cell + 4 < nc) { b0 = load_b(wnext); wnext += cell_stride; }
         if (cell + 1 < nc) {
-            c = phys(cell + 1);
-            process(start[c], start[c + 1], b1);
-            if (cell + 5 < nc) b1 = load_b(phys(cell + 5));
+            process(start[cell + 1], start[cell + 2], b1);
+            if (cell + 5 < nc) { b1 = load_b(wnext); wnext += cell_stride; }
         }
         if (cell + 2 < nc) {
-            c = phys(cell + 2);
-            process(start[c], start[c + 1], b2);
-            if (cell + 6 < nc) b2 = load_b(phys(cell + 6));
+            process(start[cell + 2], start[cell + 3], b2);
+            if (cell + 6 < nc) { b2 = load_b(wnext); wnext += cell_stride; }
         }
         if (cell + 3 < nc) {
-            c = phys(cell + 3);
-            process(start[c], start[c + 1], b3);
-            if (cell + 7 < nc) b3 = load_b(phys(cell + 7));
+            process(start[cell + 3], start[cell + 4], b3);
+            if (cell + 7 < nc) { b3 = load_b(wnext); wnext += cell_stride; }
         }
     }
-    if (dbg && lane == 0) dbg[2 + (warp & 3)] = clock64();      // main loop end of warps 0..3
     __syncthreads();
-    if (dbg && tid == 0) dbg[6] = clock64();
     {
         const int col = chunk0 + tid;
         if (col < p.OUT) {
@@ -836,7 +787,6 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
             }
         }
     }
-    if (dbg && tid == 0) dbg[7] = clock64();
 }
 
 static size_t l1_mma_smem_bytes(int cap, int cells, int nm1) {
@@ -1052,34 +1002,6 @@ __global__ void __launch_bounds__(kRowsThreads, 1) pool_rows_kernel(RowsParams p
     }
 }
 
-// Dense grid row of every pedestrian for the wgmma first Linear (occupancy / directional): [M][Kp] bf16 (hi, lo),
-// (value - constant) at the winners' (cell, channel) columns, zero elsewhere (the bias carries constant * sum W).
-// One warp per row.
-__global__ void __launch_bounds__(256) grid_rows_split_kernel(const int* __restrict__ win_count, const uint32_t* __restrict__ win_ent,
-                                                              const float* __restrict__ win_val, int M, int C, int nm1, int Kp,
-                                                              float constant, __nv_bfloat16* __restrict__ hi,
-                                                              __nv_bfloat16* __restrict__ lo) {
-    grid_dep_wait();
-    grid_dep_launch();
-    const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-    if (row >= M) return;
-    uint4* h4 = reinterpret_cast<uint4*>(hi + (size_t)row * Kp);
-    uint4* l4 = reinterpret_cast<uint4*>(lo + (size_t)row * Kp);
-    for (int i = lane; i < Kp / 8; i += 32) { h4[i] = make_uint4(0u, 0u, 0u, 0u); l4[i] = make_uint4(0u, 0u, 0u, 0u); }
-    __syncwarp();
-    const int cnt = win_count[row];
-    for (int e = lane; e < cnt; e += 32) {
-        const uint32_t ent = win_ent[(size_t)row * nm1 + e];
-        const int cell = (int)(ent >> 16);
-        for (int c = 0; c < C; ++c) {
-            const float v = win_val[((size_t)row * nm1 + e) * 2 + c] - constant;
-            const __nv_bfloat16 h = __float2bfloat16_rn(v);
-            hi[(size_t)row * Kp + cell * C + c] = h;
-            lo[(size_t)row * Kp + cell * C + c] = __float2bfloat16_rn(v - __bfloat162float(h));
-        }
-    }
-}
-
 // returns the column chunk width the row kernel can use for this model (0 = does not fit)
 static int pool_rows_chunk(const tb2_lstm* m, int OUT) {
     if (m->cfg.pool_type == TB2_POOL_SOCIAL || m->C > 2) return 0;
@@ -1136,9 +1058,9 @@ static int launch_l1_t(const L1Params& p, int groups, size_t smem, cudaStream_t 
 
 // Grid -> pooled vector (GridBasedPooling.forward after the grid is known, :106-110).
 int launch_pool_mlp(const tb2_lstm* m, const tb2_layout* l, Workspace* ws, float* pooled_out,
-                    void* pool_hi, void* pool_lo, cudaStream_t st, bool keep_hidden) {
+                    void* pool_hi, void* pool_lo, cudaStream_t st) {
     const int nm1 = l->n_max > 1 ? l->n_max - 1 : 1;
-    // producers that cannot write the bf16 split themselves go through fp32 scratch + split_rows
+    // producers that cannot write the bf16 split themselves go through fp32 scratch + launch_split_bf16
     const bool want_split = pool_hi != nullptr;
     const bool last_is_l1 = m->n_mlp == 1;
     const bool last_is_tc = m->n_mlp == 2 && m->W_hi[1] != nullptr;
@@ -1150,7 +1072,7 @@ int launch_pool_mlp(const tb2_lstm* m, const tb2_layout* l, Workspace* ws, float
                                                 l->row_scene, l->scene_off, m->benc, pooled_out, m->C,
                                                 m->cells, nm1, m->cfg.constant, m->cfg.pool_type);
         TB2_LAUNCH_CHECK();
-        if (want_split) rc_all = launch_split_rows(pooled_out, pool_hi, pool_lo, (size_t)l->M * m->pool_out, st);
+        if (want_split) rc_all = launch_split_bf16(pooled_out, pool_hi, pool_lo, (size_t)l->M * m->pool_out, st);
         return rc_all;
     }
     const int d1 = m->mlp_dims[1];
@@ -1192,30 +1114,7 @@ int launch_pool_mlp(const tb2_lstm* m, const tb2_layout* l, Workspace* ws, float
         p.out_lo = reinterpret_cast<__nv_bfloat16*>(pool_lo);
     }
     int rc;
-    const char* sp_env = getenv("TB2_SPARSE");       // debug knob: "bucket" sends occupancy / directional to the
-    const bool allow_rows = !(sp_env && sp_env[0] == 'b');   // per-cell bucket kernel instead of pool_rows
-    // TB2_GRID_TC=1 (opt-in): explicit grid rows + the dense wgmma GEMM; two launches and tensor-map encodes per call
-    // instead of pool_rows' one launch, so it is not the default
-    const char* gtc = getenv("TB2_GRID_TC");
-    const int k0p = (m->C * m->cells + 63) / 64 * 64;
-    size_t wmax_floats = 1;
-    for (int i = 1; i <= m->n_mlp; ++i) wmax_floats = std::max(wmax_floats, (size_t)m->mlp_dims[i]);
-    if (!social && m->W_hi[0] != nullptr && gtc && gtc[0] == '1' && (size_t)k0p * 2 <= wmax_floats * sizeof(float) &&
-        m->n_mlp == 1) {     // deeper embeddings keep their layer-1 output in the same scratch
-        // occupancy / directional: explicit grid rows (bf16 hi | lo, in the activation scratch) -> dense 3-pass wgmma GEMM
-        __nv_bfloat16* a_hi = reinterpret_cast<__nv_bfloat16*>(ws->act[0]);
-        __nv_bfloat16* a_lo = reinterpret_cast<__nv_bfloat16*>(ws->act[1]);
-        {
-            KernelTimer kt("grid_rows_split", st);
-            launch_pdl(grid_rows_split_kernel, dim3((l->M + 7) / 8), dim3(256), 0, st, (const int*)ws->win_count,
-                       (const uint32_t*)ws->win_ent, (const float*)ws->win_val, l->M, m->C, nm1, k0p, m->cfg.constant, a_hi, a_lo);
-        }
-        TB2_LAUNCH_CHECK();
-        float* y = p.out;
-        if (y == nullptr && p.out_hi == nullptr) y = ws->pooled;
-        rc = launch_dense_tc(a_hi, a_lo, m->W_hi[0], m->W_lo[0], m->base1, y, p.out_hi, p.out_lo, l->M, k0p, d1, 1, st);
-    } else
-    if (allow_rows && pool_rows_chunk(m, d1) > 0) {   // occupancy / directional: weights resident in smem
+    if (pool_rows_chunk(m, d1) > 0) {   // occupancy / directional: weights resident in smem
         rc = launch_pool_rows(m, l, ws, d1, nm1, p.out, p.out_hi, p.out_lo, st);
     } else
     if (m->Wt1_hi != nullptr) {      // social, 16 latent channels: warp-level tensor-core path
@@ -1230,15 +1129,6 @@ int launch_pool_mlp(const tb2_lstm* m, const tb2_layout* l, Workspace* ws, float
         q.base = m->base1; q.out = p.out; q.out_hi = p.out_hi; q.out_lo = p.out_lo;
         q.OUT = d1; q.cells = m->cells; q.nm1 = nm1; q.cap = l->group_cap[gm]; q.relu = 1;
         q.constant = m->cfg.constant;
-        q.dbg = nullptr;
-        static long long* dbg_buf = nullptr;
-        static int dbg_calls = 0;
-        const char* dbgenv = getenv("TB2_L1_DEBUG");
-        const int n_cta = l->num_groups[gm] * ((d1 + kL1Cols - 1) / kL1Cols);
-        if (dbgenv && dbgenv[0] == '1') {
-            if (!dbg_buf) cudaMalloc(&dbg_buf, (size_t)n_cta * 8 * sizeof(long long));
-            q.dbg = dbg_buf;
-        }
         static DynSmemConfig configured;
         TB2_CHECK_CUDA(configured.ensure(sparse_layer1_mma_kernel, sm));
         dim3 grid(l->num_groups[gm], (d1 + kL1Cols - 1) / kL1Cols);
@@ -1247,20 +1137,6 @@ int launch_pool_mlp(const tb2_lstm* m, const tb2_layout* l, Workspace* ws, float
             sparse_layer1_mma_kernel<<<grid, kMmaThreads, sm, st>>>(q);
         }
         TB2_LAUNCH_CHECK();
-        if (q.dbg && ++dbg_calls == 60) {       // one warm launch, printed once
-            std::vector<long long> hbuf((size_t)n_cta * 8);
-            cudaStreamSynchronize(st);
-            cudaMemcpy(hbuf.data(), dbg_buf, hbuf.size() * sizeof(long long), cudaMemcpyDeviceToHost);
-            double setup = 0, loop = 0, tail = 0, epi = 0;
-            for (int c = 0; c < n_cta; ++c) {
-                const long long* d = &hbuf[(size_t)c * 8];
-                long long lmax = std::max(std::max(d[2], d[3]), std::max(d[4], d[5]));
-                long long lmin = std::min(std::min(d[2], d[3]), std::min(d[4], d[5]));
-                setup += d[1] - d[0]; loop += lmin - d[1]; tail += lmax - lmin; epi += d[7] - d[6];
-            }
-            fprintf(stderr, "[tb2 l1 debug] per-CTA cycles: setup %.0f  main loop (fastest of 4 warps) %.0f  "
-                            "spread %.0f  epilogue %.0f\n", setup / n_cta, loop / n_cta, tail / n_cta, epi / n_cta);
-        }
         rc = TB2_OK;
     } else
     switch (m->cfg.pool_type) {
@@ -1292,7 +1168,7 @@ int launch_pool_mlp(const tb2_lstm* m, const tb2_layout* l, Workspace* ws, float
         if (rc != TB2_OK) return rc;
         x = y;
     }
-    if (want_split && !direct_split) return launch_split_rows(pooled_out, pool_hi, pool_lo, (size_t)l->M * m->pool_out, st);
+    if (want_split && !direct_split) return launch_split_bf16(pooled_out, pool_hi, pool_lo, (size_t)l->M * m->pool_out, st);
     return TB2_OK;
 }
 

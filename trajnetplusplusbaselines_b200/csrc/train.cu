@@ -748,21 +748,6 @@ __global__ void __launch_bounds__(256) social_dgrid_kernel(const unsigned* __res
 // contiguous bytes of a dz1 row per load) and are split into (hi, lo) in registers.  The FFMA version above needed
 // five shared-memory loads per 16 FMAs and ran at 8.6 TFLOP/s.
 // ------------------------------------------------------------------------------------------
-__global__ void split_bf16_flat_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ hi,
-                                  __nv_bfloat16* __restrict__ lo, size_t n) {
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-        const float v = src[i];
-        const __nv_bfloat16 h = __float2bfloat16_rn(v);
-        hi[i] = h;
-        lo[i] = __float2bfloat16_rn(v - __bfloat162float(h));
-    }
-}
-
-__device__ __forceinline__ void mma_bf16_16816(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-    asm volatile("mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0, %1, %2, %3}, {%4, %5, %6, %7}, {%8, %9}, {%0, %1, %2, %3};"
-                 : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-                 : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
 __device__ __forceinline__ void split2(const float2 v, uint32_t& hi, uint32_t& lo) {
     const __nv_bfloat162 h = __floats2bfloat162_rn(v.x, v.y);
     const __nv_bfloat162 l = __floats2bfloat162_rn(v.x - __low2float(h), v.y - __high2float(h));
@@ -1051,21 +1036,17 @@ static bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 
 
 
 // ------------------------------------------------------------------------------------------
-// Large plain GEMMs of the all-row (social) backward: cuBLAS with FP32 emulation on the bf16 tensor cores
-// (CUBLAS_COMPUTE_32F_EMULATED_16BFX9: every fp32 operand is split into three bf16 values, nine products,
-// fp32-accurate) -- library code for plain library GEMMs; everything with a gather, a mask or a fused epilogue
-// stays in the kernels of this file.  TB2_CUBLAS=0 forces the FFMA kernels (A/B), =2 plain fp32 cuBLAS.
+// Large plain GEMMs of the all-row (social) backward: cuBLAS in fp32 (CUBLAS_COMPUTE_32F) -- library code for
+// plain library GEMMs; everything with a gather, a mask or a fused epilogue stays in the kernels of this file.
 // ------------------------------------------------------------------------------------------
 // cuBLAS is bound at run time (dlopen): inside a torch process the already loaded libcublas.so.12 is used, whatever
-// its minor version; entry points a build does not have (cublasSetEmulationStrategy) are simply skipped, and without
-// the library the FFMA kernels below do the work.
+// its minor version.  Without the library, or when a call fails, the FFMA kernels below do the work.
 struct CublasApi {
     cublasStatus_t (*create)(cublasHandle_t*) = nullptr;
     cublasStatus_t (*set_stream)(cublasHandle_t, cudaStream_t) = nullptr;
     cublasStatus_t (*gemm_ex)(cublasHandle_t, cublasOperation_t, cublasOperation_t, int, int, int, const void*, const void*,
                               cudaDataType, int, const void*, cudaDataType, int, const void*, void*, cudaDataType, int,
                               cublasComputeType_t, cublasGemmAlgo_t) = nullptr;
-    cublasStatus_t (*set_emulation)(cublasHandle_t, cublasEmulationStrategy_t) = nullptr;
     bool ok = false;
 };
 static const CublasApi& cublas_api() {
@@ -1078,31 +1059,20 @@ static const CublasApi& cublas_api() {
         api.create = reinterpret_cast<decltype(api.create)>(dlsym(lib, "cublasCreate_v2"));
         api.set_stream = reinterpret_cast<decltype(api.set_stream)>(dlsym(lib, "cublasSetStream_v2"));
         api.gemm_ex = reinterpret_cast<decltype(api.gemm_ex)>(dlsym(lib, "cublasGemmEx"));
-        api.set_emulation = reinterpret_cast<decltype(api.set_emulation)>(dlsym(lib, "cublasSetEmulationStrategy"));
         api.ok = api.create && api.set_stream && api.gemm_ex;
     });
     return api;
 }
 
-static cublasHandle_t cublas_for_device(int* mode_out) {
+static cublasHandle_t cublas_for_device() {
     static std::mutex mu;
     static cublasHandle_t handles[64] = {nullptr};
-    static int mode = -1;            // 0 off, 1 emulated bf16x9, 2 fp32
+    if (!cublas_api().ok) return nullptr;
     std::lock_guard<std::mutex> lock(mu);
-    if (mode < 0) {
-        const char* e = getenv("TB2_CUBLAS");
-        mode = e ? atoi(e) : 1;
-        if (mode != 0 && !cublas_api().ok) mode = 0;
-    }
-    *mode_out = mode;
-    if (mode == 0) return nullptr;
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess) return nullptr;
     cublasHandle_t& h = handles[dev & 63];
-    if (!h) {
-        if (cublas_api().create(&h) != CUBLAS_STATUS_SUCCESS) { h = nullptr; return nullptr; }
-        if (mode == 1 && cublas_api().set_emulation) cublas_api().set_emulation(h, CUBLAS_EMULATION_STRATEGY_EAGER);
-    }
+    if (!h && cublas_api().create(&h) != CUBLAS_STATUS_SUCCESS) h = nullptr;
     return h;
 }
 
@@ -1110,24 +1080,14 @@ static cublasHandle_t cublas_for_device(int* mode_out) {
 static bool cublas_gemm(cublasOperation_t ta, cublasOperation_t tb, int m, int n, int k, const float* A, int lda,
                         const float* B, int ldb, float beta, float* C, int ldc, const char* name, cudaStream_t st) {
     if ((double)m * n * k < 3.2e7) return false;            // small problems: the FFMA kernels (deterministic split order)
-    int mode = 0;
-    cublasHandle_t h = cublas_for_device(&mode);
+    cublasHandle_t h = cublas_for_device();
     if (!h) return false;
     const CublasApi& api = cublas_api();
-    static bool emulation_ok = true;
     const float alpha = 1.f;
     KernelTimer kt(name, st);
     if (api.set_stream(h, st) != CUBLAS_STATUS_SUCCESS) return false;
-    cublasStatus_t rc = CUBLAS_STATUS_NOT_SUPPORTED;
-    if (mode == 1 && emulation_ok) {
-        rc = api.gemm_ex(h, ta, tb, m, n, k, &alpha, A, CUDA_R_32F, lda, B, CUDA_R_32F, ldb, &beta, C, CUDA_R_32F, ldc,
-                         CUBLAS_COMPUTE_32F_EMULATED_16BFX9, CUBLAS_GEMM_DEFAULT);
-        if (rc != CUBLAS_STATUS_SUCCESS) emulation_ok = false;
-    }
-    if (rc != CUBLAS_STATUS_SUCCESS)
-        rc = api.gemm_ex(h, ta, tb, m, n, k, &alpha, A, CUDA_R_32F, lda, B, CUDA_R_32F, ldb, &beta, C, CUDA_R_32F, ldc,
-                         CUBLAS_COMPUTE_32F, CUBLAS_GEMM_DEFAULT);
-    return rc == CUBLAS_STATUS_SUCCESS;
+    return api.gemm_ex(h, ta, tb, m, n, k, &alpha, A, CUDA_R_32F, lda, B, CUDA_R_32F, ldb, &beta, C, CUDA_R_32F, ldc,
+                       CUBLAS_COMPUTE_32F, CUBLAS_GEMM_DEFAULT) == CUBLAS_STATUS_SUCCESS;
 }
 
 __global__ void fill_bias_rows_kernel(float* __restrict__ C, int ldc, int M, int N, const float* __restrict__ bias) {
@@ -1401,8 +1361,7 @@ static size_t carve_social(const tb2_lstm* m, const tb2_layout* l, size_t S, voi
 template <int C>
 static int social_pair_kernels(const tb2_lstm* m, const tb2_layout* l, const SocBuffers& b, const float* lat,
                                int nm1, int d1, cudaStream_t st) {
-    const char* nomma = getenv("TB2_DGRID_FFMA");               // A/B knob: the fp32 FFMA kernel
-    if (C == 16 && d1 % 32 == 0 && b.Wt1_hi != nullptr && dgrid_mma_smem(d1) <= 200 * 1024 && !(nomma && nomma[0] == '1')) {
+    if (C == 16 && d1 % 32 == 0 && b.Wt1_hi != nullptr && dgrid_mma_smem(d1) <= 200 * 1024) {
         static DynSmemConfig configured;
         TB2_CHECK_CUDA(configured.ensure(social_dgrid_mma_kernel, dgrid_mma_smem(d1), 48 * 1024));
         KernelTimer kt("social_dgrid_mma", st);
@@ -1414,7 +1373,7 @@ static int social_pair_kernels(const tb2_lstm* m, const tb2_layout* l, const Soc
             b.sorted, b.start, b.DH1, d1, m->Wt1, nm1, b.DGRID);
     }
     TB2_LAUNCH_CHECK();
-    if (C == 16 && d1 % 32 == 0 && !(nomma && nomma[0] == '1')) {
+    if (C == 16 && d1 % 32 == 0) {
         KernelTimer kt("social_dw1_mma", st);
         social_dw1_mma_kernel<<<dim3(m->cells, (d1 + 255) / 256), 256, 0, st>>>(
             b.sorted, b.start, nm1, l->row_scene, l->scene_off, lat, b.DH1, d1, b.dWt1);
@@ -1457,9 +1416,8 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
     TB2_CHECK_CUDA(cudaMemsetAsync(b.zero_h, 0, M * 128 * sizeof(float), st));      // state before step 0
     iota_kernel<<<(Mi + 255) / 256, 256, 0, st>>>(b.rows, Mi);
     TB2_LAUNCH_CHECK();
-    split_bf16_flat_kernel<<<1184, 256, 0, st>>>(m->Wt1, b.Wt1_hi, b.Wt1_lo, (size_t)cells * C * d1);
-    TB2_LAUNCH_CHECK();
     int rc;
+    if ((rc = launch_split_bf16(m->Wt1, b.Wt1_hi, b.Wt1_lo, (size_t)cells * C * d1, st))) return rc;
     const bool tc2 = two && m->W_hi[1] != nullptr;
     // (A) forward quantities of every step: winners + lat, hidden1, X = [emb | pooled | h_prev]
     for (int s = 0; s < S; ++s) {
@@ -1487,7 +1445,7 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
             TB2_LAUNCH_CHECK();
         } else {
         if ((rc = launch_pool_prepare(m, l, h_prev ? h_prev : b.zero_h, o1, o2, 1, 1, 0, &w2, st))) return rc;
-        if ((rc = launch_pool_mlp(m, l, &w2, ws.pooled, nullptr, nullptr, st, /*keep_hidden=*/true))) return rc;
+        if ((rc = launch_pool_mlp(m, l, &w2, ws.pooled, nullptr, nullptr, st))) return rc;
         if (two) {
             merge_split_kernel<<<1024, 256, 0, st>>>(tc2 ? (const __nv_bfloat16*)ws.act[0] : nullptr,
                                                      tc2 ? (const __nv_bfloat16*)ws.act[1] : nullptr, ws.act[0],
@@ -1506,9 +1464,8 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
     }
     // The row GEMMs (rows = all tracks) run on the 3-pass wgmma kernel of the forward (dense_layer_tc_kernel:
     // Y = A . W^T + bias, bf16 (hi, lo) operands, fp32 accumulation) when the shapes allow it: A and the (transposed)
-    // weights are split once, the outputs stay fp32.  TB2_BWD_TC=0: cuBLAS / FFMA GEMMs (A/B).
-    const char* notc = getenv("TB2_BWD_TC");
-    const bool tcg = !(notc && notc[0] == '0') && K == EP + 128 && dense_tc_supported(K, 512) && dense_tc_supported(512, 128) &&
+    // weights are split once, the outputs stay fp32.  Other shapes: cuBLAS / FFMA GEMMs.
+    const bool tcg = K == EP + 128 && dense_tc_supported(K, 512) && dense_tc_supported(512, 128) &&
                      dense_tc_supported(512, EP) && (!two || dense_tc_supported(P, d1));
     if (tcg) {
         TB2_CHECK_CUDA(cudaMemsetAsync(b.zero_bias, 0, (size_t)(d1 > 512 ? d1 : 512) * sizeof(float), st));
@@ -1677,12 +1634,6 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
             return rc;
     }
     if ((rc = colsum(b.DLAT, C, S * Mi, C, g->pool_encoding_bias, nullptr, b.scratch, b.scratch_floats, st))) return rc;
-    if (const char* dump = getenv("TB2_DUMP_DLAT")) {       // debug: d lat of every (step, track) as raw fp32 [S, M, C]
-        std::vector<float> host((size_t)S * M * C);
-        cudaStreamSynchronize(st);
-        cudaMemcpy(host.data(), b.DLAT, host.size() * sizeof(float), cudaMemcpyDeviceToHost);
-        if (FILE* f = fopen(dump, "wb")) { fwrite(host.data(), sizeof(float), host.size(), f); fclose(f); }
-    }
     return TB2_OK;
 }
 }  // namespace tb2
