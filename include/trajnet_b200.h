@@ -400,6 +400,40 @@ int64_t tb2_ndjson_format(int64_t num_scenes, const int64_t* scene_id, const int
                           const int64_t* row_ped, const double* row_x, const double* row_y, const int64_t* row_mode,
                           char* out, int64_t capacity);
 
+/* tb2_ndjson_parse_meta -- tb2_ndjson_parse plus the metadata the scorer reads: per track row prediction_number and
+ *   scene_id (-1 where the key is absent), per scene row the tag as main type (-1 where absent) and sub-types as a
+ *   bitmask (bit k = sub-type k).  A tag is an integer or [main, [sub, ...]] with sub-types 0..62; prediction_number and
+ *   scene_id are non-negative integers.  Anything else in those keys refuses the line, as above. */
+int tb2_ndjson_parse_meta(const char* text, size_t len, int64_t max_rows, int64_t* track_frame, int64_t* track_ped,
+                          double* track_x, double* track_y, int64_t* track_prediction_number, int64_t* track_scene_id,
+                          int64_t* num_tracks_out, int64_t* scene_id, int64_t* scene_ped, int64_t* scene_start,
+                          int64_t* scene_end, int64_t* scene_tag, int64_t* scene_sub_tags, int64_t* num_scenes_out,
+                          int64_t* refused_line_out);
+
+/* ---------------------------------------------------------------------------------------
+ * Scoring of predictions (evaluator/trajnet_evaluator.py TrajnetEvaluator.aggregate, evaluator/eval_utils.py): one launch
+ * per file, one record per scene, no atomics (bit-identical from run to run).  S scenes, T = pred_length frames, K modes.
+ * All positions are float64 (x, y) pairs on the ground truth's last T frames of the primary, read as double2 (the four
+ * position arrays must be 16-byte aligned; TB2_ERR_INVALID otherwise); pred_length 1..1024:
+ *   gt_primary_dev      [S, T, 2]      ground-truth primary
+ *   pred_primary_dev    [S, K, T, 2]   predicted primary per mode (modes >= num_modes_dev[s] are not read)
+ *   num_modes_dev       [S] int32      modes of scene s (>= 1)
+ *   gt_neigh_off_dev    [S + 1] int32  scene s owns ground-truth neighbours gt_neigh_off[s] .. gt_neigh_off[s + 1] - 1
+ *   gt_neigh_dev        [G, T, 2], gt_neigh_mask_dev [G, T] uint8 (1 = the neighbour has a row at that frame)
+ *   pred_neigh_*        the same for the predicted neighbours (mode 0)
+ * Outputs: ade_out / fde_out [S, K] per mode (NaN for absent modes); flags_out [S] (TB2_SCORE_* bits; the collisions use
+ * mode 0); with_nll != 0: nll_out [S] = -(mean over the kept timesteps of the clipped KDE log-density), NaN and
+ * TB2_SCORE_NLL_ALL_SKIPPED when no timestep is kept. */
+#define TB2_SCORE_COL_GT 1
+#define TB2_SCORE_COL_PRED 2
+#define TB2_SCORE_NEIGH_COUNT_DIFFERS 4
+#define TB2_SCORE_NLL_ALL_SKIPPED 8
+int tb2_score_scenes(int32_t num_scenes, int32_t pred_length, int32_t max_modes, const double* gt_primary_dev,
+                     const double* pred_primary_dev, const int32_t* num_modes_dev, const int32_t* gt_neigh_off_dev,
+                     const double* gt_neigh_dev, const uint8_t* gt_neigh_mask_dev, const int32_t* pred_neigh_off_dev,
+                     const double* pred_neigh_dev, const uint8_t* pred_neigh_mask_dev, int32_t with_nll,
+                     double* ade_out_dev, double* fde_out_dev, double* nll_out_dev, int32_t* flags_out_dev, void* stream);
+
 /* ---------------------------------------------------------------------------------------
  * Classical crowd simulators (classical/socialforce.py, classical/orca.py).  One simulator
  * per scene, all scenes stepped in lockstep by one persistent kernel; no collective.

@@ -12,6 +12,7 @@ LIB_PATH = os.path.join(_HERE, "libtrajnet_b200.so")
 
 POOL_NONE, POOL_OCCUPANCY, POOL_DIRECTIONAL, POOL_SOCIAL, POOL_HIDDEN_MLP, POOL_NN_MLP, POOL_ATTN_MLP, POOL_NN_LSTM, POOL_TRAJECTRON = 0, 1, 2, 3, 4, 5, 6, 7, 8
 PHASE_ENCODER, PHASE_DECODER = 0, 1
+SCORE_COL_GT, SCORE_COL_PRED, SCORE_NEIGH_COUNT_DIFFERS, SCORE_NLL_ALL_SKIPPED = 1, 2, 4, 8     # tb2_score_scenes flags
 
 _c_float_p = ctypes.c_void_p   # device pointers travel as integers
 
@@ -159,6 +160,8 @@ PROTOTYPES = {
     "tb2_scenes_inverse": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp]),
     "tb2_ndjson_parse": (ctypes.c_int, [_vp, _sz, ctypes.c_int64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "tb2_ndjson_format": (ctypes.c_int64, [ctypes.c_int64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_int64]),
+    "tb2_ndjson_parse_meta": (ctypes.c_int, [_vp, _sz, ctypes.c_int64] + [_vp] * 15),
+    "tb2_score_scenes": (ctypes.c_int, [_i32, _i32, _i32] + [_vp] * 9 + [_i32] + [_vp] * 5),
     "tb2_sf_simulate": (ctypes.c_int, [_vp, ctypes.POINTER(SfParams), _vp, _vp, _vp]),
     "tb2_kalman_predict": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
     "tb2_orca_simulate": (ctypes.c_int, [_vp, ctypes.POINTER(OrcaParams), _vp, _vp, _vp, _vp, _vp, _vp]),

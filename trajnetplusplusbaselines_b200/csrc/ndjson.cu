@@ -8,6 +8,8 @@
 //                      holds ({"track": {...}} / {"scene": {...}}, any key order, any JSON whitespace) and REFUSES a line it
 //                      is not sure about (escapes, a non-integer frame, unknown record types ...): the caller then takes the
 //                      json.loads path for the whole file, so the result never depends on which parser ran.
+//   tb2_ndjson_parse_meta  the same pass, plus the metadata the scorer reads: prediction_number / scene_id of the track
+//                      rows and the tag of the scene rows (main type + sub-type bitmask), refusing anything unusual there.
 //   tb2_ndjson_format  prediction records -> text, byte-identical to json.dumps of the reference writer's dictionaries:
 //                      coordinates are round(x, 2) printed like repr(float) ("%.2f" is the same correctly rounded decimal;
 //                      trailing zero stripped down to one decimal), NaN / Infinity spelled as json.dumps spells them.
@@ -214,20 +216,51 @@ inline int put(char* out, const char* lit) {
     return (int)n;
 }
 
-}  // namespace
-}  // namespace tb2
+// "tag" of a scene row as the TrajNet++ categorisation writes it: an integer, or [main, [sub, ...]] with sub-types 0..62
+// (returned as bit `sub` of *subs).  Anything else is refused.
+bool parse_tag(Cursor& c, long long* main_type, long long* subs) {
+    long long iv = 0;
+    double dv = 0.0;
+    *subs = 0;
+    if (c.p < c.end && *c.p != '[') {
+        if (parse_value(c, &iv, &dv) != V_INT || iv < 0) return false;
+        *main_type = iv;
+        return true;
+    }
+    ++c.p;
+    skip_ws(c);
+    if (parse_value(c, &iv, &dv) != V_INT || iv < 0) return false;
+    *main_type = iv;
+    skip_ws(c);
+    if (c.p >= c.end || *c.p != ',') return false;
+    ++c.p;
+    skip_ws(c);
+    if (c.p >= c.end || *c.p != '[') return false;
+    ++c.p;
+    skip_ws(c);
+    if (c.p < c.end && *c.p == ']') ++c.p;
+    else
+        for (;;) {
+            skip_ws(c);
+            if (parse_value(c, &iv, &dv) != V_INT || iv < 0 || iv > 62) return false;
+            *subs |= 1ll << iv;
+            skip_ws(c);
+            if (c.p < c.end && *c.p == ',') { ++c.p; continue; }
+            if (c.p < c.end && *c.p == ']') { ++c.p; break; }
+            return false;
+        }
+    skip_ws(c);
+    if (c.p >= c.end || *c.p != ']') return false;
+    ++c.p;
+    return true;
+}
 
-using namespace tb2;
-
-extern "C" {
-
-int tb2_ndjson_parse(const char* text, size_t len, int64_t max_rows, int64_t* track_frame, int64_t* track_ped, double* track_x,
-                     double* track_y, int64_t* num_tracks_out, int64_t* scene_id, int64_t* scene_ped, int64_t* scene_start,
-                     int64_t* scene_end, int64_t* num_scenes_out, int64_t* refused_line_out) {
-    TB2_REQUIRE(text || len == 0, "null text");
-    TB2_REQUIRE(track_frame && track_ped && track_x && track_y && num_tracks_out && scene_id && scene_ped && scene_start &&
-                    scene_end && num_scenes_out && refused_line_out,
-                "null argument");
+// The parse of tb2_ndjson_parse; with track_pn != nullptr also the metadata columns of tb2_ndjson_parse_meta.
+int parse_rows(const char* text, size_t len, int64_t max_rows, int64_t* track_frame, int64_t* track_ped, double* track_x,
+               double* track_y, int64_t* track_pn, int64_t* track_sid, int64_t* num_tracks_out, int64_t* scene_id,
+               int64_t* scene_ped, int64_t* scene_start, int64_t* scene_end, int64_t* scene_tag, int64_t* scene_subs,
+               int64_t* num_scenes_out, int64_t* refused_line_out) {
+    const bool meta = track_pn != nullptr;
     int64_t nt = 0, ns = 0, line_no = 0;
     *refused_line_out = -1;
     const char* p = text;
@@ -257,6 +290,7 @@ int tb2_ndjson_parse(const char* text, size_t len, int64_t max_rows, int64_t* tr
             if (c.p >= c.end || *c.p != '{') break;
             ++c.p;
             long long f0 = 0, f1 = 0, f2 = 0, f3 = 0;                  // track: f, p | scene: id, p, s, e
+            long long m0 = -1, m1 = -1;                                // track: prediction_number, scene_id | scene: tag
             double x = 0.0, y = 0.0;
             unsigned have = 0;
             bool inner_ok = false;
@@ -272,7 +306,8 @@ int tb2_ndjson_parse(const char* text, size_t len, int64_t max_rows, int64_t* tr
                     skip_ws(c);
                     long long iv = 0;
                     double dv = 0.0;
-                    const ValueKind kind = parse_value(c, &iv, &dv);
+                    const bool tag = meta && !is_track && key_is(k, kn, "tag");
+                    const ValueKind kind = tag ? (parse_tag(c, &m0, &m1) ? V_OTHER : V_BAD) : parse_value(c, &iv, &dv);
                     if (kind == V_BAD) break;
                     bool bad = false;
                     if (is_track) {
@@ -280,6 +315,8 @@ int tb2_ndjson_parse(const char* text, size_t len, int64_t max_rows, int64_t* tr
                         else if (key_is(k, kn, "p")) { if (kind != V_INT) bad = true; f1 = iv; have |= 2; }
                         else if (key_is(k, kn, "x")) { if (kind == V_OTHER) bad = true; x = dv; have |= 4; }
                         else if (key_is(k, kn, "y")) { if (kind == V_OTHER) bad = true; y = dv; have |= 8; }
+                        else if (meta && key_is(k, kn, "prediction_number")) { if (kind != V_INT || iv < 0) bad = true; m0 = iv; }
+                        else if (meta && key_is(k, kn, "scene_id")) { if (kind != V_INT || iv < 0) bad = true; m1 = iv; }
                     } else {
                         if (key_is(k, kn, "id")) { if (kind != V_INT) bad = true; f0 = iv; have |= 1; }
                         else if (key_is(k, kn, "p")) { if (kind != V_INT) bad = true; f1 = iv; have |= 2; }
@@ -301,10 +338,12 @@ int tb2_ndjson_parse(const char* text, size_t len, int64_t max_rows, int64_t* tr
             if (is_track) {
                 if (nt >= max_rows) break;
                 track_frame[nt] = f0; track_ped[nt] = f1; track_x[nt] = x; track_y[nt] = y;
+                if (meta) { track_pn[nt] = m0; track_sid[nt] = m1; }
                 ++nt;
             } else {
                 if (ns >= max_rows) break;
                 scene_id[ns] = f0; scene_ped[ns] = f1; scene_start[ns] = f2; scene_end[ns] = f3;
+                if (meta) { scene_tag[ns] = m0; scene_subs[ns] = m0 < 0 ? 0 : m1; }
                 ++ns;
             }
             ok = true;
@@ -317,6 +356,39 @@ int tb2_ndjson_parse(const char* text, size_t len, int64_t max_rows, int64_t* tr
     *num_tracks_out = nt;
     *num_scenes_out = ns;
     return TB2_OK;
+}
+
+}  // namespace
+}  // namespace tb2
+
+using namespace tb2;
+
+extern "C" {
+
+int tb2_ndjson_parse(const char* text, size_t len, int64_t max_rows, int64_t* track_frame, int64_t* track_ped, double* track_x,
+                     double* track_y, int64_t* num_tracks_out, int64_t* scene_id, int64_t* scene_ped, int64_t* scene_start,
+                     int64_t* scene_end, int64_t* num_scenes_out, int64_t* refused_line_out) {
+    TB2_REQUIRE(text || len == 0, "null text");
+    TB2_REQUIRE(track_frame && track_ped && track_x && track_y && num_tracks_out && scene_id && scene_ped && scene_start &&
+                    scene_end && num_scenes_out && refused_line_out,
+                "null argument");
+    return parse_rows(text, len, max_rows, track_frame, track_ped, track_x, track_y, nullptr, nullptr, num_tracks_out, scene_id,
+                      scene_ped, scene_start, scene_end, nullptr, nullptr, num_scenes_out, refused_line_out);
+}
+
+int tb2_ndjson_parse_meta(const char* text, size_t len, int64_t max_rows, int64_t* track_frame, int64_t* track_ped,
+                          double* track_x, double* track_y, int64_t* track_prediction_number, int64_t* track_scene_id,
+                          int64_t* num_tracks_out, int64_t* scene_id, int64_t* scene_ped, int64_t* scene_start,
+                          int64_t* scene_end, int64_t* scene_tag, int64_t* scene_sub_tags, int64_t* num_scenes_out,
+                          int64_t* refused_line_out) {
+    TB2_REQUIRE(text || len == 0, "null text");
+    TB2_REQUIRE(track_frame && track_ped && track_x && track_y && track_prediction_number && track_scene_id && num_tracks_out &&
+                    scene_id && scene_ped && scene_start && scene_end && scene_tag && scene_sub_tags && num_scenes_out &&
+                    refused_line_out,
+                "null argument");
+    return parse_rows(text, len, max_rows, track_frame, track_ped, track_x, track_y, track_prediction_number, track_scene_id,
+                      num_tracks_out, scene_id, scene_ped, scene_start, scene_end, scene_tag, scene_sub_tags, num_scenes_out,
+                      refused_line_out);
 }
 
 // Text of the prediction records of `num_scenes` scenes, each = one scene line followed by its rows_per_scene[i] track

@@ -166,8 +166,9 @@ def get_predictions(args, load_predictor=None):
 
 def main(argv=None):
     """`python -m trajnetplusplusbaselines_b200.evaluator --path <dataset> --output model.pkl ...`: the
-    prediction-writing half of `python -m trajnetbaselines.lstm.trajnet_evaluator` (same flags); the
-    metric half (`evaluator.trajnet_evaluator.trajnet_evaluate`) reads the files it writes."""
+    prediction-writing half of `python -m trajnetbaselines.lstm.trajnet_evaluator` (same flags).  With --evaluate the
+    files it writes are then scored against DATA_BLOCK/<dataset>/test_private (scoring.trajnet_evaluate, the metric half
+    of the reference's evaluator) and the results table is printed."""
     import argparse
     parser = argparse.ArgumentParser()
     parser.add_argument('--path', default='trajdata', help='directory of data to test')
@@ -177,11 +178,12 @@ def main(argv=None):
     parser.add_argument('--normalize_scene', action='store_true')
     parser.add_argument('--modes', default=1, type=int)
     parser.add_argument('--chunk', default=1024, type=int, help='scenes per batched forward')
-    # flags of the reference's evaluator CLI that only steer its scoring / plotting stage (not built here):
-    # accepted and ignored so that the documented commands (e.g. `--write_only`) keep working
-    parser.add_argument('--write_only', action='store_true', help='accepted for compatibility: this tool only writes')
-    parser.add_argument('--disable-collision', action='store_true', help='accepted for compatibility (scoring option)')
-    parser.add_argument('--labels', nargs='+', help='accepted for compatibility (table labels)')
+    parser.add_argument('--evaluate', action='store_true',
+                        help='after writing the predictions, score them against test_private and print the table')
+    # the reference's scoring flags: they take effect with --evaluate (without it this tool only writes)
+    parser.add_argument('--write_only', action='store_true', help='write the predictions only (the default without --evaluate)')
+    parser.add_argument('--disable-collision', action='store_true', help='with --evaluate: do not score collisions')
+    parser.add_argument('--labels', nargs='+', help='with --evaluate: model names in the table')
     args = parser.parse_args(argv)
     args.output = args.output if args.output is not None else []
     args.path = os.path.join('DATA_BLOCK', args.path, 'test_pred') + os.sep
@@ -196,6 +198,9 @@ def main(argv=None):
     if _rank_world()[0] == 0:
         for name, n in written.items():
             print('{}: {} scenes written'.format(name, n))
+        if args.evaluate and not args.write_only:
+            from .scoring import trajnet_evaluate
+            trajnet_evaluate(args)
     if world > 1:
         import torch.distributed as dist
         dist.destroy_process_group()
