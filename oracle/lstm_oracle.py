@@ -599,6 +599,16 @@ def synthetic_scenes(num_scenes, peds_per_scene, n_frames=21, seed=0, ragged=Fal
     return xy, bs
 
 
+def scenes_of_sizes(sizes, n_frames=21, seed=0):
+    """Seeded random-walk scenes with the given numbers of tracks (e.g. one crowded scene next to small
+    ones): start ~ N(0, 9 I), per-frame velocity ~ N(0, 0.09 I); xy [T, M, 2] fp32, batch_split int64."""
+    rng = np.random.RandomState(seed)
+    xs = [rng.randn(n, 2)[None] * 3.0 + np.cumsum(rng.randn(n_frames, n, 2) * 0.3, axis=0) for n in sizes]
+    xy = np.concatenate(xs, axis=1).astype(F32)
+    bs = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
+    return xy, bs
+
+
 # ----------------------------------------------------------------------------------------
 # model specs + seeded weights (shapes = the reference's state_dict, SURVEY.md 8b/B2)
 # ----------------------------------------------------------------------------------------
@@ -618,6 +628,17 @@ MODEL_SPECS = {
                               embedding_arch="one_layer", constant=1),
     "occupancy_front": dict(type_="occupancy", hidden_dim=128, cell_side=0.7, n=8, out_dim=32,
                             embedding_arch="three_layer", layer_dims=[80, 56], front=True),
+    # social pooling in each configuration the CUDA library dispatches differently (tests/test_social_backward.py)
+    "social_default": dict(type_="social", hidden_dim=128, cell_side=0.6, n=12, out_dim=256,    # reference trainer's
+                           embedding_arch="one_layer", latent_dim=16),                          # --type social defaults
+    "social_c4": dict(type_="social", hidden_dim=128, cell_side=0.6, n=12, out_dim=128,
+                      embedding_arch="one_layer", latent_dim=4),
+    "social_c32": dict(type_="social", hidden_dim=128, cell_side=0.7, n=8, out_dim=64,
+                       embedding_arch="two_layer", layer_dims=[128], latent_dim=32),
+    "social_d96": dict(type_="social", hidden_dim=128, cell_side=0.6, n=10, out_dim=128,
+                       embedding_arch="two_layer", layer_dims=[96], latent_dim=16),
+    "social_d200": dict(type_="social", hidden_dim=128, cell_side=0.6, n=10, out_dim=128,
+                        embedding_arch="two_layer", layer_dims=[200], latent_dim=16),
 }
 
 
@@ -672,9 +693,14 @@ def pool_config(kind):
     return None if spec is None else PoolConfig(**spec)
 
 
-def random_weights(kind, seed=0, scale=1.0, embedding_dim=64, hidden_dim=128):
+def random_weights(kind, seed=0, scale=1.0, embedding_dim=64, hidden_dim=128, relu_bias=None):
     """Seeded weights in the reference's state_dict layout (uniform(-1/sqrt(fan_in), ..) like
-    torch's default init, times `scale`).  numpy RandomState => identical on every machine."""
+    torch's default init, times `scale`).  numpy RandomState => identical on every machine.
+
+    relu_bias = beta: the biases of the grid embedding's Linears (pool.embedding.*.bias) become +beta
+    (even units) and -beta (odd units).  The pre-activations of those ReLUs then stay far from 0, so
+    rounding differences between implementations cannot flip a ReLU mask, and half of the units are
+    still dead, so a backward that ignores the mask is still caught.  The other weights are unchanged."""
     rng = np.random.RandomState(seed)
     cfg = pool_config(kind)
     W = {}
@@ -741,4 +767,10 @@ def random_weights(kind, seed=0, scale=1.0, embedding_dim=64, hidden_dim=128):
         W[ph + ".bias_ih"] = rng.uniform(-k, k, size=(4 * H,)).astype(F32)
         W[ph + ".bias_hh"] = rng.uniform(-k, k, size=(4 * H,)).astype(F32)
     lin("hidden2normal.linear.weight", "hidden2normal.linear.bias", 5, H)
+    if relu_bias is not None:
+        for name in W:
+            if name.startswith("pool.embedding.") and name.endswith(".bias"):
+                b = np.full(W[name].shape, relu_bias, dtype=F32)
+                b[1::2] = -relu_bias
+                W[name] = b
     return W

@@ -62,6 +62,20 @@ def check_summary(name, grad, golden, rtol, atol):
     return dev
 
 
+def rel_to_max(name, grad, golden):
+    """max |grad - reference| / max |reference| over the stored entries of a gradient tensor."""
+    g = np.asarray(grad, dtype=np.float32)
+    if name + "/full" in golden:
+        ref = golden[name + "/full"]
+        assert ref.shape == g.shape, name
+        got = g
+    else:
+        idx = np.random.RandomState(12345).randint(0, g.size, size=N_SAMPLES)
+        ref = golden[name + "/samples"]
+        got = g.reshape(-1)[idx]
+    return float(np.abs(got - ref).max()) / max(float(np.abs(ref).max()), 1e-12)
+
+
 def main():
     import_reference()
     from trajnetbaselines.lstm import PredictionLoss

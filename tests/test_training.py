@@ -11,7 +11,7 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import torch_ref as TR  # noqa: E402
 from oracle import lstm_oracle as O  # noqa: E402
-from oracle.make_train_golden import TRAIN_CASES, check_summary  # noqa: E402
+from oracle.make_train_golden import TRAIN_CASES, check_summary, rel_to_max  # noqa: E402
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -21,10 +21,7 @@ def train_golden():
     return np.load(os.path.join(ROOT, "tests", "golden", "train_golden.npz"))
 
 
-TORCH_REF_CASES = [c for c in TRAIN_CASES if "social" not in c[1]]     # torch_ref.py covers the non-social pools
-
-
-@pytest.mark.parametrize("case", TORCH_REF_CASES, ids=[c[0] for c in TORCH_REF_CASES])
+@pytest.mark.parametrize("case", TRAIN_CASES, ids=[c[0] for c in TRAIN_CASES])
 def test_torch_restatement_matches_reference_gradients(train_golden, case):
     """CPU: pins tests/torch_ref.py (the checker of the CUDA backward) to the reference."""
     name, kind, B, N, ragged, nan_tracks, dseed, wseed = case
@@ -37,20 +34,6 @@ def test_torch_restatement_matches_reference_gradients(train_golden, case):
             assert pname.startswith("goal_embedding")
             continue
         check_summary(name + "/" + pname, g, train_golden, rtol=2e-3, atol=2e-5)
-
-
-def _rel_to_max(name, grad, golden):
-    """max |grad - reference| / max |reference| over the stored entries of a gradient tensor."""
-    from oracle.make_train_golden import N_SAMPLES
-    g = np.asarray(grad, dtype=np.float32)
-    if name + "/full" in golden:
-        ref = golden[name + "/full"]
-        got = g
-    else:
-        idx = np.random.RandomState(12345).randint(0, g.size, size=N_SAMPLES)
-        ref = golden[name + "/samples"]
-        got = g.reshape(-1)[idx]
-    return float(np.abs(got - ref).max()) / max(float(np.abs(ref).max()), 1e-12)
 
 
 def _cuda_train_step(kind, W, xy, bs):
@@ -88,7 +71,7 @@ def test_cuda_backward_matches_reference_gradients(train_golden, case):
             continue
         assert p.grad is not None, pname
         g = p.grad.cpu().numpy()
-        rel = _rel_to_max(name + "/" + pname, g, train_golden)
+        rel = rel_to_max(name + "/" + pname, g, train_golden)
         if rel > worst:
             worst, worst_name = rel, pname
         # every parameter tensor within 1e-4 of its largest reference entry (measured: a few 1e-6, the fp32
@@ -99,7 +82,7 @@ def test_cuda_backward_matches_reference_gradients(train_golden, case):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("kind", ["vanilla", "directional"])
+@pytest.mark.parametrize("kind", ["vanilla", "directional", "occupancy"])
 def test_cuda_backward_baseline_shape_vs_torch(kind):
     """N = 20, T = 9 + 12 (BASELINE D-LSTM training shape) at a batch the CPU autograd finishes
     in seconds; every gradient tensor compared in full."""
@@ -116,6 +99,30 @@ def test_cuda_backward_baseline_shape_vs_torch(kind):
         g = p.grad.cpu().numpy()
         scale = max(np.abs(g_ref).max(), 1e-6)
         assert np.abs(g - g_ref).max() < 1e-4 * scale + 1e-7, (pname, float(np.abs(g - g_ref).max() / scale))
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("kind", ["directional", "occupancy"])
+def test_cuda_backward_large_scene_vs_torch(kind):
+    """A 90-pedestrian scene next to scenes of 3 and 40: the grid kernels at a large n_max.  The pool
+    biases are +-3 (random_weights(relu_bias=3)), so no ReLU mask can flip between the two forwards; the
+    precondition is asserted, with the distance of the fed-back primaries' offsets to a cell edge."""
+    xy, bs = O.scenes_of_sizes([90, 3, 40], seed=1)
+    W = O.random_weights(kind, seed=51, relu_bias=3.0)
+    stats = {}
+    loss_ref, grads_ref = TR.train_loss_and_grads(W, O.pool_config(kind), xy, bs, dtype=torch.float64,
+                                                  stats=stats)
+    assert stats["relu_pool0"] >= 1e-2 and stats["edge_primary"] >= 1e-5, stats
+    model, loss = _cuda_train_step(kind, W, xy, bs)
+    assert abs(loss - loss_ref) < 1e-5 * abs(loss_ref)
+    for pname, p in model.named_parameters():
+        g_ref = grads_ref[pname]
+        if g_ref is None:
+            assert p.grad is None
+            continue
+        g = p.grad.cpu().numpy()
+        scale = max(np.abs(g_ref).max(), 1e-6)
+        assert np.abs(g - g_ref).max() < 1e-4 * scale, (pname, float(np.abs(g - g_ref).max() / scale))
 
 
 @pytest.mark.gpu
@@ -209,13 +216,9 @@ def test_optimizer_updates_reach_the_device_weights(fused):
 @pytest.mark.gpu
 def test_social_training_large_scene():
     """BPTT through social pooling with a 70-pedestrian scene next to small ones: finite, repeatable,
-    and the primaries' loss matches the value the oracle computes for the same forward."""
-    from trajnetplusplusbaselines_b200.lstm import PredictionLoss
-    rng = np.random.RandomState(3)
-    sizes = [70, 2, 25]
-    xs = [rng.randn(n, 2)[None] * 3.0 + np.cumsum(rng.randn(21, n, 2) * 0.3, axis=0) for n in sizes]
-    xy = np.concatenate(xs, axis=1).astype(np.float32)
-    bs = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
+    and the primaries' loss matches the value the oracle computes for the same forward (default weights;
+    the gradients of this layout are compared with the float64 restatement in test_social_backward.py)."""
+    xy, bs = O.scenes_of_sizes([70, 2, 25], seed=3)
     W = O.random_weights("social", seed=6)
     m1, loss1 = _cuda_train_step("social", W, xy, bs)
     m2, loss2 = _cuda_train_step("social", W, xy, bs)

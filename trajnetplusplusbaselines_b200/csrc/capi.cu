@@ -217,6 +217,7 @@ int tb2_lstm_create(const tb2_lstm_config* cfg, tb2_lstm** out) {
     m->H = cfg->hidden_dim;
     m->E = cfg->embedding_dim;
     m->weights_set = false;
+    m->tc_disabled = tensor_cores_disabled();
     m->C = 0; m->cells = 0; m->n_mlp = 0; m->P = 0; m->pool_out = 0;
     m->We = m->be = m->Wn = m->bn = m->WencT = m->benc = m->Wt1 = m->base1 = nullptr;
     m->Wt1_hi = m->Wt1_lo = nullptr;
@@ -307,7 +308,7 @@ int tb2_lstm_create(const tb2_lstm_config* cfg, tb2_lstm** out) {
         ALLOC(m->WgT[ph], (size_t)m->K_gate_pad * 4 * m->H);
         ALLOC(m->bg[ph], 4 * m->H);
     }
-    const bool no_tc = tensor_cores_disabled();
+    const bool no_tc = m->tc_disabled;
     if (!no_tc && gates_tc_supported(m)) {
         const size_t half = ((size_t)4 * m->H * m->K_gate + 1) / 2;
         for (int ph = 0; ph < 2; ++ph) {

@@ -115,6 +115,7 @@ struct tb2_lstm {
     int mlp_dims[tb2::kMaxMlpLayers + 1];  // [grid_dim, d1, ..]
     int K_gate, K_gate_pad;
     bool weights_set;
+    bool tc_disabled;      // TB2_DISABLE_TC=1 at creation: every kernel choice takes the fp32 FFMA version
     // device buffers (owned)
     float* We;             // [E-2, 2]
     float* be;             // [E-2]

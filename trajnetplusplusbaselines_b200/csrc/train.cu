@@ -1361,7 +1361,8 @@ static size_t carve_social(const tb2_lstm* m, const tb2_layout* l, size_t S, voi
 template <int C>
 static int social_pair_kernels(const tb2_lstm* m, const tb2_layout* l, const SocBuffers& b, const float* lat,
                                int nm1, int d1, cudaStream_t st) {
-    if (C == 16 && d1 % 32 == 0 && b.Wt1_hi != nullptr && dgrid_mma_smem(d1) <= 200 * 1024) {
+    const bool mma = C == 16 && d1 % 32 == 0 && !m->tc_disabled;
+    if (mma && b.Wt1_hi != nullptr && dgrid_mma_smem(d1) <= 200 * 1024) {
         static DynSmemConfig configured;
         TB2_CHECK_CUDA(configured.ensure(social_dgrid_mma_kernel, dgrid_mma_smem(d1), 48 * 1024));
         KernelTimer kt("social_dgrid_mma", st);
@@ -1373,7 +1374,7 @@ static int social_pair_kernels(const tb2_lstm* m, const tb2_layout* l, const Soc
             b.sorted, b.start, b.DH1, d1, m->Wt1, nm1, b.DGRID);
     }
     TB2_LAUNCH_CHECK();
-    if (C == 16 && d1 % 32 == 0) {
+    if (mma) {
         KernelTimer kt("social_dw1_mma", st);
         social_dw1_mma_kernel<<<dim3(m->cells, (d1 + 255) / 256), 256, 0, st>>>(
             b.sorted, b.start, nm1, l->row_scene, l->scene_off, lat, b.DH1, d1, b.dWt1);
@@ -1464,8 +1465,8 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
     }
     // The row GEMMs (rows = all tracks) run on the 3-pass wgmma kernel of the forward (dense_layer_tc_kernel:
     // Y = A . W^T + bias, bf16 (hi, lo) operands, fp32 accumulation) when the shapes allow it: A and the (transposed)
-    // weights are split once, the outputs stay fp32.  Other shapes: cuBLAS / FFMA GEMMs.
-    const bool tcg = K == EP + 128 && dense_tc_supported(K, 512) && dense_tc_supported(512, 128) &&
+    // weights are split once, the outputs stay fp32.  Other shapes, and TB2_DISABLE_TC=1: cuBLAS / FFMA GEMMs.
+    const bool tcg = !m->tc_disabled && K == EP + 128 && dense_tc_supported(K, 512) && dense_tc_supported(512, 128) &&
                      dense_tc_supported(512, EP) && (!two || dense_tc_supported(P, d1));
     if (tcg) {
         TB2_CHECK_CUDA(cudaMemsetAsync(b.zero_bias, 0, (size_t)(d1 > 512 ? d1 : 512) * sizeof(float), st));
