@@ -576,12 +576,16 @@ __global__ void __launch_bounds__(kL1Threads, 1) sparse_layer1_kernel(L1Params p
 //   neighbours) and the cell's weight slab is B [16 x 256]; pairs-per-cell is ~10, far below the
 //   64-row minimum of wgmma, so this irregular piece uses warp-level
 //   mma.sync.m16n8k16 (bf16 inputs, fp32 accumulate) with the same 3-pass (hi, lo) split as the
-//   dense layers.  Warp w owns output columns [32w, 32w+32) of the chunk for ALL pedestrians of
-//   the scene group, so accumulator rows are never shared between warps: no atomics, no
-//   barriers inside the cell loop, deterministic ascending-cell summation.
+//   dense layers.  Warp w owns output columns [16w, 16w+16) of the chunk (two n-tiles) for ALL
+//   pedestrians of the scene group, so accumulator rows are never shared between warps: no
+//   atomics, no barriers inside the cell loop, deterministic ascending-cell summation.
+//   Per cell a warp runs a short dependent chain (entry -> A fragments -> 3 mma -> accumulator
+//   read-modify-write) for ~1 tile; 16 warps of 2 n-tiles give each scheduler 4 such chains to
+//   interleave where 8 warps of 4 n-tiles gave it 2, at the price of loading each A fragment
+//   twice as often (see DESIGN §8 for what bounds the kernel).
 //   smem: acc[P][264] fp32 | lat_hi, lat_lo [P+1][16] bf16 (k-permuted) | buckets | entries
 //   Weights: Wt_hi / Wt_lo [cell][OUT][16] bf16, k permuted so a lane's B fragment is one 8-byte
-//   load (position 4t..4t+3 = k {2t, 2t+1, 2t+8, 2t+9}); next cell's fragments are prefetched.
+//   load (position 4t..4t+3 = k {2t, 2t+1, 2t+8, 2t+9}).
 // ------------------------------------------------------------------------------------------
 constexpr int kMmaAccStride = kL1Cols + 8;
 
@@ -604,7 +608,8 @@ struct L1MmaParams {
     float constant;
 };
 
-constexpr int kMmaThreads = 256;          // 8 warps x 32 output columns
+constexpr int kMmaThreads = 512;          // 16 warps x 16 output columns
+constexpr int kMmaDepth = 8;              // cells of B fragments a lane has requested ahead of use (4 and 12: within 2 %)
 
 __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1MmaParams p) {
     extern __shared__ __align__(16) unsigned char smem_l1m[];
@@ -648,10 +653,9 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
         latH[dst] = h;
         latL[dst] = __float2bfloat16_rn(v - __bfloat162float(h));
     }
-    {
-        const int col = chunk0 + tid;                     // 256 threads = 256 columns of the chunk
-        const float b = col < p.OUT ? p.base[col] : 0.f;
-        for (int r = 0; r < P; ++r) acc[r * kMmaAccStride + tid] = b;
+    for (int idx = tid; idx < P * kL1Cols; idx += kMmaThreads) {
+        const int r = idx / kL1Cols, c = idx % kL1Cols;
+        acc[r * kMmaAccStride + c] = chunk0 + c < p.OUT ? p.base[chunk0 + c] : 0.f;
     }
     __syncthreads();
     const int total = P * p.nm1;
@@ -695,18 +699,18 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
     // padding rows of a tile: zero latent row, per-lane dummy accumulator rows
     const uint32_t dummy0 = ((uint32_t)(p.cap + 1) << 16) | (uint32_t)(p.cap + g);
     const uint32_t dummy1 = ((uint32_t)(p.cap + 1) << 16) | (uint32_t)(p.cap + 8 + g);
-    // this lane loads, for n-tile j (j = 0..3), column chunk0 + 32 warp + 8 j + g
-    const int ncol0 = chunk0 + warp * 32 + g;
+    // this lane loads, for n-tile j (j = 0, 1), column chunk0 + 16 warp + 8 j + g
+    const int ncol0 = chunk0 + warp * 16 + g;
     const size_t cell_stride = (size_t)p.OUT * 32;       // bf16 elements per cell (hi + lo interleaved)
     const __nv_bfloat16* wh = p.Wt_hi + (size_t)ncol0 * 32 + 8 * t;
-    bool okc[4];
+    bool okc[2];
 #pragma unroll
-    for (int j = 0; j < 4; ++j) okc[j] = ncol0 + 8 * j < p.OUT;
-    struct BFrag { uint2 h[4], l[4]; };
+    for (int j = 0; j < 2; ++j) okc[j] = ncol0 + 8 * j < p.OUT;
+    struct BFrag { uint2 h[2], l[2]; };
     auto load_b = [&](const __nv_bfloat16* w) -> BFrag {      // w: this lane's fragments of one cell
         BFrag f;
 #pragma unroll
-        for (int j = 0; j < 4; ++j) {
+        for (int j = 0; j < 2; ++j) {
             // one 16-byte L2 load per n-tile: (hi.x, hi.y, lo.x, lo.y) fragments of column ncol0 + 8 j
             const uint4 v = okc[j] ? __ldcg(reinterpret_cast<const uint4*>(w + (size_t)j * 8 * 32))
                                    : make_uint4(0u, 0u, 0u, 0u);
@@ -715,7 +719,7 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
         }
         return f;
     };
-    float* accw = acc + warp * 32 + 2 * t;
+    float* accw = acc + warp * 16 + 2 * t;
     const uint32_t* latHw = reinterpret_cast<const uint32_t*>(latH) + 2 * t;   // 32-bit words: row stride 8
     const uint32_t* latLw = reinterpret_cast<const uint32_t*>(latL) + 2 * t;
     auto process = [&](int e0, int e1, const BFrag& b) {
@@ -730,7 +734,7 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
             float* a0 = accw + (en0 & 0xffffu) * kMmaAccStride;
             float* a1 = accw + (en1 & 0xffffu) * kMmaAccStride;
 #pragma unroll
-            for (int j = 0; j < 4; ++j) {
+            for (int j = 0; j < 2; ++j) {
                 float d[4] = {0.f, 0.f, 0.f, 0.f};
                 mma_bf16_16816(d, ah, b.h[j].x, b.h[j].y);
                 mma_bf16_16816(d, ah, b.l[j].x, b.l[j].y);
@@ -743,48 +747,36 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
             }
         }
     };
-    // register ring of 4 fragment sets: the slab of cell c+4 is requested right after cell c is
-    // consumed, i.e. three cell-times ahead of its use
+    // register ring of kMmaDepth fragment sets: the slab of cell c + kMmaDepth is requested right
+    // after cell c is consumed.  The requested slab advances by one cell per request: a loop-carried
+    // pointer keeps ptxas from recomputing the addresses from the kernel parameters every cell.
     const int nc = p.cells;
-    BFrag b0 = load_b(wh);
-    BFrag b1 = load_b(wh + (size_t)min(1, nc - 1) * cell_stride);
-    BFrag b2 = load_b(wh + (size_t)min(2, nc - 1) * cell_stride);
-    BFrag b3 = load_b(wh + (size_t)min(3, nc - 1) * cell_stride);
-    // the slab requested next (cell + 4) advances by one cell per request: a loop-carried pointer keeps ptxas from
-    // recomputing the addresses from the kernel parameters every cell
-    const __nv_bfloat16* wnext = wh + 4 * cell_stride;
-    for (int cell = 0; cell < nc; cell += 4) {
-        process(start[cell], start[cell + 1], b0);
-        if (cell + 4 < nc) { b0 = load_b(wnext); wnext += cell_stride; }
-        if (cell + 1 < nc) {
-            process(start[cell + 1], start[cell + 2], b1);
-            if (cell + 5 < nc) { b1 = load_b(wnext); wnext += cell_stride; }
-        }
-        if (cell + 2 < nc) {
-            process(start[cell + 2], start[cell + 3], b2);
-            if (cell + 6 < nc) { b2 = load_b(wnext); wnext += cell_stride; }
-        }
-        if (cell + 3 < nc) {
-            process(start[cell + 3], start[cell + 4], b3);
-            if (cell + 7 < nc) { b3 = load_b(wnext); wnext += cell_stride; }
+    BFrag b[kMmaDepth];
+#pragma unroll
+    for (int i = 0; i < kMmaDepth; ++i) b[i] = load_b(wh + (size_t)min(i, nc - 1) * cell_stride);
+    const __nv_bfloat16* wnext = wh + kMmaDepth * cell_stride;
+    for (int cell = 0; cell < nc; cell += kMmaDepth) {
+#pragma unroll
+        for (int i = 0; i < kMmaDepth; ++i) {
+            if (cell + i < nc) {
+                process(start[cell + i], start[cell + i + 1], b[i]);
+                if (cell + i + kMmaDepth < nc) { b[i] = load_b(wnext); wnext += cell_stride; }
+            }
         }
     }
     __syncthreads();
-    {
-        const int col = chunk0 + tid;
-        if (col < p.OUT) {
-            for (int r = 0; r < P; ++r) {
-                float v = acc[r * kMmaAccStride + tid];
-                if (p.relu) v = fmaxf(v, 0.f);
-                const size_t o = (size_t)(row0 + r) * p.OUT + col;
-                if (p.out_hi) {
-                    const __nv_bfloat16 h = __float2bfloat16_rn(v);
-                    p.out_hi[o] = h;
-                    p.out_lo[o] = __float2bfloat16_rn(v - __bfloat162float(h));
-                } else {
-                    p.out[o] = v;
-                }
-            }
+    for (int idx = tid; idx < P * kL1Cols; idx += kMmaThreads) {
+        const int r = idx / kL1Cols, col = chunk0 + idx % kL1Cols;
+        if (col >= p.OUT) continue;
+        float v = acc[r * kMmaAccStride + idx % kL1Cols];
+        if (p.relu) v = fmaxf(v, 0.f);
+        const size_t o = (size_t)(row0 + r) * p.OUT + col;
+        if (p.out_hi) {
+            const __nv_bfloat16 h = __float2bfloat16_rn(v);
+            p.out_hi[o] = h;
+            p.out_lo[o] = __float2bfloat16_rn(v - __bfloat162float(h));
+        } else {
+            p.out[o] = v;
         }
     }
 }
@@ -797,6 +789,20 @@ static size_t l1_mma_smem_bytes(int cap, int cells, int nm1) {
     b += (size_t)cap * nm1 * sizeof(uint32_t);            // raw winner lists
     b += (size_t)cap * 2 * sizeof(int);                   // winners per row, scene base per row
     return b + 16;
+}
+
+static DynSmemConfig l1_mma_smem_config;
+
+// Launch geometry of sparse_layer1_mma at a scene-group cap: output columns per CTA, threads per CTA and how many
+// CTAs fit on one SM (scripts/layer1_bench.py reports them).
+int layer1_mma_info(int cap, int cells, int nm1, int* chunk_cols, int* threads, int* ctas_per_sm) {
+    const size_t sm = l1_mma_smem_bytes(cap, cells, nm1);
+    TB2_REQUIRE(sm <= 227 * 1024, "scene group does not fit in shared memory (scene too large)");
+    TB2_CHECK_CUDA(l1_mma_smem_config.ensure(sparse_layer1_mma_kernel, sm));
+    TB2_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, sparse_layer1_mma_kernel, kMmaThreads, sm));
+    *chunk_cols = kL1Cols;
+    *threads = kMmaThreads;
+    return TB2_OK;
 }
 
 // weight repack for the mma path: W1[o][c * cells + cell] -> (hi, lo)[cell][o][kperm(c)]
@@ -1129,8 +1135,7 @@ int launch_pool_mlp(const tb2_lstm* m, const tb2_layout* l, Workspace* ws, float
         q.base = m->base1; q.out = p.out; q.out_hi = p.out_hi; q.out_lo = p.out_lo;
         q.OUT = d1; q.cells = m->cells; q.nm1 = nm1; q.cap = l->group_cap[gm]; q.relu = 1;
         q.constant = m->cfg.constant;
-        static DynSmemConfig configured;
-        TB2_CHECK_CUDA(configured.ensure(sparse_layer1_mma_kernel, sm));
+        TB2_CHECK_CUDA(l1_mma_smem_config.ensure(sparse_layer1_mma_kernel, sm));
         dim3 grid(l->num_groups[gm], (d1 + kL1Cols - 1) / kL1Cols);
         {
             KernelTimer kt("sparse_layer1_mma", st);
