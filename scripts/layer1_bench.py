@@ -5,11 +5,18 @@
 Runs the Social-LSTM inference of bench.py (same seeded weights and scenes, an L2 flush between forwards) and times
 every sparse_layer1_mma launch with CUDA events (tb2_profile_*).  Beside the time it prints what the launch moves and
 does, computed from the shapes:
-  * L2 weight bytes per call: every CTA walks every cell's (cell, column chunk) slab of the hi/lo weight image, so
-    groups x chunks x cells x slab bytes;
+  * L2 weight bytes per call: every CTA reads the (cell, column chunk) slab of the hi/lo weight image once per
+    16-row tile of its tile list (a cell without pairs is skipped, a cell of several tiles is read once per tile),
+    so groups x chunks x tiles per CTA x slab bytes;
   * the weight stream those bytes make at the measured time;
   * MMA tiles per CTA: 16-row mma.sync tiles of one scene group summed over the cells, from the winners of the
-    observed frames 0, 8 and 20 (the model's own predictions replace them later in the forward);
+    observed frames 0, 8 and 20 (the model's own predictions replace them later in the forward), and the real and
+    padded row slots of those tiles;
+  * a model (not a measurement) of the shared-memory wavefronts of one CTA's tile loop, from the same winners, for
+    the tile layout before the flat tile list (padding rows load the zero latent row and read-modify-write dummy
+    accumulator rows; 32-bit A loads from separate hi / lo rows) and for the current one (padding rows touch no
+    accumulator; one 128-bit (hi, lo) A load per row): per warp access, the larger of the distinct 4-byte words over
+    32 and the most distinct words in one bank, times 16 warps;
   * CTAs per SM (cudaOccupancyMaxActiveBlocksPerMultiprocessor), hence the number of waves.
 Prints one JSON line with the GPU's name and power limit.
 """
@@ -31,8 +38,9 @@ GROUP_CAP = 160            # rows of a scene group at the benchmark's shape (tb2
 SLAB_BYTES_PER_COL = 64    # 16 latent channels x (hi, lo) bf16
 
 
-def winners_per_cell(xy, bs, cfg):
-    """[rows, cells] bool: row i has a winning (in-range) writer in the cell at the frame xy [M, 2]."""
+def winners_per_cell(xy, bs, cfg, with_writer=False):
+    """[rows, cells] bool: row i has a winning (in-range) writer in the cell at the frame xy [M, 2].  with_writer:
+    also the winner's scene-local pedestrian index [rows, cells]."""
     from oracle import lstm_oracle as O
     B = len(bs) - 1
     obs = xy.reshape(B, PEDS, 2)
@@ -46,6 +54,9 @@ def winners_per_cell(xy, bs, cfg):
     win = last >= 0
     r = np.arange(rows)[:, None]
     win &= in_range[r, np.maximum(last, 0)]
+    if with_writer:
+        i = np.arange(rows)[:, None] % PEDS
+        return win, last + (last >= i)                         # neighbour slot jj -> pedestrian j (diagonal removed)
     return win
 
 
@@ -57,6 +68,64 @@ def tiles_per_cta(xy_frames, bs, cfg):
         per_group = win.reshape(-1, groups * PEDS, win.shape[1]).sum(axis=1)      # [groups, cells] pairs
         out.append(float(np.ceil(per_group / 16.0).sum(axis=1).mean()))
     return float(np.mean(out))
+
+
+def tile_slots_per_cta(xy_frames, bs, cfg):
+    """(real, padded) row slots of one CTA's 16-row tiles, averaged over the groups and frames."""
+    groups = GROUP_CAP // PEDS
+    real, padded = [], []
+    for xy in xy_frames:
+        per_group = winners_per_cell(xy, bs, cfg).reshape(-1, groups * PEDS, cfg.n * cfg.n).sum(axis=1)
+        real.append(per_group.sum(axis=1).mean())
+        padded.append((16 * np.ceil(per_group / 16.0)).sum(axis=1).mean())
+    return float(np.mean(real)), float(np.mean(padded))
+
+
+def _wavefronts(words):
+    """Modelled wavefronts of one warp access touching the 4-byte shared-memory words `words`."""
+    if not words:
+        return 0
+    words = set(words)
+    return max(-(-len(words) // 32), int(np.bincount([w % 32 for w in words], minlength=32).max()))
+
+
+def wavefronts_per_cta(xy_frames, bs, cfg):
+    """(before, after) modelled shared-memory wavefronts of one CTA's tile loop (see the module docstring)."""
+    stride, cap, cells = 264, GROUP_CAP, cfg.n * cfg.n
+    rows_per_group = GROUP_CAP // PEDS * PEDS
+    tot = np.zeros(2)
+    n = 0
+    for xy in xy_frames:
+        win, writer = winners_per_cell(xy, bs, cfg, with_writer=True)
+        lat_row = writer + (np.arange(len(win)) // PEDS * PEDS % rows_per_group)[:, None]    # group-local row of j
+        for grp in range(len(win) // rows_per_group):
+            sl = slice(grp * rows_per_group, (grp + 1) * rows_per_group)
+            w, lr = win[sl], lat_row[sl]
+            for cell in range(cells):
+                rows = np.nonzero(w[:, cell])[0]
+                for e0 in range(0, len(rows), 16):
+                    slot = [(int(r), int(lr[r, cell])) for r in rows[e0:e0 + 16]]
+                    slot += [None] * (16 - len(slot))
+                    ent = 2                                      # two 32-bit slot-word loads, 8 words each
+                    old_a = new_a = old_acc = new_acc = 0
+                    for half in (0, 1):
+                        s8 = slot[8 * half:8 * half + 8]
+                        lat_old = [cap + 1 if e is None else e[1] for e in s8]
+                        for base in (0, (cap + 2) * 8):         # lat_hi, lat_lo: words 2t, 2t + 1 of 8-word rows
+                            for c in (0, 1):
+                                old_a += _wavefronts([base + 8 * l + 2 * t + c for l in lat_old for t in range(4)])
+                        # (hi, lo) of a row and lane t in 16 bytes: 16-word rows, one 128-bit load per row
+                        new_a += _wavefronts([16 * l + 4 * t + c for l in lat_old for t in range(4) for c in range(4)])
+                        for j in (0, 1):
+                            acc_old = [cap + 8 * half + g if e is None else e[0] for g, e in enumerate(s8)]
+                            acc_new = [e[0] for e in s8 if e is not None]
+                            old_acc += 2 * _wavefronts([r * stride + 8 * j + 2 * t + c for r in acc_old
+                                                        for t in range(4) for c in (0, 1)])
+                            new_acc += 2 * _wavefronts([r * stride + 8 * j + 2 * t + c for r in acc_new
+                                                        for t in range(4) for c in (0, 1)])
+                    tot += (ent + old_a + old_acc, ent + new_a + new_acc)
+            n += 1
+    return tuple(float(v) * 16 / n for v in tot)
 
 
 def main():
@@ -104,9 +173,13 @@ def main():
     _lib.check(info(GROUP_CAP, cells, nm1, ctypes.byref(chunk), ctypes.byref(threads), ctypes.byref(per_sm)))
     groups = math.ceil(args.scenes * PEDS / GROUP_CAP)
     chunks = math.ceil(d1 / chunk.value)
-    wbytes = groups * chunks * cells * chunk.value * SLAB_BYTES_PER_COL
+    frames = [xy[f] for f in (0, 8, 20)]
+    tiles = tiles_per_cta(frames, bs, cfg)
+    wbytes = groups * chunks * tiles * chunk.value * SLAB_BYTES_PER_COL
     ctas = groups * chunks
     sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    slots = tile_slots_per_cta(frames, bs, cfg)
+    wf = wavefronts_per_cta(frames, bs, cfg)
     gpu = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"],
                          capture_output=True, text=True).stdout.strip()
     print(json.dumps({
@@ -114,7 +187,9 @@ def main():
         "sparse_layer1_mma_us": us, "launches": prof["launches"],
         "grid": {"groups": groups, "chunks": chunks, "chunk_cols": chunk.value, "threads": threads.value, "ctas": ctas},
         "l2_weight_bytes_per_call": wbytes, "weight_stream_tb_s": wbytes / (us * 1e-6) / 1e12,
-        "mma_tiles_per_cta": tiles_per_cta([xy[f] for f in (0, 8, 20)], bs, cfg),
+        "mma_tiles_per_cta": tiles,
+        "tile_slots_per_cta": {"real": slots[0], "padded": slots[1]},
+        "smem_wavefronts_per_cta_model": {"before_tile_list": wf[0], "tile_list": wf[1]},
         "ctas_per_sm": per_sm.value, "sms": sms, "waves": math.ceil(ctas / (per_sm.value * sms))}))
 
 

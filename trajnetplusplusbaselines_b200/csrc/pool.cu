@@ -579,11 +579,15 @@ __global__ void __launch_bounds__(kL1Threads, 1) sparse_layer1_kernel(L1Params p
 //   dense layers.  Warp w owns output columns [16w, 16w+16) of the chunk (two n-tiles) for ALL
 //   pedestrians of the scene group, so accumulator rows are never shared between warps: no
 //   atomics, no barriers inside the cell loop, deterministic ascending-cell summation.
-//   Per cell a warp runs a short dependent chain (entry -> A fragments -> 3 mma -> accumulator
-//   read-modify-write) for ~1 tile; 16 warps of 2 n-tiles give each scheduler 4 such chains to
-//   interleave where 8 warps of 4 n-tiles gave it 2, at the price of loading each A fragment
-//   twice as often (see DESIGN §8 for what bounds the kernel).
-//   smem: acc[P][264] fp32 | lat_hi, lat_lo [P+1][16] bf16 (k-permuted) | buckets | entries
+//   The bucketing pass lays the pairs out as one flat list of 16-row tiles in ascending cell
+//   order: every cell's run starts on a multiple of 16 and its padding slots hold a padding word, so
+//   each tile carries one cell and the cell loop is a fixed-stride loop over the CTA's tiles.
+//   Padding rows read the zero latent row and never touch the accumulators.  The loop
+//   is software-pipelined one tile ahead: tile k+1's slot words and A fragments (read-only in
+//   the loop) are requested before tile k's mma, and tile k's accumulator loads are issued
+//   before its mma results are needed (see DESIGN §8 for what bounds the kernel).
+//   smem: acc[cap][264] fp32 | lat[cap+2][4 t][hi.x, hi.y, lo.x, lo.y] bf16 pairs | buckets |
+//         tiles' cells | padded entries | raw winner lists
 //   Weights: Wt_hi / Wt_lo [cell][OUT][16] bf16, k permuted so a lane's B fragment is one 8-byte
 //   load (position 4t..4t+3 = k {2t, 2t+1, 2t+8, 2t+9}).
 // ------------------------------------------------------------------------------------------
@@ -609,7 +613,11 @@ struct L1MmaParams {
 };
 
 constexpr int kMmaThreads = 512;          // 16 warps x 16 output columns
-constexpr int kMmaDepth = 8;              // cells of B fragments a lane has requested ahead of use (4 and 12: within 2 %)
+constexpr int kMmaDepth = 8;              // tiles of B fragments a lane has requested ahead of use
+
+// Tiles a scene group can need: every cell's run of pairs is rounded up to 16 rows, and the pairs of a group number at
+// most cap * nm1, so the padded list holds at most cap * nm1 + 15 * cells slots.
+__host__ __device__ inline size_t l1_mma_max_tiles(int cap, int cells, int nm1) { return ((size_t)cap * nm1 + (size_t)15 * cells) / 16; }
 
 __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1MmaParams p) {
     extern __shared__ __align__(16) unsigned char smem_l1m[];
@@ -619,29 +627,40 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
     const int row0 = p.scene_off[s0];
     const int P = p.scene_off[s1] - row0;
     const int chunk0 = blockIdx.y * kL1Cols;
+    const size_t max_tiles = l1_mma_max_tiles(p.cap, p.cells, p.nm1);
 
-    // acc rows [0, cap) real, [cap, cap + 16) dummies absorbing the padding rows of an MMA tile;
-    // lat rows [0, cap) real, cap = NaN-padded slot (b_enc), cap + 1 = zeros (padding rows)
-    float* acc = reinterpret_cast<float*>(smem_l1m);                                       // [cap+16][264]
-    __nv_bfloat16* latH = reinterpret_cast<__nv_bfloat16*>(acc + (size_t)(p.cap + 16) * kMmaAccStride);   // [cap+2][16]
-    __nv_bfloat16* latL = latH + (size_t)(p.cap + 2) * 16;
-    int* start = reinterpret_cast<int*>(latL + (size_t)(p.cap + 2) * 16);                  // [cells+1]
+    // lat rows [0, cap) real, cap = NaN-padded slot (b_enc), cap + 1 = zeros (padding slots); a row is 4 x 16 bytes,
+    // lane t's (hi, lo) fragments of k {2t, 2t+1, 2t+8, 2t+9} together, the order of the weight image
+    float* acc = reinterpret_cast<float*>(smem_l1m);                                       // [cap][264]
+    __nv_bfloat16* lat = reinterpret_cast<__nv_bfloat16*>(acc + (size_t)p.cap * kMmaAccStride);   // [cap+2][32]
+    int* start = reinterpret_cast<int*>(lat + (size_t)(p.cap + 2) * 32);                   // [cells+1] padded slot offsets
     int* cursor = start + p.cells + 1;                                                     // [cells]
-    uint32_t* ent = reinterpret_cast<uint32_t*>(cursor + p.cells);                         // [cap*nm1 + 16]: lat row << 16 | acc row
-    uint32_t* raw = ent + (size_t)p.cap * p.nm1 + 16;                                      // [cap*nm1] winner lists as written by pool_prepare
+    uint16_t* tcell = reinterpret_cast<uint16_t*>(cursor + p.cells);                       // [max_tiles] cell of each tile
+    uint32_t* ent = reinterpret_cast<uint32_t*>(tcell + ((max_tiles + 1) & ~(size_t)1));  // [16 (max_tiles + kMmaDepth)]: lat row << 16 | acc row
+    uint32_t* raw = ent + 16 * max_tiles + 16 * kMmaDepth;                                 // [cap*nm1] winner lists as written by pool_prepare
     int* cnt_s = reinterpret_cast<int*>(raw + (size_t)p.cap * p.nm1);                      // [cap] winners per row
     int* sbase = cnt_s + p.cap;                                                            // [cap] first group-local row of the row's scene
 
+    // Before the wait: only the layout and the weights are read.
     for (int c = tid; c < p.cells; c += kMmaThreads) cursor[c] = 0;
+    for (int sb = s0 + warp; sb < s1; sb += kMmaThreads / 32) {
+        const int a = p.scene_off[sb] - row0, b = p.scene_off[sb + 1] - row0;
+        for (int r = a + lane; r < b; r += 32) sbase[r] = a;
+    }
+    for (int idx = tid; idx < P * kL1Cols; idx += kMmaThreads) {
+        const int r = idx / kL1Cols, c = idx % kL1Cols;
+        acc[r * kMmaAccStride + c] = chunk0 + c < p.OUT ? p.base[chunk0 + c] : 0.f;
+    }
+    // win_count / win_ent / lat come from pool_prepare.  The outputs written below are read by the previous step's
+    // dense_layer_tc: that kernel has completed once this wait returns, because every kernel between it and this one
+    // waits for its own predecessor to complete before it can complete.
+    grid_dep_wait();
+    grid_dep_launch();
     // one coalesced pass over the group's winner lists (rows of a group are contiguous in memory)
     for (int r = tid; r < P; r += kMmaThreads) cnt_s[r] = p.win_count[row0 + r];
     {
         const uint32_t* src = p.win_ent + (size_t)row0 * p.nm1;
         for (int idx = tid; idx < P * p.nm1; idx += kMmaThreads) raw[idx] = src[idx];
-    }
-    for (int sb = s0 + warp; sb < s1; sb += kMmaThreads / 32) {
-        const int a = p.scene_off[sb] - row0, b = p.scene_off[sb + 1] - row0;
-        for (int r = a + lane; r < b; r += 32) sbase[r] = a;
     }
     for (int idx = tid; idx < (P + 2) * 16; idx += kMmaThreads) {
         const int r = idx >> 4, k = idx & 15;
@@ -649,15 +668,13 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
         if (r < P) v = p.lat[(size_t)(row0 + r) * 16 + k] - p.constant;
         else if (r == P) v = p.benc[k] - p.constant;
         const __nv_bfloat16 h = __float2bfloat16_rn(v);
-        const int dst = (r < P ? r : p.cap + (r - P)) * 16 + kperm16(k);
-        latH[dst] = h;
-        latL[dst] = __float2bfloat16_rn(v - __bfloat162float(h));
-    }
-    for (int idx = tid; idx < P * kL1Cols; idx += kMmaThreads) {
-        const int r = idx / kL1Cols, c = idx % kL1Cols;
-        acc[r * kMmaAccStride + c] = chunk0 + c < p.OUT ? p.base[chunk0 + c] : 0.f;
+        const int kp = kperm16(k);                                    // = 4 t + i
+        const int dst = (r < P ? r : p.cap + (r - P)) * 32 + (kp >> 2) * 8 + (kp & 3);
+        lat[dst] = h;
+        lat[dst + 4] = __float2bfloat16_rn(v - __bfloat162float(h));
     }
     __syncthreads();
+    const uint32_t pad = ((uint32_t)(p.cap + 1) << 16) | 0xffffu;    // padding slot: zero lat row, no accumulator row
     const int total = P * p.nm1;
     for (int idx = tid; idx < total; idx += kMmaThreads) {
         int r = idx / p.nm1, k = idx - r * p.nm1;
@@ -665,10 +682,12 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
     }
     __syncthreads();
     if (tid < 32) {
+        // exclusive scan of the cells' pair counts rounded up to whole tiles; each lane marks the padding slots and
+        // the tiles of its cells
         int per = (p.cells + 31) / 32;
         int lo = tid * per, hi = min(lo + per, p.cells);
         int sum = 0;
-        for (int c = lo; c < hi; ++c) sum += cursor[c];
+        for (int c = lo; c < hi; ++c) sum += (cursor[c] + 15) & ~15;
         int incl = sum;
         for (int d = 1; d < 32; d <<= 1) {
             int v = __shfl_up_sync(0xffffffffu, incl, d);
@@ -676,12 +695,19 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
         }
         int run = incl - sum;
         for (int c = lo; c < hi; ++c) {
-            int cnt = cursor[c];
+            const int cnt = cursor[c], padded = (cnt + 15) & ~15;
             start[c] = run;
             cursor[c] = run;
-            run += cnt;
+            for (int s = run + cnt; s < run + padded; ++s) ent[s] = pad;
+            for (int k = run >> 4; k < (run + padded) >> 4; ++k) tcell[k] = (uint16_t)c;
+            run += padded;
         }
-        if (tid == 31) start[p.cells] = incl;
+        // the list runs on in all-padding tiles to a whole number of kMmaDepth-tile rounds, and one tile beyond
+        // for the loop's look-ahead
+        const int slots = __shfl_sync(0xffffffffu, incl, 31);
+        const int end = 16 * (((slots >> 4) + kMmaDepth - 1) / kMmaDepth * kMmaDepth + 1);
+        for (int s = slots + tid; s < end; s += 32) ent[s] = pad;
+        if (tid == 31) start[p.cells] = slots;
     }
     __syncthreads();
     for (int idx = tid; idx < total; idx += kMmaThreads) {
@@ -696,72 +722,80 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
     }
     __syncthreads();
 
-    // padding rows of a tile: zero latent row, per-lane dummy accumulator rows
-    const uint32_t dummy0 = ((uint32_t)(p.cap + 1) << 16) | (uint32_t)(p.cap + g);
-    const uint32_t dummy1 = ((uint32_t)(p.cap + 1) << 16) | (uint32_t)(p.cap + 8 + g);
+    const int tiles = start[p.cells] >> 4;
     // this lane loads, for n-tile j (j = 0, 1), column chunk0 + 16 warp + 8 j + g
     const int ncol0 = chunk0 + warp * 16 + g;
-    const size_t cell_stride = (size_t)p.OUT * 32;       // bf16 elements per cell (hi + lo interleaved)
+    const uint32_t cell_stride = (uint32_t)p.OUT * 32;   // bf16 elements per cell (hi + lo interleaved)
     const __nv_bfloat16* wh = p.Wt_hi + (size_t)ncol0 * 32 + 8 * t;
     bool okc[2];
 #pragma unroll
     for (int j = 0; j < 2; ++j) okc[j] = ncol0 + 8 * j < p.OUT;
     struct BFrag { uint2 h[2], l[2]; };
-    auto load_b = [&](const __nv_bfloat16* w) -> BFrag {      // w: this lane's fragments of one cell
+    auto load_b = [&](int cell) -> BFrag {      // this lane's fragments of one cell
+        const __nv_bfloat16* w = wh + (uint32_t)cell * cell_stride;
         BFrag f;
 #pragma unroll
         for (int j = 0; j < 2; ++j) {
             // one 16-byte L2 load per n-tile: (hi.x, hi.y, lo.x, lo.y) fragments of column ncol0 + 8 j
-            const uint4 v = okc[j] ? __ldcg(reinterpret_cast<const uint4*>(w + (size_t)j * 8 * 32))
+            const uint4 v = okc[j] ? __ldcg(reinterpret_cast<const uint4*>(w + j * 8 * 32))
                                    : make_uint4(0u, 0u, 0u, 0u);
             f.h[j] = make_uint2(v.x, v.y);
             f.l[j] = make_uint2(v.z, v.w);
         }
         return f;
     };
-    float* accw = acc + warp * 16 + 2 * t;
-    const uint32_t* latHw = reinterpret_cast<const uint32_t*>(latH) + 2 * t;   // 32-bit words: row stride 8
-    const uint32_t* latLw = reinterpret_cast<const uint32_t*>(latL) + 2 * t;
-    auto process = [&](int e0, int e1, const BFrag& b) {
-        for (int eb = e0; eb < e1; eb += 16) {
-            const int i0 = eb + g, i1 = i0 + 8;
-            const uint32_t en0 = i0 < e1 ? ent[i0] : dummy0;
-            const uint32_t en1 = i1 < e1 ? ent[i1] : dummy1;
-            const uint32_t l0 = (en0 >> 16) * 8, l1 = (en1 >> 16) * 8;
-            uint32_t ah[4], al[4];
-            ah[0] = latHw[l0]; ah[1] = latHw[l1]; ah[2] = latHw[l0 + 1]; ah[3] = latHw[l1 + 1];
-            al[0] = latLw[l0]; al[1] = latLw[l1]; al[2] = latLw[l0 + 1]; al[3] = latLw[l1 + 1];
-            float* a0 = accw + (en0 & 0xffffu) * kMmaAccStride;
-            float* a1 = accw + (en1 & 0xffffu) * kMmaAccStride;
-#pragma unroll
-            for (int j = 0; j < 2; ++j) {
-                float d[4] = {0.f, 0.f, 0.f, 0.f};
-                mma_bf16_16816(d, ah, b.h[j].x, b.h[j].y);
-                mma_bf16_16816(d, ah, b.l[j].x, b.l[j].y);
-                mma_bf16_16816(d, al, b.h[j].x, b.h[j].y);
-                float2* q0 = reinterpret_cast<float2*>(a0 + 8 * j);
-                float2* q1 = reinterpret_cast<float2*>(a1 + 8 * j);
-                float2 u0 = *q0, u1 = *q1;
-                u0.x += d[0]; u0.y += d[1]; u1.x += d[2]; u1.y += d[3];
-                *q0 = u0; *q1 = u1;
-            }
-        }
+    // one tile's slot words and A fragments (rows g and g + 8)
+    struct Tile { uint32_t e0, e1; uint4 a0, a1; };
+    const uint4* latT = reinterpret_cast<const uint4*>(lat) + t;
+    auto fetch = [&](int k) -> Tile {
+        Tile f;
+        f.e0 = ent[16 * k + g];
+        f.e1 = ent[16 * k + 8 + g];
+        f.a0 = latT[(f.e0 >> 16) * 4];
+        f.a1 = latT[(f.e1 >> 16) * 4];
+        return f;
     };
-    // register ring of kMmaDepth fragment sets: the slab of cell c + kMmaDepth is requested right
-    // after cell c is consumed.  The requested slab advances by one cell per request: a loop-carried
-    // pointer keeps ptxas from recomputing the addresses from the kernel parameters every cell.
-    const int nc = p.cells;
+    float* accw = acc + warp * 16 + 2 * t;
+    // register ring of kMmaDepth fragment sets: the slab of tile k + kMmaDepth is requested right after tile k is
+    // consumed (a cell of several tiles requests its slab once per tile)
     BFrag b[kMmaDepth];
 #pragma unroll
-    for (int i = 0; i < kMmaDepth; ++i) b[i] = load_b(wh + (size_t)min(i, nc - 1) * cell_stride);
-    const __nv_bfloat16* wnext = wh + kMmaDepth * cell_stride;
-    for (int cell = 0; cell < nc; cell += kMmaDepth) {
+    for (int i = 0; i < kMmaDepth; ++i) b[i] = load_b(i < tiles ? tcell[i] : 0);
+    Tile cur = fetch(0);
+    for (int k0 = 0; k0 < tiles; k0 += kMmaDepth) {
 #pragma unroll
         for (int i = 0; i < kMmaDepth; ++i) {
-            if (cell + i < nc) {
-                process(start[cell + i], start[cell + i + 1], b[i]);
-                if (cell + i + kMmaDepth < nc) { b[i] = load_b(wnext); wnext += cell_stride; }
+            const int k = k0 + i;                   // k >= tiles: an all-padding tile
+            const bool v0 = (cur.e0 & 0xffffu) != 0xffffu, v1 = (cur.e1 & 0xffffu) != 0xffffu;
+            float2* q0 = reinterpret_cast<float2*>(accw + (cur.e0 & 0xffffu) * kMmaAccStride);
+            float2* q1 = reinterpret_cast<float2*>(accw + (cur.e1 & 0xffffu) * kMmaAccStride);
+            // Accumulators of tile k, all loaded before any is stored: a row occurs at most once per cell, so rows
+            // g and g + 8 of a tile are different rows, and n-tiles j = 0 (q[0]) and j = 1 (q[4]) are different
+            // columns.  They come after tile k - 1's stores, which may hold the same rows.
+            float2 u00, u01, u10, u11;
+            if (v0) { u00 = q0[0]; u01 = q0[4]; }
+            if (v1) { u10 = q1[0]; u11 = q1[4]; }
+            const Tile nxt = fetch(k + 1);
+            const uint32_t ah[4] = {cur.a0.x, cur.a1.x, cur.a0.y, cur.a1.y};
+            const uint32_t al[4] = {cur.a0.z, cur.a1.z, cur.a0.w, cur.a1.w};
+            float d[2][4];
+#pragma unroll
+            for (int j = 0; j < 2; ++j) {
+                d[j][0] = d[j][1] = d[j][2] = d[j][3] = 0.f;
+                mma_bf16_16816(d[j], ah, b[i].h[j].x, b[i].h[j].y);
+                mma_bf16_16816(d[j], ah, b[i].l[j].x, b[i].l[j].y);
+                mma_bf16_16816(d[j], al, b[i].h[j].x, b[i].h[j].y);
             }
+            if (v0) {
+                q0[0] = make_float2(u00.x + d[0][0], u00.y + d[0][1]);
+                q0[4] = make_float2(u01.x + d[1][0], u01.y + d[1][1]);
+            }
+            if (v1) {
+                q1[0] = make_float2(u10.x + d[0][2], u10.y + d[0][3]);
+                q1[4] = make_float2(u11.x + d[1][2], u11.y + d[1][3]);
+            }
+            if (k + kMmaDepth < tiles) b[i] = load_b(tcell[k + kMmaDepth]);
+            cur = nxt;
         }
     }
     __syncthreads();
@@ -782,12 +816,14 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
 }
 
 static size_t l1_mma_smem_bytes(int cap, int cells, int nm1) {
-    size_t b = (size_t)(cap + 16) * kMmaAccStride * sizeof(float);
-    b += (size_t)(cap + 2) * 16 * 2 * sizeof(__nv_bfloat16);
-    b += (size_t)(2 * cells + 1) * sizeof(int);
-    b += ((size_t)cap * nm1 + 16) * sizeof(uint32_t);     // sorted entries
-    b += (size_t)cap * nm1 * sizeof(uint32_t);            // raw winner lists
-    b += (size_t)cap * 2 * sizeof(int);                   // winners per row, scene base per row
+    const size_t tiles = l1_mma_max_tiles(cap, cells, nm1);
+    size_t b = (size_t)cap * kMmaAccStride * sizeof(float);           // accumulators
+    b += (size_t)(cap + 2) * 32 * sizeof(__nv_bfloat16);             // latent rows (hi, lo)
+    b += (size_t)(2 * cells + 1) * sizeof(int);                       // cell starts, cursors
+    b += ((tiles + 1) & ~(size_t)1) * sizeof(uint16_t);               // cell of each tile
+    b += (16 * tiles + 16 * kMmaDepth) * sizeof(uint32_t);            // padded entries + all-padding tiles
+    b += (size_t)cap * nm1 * sizeof(uint32_t);                        // raw winner lists
+    b += (size_t)cap * 2 * sizeof(int);                               // winners per row, scene base per row
     return b + 16;
 }
 
@@ -1128,6 +1164,8 @@ int launch_pool_mlp(const tb2_lstm* m, const tb2_layout* l, Workspace* ws, float
         size_t sm = l1_mma_smem_bytes(l->group_cap[gm], m->cells, nm1);
         if (sm > 227 * 1024) { gm = 1; sm = l1_mma_smem_bytes(l->group_cap[gm], m->cells, nm1); }
         TB2_REQUIRE(sm <= 227 * 1024, "scene group does not fit in shared memory (scene too large)");
+        TB2_REQUIRE(m->cells <= 65536 && (size_t)m->cells * d1 * 32 < ((size_t)1 << 32),
+                    "grid too fine for the tensor-core first layer (16-bit tile cells, 32-bit weight offsets)");
         L1MmaParams q;
         q.group_off = l->group_off[gm]; q.scene_off = l->scene_off; q.win_count = ws->win_count;
         q.win_ent = ws->win_ent; q.lat = ws->lat; q.benc = m->benc;
@@ -1139,7 +1177,7 @@ int launch_pool_mlp(const tb2_lstm* m, const tb2_layout* l, Workspace* ws, float
         dim3 grid(l->num_groups[gm], (d1 + kL1Cols - 1) / kL1Cols);
         {
             KernelTimer kt("sparse_layer1_mma", st);
-            sparse_layer1_mma_kernel<<<grid, kMmaThreads, sm, st>>>(q);
+            launch_pdl(sparse_layer1_mma_kernel, grid, dim3(kMmaThreads), sm, st, q);
         }
         TB2_LAUNCH_CHECK();
         rc = TB2_OK;
