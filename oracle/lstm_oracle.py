@@ -639,6 +639,18 @@ MODEL_SPECS = {
                        embedding_arch="two_layer", layer_dims=[96], latent_dim=16),
     "social_d200": dict(type_="social", hidden_dim=128, cell_side=0.6, n=10, out_dim=128,
                         embedding_arch="two_layer", layer_dims=[200], latent_dim=16),
+    # occupancy / directional training in each configuration the grid backward indexes differently
+    # (tests/test_grid_backward.py): the front offset, grid sizes, pool widths up to the 1024 limit
+    "directional_front": dict(type_="directional", hidden_dim=128, cell_side=0.6, n=12, out_dim=256,
+                              embedding_arch="one_layer", front=True),
+    "occupancy_front_n4": dict(type_="occupancy", hidden_dim=128, cell_side=0.6, n=4, out_dim=256,
+                               embedding_arch="one_layer", front=True),
+    "directional_n24": dict(type_="directional", hidden_dim=128, cell_side=0.6, n=24, out_dim=256,
+                            embedding_arch="one_layer"),
+    "occupancy_p1024": dict(type_="occupancy", hidden_dim=128, cell_side=0.6, n=12, out_dim=1024,
+                            embedding_arch="one_layer"),
+    "directional_p29": dict(type_="directional", hidden_dim=128, cell_side=0.6, n=12, out_dim=29,
+                            embedding_arch="one_layer"),
 }
 
 

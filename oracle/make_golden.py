@@ -34,11 +34,11 @@ CASES = [
 ]
 
 
-def build_reference_model(kind, weights):
+def build_reference_model(kind, weights, embedding_dim=64):
     from trajnetbaselines.lstm import LSTM, GridBasedPooling
     spec = O.MODEL_SPECS[kind]
     pool = GridBasedPooling(**spec) if spec is not None else None
-    model = LSTM(pool=pool)
+    model = LSTM(embedding_dim=embedding_dim, pool=pool)
     sd = {k: torch.from_numpy(v.copy()) for k, v in weights.items()}
     model.load_state_dict(sd, strict=True)
     model.eval()

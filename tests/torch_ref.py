@@ -2,8 +2,8 @@
 
 Used only to check the hand-written CUDA backward (csrc/train.cu).  Follows oracle/lstm_oracle.py (which is
 pinned to the reference) line by line, with torch ops so autograd provides the gradients;
-test_training.py and test_social_backward.py pin THIS file's gradients to gradients of the unmodified
-reference (tests/golden/train_golden.npz, social_train_golden.npz).
+test_training.py, test_social_backward.py and test_grid_backward.py pin THIS file's gradients to gradients
+of the unmodified reference (tests/golden/train_golden.npz, social_train_golden.npz, grid_train_golden.npz).
 """
 import math
 
@@ -95,9 +95,13 @@ def _note(stats, key, value):
 
 
 def forward(W, pool_cfg, observed, batch_split, prediction_truth=None, n_predict=None, hidden_dim=128,
-            dtype=torch.float32, stats=None):
+            dtype=torch.float32, stats=None, feed_back=None):
     """W: dict of `dtype` tensors (requires_grad as wanted).  Returns rel [S, M, 5] (`dtype`), pred [S, M, 2]
-    (fp32: the positions the model feeds back are fp32 data, as in the reference).  stats: see _grid."""
+    (fp32: the positions the model feeds back are fp32 data, as in the reference).  stats: see _grid.
+
+    feed_back: fp32 positions [S(+1), M, 2] of another implementation's forward (aligned with pred).  The
+    decoder is then fed those (detached) positions instead of this forward's own, so the gradients are
+    exact for that implementation's trajectory and no fed-back position can be binned differently."""
     bs = [int(v) for v in batch_split]
     B = len(bs) - 1
     M = observed.shape[1]
@@ -140,6 +144,11 @@ def forward(W, pool_cfg, observed, batch_split, prediction_truth=None, n_predict
     normals, positions = [], []
     if observed.shape[0] == 2:
         positions = [observed[-1]]
+
+    def fed(i):     # the position fed back as step i's input (i < 0 counts from the end)
+        i = i % len(positions)
+        return feed_back[i] if feed_back is not None else positions[i].detach()
+
     for t in range(observed.shape[0] - 1):
         h, c, normal = step("encoder", h, c, observed[t], observed[t + 1])
         normals.append(normal)
@@ -148,15 +157,15 @@ def forward(W, pool_cfg, observed, batch_split, prediction_truth=None, n_predict
     for k in range(len(seq) - 1):
         obs1, obs2 = seq[k], seq[k + 1]
         if obs1 is None:
-            obs1 = positions[-2].detach()
+            obs1 = fed(-2)
         else:
             obs1 = obs1.clone()
-            obs1[prim] = positions[-2][prim].detach()
+            obs1[prim] = fed(-2)[prim]
         if obs2 is None:
-            obs2 = positions[-1].detach()
+            obs2 = fed(-1)
         else:
             obs2 = obs2.clone()
-            obs2[prim] = positions[-1][prim].detach()
+            obs2[prim] = fed(-1)[prim]
             seq[k + 1] = obs2
         h, c, normal = step("decoder", h, c, obs1, obs2)
         normals.append(normal)
@@ -191,8 +200,10 @@ def l2_loss(inputs, targets, batch_split):
     return ((inputs[:, prim][:, :, :2] - targets[:, prim]) ** 2).mean() * 100
 
 
-def collision_loss(positions, batch_split, col_wt=10.0, col_distance=0.2):
-    """Reference lstm/loss.py:138-162: the primary is penalised for neighbours within col_distance."""
+def collision_loss(positions, batch_split, col_wt=10.0, col_distance=0.2, stats=None):
+    """Reference lstm/loss.py:138-162: the primary is penalised for neighbours within col_distance.
+    stats["col_margin"]: the smallest |distance - col_distance| over the primary-neighbour pairs (a pair that
+    crosses col_distance changes the loss continuously but its gradient by ~col_wt / col_distance)."""
     batch_split = [int(v) for v in batch_split]
     pos = torch.where(torch.isnan(positions[..., :2]), torch.full_like(positions[..., :2], -1000.0), positions[..., :2])
     sizes = torch.as_tensor([b - a for a, b in zip(batch_split[:-1], batch_split[1:])])
@@ -201,22 +212,48 @@ def collision_loss(positions, batch_split, col_wt=10.0, col_distance=0.2):
     is_neigh[torch.as_tensor(batch_split[:-1])] = False
     dist = torch.norm(pos[:, prim_of_row] - pos.detach(), dim=-1)[:, is_neigh]
     hit = (dist <= col_distance).detach()
+    if dist.numel():
+        _note(stats, "col_margin", float((dist.detach() - col_distance).abs().min()))
     return col_wt * (1 - dist[hit] / col_distance).sum()
 
 
 def train_loss_and_grads(W_np, pool_cfg, xy, batch_split, obs_length=9, pred_length=12, dtype=torch.float32,
-                         stats=None):
-    """What Trainer.train_batch computes (trainer.py:252-263): teacher-forced forward, PredictionLoss
-    on the last pred_length outputs x batch_size; returns (loss, {name: grad ndarray}).  The weights and
-    the arithmetic are `dtype`; xy stays fp32 (it is data).  stats: see _grid."""
+                         stats=None, loss="pred", col_wt=0.0, col_distance=0.2, feed_back=None, outputs=None):
+    """What Trainer.train_batch computes (trainer.py:252-263): teacher-forced forward, the criterion on the
+    last pred_length outputs x batch_size; returns (loss, {name: grad ndarray}).  The weights and the
+    arithmetic are `dtype`; xy stays fp32 (it is data).  The embedding width is that of W.
+
+    loss: "pred" (PredictionLoss) or "l2" (L2Loss), with the collision term when col_wt > 0 on the
+    trainer's primary_prediction (the data with the primaries replaced by the predicted positions); like
+    the reference, each loss's multiplier (1 / 100) also scales the collision term.  Or a callable
+    loss(rel, positions) -> scalar (not scaled by the batch size).
+    stats: see _grid and collision_loss.  feed_back: see forward.  outputs: dict that receives "positions"."""
     W = {k: torch.tensor(v, dtype=dtype, requires_grad=True) for k, v in W_np.items()}
     xy = torch.tensor(xy)
     observed = xy[:obs_length]
     truth = xy[obs_length:-1]
     targets = (xy[obs_length:obs_length + pred_length] - xy[obs_length - 1:obs_length + pred_length - 1]).to(dtype)
-    rel, _ = forward(W, pool_cfg, observed, batch_split, prediction_truth=truth, dtype=dtype, stats=stats)
-    batch_size = len(batch_split) - 1
-    loss = prediction_loss(rel[-pred_length:], targets, batch_split) * batch_size
-    loss.backward()
+    fb = torch.as_tensor(feed_back) if feed_back is not None else None
+    rel, positions = forward(W, pool_cfg, observed, batch_split, prediction_truth=truth, dtype=dtype, stats=stats,
+                             feed_back=fb)
+    if callable(loss):
+        total = loss(rel, positions)
+    else:
+        batch_size = len(batch_split) - 1
+        if loss == "pred":
+            total, mult = prediction_loss(rel[-pred_length:], targets, batch_split), 1.0
+        elif loss == "l2":
+            total, mult = l2_loss(rel[-pred_length:], targets, batch_split), 100.0
+        else:
+            raise ValueError(loss)
+        if col_wt:
+            prim = torch.tensor([int(v) for v in batch_split[:-1]])
+            primary_prediction = xy[-pred_length:].clone()
+            primary_prediction[:, prim] = positions[-pred_length:, prim]
+            total = total + collision_loss(primary_prediction, batch_split, col_wt, col_distance, stats) * mult
+        total = total * batch_size
+    total.backward()
+    if outputs is not None:
+        outputs["positions"] = positions.detach().numpy()
     grads = {k: (v.grad.numpy() if v.grad is not None else None) for k, v in W.items()}
-    return float(loss.detach()), grads
+    return float(total.detach()), grads

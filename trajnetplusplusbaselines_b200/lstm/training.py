@@ -114,7 +114,10 @@ class _SequenceFn(torch.autograd.Function):
                         _ptr(ctx.truth), n_decode, _ptr(pos_steps), _ptr(ctx.states), _ptr(dn), _ptr(active), R,
                         ctypes.byref(g), _ptr(ws), need, _ptr(bws), bneed, _stream(device)))
             del keep
-        by_param = {id(p): grads[k] for k, p in targets.items()}
+        # a sequence without a decoder step (pred_length 1) never uses the decoder cell: like autograd on the
+        # reference, its parameters get no gradient (None), so optimizers leave them alone
+        unused = ("decoder_",) if S == int(ctx.obs.shape[0]) - 1 else ()
+        by_param = {id(p): grads[k] for k, p in targets.items() if not k.startswith(unused)}
         out = []
         for p in ctx.params:
             gr = by_param.get(id(p))
