@@ -474,6 +474,28 @@ int tb2_orca_simulate(const tb2_layout* layout, const tb2_orca_params* p, const 
                       const float* vel_dev, const double* goal_dev, const double* speed_dev,
                       float* out_dev, void* stream);
 
+/* Parameter sweeps: every scene under every setting in one call, only the primary's ADE / FDE written
+ * (socialforce_eval.py's per-setting re-runs, :236-258, and Evaluator.aggregate's scoring, :25-84).  Work item = (scene,
+ * setting); one CTA per scene runs all its settings, scenes of <= 32 pedestrians packed several settings per warp.  The
+ * rollout is exactly the one of tb2_sf_simulate / tb2_orca_simulate with that setting (same step code).  Scene b's
+ * pedestrian 0 is its primary:
+ *   ade_out[s * B + b] = (sum over samples j, in order, of |truth_j - position_j|) / n_samples   (float64)
+ *   fde_out[s * B + b] = |truth_last - position_last|
+ * truth_dev [B, truth_len, 2] double: the primary's true positions; its last n_samples rows are compared.  NaN propagates
+ * (a social-force primary standing on its destination has a NaN desired direction: its ADE is NaN).  No atomics: reruns
+ * are bit-identical.  Synchronous on `stream` up to the launch: the P x 3 parameters are read back to be checked.
+ * TB2_ERR_INVALID for P < 1, P x B >= 2^31, a non-finite parameter, truth_len < n_samples, and the non-positive values
+ * named below.
+ *   tb2_sf_sweep    params_dev [P, 3] double = tau (> 0), v0, sigma (> 0); the other fields from `p`
+ *   tb2_orca_sweep  params_dev [P, 3] float = neighbor_dist, time_horizon (> 0), radius (> 0); the other fields from
+ *                   `p`; positions widened to double before the difference (orca.py's astype(np.float64)) */
+int tb2_sf_sweep(const tb2_layout* layout, const tb2_sf_params* p, const double* params_dev, int32_t P,
+                 const double* state_dev, const double* truth_dev, int32_t truth_len, double* ade_out_dev,
+                 double* fde_out_dev, void* stream);
+int tb2_orca_sweep(const tb2_layout* layout, const tb2_orca_params* p, const float* params_dev, int32_t P,
+                   const float* pos_dev, const float* vel_dev, const double* goal_dev, const double* speed_dev,
+                   const double* truth_dev, int32_t truth_len, double* ade_out_dev, double* fde_out_dev, void* stream);
+
 /* Kalman predictor, HOST code (BASELINE configs[0] is CPU-only), float64.  Replaces
  * pykalman.KalmanFilter(...).em / .smooth / expected .sample rollout (classical/kalman.py:40-60).
  *   obs_host            [total_obs, 2] observed positions of all tracks, concatenated

@@ -165,6 +165,8 @@ PROTOTYPES = {
     "tb2_sf_simulate": (ctypes.c_int, [_vp, ctypes.POINTER(SfParams), _vp, _vp, _vp]),
     "tb2_kalman_predict": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
     "tb2_orca_simulate": (ctypes.c_int, [_vp, ctypes.POINTER(OrcaParams), _vp, _vp, _vp, _vp, _vp, _vp]),
+    "tb2_sf_sweep": (ctypes.c_int, [_vp, ctypes.POINTER(SfParams), _vp, _i32, _vp, _vp, _i32, _vp, _vp, _vp]),
+    "tb2_orca_sweep": (ctypes.c_int, [_vp, ctypes.POINTER(OrcaParams), _vp, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),
 }
 
 _lib = None

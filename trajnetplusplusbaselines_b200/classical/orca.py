@@ -12,7 +12,7 @@ import torch
 
 from .. import _lib
 from ..engine import SceneLayout, _ptr, _stream
-from .common import initial_states
+from .common import initial_states, sweep_params
 
 MAX_SPEED_MULTIPLIER = 1.3   # applied inside the kernel (orca.py:8,36)
 
@@ -43,6 +43,38 @@ def simulate_batch(pos, vel, goals, speeds, batch_split, orca_params=(1.5, 1.5, 
         _lib.check(lib.tb2_orca_simulate(layout.handle, ctypes.byref(p), _ptr(pos_t), _ptr(vel_t),
                                          _ptr(goal_t), _ptr(speed_t), _ptr(out), _stream(device)))
     return out
+
+
+def sweep(prepared, params, fps=20, max_neighbors=10, end_range=0.05):
+    """ADE / FDE of the primary of every scene of `prepared` (common.PreparedScenes) under every setting of params
+    [P, 3] (neighbor_dist, time_horizon, radius; float32 like RVO2) -> (ade, fde) CUDA float64 [P, B], one launch
+    (tb2_orca_sweep).  Row s equals simulate_batch(...(params[s]), n_steps=sampling_rate * pred_length + 1) with the
+    float positions widened to double and scored against prepared.truth: distances in sample order summed in float64,
+    ADE = sum / pred_length, FDE = the last distance."""
+    B, T = int(prepared.truth.shape[0]), int(prepared.truth.shape[1])
+    prm = sweep_params(params, np.float32, ("neighbor_dist", "time_horizon", "radius"), (1, 2), B)
+    _lib.require_cuda()
+    lib = _lib.load()
+    sampling_rate = int(fps / 2.5)
+    p = _lib.OrcaParams()
+    p.time_step = 1.0 / fps
+    p.neighbor_dist, p.time_horizon, p.radius = (float(v) for v in prm[0])
+    p.max_neighbors = int(max_neighbors)
+    p.end_range = float(end_range)
+    p.n_steps, p.sample_every = sampling_rate * T + 1, sampling_rate
+    device = prepared.state.device
+    st = prepared.state
+    pos = st[:, 0:2].to(torch.float32).contiguous()
+    vel = st[:, 2:4].to(torch.float32).contiguous()
+    goal = st[:, 4:6].contiguous()
+    prm_t = torch.from_numpy(prm).to(device)
+    ade = torch.empty((len(prm), B), dtype=torch.float64, device=device)
+    fde = torch.empty_like(ade)
+    with torch.cuda.device(device):
+        _lib.check(lib.tb2_orca_sweep(prepared.layout.handle, ctypes.byref(p), _ptr(prm_t), len(prm), _ptr(pos), _ptr(vel),
+                                      _ptr(goal), _ptr(prepared.speeds), _ptr(prepared.truth), T, _ptr(ade), _ptr(fde),
+                                      _stream(device)))
+    return ade, fde
 
 
 def predict(input_paths, dest_dict=None, dest_type='interp', orca_params=[1.5, 1.5, 0.4],

@@ -12,7 +12,7 @@ import torch
 
 from .. import _lib
 from ..engine import SceneLayout, _ptr, _stream
-from .common import initial_states
+from .common import initial_states, sweep_params
 
 
 def simulate_batch(states, batch_split, sf_params=(0.5, 2.1, 0.3), n_steps=96, sample_every=8, fps=20,
@@ -35,6 +35,31 @@ def simulate_batch(states, batch_split, sf_params=(0.5, 2.1, 0.3), n_steps=96, s
     with torch.cuda.device(device):
         _lib.check(lib.tb2_sf_simulate(layout.handle, ctypes.byref(p), _ptr(st), _ptr(out), _stream(device)))
     return out
+
+
+def sweep(prepared, params, fps=20):
+    """ADE / FDE of the primary of every scene of `prepared` (common.PreparedScenes) under every setting of params
+    [P, 3] (tau, v0, sigma) -> (ade, fde) CUDA float64 [P, B], one launch (tb2_sf_sweep).  Row s equals
+    simulate_batch(state, agent_offsets, params[s], n_steps=pred_length * sampling_rate, sample_every=sampling_rate)
+    scored against prepared.truth: distances in sample order summed in float64, ADE = sum / pred_length, FDE = the
+    last distance.  The trajectories never reach device memory."""
+    B, T = int(prepared.truth.shape[0]), int(prepared.truth.shape[1])
+    prm = sweep_params(params, np.float64, ("tau", "v0", "sigma"), (0, 2), B)
+    _lib.require_cuda()
+    lib = _lib.load()
+    sampling_rate = int(fps / 2.5)
+    p = _lib.SfParams()
+    p.delta_t = 1.0 / fps
+    p.tau, p.v0, p.sigma = (float(v) for v in prm[0])
+    p.n_steps, p.sample_every = T * sampling_rate, sampling_rate
+    device = prepared.state.device
+    prm_t = torch.from_numpy(prm).to(device)
+    ade = torch.empty((len(prm), B), dtype=torch.float64, device=device)
+    fde = torch.empty_like(ade)
+    with torch.cuda.device(device):
+        _lib.check(lib.tb2_sf_sweep(prepared.layout.handle, ctypes.byref(p), _ptr(prm_t), len(prm), _ptr(prepared.state),
+                                    _ptr(prepared.truth), T, _ptr(ade), _ptr(fde), _stream(device)))
+    return ade, fde
 
 
 def predict(input_paths, dest_dict=None, dest_type='interp', sf_params=[0.5, 2.1, 0.3],

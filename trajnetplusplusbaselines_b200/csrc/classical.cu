@@ -13,6 +13,8 @@
 // CUDA result is comparable operation by operation with the CPU restatement.
 #include <math_constants.h>
 
+#include <cmath>
+
 #include "common.cuh"
 
 namespace tb2 {
@@ -47,6 +49,62 @@ __device__ __forceinline__ void scene_sync() {
     else __syncthreads();
 }
 
+// One pedestrian of a social-force rollout: position, velocity, destination, initial and maximum speed
+// (Simulator.__init__: initial_speeds, max_speeds = 1.3 x).
+struct SfAgent { double x, y, ux, uy, dx, dy, s0, smax; };
+
+__device__ __forceinline__ SfAgent sf_agent_init(const double* st) {
+    SfAgent g;
+    g.x = st[0]; g.y = st[1]; g.ux = st[2]; g.uy = st[3]; g.dx = st[4]; g.dy = st[5];
+    g.s0 = sqrt(g.ux * g.ux + g.uy * g.uy);
+    g.smax = 1.3 * g.s0;
+    return g;
+}
+
+__device__ __forceinline__ double sf_cosphi() { return cos(200.0 / 2.0 / 180.0 * 3.141592653589793); }   // FieldOfView(twophi=200)
+
+// First half of a step: the desired direction (NaN at the destination, as upstream), published with the state for the
+// neighbour loop of every pedestrian of the scene.
+__device__ __forceinline__ void sf_publish(const SfAgent& g, const SfScene& sc, int a, double& eax, double& eay) {
+    const double gx = g.dx - g.x, gy = g.dy - g.y;
+    const double gn = sqrt(gx * gx + gy * gy);
+    eax = gx / gn; eay = gy / gn;
+    sc.px[a] = g.x; sc.py[a] = g.y; sc.vx[a] = g.ux; sc.vy[a] = g.uy; sc.ex[a] = eax; sc.ey[a] = eay;
+    sc.sp[a] = sqrt(g.ux * g.ux + g.uy * g.uy);
+}
+
+// Second half: driving force + pairwise repulsion over b = 0 .. n-1 in index order, speed clip, position update.
+__device__ __forceinline__ void sf_advance(SfAgent& g, const SfScene& sc, int a, int n, double eax, double eay,
+                                           double dt, double tau, double v0, double sigma, double cosphi) {
+    const double fd = 1e-3;
+    double Fx = 1.0 / tau * (g.s0 * eax - g.ux);
+    double Fy = 1.0 / tau * (g.s0 * eay - g.uy);
+    double sumx = 0.0, sumy = 0.0;
+    for (int b = 0; b < n; ++b) {
+        double fx = 0.0, fy = 0.0, w = 0.0;
+        if (b != a) {
+            const double rx = g.x - sc.px[b], ry = g.y - sc.py[b];
+            const double sb = sc.sp[b], ebx = sc.ex[b], eby = sc.ey[b];
+            const double v = sf_potential(rx, ry, sb, ebx, eby, dt, v0, sigma);
+            const double dvdx = (sf_potential(rx + fd, ry, sb, ebx, eby, dt, v0, sigma) - v) / fd;
+            const double dvdy = (sf_potential(rx, ry + fd, sb, ebx, eby, dt, v0, sigma) - v) / fd;
+            fx = -1.0 * dvdx; fy = -1.0 * dvdy;               // f_ab = -grad V
+            const double gx = -fx, gy = -fy;                  // w(e, -f_ab)
+            const bool in_sight = (eax * gx + eay * gy) > sqrt(gx * gx + gy * gy) * cosphi;
+            w = in_sight ? 1.0 : 0.5;
+        }
+        sumx += w * fx;
+        sumy += w * fy;
+    }
+    Fx += sumx; Fy += sumy;
+    const double wx = g.ux + dt * Fx, wy = g.uy + dt * Fy;
+    const double wn = sqrt(wx * wx + wy * wy);
+    const double q = g.smax / wn;
+    const double factor = isnan(q) ? q : (q < 1.0 ? q : 1.0);       // numpy.minimum(1, q)
+    g.ux = wx * factor; g.uy = wy * factor;
+    g.x = g.x + g.ux * dt; g.y = g.y + g.uy * dt;
+}
+
 template <bool kWarpScenes>
 __global__ void sf_simulate_kernel(const int* __restrict__ scene_off, const double* __restrict__ state,
                                    double* __restrict__ out, int A, int B, int n_max, tb2_sf_params p) {
@@ -57,68 +115,127 @@ __global__ void sf_simulate_kernel(const int* __restrict__ scene_off, const doub
     const int n = scene_off[scene + 1] - row0;
     const int a = kWarpScenes ? (int)(threadIdx.x & 31) : (int)threadIdx.x;
     double* px = smem_sf + (kWarpScenes ? (size_t)(threadIdx.x >> 5) * n_max * 7 : 0);
-    double* py = px + n;
-    double* vx = py + n;
-    double* vy = vx + n;
-    double* ex = vy + n;
-    double* ey = ex + n;
-    double* sp = ey + n;
+    const SfScene sc{px, px + n, px + 2 * n, px + 3 * n, px + 4 * n, px + 5 * n, px + 6 * n};
 
     const double dt = (double)p.delta_t, tau = (double)p.tau, v0 = (double)p.v0, sigma = (double)p.sigma;
-    const double fd = 1e-3;
-    const double cosphi = cos(200.0 / 2.0 / 180.0 * 3.141592653589793);   // FieldOfView(twophi=200)
-    double x = 0, y = 0, ux = 0, uy = 0, dx = 0, dy = 0, s0 = 0, smax = 0;
-    if (a < n) {
-        const double* st = state + (size_t)(row0 + a) * 6;
-        x = st[0]; y = st[1]; ux = st[2]; uy = st[3]; dx = st[4]; dy = st[5];
-        s0 = sqrt(ux * ux + uy * uy);            // Simulator.__init__: initial_speeds
-        smax = 1.3 * s0;                         // max_speeds
-    }
+    const double cosphi = sf_cosphi();
+    SfAgent g = {};
+    if (a < n) g = sf_agent_init(state + (size_t)(row0 + a) * 6);
     int sample = 0;
     for (int k = 0; k < p.n_steps; ++k) {
         double eax = 0, eay = 0;
-        if (a < n) {
-            const double gx = dx - x, gy = dy - y;
-            const double gn = sqrt(gx * gx + gy * gy);
-            eax = gx / gn; eay = gy / gn;        // desired direction (NaN at the destination, as upstream)
-            px[a] = x; py[a] = y; vx[a] = ux; vy[a] = uy; ex[a] = eax; ey[a] = eay;
-            sp[a] = sqrt(ux * ux + uy * uy);
-        }
+        if (a < n) sf_publish(g, sc, a, eax, eay);
         scene_sync<kWarpScenes>();
         if (a < n) {
-            double Fx = 1.0 / tau * (s0 * eax - ux);
-            double Fy = 1.0 / tau * (s0 * eay - uy);
-            double sumx = 0.0, sumy = 0.0;
-            for (int b = 0; b < n; ++b) {
-                double fx = 0.0, fy = 0.0, w = 0.0;
-                if (b != a) {
-                    const double rx = x - px[b], ry = y - py[b];
-                    const double sb = sp[b], ebx = ex[b], eby = ey[b];
-                    const double v = sf_potential(rx, ry, sb, ebx, eby, dt, v0, sigma);
-                    const double dvdx = (sf_potential(rx + fd, ry, sb, ebx, eby, dt, v0, sigma) - v) / fd;
-                    const double dvdy = (sf_potential(rx, ry + fd, sb, ebx, eby, dt, v0, sigma) - v) / fd;
-                    fx = -1.0 * dvdx; fy = -1.0 * dvdy;               // f_ab = -grad V
-                    const double gx = -fx, gy = -fy;                  // w(e, -f_ab)
-                    const bool in_sight = (eax * gx + eay * gy) > sqrt(gx * gx + gy * gy) * cosphi;
-                    w = in_sight ? 1.0 : 0.5;
-                }
-                sumx += w * fx;
-                sumy += w * fy;
-            }
-            Fx += sumx; Fy += sumy;
-            const double wx = ux + dt * Fx, wy = uy + dt * Fy;
-            const double wn = sqrt(wx * wx + wy * wy);
-            const double q = smax / wn;
-            const double factor = isnan(q) ? q : (q < 1.0 ? q : 1.0);       // numpy.minimum(1, q)
-            ux = wx * factor; uy = wy * factor;
-            x = x + ux * dt; y = y + uy * dt;
+            sf_advance(g, sc, a, n, eax, eay, dt, tau, v0, sigma, cosphi);
             if (k % p.sample_every == 0) {
                 double* o = out + ((size_t)sample * A + row0 + a) * 2;
-                o[0] = x; o[1] = y;
+                o[0] = g.x; o[1] = g.y;
             }
         }
         if (k % p.sample_every == 0) ++sample;
         scene_sync<kWarpScenes>();
+    }
+}
+
+// -----------------------------------------------------------------------------------------
+// Parameter sweeps: a work item is (scene, setting); only the primary's ADE / FDE leave the chip.
+// One CTA per scene runs every setting of it.  kPacked (scene of n <= 32): lane segments of W = next power of two >= n,
+// each segment its own setting with its own scene arrays, 32 / W settings per warp in lockstep under __syncwarp.
+// Otherwise the whole CTA is one item, looping over the settings.  Each thread keeps its pedestrian's initial state in
+// registers (the lane -> pedestrian map is fixed for the scene); the primary's truth sits in shared memory.  The primary
+// (pedestrian 0) accumulates |truth - position| in float64, sequentially over the samples: ADE = sum / n_samples,
+// FDE = the last distance.  No atomics: reruns are bit-identical.
+// -----------------------------------------------------------------------------------------
+constexpr int kSweepWarps = 4;
+
+__device__ __forceinline__ int sweep_width(int n) {
+    int w = 1;
+    while (w < n) w <<= 1;
+    return w;
+}
+
+// Lane geometry of one item: pedestrian index a, first setting `slot`, settings per round `nslots`, array stride.
+struct SweepLane { int a, slot, nslots, stride, warp_first; };
+
+template <bool kPacked>
+__device__ __forceinline__ SweepLane sweep_lane(int n) {
+    SweepLane L;
+    if (kPacked) {
+        const int W = sweep_width(n), per_warp = 32 / W, lane = (int)(threadIdx.x & 31), warp = (int)(threadIdx.x >> 5);
+        L.a = lane & (W - 1);
+        L.warp_first = warp * per_warp;
+        L.slot = L.warp_first + lane / W;
+        L.nslots = (int)(blockDim.x >> 5) * per_warp;
+        L.stride = W;
+    } else {
+        L.a = (int)threadIdx.x;
+        L.warp_first = L.slot = 0;
+        L.nslots = 1;
+        L.stride = n;
+    }
+    return L;
+}
+
+// Loads the primary's last n_samples truth rows into shared memory; returns false when the CTA's scene is not of
+// this form (packed: n <= 32; CTA: n > 32).
+template <bool kPacked>
+__device__ __forceinline__ bool sweep_scene(const int* scene_off, const double* truth, int T, int n_samples,
+                                            double* tr, int& row0, int& n) {
+    row0 = scene_off[blockIdx.x];
+    n = scene_off[blockIdx.x + 1] - row0;
+    if (kPacked ? n > 32 : n <= 32) return false;            // whole CTA
+    const double* src = truth + ((size_t)blockIdx.x * T + (T - n_samples)) * 2;
+    for (int i = (int)threadIdx.x; i < 2 * n_samples; i += (int)blockDim.x) tr[i] = src[i];
+    __syncthreads();
+    return true;
+}
+
+template <bool kPacked>
+__global__ void sf_sweep_kernel(const int* __restrict__ scene_off, const double* __restrict__ state,
+                                const double* __restrict__ params, int P, const double* __restrict__ truth, int T,
+                                double* __restrict__ ade, double* __restrict__ fde, int B, tb2_sf_params p) {
+    extern __shared__ double smem_sfs[];
+    const int n_samples = (p.n_steps + p.sample_every - 1) / p.sample_every;
+    double* tr = smem_sfs;
+    int row0, n;
+    if (!sweep_scene<kPacked>(scene_off, truth, T, n_samples, tr, row0, n)) return;
+    const SweepLane L = sweep_lane<kPacked>(n);
+    double* px = tr + 2 * n_samples + (kPacked ? (size_t)(threadIdx.x - L.a) * 7 : 0);    // this segment's arrays
+    const SfScene sc{px, px + L.stride, px + 2 * L.stride, px + 3 * L.stride, px + 4 * L.stride, px + 5 * L.stride,
+                     px + 6 * L.stride};
+    const double dt = (double)p.delta_t;
+    const double cosphi = sf_cosphi();
+    SfAgent g0 = {};
+    if (L.a < n) g0 = sf_agent_init(state + (size_t)(row0 + L.a) * 6);
+    for (int base = 0; base < P; base += L.nslots) {
+        if (kPacked && base + L.warp_first >= P) break;     // warp-uniform: no setting left for this warp
+        const int s = base + L.slot;
+        const bool on = L.a < n && s < P;
+        double tau = 1.0, v0 = 0.0, sigma = 1.0;
+        if (on) { tau = params[(size_t)s * 3]; v0 = params[(size_t)s * 3 + 1]; sigma = params[(size_t)s * 3 + 2]; }
+        SfAgent g = g0;
+        double sum = 0.0, last = 0.0;
+        int sample = 0;
+        for (int k = 0; k < p.n_steps; ++k) {
+            double eax = 0, eay = 0;
+            if (on) sf_publish(g, sc, L.a, eax, eay);
+            scene_sync<kPacked>();
+            if (on) {
+                sf_advance(g, sc, L.a, n, eax, eay, dt, tau, v0, sigma, cosphi);
+                if (L.a == 0 && k % p.sample_every == 0) {
+                    const double ex = tr[2 * sample] - g.x, ey = tr[2 * sample + 1] - g.y;
+                    last = sqrt(ex * ex + ey * ey);
+                    sum += last;
+                }
+            }
+            if (k % p.sample_every == 0) ++sample;
+            scene_sync<kPacked>();
+        }
+        if (on && L.a == 0) {
+            ade[(size_t)s * B + blockIdx.x] = sum / (double)n_samples;
+            fde[(size_t)s * B + blockIdx.x] = last;
+        }
     }
 }
 
@@ -213,6 +330,110 @@ __device__ void orca_lp3(const Line* lines, int n, int begin, float radius, floa
     }
 }
 
+// One ORCA agent: position and velocity (float, like RVO2), preferred velocity, goal and initial speed (double, like the
+// reference's numpy code), maximum speed 1.3 x the initial speed (orca.py:36,55  MAX_SPEED_MULTIPLIER).
+struct OrcaAgent { float2 pos, vel, pref; double2 goal; double speed; float maxsp; };
+
+__device__ __forceinline__ OrcaAgent orca_agent_init(float2 pos, float2 vel, double2 goal, double speed) {
+    OrcaAgent g;
+    g.pos = pos; g.vel = vel; g.pref = f2(0.f, 0.f); g.goal = goal; g.speed = speed;
+    g.maxsp = (float)(1.3 * speed);
+    return g;
+}
+
+// Per-setting constants of a step (RVO2 computeNewVelocity).
+struct OrcaStep {
+    float range_sq, inv_th, inv_ts, cr, crsq;
+    int max_nb;
+};
+
+__device__ __forceinline__ OrcaStep orca_step_consts(float time_step, float neighbor_dist, float time_horizon, float radius,
+                                                     int max_nb) {
+    OrcaStep c;
+    c.inv_th = 1.0f / time_horizon;
+    c.inv_ts = 1.0f / time_step;
+    c.cr = radius + radius;
+    c.crsq = c.cr * c.cr;
+    c.range_sq = neighbor_dist * neighbor_dist;
+    c.max_nb = max_nb;
+    return c;
+}
+
+// First half of a step: the new velocity of agent a from the scene's published positions / velocities (neighbours
+// b = 0 .. n-1 in index order, ORCA lines, linear programs 2 and 3).
+__device__ __forceinline__ float2 orca_new_velocity(const float2* pos, const float2* vel, int a, int n, const OrcaAgent& g,
+                                                    const OrcaStep& c) {
+    const float2 mypos = g.pos, myvel = g.vel;
+    int nb[kOrcaMaxNeigh];
+    float nd[kOrcaMaxNeigh];
+    int nn = 0;
+    float range_sq = c.range_sq;
+    for (int b = 0; b < n; ++b) {
+        if (b == a) continue;
+        const float dsq = vabssq(vsub(mypos, pos[b]));
+        if (dsq < range_sq) {
+            if (nn < c.max_nb) { nb[nn] = b; nd[nn] = dsq; ++nn; }
+            int i = nn - 1;
+            while (i != 0 && dsq < nd[i - 1]) { nb[i] = nb[i - 1]; nd[i] = nd[i - 1]; --i; }
+            nb[i] = b; nd[i] = dsq;
+            if (nn == c.max_nb) range_sq = nd[nn - 1];
+        }
+    }
+    Line lines[kOrcaMaxNeigh];
+    for (int k = 0; k < nn; ++k) {
+        const int b = nb[k];
+        const float2 rp = vsub(pos[b], mypos);
+        const float2 rv = vsub(myvel, vel[b]);
+        const float dsq = vabssq(rp);
+        Line l;
+        float2 u;
+        if (dsq > c.crsq) {
+            const float2 w = vsub(rv, vmul(c.inv_th, rp));
+            const float wsq = vabssq(w);
+            const float dp1 = vdot(w, rp);
+            if (dp1 < 0.0f && dp1 * dp1 > c.crsq * wsq) {
+                const float wl = sqrtf(wsq);
+                const float2 uw = f2(w.x / wl, w.y / wl);
+                l.dir = f2(uw.y, -uw.x);
+                u = vmul(c.cr * c.inv_th - wl, uw);
+            } else {
+                const float leg = sqrtf(dsq - c.crsq);
+                if (vdet(rp, w) > 0.0f) {
+                    l.dir = f2((rp.x * leg - rp.y * c.cr) / dsq, (rp.x * c.cr + rp.y * leg) / dsq);
+                } else {
+                    l.dir = f2(-(rp.x * leg + rp.y * c.cr) / dsq, -(-rp.x * c.cr + rp.y * leg) / dsq);
+                }
+                const float dp2 = vdot(rv, l.dir);
+                u = vsub(vmul(dp2, l.dir), rv);
+            }
+        } else {
+            const float2 w = vsub(rv, vmul(c.inv_ts, rp));
+            const float wl = sqrtf(vabssq(w));
+            const float2 uw = f2(w.x / wl, w.y / wl);
+            l.dir = f2(uw.y, -uw.x);
+            u = vmul(c.cr * c.inv_ts - wl, uw);
+        }
+        l.point = vadd(myvel, vmul(0.5f, u));
+        lines[k] = l;
+    }
+    float2 res;
+    const int fail = orca_lp2(lines, nn, g.maxsp, g.pref, false, res);
+    if (fail < nn) orca_lp3(lines, nn, fail, g.maxsp, res);
+    return res;
+}
+
+// Second half: take the new velocity, move, and steer the preferred velocity at the goal (orca.py:111-119, double like
+// the reference's numpy code).
+__device__ __forceinline__ void orca_advance(OrcaAgent& g, float2 newv, float time_step, double end_range) {
+    g.vel = newv;
+    g.pos = vadd(g.pos, vmul(time_step, g.vel));
+    const double gx = g.goal.x - (double)g.pos.x, gy = g.goal.y - (double)g.pos.y;
+    const double dist = sqrt(gx * gx + gy * gy);
+    if (dist < end_range) g.pref = f2(0.f, 0.f);
+    else if (dist > g.speed) g.pref = f2((float)(g.speed * gx / dist), (float)(g.speed * gy / dist));
+    else g.pref = f2((float)gx, (float)gy);
+}
+
 template <bool kWarpScenes>
 __global__ void orca_simulate_kernel(const int* __restrict__ scene_off, const float2* __restrict__ pos_in,
                                      const float2* __restrict__ vel_in, const double2* __restrict__ goal_in,
@@ -227,108 +448,129 @@ __global__ void orca_simulate_kernel(const int* __restrict__ scene_off, const fl
     float2* pos = smem_orca + (kWarpScenes ? (size_t)(threadIdx.x >> 5) * n_max * 2 : 0);
     float2* vel = pos + n;
 
-    float2 mypos = f2(0.f, 0.f), myvel = f2(0.f, 0.f), pref = f2(0.f, 0.f);
-    double2 goal = make_double2(0.0, 0.0);
-    double speed = 0.0;
-    float maxsp = 0.f;
+    OrcaAgent g = {};
     if (a < n) {
-        mypos = pos_in[row0 + a];
-        myvel = vel_in[row0 + a];
-        goal = goal_in[row0 + a];
-        speed = speed_in[row0 + a];
-        maxsp = (float)(1.3 * speed);               // orca.py:36,55  MAX_SPEED_MULTIPLIER
-        pos[a] = mypos;
-        vel[a] = myvel;
+        g = orca_agent_init(pos_in[row0 + a], vel_in[row0 + a], goal_in[row0 + a], speed_in[row0 + a]);
+        pos[a] = g.pos;
+        vel[a] = g.vel;
     }
     scene_sync<kWarpScenes>();
-    const float inv_th = 1.0f / p.time_horizon;
-    const float inv_ts = 1.0f / p.time_step;
-    const float cr = p.radius + p.radius;
-    const float crsq = cr * cr;
-    const int max_nb = p.max_neighbors;
+    const OrcaStep c = orca_step_consts(p.time_step, p.neighbor_dist, p.time_horizon, p.radius, p.max_neighbors);
     int sample = 0;
     for (int count = 1; count <= p.n_steps; ++count) {
-        float2 newv = myvel;
-        if (a < n) {
-            int nb[kOrcaMaxNeigh];
-            float nd[kOrcaMaxNeigh];
-            int nn = 0;
-            float range_sq = p.neighbor_dist * p.neighbor_dist;
-            for (int b = 0; b < n; ++b) {
-                if (b == a) continue;
-                const float dsq = vabssq(vsub(mypos, pos[b]));
-                if (dsq < range_sq) {
-                    if (nn < max_nb) { nb[nn] = b; nd[nn] = dsq; ++nn; }
-                    int i = nn - 1;
-                    while (i != 0 && dsq < nd[i - 1]) { nb[i] = nb[i - 1]; nd[i] = nd[i - 1]; --i; }
-                    nb[i] = b; nd[i] = dsq;
-                    if (nn == max_nb) range_sq = nd[nn - 1];
-                }
-            }
-            Line lines[kOrcaMaxNeigh];
-            for (int k = 0; k < nn; ++k) {
-                const int b = nb[k];
-                const float2 rp = vsub(pos[b], mypos);
-                const float2 rv = vsub(myvel, vel[b]);
-                const float dsq = vabssq(rp);
-                Line l;
-                float2 u;
-                if (dsq > crsq) {
-                    const float2 w = vsub(rv, vmul(inv_th, rp));
-                    const float wsq = vabssq(w);
-                    const float dp1 = vdot(w, rp);
-                    if (dp1 < 0.0f && dp1 * dp1 > crsq * wsq) {
-                        const float wl = sqrtf(wsq);
-                        const float2 uw = f2(w.x / wl, w.y / wl);
-                        l.dir = f2(uw.y, -uw.x);
-                        u = vmul(cr * inv_th - wl, uw);
-                    } else {
-                        const float leg = sqrtf(dsq - crsq);
-                        if (vdet(rp, w) > 0.0f) {
-                            l.dir = f2((rp.x * leg - rp.y * cr) / dsq, (rp.x * cr + rp.y * leg) / dsq);
-                        } else {
-                            l.dir = f2(-(rp.x * leg + rp.y * cr) / dsq, -(-rp.x * cr + rp.y * leg) / dsq);
-                        }
-                        const float dp2 = vdot(rv, l.dir);
-                        u = vsub(vmul(dp2, l.dir), rv);
-                    }
-                } else {
-                    const float2 w = vsub(rv, vmul(inv_ts, rp));
-                    const float wl = sqrtf(vabssq(w));
-                    const float2 uw = f2(w.x / wl, w.y / wl);
-                    l.dir = f2(uw.y, -uw.x);
-                    u = vmul(cr * inv_ts - wl, uw);
-                }
-                l.point = vadd(myvel, vmul(0.5f, u));
-                lines[k] = l;
-            }
-            float2 res;
-            const int fail = orca_lp2(lines, nn, maxsp, pref, false, res);
-            if (fail < nn) orca_lp3(lines, nn, fail, maxsp, res);
-            newv = res;
-        }
+        float2 newv = g.vel;
+        if (a < n) newv = orca_new_velocity(pos, vel, a, n, g, c);
         scene_sync<kWarpScenes>();                       // every agent has read the old positions / velocities
         if (a < n) {
-            myvel = newv;
-            mypos = vadd(mypos, vmul(p.time_step, myvel));
-            pos[a] = mypos;
-            vel[a] = myvel;
-            if (count % p.sample_every == 0) out[(size_t)sample * A + row0 + a] = mypos;
-            // orca.py:111-119 (double, like the reference's numpy code)
-            const double gx = goal.x - (double)mypos.x, gy = goal.y - (double)mypos.y;
-            const double dist = sqrt(gx * gx + gy * gy);
-            if (dist < (double)p.end_range) pref = f2(0.f, 0.f);
-            else if (dist > speed) pref = f2((float)(speed * gx / dist), (float)(speed * gy / dist));
-            else pref = f2((float)gx, (float)gy);
+            orca_advance(g, newv, p.time_step, p.end_range);
+            pos[a] = g.pos;
+            vel[a] = g.vel;
+            if (count % p.sample_every == 0) out[(size_t)sample * A + row0 + a] = g.pos;
         }
         if (count % p.sample_every == 0) ++sample;
         scene_sync<kWarpScenes>();
     }
 }
 
+// Parameter sweep of ORCA (see sf_sweep_kernel): params [P, 3] = neighbor_dist, time_horizon, radius.  The primary's
+// float positions are widened to double before the difference with the truth (the adapter's astype(np.float64)).
+template <bool kPacked>
+__global__ void orca_sweep_kernel(const int* __restrict__ scene_off, const float2* __restrict__ pos_in,
+                                  const float2* __restrict__ vel_in, const double2* __restrict__ goal_in,
+                                  const double* __restrict__ speed_in, const float* __restrict__ params, int P,
+                                  const double* __restrict__ truth, int T, double* __restrict__ ade,
+                                  double* __restrict__ fde, int B, tb2_orca_params p) {
+    extern __shared__ double smem_os[];
+    const int n_samples = p.n_steps / p.sample_every;
+    double* tr = smem_os;
+    int row0, n;
+    if (!sweep_scene<kPacked>(scene_off, truth, T, n_samples, tr, row0, n)) return;
+    const SweepLane L = sweep_lane<kPacked>(n);
+    float2* pos = reinterpret_cast<float2*>(tr + 2 * n_samples) + (kPacked ? (size_t)(threadIdx.x - L.a) * 2 : 0);
+    float2* vel = pos + L.stride;
+    OrcaAgent g0 = {};
+    if (L.a < n) g0 = orca_agent_init(pos_in[row0 + L.a], vel_in[row0 + L.a], goal_in[row0 + L.a], speed_in[row0 + L.a]);
+    for (int base = 0; base < P; base += L.nslots) {
+        if (kPacked && base + L.warp_first >= P) break;     // warp-uniform: no setting left for this warp
+        const int s = base + L.slot;
+        const bool on = L.a < n && s < P;
+        OrcaStep c = {};
+        if (on) c = orca_step_consts(p.time_step, params[(size_t)s * 3], params[(size_t)s * 3 + 1],
+                                     params[(size_t)s * 3 + 2], p.max_neighbors);
+        OrcaAgent g = g0;
+        if (on) { pos[L.a] = g.pos; vel[L.a] = g.vel; }
+        scene_sync<kPacked>();
+        double sum = 0.0, last = 0.0;
+        int sample = 0;
+        for (int count = 1; count <= p.n_steps; ++count) {
+            float2 newv = g.vel;
+            if (on) newv = orca_new_velocity(pos, vel, L.a, n, g, c);
+            scene_sync<kPacked>();
+            if (on) {
+                orca_advance(g, newv, p.time_step, p.end_range);
+                pos[L.a] = g.pos;
+                vel[L.a] = g.vel;
+                if (L.a == 0 && count % p.sample_every == 0) {
+                    const double ex = tr[2 * sample] - (double)g.pos.x, ey = tr[2 * sample + 1] - (double)g.pos.y;
+                    last = sqrt(ex * ex + ey * ey);
+                    sum += last;
+                }
+            }
+            if (count % p.sample_every == 0) ++sample;
+            scene_sync<kPacked>();
+        }
+        if (on && L.a == 0) {
+            ade[(size_t)s * B + blockIdx.x] = sum / (double)n_samples;
+            fde[(size_t)s * B + blockIdx.x] = last;
+        }
+    }
+}
+
 }  // namespace tb2
 
 using namespace tb2;
+
+// Host-side checks shared by the sweeps: counts, then the parameters read back from the device (P x 3 values).
+template <typename T>
+static int sweep_params_host(const T* params_dev, int P, std::vector<T>& h, cudaStream_t st) {
+    h.resize((size_t)P * 3);
+    TB2_CHECK_CUDA(cudaMemcpyAsync(h.data(), params_dev, h.size() * sizeof(T), cudaMemcpyDeviceToHost, st));
+    TB2_CHECK_CUDA(cudaStreamSynchronize(st));
+    for (T v : h) TB2_REQUIRE(isfinite((double)v), "non-finite sweep parameter");
+    return TB2_OK;
+}
+
+static int sweep_counts(const tb2_layout* l, int P, int T, int n_samples) {
+    TB2_REQUIRE(l->B >= 1, "no scenes");
+    TB2_REQUIRE(P >= 1, "P < 1 settings");
+    TB2_REQUIRE((int64_t)P * l->B < ((int64_t)1 << 31), "P x B >= 2^31");
+    TB2_REQUIRE(l->n_max <= 1024, "scene larger than 1024 pedestrians");
+    TB2_REQUIRE(n_samples >= 1 && n_samples <= 1024, "sample count must be in [1, 1024]");
+    TB2_REQUIRE(T >= n_samples, "truth shorter than the sample count");
+    return TB2_OK;
+}
+
+// Launches both forms over every scene; each CTA keeps only the scenes of its form (packed: n <= 32, CTA: n > 32).
+template <typename KPacked, typename KCta, typename... Args>
+static int sweep_launch(const char* name, KPacked kp, KCta kc, const tb2_layout* l, int P, int n_samples,
+                        size_t per_thread, cudaStream_t st, Args... args) {
+    const size_t truth_bytes = (size_t)n_samples * 2 * sizeof(double);
+    const int w_max = l->n_max >= 32 ? 32 : (l->n_max <= 1 ? 1 : 1 << (32 - __builtin_clz(l->n_max - 1)));
+    const int64_t want = ((int64_t)P * w_max + 31) / 32;
+    const int warps = (int)(want < kSweepWarps ? want : kSweepWarps);
+    KernelTimer kt(name, st);
+    kp<<<l->B, 32 * warps, truth_bytes + (size_t)32 * warps * per_thread, st>>>(args...);
+    TB2_LAUNCH_CHECK();
+    if (l->n_max > 32) {
+        const int threads = (l->n_max + 31) / 32 * 32;
+        const size_t smem = truth_bytes + (size_t)l->n_max * per_thread;
+        static DynSmemConfig configured;
+        TB2_CHECK_CUDA(configured.ensure(kc, smem, 48 * 1024));
+        kc<<<l->B, threads, smem, st>>>(args...);
+        TB2_LAUNCH_CHECK();
+    }
+    return TB2_OK;
+}
 
 extern "C" {
 
@@ -376,6 +618,42 @@ int tb2_orca_simulate(const tb2_layout* l, const tb2_orca_params* p, const float
     }
     TB2_LAUNCH_CHECK();
     return TB2_OK;
+}
+
+int tb2_sf_sweep(const tb2_layout* l, const tb2_sf_params* p, const double* params, int32_t P, const double* state,
+                 const double* truth, int32_t truth_len, double* ade_out, double* fde_out, void* stream) {
+    TB2_REQUIRE(l && p && params && state && truth && ade_out && fde_out, "null argument");
+    TB2_REQUIRE(p->n_steps >= 1 && p->sample_every >= 1, "bad step counts");
+    const int n_samples = (p->n_steps + p->sample_every - 1) / p->sample_every;
+    int rc = sweep_counts(l, P, truth_len, n_samples);
+    if (rc != TB2_OK) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    std::vector<double> h;
+    rc = sweep_params_host(params, P, h, st);
+    if (rc != TB2_OK) return rc;
+    for (int s = 0; s < P; ++s) TB2_REQUIRE(h[s * 3] > 0.0 && h[s * 3 + 2] > 0.0, "tau and sigma must be > 0");
+    return sweep_launch("sf_sweep", sf_sweep_kernel<true>, sf_sweep_kernel<false>, l, P, n_samples, 7 * sizeof(double), st,
+                        (const int*)l->scene_off, state, params, (int)P, truth, (int)truth_len, ade_out, fde_out, l->B, *p);
+}
+
+int tb2_orca_sweep(const tb2_layout* l, const tb2_orca_params* p, const float* params, int32_t P, const float* pos,
+                   const float* vel, const double* goal, const double* speed, const double* truth, int32_t truth_len,
+                   double* ade_out, double* fde_out, void* stream) {
+    TB2_REQUIRE(l && p && params && pos && vel && goal && speed && truth && ade_out && fde_out, "null argument");
+    TB2_REQUIRE(p->n_steps >= 1 && p->sample_every >= 1, "bad step counts");
+    TB2_REQUIRE(p->max_neighbors >= 1 && p->max_neighbors <= kOrcaMaxNeigh, "max_neighbors must be in [1, 16]");
+    const int n_samples = p->n_steps / p->sample_every;
+    int rc = sweep_counts(l, P, truth_len, n_samples);
+    if (rc != TB2_OK) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    std::vector<float> h;
+    rc = sweep_params_host(params, P, h, st);
+    if (rc != TB2_OK) return rc;
+    for (int s = 0; s < P; ++s)
+        TB2_REQUIRE(h[s * 3 + 1] > 0.0f && h[s * 3 + 2] > 0.0f, "time_horizon and radius must be > 0");
+    return sweep_launch("orca_sweep", orca_sweep_kernel<true>, orca_sweep_kernel<false>, l, P, n_samples,
+                        2 * sizeof(float2), st, (const int*)l->scene_off, (const float2*)pos, (const float2*)vel,
+                        (const double2*)goal, speed, params, (int)P, truth, (int)truth_len, ade_out, fde_out, l->B, *p);
 }
 
 }  // extern "C"
