@@ -254,6 +254,26 @@ int tb2_sgan_add_noise(const float* weight_dev, const float* bias_dev, const flo
 int tb2_vae_scale_hidden(const float* weight_dev, const float* bias_dev, const float* z_dev, float* h_dev,
                          int32_t M, int32_t H, int32_t latent_dim, void* stream);
 
+/* Decoder starting state of k modes in one pass over the encoder state (M tracks), mode-major:
+ * output row q * M + m is track m in mode q, for q < k.
+ *   h_out[q*M + m] = cat(ReLU(weight . h_enc[m] + bias), noise[q * num_groups + group_of_row[m]])
+ *   c_out[q*M + m] = c_enc[m]
+ * weight [H - noise_dim, H]; noise [k * num_groups, noise_dim] holds one vector per (mode, scene);
+ * group_of_row [M] is the scene of every track.  ReLU(weight . h + bias) is computed once per track; every
+ * replica row is bit-identical to tb2_sgan_add_noise on a copy of h_enc with that row's noise vector.
+ * h_out / c_out [k * M, H] must not overlap the inputs. */
+int tb2_sgan_decoder_context(const float* weight_dev, const float* bias_dev, const float* noise_dev,
+                             const int32_t* group_of_row_dev, int32_t num_groups, const float* h_enc_dev,
+                             const float* c_enc_dev, int32_t M, int32_t H, int32_t noise_dim, int32_t k,
+                             float* h_out_dev, float* c_out_dev, void* stream);
+
+/* The VAE's counterpart, mode-major like tb2_sgan_decoder_context, with one latent sample per (mode, track):
+ *   h_out[q*M + m] = h_enc[m] * ReLU(weight . z[q*M + m] + bias),   c_out[q*M + m] = c_enc[m]
+ * weight [H, latent_dim], z [k * M, latent_dim]; bit-identical to tb2_vae_scale_hidden on a copy of h_enc. */
+int tb2_vae_decoder_context(const float* weight_dev, const float* bias_dev, const float* z_dev,
+                            const float* h_enc_dev, const float* c_enc_dev, int32_t M, int32_t H,
+                            int32_t latent_dim, int32_t k, float* h_out_dev, float* c_out_dev, void* stream);
+
 /* ---------------------------------------------------------------------------------------
  * Training: backward of the whole time loop (what autograd does for Trainer.train_batch,
  * lstm/trainer.py:229-269, through LSTM.forward).  Gradient accumulators are fp32 device

@@ -152,6 +152,8 @@ PROTOTYPES = {
                                                          _vp, _sz, _vp, _sz, _vp, _sz, _vp]),
     "tb2_sgan_add_noise": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp]),
     "tb2_vae_scale_hidden": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp]),
+    "tb2_sgan_decoder_context": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
+    "tb2_vae_decoder_context": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),
     "tb2_prediction_loss": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, ctypes.c_float, _vp, _vp, _vp]),
     "tb2_l2_loss": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp]),
     "tb2_collision_loss": (ctypes.c_int, [_vp, _vp, _i32, ctypes.c_float, ctypes.c_float, _vp, _vp, _vp]),

@@ -8,10 +8,12 @@ Multi-GPU (SURVEY.md 8e: scenes are independent, no data-path collective): under
 range of the file's scenes (balanced by sum N^2, parallel.shard_scenes), writes its records to `<outfile>.part<rank>`, and
 rank 0 concatenates the parts in rank order after a barrier -- the file is byte-identical to the single-process one.
 """
+import inspect
 import os
 import shutil
 
-from .data import load_test_scenes_xy, preprocess_test, read_ndjson_scenes, write_predictions, write_predictions_xy
+from .data import (load_test_scenes_xy, paths_to_xy, preprocess_test, read_ndjson_scenes, write_predictions,
+                   write_predictions_xy)
 
 
 def load_test_scenes(filename, obs_length=9):
@@ -28,11 +30,40 @@ def load_test_scenes(filename, obs_length=9):
     return [(name, scene_id, preprocess_test(paths, obs_length)) for scene_id, paths in read_ndjson_scenes(filename)]
 
 
+def _takes_modes(predictor):
+    fn = getattr(predictor, 'predict_batch_xy', None)
+    if fn is None:
+        return False
+    try:
+        return 'modes' in inspect.signature(fn).parameters
+    except (TypeError, ValueError):
+        return False
+
+
+def batches_modes(predictor):
+    """True for a predictor whose predict_batch_xy takes `modes` (S-GAN / VAE: every mode of every scene of a chunk in
+    one batched decode, multimodal.py) and can decode its model that way."""
+    supported = getattr(predictor, 'batch_decode_supported', None)
+    return _takes_modes(predictor) and (supported is None or bool(supported()))
+
+
+def _predict_xy(predictor, xys, pred_length, obs_length, modes, args):
+    if batches_modes(predictor):
+        return predictor.predict_batch_xy(xys, n_predict=pred_length, obs_length=obs_length, args=args, modes=modes)
+    return predictor.predict_batch_xy(xys, n_predict=pred_length, obs_length=obs_length, args=args)
+
+
 def predict_scenes(predictor, scenes, obs_length=9, pred_length=12, modes=1, chunk=1024, args=None):
     """Predictions for a list of (filename, scene_id, paths), in order.  A predictor with
-    predict_batch (LSTMPredictor) gets `chunk` scenes per forward; any other predictor of the
-    reference's call signature (S-GAN / VAE / classical) is called scene by scene."""
+    predict_batch (LSTMPredictor) gets `chunk` scenes per forward at modes 1, one whose predict_batch_xy takes `modes`
+    (S-GAN / VAE) `chunk` scenes per decode of all modes; any other predictor of the reference's call signature
+    (classical, LSTM at modes > 1) is called scene by scene."""
     out = []
+    if batches_modes(predictor):
+        for i in range(0, len(scenes), chunk):
+            xys = [paths_to_xy(paths) for _, _, paths in scenes[i:i + chunk]]
+            out.extend(_predict_xy(predictor, xys, pred_length, obs_length, modes, args))
+        return out
     if hasattr(predictor, 'predict_batch') and modes == 1:
         for i in range(0, len(scenes), chunk):
             part = [paths for _, _, paths in scenes[i:i + chunk]]
@@ -69,8 +100,11 @@ def _barrier():
 
 def _column_pipeline(predictor, modes):
     """The column pipeline (data.load_test_scenes_xy -> predict_batch_xy -> data.write_predictions_xy: native text passes,
-    no Python object per track row) serves predictors that take arrays; it writes the same bytes as the row pipeline."""
-    return hasattr(predictor, 'predict_batch_xy') and modes == 1
+    no Python object per track row) serves predictors that take arrays: at any `modes` when predict_batch_xy takes them
+    (S-GAN / VAE), else at modes 1.  It writes the same bytes as the row pipeline."""
+    if batches_modes(predictor):
+        return True
+    return hasattr(predictor, 'predict_batch_xy') and modes == 1 and not _takes_modes(predictor)
 
 
 def evaluate_file(predictor, infile, outfile, obs_length=9, pred_length=12, modes=1, chunk=1024, args=None,
@@ -86,8 +120,8 @@ def evaluate_file(predictor, infile, outfile, obs_length=9, pred_length=12, mode
         def run(part, filename):
             preds = []
             for i in range(0, len(part), chunk):
-                preds.extend(predictor.predict_batch_xy([xy for xy, _ in part[i:i + chunk]], n_predict=pred_length,
-                                                        obs_length=obs_length, args=args))
+                preds.extend(_predict_xy(predictor, [xy for xy, _ in part[i:i + chunk]], pred_length, obs_length, modes,
+                                         args))
             write_predictions_xy(preds, [meta for _, meta in part], filename, obs_length=obs_length, pred_length=pred_length)
     else:
         scenes = load_test_scenes(infile, obs_length)                    # [(filename, scene_id, paths)]

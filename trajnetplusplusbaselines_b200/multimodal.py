@@ -1,0 +1,168 @@
+"""Every mode of every scene in one batched decode: the evaluator path of the multi-modal predictors (S-GAN, VAE).
+
+The per-scene predictors (SGANPredictor / VAEPredictor.__call__) run one encoder pass and then k decoder passes of
+pred_length - 1 steps each over the 5-50 tracks of one scene.  Here the encoder runs once over the B scenes of a chunk
+(M tracks) and the k decoders run as ONE decode over k * M rows, laid out mode-major: row q * M + m is track m in mode
+q, and replica q * B + b is scene b of mode q, a separate scene of one layout.  The layouts use per-scene semantics
+(tb2_layout_set_padding(0)), so no pooling ever mixes two modes or two scenes, and every row computes what the
+per-scene call computes.  The decoder's starting state comes from one kernel over the encoder state
+(tb2_sgan_decoder_context / tb2_vae_decoder_context, csrc/sgan.cu); the replicated observations and encoder positions
+are torch copies on the device.
+
+One decode is capped at `rows_per_decode` rows (the engine's workspace per row plus the replicated state per row,
+within DECODE_BYTES); above the cap the modes are split into groups.  The random draws are made for all modes before
+the split, so the results do not depend on the grouping.
+"""
+import numpy as np
+import torch
+
+from . import _lib
+from .engine import _ptr, _stream
+
+# device memory one decode may take: the engine's workspace for its rows plus their replicated state
+DECODE_BYTES = 2 << 30
+
+
+def stateful_pool(body):
+    """True for interaction modules that carry an LSTM state of their own through the time loop (NearestNeighborLSTM,
+    TrajectronPooling): that state lives in the engine's workspace and is not replicated per mode."""
+    pool = body.pool
+    if pool is None or not hasattr(pool, 'fill_config'):
+        return False
+    cfg = _lib.LstmConfig()
+    pool.fill_config(cfg)
+    return cfg.pool_type in (_lib.POOL_NN_LSTM, _lib.POOL_TRAJECTRON)
+
+
+def replicated_split(split, k):
+    """batch_split of k mode-major replicas of the scenes `split` (int64 [B + 1]) -> int64 [k * B + 1]."""
+    split = np.asarray(split, dtype=np.int64)
+    M = int(split[-1])
+    out = np.empty(k * (len(split) - 1) + 1, dtype=np.int64)
+    out[:-1] = (split[:-1][None, :] + M * np.arange(k, dtype=np.int64)[:, None]).reshape(-1)
+    out[-1] = k * M
+    return out
+
+
+def rows_per_decode(handle, layout, num_steps, obs_length, budget=DECODE_BYTES):
+    """Rows of one decode: `budget` over the bytes one row takes, i.e. its share of the engine's workspace (which
+    grows linearly with the rows of a layout of the same largest scene) plus its replicated observations, normals,
+    positions and (h, c) state."""
+    M = max(layout.num_tracks, 1)
+    ws = int(_lib.load().tb2_lstm_workspace_bytes(handle.handle, layout.handle))
+    state = 4 * (num_steps * 7 + obs_length * 2 + 2 * int(handle.config.hidden_dim))
+    return max(int(budget // (ws / M + state)), 1)
+
+
+def observed_batch(body, xys, obs_length, start_length, normalize):
+    """(observed float32 [obs_length - start_length, M, 2] on the model's device, batch_split int64 [B + 1],
+    rotation [B], centre [B, 2]): the inputs of the per-scene call for every scene, centred / rotated on the device
+    (lstm/scene_ops.py) when `normalize`."""
+    split = np.zeros(len(xys) + 1, dtype=np.int64)
+    split[1:] = np.cumsum([xy.shape[1] for xy in xys])
+    device = body._device()
+    if normalize:
+        from .lstm.scene_ops import preprocess_scenes
+        observed, _, _, rotation, center = preprocess_scenes([xy[:obs_length] for xy in xys], device=device,
+                                                             normalize_scene=True, obs_length=obs_length)
+        return observed[start_length:].contiguous(), split, rotation, center
+    host = np.concatenate([xy[start_length:obs_length] for xy in xys], axis=1)
+    return torch.from_numpy(host.astype(np.float32)).to(device), split, None, None
+
+
+def predict_modes(body, observed, split, n_predict, modes, context, max_rows=None):
+    """Encoder once over the scenes of `split`, then the decoders of all `modes` modes.
+
+    context(h_enc, c_enc, q0, q1, h_out, c_out) writes the decoder starting state of modes [q0, q1) into
+    h_out / c_out [(q1 - q0) * M, H].  Returns the positions of the last n_predict steps, float32 [n_predict,
+    modes * M, 2] on the device, mode-major."""
+    handle = body._engine()
+    device = handle.device
+    layout = body._layouts.get(split.tolist(), False, device=device)
+    M = layout.num_tracks
+    obs_length = int(observed.shape[0])
+    n_decode = int(n_predict) - 1
+    S_enc = obs_length - 1
+    S = S_enc + n_decode
+    H = int(body.hidden_dim)
+    f32 = dict(dtype=torch.float32, device=device)
+    normals0, positions0 = torch.empty((S, M, 5), **f32), torch.empty((S, M, 2), **f32)
+    h0, c0 = torch.empty((M, H), **f32), torch.empty((M, H), **f32)
+    handle.forward_steps(layout, observed, None, n_decode, 0, S_enc, normals0, positions0, h0, c0)
+    cap = rows_per_decode(handle, layout, S, obs_length) if max_rows is None else int(max_rows)
+    per_group = max(1, min(modes, cap // max(M, 1)))
+    out = torch.empty((n_predict, modes * M, 2), **f32)
+    for q0 in range(0, modes, per_group):
+        q1 = min(q0 + per_group, modes)
+        kq = q1 - q0
+        rows = kq * M
+        rep = body._layouts.get(replicated_split(split, kq).tolist(), False, device=device)
+        obs_rep = observed.repeat(1, kq, 1)
+        normals, positions = torch.empty((S, rows, 5), **f32), torch.empty((S, rows, 2), **f32)
+        positions[:S_enc] = positions0[:S_enc].repeat(1, kq, 1)      # the decoder's first inputs
+        h, c = torch.empty((rows, H), **f32), torch.empty((rows, H), **f32)
+        context(h0, c0, q0, q1, h, c)
+        handle.forward_steps(rep, obs_rep, None, n_decode, S_enc, S, normals, positions, h, c)
+        out[:, q0 * M:q1 * M] = positions[S - n_predict:]
+    return out
+
+
+def scene_results(pred, split, modes, n_predict, normalize, rotation=None, center=None):
+    """Per scene {mode: [primary [n_predict, 2], neighbours [n_predict, N - 1, 2] if mode == 0 else []]} -- the
+    dictionary of the per-scene __call__ -- from the mode-major positions of predict_modes."""
+    B = len(split) - 1
+    M = int(split[-1])
+    if normalize:
+        from .lstm.scene_ops import inverse_scenes
+        pred = inverse_scenes(pred, replicated_split(split, modes), np.tile(rotation, modes),
+                              np.tile(np.asarray(center).reshape(B, 2), (modes, 1)))
+    else:
+        pred = pred.cpu().numpy()
+    pred = pred.reshape(n_predict, modes, M, 2)
+    results = []
+    for i in range(B):
+        lo, hi = int(split[i]), int(split[i + 1])
+        out = {q: [np.array(pred[:, q, lo]), []] for q in range(modes)}
+        out[0][1] = np.array(pred[:, 0, lo + 1:hi])
+        results.append(out)
+    return results
+
+
+def group_of_rows(split, device):
+    """Scene index of every track, int32 [M] on `device`."""
+    split = np.asarray(split, dtype=np.int64)
+    return torch.from_numpy(np.repeat(np.arange(len(split) - 1, dtype=np.int32), np.diff(split))).to(device)
+
+
+def sgan_context(weight, bias, noise, groups, num_groups, noise_dim):
+    """context() of predict_modes for the S-GAN generator: noise [k, num_groups, noise_dim] (None: no noise)."""
+    lib = _lib.load()
+
+    def run(h_enc, c_enc, q0, q1, h_out, c_out):
+        kq = q1 - q0
+        if noise is None:                      # no_noise: the decoder starts from the encoder state (sgan.py:200-204)
+            h_out.copy_(h_enc.repeat(kq, 1))
+            c_out.copy_(c_enc.repeat(kq, 1))
+            return
+        part = noise[q0:q1].contiguous()
+        device = h_enc.device
+        with torch.cuda.device(device):
+            _lib.check(lib.tb2_sgan_decoder_context(
+                _ptr(weight), _ptr(bias), _ptr(part), _ptr(groups), int(num_groups), _ptr(h_enc), _ptr(c_enc),
+                int(h_enc.shape[0]), int(h_enc.shape[1]), int(noise_dim), int(kq), _ptr(h_out), _ptr(c_out),
+                _stream(device)))
+    return run
+
+
+def vae_context(weight, bias, z, latent_dim):
+    """context() of predict_modes for the VAE: z [k, M, latent_dim], one latent sample per (mode, track)."""
+    lib = _lib.load()
+
+    def run(h_enc, c_enc, q0, q1, h_out, c_out):
+        part = z[q0:q1].contiguous()
+        device = h_enc.device
+        with torch.cuda.device(device):
+            _lib.check(lib.tb2_vae_decoder_context(
+                _ptr(weight), _ptr(bias), _ptr(part), _ptr(h_enc), _ptr(c_enc), int(h_enc.shape[0]),
+                int(h_enc.shape[1]), int(latent_dim), int(q1 - q0), _ptr(h_out), _ptr(c_out), _stream(device)))
+    return run

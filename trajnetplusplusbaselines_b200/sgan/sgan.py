@@ -8,7 +8,8 @@ encoder and decoder (adding_noise :200-221 -> tb2_sgan_add_noise) and the k-mode
 is deterministic, so it runs ONCE and every mode restarts from a copy of its state
 (tb2_lstm_forward_steps); the reference re-runs it per mode.  Same constructor arguments and
 state_dict keys (reference checkpoints load verbatim).  GAN training (variety loss, discriminator
-steps) is not built: forward under grad mode raises.
+steps) is not built: forward under grad mode raises.  SGANPredictor.predict_batch_xy decodes every mode
+of many scenes at once (the evaluator's path, ../multimodal.py).
 """
 import ctypes
 
@@ -16,7 +17,7 @@ import numpy as np
 import torch
 from torch import nn
 
-from .. import _lib
+from .. import _lib, multimodal
 from ..data import paths_to_xy
 from ..engine import _ptr, _stream
 from ..lstm.lstm import LSTM, center_scene, drop_distant, inverse_scene  # noqa: F401
@@ -246,3 +247,49 @@ class SGANPredictor(object):
                 output_neighs = output_scenes[-n_predict:, 1:]
                 multimodal_outputs[num_p] = [output_primary, output_neighs if num_p == 0 else []]
         return multimodal_outputs
+
+    def batch_decode_supported(self):
+        """predict_batch_xy serves every generator except those whose interaction module carries its own LSTM state
+        (NearestNeighborLSTM, TrajectronPooling): that state is not replicated per mode."""
+        return not multimodal.stateful_pool(self.model.generator)
+
+    def predict_batch_xy(self, xys, scene_goals=None, n_predict=12, obs_length=9, start_length=0, args=None, modes=1,
+                         noise=None, max_rows=None):
+        """Every mode of many scenes in one batched decode (the evaluator's column pipeline, multimodal.py).
+
+        xys: list of float64 [n_frames, N_i, 2] as paths_to_xy returns them.  Returns per scene the dictionary of
+        __call__, {mode: [primary [n_predict, 2], neighbours if mode == 0 else []]}.  The noise is drawn once per call,
+        on the device, one vector per (mode, scene) like the per-scene decodes draw it; `fixed_noise` and `no_noise`
+        of the generator apply as in __call__.  noise: explicit [modes, B, noise_dim] vectors instead of the draw.
+        max_rows: rows of one decode (default: multimodal.rows_per_decode); more modes are decoded in groups."""
+        gen = self.model.generator
+        if not self.batch_decode_supported():
+            raise NotImplementedError("batched decoding of a generator whose interaction module keeps an LSTM state "
+                                      "is not built; call the predictor scene by scene")
+        self.model.eval()
+        modes = int(modes)
+        if modes < 1:
+            raise ValueError("modes must be >= 1")
+        if not xys:
+            return []
+        normalize = bool(getattr(args, 'normalize_scene', False))
+        with torch.no_grad():
+            # sgan.py:603 feeds xy[:obs_length]: start_length does not apply to the generator
+            observed, split, rotation, center = multimodal.observed_batch(gen, xys, obs_length, 0, normalize)
+            device = observed.device
+            B, nd = len(xys), int(gen.noise_dim)
+            if gen.no_noise:
+                noise = None
+            elif noise is not None:
+                noise = torch.as_tensor(noise, dtype=torch.float32).to(device).reshape(modes, B, nd).contiguous()
+            elif gen.fixed_noise is not None:
+                fixed = torch.as_tensor(gen.fixed_noise, dtype=torch.float32).to(device).reshape(1, 1, nd)
+                noise = fixed.expand(modes, B, nd).contiguous()
+            else:
+                noise = get_noise((modes, B, nd), gen.noise_type, device=device).float().contiguous()
+            lin = gen.mlp_decoder_context[0]
+            w = lin.weight.detach().to(device=device, dtype=torch.float32).contiguous()
+            b = lin.bias.detach().to(device=device, dtype=torch.float32).contiguous()
+            context = multimodal.sgan_context(w, b, noise, multimodal.group_of_rows(split, device), B, nd)
+            pred = multimodal.predict_modes(gen, observed, split, n_predict, modes, context, max_rows)
+            return multimodal.scene_results(pred, split, modes, n_predict, normalize, rotation, center)

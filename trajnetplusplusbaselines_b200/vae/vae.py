@@ -6,14 +6,15 @@ LSTM step of lstm/lstm.py (same kernels, `obs_encoder` in the encoder slot); at 
 sample rescales the encoder state, h <- h * ReLU(fc z) (add_noise :87-106 -> tb2_vae_scale_hidden),
 and each of the num_modes decodes from that state.  The observation encoder runs once.  Same
 constructor arguments and state_dict keys.  Training (prediction encoder, KL term) is not built:
-model.train() + forward raises.
+model.train() + forward raises.  VAEPredictor.predict_batch_xy decodes every mode of many scenes at
+once (the evaluator's path, ../multimodal.py).
 """
 import ctypes
 
 import numpy as np
 import torch
 
-from .. import _lib
+from .. import _lib, multimodal
 from ..data import paths_to_xy
 from ..engine import _ptr, _stream
 from ..lstm.lstm import LSTM, center_scene, drop_distant, inverse_scene  # noqa: F401
@@ -180,3 +181,48 @@ class VAEPredictor(object):
                 output_neighs = output_scenes[-n_predict:, 1:]
                 multimodal_outputs[num_p] = [output_primary, output_neighs if num_p == 0 else []]
         return multimodal_outputs
+
+    def batch_decode_supported(self):
+        """predict_batch_xy serves every model except those whose interaction module carries its own LSTM state
+        (NearestNeighborLSTM, TrajectronPooling): that state is not replicated per mode."""
+        return not multimodal.stateful_pool(self.model._body[0])
+
+    def predict_batch_xy(self, xys, scene_goals=None, n_predict=12, obs_length=9, start_length=0, args=None, modes=1,
+                         z=None, max_rows=None):
+        """Every mode of many scenes in one batched decode (the evaluator's column pipeline, multimodal.py).
+
+        xys: list of float64 [n_frames, N_i, 2] as paths_to_xy returns them.  Returns per scene the dictionary of
+        __call__, {mode: [primary [n_predict, 2], neighbours if mode == 0 else []]}.  The latent samples are drawn once
+        per call, on the device, one per (mode, track) from the prior N(0, e I) as in __call__; the model's `fixed_z`
+        ([modes, M, latent_dim] over the M tracks of all scenes) replaces the draw, and so does z (same shape).
+        max_rows: rows of one decode (default: multimodal.rows_per_decode); more modes are decoded in groups."""
+        body = self.model._body[0]
+        if not self.batch_decode_supported():
+            raise NotImplementedError("batched decoding of a model whose interaction module keeps an LSTM state "
+                                      "is not built; call the predictor scene by scene")
+        self.model.eval()
+        if not self.model.desire:
+            raise NotImplementedError("desire=False (latent prior from vae_encoder_x) is not built")
+        modes = int(modes)
+        if modes < 1:
+            raise ValueError("modes must be >= 1")
+        if not xys:
+            return []
+        normalize = bool(getattr(args, 'normalize_scene', False))
+        with torch.no_grad():
+            observed, split, rotation, center = multimodal.observed_batch(body, xys, obs_length, start_length,
+                                                                          normalize)
+            device = observed.device
+            M, L = int(split[-1]), int(self.model.latent_dim)
+            if z is None:
+                z = self.model.fixed_z
+            if z is not None:
+                z = torch.as_tensor(z, dtype=torch.float32).to(device).reshape(modes, M, L).contiguous()
+            else:      # prior N(0, exp(1) I): z_mu_obs = 0, z_var_log_obs = 1 (vae.py:277-278)
+                z = torch.randn((modes, M, L), device=device).mul_(float(np.exp(0.5)))
+            fc = self.model.vae_decoder.fc
+            w = fc.weight.detach().to(device=device, dtype=torch.float32).contiguous()
+            b = fc.bias.detach().to(device=device, dtype=torch.float32).contiguous()
+            pred = multimodal.predict_modes(body, observed, split, n_predict, modes,
+                                            multimodal.vae_context(w, b, z, L), max_rows)
+            return multimodal.scene_results(pred, split, modes, n_predict, normalize, rotation, center)
