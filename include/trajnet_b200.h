@@ -528,6 +528,28 @@ int tb2_kalman_predict(const double* obs_host, const int64_t* track_offsets_host
                        int32_t n_predict, int32_t em_iterations, double* pred_out_host,
                        double* q_out_host, double* r_out_host, double* last_state_out_host);
 
+/* The same predictor on the device: one thread per track runs the EM / smoother code of tb2_kalman_predict (shared
+ * source, no FMA contraction on either side), so pred (without noise), q, r and last state equal the host's bit for bit.
+ *   obs_dev [total_obs, 2], track_offsets_dev [n_tracks + 1]; track_offsets_host: the same offsets on the host, checked
+ *   before the launch (TB2_ERR_INVALID for a track of fewer than 2 observations, like the host; nothing is launched).
+ *   eps_dev [n_tracks, n_predict, 6] standard normals (4 transition + 2 observation per step) or NULL.  With eps_dev and
+ *   n_samples >= 1, pred gets the noise of the mean of n_samples sampled rollouts (kalman.py:53-60), i.e. one rollout
+ *   driven by Q / n_samples and R / n_samples (Cholesky factors with a zero-pivot guard; z_0 dropped like the
+ *   reference's [1:]); eps_dev = NULL or n_samples = 0: the expectation.
+ *   pred_out_dev [n_tracks, n_predict, 2]; q_out_dev [n_tracks,4,4], r_out_dev [n_tracks,2,2],
+ *   last_state_out_dev [n_tracks,4] optional (NULL to skip).  A track whose predicted covariance is singular (the
+ *   host's error) gets NaN in every output.
+ *   workspace_dev: caller-owned, >= tb2_kalman_workspace_bytes(track_offsets_host, n_tracks) bytes
+ *   (T_max x 76 doubles per track: the smoother's per-step arrays, interleaved over the tracks).
+ * Asynchronous on `stream`; n_tracks = 0 launches nothing. */
+size_t tb2_kalman_workspace_bytes(const int64_t* track_offsets_host, int32_t n_tracks);
+int tb2_kalman_predict_device(const double* obs_dev, const int64_t* track_offsets_host,
+                              const int64_t* track_offsets_dev, int32_t n_tracks, int32_t n_predict,
+                              int32_t em_iterations, int32_t n_samples, const double* eps_dev,
+                              double* pred_out_dev, double* q_out_dev, double* r_out_dev,
+                              double* last_state_out_dev, void* workspace_dev, size_t workspace_bytes,
+                              void* stream);
+
 #ifdef __cplusplus
 }
 #endif

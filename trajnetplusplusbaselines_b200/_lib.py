@@ -166,6 +166,9 @@ PROTOTYPES = {
     "tb2_score_scenes": (ctypes.c_int, [_i32, _i32, _i32] + [_vp] * 9 + [_i32] + [_vp] * 5),
     "tb2_sf_simulate": (ctypes.c_int, [_vp, ctypes.POINTER(SfParams), _vp, _vp, _vp]),
     "tb2_kalman_predict": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
+    "tb2_kalman_workspace_bytes": (_sz, [_vp, _i32]),
+    "tb2_kalman_predict_device": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp,
+                                                 _sz, _vp]),
     "tb2_orca_simulate": (ctypes.c_int, [_vp, ctypes.POINTER(OrcaParams), _vp, _vp, _vp, _vp, _vp, _vp]),
     "tb2_sf_sweep": (ctypes.c_int, [_vp, ctypes.POINTER(SfParams), _vp, _i32, _vp, _vp, _i32, _vp, _vp, _vp]),
     "tb2_orca_sweep": (ctypes.c_int, [_vp, ctypes.POINTER(OrcaParams), _vp, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),

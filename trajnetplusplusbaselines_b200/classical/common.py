@@ -74,7 +74,7 @@ def xy_representable(xy):
     return xy.shape[1] > 0 and not np.isnan(xy[:, 0]).any()
 
 
-def initial_states_xy(xy_list, obs_length=9, pred_length=12, dest_type='interp', dest_dict=None):
+def initial_states_xy(xy_list, obs_length=9, pred_length=12, dest_type='interp', dest_dict=None, truth=True):
     """initial_states for every scene of a list, from xy arrays instead of track rows.
 
     xy_list: [(scene_id, scene)] as data.load_scenes_xy returns it, `scene` an xy array [n_frames, n_peds, 2] (NaN =
@@ -88,10 +88,12 @@ def initial_states_xy(xy_list, obs_length=9, pred_length=12, dest_type='interp',
 
     Returns numpy arrays: state [A, 6] float64, speeds [A], agent_offsets [B + 1] int64 (scene b owns rows
     agent_offsets[b] .. agent_offsets[b + 1] - 1, its primary first), truth [B, pred_length, 2] float64 (the primary's
-    last pred_length rows, what metrics.average_l2(paths[0], prediction) compares against).
+    last pred_length rows, what metrics.average_l2(paths[0], prediction) compares against).  truth=False: None instead
+    (test scenes, which hold the observation only).
     """
     if dest_type not in ('interp', 'vel', 'pred_end', 'true'):
         raise NotImplementedError(dest_type)
+    want_truth = truth
     states, speeds, counts, truth = [], [], [], []
     t0 = obs_length - 1
     for _, scene in xy_list:
@@ -106,7 +108,7 @@ def initial_states_xy(xy_list, obs_length=9, pred_length=12, dest_type='interp',
                 raise ValueError("xy array without its primary at every frame: pass the scene's paths")
             st, sp = _initial_states_xy_scene(scene, t0, pred_length, dest_type)
             tr = scene[-pred_length:, 0]
-        if len(tr) < pred_length:
+        if want_truth and len(tr) < pred_length:
             raise ValueError("the primary has %d rows, %d needed for the truth" % (len(tr), pred_length))
         states.append(st)
         speeds.append(sp)
@@ -116,7 +118,7 @@ def initial_states_xy(xy_list, obs_length=9, pred_length=12, dest_type='interp',
     offsets[1:] = np.cumsum(counts)
     return (np.concatenate(states).reshape(-1, 6) if states else np.zeros((0, 6)),
             np.concatenate(speeds) if speeds else np.zeros(0), offsets,
-            np.array(truth, dtype=np.float64).reshape(len(truth), pred_length, 2))
+            np.array(truth, dtype=np.float64).reshape(len(truth), pred_length, 2) if want_truth else None)
 
 
 def _initial_states_xy_scene(xy, t0, pred_length, dest_type):
