@@ -388,7 +388,16 @@ int tb2_collision_loss(const tb2_layout* layout, const float* positions_dev, int
  *   aug [B, 2] = cos(theta), sin(theta); NULL: skip); xy_out float32 [T, M_out, 2].  The O(B) scalars of `frame` / `aug` come
  *   from the caller (the reference's own libm calls on the primary's last two observed positions).
  * tb2_scenes_inverse -- inverse_scene (augmentation.py:65-68) of float32 predictions [S, M, 2]: rotation by
- *   frame [B, 4] = centre x, centre y, cos(-rotation), sin(-rotation), then + centre; xy_out float64 [S, M, 2]. */
+ *   frame [B, 4] = centre x, centre y, cos(-rotation), sin(-rotation), then + centre; xy_out float64 [S, M, 2].
+ * tb2_scenes_gather_epoch -- every batch of a training epoch (lstm/trainer.py:96-133) in one launch, from a scene store
+ *   xy [T, M] with scene_off [n_store + 1], the drop_distant mask `keep` [M] (NULL: keep all) and kept_count [n_store].
+ *   Epoch position p holds store scene perm[p] (p < n) and belongs to batch p / batch_size.  Batch k is written as ONE
+ *   contiguous float32 block [T, batch_tracks[k], 2] starting at float2 element batch_base[k] of xy_out; inside it the
+ *   scenes' kept tracks follow in position order (np.concatenate(axis=1)).  Per scene, in the reference's order: ordered
+ *   compaction by `keep`, center_scene (frame [n_store, 4] indexed by STORE scene; NULL: skip), random_rotation
+ *   (aug [n, 2] = cos, sin of theta indexed by epoch POSITION; NULL: skip), add_noise(ped='neigh') = `+=` of the float64
+ *   values noise[noise_off[p] + (t * (kept - 1) + j - 1) * 2 + c] on frames t < noise_frames of kept columns j >= 1
+ *   (NULL: skip; the reference's window is 9 frames whatever obs_length is), then one rounding to float32. */
 int tb2_scenes_drop_distant(const double* xy_dev, const int32_t* scene_off_dev, int32_t T, int32_t M, int32_t B,
                             double r_squared, uint8_t* keep_out_dev, int32_t* kept_count_out_dev, void* stream);
 int tb2_scenes_transform(const double* xy_dev, const int32_t* scene_off_dev, const uint8_t* keep_dev,
@@ -396,6 +405,11 @@ int tb2_scenes_transform(const double* xy_dev, const int32_t* scene_off_dev, con
                          const double* frame_dev, const double* aug_dev, float* xy_out_dev, void* stream);
 int tb2_scenes_inverse(const float* xy_dev, const int32_t* scene_off_dev, int32_t S, int32_t M, int32_t B,
                        const double* frame_dev, double* xy_out_dev, void* stream);
+int tb2_scenes_gather_epoch(const double* xy_dev, const int32_t* scene_off_dev, const uint8_t* keep_dev,
+                            const int32_t* kept_count_dev, int32_t T, int32_t M, const int32_t* perm_dev, int32_t n,
+                            int32_t batch_size, const int64_t* batch_base_dev, const int32_t* batch_tracks_dev,
+                            const double* frame_dev, const double* aug_dev, const double* noise_dev,
+                            const int64_t* noise_off_dev, int32_t noise_frames, float* xy_out_dev, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Host-side ndjson codec of the batched evaluator path (SURVEY.md 8f rank 1; no CUDA).  The TrajNet++ on-disk format as the

@@ -160,6 +160,8 @@ PROTOTYPES = {
     "tb2_scenes_drop_distant": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i32, ctypes.c_double, _vp, _vp, _vp]),
     "tb2_scenes_transform": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
     "tb2_scenes_inverse": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i32, _vp, _vp, _vp]),
+    "tb2_scenes_gather_epoch": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp,
+                                               _vp, _i32, _vp, _vp]),
     "tb2_ndjson_parse": (ctypes.c_int, [_vp, _sz, ctypes.c_int64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "tb2_ndjson_format": (ctypes.c_int64, [ctypes.c_int64, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, ctypes.c_int64]),
     "tb2_ndjson_parse_meta": (ctypes.c_int, [_vp, _sz, ctypes.c_int64] + [_vp] * 15),
