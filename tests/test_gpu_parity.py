@@ -420,16 +420,28 @@ def test_evaluate_file_batched_equals_per_scene(tmp_path):
         assert np.allclose([[r.x, r.y] for r in got[sid][0]], np.round(single[0], 2), atol=0.011)
 
 
+def _pool_of(kind):
+    """The interaction module of an oracle spec name (grid or non-grid)."""
+    from trajnetplusplusbaselines_b200 import lstm as L
+    for specs, cls in ((O.NONGRID_SPECS, L.HiddenStateMLPPooling), (O.ATTN_SPECS, L.AttentionMLPPooling),
+                       (O.NN_SPECS, L.NearestNeighborMLP), (O.NN_LSTM_SPECS, L.NearestNeighborLSTM),
+                       (O.TRAJ_SPECS, L.TrajectronPooling), (O.MODEL_SPECS, L.GridBasedPooling)):
+        if kind in specs:
+            return cls(**specs[kind])
+    raise KeyError(kind)
+
+
 @pytest.mark.gpu
-@pytest.mark.parametrize("kind", ["social", "occupancy"])
+@pytest.mark.parametrize("kind", ["social", "occupancy", "hiddenstatemlp", "attentionmlp", "nn", "nn_lstm", "traj_pool"])
 def test_per_scene_layout_equals_single_scene_calls(kind):
-    """Ragged batch with tb2_layout_set_padding(0) == every scene forwarded alone, bit for bit; with the
-    default (trainer) padding the small scenes see the padded slots, as in the reference's batched call."""
-    from trajnetplusplusbaselines_b200.lstm import LSTM, GridBasedPooling
+    """Ragged batch with tb2_layout_set_padding(0) == every scene forwarded alone, bit for bit (every non-grid kernel
+    works per scene or per row); with the default (trainer) padding the small scenes see the padded slots, as in the
+    reference's batched call."""
+    from trajnetplusplusbaselines_b200.lstm import LSTM
     xy, bs = O.synthetic_scenes(10, 9, seed=77, ragged=True, nan_tracks=True)
     xy[:, :, :] = xy * 1.6                 # spread: more neighbours out of range / in the corner cell
     W = O.random_weights(kind, seed=12)
-    model = LSTM(pool=GridBasedPooling(**O.MODEL_SPECS[kind]))
+    model = LSTM(pool=_pool_of(kind))
     model.load_state_dict({k: torch.from_numpy(v.copy()) for k, v in W.items()})
     model = model.cuda().eval()
     obs = torch.from_numpy(xy[:9]).cuda()

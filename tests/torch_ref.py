@@ -1,9 +1,13 @@
 """Differentiable torch restatement of LSTM.forward + PredictionLoss (fp32 or fp64) -- TEST INFRASTRUCTURE.
 
-Used only to check the hand-written CUDA backward (csrc/train.cu).  Follows oracle/lstm_oracle.py (which is
+Used to check the hand-written CUDA backward (csrc/train.cu).  Follows oracle/lstm_oracle.py (which is
 pinned to the reference) line by line, with torch ops so autograd provides the gradients;
 test_training.py, test_social_backward.py and test_grid_backward.py pin THIS file's gradients to gradients
 of the unmodified reference (tests/golden/train_golden.npz, social_train_golden.npz, grid_train_golden.npz).
+
+The non-grid interaction modules (nongrid_pool, and `forward` with such a pool) are restated from the reference's
+lstm/non_gridbased_pooling.py directly, not from the oracle, and checked against csrc/mlp_pool.cu in
+test_nongrid_kernels.py; that file pins them to tests/golden/nongrid_golden.npz.
 """
 import math
 
@@ -94,14 +98,196 @@ def _note(stats, key, value):
         stats[key] = min(value, stats.get(key, math.inf))
 
 
+NONGRID = ("hiddenstatemlp", "attentionmlp", "nn", "nn_lstm", "traj_pool")
+
+
+def _embed_masked(x, w, b, fill):
+    """embed_with_masking (non_gridbased_pooling.py:52-60): relu(Linear(x)) where x has no NaN, else `fill`."""
+    bad = torch.isnan(x).any(dim=-1, keepdim=True)
+    y = torch.relu(torch.nan_to_num(x) @ w.T + b)
+    return torch.where(bad, torch.full_like(y, float(fill)), y)
+
+
+def _pad_slots(x, slots):
+    """[n, ...] -> [slots, ...]: the slots past the scene's tracks are absent tracks (NaN)."""
+    return torch.cat([x, torch.full((slots - x.shape[0],) + tuple(x.shape[1:]), NAN, dtype=x.dtype)])
+
+
+def _hidden_mlp(cfg, W, hid, p1, p2):
+    """HiddenStateMLPPooling (:197-239) on one scene [N, ...]: max over every slot j (i included) of
+    [spatial(p_j - p_i) | hidden(h_j) | vel(4 (v_j - v_i))], NaN inputs -> -100, then out_projection."""
+    N = p2.shape[0]
+    parts = [_embed_masked(p2[None, :, :] - p2[:, None, :], W["pool.spatial_embedding.0.weight"],
+                           W["pool.spatial_embedding.0.bias"], -100.0)]
+    if cfg.mlp_dim_hidden:
+        e = _embed_masked(hid, W["pool.hidden_embedding.0.weight"], W["pool.hidden_embedding.0.bias"], -100.0)
+        parts.append(e[None].expand(N, N, e.shape[-1]))
+    if cfg.mlp_dim_vel:
+        v = p2 - p1
+        parts.append(_embed_masked((v[None, :, :] - v[:, None, :]) * 4.0, W["pool.vel_embedding.0.weight"],
+                                   W["pool.vel_embedding.0.bias"], -100.0))
+    pooled = torch.cat(parts, dim=-1).max(dim=1).values
+    return pooled @ W["pool.out_projection.weight"].T + W["pool.out_projection.bias"]
+
+
+def _attention(cfg, W, hid, p1, p2, n, stats=None, rows=None):
+    """AttentionMLPPooling (:297-351) on one scene of N slots whose first n are tracks: for track i the sequence is
+    e_ij over every slot j, NaN inputs -> fill_value (spatial, velocity) / 0 (hidden); wq / wk / wv, then one-head
+    MultiheadAttention computed the plain way (in-projection, softmax(q k / sqrt(E)), value sum, out_proj); the
+    output at position i, then out_projection.  The slots past n all embed to one vector: its key and value are
+    computed once and repeated.  rows: only the first `rows` tracks query (default n).
+    stats["attn_span"]: the smallest (over the tracks) max - min of a track's logits."""
+    N, E, fill = p2.shape[0], cfg.mlp_dim, float(cfg.fill_value)
+
+    def emb(rel, h, relv):
+        parts = [_embed_masked(rel, W["pool.spatial_embedding.0.weight"], W["pool.spatial_embedding.0.bias"], fill)]
+        if cfg.mlp_dim_hidden:
+            parts.append(_embed_masked(h, W["pool.hidden_embedding.0.weight"], W["pool.hidden_embedding.0.bias"], 0.0))
+        if cfg.mlp_dim_vel:
+            parts.append(_embed_masked(relv, W["pool.vel_embedding.0.weight"], W["pool.vel_embedding.0.bias"], fill))
+        return torch.cat(parts, dim=-1)
+
+    v = p2 - p1
+    r = n if rows is None else rows
+    e = emb((p2[None, :n] - p2[:r, None]), hid[None, :n].expand(r, n, hid.shape[-1]),
+            (v[None, :n] - v[:r, None]) * 4.0)                                   # [i < r, j < n, E]
+    nan2 = torch.full((2,), NAN, dtype=p2.dtype)
+    e_pad = emb(nan2, torch.full((hid.shape[-1],), NAN, dtype=p2.dtype), nan2)  # [E]: a slot past n
+    Win, bin_ = W["pool.multihead_attn.in_proj_weight"], W["pool.multihead_attn.in_proj_bias"]
+    diag = torch.arange(r)
+    q = (e[diag, diag] @ W["pool.wq.weight"].T) @ Win[:E].T + bin_[:E]         # [i, E]: the query at position i
+
+    def kv(x, r):
+        return (x @ W["pool.w%s.weight" % "kv"[r]].T) @ Win[(r + 1) * E:(r + 2) * E].T + bin_[(r + 1) * E:(r + 2) * E]
+    k = torch.cat([kv(e, 0), kv(e_pad, 0)[None, None].expand(r, N - n, E)], dim=1)
+    val = torch.cat([kv(e, 1), kv(e_pad, 1)[None, None].expand(r, N - n, E)], dim=1)
+    s = torch.einsum("ie,ije->ij", q, k) / math.sqrt(E)
+    _note(stats, "attn_span", float((s.max(dim=1).values - s.min(dim=1).values).min()))
+    a = torch.exp(s - s.max(dim=1, keepdim=True).values)
+    a = a / a.sum(dim=1, keepdim=True)
+    att = torch.einsum("ij,ije->ie", a, val)
+    att = att @ W["pool.multihead_attn.out_proj.weight"].T + W["pool.multihead_attn.out_proj.bias"]
+    return att @ W["pool.out_projection.weight"].T + W["pool.out_projection.bias"]
+
+
+def _nearest(cfg, W, p1, p2, stats):
+    """NearestNeighborMLP (:96-147) on one scene [N, 2]: the n nearest other slots in ascending distance (NaN -> 1000),
+    features [p_j - p_i | v_j - v_i] (NaN -> 0; zero rows when there are fewer than n), shared Linear + ReLU.
+
+    stats["nn_gap"]: the smallest gap between consecutive ranks up to rank n + 1 of a track whose two neighbours have
+    different features (a tie between equal feature rows cannot change the output)."""
+    N, nn = p2.shape[0], cfg.n
+    keep = ~torch.eye(N, dtype=torch.bool)
+    rel = (p2[None, :, :] - p2[:, None, :])[keep].reshape(N, N - 1, 2)
+    feat = rel
+    if not cfg.no_vel:
+        v = p2 - p1
+        feat = torch.cat([rel, (v[None, :, :] - v[:, None, :])[keep].reshape(N, N - 1, 2)], dim=-1)
+    feat = torch.nan_to_num(feat)
+    dist = torch.nan_to_num(torch.sqrt(rel[..., 0] ** 2 + rel[..., 1] ** 2), nan=1000.0)
+    d_sorted, order = torch.sort(dist, dim=1, stable=True)
+    g = torch.gather(feat, 1, order[..., None].expand(N, N - 1, feat.shape[-1]))
+    r = min(nn + 1, N - 1)
+    if stats is not None and r >= 2:
+        gap = d_sorted[:, 1:r] - d_sorted[:, :r - 1]
+        same = (g[:, 1:r] == g[:, :r - 1]).all(dim=-1)
+        gap = gap[~same]
+        if gap.numel():
+            _note(stats, "nn_gap", float(gap.min()))
+    g = g[:, :nn]
+    if g.shape[1] < nn:
+        g = torch.cat([g, torch.zeros(N, nn - g.shape[1], g.shape[-1], dtype=g.dtype)], dim=1)
+    return torch.relu(g @ W["pool.embedding.0.weight"].T + W["pool.embedding.0.bias"]).reshape(N, -1)
+
+
+def _pool_lstm(W, x, state):
+    """The interaction-encoder LSTMCell (:445-451): advances state = {"h", "c"} row by row, returns hidden2pool(h')."""
+    g = x @ W["pool.pool_lstm.weight_ih"].T + W["pool.pool_lstm.bias_ih"] + \
+        state["h"] @ W["pool.pool_lstm.weight_hh"].T + W["pool.pool_lstm.bias_hh"]
+    H = state["h"].shape[1]
+    c2 = torch.sigmoid(g[:, H:2 * H]) * state["c"] + torch.sigmoid(g[:, :H]) * torch.tanh(g[:, 2 * H:3 * H])
+    h2 = torch.sigmoid(g[:, 3 * H:]) * torch.tanh(c2)
+    state["h"], state["c"] = h2, c2
+    return h2 @ W["pool.hidden2pool.weight"].T + W["pool.hidden2pool.bias"]
+
+
+def _trajectron_feat(W, p1, p2):
+    """TrajectronPooling's features (:509-529) over the rows it is given (the whole flattened batch): a visible row
+    embeds [own (pos, vel) | sum of (pos, vel) over the OTHER visible rows], an invisible row is 0."""
+    st = torch.cat([p2, p2 - p1], dim=-1)
+    vis = ~torch.isnan(st).any(dim=-1)
+    others = st[vis].sum(dim=0)[None] - st
+    y = torch.relu(torch.cat([st, others], dim=-1) @ W["pool.embedding.0.weight"].T + W["pool.embedding.0.bias"])
+    return torch.where(vis[:, None], y, torch.zeros_like(y))
+
+
+def nongrid_pool(cfg, W, hidden, obs1, obs2, dtype=torch.float64, state=None, stats=None):
+    """The stand-alone plug of a non-grid module: hidden [B, N, H] (or None), obs1 / obs2 [B, N, 2] fp32 (NaN = absent)
+    -> [B * N, out_dim] in `dtype`.  state: {"h", "c"} [B * N, Hp] of nn_lstm / traj_pool, advanced in place.
+    stats: see _nearest."""
+    W = {k: torch.as_tensor(v).to(dtype) for k, v in W.items() if k.startswith("pool.")}
+    p1, p2 = torch.as_tensor(obs1).to(dtype), torch.as_tensor(obs2).to(dtype)
+    B, N, _ = p2.shape
+    hid = torch.as_tensor(hidden).to(dtype) if hidden is not None else None
+    if cfg.type_ == "traj_pool":
+        return _pool_lstm(W, _trajectron_feat(W, p1.reshape(B * N, 2), p2.reshape(B * N, 2)), state)
+    out = []
+    for b in range(B):
+        if cfg.type_ == "hiddenstatemlp":
+            out.append(_hidden_mlp(cfg, W, hid[b], p1[b], p2[b]))
+        elif cfg.type_ == "attentionmlp":
+            out.append(_attention(cfg, W, hid[b], p1[b], p2[b], N, stats))
+        else:
+            out.append(_nearest(cfg, W, p1[b], p2[b], stats))
+    out = torch.cat(out)
+    return _pool_lstm(W, out, state) if cfg.type_ == "nn_lstm" else out
+
+
+def nongrid_pool_ragged(pool_cfg, W, h, obs1, obs2, bs, pad_to_batch_max=True, dtype=torch.float64, pool_state=None,
+                        stats=None):
+    """The non-grid pool as LSTM.step calls it, on ragged rows: h [M, H] (or None), obs1 / obs2 [M, 2] -> [M, out_dim].
+    Scenes padded to the batch maximum (the reference's batched call) or each scene on its own slots
+    (pad_to_batch_max=False); the interaction-encoder state is one row per track."""
+    bs = [int(v) for v in bs]
+    B = len(bs) - 1
+    n_max = max(bs[b + 1] - bs[b] for b in range(B))
+    p1, p2 = torch.as_tensor(obs1).to(dtype), torch.as_tensor(obs2).to(dtype)
+    h = torch.as_tensor(h).to(dtype) if h is not None else torch.full((bs[-1], 1), NAN, dtype=dtype)
+    Wp = {k: torch.as_tensor(v).to(dtype) for k, v in W.items() if k.startswith("pool.")}
+    if pool_cfg.type_ == "traj_pool":
+        if pad_to_batch_max:
+            feat = _trajectron_feat(Wp, p1, p2)
+        else:
+            feat = torch.cat([_trajectron_feat(Wp, p1[bs[b]:bs[b + 1]], p2[bs[b]:bs[b + 1]]) for b in range(B)])
+        return _pool_lstm(Wp, feat, pool_state)
+    out = []
+    for b in range(B):
+        s, e = bs[b], bs[b + 1]
+        n = e - s
+        slots = n_max if pad_to_batch_max else n
+        q1, q2 = _pad_slots(p1[s:e], slots), _pad_slots(p2[s:e], slots)
+        if pool_cfg.type_ == "hiddenstatemlp":
+            y = _hidden_mlp(pool_cfg, Wp, _pad_slots(h[s:e], slots), q1, q2)
+        elif pool_cfg.type_ == "attentionmlp":
+            y = _attention(pool_cfg, Wp, _pad_slots(h[s:e], slots), q1, q2, n, stats)
+        else:
+            y = _nearest(pool_cfg, Wp, q1, q2, stats)
+        out.append(y[:n])
+    out = torch.cat(out)
+    return _pool_lstm(Wp, out, pool_state) if pool_cfg.type_ == "nn_lstm" else out
+
+
 def forward(W, pool_cfg, observed, batch_split, prediction_truth=None, n_predict=None, hidden_dim=128,
-            dtype=torch.float32, stats=None, feed_back=None):
+            dtype=torch.float32, stats=None, feed_back=None, pad_to_batch_max=True):
     """W: dict of `dtype` tensors (requires_grad as wanted).  Returns rel [S, M, 5] (`dtype`), pred [S, M, 2]
     (fp32: the positions the model feeds back are fp32 data, as in the reference).  stats: see _grid.
 
     feed_back: fp32 positions [S(+1), M, 2] of another implementation's forward (aligned with pred).  The
     decoder is then fed those (detached) positions instead of this forward's own, so the gradients are
-    exact for that implementation's trajectory and no fed-back position can be binned differently."""
+    exact for that implementation's trajectory and no fed-back position can be binned differently.
+
+    pad_to_batch_max: with a non-grid pool, False gives each scene its own slots (the per-scene layout): the
+    attention keys stop at the scene's tracks and Trajectron's sums at its scene."""
     bs = [int(v) for v in batch_split]
     B = len(bs) - 1
     M = observed.shape[1]
@@ -110,6 +296,11 @@ def forward(W, pool_cfg, observed, batch_split, prediction_truth=None, n_predict
     h = torch.zeros(M, hidden_dim, dtype=dtype)
     c = torch.zeros(M, hidden_dim, dtype=dtype)
     truth = [None] * (n_predict - 1) if n_predict is not None else [t.clone() for t in prediction_truth]
+    nongrid = getattr(pool_cfg, "type_", None) in NONGRID
+    pool_state = None
+    if nongrid and pool_cfg.type_ in ("nn_lstm", "traj_pool"):      # pool.reset(...) at the start (lstm.py:213-216)
+        pool_state = {"h": torch.zeros(M, pool_cfg.hidden_dim, dtype=dtype),
+                      "c": torch.zeros(M, pool_cfg.hidden_dim, dtype=dtype)}
 
     def pad(x, fill):
         out = torch.full((B, n_max) + tuple(x.shape[1:]), fill, dtype=x.dtype)
@@ -123,7 +314,10 @@ def forward(W, pool_cfg, observed, batch_split, prediction_truth=None, n_predict
         e = torch.relu((vel * 4.0) @ W["input_embedding.input_embeddings.0.weight"].T +
                        W["input_embedding.input_embeddings.0.bias"])
         x = torch.cat([e, torch.zeros(e.shape[0], 2, dtype=dtype)], dim=1)
-        if pool_cfg is not None:
+        if nongrid:
+            pooled = nongrid_pool_ragged(pool_cfg, W, h.detach(), obs1, obs2, bs, pad_to_batch_max, dtype, pool_state, stats)
+            x = torch.cat([x, pooled[mask]], dim=1)
+        elif pool_cfg is not None:
             pooled = _grid(pool_cfg, W, pad(obs1, NAN), pad(obs2, NAN), pad(h, NAN), dtype, stats,
                            primary_edges=phase == "decoder")
             x = torch.cat([x, pooled[pad(mask, False).reshape(-1)]], dim=1)

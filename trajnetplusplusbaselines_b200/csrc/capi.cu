@@ -224,7 +224,7 @@ int tb2_lstm_create(const tb2_lstm_config* cfg, tb2_lstm** out) {
     for (int i = 0; i < 2; ++i) { m->WgT[i] = m->bg[i] = nullptr; m->Wg_hi[i] = m->Wg_lo[i] = nullptr; }
     for (int i = 0; i < kMaxMlpLayers; ++i) { m->WT[i] = m->bl[i] = nullptr; m->W_hi[i] = m->W_lo[i] = nullptr; }
     m->mp_Ws = m->mp_bs = m->mp_Wv = m->mp_bv = m->mp_WhT = m->mp_bh = m->mp_WoT = m->mp_bo = nullptr;
-    m->at_AqT = m->at_AkT = m->at_AvT = m->at_bqkv = m->at_WoT = m->at_bo = nullptr;
+    m->at_AqT = m->at_Ak = m->at_AvT = m->at_bqkv = m->at_WoT = m->at_bo = nullptr;
     m->pl_WihT = m->pl_WhhT = m->pl_b = nullptr;
     auto fail = [&](int rc) { tb2_lstm_destroy(m); return rc; };
     if (cfg->pool_type == TB2_POOL_TRAJECTRON) {
@@ -342,7 +342,7 @@ int tb2_lstm_create(const tb2_lstm_config* cfg, tb2_lstm** out) {
     if (cfg->pool_type == TB2_POOL_ATTN_MLP) {
         const size_t Ea = (size_t)(cfg->mlp_dim_spatial + cfg->mlp_dim_vel + cfg->mlp_dim_hidden);
         ALLOC(m->at_AqT, Ea * Ea);
-        ALLOC(m->at_AkT, Ea * Ea);
+        ALLOC(m->at_Ak, Ea * Ea);
         ALLOC(m->at_AvT, Ea * Ea);
         ALLOC(m->at_bqkv, 3 * Ea);
         ALLOC(m->at_WoT, Ea * Ea);

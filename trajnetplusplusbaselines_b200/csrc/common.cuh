@@ -136,9 +136,9 @@ struct tb2_lstm {
     std::vector<cudaEvent_t> step_events;     // tb2_lstm_forward_sequence_host: one event per recurrence step
     // HiddenStateMLPPooling (TB2_POOL_HIDDEN_MLP)
     float *mp_Ws, *mp_bs, *mp_Wv, *mp_bv, *mp_WhT, *mp_bh, *mp_WoT, *mp_bo;
-    // AttentionMLPPooling (TB2_POOL_ATTN_MLP): in-projection . wq / wk / wv combined and transposed [E in][E out], biases,
-    // out-projection transposed
-    float *at_AqT, *at_AkT, *at_AvT, *at_bqkv, *at_WoT, *at_bo;
+    // AttentionMLPPooling (TB2_POOL_ATTN_MLP): in-projection . wq / wk / wv combined, q and v transposed [E in][E out],
+    // k [E out][E in]; biases, out-projection transposed
+    float *at_AqT, *at_Ak, *at_AvT, *at_bqkv, *at_WoT, *at_bo;
     // NearestNeighborLSTM (TB2_POOL_NN_LSTM): interaction-encoder LSTMCell, weights transposed [in][4 Hp], fused bias
     float *pl_WihT, *pl_WhhT, *pl_b;
     void* Wg_hi[2];        // gate weights [4H (rank, gate, unit), K_gate] bf16 split (null: FFMA gates)

@@ -288,13 +288,15 @@ __global__ void add_bias_kernel(const float* __restrict__ a, const float* __rest
 }
 
 // outT[c][o] = sum_m Win[o][m] * w[m][c]   (E x E matrices; AttentionMLPPooling: in-projection after wq / wk / wv)
-__global__ void combine_proj_kernel(const float* __restrict__ Win, const float* __restrict__ w, float* __restrict__ outT, int E) {
+// out_major = 0: stored transposed [c][o]; 1: stored [o][c]
+__global__ void combine_proj_kernel(const float* __restrict__ Win, const float* __restrict__ w, float* __restrict__ out, int E,
+                                    int out_major) {
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
     if (idx >= E * E) return;
     const int c = idx / E, o = idx - c * E;
     float acc = 0.f;
     for (int mm = 0; mm < E; ++mm) acc = fmaf(Win[(size_t)o * E + mm], w[(size_t)mm * E + c], acc);
-    outT[idx] = acc;
+    out[out_major ? (size_t)o * E + c : (size_t)idx] = acc;
 }
 
 __global__ void transpose_kernel(const float* __restrict__ W, float* __restrict__ WT, int N, int K) {
@@ -397,12 +399,13 @@ int launch_repack(tb2_lstm* m, const tb2_lstm_weights* w, cudaStream_t st) {
         TB2_REQUIRE(w->pool_attn_wq && w->pool_attn_wk && w->pool_attn_wv && w->pool_attn_in_proj_weight &&
                     w->pool_attn_in_proj_bias && w->pool_attn_out_proj_weight && w->pool_attn_out_proj_bias,
                     "pool.wq / wk / wv / multihead_attn parameters missing");
-        // in-projection . w{q,k,v}: A[o][c] = sum_m Win[o][m] w[m][c], stored transposed [c][o]
+        // in-projection . w{q,k,v}: A[o][c] = sum_m Win[o][m] w[m][c], stored transposed [c][o] for q and v, [o][c] for k
+        // (attn_mlp_pool_kernel reads Ak^T q with a lane per c)
         const float* wqkv[3] = {w->pool_attn_wq, w->pool_attn_wk, w->pool_attn_wv};
-        float* outT[3] = {m->at_AqT, m->at_AkT, m->at_AvT};
+        float* outA[3] = {m->at_AqT, m->at_Ak, m->at_AvT};
         for (int i = 0; i < 3; ++i) {
             combine_proj_kernel<<<(Ea * Ea + 255) / 256, 256, 0, st>>>(w->pool_attn_in_proj_weight + (size_t)i * Ea * Ea, wqkv[i],
-                                                                     outT[i], Ea);
+                                                                     outA[i], Ea, i == 1);
             TB2_LAUNCH_CHECK();
         }
         if ((rc = copy_dev(w->pool_attn_in_proj_bias, m->at_bqkv, (size_t)3 * Ea, st))) return rc;

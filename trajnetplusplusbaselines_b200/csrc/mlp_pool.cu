@@ -146,10 +146,14 @@ int launch_hidden_mlp_pool(const tb2_lstm* m, const tb2_layout* l, const float* 
 //   q = (Aq e + bq) / sqrt(E), k = Ak e + bk, v = Av e + bv with A* = in-projection . w{q,k,v} (combined at
 //   tb2_lstm_set_weights), out_i = Wout (Wo (softmax_j(q_i . k_ij) v_ij) + bo) + bout.
 //
-// The key / value maps are linear, so the pair part is folded: with f_ij the (spatial | velocity) features,
-//   q_i . k_ij = u_i . f_ij + q_i . Hk_j,   u_i = Ak_sv^T q_i,   Hk_j = Ak_h hemb_j + bk   (per track, not per pair)
-//   sum_j a_ij v_ij = Av_sv (sum_j a_ij f_ij) + sum_j a_ij Hv_j
-// which leaves ~200 FMAs per pair instead of 2 x E x E.  One CTA per scene, one warp per track, online softmax.
+// The key / value maps are linear, so the whole pair part is folded:
+//   q_i . k_ij = u_i . e_ij + q_i . bk,   u_i = Ak^T q_i   (per track, not per pair; q_i . bk is the same for every j
+//                                                            and cancels in the softmax, so it is dropped)
+//   sum_j a_ij v_ij = Av (sum_j a_ij e_ij) + bv             (the weights a_ij sum to 1)
+// which leaves ~4 E operations per pair instead of 2 x E x E.  One CTA per scene, one warp per track, online softmax.
+// Shared memory holds what every warp reads -- pos, vel and the hidden embedding of every slot, (4 + dh) floats per
+// slot -- and the queries / attention outputs of one chunk of 32 tracks (2 x 32 x E floats), whose projections run over
+// the whole CTA; a scene of (200 KB - 32 KB) / ((4 + dh) x 4 B) slots fits: 632 at the default widths (dh = 64).
 // ------------------------------------------------------------------------------------------
 struct AttnPoolParams {
     const float2* obs1;
@@ -157,7 +161,7 @@ struct AttnPoolParams {
     const float* hidden;
     const int* scene_off;
     const float *Ws, *bs, *Wv, *bv, *WhT, *bh;      // embeddings (WhT [H][dh])
-    const float *AqT, *AkT, *AvT, *bqkv;            // [E][E] transposed (input-major), biases [3E]
+    const float *AqT, *Ak, *AvT, *bqkv;             // [E][E]: Aq, Av transposed (input-major), Ak output-major; biases [3E]
     const float *WoT, *bo;                          // attention out-projection [E][E] transposed, [E]
     const float *WoutT, *bout;                      // out_projection [E][out_dim] transposed, [out_dim]
     float* out;
@@ -165,33 +169,32 @@ struct AttnPoolParams {
     float fill;
 };
 
-__global__ void __launch_bounds__(256) attn_mlp_pool_kernel(AttnPoolParams p) {
+constexpr int kAtThreads = 256, kAtWarps = kAtThreads / 32, kAtChunk = 32;
+
+__global__ void __launch_bounds__(kAtThreads) attn_mlp_pool_kernel(AttnPoolParams p) {
     extern __shared__ __align__(16) float smem_at[];
     const int scene = blockIdx.x;
     const int row0 = p.scene_off[scene];
     const int n = p.scene_off[scene + 1] - row0;
     const int ns = p.pad_to_max ? p.n_max : n;                     // slots of the sequence (padded slots are absent tracks)
-    const int E = p.ds + p.dh + p.dv, dsv = p.ds + p.dv;
-    float2* pos = reinterpret_cast<float2*>(smem_at);              // [ns] obs2 (NaN kept / NaN for padded slots)
+    const int E = p.ds + p.dh + p.dv, dsh = p.ds + p.dh;
+    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    float* qb = smem_at;                                           // [kAtChunk][E] scaled queries, later Wo att + bo
+    float* ab = qb + (size_t)kAtChunk * E;                         // [kAtChunk][E] attention outputs
+    float2* pos = reinterpret_cast<float2*>(ab + (size_t)kAtChunk * E);   // [ns] obs2 (NaN for padded slots)
     float2* vel = pos + ns;                                        // [ns] 4 x velocity is applied at use
     float* hemb = reinterpret_cast<float*>(vel + ns);              // [ns][dh]  (0 for absent rows)
-    float* Hk = hemb + (size_t)ns * p.dh;                          // [ns][E]
-    float* Hv = Hk + (size_t)ns * E;                               // [ns][E]
-    float* q = Hv + (size_t)ns * E;                                // [n][E]   (scaled query)
-    float* att = q + (size_t)n * E;                                // [n][E]   attention output before the projections
-    float* tmp = att + (size_t)n * E;                              // [n][E]
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, nwarps = blockDim.x >> 5;
-    const float scale = rsqrtf((float)E) ;
+    const float scale = rsqrtf((float)E);
     grid_dep_wait();
     grid_dep_launch();
-    for (int j = tid; j < ns; j += blockDim.x) {
+    for (int j = tid; j < ns; j += kAtThreads) {
         float2 a = make_float2(CUDART_NAN_F, CUDART_NAN_F), b = a;
         if (j < n) { a = p.obs1[row0 + j]; b = p.obs2[row0 + j]; }
         pos[j] = b;
         vel[j] = make_float2(b.x - a.x, b.y - a.y);
     }
     // hidden embedding of every slot (a row with a NaN, or a padded slot, embeds to 0)
-    for (int idx = tid; idx < ns * p.dh; idx += blockDim.x) {
+    for (int idx = tid; idx < ns * p.dh; idx += kAtThreads) {
         const int j = idx / p.dh, k = idx - j * p.dh;
         float val = 0.f;
         if (j < n) {
@@ -208,112 +211,102 @@ __global__ void __launch_bounds__(256) attn_mlp_pool_kernel(AttnPoolParams p) {
         hemb[idx] = val;
     }
     __syncthreads();
-    // Hk_j = Ak[:, hidden part] hemb_j + bk,  Hv_j likewise
-    for (int idx = tid; idx < ns * E; idx += blockDim.x) {
-        const int j = idx / E, o = idx - j * E;
-        float ak = p.bqkv[E + o], av = p.bqkv[2 * E + o];
-        for (int c = 0; c < p.dh; ++c) {
-            const float hv = hemb[j * p.dh + c];
-            ak = fmaf(__ldg(p.AkT + (size_t)(p.ds + c) * E + o), hv, ak);
-            av = fmaf(__ldg(p.AvT + (size_t)(p.ds + c) * E + o), hv, av);
+    // the tracks in chunks of kAtChunk: the projections run over the whole CTA, the attention one warp per track
+    for (int i0 = 0; i0 < n; i0 += kAtChunk) {
+        const int nc = min(kAtChunk, n - i0);
+        // q_i = (Aq e_ii + bq) / sqrt(E), e_ii = [relu(bs) | hemb_i | relu(bv)] (fill where the track itself is absent)
+        for (int idx = tid; idx < nc * E; idx += kAtThreads) {
+            const int t = idx / E, o = idx - t * E, i = i0 + t;
+            const bool pbad = isnan(pos[i].x) || isnan(pos[i].y), vbad = isnan(vel[i].x) || isnan(vel[i].y);
+            float acc = p.bqkv[o];
+            for (int c = 0; c < p.ds; ++c) acc = fmaf(__ldg(p.AqT + (size_t)c * E + o), pbad ? p.fill : fmaxf(p.bs[c], 0.f), acc);
+            for (int c = 0; c < p.dh; ++c) acc = fmaf(__ldg(p.AqT + (size_t)(p.ds + c) * E + o), hemb[i * p.dh + c], acc);
+            for (int c = 0; c < p.dv; ++c)
+                acc = fmaf(__ldg(p.AqT + (size_t)(dsh + c) * E + o), vbad ? p.fill : fmaxf(p.bv[c], 0.f), acc);
+            qb[idx] = acc * scale;
         }
-        Hk[idx] = ak;
-        Hv[idx] = av;
-    }
-    // q_i = (Aq e_ii + bq) / sqrt(E), e_ii = [relu(bs) | hemb_i | relu(bv)] (fill where the track itself is absent)
-    for (int idx = tid; idx < n * E; idx += blockDim.x) {
-        const int i = idx / E, o = idx - i * E;
-        const bool pbad = isnan(pos[i].x) || isnan(pos[i].y), vbad = isnan(vel[i].x) || isnan(vel[i].y);
-        float acc = p.bqkv[o];
-        for (int c = 0; c < p.ds; ++c) acc = fmaf(__ldg(p.AqT + (size_t)c * E + o), pbad ? p.fill : fmaxf(p.bs[c], 0.f), acc);
-        for (int c = 0; c < p.dh; ++c) acc = fmaf(__ldg(p.AqT + (size_t)(p.ds + c) * E + o), hemb[i * p.dh + c], acc);
-        for (int c = 0; c < p.dv; ++c)
-            acc = fmaf(__ldg(p.AqT + (size_t)(p.ds + p.dh + c) * E + o), vbad ? p.fill : fmaxf(p.bv[c], 0.f), acc);
-        q[idx] = acc * scale;
-    }
-    __syncthreads();
-    // attention of track i over the slots j: lane owns features c = lane + 32 r and outputs o = lane + 32 r (r < 4)
-    for (int i = warp; i < n; i += nwarps) {
-        const float* qi = q + (size_t)i * E;
-        float u[4] = {0.f, 0.f, 0.f, 0.f};                           // u_i[c] = sum_o q_i[o] Ak[o][row(c)]
-#pragma unroll
-        for (int r = 0; r < 4; ++r) {
-            const int c = lane + 32 * r;
-            if (c < dsv) {
-                const int row = c < p.ds ? c : c + p.dh;
-                float acc = 0.f;
-                for (int o = 0; o < E; ++o) acc = fmaf(qi[o], __ldg(p.AkT + (size_t)row * E + o), acc);
-                u[r] = acc;
-            }
-        }
-        const float2 pi = pos[i], vi = vel[i];
-        float m_run = -CUDART_INF_F, l_run = 0.f;
-        float accf[4] = {0.f, 0.f, 0.f, 0.f}, acch[4] = {0.f, 0.f, 0.f, 0.f};
-        for (int j = 0; j < ns; ++j) {
-            const float rx = pos[j].x - pi.x, ry = pos[j].y - pi.y;
-            const float wx = (vel[j].x - vi.x) * 4.f, wy = (vel[j].y - vi.y) * 4.f;
-            const bool pbad = isnan(rx) || isnan(ry), vbad = isnan(wx) || isnan(wy);
-            float f[4] = {0.f, 0.f, 0.f, 0.f};
-            float part = 0.f;
+        __syncthreads();
+        // attention of track i over the slots j: lane owns the features c = lane + 32 r (r < 4) of e_ij = [spatial | hidden | velocity]
+        for (int t = warp; t < nc; t += kAtWarps) {
+            const int i = i0 + t;
+            const float* qi = qb + (size_t)t * E;
+            float u[4] = {0.f, 0.f, 0.f, 0.f};                       // u_i[c] = sum_o q_i[o] Ak[o][c]
 #pragma unroll
             for (int r = 0; r < 4; ++r) {
                 const int c = lane + 32 * r;
-                if (c < p.ds) f[r] = pbad ? p.fill : fmaxf(fmaf(ry, p.Ws[2 * c + 1], fmaf(rx, p.Ws[2 * c], p.bs[c])), 0.f);
-                else if (c < dsv) {
-                    const int cv = c - p.ds;
-                    f[r] = vbad ? p.fill : fmaxf(fmaf(wy, p.Wv[2 * cv + 1], fmaf(wx, p.Wv[2 * cv], p.bv[cv])), 0.f);
+                if (c < E) {
+                    float acc = 0.f;
+                    for (int o = 0; o < E; ++o) acc = fmaf(qi[o], __ldg(p.Ak + (size_t)o * E + c), acc);
+                    u[r] = acc;
                 }
-                part = fmaf(u[r], f[r], part);
-                const int o = lane + 32 * r;
-                if (o < E) part = fmaf(qi[o], Hk[(size_t)j * E + o], part);
             }
+            const float2 pi = pos[i], vi = vel[i];
+            float m_run = -CUDART_INF_F, l_run = 0.f;
+            float acc[4] = {0.f, 0.f, 0.f, 0.f};
+            for (int j = 0; j < ns; ++j) {
+                const float rx = pos[j].x - pi.x, ry = pos[j].y - pi.y;
+                const float wx = (vel[j].x - vi.x) * 4.f, wy = (vel[j].y - vi.y) * 4.f;
+                const bool pbad = isnan(rx) || isnan(ry), vbad = isnan(wx) || isnan(wy);
+                float f[4] = {0.f, 0.f, 0.f, 0.f};
+                float part = 0.f;
 #pragma unroll
-            for (int off = 16; off > 0; off >>= 1) part += __shfl_xor_sync(0xffffffffu, part, off);
-            const float m_new = fmaxf(m_run, part);
-            const float corr = __expf(m_run - m_new), a = __expf(part - m_new);      // first slot: corr = exp(-inf) = 0
-            l_run = l_run * corr + a;
+                for (int r = 0; r < 4; ++r) {
+                    const int c = lane + 32 * r;
+                    if (c < p.ds) f[r] = pbad ? p.fill : fmaxf(fmaf(ry, p.Ws[2 * c + 1], fmaf(rx, p.Ws[2 * c], p.bs[c])), 0.f);
+                    else if (c < dsh) f[r] = hemb[(size_t)j * p.dh + (c - p.ds)];
+                    else if (c < E) {
+                        const int cv = c - dsh;
+                        f[r] = vbad ? p.fill : fmaxf(fmaf(wy, p.Wv[2 * cv + 1], fmaf(wx, p.Wv[2 * cv], p.bv[cv])), 0.f);
+                    }
+                    part = fmaf(u[r], f[r], part);
+                }
+#pragma unroll
+                for (int off = 16; off > 0; off >>= 1) part += __shfl_xor_sync(0xffffffffu, part, off);
+                const float m_new = fmaxf(m_run, part);
+                const float corr = __expf(m_run - m_new), a = __expf(part - m_new);  // first slot: corr = exp(-inf) = 0
+                l_run = l_run * corr + a;
+#pragma unroll
+                for (int r = 0; r < 4; ++r) acc[r] = acc[r] * corr + a * f[r];
+                m_run = m_new;
+            }
+            const float inv = 1.f / l_run;
+            // att_i = Av (sum_j a_ij e_ij) + bv   (features are spread over the lanes: broadcast each one)
+            float o4[4];
 #pragma unroll
             for (int r = 0; r < 4; ++r) {
-                accf[r] = accf[r] * corr + a * f[r];
                 const int o = lane + 32 * r;
-                if (o < E) acch[r] = acch[r] * corr + a * Hv[(size_t)j * E + o];
+                o4[r] = o < E ? p.bqkv[2 * E + o] : 0.f;
             }
-            m_run = m_new;
-        }
-        const float inv = 1.f / l_run;
-        // att_i = Av_sv (sum a f) + sum a Hv   (features are spread over the lanes: broadcast each one)
-        float o4[4];
+            for (int c = 0; c < E; ++c) {
+                const float fc = __shfl_sync(0xffffffffu, acc[c >> 5], c & 31) * inv;
 #pragma unroll
-        for (int r = 0; r < 4; ++r) o4[r] = acch[r] * inv;
-        for (int c = 0; c < dsv; ++c) {
-            const float fc = __shfl_sync(0xffffffffu, accf[c >> 5], c & 31) * inv;
-            const int row = c < p.ds ? c : c + p.dh;
+                for (int r = 0; r < 4; ++r) {
+                    const int o = lane + 32 * r;
+                    if (o < E) o4[r] = fmaf(__ldg(p.AvT + (size_t)c * E + o), fc, o4[r]);
+                }
+            }
 #pragma unroll
             for (int r = 0; r < 4; ++r) {
                 const int o = lane + 32 * r;
-                if (o < E) o4[r] = fmaf(__ldg(p.AvT + (size_t)row * E + o), fc, o4[r]);
+                if (o < E) ab[(size_t)t * E + o] = o4[r];
             }
         }
-#pragma unroll
-        for (int r = 0; r < 4; ++r) {
-            const int o = lane + 32 * r;
-            if (o < E) att[(size_t)i * E + o] = o4[r];
+        __syncthreads();
+        // attention out-projection (into the query buffer), then out_projection
+        for (int idx = tid; idx < nc * E; idx += kAtThreads) {
+            const int t = idx / E, o = idx - t * E;
+            float acc = p.bo[o];
+            for (int c = 0; c < E; ++c) acc = fmaf(ab[(size_t)t * E + c], __ldg(p.WoT + (size_t)c * E + o), acc);
+            qb[idx] = acc;
         }
-    }
-    __syncthreads();
-    // attention out-projection, then out_projection
-    for (int idx = tid; idx < n * E; idx += blockDim.x) {
-        const int i = idx / E, o = idx - i * E;
-        float acc = p.bo[o];
-        for (int c = 0; c < E; ++c) acc = fmaf(att[(size_t)i * E + c], __ldg(p.WoT + (size_t)c * E + o), acc);
-        tmp[idx] = acc;
-    }
-    __syncthreads();
-    for (int idx = tid; idx < n * p.out_dim; idx += blockDim.x) {
-        const int i = idx / p.out_dim, o = idx - i * p.out_dim;
-        float acc = p.bout[o];
-        for (int c = 0; c < E; ++c) acc = fmaf(tmp[(size_t)i * E + c], __ldg(p.WoutT + (size_t)c * p.out_dim + o), acc);
-        p.out[(size_t)(row0 + i) * p.out_dim + o] = acc;
+        __syncthreads();
+        for (int idx = tid; idx < nc * p.out_dim; idx += kAtThreads) {
+            const int t = idx / p.out_dim, o = idx - t * p.out_dim;
+            float acc = p.bout[o];
+            for (int c = 0; c < E; ++c) acc = fmaf(qb[(size_t)t * E + c], __ldg(p.WoutT + (size_t)c * p.out_dim + o), acc);
+            p.out[(size_t)(row0 + i0 + t) * p.out_dim + o] = acc;
+        }
+        __syncthreads();                                             // qb / ab are rewritten by the next chunk
     }
 }
 
@@ -325,7 +318,7 @@ int launch_attn_mlp_pool(const tb2_lstm* m, const tb2_layout* l, const float* hi
     p.hidden = hidden;
     p.scene_off = l->scene_off;
     p.Ws = m->mp_Ws; p.bs = m->mp_bs; p.Wv = m->mp_Wv; p.bv = m->mp_bv; p.WhT = m->mp_WhT; p.bh = m->mp_bh;
-    p.AqT = m->at_AqT; p.AkT = m->at_AkT; p.AvT = m->at_AvT; p.bqkv = m->at_bqkv;
+    p.AqT = m->at_AqT; p.Ak = m->at_Ak; p.AvT = m->at_AvT; p.bqkv = m->at_bqkv;
     p.WoT = m->at_WoT; p.bo = m->at_bo;
     p.WoutT = m->mp_WoT; p.bout = m->mp_bo;
     p.out = out;
@@ -336,13 +329,13 @@ int launch_attn_mlp_pool(const tb2_lstm* m, const tb2_layout* l, const float* hi
     p.pad_to_max = l->pad_to_max;
     p.fill = m->cfg.attn_fill;
     const int E = p.ds + p.dh + p.dv;
-    const size_t smem = ((size_t)l->n_max * (4 + p.dh + 2 * E) + (size_t)l->n_max * 3 * E) * sizeof(float) + 16;
+    const size_t smem = ((size_t)kAtChunk * 2 * E + (size_t)l->n_max * (4 + p.dh)) * sizeof(float);
     TB2_REQUIRE(smem <= 200 * 1024, "scene too large for the attention pooling kernel");
     static DynSmemConfig configured;
     TB2_CHECK_CUDA(configured.ensure(attn_mlp_pool_kernel, smem, 48 * 1024));
     {
         KernelTimer kt("attn_mlp_pool", st);
-        launch_pdl(attn_mlp_pool_kernel, dim3(l->B), dim3(256), smem, st, p);
+        launch_pdl(attn_mlp_pool_kernel, dim3(l->B), dim3(kAtThreads), smem, st, p);
     }
     TB2_LAUNCH_CHECK();
     return TB2_OK;
@@ -463,9 +456,11 @@ int launch_trajectron_feat(const tb2_lstm* m, const tb2_layout* l, const float* 
 //   gates = W_ih feat + b_ih + W_hh h + b_hh (order i, f, g, o); c' = sigma(f) c + sigma(i) tanh(g); h' = sigma(o) tanh(c');
 //   out = hidden2pool(h').   Every track is updated every step (absent ones with zero features).
 // One CTA per 16 tracks: the inputs [feat | h] of its rows sit in shared memory, thread = gate column(s), the transposed
-// weights stream coalesced from L2 with 16 accumulators per column; FP32 FFMA, accurate expf / tanhf.
+// weights stream coalesced from L2 with 16 accumulators per column; FP32 FFMA, accurate expf / tanhf.  The CTA's shared
+// memory is Rows x (D + 6 Hp) floats; where 16 rows exceed 200 KB (D + 6 Hp > 3200, e.g. Hp = 512 with D >= 128) the
+// tile is 8 rows, which holds every width the constructors accept (D <= 1024, Hp <= 512: 128 KB).  A row's arithmetic
+// is the same in either tile.
 // ------------------------------------------------------------------------------------------
-constexpr int kPlRows = 16;
 
 struct PoolLstmParams {
     const float* feat;     // [M, D]
@@ -480,6 +475,7 @@ struct PoolLstmParams {
     int M, D, Hp;
 };
 
+template <int kPlRows>
 __global__ void __launch_bounds__(256) pool_lstm_cell_kernel(PoolLstmParams p) {
     extern __shared__ __align__(16) float smem_pl[];
     const int K = p.D + p.Hp, G = 4 * p.Hp;
@@ -549,13 +545,19 @@ int launch_pool_lstm_cell(const tb2_lstm* m, const tb2_layout* l, const float* f
     p.WihT = m->pl_WihT; p.WhhT = m->pl_WhhT; p.b = m->pl_b; p.WoT = m->mp_WoT; p.bo = m->mp_bo;
     p.out = out;
     p.M = l->M; p.D = m->cfg.out_dim; p.Hp = m->cfg.mlp_dim_hidden;
-    const size_t smem = ((size_t)(p.D + p.Hp) * kPlRows + (size_t)kPlRows * 4 * p.Hp + (size_t)kPlRows * p.Hp) * sizeof(float);
-    TB2_REQUIRE(smem <= 200 * 1024, "interaction-encoder LSTM too wide for the kernel");
-    static DynSmemConfig configured;
-    TB2_CHECK_CUDA(configured.ensure(pool_lstm_cell_kernel, smem, 48 * 1024));
+    const size_t row_bytes = (size_t)(p.D + 6 * p.Hp) * sizeof(float);      // [feat | h], 4 gates, h' of one row
+    TB2_REQUIRE(8 * row_bytes <= 200 * 1024, "interaction-encoder LSTM too wide for the kernel");
     {
         KernelTimer kt("pool_lstm_cell", st);
-        launch_pdl(pool_lstm_cell_kernel, dim3((l->M + kPlRows - 1) / kPlRows), dim3(256), smem, st, p);
+        if (16 * row_bytes <= 200 * 1024) {
+            static DynSmemConfig configured;
+            TB2_CHECK_CUDA(configured.ensure(pool_lstm_cell_kernel<16>, 16 * row_bytes, 48 * 1024));
+            launch_pdl(pool_lstm_cell_kernel<16>, dim3((l->M + 15) / 16), dim3(256), 16 * row_bytes, st, p);
+        } else {
+            static DynSmemConfig configured;
+            TB2_CHECK_CUDA(configured.ensure(pool_lstm_cell_kernel<8>, 8 * row_bytes, 48 * 1024));
+            launch_pdl(pool_lstm_cell_kernel<8>, dim3((l->M + 7) / 8), dim3(256), 8 * row_bytes, st, p);
+        }
     }
     TB2_LAUNCH_CHECK();
     return TB2_OK;

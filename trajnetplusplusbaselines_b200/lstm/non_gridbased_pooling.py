@@ -27,7 +27,35 @@ from .. import _lib
 from ..engine import LayoutCache, ModelHandle, plug_getstate, weights_key
 
 
-class HiddenStateMLPPooling(torch.nn.Module):
+class _StandalonePlug:
+    """Shared stand-alone path of the non-grid plugs: a model handle whose LSTM-cell slots hold zeros."""
+
+    def _plug_handle(self, device):
+        if self._handle is None or self._handle.device != device:
+            cfg = _lib.LstmConfig()
+            cfg.hidden_dim = 128            # the stand-alone plug does not touch the LSTM cell
+            cfg.embedding_dim = 64
+            cfg.pool_to_input = 1
+            self.fill_config(cfg)
+            self._handle = ModelHandle(cfg, device)
+            self._standalone_dummy = None
+        if getattr(self, '_standalone_dummy', None) is None:
+            z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=device)
+            in_dim = 64 + self.out_dim
+            self._standalone_dummy = dict(
+                input_embedding_weight=z(62, 2), input_embedding_bias=z(62),
+                encoder_weight_ih=z(512, in_dim), encoder_weight_hh=z(512, 128),
+                encoder_bias_ih=z(512), encoder_bias_hh=z(512),
+                decoder_weight_ih=z(512, in_dim), decoder_weight_hh=z(512, 128),
+                decoder_bias_ih=z(512), decoder_bias_hh=z(512),
+                hidden2normal_weight=z(5, 128), hidden2normal_bias=z(5))
+        fields = dict(self._standalone_dummy)
+        fields.update(self.weight_fields())
+        self._handle.set_weights(fields, key=self.weights_version())
+        return self._handle
+
+
+class HiddenStateMLPPooling(torch.nn.Module, _StandalonePlug):
     def __init__(self, hidden_dim=128, mlp_dim=128, mlp_dim_spatial=32, mlp_dim_vel=32, out_dim=None):
         """Same arguments and sub-module names as the reference (non_gridbased_pooling.py:166-193)."""
         super().__init__()
@@ -85,62 +113,14 @@ class HiddenStateMLPPooling(torch.nn.Module):
             raise RuntimeError("HiddenStateMLPPooling runs on CUDA only: move the module to the GPU (module.cuda())")
         if hidden_states.size(-1) != self.hidden_dim:
             raise ValueError("hidden_states width != hidden_dim")
-        if self._handle is None or self._handle.device != device:
-            cfg = _lib.LstmConfig()
-            cfg.hidden_dim = 128            # the stand-alone plug does not touch the LSTM cell
-            cfg.embedding_dim = 64
-            cfg.pool_to_input = 1
-            self.fill_config(cfg)
-            self._handle = ModelHandle(cfg, device)
-            self._standalone_dummy = None
-        if getattr(self, '_standalone_dummy', None) is None:
-            z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=device)
-            in_dim = 64 + self.out_dim
-            self._standalone_dummy = dict(
-                input_embedding_weight=z(62, 2), input_embedding_bias=z(62),
-                encoder_weight_ih=z(512, in_dim), encoder_weight_hh=z(512, 128),
-                encoder_bias_ih=z(512), encoder_bias_hh=z(512),
-                decoder_weight_ih=z(512, in_dim), decoder_weight_hh=z(512, 128),
-                decoder_bias_ih=z(512), decoder_bias_hh=z(512),
-                hidden2normal_weight=z(5, 128), hidden2normal_bias=z(5))
-        fields = dict(self._standalone_dummy)
-        fields.update(self.weight_fields())
-        self._handle.set_weights(fields, key=self.weights_version())
+        handle = self._plug_handle(device)
         layout = self._layouts.get(range(0, batch_size * num_tracks + 1, num_tracks), device=device)
         f32 = dict(device=device, dtype=torch.float32)
         o1 = obs1.detach().to(**f32).reshape(-1, 2).contiguous()
         o2 = obs2.detach().to(**f32).reshape(-1, 2).contiguous()
         hid = hidden_states.detach().to(**f32).reshape(batch_size * num_tracks, -1).contiguous()
-        out = self._handle.pool_forward(layout, hid, o1, o2, self.out_dim)
+        out = handle.pool_forward(layout, hid, o1, o2, self.out_dim)
         return out.to(obs2.device) if obs2.device != device else out
-
-
-class _StandalonePlug:
-    """Shared stand-alone path of the non-grid plugs: a model handle whose LSTM-cell slots hold zeros."""
-
-    def _plug_handle(self, device):
-        if self._handle is None or self._handle.device != device:
-            cfg = _lib.LstmConfig()
-            cfg.hidden_dim = 128            # the stand-alone plug does not touch the LSTM cell
-            cfg.embedding_dim = 64
-            cfg.pool_to_input = 1
-            self.fill_config(cfg)
-            self._handle = ModelHandle(cfg, device)
-            self._standalone_dummy = None
-        if getattr(self, '_standalone_dummy', None) is None:
-            z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=device)
-            in_dim = 64 + self.out_dim
-            self._standalone_dummy = dict(
-                input_embedding_weight=z(62, 2), input_embedding_bias=z(62),
-                encoder_weight_ih=z(512, in_dim), encoder_weight_hh=z(512, 128),
-                encoder_bias_ih=z(512), encoder_bias_hh=z(512),
-                decoder_weight_ih=z(512, in_dim), decoder_weight_hh=z(512, 128),
-                decoder_bias_ih=z(512), decoder_bias_hh=z(512),
-                hidden2normal_weight=z(5, 128), hidden2normal_bias=z(5))
-        fields = dict(self._standalone_dummy)
-        fields.update(self.weight_fields())
-        self._handle.set_weights(fields, key=self.weights_version())
-        return self._handle
 
 
 class NearestNeighborMLP(torch.nn.Module, _StandalonePlug):
