@@ -74,7 +74,8 @@ int tb2_profile_end(char* json_out, size_t capacity);
  * GridBasedPooling (lstm/gridbased_pooling.py:16-19).
  * ------------------------------------------------------------------------------------- */
 typedef struct tb2_lstm_config {
-    int32_t hidden_dim;      /* LSTM hidden_dim (128)                              */
+    int32_t hidden_dim;      /* LSTM hidden_dim: 32, 64, 96, ..., 256 (default 128); any other width
+                              * fails tb2_lstm_create with TB2_ERR_UNSUPPORTED     */
     int32_t embedding_dim;   /* LSTM embedding_dim (64); Linear(2, E-2)+2 zero tags */
     int32_t pool_type;       /* TB2_POOL_*                                         */
     int32_t pool_to_input;   /* 1: concat pooled to LSTM input, 0: h += pooled     */

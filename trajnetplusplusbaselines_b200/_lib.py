@@ -12,6 +12,9 @@ LIB_PATH = os.path.join(_HERE, "libtrajnet_b200.so")
 
 POOL_NONE, POOL_OCCUPANCY, POOL_DIRECTIONAL, POOL_SOCIAL, POOL_HIDDEN_MLP, POOL_NN_MLP, POOL_ATTN_MLP, POOL_NN_LSTM, POOL_TRAJECTRON = 0, 1, 2, 3, 4, 5, 6, 7, 8
 PHASE_ENCODER, PHASE_DECODER = 0, 1
+# LSTM widths the kernels are built for, and tb2_lstm_create's refusal of any other (kHiddenDimMessage, csrc/common.cuh)
+HIDDEN_DIMS = tuple(range(32, 257, 32))
+HIDDEN_DIM_MESSAGE = "hidden_dim must be a multiple of 32 from 32 to 256 (32, 64, 96, ..., 256)"
 SCORE_COL_GT, SCORE_COL_PRED, SCORE_NEIGH_COUNT_DIFFERS, SCORE_NLL_ALL_SKIPPED = 1, 2, 4, 8     # tb2_score_scenes flags
 
 _c_float_p = ctypes.c_void_p   # device pointers travel as integers

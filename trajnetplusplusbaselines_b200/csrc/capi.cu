@@ -78,8 +78,8 @@ size_t carve_workspace(const tb2_lstm* m, const tb2_layout* l, void* base, Works
     w.pool_hi = take(M * (size_t)std::max(m->P, 1) * 2);
     w.pool_lo = take(M * (size_t)std::max(m->P, 1) * 2);
     for (int i = 0; i < 2; ++i) {
-        w.hs_hi[i] = take(M * 128 * 2);
-        w.hs_lo[i] = take(M * 128 * 2);
+        w.hs_hi[i] = take(M * (size_t)m->H * 2);
+        w.hs_lo[i] = take(M * (size_t)m->H * 2);
     }
     w.pool_feat = w.pool_h = w.pool_c = w.scene_sum = nullptr;
     if (m->cfg.pool_type == TB2_POOL_TRAJECTRON) w.scene_sum = (float*)take((size_t)l->B * 4 * sizeof(float));
@@ -208,7 +208,10 @@ int tb2_profile_end(char* json_out, size_t capacity) {
 int tb2_lstm_create(const tb2_lstm_config* cfg, tb2_lstm** out) {
     TB2_REQUIRE(cfg && out, "null argument");
     *out = nullptr;
-    TB2_REQUIRE(cfg->hidden_dim == 128, "hidden_dim must be 128 (kernel specialisation)");
+    if (!hidden_dim_supported(cfg->hidden_dim)) {
+        set_error(kHiddenDimMessage);
+        return TB2_ERR_UNSUPPORTED;
+    }
     TB2_REQUIRE(cfg->embedding_dim >= 4 && cfg->embedding_dim <= 1024, "embedding_dim out of range");
     TB2_REQUIRE(cfg->pool_type >= TB2_POOL_NONE && cfg->pool_type <= TB2_POOL_TRAJECTRON, "bad pool_type");
     tb2_lstm* m = new (std::nothrow) tb2_lstm();

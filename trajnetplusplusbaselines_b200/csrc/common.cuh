@@ -71,6 +71,27 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
     cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
+
+// launch_pdl with clusters of cluster_x CTAs along x, chosen at launch (the kernel carries no __cluster_dims__)
+template <typename... KArgs, typename... Args>
+inline cudaError_t launch_pdl_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
+                                      unsigned cluster_x, Args&&... args) {
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = grid;
+    cfg.blockDim = block;
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = st;
+    cudaLaunchAttribute attr[2];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    attr[1].id = cudaLaunchAttributeClusterDimension;
+    attr[1].val.clusterDim.x = cluster_x;
+    attr[1].val.clusterDim.y = 1;
+    attr[1].val.clusterDim.z = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 2;
+    return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
+}
 #endif
 
 // cudaFuncSetAttribute(MaxDynamicSharedMemorySize) applies to the CURRENT device: the size a launch
@@ -102,6 +123,10 @@ struct KernelTimer {
 };
 
 constexpr int kMaxMlpLayers = 3;
+// LSTM widths the gate and backward kernels are built for: 32, 64, ..., 256
+constexpr int kMaxHidden = 256;
+inline bool hidden_dim_supported(int H) { return H >= 32 && H <= kMaxHidden && H % 32 == 0; }
+constexpr const char* kHiddenDimMessage = "hidden_dim must be a multiple of 32 from 32 to 256 (32, 64, 96, ..., 256)";
 constexpr int kGateBK = 16;        // K-chunk of the gate GEMM; weight rows are padded to it
 
 }  // namespace tb2
@@ -178,7 +203,7 @@ struct Workspace {
     void* emb_lo;
     void* pool_hi;         // [M, P]
     void* pool_lo;
-    void* hs_hi[2];        // [M, 128] ping-pong split of the hidden state
+    void* hs_hi[2];        // [M, H] ping-pong split of the hidden state
     void* hs_lo[2];
     size_t bytes;
     int write_pairs;       // pool_prepare also exports the pair tables (training forward with a cache)

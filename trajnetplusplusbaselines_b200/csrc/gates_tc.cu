@@ -2,22 +2,23 @@
 // with the cell update, the Gaussian head and the position feedback in the epilogue.
 //
 // Same contract as lstm_gates_kernel (csrc/lstm_step.cu; reference LSTM.step lstm.py:118-168,
-// torch.nn.LSTMCell, Hidden2Normal modules.py:56-64), specialised for E = 64, H = 128,
-// pool_to_input: gates[M, 512] = [emb | pooled | h][M, K] . [W_ih | W_hh]^T, K = 64 + P + 128.
+// torch.nn.LSTMCell, Hidden2Normal modules.py:56-64), specialised for E = 64, H = 64, 128, 192 or 256,
+// pool_to_input: gates[M, 4H] = [emb | pooled | h][M, K] . [W_ih | W_hh]^T, K = 64 + P + H.
 //
 // All three K segments arrive as bf16 (hi, lo) pairs written by their producers (embed_split,
 // the grid-embedding layer's epilogue, the previous step's epilogue) and the product is the
 // 3-pass split  A_hi.W_hi + A_hi.W_lo + A_lo.W_hi  accumulated in fp32 registers.
 //
-// Grid: (2, ceil(M / 128)) with __cluster_dims__(2, 1, 1).  The two CTAs of a cluster share a
-// 128-row tile and each owns 64 hidden units x 4 gates (N = 256; W rows are permuted at repack so
-// a CTA's tile holds complete i/f/g/o quadruples).  Warpgroup 2 is the TMA producer; warpgroups 0
+// Grid: (H / 64, ceil(M / 128)) in clusters of H / 64 CTAs along x (set at launch).  The CTAs of a
+// cluster share a 128-row tile and rank r owns hidden units [64 r, 64 r + 64) x 4 gates (N = 256;
+// W rows are permuted at repack so a CTA's tile holds complete i/f/g/o quadruples).  Warpgroup 2 is the TMA producer; warpgroups 0
 // and 1 each run wgmma.m64n256k16 on 64 rows.  In the accumulator fragment (wgmma.cuh) the four
 // gates of a unit sit in the same thread (columns u, 64 + u, 128 + u, 192 + u), so the epilogue
 // updates c / h (fp32 state + bf16 split for the next step) straight from registers and
 // accumulates its share of the 5-wide Hidden2Normal dot products; the four threads of a row add
-// theirs with shuffles, rank 1 ships its partial sums to rank 0 through distributed shared memory
-// and rank 0 finishes mu / sigma / rho and the fed-back position.
+// theirs with shuffles, ranks 1 .. H/64 - 1 ship their partial sums to rank 0 through distributed
+// shared memory and rank 0 adds them in rank order and finishes mu / sigma / rho and the fed-back
+// position.
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <math_constants.h>
@@ -36,7 +37,6 @@ constexpr int kGtBK = 64;
 constexpr int kGtStages = 2;
 constexpr int kGtThreads = 384;     // two MMA + epilogue warpgroups, one producer warpgroup
 constexpr int kGtConsumerWarps = 8;
-constexpr int kGtH = 128;
 constexpr uint32_t kGtABytes = kGtBM * kGtBK * 2;      // 16 KB
 constexpr uint32_t kGtBBytes = kGtBN * kGtBK * 2;      // 32 KB
 constexpr uint32_t kGtStageBytes = 2 * kGtABytes + 2 * kGtBBytes;   // 96 KB
@@ -50,21 +50,23 @@ __device__ __forceinline__ float g_tanh(float x) { return 1.f - __fdividef(2.f, 
 struct GateTcParams {
     const float2* obs1;
     const float2* obs2;
-    const float* h_in;          // [M, 128] fp32 state before the step
+    const float* h_in;          // [M, H] fp32 state before the step
     const float* c_in;
     float* h_out;
     float* c_out;
-    __nv_bfloat16* hs_out_hi;   // [M, 128] split of h_out for the next step
+    __nv_bfloat16* hs_out_hi;   // [M, H] split of h_out for the next step
     __nv_bfloat16* hs_out_lo;
     float* normal_out;          // [M, 5]
     float2* pos_out;            // [M] or null
-    const float* bg;            // [512] b_ih + b_hh, original gate order
-    const float* Wn;            // [5, 128]
+    const float* bg;            // [4H] b_ih + b_hh, original gate order
+    const float* Wn;            // [5, H]
     const float* bn;            // [5]
     int M, P;
 };
 
-__global__ void __cluster_dims__(2, 1, 1) __launch_bounds__(kGtThreads, 1)
+// R = cluster size = H / 64 (1 to 4; a cluster of one at H = 64): the strides and the rank loop of the epilogue are compile-time constants
+template <int R>
+__global__ void __launch_bounds__(kGtThreads, 1)
 lstm_gates_tc_kernel(const __grid_constant__ CUtensorMap map_emb_hi, const __grid_constant__ CUtensorMap map_emb_lo,
                      const __grid_constant__ CUtensorMap map_pool_hi, const __grid_constant__ CUtensorMap map_pool_lo,
                      const __grid_constant__ CUtensorMap map_h_hi, const __grid_constant__ CUtensorMap map_h_lo,
@@ -75,17 +77,18 @@ lstm_gates_tc_kernel(const __grid_constant__ CUtensorMap map_emb_hi, const __gri
     __shared__ __align__(8) uint64_t empty_bar[kGtStages];
     __shared__ float wn_s[5][64];          // Hidden2Normal weights of this CTA's 64 units
     __shared__ float bg_s[4][64];          // fused gate bias of this CTA's units
-    __shared__ float peer_part[kGtBM][5];  // rank 0: partial head sums received from rank 1
+    constexpr int H = 64 * R;
+    __shared__ float peer_part[R > 1 ? R - 1 : 1][kGtBM][5];  // rank 0: partial head sums of ranks 1, 2, ..
 
     const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int rank = blockIdx.x;           // cluster rank == n-tile: units [64 rank, 64 rank + 64)
     const int m0 = blockIdx.y * kGtBM;
-    const int kb_pool = p.P / kGtBK;       // k-blocks: [emb | pooled x kb_pool | h x 2]
-    const int num_kb = 1 + kb_pool + 2;
+    const int kb_pool = p.P / kGtBK;       // k-blocks: [emb | pooled x kb_pool | h x H / 64]
+    const int num_kb = 1 + kb_pool + H / kGtBK;
     const uint32_t ring = (smem_u32(smem_gt) + 1023u) & ~1023u;
 
-    for (int i = threadIdx.x; i < 5 * 64; i += kGtThreads) wn_s[i / 64][i % 64] = p.Wn[(i / 64) * kGtH + rank * 64 + (i % 64)];
-    for (int i = threadIdx.x; i < 4 * 64; i += kGtThreads) bg_s[i / 64][i % 64] = p.bg[(i / 64) * kGtH + rank * 64 + (i % 64)];
+    for (int i = threadIdx.x; i < 5 * 64; i += kGtThreads) wn_s[i / 64][i % 64] = p.Wn[(i / 64) * H + rank * 64 + (i % 64)];
+    for (int i = threadIdx.x; i < 4 * 64; i += kGtThreads) bg_s[i / 64][i % 64] = p.bg[(i / 64) * H + rank * 64 + (i % 64)];
 
     if (threadIdx.x == 0) {
         for (int s = 0; s < kGtStages; ++s) {
@@ -163,7 +166,7 @@ lstm_gates_tc_kernel(const __grid_constant__ CUtensorMap map_emb_hi, const __gri
 #pragma unroll
             for (int n8 = 0; n8 < 8; ++n8) {
                 const int u = 8 * n8 + 2 * (lane & 3);
-                const size_t o = (size_t)row * kGtH + rank * 64 + u;
+                const size_t o = (size_t)row * H + rank * 64 + u;
                 float2 c = *reinterpret_cast<const float2*>(p.c_in + o);
                 float2 h;
                 if (!masked) {
@@ -206,14 +209,14 @@ lstm_gates_tc_kernel(const __grid_constant__ CUtensorMap map_emb_hi, const __gri
                 part[hr][q] += __shfl_xor_sync(0xffffffffu, part[hr][q], 1);
                 part[hr][q] += __shfl_xor_sync(0xffffffffu, part[hr][q], 2);
             }
-        if (rank == 1) {
-            asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");     // phase 1: peer is resident
+        if (rank > 0) {
+            asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");     // phase 1: rank 0 is resident
             waited_phase1 = true;
-            // ship this half's head sums to rank 0 through distributed shared memory
+            // ship this rank's head sums to rank 0 through distributed shared memory
             if ((lane & 3) == 0) {
 #pragma unroll
                 for (int hr = 0; hr < 2; ++hr) {
-                    const uint32_t local = smem_u32(&peer_part[rl + 8 * hr][0]);
+                    const uint32_t local = smem_u32(&peer_part[rank - 1][rl + 8 * hr][0]);
                     uint32_t remote;
                     asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(local), "r"(0));
 #pragma unroll
@@ -224,7 +227,7 @@ lstm_gates_tc_kernel(const __grid_constant__ CUtensorMap map_emb_hi, const __gri
             __syncwarp();
         }
     }
-    // cluster barrier phase 2: rank 1's partial sums are visible in rank 0's shared memory afterwards
+    // cluster barrier phase 2: the other ranks' partial sums are visible in rank 0's shared memory afterwards
     if (!waited_phase1) asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
     asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
     asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
@@ -242,7 +245,12 @@ lstm_gates_tc_kernel(const __grid_constant__ CUtensorMap map_emb_hi, const __gri
             } else {
                 float s[5];
 #pragma unroll
-                for (int q = 0; q < 5; ++q) s[q] = part[hr][q] + peer_part[rl + 8 * hr][q] + p.bn[q];
+                for (int q = 0; q < 5; ++q) {
+                    s[q] = part[hr][q];
+#pragma unroll
+                    for (int r = 1; r < R; ++r) s[q] += peer_part[r - 1][rl + 8 * hr][q];
+                    s[q] += p.bn[q];
+                }
                 const float n0 = s[0], n1 = s[1];
                 no[0] = n0;
                 no[1] = n1;
@@ -300,7 +308,7 @@ __global__ void repack_gates_tc_kernel(const float* __restrict__ w_ih, const flo
 int make_bf16_tile_map(CUtensorMap* map, const void* base, int rows, int cols, int box_rows);
 
 bool gates_tc_supported(const tb2_lstm* m) {
-    if (m->H != kGtH || m->E != 64) return false;
+    if (m->H % 64 != 0 || m->E != 64) return false;
     if (m->cfg.pool_type != TB2_POOL_NONE && !m->cfg.pool_to_input) return false;
     if (m->P % kGtBK != 0) return false;
     return true;
@@ -326,6 +334,23 @@ int launch_embed_split(const tb2_lstm* m, int M, const float* obs1, const float*
     return TB2_OK;
 }
 
+template <int R>
+static int launch_gates_tc_t(const CUtensorMap& me_hi, const CUtensorMap& me_lo, const CUtensorMap& mp_hi,
+                             const CUtensorMap& mp_lo, const CUtensorMap& mh_hi, const CUtensorMap& mh_lo,
+                             const CUtensorMap& mw_hi, const CUtensorMap& mw_lo, const GateTcParams& p, cudaStream_t st) {
+    const size_t smem = (size_t)kGtStages * kGtStageBytes + 1024;
+    static DynSmemConfig configured;
+    TB2_CHECK_CUDA(configured.ensure(lstm_gates_tc_kernel<R>, smem));
+    dim3 grid(R, (p.M + kGtBM - 1) / kGtBM);
+    {
+        KernelTimer kt("lstm_gates_tc", st);
+        launch_pdl_cluster(lstm_gates_tc_kernel<R>, grid, dim3(kGtThreads), smem, st, (unsigned)R, me_hi, me_lo, mp_hi,
+                           mp_lo, mh_hi, mh_lo, mw_hi, mw_lo, p);
+    }
+    TB2_LAUNCH_CHECK();
+    return TB2_OK;
+}
+
 int launch_gates_tc(const tb2_lstm* m, const tb2_layout* l, int phase, const float* obs1, const float* obs2,
                     const void* emb_hi, const void* emb_lo, const void* pool_hi, const void* pool_lo,
                     const void* hs_in_hi, const void* hs_in_lo, void* hs_out_hi, void* hs_out_lo,
@@ -343,10 +368,10 @@ int launch_gates_tc(const tb2_lstm* m, const tb2_layout* l, int phase, const flo
         mp_hi = me_hi;
         mp_lo = me_lo;
     }
-    if ((rc = make_bf16_tile_map(&mh_hi, hs_in_hi, M, kGtH, kGtBM))) return rc;
-    if ((rc = make_bf16_tile_map(&mh_lo, hs_in_lo, M, kGtH, kGtBM))) return rc;
-    if ((rc = make_bf16_tile_map(&mw_hi, m->Wg_hi[phase], 4 * kGtH, m->K_gate, kGtBN))) return rc;
-    if ((rc = make_bf16_tile_map(&mw_lo, m->Wg_lo[phase], 4 * kGtH, m->K_gate, kGtBN))) return rc;
+    if ((rc = make_bf16_tile_map(&mh_hi, hs_in_hi, M, m->H, kGtBM))) return rc;
+    if ((rc = make_bf16_tile_map(&mh_lo, hs_in_lo, M, m->H, kGtBM))) return rc;
+    if ((rc = make_bf16_tile_map(&mw_hi, m->Wg_hi[phase], 4 * m->H, m->K_gate, kGtBN))) return rc;
+    if ((rc = make_bf16_tile_map(&mw_lo, m->Wg_lo[phase], 4 * m->H, m->K_gate, kGtBN))) return rc;
     GateTcParams p;
     p.obs1 = (const float2*)obs1;
     p.obs2 = (const float2*)obs2;
@@ -359,17 +384,15 @@ int launch_gates_tc(const tb2_lstm* m, const tb2_layout* l, int phase, const flo
     p.bn = m->bn;
     p.M = M;
     p.P = m->P;
-    const size_t smem = (size_t)kGtStages * kGtStageBytes + 1024;
-    static DynSmemConfig configured;
-    TB2_CHECK_CUDA(configured.ensure(lstm_gates_tc_kernel, smem));
-    dim3 grid(2, (M + kGtBM - 1) / kGtBM);
-    {
-        KernelTimer kt("lstm_gates_tc", st);
-        launch_pdl(lstm_gates_tc_kernel, grid, dim3(kGtThreads), smem, st, me_hi, me_lo, mp_hi, mp_lo, mh_hi, mh_lo,
-                   mw_hi, mw_lo, p);
+    switch (m->H) {
+        case 64: return launch_gates_tc_t<1>(me_hi, me_lo, mp_hi, mp_lo, mh_hi, mh_lo, mw_hi, mw_lo, p, st);
+        case 128: return launch_gates_tc_t<2>(me_hi, me_lo, mp_hi, mp_lo, mh_hi, mh_lo, mw_hi, mw_lo, p, st);
+        case 192: return launch_gates_tc_t<3>(me_hi, me_lo, mp_hi, mp_lo, mh_hi, mh_lo, mw_hi, mw_lo, p, st);
+        case 256: return launch_gates_tc_t<4>(me_hi, me_lo, mp_hi, mp_lo, mh_hi, mh_lo, mw_hi, mw_lo, p, st);
+        default: break;
     }
-    TB2_LAUNCH_CHECK();
-    return TB2_OK;
+    set_error(kHiddenDimMessage);
+    return TB2_ERR_UNSUPPORTED;
 }
 
 }  // namespace tb2

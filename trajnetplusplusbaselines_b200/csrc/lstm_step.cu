@@ -8,19 +8,17 @@
 // stacks/unstacks them every step; here they are flat [M, H] arrays updated in place.
 //
 // Tiling: CTA = 32 tracks x all 4H gate columns, 256 threads; thread (warp w, lane l) owns
-// rows 4w..4w+3 and hidden units 4l..4l+3 of all four gates, so the LSTM pointwise math needs
-// no exchange and the 5-wide Gaussian head is a warp-shuffle reduction.  The A operand
+// rows 4w..4w+3 and hidden units U l..U l+U-1 (U = H / 32) of all four gates, so the LSTM pointwise
+// math needs no exchange and the 5-wide Gaussian head is a warp-shuffle reduction.  The A operand
 // [emb | pooled | h] is assembled on the fly in shared memory (the embedding is recomputed
 // from the 2-float velocity, never stored); W^T streams from L2 through a cp.async
-// double buffer.
+// double buffer (16 x 4H floats per stage: 128 KB in all at H = 256).
 #include <math_constants.h>
 
 #include "common.cuh"
 
 namespace tb2 {
 
-constexpr int kGH = 128;            // hidden_dim this kernel is specialised for
-constexpr int kGN = 4 * kGH;        // gate columns
 constexpr int kGM = 32;             // tracks per CTA
 constexpr int kGThreads = 256;
 
@@ -53,10 +51,48 @@ __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commi
 template <int N>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;\n" ::"n"(N)); }
 
-__global__ void __launch_bounds__(kGThreads, 2) lstm_gates_kernel(GateParams p) {
+// U consecutive floats, in the widest vector accesses U allows (the address is aligned to them)
+template <int U>
+__device__ __forceinline__ void ld_units(const float* src, float (&v)[U]) {
+    if constexpr (U % 4 == 0) {
+#pragma unroll
+        for (int q = 0; q < U / 4; ++q) {
+            const float4 t = reinterpret_cast<const float4*>(src)[q];
+            v[4 * q] = t.x; v[4 * q + 1] = t.y; v[4 * q + 2] = t.z; v[4 * q + 3] = t.w;
+        }
+    } else if constexpr (U % 2 == 0) {
+#pragma unroll
+        for (int q = 0; q < U / 2; ++q) {
+            const float2 t = reinterpret_cast<const float2*>(src)[q];
+            v[2 * q] = t.x; v[2 * q + 1] = t.y;
+        }
+    } else {
+#pragma unroll
+        for (int q = 0; q < U; ++q) v[q] = src[q];
+    }
+}
+template <int U>
+__device__ __forceinline__ void st_units(float* dst, const float (&v)[U]) {
+    if constexpr (U % 4 == 0) {
+#pragma unroll
+        for (int q = 0; q < U / 4; ++q)
+            reinterpret_cast<float4*>(dst)[q] = make_float4(v[4 * q], v[4 * q + 1], v[4 * q + 2], v[4 * q + 3]);
+    } else if constexpr (U % 2 == 0) {
+#pragma unroll
+        for (int q = 0; q < U / 2; ++q) reinterpret_cast<float2*>(dst)[q] = make_float2(v[2 * q], v[2 * q + 1]);
+    } else {
+#pragma unroll
+        for (int q = 0; q < U; ++q) dst[q] = v[q];
+    }
+}
+
+// U = hidden units per lane (H = 32 U)
+template <int U>
+__global__ void __launch_bounds__(kGThreads, U <= 4 ? 2 : 1) lstm_gates_kernel(GateParams p) {
+    constexpr int H = 32 * U, N = 4 * H;
     extern __shared__ __align__(16) float smem_gates[];
-    float (*Ws)[kGateBK][kGN] = reinterpret_cast<float (*)[kGateBK][kGN]>(smem_gates);               // 64 KB
-    float (*As)[kGateBK][kGM] = reinterpret_cast<float (*)[kGateBK][kGM]>(smem_gates + 2 * kGateBK * kGN);  // 4 KB
+    float (*Ws)[kGateBK][N] = reinterpret_cast<float (*)[kGateBK][N]>(smem_gates);                   // 2 x 16 x 4H
+    float (*As)[kGateBK][kGM] = reinterpret_cast<float (*)[kGateBK][kGM]>(smem_gates + 2 * kGateBK * N);  // 4 KB
     __shared__ float2 vel4[kGM];                            // 4 * (obs2 - obs1)
     __shared__ float2 obs2s[kGM];
     __shared__ int maskS[kGM];
@@ -77,22 +113,22 @@ __global__ void __launch_bounds__(kGThreads, 2) lstm_gates_kernel(GateParams p) 
     }
     __syncthreads();
 
-    float acc[4][4][4];   // [row][gate][unit]
+    float acc[4][4][U];   // [row][gate][unit]
 #pragma unroll
     for (int r = 0; r < 4; ++r)
 #pragma unroll
         for (int g = 0; g < 4; ++g)
 #pragma unroll
-            for (int u = 0; u < 4; ++u) acc[r][g][u] = 0.f;
+            for (int u = 0; u < U; ++u) acc[r][g][u] = 0.f;
 
     const int nchunks = p.K_pad / kGateBK;
 
     auto load_w = [&](int buf, int chunk) {
-        // 16 x 512 floats = 2048 float4, 8 per thread
-        const float4* src = reinterpret_cast<const float4*>(p.WgT + (size_t)chunk * kGateBK * kGN);
+        // 16 x 4H floats = 16 H float4, 2 U per thread
+        const float4* src = reinterpret_cast<const float4*>(p.WgT + (size_t)chunk * kGateBK * N);
         float4* dst = reinterpret_cast<float4*>(&Ws[buf][0][0]);
 #pragma unroll
-        for (int q = 0; q < (kGateBK * kGN / 4) / kGThreads; ++q) {
+        for (int q = 0; q < (kGateBK * N / 4) / kGThreads; ++q) {
             int idx = tid + q * kGThreads;
             cp_async16(dst + idx, src + idx);
         }
@@ -117,8 +153,8 @@ __global__ void __launch_bounds__(kGThreads, 2) lstm_gates_kernel(GateParams p) 
                     v = p.pooled[(size_t)m * p.P + (k - p.E)];
                 } else if (k < p.K) {
                     int u = k - p.E - p.P;
-                    v = p.h_in[(size_t)m * kGH + u];
-                    if (p.add_pooled_to_h) v += p.pooled[(size_t)m * kGH + u];   // lstm.py:151
+                    v = p.h_in[(size_t)m * H + u];
+                    if (p.add_pooled_to_h) v += p.pooled[(size_t)m * H + u];   // lstm.py:151
                 }
             }
             As[buf][kk][r] = v;
@@ -145,48 +181,46 @@ __global__ void __launch_bounds__(kGThreads, 2) lstm_gates_kernel(GateParams p) 
             const float a[4] = {a4.x, a4.y, a4.z, a4.w};
 #pragma unroll
             for (int g = 0; g < 4; ++g) {
-                const float4 w4 = *reinterpret_cast<const float4*>(&Ws[buf][kk][g * kGH + lane * 4]);
-                const float w[4] = {w4.x, w4.y, w4.z, w4.w};
+                float w[U];
+                ld_units<U>(&Ws[buf][kk][g * H + lane * U], w);
 #pragma unroll
                 for (int r = 0; r < 4; ++r)
 #pragma unroll
-                    for (int u = 0; u < 4; ++u) acc[r][g][u] = fmaf(a[r], w[u], acc[r][g][u]);
+                    for (int u = 0; u < U; ++u) acc[r][g][u] = fmaf(a[r], w[u], acc[r][g][u]);
             }
         }
         __syncthreads();
     }
 
     // epilogue: LSTM pointwise + Gaussian head
-    float bgr[4][4];
+    float bgr[4][U];
 #pragma unroll
-    for (int g = 0; g < 4; ++g) {
-        const float4 b4 = *reinterpret_cast<const float4*>(p.bg + g * kGH + lane * 4);
-        bgr[g][0] = b4.x; bgr[g][1] = b4.y; bgr[g][2] = b4.z; bgr[g][3] = b4.w;
-    }
-    float wn[5][4];
+    for (int g = 0; g < 4; ++g) ld_units<U>(p.bg + g * H + lane * U, bgr[g]);
+    float wn[5][U];
 #pragma unroll
-    for (int o = 0; o < 5; ++o) {
-        const float4 w4 = *reinterpret_cast<const float4*>(p.Wn + o * kGH + lane * 4);
-        wn[o][0] = w4.x; wn[o][1] = w4.y; wn[o][2] = w4.z; wn[o][3] = w4.w;
-    }
+    for (int o = 0; o < 5; ++o) ld_units<U>(p.Wn + o * H + lane * U, wn[o]);
 #pragma unroll
     for (int r = 0; r < 4; ++r) {
         const int rl = warp * 4 + r;
         const int m = row0 + rl;
         if (m >= p.M) continue;                       // warp-uniform
-        const size_t off = (size_t)m * kGH + lane * 4;
-        const float4 c4 = *reinterpret_cast<const float4*>(p.c_in + off);
+        const size_t off = (size_t)m * H + lane * U;
+        float cold[U];
+        ld_units<U>(p.c_in + off, cold);
         if (!maskS[rl]) {                             // warp-uniform: absent track keeps its state
-            if (p.h_out != p.h_in) *reinterpret_cast<float4*>(p.h_out + off) = *reinterpret_cast<const float4*>(p.h_in + off);
-            if (p.c_out != p.c_in) *reinterpret_cast<float4*>(p.c_out + off) = c4;
+            if (p.h_out != p.h_in) {
+                float hv[U];
+                ld_units<U>(p.h_in + off, hv);
+                st_units<U>(p.h_out + off, hv);
+            }
+            if (p.c_out != p.c_in) st_units<U>(p.c_out + off, cold);
             if (lane < 5) p.normal_out[(size_t)m * 5 + lane] = CUDART_NAN_F;
             if (lane == 0 && p.pos_out) p.pos_out[m] = make_float2(CUDART_NAN_F, CUDART_NAN_F);
             continue;
         }
-        const float cold[4] = {c4.x, c4.y, c4.z, c4.w};
-        float hn[4], cn[4];
+        float hn[U], cn[U];
 #pragma unroll
-        for (int u = 0; u < 4; ++u) {
+        for (int u = 0; u < U; ++u) {
             float ig = sigmoidf_(acc[r][0][u] + bgr[0][u]);
             float fg = sigmoidf_(acc[r][1][u] + bgr[1][u]);
             float gg = tanhf(acc[r][2][u] + bgr[2][u]);
@@ -194,14 +228,14 @@ __global__ void __launch_bounds__(kGThreads, 2) lstm_gates_kernel(GateParams p) 
             cn[u] = fg * cold[u] + ig * gg;
             hn[u] = og * tanhf(cn[u]);
         }
-        *reinterpret_cast<float4*>(p.h_out + off) = make_float4(hn[0], hn[1], hn[2], hn[3]);
-        *reinterpret_cast<float4*>(p.c_out + off) = make_float4(cn[0], cn[1], cn[2], cn[3]);
+        st_units<U>(p.h_out + off, hn);
+        st_units<U>(p.c_out + off, cn);
         float part[5];
 #pragma unroll
         for (int o = 0; o < 5; ++o) {
             float s = 0.f;
 #pragma unroll
-            for (int u = 0; u < 4; ++u) s = fmaf(hn[u], wn[o][u], s);
+            for (int u = 0; u < U; ++u) s = fmaf(hn[u], wn[o][u], s);
             part[o] = s;
         }
 #pragma unroll
@@ -223,10 +257,23 @@ __global__ void __launch_bounds__(kGThreads, 2) lstm_gates_kernel(GateParams p) 
     }
 }
 
+template <int U>
+static int launch_gates_t(const GateParams& p, cudaStream_t st) {
+    const size_t smem = (size_t)2 * kGateBK * (4 * 32 * U + kGM) * sizeof(float);
+    static DynSmemConfig configured;
+    TB2_CHECK_CUDA(configured.ensure(lstm_gates_kernel<U>, smem));
+    const int blocks = (p.M + kGM - 1) / kGM;
+    {
+        KernelTimer kt("lstm_gates", st);
+        lstm_gates_kernel<U><<<blocks, kGThreads, smem, st>>>(p);
+    }
+    TB2_LAUNCH_CHECK();
+    return TB2_OK;
+}
+
 int launch_gates(const tb2_lstm* m, const tb2_layout* l, int phase, const float* obs1,
                  const float* obs2, const float* pooled, const float* h_in, const float* c_in,
                  float* h_out, float* c_out, float* normal_out, float* pos_out, cudaStream_t st) {
-    TB2_REQUIRE(m->H == kGH, "hidden_dim must be 128");
     GateParams p;
     p.obs1 = (const float2*)obs1;
     p.obs2 = (const float2*)obs2;
@@ -249,16 +296,19 @@ int launch_gates(const tb2_lstm* m, const tb2_layout* l, int phase, const float*
     p.K = m->K_gate;
     p.K_pad = m->K_gate_pad;
     p.add_pooled_to_h = (m->cfg.pool_type != TB2_POOL_NONE && !m->cfg.pool_to_input) ? 1 : 0;
-    const size_t smem = (size_t)2 * kGateBK * (kGN + kGM) * sizeof(float);
-    static DynSmemConfig configured;
-    TB2_CHECK_CUDA(configured.ensure(lstm_gates_kernel, smem));
-    int blocks = (l->M + kGM - 1) / kGM;
-    {
-        KernelTimer kt("lstm_gates", st);
-        lstm_gates_kernel<<<blocks, kGThreads, smem, st>>>(p);
+    switch (m->H) {
+        case 32: return launch_gates_t<1>(p, st);
+        case 64: return launch_gates_t<2>(p, st);
+        case 96: return launch_gates_t<3>(p, st);
+        case 128: return launch_gates_t<4>(p, st);
+        case 160: return launch_gates_t<5>(p, st);
+        case 192: return launch_gates_t<6>(p, st);
+        case 224: return launch_gates_t<7>(p, st);
+        case 256: return launch_gates_t<8>(p, st);
+        default: break;
     }
-    TB2_LAUNCH_CHECK();
-    return TB2_OK;
+    set_error(kHiddenDimMessage);
+    return TB2_ERR_UNSUPPORTED;
 }
 
 // ------------------------------------------------------------------------------------------

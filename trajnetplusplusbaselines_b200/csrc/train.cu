@@ -29,8 +29,6 @@
 
 namespace tb2 {
 
-constexpr int kBH = 128;
-
 __device__ __forceinline__ float sigm(float x) { return 1.f / (1.f + expf(-x)); }
 
 // X[r] = [emb(vel) | pooled | h_prev] for the active rows (one CTA per row).  The pooled part is
@@ -42,7 +40,7 @@ __global__ void __launch_bounds__(256) bwd_gather_kernel(
     const int* __restrict__ win_count, const uint32_t* __restrict__ win_ent, const float* __restrict__ win_val,
     const float* __restrict__ Wt1, const float* __restrict__ base1, int nm1, int C, int cells,
     const float* __restrict__ pooled_src, float* __restrict__ X, float* __restrict__ G, float* __restrict__ vel,
-    int* __restrict__ masked, int E, int P, int K) {
+    int* __restrict__ masked, int E, int P, int K, int H) {
     __shared__ uint32_t ent_s[64];
     __shared__ float val_s[64][2];
     const int r = blockIdx.x;
@@ -66,8 +64,8 @@ __global__ void __launch_bounds__(256) bwd_gather_kernel(
     }
     for (int k = threadIdx.x; k < E; k += blockDim.x)
         x[k] = k < E - 2 ? fmaxf(fmaf(We[2 * k + 1], vy, fmaf(We[2 * k], vx, be[k])), 0.f) : 0.f;
-    for (int k = threadIdx.x; k < kBH; k += blockDim.x)
-        x[E + P + k] = h_prev ? h_prev[(size_t)m * kBH + k] : 0.f;
+    for (int k = threadIdx.x; k < H; k += blockDim.x)
+        x[E + P + k] = h_prev ? h_prev[(size_t)m * H + k] : 0.f;
     if (pooled_src) {      // pooled vector of this row as the forward kernels produced it
         for (int o = threadIdx.x; o < P; o += blockDim.x) x[E + o] = pooled_src[(size_t)m * P + o];
     } else if (P > 0) {
@@ -112,75 +110,77 @@ __global__ void __launch_bounds__(256) bwd_gather_kernel(
     }
 }
 
-// Backward of LSTMCell + Hidden2Normal for one active row per CTA (128 threads = units): the only
-// kernel on the sequential chain of the BPTT.
-//   in : gates_pre [R,512] of this step (with bias), c_prev (state before the step, null = zeros),
+// Backward of LSTMCell + Hidden2Normal for one active row per CTA (4H threads; the first H, one per unit, do the cell
+// and head math): the only kernel on the sequential chain of the BPTT.
+//   in : gates_pre [R,4H] of this step (with bias), c_prev (state before the step, null = zeros),
 //        incoming dh = dg_next[r] . Whh_next (recurrent part of the LATER step's gate gradient,
 //        W_hh in torch layout [4H, H]) + pass_prev[r] (what by-passed the cell there); both null
-//        at the last step.  dc [R,128] in place; upstream dnormal [M,5] (row-indexed by track)
-//   out: dgates [R,512], dc (gradient wrt c_prev), hs [R,128] (h of this step), dn_raw [R,8],
-//        pass_cur [R,128] (masked rows: dh goes straight through, lstm.py:158-166)
-__global__ void __launch_bounds__(4 * kBH) bwd_cell_head_kernel(
+//        at the last step.  dc [R,H] in place; upstream dnormal [M,5] (row-indexed by track)
+//   out: dgates [R,4H], dc (gradient wrt c_prev), hs [R,H] (h of this step), dn_raw [R,8],
+//        pass_cur [R,H] (masked rows: dh goes straight through, lstm.py:158-166)
+template <int H>
+__global__ void __launch_bounds__(4 * H) bwd_cell_head_kernel(
     const int* __restrict__ rows, const int* __restrict__ masked, const float* __restrict__ gates_pre,
     const float* __restrict__ c_prev, const float* __restrict__ dg_next, const float* __restrict__ Whh_next,
     const float* __restrict__ dh_rec, const float* __restrict__ pass_prev, float* __restrict__ pass_cur,
     float* __restrict__ dc,
     const float* __restrict__ dnormal, const float* __restrict__ Wn, const float* __restrict__ bn,
     float* __restrict__ dgates, float* __restrict__ hs, float* __restrict__ dn_raw, int R) {
-    __shared__ float red[5][kBH];
+    constexpr int kPow2 = H <= 32 ? 32 : H <= 64 ? 64 : H <= 128 ? 128 : 256;     // tree width of the head sums
+    __shared__ float red[5][H];
     __shared__ float dn_s[5];
-    __shared__ __align__(16) float dgn_s[4 * kBH];
-    __shared__ float part_s[4][kBH];
-    const int r = blockIdx.x, u = threadIdx.x & (kBH - 1), quarter = threadIdx.x >> 7;
+    __shared__ __align__(16) float dgn_s[4 * H];
+    __shared__ float part_s[4][H];
+    const int r = blockIdx.x, u = threadIdx.x % H, quarter = threadIdx.x / H;
     const int m = rows[r];
-    float* dg = dgates + (size_t)r * 4 * kBH;
+    float* dg = dgates + (size_t)r * 4 * H;
     float dh_in = 0.f;
     if (dh_rec) {       // many rows: dg_next . W_hh was done as one GEMM
-        dh_in = dh_rec[(size_t)r * kBH + u] + pass_prev[(size_t)r * kBH + u];
-    } else if (dg_next) {      // 4 x 128 threads: each quarter of the CTA reduces one gate block of the mat-vec
-        dgn_s[threadIdx.x] = dg_next[(size_t)r * 4 * kBH + threadIdx.x];
+        dh_in = dh_rec[(size_t)r * H + u] + pass_prev[(size_t)r * H + u];
+    } else if (dg_next) {      // 4 x H threads: each quarter of the CTA reduces one gate block of the mat-vec
+        dgn_s[threadIdx.x] = dg_next[(size_t)r * 4 * H + threadIdx.x];
         __syncthreads();
         float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
-        const float* wq = Whh_next + (size_t)quarter * kBH * kBH + u;
-        const float* dq = dgn_s + quarter * kBH;
+        const float* wq = Whh_next + (size_t)quarter * H * H + u;
+        const float* dq = dgn_s + quarter * H;
 #pragma unroll 4
-        for (int g = 0; g < kBH; g += 4) {
-            a0 = fmaf(dq[g + 0], wq[(size_t)(g + 0) * kBH], a0);
-            a1 = fmaf(dq[g + 1], wq[(size_t)(g + 1) * kBH], a1);
-            a2 = fmaf(dq[g + 2], wq[(size_t)(g + 2) * kBH], a2);
-            a3 = fmaf(dq[g + 3], wq[(size_t)(g + 3) * kBH], a3);
+        for (int g = 0; g < H; g += 4) {
+            a0 = fmaf(dq[g + 0], wq[(size_t)(g + 0) * H], a0);
+            a1 = fmaf(dq[g + 1], wq[(size_t)(g + 1) * H], a1);
+            a2 = fmaf(dq[g + 2], wq[(size_t)(g + 2) * H], a2);
+            a3 = fmaf(dq[g + 3], wq[(size_t)(g + 3) * H], a3);
         }
         part_s[quarter][u] = (a0 + a1) + (a2 + a3);
         __syncthreads();
-        dh_in = (part_s[0][u] + part_s[1][u]) + (part_s[2][u] + part_s[3][u]) + pass_prev[(size_t)r * kBH + u];
+        dh_in = (part_s[0][u] + part_s[1][u]) + (part_s[2][u] + part_s[3][u]) + pass_prev[(size_t)r * H + u];
     }
-    if (quarter != 0) return;       // the cell / head math below is one thread per unit
+    if (quarter != 0) return;       // the cell / head math below is one thread per unit (warps 0 .. H/32 - 1)
     if (masked[r]) {   // absent track: state passes through, no parameter gradient
 #pragma unroll
-        for (int g = 0; g < 4; ++g) dg[g * kBH + u] = 0.f;
-        hs[(size_t)r * kBH + u] = 0.f;
+        for (int g = 0; g < 4; ++g) dg[g * H + u] = 0.f;
+        hs[(size_t)r * H + u] = 0.f;
         if (u < 8) dn_raw[r * 8 + u] = 0.f;
-        pass_cur[(size_t)r * kBH + u] = dh_in;
+        pass_cur[(size_t)r * H + u] = dh_in;
         return;        // dc stays as it is
     }
-    pass_cur[(size_t)r * kBH + u] = 0.f;
-    const float* gp = gates_pre + (size_t)r * 4 * kBH;
-    const float ig = sigm(gp[u]), fg = sigm(gp[kBH + u]), gg = tanhf(gp[2 * kBH + u]), og = sigm(gp[3 * kBH + u]);
-    const float cp = c_prev ? c_prev[(size_t)m * kBH + u] : 0.f;
+    pass_cur[(size_t)r * H + u] = 0.f;
+    const float* gp = gates_pre + (size_t)r * 4 * H;
+    const float ig = sigm(gp[u]), fg = sigm(gp[H + u]), gg = tanhf(gp[2 * H + u]), og = sigm(gp[3 * H + u]);
+    const float cp = c_prev ? c_prev[(size_t)m * H + u] : 0.f;
     const float cn = fg * cp + ig * gg;
     const float tc = tanhf(cn);
     const float hn = og * tc;
-    hs[(size_t)r * kBH + u] = hn;
+    hs[(size_t)r * H + u] = hn;
     // head: n_raw = Wn h + bn (modules.py:57); recomputed for the sigmoid derivatives
 #pragma unroll
-    for (int o = 0; o < 5; ++o) red[o][u] = Wn[o * kBH + u] * hn;
-    asm volatile("bar.sync 1, 128;" ::: "memory");
-    for (int s = kBH / 2; s > 0; s >>= 1) {
-        if (u < s) {
+    for (int o = 0; o < 5; ++o) red[o][u] = Wn[o * H + u] * hn;
+    asm volatile("bar.sync 1, %0;" ::"n"(H) : "memory");
+    for (int s = kPow2 / 2; s > 0; s >>= 1) {
+        if (u < s && u + s < H) {
 #pragma unroll
             for (int o = 0; o < 5; ++o) red[o][u] += red[o][u + s];
         }
-        asm volatile("bar.sync 1, 128;" ::: "memory");
+        asm volatile("bar.sync 1, %0;" ::"n"(H) : "memory");
     }
     if (u < 8) {
         float d = 0.f;
@@ -196,18 +196,18 @@ __global__ void __launch_bounds__(4 * kBH) bwd_cell_head_kernel(
         }
         dn_raw[r * 8 + u] = d;
     }
-    asm volatile("bar.sync 1, 128;" ::: "memory");
+    asm volatile("bar.sync 1, %0;" ::"n"(H) : "memory");
     float dht = dh_in;
 #pragma unroll
-    for (int o = 0; o < 5; ++o) dht = fmaf(Wn[o * kBH + u], dn_s[o], dht);
-    float dct = dc[(size_t)r * kBH + u] + dht * og * (1.f - tc * tc);
+    for (int o = 0; o < 5; ++o) dht = fmaf(Wn[o * H + u], dn_s[o], dht);
+    float dct = dc[(size_t)r * H + u] + dht * og * (1.f - tc * tc);
     const float dog = dht * tc;
     const float dig = dct * gg, dgg = dct * ig, dfg = dct * cp;
     dg[u] = dig * ig * (1.f - ig);
-    dg[kBH + u] = dfg * fg * (1.f - fg);
-    dg[2 * kBH + u] = dgg * (1.f - gg * gg);
-    dg[3 * kBH + u] = dog * og * (1.f - og);
-    dc[(size_t)r * kBH + u] = dct * fg;
+    dg[H + u] = dfg * fg * (1.f - fg);
+    dg[2 * H + u] = dgg * (1.f - gg * gg);
+    dg[3 * H + u] = dog * og * (1.f - og);
+    dc[(size_t)r * H + u] = dct * fg;
 }
 
 // ------------------------------------------------------------------------------------------
@@ -844,7 +844,7 @@ __global__ void __launch_bounds__(256) social_dgrid_mma_kernel(const unsigned* _
 __global__ void __launch_bounds__(256) social_scene_reduce_kernel(
     const int* __restrict__ scene_off, const int* __restrict__ masked, const uint8_t* __restrict__ pair_flag,
     int nm1, int C, const float* __restrict__ dgrid, const float* __restrict__ Wenc, float* __restrict__ dlat,
-    float* __restrict__ dh_add) {
+    float* __restrict__ dh_add, int H) {
     extern __shared__ float dl_s[];       // [n_s][C]
     const int b = blockIdx.x, row0 = scene_off[b], n_s = scene_off[b + 1] - row0;
     for (int idx = threadIdx.x; idx < n_s * C; idx += blockDim.x) {
@@ -860,11 +860,11 @@ __global__ void __launch_bounds__(256) social_scene_reduce_kernel(
     }
     __syncthreads();
     if (dh_add) {
-        for (int idx = threadIdx.x; idx < n_s * kBH; idx += blockDim.x) {
-            const int j = idx / kBH, u = idx - j * kBH;
+        for (int idx = threadIdx.x; idx < n_s * H; idx += blockDim.x) {
+            const int j = idx / H, u = idx - j * H;
             float a = 0.f;
-            for (int ch = 0; ch < C; ++ch) a = fmaf(dl_s[j * C + ch], Wenc[ch * kBH + u], a);
-            dh_add[(size_t)(row0 + j) * kBH + u] += a;
+            for (int ch = 0; ch < C; ++ch) a = fmaf(dl_s[j * C + ch], Wenc[ch * H + u], a);
+            dh_add[(size_t)(row0 + j) * H + u] += a;
         }
     }
 }
@@ -1192,11 +1192,29 @@ static int colsum(const float* A, int lda, int R, int N, float* out, float* out2
     return TB2_OK;
 }
 
+// bwd_cell_head_kernel at the model's width (4H threads per row)
+template <typename... Args>
+static int launch_cell_head(int H, int rows, cudaStream_t st, Args... args) {
+    switch (H) {
+        case 32: bwd_cell_head_kernel<32><<<rows, 4 * 32, 0, st>>>(args...); break;
+        case 64: bwd_cell_head_kernel<64><<<rows, 4 * 64, 0, st>>>(args...); break;
+        case 96: bwd_cell_head_kernel<96><<<rows, 4 * 96, 0, st>>>(args...); break;
+        case 128: bwd_cell_head_kernel<128><<<rows, 4 * 128, 0, st>>>(args...); break;
+        case 160: bwd_cell_head_kernel<160><<<rows, 4 * 160, 0, st>>>(args...); break;
+        case 192: bwd_cell_head_kernel<192><<<rows, 4 * 192, 0, st>>>(args...); break;
+        case 224: bwd_cell_head_kernel<224><<<rows, 4 * 224, 0, st>>>(args...); break;
+        case 256: bwd_cell_head_kernel<256><<<rows, 4 * 256, 0, st>>>(args...); break;
+        default: set_error(kHiddenDimMessage); return TB2_ERR_UNSUPPORTED;
+    }
+    TB2_LAUNCH_CHECK();
+    return TB2_OK;
+}
+
 // Carving of the backward workspace (floats).  Per (step, row) records are kept so that every
 // weight gradient is one reduction over all S * R rows after the time loop.
 struct BwdBuffers {
-    float *X, *GP, *DG, *HS, *DN, *VEL, *DXIN, *G;     // [S][R][K | 512 | 512 | 128 | 8 | 2 | E+P | C n n]
-    float *pass[2], *dc;                               // [R][128] chain state
+    float *X, *GP, *DG, *HS, *DN, *VEL, *DXIN, *G;     // [S][R][K | G4 | G4 | H | 8 | 2 | E+P | C n n]
+    float *pass[2], *dc;                               // [R][H] chain state
     float* scratch;                                    // partial sums of the row-split reductions
     size_t scratch_floats;
     int* masked;                                       // [S][R]
@@ -1204,6 +1222,7 @@ struct BwdBuffers {
 
 static size_t carve_bwd(const tb2_lstm* m, size_t R, size_t S, void* base, BwdBuffers* b) {
     const size_t K = (size_t)m->K_gate, E = (size_t)m->E, P = (size_t)(m->P > 0 ? m->P : 0);
+    const size_t H = (size_t)m->H, G4 = 4 * H;
     size_t off = 0;
     auto take = [&](size_t n) {
         float* p = base ? reinterpret_cast<float*>(base) + off : nullptr;
@@ -1214,17 +1233,17 @@ static size_t carve_bwd(const tb2_lstm* m, size_t R, size_t S, void* base, BwdBu
     BwdBuffers* o = b ? b : &tmp;
     const size_t CG = (size_t)m->C * (size_t)m->cells;
     o->X = take(S * R * K);
-    o->GP = take(S * R * 512);
-    o->DG = take(S * R * 512);
-    o->HS = take(S * R * 128);
+    o->GP = take(S * R * G4);
+    o->DG = take(S * R * G4);
+    o->HS = take(S * R * H);
     o->DN = take(S * R * 8);
     o->VEL = take(S * R * 2);
     o->DXIN = take(S * R * (E + P));
     o->G = take(P ? S * R * CG : 4);
-    o->pass[0] = take(R * 128);
-    o->pass[1] = take(R * 128);
-    o->dc = take(R * 128);
-    size_t big = 512 * K;
+    o->pass[0] = take(R * H);
+    o->pass[1] = take(R * H);
+    o->dc = take(R * H);
+    size_t big = G4 * K;
     if (P * CG > big) big = P * CG;
     o->scratch_floats = 8 * big;
     o->scratch = take(o->scratch_floats);
@@ -1283,19 +1302,20 @@ struct SocBuffers {
     __nv_bfloat16 *Wt1_hi, *Wt1_lo;                       // bf16 split of the cell-major first-layer weights (dgrid on mma.sync)
     // 3-pass wgmma versions of the row GEMMs (dense_layer_tc_kernel): bf16 (hi, lo) operands
     __nv_bfloat16 *X_hi, *X_lo;                           // [S][M][K]
-    __nv_bfloat16 *DG_hi[2], *DG_lo[2];                   // [M][512], steps s and s + 1
+    __nv_bfloat16 *DG_hi[2], *DG_lo[2];                   // [M][G4], steps s and s + 1
     __nv_bfloat16 *DZ2_hi, *DZ2_lo;                       // [M][P]
-    __nv_bfloat16 *Wcat_hi[2], *Wcat_lo[2];               // [512][K] = [W_ih | W_hh] per phase
-    __nv_bfloat16 *WhhT_hi[2], *WhhT_lo[2];               // [128][512]
-    __nv_bfloat16 *WihT_hi[2], *WihT_lo[2];               // [E + P][512]
+    __nv_bfloat16 *Wcat_hi[2], *Wcat_lo[2];               // [G4][K] = [W_ih | W_hh] per phase
+    __nv_bfloat16 *WhhT_hi[2], *WhhT_lo[2];               // [H][G4]
+    __nv_bfloat16 *WihT_hi[2], *WihT_lo[2];               // [E + P][G4]
     __nv_bfloat16 *W2T_hi, *W2T_lo;                       // [d1][P]
-    float* zero_bias;                                     // [max(d1, 512)]
+    float* zero_bias;                                     // [max(d1, G4)]
 };
 
 static size_t carve_social(const tb2_lstm* m, const tb2_layout* l, size_t S, void* basep, SocBuffers* b) {
     const size_t M = (size_t)l->M, K = (size_t)m->K_gate, E = (size_t)m->E, P = (size_t)m->P;
     const size_t d1 = (size_t)m->mlp_dims[1], C = (size_t)m->C, cells = (size_t)m->cells;
     const size_t nm1 = (size_t)(l->n_max > 1 ? l->n_max - 1 : 1);
+    const size_t H = (size_t)m->H, G4 = 4 * H;
     size_t off = 0;
     auto take = [&](size_t n) {
         float* p = basep ? reinterpret_cast<float*>(basep) + off : nullptr;
@@ -1305,23 +1325,23 @@ static size_t carve_social(const tb2_lstm* m, const tb2_layout* l, size_t S, voi
     SocBuffers tmp;
     SocBuffers* o = b ? b : &tmp;
     o->X = take(S * M * K);
-    o->GP = take(S * M * 512);
-    o->DG = take(S * M * 512);
-    o->HS = take(S * M * 128);
+    o->GP = take(S * M * G4);
+    o->DG = take(S * M * G4);
+    o->HS = take(S * M * H);
     o->DN = take(S * M * 8);
     o->VEL = take(S * M * 2);
     o->DXIN = take(S * M * (E + P));
     o->H1 = take(m->n_mlp == 2 ? S * M * d1 : 4);
-    o->DH1 = take(M * (d1 > 128 ? d1 : 128));     // also holds the [M,128] recurrent d h of a step
+    o->DH1 = take(M * (d1 > H ? d1 : H));     // also holds the [M,H] recurrent d h of a step
     o->LAT = take(S * M * C);
     o->DLAT = take(S * M * C);
     o->DGRID = take(M * nm1 * C);
     o->dWt1 = take(cells * C * d1);
-    o->pass[0] = take(M * 128);
-    o->pass[1] = take(M * 128);
-    o->dc = take(M * 128);
-    o->zero_h = take(M * 128);
-    size_t big = 512 * K;
+    o->pass[0] = take(M * H);
+    o->pass[1] = take(M * H);
+    o->dc = take(M * H);
+    o->zero_h = take(M * H);
+    size_t big = G4 * K;
     if (P * d1 > big) big = P * d1;
     o->scratch_floats = 8 * big;
     o->scratch = take(o->scratch_floats);
@@ -1341,20 +1361,20 @@ static size_t carve_social(const tb2_lstm* m, const tb2_layout* l, size_t S, voi
     o->X_hi = take_bf16(S * M * K);
     o->X_lo = take_bf16(S * M * K);
     for (int i = 0; i < 2; ++i) {
-        o->DG_hi[i] = take_bf16(M * 512);
-        o->DG_lo[i] = take_bf16(M * 512);
-        o->Wcat_hi[i] = take_bf16(512 * K);
-        o->Wcat_lo[i] = take_bf16(512 * K);
-        o->WhhT_hi[i] = take_bf16(128 * 512);
-        o->WhhT_lo[i] = take_bf16(128 * 512);
-        o->WihT_hi[i] = take_bf16((E + P) * 512);
-        o->WihT_lo[i] = take_bf16((E + P) * 512);
+        o->DG_hi[i] = take_bf16(M * G4);
+        o->DG_lo[i] = take_bf16(M * G4);
+        o->Wcat_hi[i] = take_bf16(G4 * K);
+        o->Wcat_lo[i] = take_bf16(G4 * K);
+        o->WhhT_hi[i] = take_bf16(H * G4);
+        o->WhhT_lo[i] = take_bf16(H * G4);
+        o->WihT_hi[i] = take_bf16((E + P) * G4);
+        o->WihT_lo[i] = take_bf16((E + P) * G4);
     }
     o->DZ2_hi = take_bf16(M * P);
     o->DZ2_lo = take_bf16(M * P);
     o->W2T_hi = take_bf16(d1 * P);
     o->W2T_lo = take_bf16(d1 * P);
-    o->zero_bias = take(d1 > 512 ? d1 : 512);
+    o->zero_bias = take(d1 > G4 ? d1 : G4);
     return off * sizeof(float) + 256;
 }
 
@@ -1396,6 +1416,7 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
                            const TrainCache* cache = nullptr) {
     const int S = obs_length - 1 + n_decode, S_enc = obs_length - 1;
     const int Mi = l->M, K = m->K_gate, E = m->E, P = m->P, EP = E + P, C = m->C, cells = m->cells;
+    const int H = m->H, G4 = 4 * H;
     const int d1 = m->mlp_dims[1];
     const bool two = m->n_mlp == 2;
     const size_t M = (size_t)Mi;
@@ -1412,9 +1433,9 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
         b.pcell = cache->pair_cell;
         b.pflag = cache->pair_flag;
     }
-    TB2_CHECK_CUDA(cudaMemsetAsync(b.dc, 0, M * 128 * sizeof(float), st));
+    TB2_CHECK_CUDA(cudaMemsetAsync(b.dc, 0, M * H * sizeof(float), st));
     TB2_CHECK_CUDA(cudaMemsetAsync(b.dWt1, 0, (size_t)cells * C * d1 * sizeof(float), st));
-    TB2_CHECK_CUDA(cudaMemsetAsync(b.zero_h, 0, M * 128 * sizeof(float), st));      // state before step 0
+    TB2_CHECK_CUDA(cudaMemsetAsync(b.zero_h, 0, M * H * sizeof(float), st));      // state before step 0
     iota_kernel<<<(Mi + 255) / 256, 256, 0, st>>>(b.rows, Mi);
     TB2_LAUNCH_CHECK();
     int rc;
@@ -1425,7 +1446,7 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
         const float *o1, *o2;
         int phase;
         if ((rc = resolve_step_inputs(l, observed, obs_length, truth, positions, s, &ws, &o1, &o2, &phase, st))) return rc;
-        const float* h_prev = s > 0 ? states + ((size_t)(s - 1) * 2 + 0) * M * kBH : nullptr;
+        const float* h_prev = s > 0 ? states + ((size_t)(s - 1) * 2 + 0) * M * H : nullptr;
         Workspace w2 = ws;
         w2.lat = b.LAT + (size_t)s * M * C;
         w2.win_count = b.winc + (size_t)s * M;
@@ -1459,25 +1480,26 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
             bwd_gather_kernel<<<Mi, 256, 0, st>>>(b.rows, Mi, (const float2*)o1, (const float2*)o2, m->We, m->be,
                                                   h_prev, nullptr, nullptr, nullptr, nullptr, nullptr, nm1, C, cells,
                                                   ws.pooled, b.X + (size_t)s * M * K, nullptr,
-                                                  b.VEL + (size_t)s * M * 2, b.masked + (size_t)s * M, E, P, K);
+                                                  b.VEL + (size_t)s * M * 2, b.masked + (size_t)s * M, E, P, K, H);
         }
         TB2_LAUNCH_CHECK();
     }
     // The row GEMMs (rows = all tracks) run on the 3-pass wgmma kernel of the forward (dense_layer_tc_kernel:
     // Y = A . W^T + bias, bf16 (hi, lo) operands, fp32 accumulation) when the shapes allow it: A and the (transposed)
     // weights are split once, the outputs stay fp32.  Other shapes, and TB2_DISABLE_TC=1: cuBLAS / FFMA GEMMs.
-    const bool tcg = !m->tc_disabled && K == EP + 128 && dense_tc_supported(K, 512) && dense_tc_supported(512, 128) &&
-                     dense_tc_supported(512, EP) && (!two || dense_tc_supported(P, d1));
+    // H % 128: the wgmma row GEMMs of the recurrent d h then use the 128-column tiles the H = 128 build was checked with
+    const bool tcg = !m->tc_disabled && H % 128 == 0 && dense_tc_supported(K, G4) && dense_tc_supported(G4, H) &&
+                     dense_tc_supported(G4, EP) && (!two || dense_tc_supported(P, d1));
     if (tcg) {
-        TB2_CHECK_CUDA(cudaMemsetAsync(b.zero_bias, 0, (size_t)(d1 > 512 ? d1 : 512) * sizeof(float), st));
+        TB2_CHECK_CUDA(cudaMemsetAsync(b.zero_bias, 0, (size_t)(d1 > G4 ? d1 : G4) * sizeof(float), st));
         for (int phase = 0; phase < 2; ++phase) {
             const float* Wih_p = phase == TB2_PHASE_ENCODER ? w->encoder_weight_ih : w->decoder_weight_ih;
             const float* Whh_p = phase == TB2_PHASE_ENCODER ? w->encoder_weight_hh : w->decoder_weight_hh;
-            if ((rc = split2d(Wih_p, EP, 512, EP, b.Wcat_hi[phase], b.Wcat_lo[phase], K, 0, st))) return rc;
-            if ((rc = split2d(Whh_p, 128, 512, 128, b.Wcat_hi[phase], b.Wcat_lo[phase], K, EP, st))) return rc;
-            transpose_split_kernel<<<256, 256, 0, st>>>(Whh_p, 512, 128, b.WhhT_hi[phase], b.WhhT_lo[phase]);
+            if ((rc = split2d(Wih_p, EP, G4, EP, b.Wcat_hi[phase], b.Wcat_lo[phase], K, 0, st))) return rc;
+            if ((rc = split2d(Whh_p, H, G4, H, b.Wcat_hi[phase], b.Wcat_lo[phase], K, EP, st))) return rc;
+            transpose_split_kernel<<<256, 256, 0, st>>>(Whh_p, G4, H, b.WhhT_hi[phase], b.WhhT_lo[phase]);
             TB2_LAUNCH_CHECK();
-            transpose_split_kernel<<<512, 256, 0, st>>>(Wih_p, 512, EP, b.WihT_hi[phase], b.WihT_lo[phase]);
+            transpose_split_kernel<<<512, 256, 0, st>>>(Wih_p, G4, EP, b.WihT_hi[phase], b.WihT_lo[phase]);
             TB2_LAUNCH_CHECK();
         }
         if (two) {
@@ -1493,13 +1515,13 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
         if (ns <= 0) continue;
         if (tcg) {
             if ((rc = launch_dense_tc(b.X_hi + (size_t)s0 * M * K, b.X_lo + (size_t)s0 * M * K, b.Wcat_hi[phase],
-                                      b.Wcat_lo[phase], m->bg[phase], b.GP + (size_t)s0 * M * 512, nullptr, nullptr, ns * Mi,
-                                      K, 512, 0, st)))
+                                      b.Wcat_lo[phase], m->bg[phase], b.GP + (size_t)s0 * M * G4, nullptr, nullptr, ns * Mi,
+                                      K, G4, 0, st)))
                 return rc;
             continue;
         }
-        if ((rc = gemm_nn(b.X + (size_t)s0 * M * K, K, m->WgT[phase], 512, b.GP + (size_t)s0 * M * 512, 512,
-                          ns * Mi, 512, K, m->bg[phase], st)))
+        if ((rc = gemm_nn(b.X + (size_t)s0 * M * K, K, m->WgT[phase], G4, b.GP + (size_t)s0 * M * G4, G4,
+                          ns * Mi, G4, K, m->bg[phase], st)))
             return rc;
     }
     // (C) reverse time: cell -> input gradient -> grid MLP -> scatter to the neighbours' hidden states
@@ -1512,12 +1534,12 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
     int cur = 0;
     for (int s = S - 1; s >= 0; --s, cur ^= 1) {
         const int phase = s < S_enc ? TB2_PHASE_ENCODER : TB2_PHASE_DECODER;
-        const float* c_prev = s > 0 ? states + ((size_t)(s - 1) * 2 + 1) * M * kBH : nullptr;
+        const float* c_prev = s > 0 ? states + ((size_t)(s - 1) * 2 + 1) * M * H : nullptr;
         const bool last = s == S - 1;
         const int next_phase = (s + 1) < S_enc ? TB2_PHASE_ENCODER : TB2_PHASE_DECODER;
         const float* Whh_next = next_phase == TB2_PHASE_ENCODER ? w->encoder_weight_hh : w->decoder_weight_hh;
         const float* Wih = phase == TB2_PHASE_ENCODER ? w->encoder_weight_ih : w->decoder_weight_ih;
-        float* DGs = b.DG + (size_t)s * M * 512;
+        float* DGs = b.DG + (size_t)s * M * G4;
         float* DXs = b.DXIN + (size_t)s * M * EP;
         const float* Xs = b.X + (size_t)s * M * K;
         // recurrent part of d h: all rows are active, so dgates(s+1) . W_hh is a GEMM (DH1 is free here)
@@ -1526,27 +1548,27 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
             dh_rec = b.DH1;
             if (tcg) {      // dgates(s + 1) was split at the end of the previous iteration
                 if ((rc = launch_dense_tc(b.DG_hi[(s + 1) & 1], b.DG_lo[(s + 1) & 1], b.WhhT_hi[next_phase], b.WhhT_lo[next_phase],
-                                          b.zero_bias, dh_rec, nullptr, nullptr, Mi, 512, 128, 0, st)))
+                                          b.zero_bias, dh_rec, nullptr, nullptr, Mi, G4, H, 0, st)))
                     return rc;
-            } else if ((rc = gemm_nn(b.DG + (size_t)(s + 1) * M * 512, 512, Whh_next, 128, dh_rec, 128, Mi, 128, 512, nullptr,
+            } else if ((rc = gemm_nn(b.DG + (size_t)(s + 1) * M * G4, G4, Whh_next, H, dh_rec, H, Mi, H, G4, nullptr,
                                      st)))
                 return rc;
         }
         {
             KernelTimer kt("bwd_cell_head", st);
-            bwd_cell_head_kernel<<<Mi, 4 * kBH, 0, st>>>(
-                b.rows, b.masked + (size_t)s * M, b.GP + (size_t)s * M * 512, c_prev, nullptr, Whh_next, dh_rec,
+            rc = launch_cell_head(H, Mi, st,
+                b.rows, b.masked + (size_t)s * M, b.GP + (size_t)s * M * G4, c_prev, nullptr, Whh_next, dh_rec,
                 b.pass[cur ^ 1], b.pass[cur], b.dc,
-                d_normals + (size_t)s * M * 5, m->Wn, m->bn, DGs, b.HS + (size_t)s * M * 128,
+                d_normals + (size_t)s * M * 5, m->Wn, m->bn, DGs, b.HS + (size_t)s * M * H,
                 b.DN + (size_t)s * M * 8, Mi);
         }
-        TB2_LAUNCH_CHECK();
+        if (rc) return rc;
         if (tcg) {
-            if ((rc = split2d(DGs, 512, M, 512, b.DG_hi[s & 1], b.DG_lo[s & 1], 512, 0, st))) return rc;
+            if ((rc = split2d(DGs, G4, M, G4, b.DG_hi[s & 1], b.DG_lo[s & 1], G4, 0, st))) return rc;
             if ((rc = launch_dense_tc(b.DG_hi[s & 1], b.DG_lo[s & 1], b.WihT_hi[phase], b.WihT_lo[phase], b.zero_bias, DXs,
-                                      nullptr, nullptr, Mi, 512, EP, 0, st)))
+                                      nullptr, nullptr, Mi, G4, EP, 0, st)))
                 return rc;
-        } else if ((rc = gemm_nn(DGs, 512, Wih, EP, DXs, EP, Mi, EP, 512, nullptr, st))) return rc;
+        } else if ((rc = gemm_nn(DGs, G4, Wih, EP, DXs, EP, Mi, EP, G4, nullptr, st))) return rc;
         const unsigned eb = (unsigned)((M * d1 + 255) / 256);
         if (two) {
             const float* H1s = b.H1 + (size_t)s * M * d1;
@@ -1594,7 +1616,7 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
             KernelTimer kt("social_scene_reduce", st);
             social_scene_reduce_kernel<<<l->B, 256, (size_t)l->n_max * C * sizeof(float), st>>>(
                 l->scene_off, msk, pflag, nm1, C, b.DGRID, w->pool_encoding_weight, b.DLAT + (size_t)s * M * C,
-                s > 0 ? b.pass[cur] : nullptr);
+                s > 0 ? b.pass[cur] : nullptr, H);
         }
         TB2_LAUNCH_CHECK();
     }
@@ -1608,18 +1630,18 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
         const int s0 = phase == TB2_PHASE_ENCODER ? 0 : S_enc;
         const int ns = phase == TB2_PHASE_ENCODER ? S_enc : S - S_enc;
         if (ns <= 0) continue;
-        const float* DG = b.DG + (size_t)s0 * M * 512;
+        const float* DG = b.DG + (size_t)s0 * M * G4;
         const float* X = b.X + (size_t)s0 * M * K;
         const int rows = ns * Mi;
         float* gWih = phase == TB2_PHASE_ENCODER ? g->encoder_weight_ih : g->decoder_weight_ih;
         float* gWhh = phase == TB2_PHASE_ENCODER ? g->encoder_weight_hh : g->decoder_weight_hh;
         float* gbih = phase == TB2_PHASE_ENCODER ? g->encoder_bias_ih : g->decoder_bias_ih;
         float* gbhh = phase == TB2_PHASE_ENCODER ? g->encoder_bias_hh : g->decoder_bias_hh;
-        if ((rc = gemm_tn(DG, 512, X, K, gWih, EP, rows, 512, EP, b.scratch, b.scratch_floats, st))) return rc;
-        if ((rc = gemm_tn(DG, 512, X + EP, K, gWhh, 128, rows, 512, 128, b.scratch, b.scratch_floats, st))) return rc;
-        if ((rc = colsum(DG, 512, rows, 512, gbih, gbhh, b.scratch, b.scratch_floats, st))) return rc;
+        if ((rc = gemm_tn(DG, G4, X, K, gWih, EP, rows, G4, EP, b.scratch, b.scratch_floats, st))) return rc;
+        if ((rc = gemm_tn(DG, G4, X + EP, K, gWhh, H, rows, G4, H, b.scratch, b.scratch_floats, st))) return rc;
+        if ((rc = colsum(DG, G4, rows, G4, gbih, gbhh, b.scratch, b.scratch_floats, st))) return rc;
     }
-    if ((rc = gemm_tn(b.DN, 8, b.HS, 128, g->hidden2normal_weight, 128, S * Mi, 5, 128, b.scratch, b.scratch_floats, st)))
+    if ((rc = gemm_tn(b.DN, 8, b.HS, H, g->hidden2normal_weight, H, S * Mi, 5, H, b.scratch, b.scratch_floats, st)))
         return rc;
     if ((rc = colsum(b.DN, 8, S * Mi, 5, g->hidden2normal_bias, nullptr, b.scratch, b.scratch_floats, st))) return rc;
     bwd_embed_kernel<<<E - 2, 256, 0, st>>>(b.X, K, b.DXIN, EP, b.VEL, S * Mi, g->input_embedding_weight,
@@ -1629,8 +1651,8 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
     TB2_LAUNCH_CHECK();
     // lat_j = W_enc h_j + b_enc (gridbased_pooling.py:160-167): h of step s-1 is states[s-1]
     for (int s = 1; s < S; ++s) {
-        const float* h_prev = states + ((size_t)(s - 1) * 2 + 0) * M * kBH;
-        if ((rc = gemm_tn(b.DLAT + (size_t)s * M * C, C, h_prev, 128, g->pool_encoding_weight, 128, Mi, C, 128,
+        const float* h_prev = states + ((size_t)(s - 1) * 2 + 0) * M * H;
+        if ((rc = gemm_tn(b.DLAT + (size_t)s * M * C, C, h_prev, H, g->pool_encoding_weight, H, Mi, C, H,
                           b.scratch, b.scratch_floats, st)))
             return rc;
     }
@@ -1688,7 +1710,6 @@ static int sequence_backward_impl(const tb2_lstm* m, const tb2_layout* l, const 
     TB2_REQUIRE(m->weights_set, "tb2_lstm_set_weights has not been called");
     TB2_REQUIRE(observed && positions && states && d_normals && active_rows, "null argument");
     TB2_REQUIRE(obs_length >= 2 && n_decode >= 0, "need obs_length >= 2 and n_decode >= 0");
-    TB2_REQUIRE(m->H == kBH, "hidden_dim must be 128");
     const bool social = m->cfg.pool_type == TB2_POOL_SOCIAL;
     if (social && (m->n_mlp < 1 || m->n_mlp > 2 || !m->cfg.pool_to_input || m->cfg.constant != 0.f)) {
         set_error("social training backward supports one_layer / two_layer embeddings with constant = 0");
@@ -1714,11 +1735,11 @@ static int sequence_backward_impl(const tb2_lstm* m, const tb2_layout* l, const 
         return social_backward(m, l, w, observed, obs_length, truth, n_decode, positions, states, d_normals, g, ws,
                                bwd_workspace, st, cache ? &tc : nullptr);
     }
-    const int R = num_active, K = m->K_gate, E = m->E, P = m->P, EP = E + P;
+    const int R = num_active, K = m->K_gate, E = m->E, P = m->P, EP = E + P, H = m->H, G4 = 4 * H;
     const size_t M = (size_t)l->M;
     BwdBuffers b;
     carve_bwd(m, (size_t)R, (size_t)S, bwd_workspace, &b);
-    TB2_CHECK_CUDA(cudaMemsetAsync(b.dc, 0, (size_t)R * 128 * sizeof(float), st));
+    TB2_CHECK_CUDA(cudaMemsetAsync(b.dc, 0, (size_t)R * H * sizeof(float), st));
     const int nm1 = l->n_max > 1 ? l->n_max - 1 : 1;
     const bool pooled = m->cfg.pool_type != TB2_POOL_NONE;
     const size_t CG = (size_t)m->C * (size_t)m->cells;
@@ -1729,7 +1750,7 @@ static int sequence_backward_impl(const tb2_lstm* m, const tb2_layout* l, const 
         const float *o1, *o2;
         int phase;
         if ((rc = resolve_step_inputs(l, observed, obs_length, truth, positions, s, &ws, &o1, &o2, &phase, st))) return rc;
-        const float* h_prev = s > 0 ? states + ((size_t)(s - 1) * 2 + 0) * M * kBH : nullptr;
+        const float* h_prev = s > 0 ? states + ((size_t)(s - 1) * 2 + 0) * M * H : nullptr;
         if (pooled && (rc = launch_pool_prepare(m, l, h_prev, o1, o2, 1, 0, 0, &ws, st))) return rc;   // winners
         {
             KernelTimer kt("bwd_gather", st);
@@ -1737,7 +1758,7 @@ static int sequence_backward_impl(const tb2_lstm* m, const tb2_layout* l, const 
                                                  h_prev, ws.win_count, ws.win_ent, ws.win_val, m->Wt1, m->base1,
                                                  nm1, m->C, m->cells, nullptr, b.X + (size_t)s * R * K,
                                                  pooled ? b.G + (size_t)s * R * CG : nullptr,
-                                                 b.VEL + (size_t)s * R * 2, b.masked + (size_t)s * R, E, P, K);
+                                                 b.VEL + (size_t)s * R * 2, b.masked + (size_t)s * R, E, P, K, H);
         }
         TB2_LAUNCH_CHECK();
     }
@@ -1746,33 +1767,33 @@ static int sequence_backward_impl(const tb2_lstm* m, const tb2_layout* l, const 
         const int s0 = phase == TB2_PHASE_ENCODER ? 0 : S_enc;
         const int ns = phase == TB2_PHASE_ENCODER ? S_enc : S - S_enc;
         if (ns <= 0) continue;
-        if ((rc = gemm_nn(b.X + (size_t)s0 * R * K, K, m->WgT[phase], 512, b.GP + (size_t)s0 * R * 512, 512, ns * R,
-                          512, K, m->bg[phase], st)))
+        if ((rc = gemm_nn(b.X + (size_t)s0 * R * K, K, m->WgT[phase], G4, b.GP + (size_t)s0 * R * G4, G4, ns * R,
+                          G4, K, m->bg[phase], st)))
             return rc;
     }
     // (C) the sequential chain: one kernel per step
     int cur = 0;
     for (int s = S - 1; s >= 0; --s, cur ^= 1) {
-        const float* c_prev = s > 0 ? states + ((size_t)(s - 1) * 2 + 1) * M * kBH : nullptr;
+        const float* c_prev = s > 0 ? states + ((size_t)(s - 1) * 2 + 1) * M * H : nullptr;
         const bool last = s == S - 1;
         const int next_phase = (s + 1) < S_enc ? TB2_PHASE_ENCODER : TB2_PHASE_DECODER;
         const float* Whh_next = next_phase == TB2_PHASE_ENCODER ? w->encoder_weight_hh : w->decoder_weight_hh;
         {
             KernelTimer kt("bwd_cell_head", st);
-            bwd_cell_head_kernel<<<R, 4 * kBH, 0, st>>>(
-                active_rows, b.masked + (size_t)s * R, b.GP + (size_t)s * R * 512, c_prev,
-                last ? nullptr : b.DG + (size_t)(s + 1) * R * 512, Whh_next, nullptr, b.pass[cur ^ 1], b.pass[cur], b.dc,
-                d_normals + (size_t)s * M * 5, m->Wn, m->bn, b.DG + (size_t)s * R * 512,
-                b.HS + (size_t)s * R * 128, b.DN + (size_t)s * R * 8, R);
+            rc = launch_cell_head(H, R, st,
+                active_rows, b.masked + (size_t)s * R, b.GP + (size_t)s * R * G4, c_prev,
+                last ? nullptr : b.DG + (size_t)(s + 1) * R * G4, Whh_next, nullptr, b.pass[cur ^ 1], b.pass[cur], b.dc,
+                d_normals + (size_t)s * M * 5, m->Wn, m->bn, b.DG + (size_t)s * R * G4,
+                b.HS + (size_t)s * R * H, b.DN + (size_t)s * R * 8, R);
         }
-        TB2_LAUNCH_CHECK();
+        if (rc) return rc;
     }
     // (D) + (E) input gradients of all steps and the parameter gradients: one reduction per tensor
     for (int phase = 0; phase < 2; ++phase) {
         const int s0 = phase == TB2_PHASE_ENCODER ? 0 : S_enc;
         const int ns = phase == TB2_PHASE_ENCODER ? S_enc : S - S_enc;
         if (ns <= 0) continue;
-        const float* DG = b.DG + (size_t)s0 * R * 512;
+        const float* DG = b.DG + (size_t)s0 * R * G4;
         const float* X = b.X + (size_t)s0 * R * K;
         const int rows = ns * R;
         float* gWih = phase == TB2_PHASE_ENCODER ? g->encoder_weight_ih : g->decoder_weight_ih;
@@ -1781,12 +1802,12 @@ static int sequence_backward_impl(const tb2_lstm* m, const tb2_layout* l, const 
         float* gbhh = phase == TB2_PHASE_ENCODER ? g->encoder_bias_hh : g->decoder_bias_hh;
         const float* Wih = phase == TB2_PHASE_ENCODER ? w->encoder_weight_ih : w->decoder_weight_ih;
         // dX_in = dgates . W_ih   (torch layout [4H, E+P] is the [K = 4H, N = E+P] operand as it stands)
-        if ((rc = gemm_nn(DG, 512, Wih, EP, b.DXIN + (size_t)s0 * R * EP, EP, rows, EP, 512, nullptr, st))) return rc;
-        if ((rc = gemm_tn(DG, 512, X, K, gWih, EP, rows, 512, EP, b.scratch, b.scratch_floats, st))) return rc;
-        if ((rc = gemm_tn(DG, 512, X + EP, K, gWhh, 128, rows, 512, 128, b.scratch, b.scratch_floats, st))) return rc;
-        if ((rc = colsum(DG, 512, rows, 512, gbih, gbhh, b.scratch, b.scratch_floats, st))) return rc;
+        if ((rc = gemm_nn(DG, G4, Wih, EP, b.DXIN + (size_t)s0 * R * EP, EP, rows, EP, G4, nullptr, st))) return rc;
+        if ((rc = gemm_tn(DG, G4, X, K, gWih, EP, rows, G4, EP, b.scratch, b.scratch_floats, st))) return rc;
+        if ((rc = gemm_tn(DG, G4, X + EP, K, gWhh, H, rows, G4, H, b.scratch, b.scratch_floats, st))) return rc;
+        if ((rc = colsum(DG, G4, rows, G4, gbih, gbhh, b.scratch, b.scratch_floats, st))) return rc;
     }
-    if ((rc = gemm_tn(b.DN, 8, b.HS, 128, g->hidden2normal_weight, 128, S * R, 5, 128, b.scratch, b.scratch_floats, st)))
+    if ((rc = gemm_tn(b.DN, 8, b.HS, H, g->hidden2normal_weight, H, S * R, 5, H, b.scratch, b.scratch_floats, st)))
         return rc;
     if ((rc = colsum(b.DN, 8, S * R, 5, g->hidden2normal_bias, nullptr, b.scratch, b.scratch_floats, st))) return rc;
     bwd_embed_kernel<<<E - 2, 256, 0, st>>>(b.X, K, b.DXIN, EP, b.VEL, S * R, g->input_embedding_weight,

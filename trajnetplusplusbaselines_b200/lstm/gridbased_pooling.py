@@ -131,7 +131,7 @@ class GridBasedPooling(torch.nn.Module):
                 raise RuntimeError("GridBasedPooling runs on CUDA only: move the module (or inputs) to the GPU")
         if self._handle is None or self._handle.device != device:
             cfg = _lib.LstmConfig()
-            cfg.hidden_dim = 128            # the stand-alone plug does not touch the LSTM cell
+            cfg.hidden_dim = self._plug_width()
             cfg.embedding_dim = 64
             cfg.pool_to_input = 1
             self.fill_config(cfg)
@@ -151,18 +151,23 @@ class GridBasedPooling(torch.nn.Module):
         out = self._handle.pool_forward(layout, hid, o1, o2, width)
         return out.to(obs1.device) if obs1.device != device else out
 
+    def _plug_width(self):
+        # social pooling reads the hidden states; the other grids leave the handle's LSTM width unused
+        return int(self.hidden_dim) if self.type_ == 'social' else 128
+
     def _set_plug_weights(self, device):
         # the LSTM-cell slots of the handle are never read by tb2_pool_forward; feed zeros once
         if getattr(self, '_standalone_dummy', None) is None:
             z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=device)
+            H = self._plug_width()
             in_dim = 64 + (self.out_dim if self.embedding is not None else self.n * self.n * self.pooling_dim)
             self._standalone_dummy = dict(
                 input_embedding_weight=z(62, 2), input_embedding_bias=z(62),
-                encoder_weight_ih=z(512, in_dim), encoder_weight_hh=z(512, 128),
-                encoder_bias_ih=z(512), encoder_bias_hh=z(512),
-                decoder_weight_ih=z(512, in_dim), decoder_weight_hh=z(512, 128),
-                decoder_bias_ih=z(512), decoder_bias_hh=z(512),
-                hidden2normal_weight=z(5, 128), hidden2normal_bias=z(5))
+                encoder_weight_ih=z(4 * H, in_dim), encoder_weight_hh=z(4 * H, H),
+                encoder_bias_ih=z(4 * H), encoder_bias_hh=z(4 * H),
+                decoder_weight_ih=z(4 * H, in_dim), decoder_weight_hh=z(4 * H, H),
+                decoder_bias_ih=z(4 * H), decoder_bias_hh=z(4 * H),
+                hidden2normal_weight=z(5, H), hidden2normal_bias=z(5))
         fields = dict(self._standalone_dummy)
         fields.update(self.weight_fields())
         self._handle.set_weights(fields, key=self.weights_version())

@@ -29,11 +29,15 @@ from ..engine import LayoutCache, ModelHandle, plug_getstate, weights_key
 
 class _StandalonePlug:
     """Shared stand-alone path of the non-grid plugs: a model handle whose LSTM-cell slots hold zeros."""
+    _reads_hidden = False           # True: the handle's LSTM width is the width of the hidden states the plug reads
+
+    def _plug_width(self):
+        return int(self.hidden_dim) if self._reads_hidden else 128
 
     def _plug_handle(self, device):
         if self._handle is None or self._handle.device != device:
             cfg = _lib.LstmConfig()
-            cfg.hidden_dim = 128            # the stand-alone plug does not touch the LSTM cell
+            cfg.hidden_dim = self._plug_width()
             cfg.embedding_dim = 64
             cfg.pool_to_input = 1
             self.fill_config(cfg)
@@ -41,14 +45,15 @@ class _StandalonePlug:
             self._standalone_dummy = None
         if getattr(self, '_standalone_dummy', None) is None:
             z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=device)
+            H = self._plug_width()
             in_dim = 64 + self.out_dim
             self._standalone_dummy = dict(
                 input_embedding_weight=z(62, 2), input_embedding_bias=z(62),
-                encoder_weight_ih=z(512, in_dim), encoder_weight_hh=z(512, 128),
-                encoder_bias_ih=z(512), encoder_bias_hh=z(512),
-                decoder_weight_ih=z(512, in_dim), decoder_weight_hh=z(512, 128),
-                decoder_bias_ih=z(512), decoder_bias_hh=z(512),
-                hidden2normal_weight=z(5, 128), hidden2normal_bias=z(5))
+                encoder_weight_ih=z(4 * H, in_dim), encoder_weight_hh=z(4 * H, H),
+                encoder_bias_ih=z(4 * H), encoder_bias_hh=z(4 * H),
+                decoder_weight_ih=z(4 * H, in_dim), decoder_weight_hh=z(4 * H, H),
+                decoder_bias_ih=z(4 * H), decoder_bias_hh=z(4 * H),
+                hidden2normal_weight=z(5, H), hidden2normal_bias=z(5))
         fields = dict(self._standalone_dummy)
         fields.update(self.weight_fields())
         self._handle.set_weights(fields, key=self.weights_version())
@@ -56,6 +61,8 @@ class _StandalonePlug:
 
 
 class HiddenStateMLPPooling(torch.nn.Module, _StandalonePlug):
+    _reads_hidden = True
+
     def __init__(self, hidden_dim=128, mlp_dim=128, mlp_dim_spatial=32, mlp_dim_vel=32, out_dim=None):
         """Same arguments and sub-module names as the reference (non_gridbased_pooling.py:166-193)."""
         super().__init__()
@@ -175,6 +182,8 @@ class NearestNeighborMLP(torch.nn.Module, _StandalonePlug):
 
 
 class AttentionMLPPooling(torch.nn.Module, _StandalonePlug):
+    _reads_hidden = True
+
     def __init__(self, hidden_dim=128, mlp_dim=128, mlp_dim_spatial=32, mlp_dim_vel=32, out_dim=None, fill_value=-10):
         """Same arguments, sub-module names and parameters as the reference (non_gridbased_pooling.py:257-292)."""
         super().__init__()

@@ -220,13 +220,13 @@ def draw_epoch_plan(order, kept, batch_size, n_frames, obs_length=9, augment=Fal
 def check_trainable(model):
     """Raise, with the message the training path itself would raise, for a model whose training backward is not built:
     goal_flag, the non-grid interaction modules, grid embeddings other than one_layer (two_layer too for social),
-    constant != 0, pool widths above 1024, hidden_dim != 128."""
+    constant != 0, pool widths above 1024, hidden_dim outside {32, 64, ..., 256}."""
     from .training import _grad_targets
     if model.goal_flag:
         raise NotImplementedError(GOALS_MESSAGE)
     _grad_targets(model)                          # NotImplementedError for the non-grid modules
-    if model.hidden_dim != 128:
-        raise RuntimeError("invalid argument: hidden_dim must be 128")
+    if model.hidden_dim not in _lib.HIDDEN_DIMS:
+        raise RuntimeError(_lib.HIDDEN_DIM_MESSAGE)
     pool = model.pool
     if pool is None:
         return
