@@ -1,6 +1,8 @@
 """The social grid's first Linear (sparse_layer1_mma) at the benchmark's shape: time, weight stream, occupancy.
 
-    python scripts/layer1_bench.py [--scenes 256] [--forwards 5]
+    python scripts/layer1_bench.py [--scenes 256] [--forwards 5] [--lib OTHER.so] [--time-only]
+
+--lib times another build of the library (same C ABI) instead of the package's; --time-only skips the wavefront models.
 
 Runs the Social-LSTM inference of bench.py (same seeded weights and scenes, an L2 flush between forwards) and times
 every sparse_layer1_mma launch with CUDA events (tb2_profile_*).  Beside the time it prints what the launch moves and
@@ -12,11 +14,17 @@ does, computed from the shapes:
   * MMA tiles per CTA: 16-row mma.sync tiles of one scene group summed over the cells, from the winners of the
     observed frames 0, 8 and 20 (the model's own predictions replace them later in the forward), and the real and
     padded row slots of those tiles;
-  * a model (not a measurement) of the shared-memory wavefronts of one CTA's tile loop, from the same winners, for
-    the tile layout before the flat tile list (padding rows load the zero latent row and read-modify-write dummy
-    accumulator rows; 32-bit A loads from separate hi / lo rows) and for the current one (padding rows touch no
-    accumulator; one 128-bit (hi, lo) A load per row): per warp access, the larger of the distinct 4-byte words over
-    32 and the most distinct words in one bank, times 16 warps;
+  * a model (not a measurement) of the shared-memory wavefronts of one CTA's tile loop, from the same winners.  A warp
+    access costs, per group of lanes the hardware serves together, the larger of the distinct 4-byte words over 32 and
+    the most distinct words in one bank; times 16 warps.  "before_tile_list" and "tile_list" take all 32 lanes as one
+    group (the tile layout before the flat tile list: padding rows load the zero latent row and read-modify-write
+    dummy accumulator rows, 32-bit A loads from separate hi / lo rows; and the flat tile list: padding rows touch no
+    accumulator, one 128-bit (hi, lo) A load per row, two 32-bit slot words, two 64-bit loads and stores per
+    accumulator row at a 264-float stride).  "phased" serves a 64-bit access a half-warp (tile rows 4h .. 4h + 3) and
+    a 128-bit access a quarter-warp (rows 2q, 2q + 1) at a time, which is where two accumulator rows of a tile collide:
+    "tile_list_64bit_stride264" is the flat tile list again, "packed_128bit_stride<S>" the current layout (one slot
+    word, one 128-bit load and store per accumulator row, the warp's 16 columns of a row contiguous) at row strides of
+    264, 272 (the kernel's) and 280 floats;
   * CTAs per SM (cudaOccupancyMaxActiveBlocksPerMultiprocessor), hence the number of waves.
 Prints one JSON line with the GPU's name and power limit.
 """
@@ -128,16 +136,64 @@ def wavefronts_per_cta(xy_frames, bs, cfg):
     return tuple(float(v) * 16 / n for v in tot)
 
 
+ACC_STRIDES = (264, 272, 280)
+
+
+def phased_wavefronts_per_cta(xy_frames, bs, cfg):
+    """Modelled shared-memory wavefronts of one CTA's tile loop with 64-bit accesses served per half-warp and 128-bit
+    accesses per quarter-warp (see the module docstring): {layout: wavefronts}."""
+    cap, cells = GROUP_CAP, cfg.n * cfg.n
+    rows_per_group = GROUP_CAP // PEDS * PEDS
+    names = ["tile_list_64bit_stride264"] + ["packed_128bit_stride%d" % s for s in ACC_STRIDES]
+    tot = np.zeros(len(names))
+    n = 0
+    for xy in xy_frames:
+        win, writer = winners_per_cell(xy, bs, cfg, with_writer=True)
+        lat_row = writer + (np.arange(len(win)) // PEDS * PEDS % rows_per_group)[:, None]
+        for grp in range(len(win) // rows_per_group):
+            sl = slice(grp * rows_per_group, (grp + 1) * rows_per_group)
+            w, lr = win[sl], lat_row[sl]
+            for cell in range(cells):
+                rows = np.nonzero(w[:, cell])[0]
+                for e0 in range(0, len(rows), 16):
+                    slot = [(int(r), int(lr[r, cell])) for r in rows[e0:e0 + 16]]
+                    slot += [None] * (16 - len(slot))
+                    a = 0
+                    acc = np.zeros(len(names))
+                    for half in (0, 1):
+                        s8 = slot[8 * half:8 * half + 8]
+                        lat = [cap + 1 if e is None else e[1] for e in s8]
+                        for q in range(4):                      # 128-bit A loads: two rows per quarter-warp
+                            a += _wavefronts([16 * l + 4 * t + c for l in lat[2 * q:2 * q + 2]
+                                              for t in range(4) for c in range(4)])
+                        for h in (0, 1):                        # 64-bit: rows 4h .. 4h + 3, both n-tiles, load + store
+                            r4 = [e[0] for e in s8[4 * h:4 * h + 4] if e is not None]
+                            acc[0] += 2 * 2 * _wavefronts([r * 264 + 2 * t + c for r in r4
+                                                           for t in range(4) for c in (0, 1)])
+                        for i, stride in enumerate(ACC_STRIDES):
+                            for q in range(4):                  # 128-bit: rows 2q, 2q + 1, load + store
+                                r2 = [e[0] for e in s8[2 * q:2 * q + 2] if e is not None]
+                                acc[1 + i] += 2 * _wavefronts([r * stride + 4 * t + c for r in r2
+                                                               for t in range(4) for c in range(4)])
+                    tot += a + acc + np.array([2] + [1] * len(ACC_STRIDES))      # slot words
+            n += 1
+    return {k: float(v) * 16 / n for k, v in zip(names, tot)}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--scenes", type=int, default=256)
     ap.add_argument("--forwards", type=int, default=5)
+    ap.add_argument("--lib", help="time this build of the library instead of the package's")
+    ap.add_argument("--time-only", action="store_true", help="skip the shared-memory wavefront models")
     args = ap.parse_args()
     import torch
     from oracle import lstm_oracle as O
     from trajnetplusplusbaselines_b200 import _lib
     from trajnetplusplusbaselines_b200.lstm import LSTM, GridBasedPooling
     assert torch.cuda.is_available(), "layer1_bench.py needs a CUDA device"
+    if args.lib:
+        _lib.LIB_PATH = os.path.abspath(args.lib)
     lib = _lib.load()
     info = getattr(lib, "_ZN3tb215layer1_mma_infoEiiiPiS0_S0_")      # tb2::layer1_mma_info
     info.restype = ctypes.c_int
@@ -179,17 +235,18 @@ def main():
     ctas = groups * chunks
     sms = torch.cuda.get_device_properties(dev).multi_processor_count
     slots = tile_slots_per_cta(frames, bs, cfg)
-    wf = wavefronts_per_cta(frames, bs, cfg)
+    wf = (None, None) if args.time_only else wavefronts_per_cta(frames, bs, cfg)
+    phased = None if args.time_only else phased_wavefronts_per_cta(frames, bs, cfg)
     gpu = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit", "--format=csv,noheader"],
                          capture_output=True, text=True).stdout.strip()
     print(json.dumps({
-        "gpu": gpu, "scenes": args.scenes, "tracks": M,
+        "gpu": gpu, "lib": _lib.LIB_PATH, "scenes": args.scenes, "tracks": M,
         "sparse_layer1_mma_us": us, "launches": prof["launches"],
         "grid": {"groups": groups, "chunks": chunks, "chunk_cols": chunk.value, "threads": threads.value, "ctas": ctas},
         "l2_weight_bytes_per_call": wbytes, "weight_stream_tb_s": wbytes / (us * 1e-6) / 1e12,
         "mma_tiles_per_cta": tiles,
         "tile_slots_per_cta": {"real": slots[0], "padded": slots[1]},
-        "smem_wavefronts_per_cta_model": {"before_tile_list": wf[0], "tile_list": wf[1]},
+        "smem_wavefronts_per_cta_model": {"before_tile_list": wf[0], "tile_list": wf[1], "phased": phased},
         "ctas_per_sm": per_sm.value, "sms": sms, "waves": math.ceil(ctas / (per_sm.value * sms))}))
 
 

@@ -586,12 +586,24 @@ __global__ void __launch_bounds__(kL1Threads, 1) sparse_layer1_kernel(L1Params p
 //   is software-pipelined one tile ahead: tile k+1's slot words and A fragments (read-only in
 //   the loop) are requested before tile k's mma, and tile k's accumulator loads are issued
 //   before its mma results are needed (see DESIGN §8 for what bounds the kernel).
-//   smem: acc[cap][264] fp32 | lat[cap+2][4 t][hi.x, hi.y, lo.x, lo.y] bf16 pairs | buckets |
+//   An accumulator row keeps a warp's 16 columns in the order [t][n-tile][2], so the four values a lane
+//   holds of a row (columns 2t, 2t+1 of both n-tiles) are one 128-bit word; a slot is 16 bits (latent row, accumulator
+//   row) and one 32-bit word carries rows g and g + 8 of a tile.
+//   smem: acc[cap][272] fp32 | lat[cap+2][4 t][hi.x, hi.y, lo.x, lo.y] bf16 pairs | buckets |
 //         tiles' cells | padded entries | raw winner lists
 //   Weights: Wt_hi / Wt_lo [cell][OUT][16] bf16, k permuted so a lane's B fragment is one 8-byte
 //   load (position 4t..4t+3 = k {2t, 2t+1, 2t+8, 2t+9}).
 // ------------------------------------------------------------------------------------------
-constexpr int kMmaAccStride = kL1Cols + 8;
+// Accumulator row stride in floats.  A 128-bit access is served a quarter-warp (rows g = 2q, 2q + 1 of a tile) at a
+// time and a row's 16 floats span 16 banks starting at 16 (row + warp) mod 32: two rows collide only when they agree
+// mod 2 (scripts/layer1_bench.py models the strides).
+constexpr int kMmaAccStride = kL1Cols + 16;
+
+// TB2_L1_ABLATE (scripts/layer1_ablate.py, timing only, results wrong): 1 = accumulators summed in registers instead of
+// shared memory, 2 = every tile reads cell 0's weights, 3 = no mma.  Unset in the library.
+#ifndef TB2_L1_ABLATE
+#define TB2_L1_ABLATE 0
+#endif
 
 __device__ __forceinline__ int kperm16(int k) { return 4 * ((k & 7) >> 1) + 2 * (k >> 3) + (k & 1); }
 
@@ -614,10 +626,14 @@ struct L1MmaParams {
 
 constexpr int kMmaThreads = 512;          // 16 warps x 16 output columns
 constexpr int kMmaDepth = 8;              // tiles of B fragments a lane has requested ahead of use
+constexpr int kMmaMaxCap = 254;           // 8-bit slot fields: latent rows [0, cap + 1], accumulator rows [0, cap), 0xff = none
 
 // Tiles a scene group can need: every cell's run of pairs is rounded up to 16 rows, and the pairs of a group number at
 // most cap * nm1, so the padded list holds at most cap * nm1 + 15 * cells slots.
 __host__ __device__ inline size_t l1_mma_max_tiles(int cap, int cells, int nm1) { return ((size_t)cap * nm1 + (size_t)15 * cells) / 16; }
+
+// 16-bit slots of the whole tile list, the look-ahead tiles included
+__host__ __device__ inline size_t l1_mma_slots(size_t max_tiles) { return 16 * max_tiles + 16 * kMmaDepth; }
 
 __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1MmaParams p) {
     extern __shared__ __align__(16) unsigned char smem_l1m[];
@@ -631,13 +647,14 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
 
     // lat rows [0, cap) real, cap = NaN-padded slot (b_enc), cap + 1 = zeros (padding slots); a row is 4 x 16 bytes,
     // lane t's (hi, lo) fragments of k {2t, 2t+1, 2t+8, 2t+9} together, the order of the weight image
-    float* acc = reinterpret_cast<float*>(smem_l1m);                                       // [cap][264]
+    float* acc = reinterpret_cast<float*>(smem_l1m);                                       // [cap][272]
     __nv_bfloat16* lat = reinterpret_cast<__nv_bfloat16*>(acc + (size_t)p.cap * kMmaAccStride);   // [cap+2][32]
     int* start = reinterpret_cast<int*>(lat + (size_t)(p.cap + 2) * 32);                   // [cells+1] padded slot offsets
     int* cursor = start + p.cells + 1;                                                     // [cells]
     uint16_t* tcell = reinterpret_cast<uint16_t*>(cursor + p.cells);                       // [max_tiles] cell of each tile
-    uint32_t* ent = reinterpret_cast<uint32_t*>(tcell + ((max_tiles + 1) & ~(size_t)1));  // [16 (max_tiles + kMmaDepth)]: lat row << 16 | acc row
-    uint32_t* raw = ent + 16 * max_tiles + 16 * kMmaDepth;                                 // [cap*nm1] winner lists as written by pool_prepare
+    // slot = lat row << 8 | acc row; row i of tile k sits at 16 k + 2 (i & 7) + (i >> 3), so word 8 k + g is rows g, g + 8
+    uint16_t* ent = tcell + ((max_tiles + 1) & ~(size_t)1);                                // [16 (max_tiles + kMmaDepth)]
+    uint32_t* raw = reinterpret_cast<uint32_t*>(ent + l1_mma_slots(max_tiles));            // [cap*nm1] winner lists as written by pool_prepare
     int* cnt_s = reinterpret_cast<int*>(raw + (size_t)p.cap * p.nm1);                      // [cap] winners per row
     int* sbase = cnt_s + p.cap;                                                            // [cap] first group-local row of the row's scene
 
@@ -647,9 +664,23 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
         const int a = p.scene_off[sb] - row0, b = p.scene_off[sb + 1] - row0;
         for (int r = a + lane; r < b; r += 32) sbase[r] = a;
     }
-    for (int idx = tid; idx < P * kL1Cols; idx += kMmaThreads) {
-        const int r = idx / kL1Cols, c = idx % kL1Cols;
-        acc[r * kMmaAccStride + c] = chunk0 + c < p.OUT ? p.base[chunk0 + c] : 0.f;
+    {
+        // every slot starts as padding (zero lat row, no accumulator row); the bucketing pass overwrites the real ones
+        const uint32_t pad = ((uint32_t)(p.cap + 1) << 8) | 0xffu;
+        uint32_t* ent2 = reinterpret_cast<uint32_t*>(ent);
+        for (int idx = tid; idx < (int)(l1_mma_slots(max_tiles) / 2); idx += kMmaThreads) ent2[idx] = pad | (pad << 16);
+    }
+    // this thread's 128-bit word of every accumulator row: warp ew's lane-t word, columns {2 et, 2 et + 1} of both n-tiles
+    const int ew = (tid >> 2) & 15, et = tid & 3;
+    const int ecol = chunk0 + ew * 16 + 2 * et;
+    {
+        float4 b4;
+        b4.x = ecol < p.OUT ? p.base[ecol] : 0.f;
+        b4.y = ecol + 1 < p.OUT ? p.base[ecol + 1] : 0.f;
+        b4.z = ecol + 8 < p.OUT ? p.base[ecol + 8] : 0.f;
+        b4.w = ecol + 9 < p.OUT ? p.base[ecol + 9] : 0.f;
+        for (int r = tid >> 6; r < P; r += kMmaThreads / 64)
+            *reinterpret_cast<float4*>(acc + r * kMmaAccStride + ew * 16 + 4 * et) = b4;
     }
     // win_count / win_ent / lat come from pool_prepare.  The outputs written below are read by the previous step's
     // dense_layer_tc: that kernel has completed once this wait returns, because every kernel between it and this one
@@ -674,7 +705,6 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
         lat[dst + 4] = __float2bfloat16_rn(v - __bfloat162float(h));
     }
     __syncthreads();
-    const uint32_t pad = ((uint32_t)(p.cap + 1) << 16) | 0xffffu;    // padding slot: zero lat row, no accumulator row
     const int total = P * p.nm1;
     for (int idx = tid; idx < total; idx += kMmaThreads) {
         int r = idx / p.nm1, k = idx - r * p.nm1;
@@ -682,8 +712,7 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
     }
     __syncthreads();
     if (tid < 32) {
-        // exclusive scan of the cells' pair counts rounded up to whole tiles; each lane marks the padding slots and
-        // the tiles of its cells
+        // exclusive scan of the cells' pair counts rounded up to whole tiles; each lane marks the tiles of its cells
         int per = (p.cells + 31) / 32;
         int lo = tid * per, hi = min(lo + per, p.cells);
         int sum = 0;
@@ -695,19 +724,15 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
         }
         int run = incl - sum;
         for (int c = lo; c < hi; ++c) {
-            const int cnt = cursor[c], padded = (cnt + 15) & ~15;
+            const int padded = (cursor[c] + 15) & ~15;
             start[c] = run;
             cursor[c] = run;
-            for (int s = run + cnt; s < run + padded; ++s) ent[s] = pad;
             for (int k = run >> 4; k < (run + padded) >> 4; ++k) tcell[k] = (uint16_t)c;
             run += padded;
         }
-        // the list runs on in all-padding tiles to a whole number of kMmaDepth-tile rounds, and one tile beyond
-        // for the loop's look-ahead
-        const int slots = __shfl_sync(0xffffffffu, incl, 31);
-        const int end = 16 * (((slots >> 4) + kMmaDepth - 1) / kMmaDepth * kMmaDepth + 1);
-        for (int s = slots + tid; s < end; s += 32) ent[s] = pad;
-        if (tid == 31) start[p.cells] = slots;
+        // beyond the last cell the list runs on in all-padding tiles: the loop works in rounds of kMmaDepth tiles and
+        // looks one tile ahead
+        if (tid == 31) start[p.cells] = incl;
     }
     __syncthreads();
     for (int idx = tid; idx < total; idx += kMmaThreads) {
@@ -717,7 +742,7 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
             const int pos = atomicAdd(&cursor[e >> 16], 1);
             const int j = (int)(e & 0xffff);
             const uint32_t lrow = (uint32_t)(j == 0xffff ? p.cap : sbase[r] + j);
-            ent[pos] = (lrow << 16) | (uint32_t)r;
+            ent[(pos & ~15) + 2 * (pos & 7) + ((pos >> 3) & 1)] = (uint16_t)((lrow << 8) | (uint32_t)r);
         }
     }
     __syncthreads();
@@ -732,6 +757,9 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
     for (int j = 0; j < 2; ++j) okc[j] = ncol0 + 8 * j < p.OUT;
     struct BFrag { uint2 h[2], l[2]; };
     auto load_b = [&](int cell) -> BFrag {      // this lane's fragments of one cell
+#if TB2_L1_ABLATE == 2
+        cell = 0;
+#endif
         const __nv_bfloat16* w = wh + (uint32_t)cell * cell_stride;
         BFrag f;
 #pragma unroll
@@ -744,73 +772,121 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
         }
         return f;
     };
-    // one tile's slot words and A fragments (rows g and g + 8)
-    struct Tile { uint32_t e0, e1; uint4 a0, a1; };
+    // one tile's slot word (rows g and g + 8) and A fragments
+    struct Tile { uint32_t e; uint4 a0, a1; };
     const uint4* latT = reinterpret_cast<const uint4*>(lat) + t;
+    const uint32_t* ent2 = reinterpret_cast<const uint32_t*>(ent);
     auto fetch = [&](int k) -> Tile {
         Tile f;
-        f.e0 = ent[16 * k + g];
-        f.e1 = ent[16 * k + 8 + g];
-        f.a0 = latT[(f.e0 >> 16) * 4];
-        f.a1 = latT[(f.e1 >> 16) * 4];
+        f.e = ent2[8 * k + g];
+        f.a0 = latT[((f.e >> 8) & 0xffu) * 4];
+        f.a1 = latT[(f.e >> 24) * 4];
         return f;
     };
-    float* accw = acc + warp * 16 + 2 * t;
+    float* accw = acc + warp * 16 + 4 * t;
     // register ring of kMmaDepth fragment sets: the slab of tile k + kMmaDepth is requested right after tile k is
     // consumed (a cell of several tiles requests its slab once per tile)
     BFrag b[kMmaDepth];
 #pragma unroll
     for (int i = 0; i < kMmaDepth; ++i) b[i] = load_b(i < tiles ? tcell[i] : 0);
     Tile cur = fetch(0);
+#if TB2_L1_ABLATE == 1
+    float4 s0a = make_float4(0.f, 0.f, 0.f, 0.f), s1a = s0a;
+#endif
     for (int k0 = 0; k0 < tiles; k0 += kMmaDepth) {
 #pragma unroll
         for (int i = 0; i < kMmaDepth; ++i) {
             const int k = k0 + i;                   // k >= tiles: an all-padding tile
-            const bool v0 = (cur.e0 & 0xffffu) != 0xffffu, v1 = (cur.e1 & 0xffffu) != 0xffffu;
-            float2* q0 = reinterpret_cast<float2*>(accw + (cur.e0 & 0xffffu) * kMmaAccStride);
-            float2* q1 = reinterpret_cast<float2*>(accw + (cur.e1 & 0xffffu) * kMmaAccStride);
-            // Accumulators of tile k, all loaded before any is stored: a row occurs at most once per cell, so rows
-            // g and g + 8 of a tile are different rows, and n-tiles j = 0 (q[0]) and j = 1 (q[4]) are different
-            // columns.  They come after tile k - 1's stores, which may hold the same rows.
-            float2 u00, u01, u10, u11;
-            if (v0) { u00 = q0[0]; u01 = q0[4]; }
-            if (v1) { u10 = q1[0]; u11 = q1[4]; }
+            const uint32_t r0 = cur.e & 0xffu, r1 = (cur.e >> 16) & 0xffu;
+            const bool v0 = r0 != 0xffu, v1 = r1 != 0xffu;
+            float4* q0 = reinterpret_cast<float4*>(accw + r0 * kMmaAccStride);
+            float4* q1 = reinterpret_cast<float4*>(accw + r1 * kMmaAccStride);
+            // Accumulators of tile k, both loaded before either is stored: a row occurs at most once per cell, so rows
+            // g and g + 8 of a tile are different rows.  They come after tile k - 1's stores, which may hold the same
+            // rows.
+            float4 u0, u1;
+#if TB2_L1_ABLATE == 1
+            u0 = s0a; u1 = s1a;
+#else
+            if (v0) u0 = *q0;
+            if (v1) u1 = *q1;
+#endif
             const Tile nxt = fetch(k + 1);
             const uint32_t ah[4] = {cur.a0.x, cur.a1.x, cur.a0.y, cur.a1.y};
             const uint32_t al[4] = {cur.a0.z, cur.a1.z, cur.a0.w, cur.a1.w};
             float d[2][4];
 #pragma unroll
             for (int j = 0; j < 2; ++j) {
+#if TB2_L1_ABLATE == 3
+#pragma unroll
+                for (int x = 0; x < 4; ++x)
+                    d[j][x] = __uint_as_float((ah[x] ^ b[i].h[j].x ^ b[i].l[j].y) + (al[x] ^ b[i].h[j].y ^ b[i].l[j].x));
+#else
                 d[j][0] = d[j][1] = d[j][2] = d[j][3] = 0.f;
                 mma_bf16_16816(d[j], ah, b[i].h[j].x, b[i].h[j].y);
                 mma_bf16_16816(d[j], ah, b[i].l[j].x, b[i].l[j].y);
                 mma_bf16_16816(d[j], al, b[i].h[j].x, b[i].h[j].y);
+#endif
             }
-            if (v0) {
-                q0[0] = make_float2(u00.x + d[0][0], u00.y + d[0][1]);
-                q0[4] = make_float2(u01.x + d[1][0], u01.y + d[1][1]);
-            }
-            if (v1) {
-                q1[0] = make_float2(u10.x + d[0][2], u10.y + d[0][3]);
-                q1[4] = make_float2(u11.x + d[1][2], u11.y + d[1][3]);
-            }
+            u0 = make_float4(u0.x + d[0][0], u0.y + d[0][1], u0.z + d[1][0], u0.w + d[1][1]);
+            u1 = make_float4(u1.x + d[0][2], u1.y + d[0][3], u1.z + d[1][2], u1.w + d[1][3]);
+#if TB2_L1_ABLATE == 1
+            if (v0) s0a = u0;
+            if (v1) s1a = u1;
+#else
+            if (v0) *q0 = u0;
+            if (v1) *q1 = u1;
+#endif
             if (k + kMmaDepth < tiles) b[i] = load_b(tcell[k + kMmaDepth]);
             cur = nxt;
         }
     }
+#if TB2_L1_ABLATE == 1
+    if (P > 0) {
+        *reinterpret_cast<float4*>(accw + (g % P) * kMmaAccStride) = s0a;
+        __syncwarp();
+        *reinterpret_cast<float4*>(accw + ((g + 8) % P) * kMmaAccStride) = s1a;
+    }
+#endif
     __syncthreads();
-    for (int idx = tid; idx < P * kL1Cols; idx += kMmaThreads) {
-        const int r = idx / kL1Cols, col = chunk0 + idx % kL1Cols;
-        if (col >= p.OUT) continue;
-        float v = acc[r * kMmaAccStride + idx % kL1Cols];
-        if (p.relu) v = fmaxf(v, 0.f);
-        const size_t o = (size_t)(row0 + r) * p.OUT + col;
+    // Lanes et and et ^ 1 swap a column pair, so the even lane holds columns [2 et, 2 et + 4) of n-tile 0 and the odd
+    // lane columns [2 et - 2, 2 et + 2) of n-tile 1: four adjacent outputs per thread.
+    const bool odd = et & 1;
+    const int ocol = odd ? ecol + 6 : ecol;
+    const bool vec = (p.OUT & 3) == 0;              // then ocol < OUT covers all four, and the rows stay aligned
+    for (int r = tid >> 6; r < P; r += kMmaThreads / 64) {
+        const float4 a = *reinterpret_cast<const float4*>(acc + r * kMmaAccStride + ew * 16 + 4 * et);
+        const float sx = __shfl_xor_sync(0xffffffffu, odd ? a.x : a.z, 1);
+        const float sy = __shfl_xor_sync(0xffffffffu, odd ? a.y : a.w, 1);
+        float v[4] = {odd ? sx : a.x, odd ? sy : a.y, odd ? a.z : sx, odd ? a.w : sy};
+        if (p.relu) {
+#pragma unroll
+            for (int x = 0; x < 4; ++x) v[x] = fmaxf(v[x], 0.f);
+        }
+        const size_t o = (size_t)(row0 + r) * p.OUT + ocol;
         if (p.out_hi) {
-            const __nv_bfloat16 h = __float2bfloat16_rn(v);
-            p.out_hi[o] = h;
-            p.out_lo[o] = __float2bfloat16_rn(v - __bfloat162float(h));
+            __align__(8) __nv_bfloat16 h[4], l[4];
+#pragma unroll
+            for (int x = 0; x < 4; ++x) {
+                h[x] = __float2bfloat16_rn(v[x]);
+                l[x] = __float2bfloat16_rn(v[x] - __bfloat162float(h[x]));
+            }
+            if (vec) {
+                if (ocol < p.OUT) {
+                    *reinterpret_cast<uint2*>(p.out_hi + o) = *reinterpret_cast<const uint2*>(h);
+                    *reinterpret_cast<uint2*>(p.out_lo + o) = *reinterpret_cast<const uint2*>(l);
+                }
+            } else {
+#pragma unroll
+                for (int x = 0; x < 4; ++x)
+                    if (ocol + x < p.OUT) { p.out_hi[o + x] = h[x]; p.out_lo[o + x] = l[x]; }
+            }
+        } else if (vec) {
+            if (ocol < p.OUT) *reinterpret_cast<float4*>(p.out + o) = make_float4(v[0], v[1], v[2], v[3]);
         } else {
-            p.out[o] = v;
+#pragma unroll
+            for (int x = 0; x < 4; ++x)
+                if (ocol + x < p.OUT) p.out[o + x] = v[x];
         }
     }
 }
@@ -821,7 +897,7 @@ static size_t l1_mma_smem_bytes(int cap, int cells, int nm1) {
     b += (size_t)(cap + 2) * 32 * sizeof(__nv_bfloat16);             // latent rows (hi, lo)
     b += (size_t)(2 * cells + 1) * sizeof(int);                       // cell starts, cursors
     b += ((tiles + 1) & ~(size_t)1) * sizeof(uint16_t);               // cell of each tile
-    b += (16 * tiles + 16 * kMmaDepth) * sizeof(uint32_t);            // padded entries + all-padding tiles
+    b += l1_mma_slots(tiles) * sizeof(uint16_t);                      // padded entries + all-padding tiles
     b += (size_t)cap * nm1 * sizeof(uint32_t);                        // raw winner lists
     b += (size_t)cap * 2 * sizeof(int);                               // winners per row, scene base per row
     return b + 16;
@@ -833,7 +909,7 @@ static DynSmemConfig l1_mma_smem_config;
 // CTAs fit on one SM (scripts/layer1_bench.py reports them).
 int layer1_mma_info(int cap, int cells, int nm1, int* chunk_cols, int* threads, int* ctas_per_sm) {
     const size_t sm = l1_mma_smem_bytes(cap, cells, nm1);
-    TB2_REQUIRE(sm <= 227 * 1024, "scene group does not fit in shared memory (scene too large)");
+    TB2_REQUIRE(sm <= 227 * 1024 && cap <= kMmaMaxCap, "scene group does not fit in shared memory (scene too large)");
     TB2_CHECK_CUDA(l1_mma_smem_config.ensure(sparse_layer1_mma_kernel, sm));
     TB2_CHECK_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(ctas_per_sm, sparse_layer1_mma_kernel, kMmaThreads, sm));
     *chunk_cols = kL1Cols;
@@ -1163,7 +1239,7 @@ int launch_pool_mlp(const tb2_lstm* m, const tb2_layout* l, Workspace* ws, float
         int gm = 0;
         size_t sm = l1_mma_smem_bytes(l->group_cap[gm], m->cells, nm1);
         if (sm > 227 * 1024) { gm = 1; sm = l1_mma_smem_bytes(l->group_cap[gm], m->cells, nm1); }
-        TB2_REQUIRE(sm <= 227 * 1024, "scene group does not fit in shared memory (scene too large)");
+        TB2_REQUIRE(sm <= 227 * 1024 && l->group_cap[gm] <= kMmaMaxCap, "scene group does not fit in shared memory (scene too large)");
         TB2_REQUIRE(m->cells <= 65536 && (size_t)m->cells * d1 * 32 < ((size_t)1 << 32),
                     "grid too fine for the tensor-core first layer (16-bit tile cells, 32-bit weight offsets)");
         L1MmaParams q;
