@@ -8,7 +8,7 @@ Trainer.train_batch step with the tensor cores on and with TB2_DISABLE_TC=1, che
 the GEMM branches the case is meant to cover (timer names from tb2_profile_begin / end), and compares the
 loss and every parameter gradient with the float64 restatement at realistic shapes.
 
-The GEMM branches (gemm_nn / gemm_nt / gemm_tn in train.cu): a product of m * n * k >= 3.2e7 runs on cuBLAS
+The GEMM branches (gemm_nn / gemm_tn in train.cu): a product of m * n * k >= 3.2e7 runs on cuBLAS
 (bwd_gemm_cublas, bwd_gemm_tn_cublas), a smaller one on the FFMA kernels (bwd_gemm, bwd_gemm_tn), which
 load float4 only when the leading dimensions are multiples of 4 and the base pointers 16-byte aligned, and
 split the rows of a weight gradient over CTAs when its output has few tiles.

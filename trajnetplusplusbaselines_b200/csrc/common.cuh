@@ -255,6 +255,9 @@ int launch_pool_lstm_cell(const tb2_lstm* m, const tb2_layout* l, const float* f
                           cudaStream_t st);
 int launch_nn_mlp_pool(const tb2_lstm* m, const tb2_layout* l, const float* obs1, const float* obs2, float* out,
                        cudaStream_t st);
+// C = act(A . B + bias), B [K, N] row-major, on the fp32 FFMA kernel (never cuBLAS); act = ReLU when relu != 0
+int launch_gemm_ffma(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int M, int N, int K,
+                     const float* bias, int relu, const char* name, cudaStream_t st);
 bool dense_tc_supported(int K, int N);
 int launch_dense_tc(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo, const float* bias,
                     float* Y, void* Y_hi, void* Y_lo, int M, int K, int N, int relu, cudaStream_t st);

@@ -954,89 +954,6 @@ static size_t l1_smem_bytes(int cap, int C, bool social, int cells, int nm1) {
 }
 
 // ------------------------------------------------------------------------------------------
-// dense_layer: Y = act(X . W^T + b), X [M, K], WT [K, N] (transposed at repack).  fp32 FFMA,
-// 64 x 64 x 16 tiles, 4 x 4 micro-tiles.  (Layers >= 2 of the grid embedding.)
-// ------------------------------------------------------------------------------------------
-constexpr int kDT = 64, kDK = 16;
-
-__global__ void __launch_bounds__(256) dense_layer_kernel(const float* __restrict__ X,
-                                                          const float* __restrict__ WT,
-                                                          const float* __restrict__ bias,
-                                                          float* __restrict__ Y, int M, int K, int N,
-                                                          int relu) {
-    __shared__ float As[kDK][kDT + 4];
-    __shared__ float Bs[kDK][kDT];
-    const int tid = threadIdx.x;
-    const int tx = tid & 15, ty = tid >> 4;
-    const int m0 = blockIdx.y * kDT, n0 = blockIdx.x * kDT;
-    float acc[4][4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-    for (int k0 = 0; k0 < K; k0 += kDK) {
-        // A tile: 64 rows x 16 k  (thread loads 4 consecutive k of one row)
-        {
-            int r = tid >> 2, kq = (tid & 3) * 4;
-            int m = m0 + r;
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-                int k = k0 + kq + q;
-                As[kq + q][r] = (m < M && k < K) ? X[(size_t)m * K + k] : 0.f;
-            }
-        }
-        // B tile: 16 k x 64 cols
-        {
-            int kk = tid >> 4, cq = (tid & 15) * 4;
-            int k = k0 + kk;
-#pragma unroll
-            for (int q = 0; q < 4; ++q) {
-                int n = n0 + cq + q;
-                Bs[kk][cq + q] = (k < K && n < N) ? WT[(size_t)k * N + n] : 0.f;
-            }
-        }
-        __syncthreads();
-#pragma unroll
-        for (int kk = 0; kk < kDK; ++kk) {
-            float a[4], bb[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) a[i] = As[kk][ty * 4 + i];
-#pragma unroll
-            for (int j = 0; j < 4; ++j) bb[j] = Bs[kk][tx * 4 + j];
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-#pragma unroll
-                for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], bb[j], acc[i][j]);
-        }
-        __syncthreads();
-    }
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        int m = m0 + ty * 4 + i;
-        if (m >= M) continue;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            int n = n0 + tx * 4 + j;
-            if (n >= N) continue;
-            float v = acc[i][j] + bias[n];
-            if (relu) v = fmaxf(v, 0.f);
-            Y[(size_t)m * N + n] = v;
-        }
-    }
-}
-
-static int launch_dense(const float* X, const float* WT, const float* b, float* Y, int M, int K, int N,
-                        int relu, cudaStream_t st) {
-    dim3 grid((N + kDT - 1) / kDT, (M + kDT - 1) / kDT);
-    {
-        KernelTimer kt("dense_layer", st);
-        dense_layer_kernel<<<grid, 256, 0, st>>>(X, WT, b, Y, M, K, N, relu);
-    }
-    TB2_LAUNCH_CHECK();
-    return TB2_OK;
-}
-
-// ------------------------------------------------------------------------------------------
 // First Linear for occupancy / directional grids (C <= 2 payload channels): the whole weight
 // chunk [cells * C][CH output columns] fits in shared memory, so a CTA loads it once and then
 // walks its rows; each row is base + sum over its <= N-1 winners of C weight rows (a few dozen
@@ -1282,8 +1199,10 @@ int launch_pool_mlp(const tb2_lstm* m, const tb2_layout* l, Workspace* ws, float
                                  (last && direct_split) ? pooled_out : y,
                                  (last && direct_split) ? pool_hi : nullptr, (last && direct_split) ? pool_lo : nullptr,
                                  l->M, m->mlp_dims[1], m->mlp_dims[2], 1, st);
-        } else
-        rc = launch_dense(x, m->WT[layer], m->bl[layer], y, l->M, m->mlp_dims[layer], m->mlp_dims[layer + 1], 1, st);
+        } else {      // fp32 FFMA: Y = relu(X . W^T + b), W^T [K, N] transposed at repack
+            const int K = m->mlp_dims[layer], N = m->mlp_dims[layer + 1];
+            rc = launch_gemm_ffma(x, K, m->WT[layer], N, y, N, l->M, N, K, m->bl[layer], 1, "dense_layer", st);
+        }
         if (rc != TB2_OK) return rc;
         x = y;
     }

@@ -17,8 +17,11 @@
 //       over all S * R (step, row) records, rows split over CTAs with the partial sums added in a
 //       fixed order.  No floating-point atomics: results are bit-identical from run to run.
 // Social pooling couples the tracks of a scene through lat_j = W_enc h_j: every track receives
-// gradient, so social_backward (further down) runs the same phases on all M rows and adds the
-// backward of the grid MLP and of the hidden-state scatter to the chain.
+// gradient, so social_backward (further down) runs on all M rows, with its own (A) (this step's
+// forward records, from the training cache or recomputed) and its own (C), which adds the
+// backward of the grid MLP and of the hidden-state scatter to the chain.  Both drivers keep the
+// same per-(step, row) records (RowRecords) and share phase (B) (gate_preactivations) and the
+// LSTM / head / input-embedding weight gradients (lstm_weight_grads).
 #include <cublas_v2.h>
 #include <dlfcn.h>
 #include <mutex>
@@ -211,11 +214,13 @@ __global__ void __launch_bounds__(4 * H) bwd_cell_head_kernel(
 }
 
 // ------------------------------------------------------------------------------------------
-// Tiled fp32 GEMMs of the backward (64 x 64 tiles, 32-deep slices, register prefetch of the next
-// slice so one global-load latency is paid per slice instead of per 16 products).
-//   gemm_kernel<BT>:  C[M,N] = A[M,K] . op(B) (+ bias[n]);  op(B) = B[K,N] or (BT) B[N,K]^T
+// Tiled fp32 GEMMs (64 x 64 tiles, 32-deep slices, register prefetch of the next slice so one
+// global-load latency is paid per slice instead of per 16 products).
+//   gemm_kernel    :  C[M,N] = act(A[M,K] . B[K,N] (+ bias[n])), act = ReLU or none; one fmaf chain
+//                     per output in ascending k from +0, bias added last (the backward's row GEMMs
+//                     and the grid MLP's forward layers >= 2, launch_gemm_ffma)
 //   gemm_tn_kernel :  C[n][k] (+)= sum_r A[r][n] * B[r][k]   (weight gradients; one CTA owns a
-//                     tile of C and walks all rows: deterministic)
+//                     tile of C and walks all rows of its slice: deterministic)
 // ------------------------------------------------------------------------------------------
 constexpr int kGT = 64, kGK = 32;
 
@@ -233,11 +238,11 @@ __device__ __forceinline__ float4 ld4(const float* base, size_t row, int ld, int
     return v;
 }
 
-template <bool BT, int TM>
+template <int TM>
 __global__ void __launch_bounds__(TM * 4) gemm_kernel(const float* __restrict__ A, int lda,
                                                       const float* __restrict__ B, int ldb,
                                                       float* __restrict__ Cm, int ldc, int M, int N, int K,
-                                                      const float* __restrict__ bias, int vec) {
+                                                      const float* __restrict__ bias, int relu, int vec) {
     constexpr int NT = TM * 4;                 // threads; each owns a 4 x 4 micro-tile of TM x 64
     constexpr int LA = TM * 8 / NT;            // float4 loads per thread for the A slice (TM x 32) = 2
     constexpr int LB = 64 * 8 / NT;            // ... for the B slice (64 x 32): 2 (TM = 64) or 4 (TM = 32)
@@ -259,14 +264,8 @@ __global__ void __launch_bounds__(TM * 4) gemm_kernel(const float* __restrict__ 
         }
 #pragma unroll
         for (int i = 0; i < LB; ++i) {
-            const int f = tid + i * NT;
-            if (BT) {
-                const int row = f >> 3, kq = (f & 7) * 4;                    // 64 n x 32 k
-                rb[i] = ld4(B, (size_t)(n0 + row), ldb, k0 + kq, N, K, vec);
-            } else {
-                const int kk = f >> 4, nq = (f & 15) * 4;                    // 32 k x 64 n
-                rb[i] = ld4(B, (size_t)(k0 + kk), ldb, n0 + nq, K, N, vec);
-            }
+            const int f = tid + i * NT, kk = f >> 4, nq = (f & 15) * 4;     // 32 k x 64 n
+            rb[i] = ld4(B, (size_t)(k0 + kk), ldb, n0 + nq, K, N, vec);
         }
     };
     auto store = [&]() {
@@ -277,14 +276,8 @@ __global__ void __launch_bounds__(TM * 4) gemm_kernel(const float* __restrict__ 
         }
 #pragma unroll
         for (int i = 0; i < LB; ++i) {
-            const int f = tid + i * NT;
-            if (BT) {
-                const int row = f >> 3, kq = (f & 7) * 4;
-                Bs[kq + 0][row] = rb[i].x; Bs[kq + 1][row] = rb[i].y; Bs[kq + 2][row] = rb[i].z; Bs[kq + 3][row] = rb[i].w;
-            } else {
-                const int kk = f >> 4, nq = (f & 15) * 4;
-                *reinterpret_cast<float4*>(&Bs[kk][nq]) = rb[i];
-            }
+            const int f = tid + i * NT, kk = f >> 4, nq = (f & 15) * 4;
+            *reinterpret_cast<float4*>(&Bs[kk][nq]) = rb[i];
         }
     };
     load(0);
@@ -316,97 +309,25 @@ __global__ void __launch_bounds__(TM * 4) gemm_kernel(const float* __restrict__ 
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const int n = n0 + tx * 4 + j;
-            if (n < N) Cm[(size_t)m * ldc + n] = acc[i][j] + (bias ? bias[n] : 0.f);
+            if (n >= N) continue;
+            float v = acc[i][j] + (bias ? bias[n] : 0.f);
+            if (relu) v = fmaxf(v, 0.f);
+            Cm[(size_t)m * ldc + n] = v;
         }
     }
 }
 
-template <int TN>
+// SPLIT: rows split over gridDim.z, slice z writes its partial tile sums to C + z * N * Kc (dense
+// N x Kc, ldc = Kc) and reduce_partials_kernel adds the slices in a fixed order; otherwise a single
+// slice (rows_per_slice = R) adds its sums to C.
+template <int TN, bool SPLIT>
 __global__ void __launch_bounds__(TN * 4) gemm_tn_kernel(const float* __restrict__ A, int lda,
                                                          const float* __restrict__ B, int ldb,
                                                          float* __restrict__ Cm, int ldc, int R, int N, int Kc,
-                                                         int vec) {
+                                                         int rows_per_slice, int vec) {
     constexpr int NT = TN * 4;
     constexpr int LA = TN * 8 / NT;            // A slice: 32 rows x TN cols
     constexpr int LB = 64 * 8 / NT;            // B slice: 32 rows x 64 cols
-    __shared__ __align__(16) float As[kGK][TN + 4];
-    __shared__ __align__(16) float Bs[kGK][kGT + 4];
-    const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
-    const int n0 = blockIdx.y * TN, k0c = blockIdx.x * kGT;
-    float acc[4][4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-    float4 ra[LA], rb[LB];
-    auto load = [&](int r0) {
-#pragma unroll
-        for (int i = 0; i < LA; ++i) {
-            const int f = tid + i * NT, rr = f / (TN / 4), cq = (f % (TN / 4)) * 4;
-            ra[i] = ld4(A, (size_t)(r0 + rr), lda, n0 + cq, R, N, vec);
-        }
-#pragma unroll
-        for (int i = 0; i < LB; ++i) {
-            const int f = tid + i * NT, rr = f >> 4, cq = (f & 15) * 4;
-            rb[i] = ld4(B, (size_t)(r0 + rr), ldb, k0c + cq, R, Kc, vec);
-        }
-    };
-    auto store = [&]() {
-#pragma unroll
-        for (int i = 0; i < LA; ++i) {
-            const int f = tid + i * NT, rr = f / (TN / 4), cq = (f % (TN / 4)) * 4;
-            *reinterpret_cast<float4*>(&As[rr][cq]) = ra[i];
-        }
-#pragma unroll
-        for (int i = 0; i < LB; ++i) {
-            const int f = tid + i * NT, rr = f >> 4, cq = (f & 15) * 4;
-            *reinterpret_cast<float4*>(&Bs[rr][cq]) = rb[i];
-        }
-    };
-    load(0);
-    store();
-    __syncthreads();
-    for (int r0 = 0; r0 < R; r0 += kGK) {
-        const bool more = r0 + kGK < R;
-        if (more) load(r0 + kGK);
-#pragma unroll
-        for (int rr = 0; rr < kGK; ++rr) {
-            const float4 a = *reinterpret_cast<const float4*>(&As[rr][ty * 4]);
-            const float4 b = *reinterpret_cast<const float4*>(&Bs[rr][tx * 4]);
-            const float av[4] = {a.x, a.y, a.z, a.w}, bv[4] = {b.x, b.y, b.z, b.w};
-#pragma unroll
-            for (int i = 0; i < 4; ++i)
-#pragma unroll
-                for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(av[i], bv[j], acc[i][j]);
-        }
-        __syncthreads();
-        if (more) {
-            store();
-            __syncthreads();
-        }
-    }
-#pragma unroll
-    for (int i = 0; i < 4; ++i) {
-        const int n = n0 + ty * 4 + i;
-        if (n >= N) continue;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-            const int k = k0c + tx * 4 + j;
-            if (k < Kc) Cm[(size_t)n * ldc + k] += acc[i][j];
-        }
-    }
-}
-
-// same product, rows split over gridDim.z: slice z writes its partial tile sums to part[z][n][k]
-// (dense N x Kc); reduce_partials_kernel adds the slices in a fixed order.
-template <int TN>
-__global__ void __launch_bounds__(TN * 4) gemm_tn_split_kernel(const float* __restrict__ A, int lda,
-                                                               const float* __restrict__ B, int ldb,
-                                                               float* __restrict__ part, int R, int N, int Kc,
-                                                               int rows_per_slice, int vec) {
-    constexpr int NT = TN * 4;
-    constexpr int LA = TN * 8 / NT;
-    constexpr int LB = 64 * 8 / NT;
     __shared__ __align__(16) float As[kGK][TN + 4];
     __shared__ __align__(16) float Bs[kGK][kGT + 4];
     const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
@@ -466,7 +387,7 @@ __global__ void __launch_bounds__(TN * 4) gemm_tn_split_kernel(const float* __re
             __syncthreads();
         }
     }
-    float* out = part + (size_t)blockIdx.z * N * Kc;
+    float* out = SPLIT ? Cm + (size_t)blockIdx.z * N * Kc : Cm;
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
         const int n = n0 + ty * 4 + i;
@@ -474,7 +395,9 @@ __global__ void __launch_bounds__(TN * 4) gemm_tn_split_kernel(const float* __re
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
             const int k = k0c + tx * 4 + j;
-            if (k < Kc) out[(size_t)n * Kc + k] = acc[i][j];
+            if (k >= Kc) continue;
+            if (SPLIT) out[(size_t)n * ldc + k] = acc[i][j];
+            else out[(size_t)n * ldc + k] += acc[i][j];
         }
     }
 }
@@ -1099,7 +1022,24 @@ __global__ void fill_bias_rows_kernel(float* __restrict__ C, int ldc, int M, int
     }
 }
 
-// C = A . B (+bias), B [K, N] row-major
+int launch_gemm_ffma(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int M, int N, int K,
+                     const float* bias, int relu, const char* name, cudaStream_t st) {
+    const int vec = (lda % 4 == 0 && ldb % 4 == 0 && aligned16(A) && aligned16(B)) ? 1 : 0;
+    const bool small = (size_t)((M + 63) / 64) * ((N + kGT - 1) / kGT) < 148;     // few tiles: halve them
+    {
+        KernelTimer kt(name, st);
+        if (small)
+            gemm_kernel<32><<<dim3((N + kGT - 1) / kGT, (M + 31) / 32), 128, 0, st>>>(A, lda, B, ldb, C, ldc, M, N, K,
+                                                                                   bias, relu, vec);
+        else
+            gemm_kernel<64><<<dim3((N + kGT - 1) / kGT, (M + 63) / 64), 256, 0, st>>>(A, lda, B, ldb, C, ldc, M, N, K,
+                                                                                   bias, relu, vec);
+    }
+    TB2_LAUNCH_CHECK();
+    return TB2_OK;
+}
+
+// C = A . B (+bias), B [K, N] row-major; large products on cuBLAS
 static int gemm_nn(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int M, int N, int K,
                    const float* bias, cudaStream_t st) {
     {   // row-major C = A . B  <=>  column-major C^T (N x M) = B^T-view (N x K) . A^T-view (K x M)
@@ -1113,39 +1053,7 @@ static int gemm_nn(const float* A, int lda, const float* B, int ldb, float* C, i
                 return TB2_OK;
         }
     }
-    const int vec = (lda % 4 == 0 && ldb % 4 == 0 && aligned16(A) && aligned16(B)) ? 1 : 0;
-    const bool small = (size_t)((M + 63) / 64) * ((N + kGT - 1) / kGT) < 148;     // few tiles: halve them
-    {
-        KernelTimer kt("bwd_gemm", st);
-        if (small)
-            gemm_kernel<false, 32><<<dim3((N + kGT - 1) / kGT, (M + 31) / 32), 128, 0, st>>>(A, lda, B, ldb, C, ldc, M,
-                                                                                         N, K, bias, vec);
-        else
-            gemm_kernel<false, 64><<<dim3((N + kGT - 1) / kGT, (M + 63) / 64), 256, 0, st>>>(A, lda, B, ldb, C, ldc, M,
-                                                                                         N, K, bias, vec);
-    }
-    TB2_LAUNCH_CHECK();
-    return TB2_OK;
-}
-
-// C = A . B^T, B [N, K] row-major
-static int gemm_nt(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int M, int N, int K,
-                   cudaStream_t st) {
-    // row-major C = A . B^T, B [N, K]  <=>  column-major C^T (N x M) = (B-view (K x N))^T . A-view (K x M)
-    if (cublas_gemm(CUBLAS_OP_T, CUBLAS_OP_N, N, M, K, B, ldb, A, lda, 0.f, C, ldc, "bwd_gemm_cublas", st)) return TB2_OK;
-    const int vec = (lda % 4 == 0 && ldb % 4 == 0 && aligned16(A) && aligned16(B)) ? 1 : 0;
-    const bool small = (size_t)((M + 63) / 64) * ((N + kGT - 1) / kGT) < 148;
-    {
-        KernelTimer kt("bwd_gemm", st);
-        if (small)
-            gemm_kernel<true, 32><<<dim3((N + kGT - 1) / kGT, (M + 31) / 32), 128, 0, st>>>(A, lda, B, ldb, C, ldc, M,
-                                                                                        N, K, nullptr, vec);
-        else
-            gemm_kernel<true, 64><<<dim3((N + kGT - 1) / kGT, (M + 63) / 64), 256, 0, st>>>(A, lda, B, ldb, C, ldc, M,
-                                                                                        N, K, nullptr, vec);
-    }
-    TB2_LAUNCH_CHECK();
-    return TB2_OK;
+    return launch_gemm_ffma(A, lda, B, ldb, C, ldc, M, N, K, bias, 0, "bwd_gemm", st);
 }
 
 // C[n][k] += sum_r A[r][n] B[r][k]; rows are split over CTAs when the output has few tiles
@@ -1162,14 +1070,14 @@ static int gemm_tn(const float* A, int lda, const float* B, int ldb, float* C, i
     while (Z > 1 && (size_t)Z * N * Kc > scratch_floats) --Z;
     if (Z <= 1) {
         KernelTimer kt("bwd_gemm_tn", st);
-        gemm_tn_kernel<32><<<dim3((Kc + kGT - 1) / kGT, (N + 31) / 32), 128, 0, st>>>(A, lda, B, ldb, C, ldc, R, N, Kc,
-                                                                                  vec);
+        gemm_tn_kernel<32, false><<<dim3((Kc + kGT - 1) / kGT, (N + 31) / 32), 128, 0, st>>>(A, lda, B, ldb, C, ldc, R, N,
+                                                                                         Kc, R, vec);
     } else {
         int rps = (R + Z - 1) / Z;
         rps = (rps + kGK - 1) / kGK * kGK;
         Z = (R + rps - 1) / rps;
         KernelTimer kt("bwd_gemm_tn", st);
-        gemm_tn_split_kernel<32><<<dim3((Kc + kGT - 1) / kGT, (N + 31) / 32, Z), 128, 0, st>>>(A, lda, B, ldb, scratch,
+        gemm_tn_kernel<32, true><<<dim3((Kc + kGT - 1) / kGT, (N + 31) / 32, Z), 128, 0, st>>>(A, lda, B, ldb, scratch, Kc,
                                                                                            R, N, Kc, rps, vec);
         reduce_partials_kernel<<<(unsigned)(((size_t)N * Kc + 255) / 256), 256, 0, st>>>(scratch, Z, N, Kc, C, ldc,
                                                                                       nullptr);
@@ -1210,49 +1118,59 @@ static int launch_cell_head(int H, int rows, cudaStream_t st, Args... args) {
     return TB2_OK;
 }
 
-// Carving of the backward workspace (floats).  Per (step, row) records are kept so that every
-// weight gradient is one reduction over all S * R rows after the time loop.
-struct BwdBuffers {
-    float *X, *GP, *DG, *HS, *DN, *VEL, *DXIN, *G;     // [S][R][K | G4 | G4 | H | 8 | 2 | E+P | C n n]
-    float *pass[2], *dc;                               // [R][H] chain state
-    float* scratch;                                    // partial sums of the row-split reductions
+// Carving of the backward workspace in floats, every array 16-byte aligned; a null base only counts the bytes
+struct Carve {
+    void* base;
+    size_t off = 0;
+    float* take(size_t n) {
+        float* p = base ? reinterpret_cast<float*>(base) + off : nullptr;
+        off += (n + 3) & ~(size_t)3;
+        return p;
+    }
+    size_t bytes() const { return off * sizeof(float) + 256; }
+};
+
+// Per (step, row) records of both backward drivers (rows = the active rows, or all M tracks with social pooling),
+// kept so that every weight gradient is one reduction over all S * rows records after the time loop.
+struct RowRecords {
+    float *X, *GP, *DG, *HS, *DN, *VEL, *DXIN;     // [S][rows][K | G4 | G4 | H | 8 | 2 | E+P]
+    float *pass[2], *dc;                           // [rows][H] chain state
+    float* scratch;                                // partial sums of the row-split reductions
     size_t scratch_floats;
-    int* masked;                                       // [S][R]
+    int* masked;                                   // [S][rows]
+};
+
+// extra_grad: floats of the largest weight gradient the driver reduces besides the LSTM's own (sizes `scratch`)
+static void carve_records(const tb2_lstm* m, size_t rows, size_t S, size_t extra_grad, Carve& c, RowRecords* o) {
+    const size_t K = (size_t)m->K_gate, EP = (size_t)(m->E + m->P), H = (size_t)m->H, G4 = 4 * H;
+    o->X = c.take(S * rows * K);
+    o->GP = c.take(S * rows * G4);
+    o->DG = c.take(S * rows * G4);
+    o->HS = c.take(S * rows * H);
+    o->DN = c.take(S * rows * 8);
+    o->VEL = c.take(S * rows * 2);
+    o->DXIN = c.take(S * rows * EP);
+    o->pass[0] = c.take(rows * H);
+    o->pass[1] = c.take(rows * H);
+    o->dc = c.take(rows * H);
+    o->scratch_floats = 8 * (extra_grad > G4 * K ? extra_grad : G4 * K);
+    o->scratch = c.take(o->scratch_floats);
+    o->masked = reinterpret_cast<int*>(c.take(S * rows));
+}
+
+struct BwdBuffers : RowRecords {
+    float* G;                                      // [S][R][C n n] grid rows
 };
 
 static size_t carve_bwd(const tb2_lstm* m, size_t R, size_t S, void* base, BwdBuffers* b) {
-    const size_t K = (size_t)m->K_gate, E = (size_t)m->E, P = (size_t)(m->P > 0 ? m->P : 0);
-    const size_t H = (size_t)m->H, G4 = 4 * H;
-    size_t off = 0;
-    auto take = [&](size_t n) {
-        float* p = base ? reinterpret_cast<float*>(base) + off : nullptr;
-        off += (n + 3) & ~(size_t)3;       // keep every array 16-byte aligned
-        return p;
-    };
+    const size_t P = (size_t)m->P, CG = (size_t)m->C * (size_t)m->cells;
     BwdBuffers tmp;
     BwdBuffers* o = b ? b : &tmp;
-    const size_t CG = (size_t)m->C * (size_t)m->cells;
-    o->X = take(S * R * K);
-    o->GP = take(S * R * G4);
-    o->DG = take(S * R * G4);
-    o->HS = take(S * R * H);
-    o->DN = take(S * R * 8);
-    o->VEL = take(S * R * 2);
-    o->DXIN = take(S * R * (E + P));
-    o->G = take(P ? S * R * CG : 4);
-    o->pass[0] = take(R * H);
-    o->pass[1] = take(R * H);
-    o->dc = take(R * H);
-    size_t big = G4 * K;
-    if (P * CG > big) big = P * CG;
-    o->scratch_floats = 8 * big;
-    o->scratch = take(o->scratch_floats);
-    o->masked = reinterpret_cast<int*>(take(S * R));
-    return off * sizeof(float) + 256;
+    Carve c{base};
+    carve_records(m, R, S, P * CG, c, o);
+    o->G = c.take(P ? S * R * CG : 4);
+    return c.bytes();
 }
-}  // namespace tb2
-
-namespace tb2 {
 
 
 // fp32 window [rows x cols] (leading dimension ld_src) -> bf16 (hi, lo) at column col_off of a [rows x ld_dst] matrix
@@ -1291,11 +1209,9 @@ static int split2d(const float* src, int ld_src, size_t rows, int cols, __nv_bfl
     return TB2_OK;
 }
 
-struct SocBuffers {
-    float *X, *GP, *DG, *HS, *DN, *VEL, *DXIN, *H1, *DH1, *LAT, *DLAT, *DGRID, *dWt1;
-    float *pass[2], *dc, *zero_h, *scratch;
-    size_t scratch_floats;
-    int *masked, *rows, *winc, *counts, *base, *start, *pcell;
+struct SocBuffers : RowRecords {
+    float *H1, *DH1, *LAT, *DLAT, *DGRID, *dWt1, *zero_h;
+    int *rows, *winc, *counts, *base, *start, *pcell;
     unsigned* sorted;
     uint8_t* pflag;
     uint32_t* wine;
@@ -1316,48 +1232,29 @@ static size_t carve_social(const tb2_lstm* m, const tb2_layout* l, size_t S, voi
     const size_t d1 = (size_t)m->mlp_dims[1], C = (size_t)m->C, cells = (size_t)m->cells;
     const size_t nm1 = (size_t)(l->n_max > 1 ? l->n_max - 1 : 1);
     const size_t H = (size_t)m->H, G4 = 4 * H;
-    size_t off = 0;
-    auto take = [&](size_t n) {
-        float* p = basep ? reinterpret_cast<float*>(basep) + off : nullptr;
-        off += (n + 3) & ~(size_t)3;
-        return p;
-    };
     SocBuffers tmp;
     SocBuffers* o = b ? b : &tmp;
-    o->X = take(S * M * K);
-    o->GP = take(S * M * G4);
-    o->DG = take(S * M * G4);
-    o->HS = take(S * M * H);
-    o->DN = take(S * M * 8);
-    o->VEL = take(S * M * 2);
-    o->DXIN = take(S * M * (E + P));
-    o->H1 = take(m->n_mlp == 2 ? S * M * d1 : 4);
-    o->DH1 = take(M * (d1 > H ? d1 : H));     // also holds the [M,H] recurrent d h of a step
-    o->LAT = take(S * M * C);
-    o->DLAT = take(S * M * C);
-    o->DGRID = take(M * nm1 * C);
-    o->dWt1 = take(cells * C * d1);
-    o->pass[0] = take(M * H);
-    o->pass[1] = take(M * H);
-    o->dc = take(M * H);
-    o->zero_h = take(M * H);
-    size_t big = G4 * K;
-    if (P * d1 > big) big = P * d1;
-    o->scratch_floats = 8 * big;
-    o->scratch = take(o->scratch_floats);
-    o->masked = reinterpret_cast<int*>(take(S * M));
-    o->rows = reinterpret_cast<int*>(take(M));
-    o->winc = reinterpret_cast<int*>(take(S * M));
-    o->wine = reinterpret_cast<uint32_t*>(take(S * M * nm1));
-    o->sorted = reinterpret_cast<unsigned*>(take(M * nm1));
-    o->pcell = reinterpret_cast<int*>(take(S * M * nm1));
-    o->pflag = reinterpret_cast<uint8_t*>(take((S * M * nm1 + 3) / 4));
-    o->counts = reinterpret_cast<int*>(take((size_t)l->B * cells));
-    o->base = reinterpret_cast<int*>(take((size_t)l->B * cells));
-    o->start = reinterpret_cast<int*>(take(cells + 1));
-    o->Wt1_hi = reinterpret_cast<__nv_bfloat16*>(take((cells * C * d1 + 1) / 2));
-    o->Wt1_lo = reinterpret_cast<__nv_bfloat16*>(take((cells * C * d1 + 1) / 2));
-    auto take_bf16 = [&](size_t n) { return reinterpret_cast<__nv_bfloat16*>(take((n + 1) / 2)); };
+    Carve c{basep};
+    carve_records(m, M, S, P * d1, c, o);
+    o->H1 = c.take(m->n_mlp == 2 ? S * M * d1 : 4);
+    o->DH1 = c.take(M * (d1 > H ? d1 : H));     // also holds the [M,H] recurrent d h of a step
+    o->LAT = c.take(S * M * C);
+    o->DLAT = c.take(S * M * C);
+    o->DGRID = c.take(M * nm1 * C);
+    o->dWt1 = c.take(cells * C * d1);
+    o->zero_h = c.take(M * H);
+    o->rows = reinterpret_cast<int*>(c.take(M));
+    o->winc = reinterpret_cast<int*>(c.take(S * M));
+    o->wine = reinterpret_cast<uint32_t*>(c.take(S * M * nm1));
+    o->sorted = reinterpret_cast<unsigned*>(c.take(M * nm1));
+    o->pcell = reinterpret_cast<int*>(c.take(S * M * nm1));
+    o->pflag = reinterpret_cast<uint8_t*>(c.take((S * M * nm1 + 3) / 4));
+    o->counts = reinterpret_cast<int*>(c.take((size_t)l->B * cells));
+    o->base = reinterpret_cast<int*>(c.take((size_t)l->B * cells));
+    o->start = reinterpret_cast<int*>(c.take(cells + 1));
+    o->Wt1_hi = reinterpret_cast<__nv_bfloat16*>(c.take((cells * C * d1 + 1) / 2));
+    o->Wt1_lo = reinterpret_cast<__nv_bfloat16*>(c.take((cells * C * d1 + 1) / 2));
+    auto take_bf16 = [&](size_t n) { return reinterpret_cast<__nv_bfloat16*>(c.take((n + 1) / 2)); };
     o->X_hi = take_bf16(S * M * K);
     o->X_lo = take_bf16(S * M * K);
     for (int i = 0; i < 2; ++i) {
@@ -1374,8 +1271,67 @@ static size_t carve_social(const tb2_lstm* m, const tb2_layout* l, size_t S, voi
     o->DZ2_lo = take_bf16(M * P);
     o->W2T_hi = take_bf16(d1 * P);
     o->W2T_lo = take_bf16(d1 * P);
-    o->zero_bias = take(d1 > G4 ? d1 : G4);
-    return off * sizeof(float) + 256;
+    o->zero_bias = c.take(d1 > G4 ? d1 : G4);
+    return c.bytes();
+}
+
+// (B) gate pre-activations of all steps: one GEMM per cell (encoder / decoder weights).  wgmma (the social backward,
+// when its row GEMMs run on the tensor cores): the 3-pass wgmma kernel on the bf16 splits of X and [W_ih | W_hh]
+// there; otherwise gemm_nn.
+static int gate_preactivations(const tb2_lstm* m, const RowRecords& b, int rows, int S, int S_enc,
+                               const SocBuffers* wgmma, cudaStream_t st) {
+    const int K = m->K_gate, G4 = 4 * m->H;
+    for (int phase = 0; phase < 2; ++phase) {
+        const int s0 = phase == TB2_PHASE_ENCODER ? 0 : S_enc;
+        const int ns = phase == TB2_PHASE_ENCODER ? S_enc : S - S_enc;
+        if (ns <= 0) continue;
+        const size_t x0 = (size_t)s0 * rows * K;
+        float* GP = b.GP + (size_t)s0 * rows * G4;
+        const int rc = wgmma ? launch_dense_tc(wgmma->X_hi + x0, wgmma->X_lo + x0, wgmma->Wcat_hi[phase],
+                                               wgmma->Wcat_lo[phase], m->bg[phase], GP, nullptr, nullptr, ns * rows, K,
+                                               G4, 0, st)
+                             : gemm_nn(b.X + x0, K, m->WgT[phase], G4, GP, G4, ns * rows, G4, K, m->bg[phase], st);
+        if (rc) return rc;
+    }
+    return TB2_OK;
+}
+
+// LSTM, Hidden2Normal and InputEmbedding weight gradients: one reduction over all S * rows (step, row) records per
+// tensor.  input_grads: each cell first computes dX_in = dgates . W_ih of all its steps (the social backward computes
+// dX_in step by step inside its time loop instead, where the grid MLP's backward needs it).
+static int lstm_weight_grads(const tb2_lstm* m, const tb2_lstm_weights* w, const tb2_lstm_grads* g, const RowRecords& b,
+                             int rows, int S, int S_enc, bool input_grads, cudaStream_t st) {
+    const int K = m->K_gate, E = m->E, EP = E + m->P, H = m->H, G4 = 4 * H;
+    int rc;
+    for (int phase = 0; phase < 2; ++phase) {
+        const int s0 = phase == TB2_PHASE_ENCODER ? 0 : S_enc;
+        const int ns = phase == TB2_PHASE_ENCODER ? S_enc : S - S_enc;
+        if (ns <= 0) continue;
+        const bool enc = phase == TB2_PHASE_ENCODER;
+        const float* DG = b.DG + (size_t)s0 * rows * G4;
+        const float* X = b.X + (size_t)s0 * rows * K;
+        const int n = ns * rows;
+        // dX_in = dgates . W_ih   (torch layout [4H, E+P] is the [K = 4H, N = E+P] operand as it stands)
+        if (input_grads && (rc = gemm_nn(DG, G4, enc ? w->encoder_weight_ih : w->decoder_weight_ih, EP,
+                                         b.DXIN + (size_t)s0 * rows * EP, EP, n, EP, G4, nullptr, st)))
+            return rc;
+        if ((rc = gemm_tn(DG, G4, X, K, enc ? g->encoder_weight_ih : g->decoder_weight_ih, EP, n, G4, EP, b.scratch,
+                          b.scratch_floats, st)))
+            return rc;
+        if ((rc = gemm_tn(DG, G4, X + EP, K, enc ? g->encoder_weight_hh : g->decoder_weight_hh, H, n, G4, H, b.scratch,
+                          b.scratch_floats, st)))
+            return rc;
+        if ((rc = colsum(DG, G4, n, G4, enc ? g->encoder_bias_ih : g->decoder_bias_ih,
+                         enc ? g->encoder_bias_hh : g->decoder_bias_hh, b.scratch, b.scratch_floats, st)))
+            return rc;
+    }
+    if ((rc = gemm_tn(b.DN, 8, b.HS, H, g->hidden2normal_weight, H, S * rows, 5, H, b.scratch, b.scratch_floats, st)))
+        return rc;
+    if ((rc = colsum(b.DN, 8, S * rows, 5, g->hidden2normal_bias, nullptr, b.scratch, b.scratch_floats, st))) return rc;
+    bwd_embed_kernel<<<E - 2, 256, 0, st>>>(b.X, K, b.DXIN, EP, b.VEL, S * rows, g->input_embedding_weight,
+                                            g->input_embedding_bias);
+    TB2_LAUNCH_CHECK();
+    return TB2_OK;
 }
 
 template <int C>
@@ -1404,6 +1360,47 @@ static int social_pair_kernels(const tb2_lstm* m, const tb2_layout* l, const Soc
             b.sorted, b.start, nm1, l->row_scene, l->scene_off, lat, b.DH1, d1, b.dWt1);
     }
     TB2_LAUNCH_CHECK();
+    return TB2_OK;
+}
+
+// (A) this step's forward records: winners and pair tables, latent vectors (b.LAT), hidden1 (b.H1, two_layer) and the
+// pooled vector (ws.pooled).  With a training cache the forward kept them; otherwise they are recomputed from h_prev.
+static int social_step_records(const tb2_lstm* m, const tb2_layout* l, const SocBuffers& b, const Workspace& ws,
+                               const TrainCache* cache, int s, const float* h_prev, const float* o1, const float* o2,
+                               cudaStream_t st) {
+    const size_t M = (size_t)l->M, P = (size_t)m->P, d1 = (size_t)m->mlp_dims[1], C = (size_t)m->C;
+    const size_t nm1 = (size_t)(l->n_max > 1 ? l->n_max - 1 : 1);
+    const bool two = m->n_mlp == 2;
+    float* H1 = b.H1 + (size_t)s * M * d1;
+    if (cache) {
+        // hidden1 and the pooled vector of the forward, as fp32 (hi + lo of the bf16 pair the next kernel consumed)
+        if (two) {
+            merge_split_kernel<<<1024, 256, 0, st>>>((const __nv_bfloat16*)cache->h1_hi + (size_t)s * M * d1,
+                                                     (const __nv_bfloat16*)cache->h1_lo + (size_t)s * M * d1, nullptr,
+                                                     H1, M * d1);
+            TB2_LAUNCH_CHECK();
+        }
+        merge_split_kernel<<<512, 256, 0, st>>>((const __nv_bfloat16*)cache->pool_hi + (size_t)s * M * P,
+                                                (const __nv_bfloat16*)cache->pool_lo + (size_t)s * M * P, nullptr, ws.pooled,
+                                                M * P);
+        TB2_LAUNCH_CHECK();
+        return TB2_OK;
+    }
+    Workspace w2 = ws;
+    w2.lat = b.LAT + (size_t)s * M * C;
+    w2.win_count = b.winc + (size_t)s * M;
+    w2.win_ent = b.wine + (size_t)s * M * nm1;
+    w2.pair_cell = b.pcell + (size_t)s * M * nm1;
+    w2.pair_flag = b.pflag + (size_t)s * M * nm1;
+    int rc;
+    if ((rc = launch_pool_prepare(m, l, h_prev ? h_prev : b.zero_h, o1, o2, 1, 1, 0, &w2, st))) return rc;
+    if ((rc = launch_pool_mlp(m, l, &w2, ws.pooled, nullptr, nullptr, st))) return rc;
+    if (two) {      // a tensor-core second Linear read hidden1 as the bf16 (hi, lo) pair in act[0] / act[1]
+        const bool tc2 = m->W_hi[1] != nullptr;
+        merge_split_kernel<<<1024, 256, 0, st>>>(tc2 ? (const __nv_bfloat16*)ws.act[0] : nullptr,
+                                                 tc2 ? (const __nv_bfloat16*)ws.act[1] : nullptr, ws.act[0], H1, M * d1);
+        TB2_LAUNCH_CHECK();
+    }
     return TB2_OK;
 }
 
@@ -1440,41 +1437,13 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
     TB2_LAUNCH_CHECK();
     int rc;
     if ((rc = launch_split_bf16(m->Wt1, b.Wt1_hi, b.Wt1_lo, (size_t)cells * C * d1, st))) return rc;
-    const bool tc2 = two && m->W_hi[1] != nullptr;
     // (A) forward quantities of every step: winners + lat, hidden1, X = [emb | pooled | h_prev]
     for (int s = 0; s < S; ++s) {
         const float *o1, *o2;
         int phase;
         if ((rc = resolve_step_inputs(l, observed, obs_length, truth, positions, s, &ws, &o1, &o2, &phase, st))) return rc;
         const float* h_prev = s > 0 ? states + ((size_t)(s - 1) * 2 + 0) * M * H : nullptr;
-        Workspace w2 = ws;
-        w2.lat = b.LAT + (size_t)s * M * C;
-        w2.win_count = b.winc + (size_t)s * M;
-        w2.win_ent = b.wine + (size_t)s * M * nm1;
-        w2.pair_cell = b.pcell + (size_t)s * M * nm1;
-        w2.pair_flag = b.pflag + (size_t)s * M * nm1;
-        if (cache) {
-            // hidden1 and the pooled vector of the forward, as fp32 (hi + lo of the bf16 pair the next kernel consumed)
-            if (two) {
-                merge_split_kernel<<<1024, 256, 0, st>>>((const __nv_bfloat16*)cache->h1_hi + (size_t)s * M * d1,
-                                                         (const __nv_bfloat16*)cache->h1_lo + (size_t)s * M * d1, nullptr,
-                                                         b.H1 + (size_t)s * M * d1, M * d1);
-                TB2_LAUNCH_CHECK();
-            }
-            merge_split_kernel<<<512, 256, 0, st>>>((const __nv_bfloat16*)cache->pool_hi + (size_t)s * M * P,
-                                                    (const __nv_bfloat16*)cache->pool_lo + (size_t)s * M * P, nullptr, ws.pooled,
-                                                    M * P);
-            TB2_LAUNCH_CHECK();
-        } else {
-        if ((rc = launch_pool_prepare(m, l, h_prev ? h_prev : b.zero_h, o1, o2, 1, 1, 0, &w2, st))) return rc;
-        if ((rc = launch_pool_mlp(m, l, &w2, ws.pooled, nullptr, nullptr, st))) return rc;
-        if (two) {
-            merge_split_kernel<<<1024, 256, 0, st>>>(tc2 ? (const __nv_bfloat16*)ws.act[0] : nullptr,
-                                                     tc2 ? (const __nv_bfloat16*)ws.act[1] : nullptr, ws.act[0],
-                                                     b.H1 + (size_t)s * M * d1, M * d1);
-            TB2_LAUNCH_CHECK();
-        }
-        }
+        if ((rc = social_step_records(m, l, b, ws, cache, s, h_prev, o1, o2, st))) return rc;
         {
             KernelTimer kt("bwd_gather", st);
             bwd_gather_kernel<<<Mi, 256, 0, st>>>(b.rows, Mi, (const float2*)o1, (const float2*)o2, m->We, m->be,
@@ -1508,22 +1477,7 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
         }
         if ((rc = split2d(b.X, K, (size_t)S * M, K, b.X_hi, b.X_lo, K, 0, st))) return rc;
     }
-    // (B) gate pre-activations of all steps
-    for (int phase = 0; phase < 2; ++phase) {
-        const int s0 = phase == TB2_PHASE_ENCODER ? 0 : S_enc;
-        const int ns = phase == TB2_PHASE_ENCODER ? S_enc : S - S_enc;
-        if (ns <= 0) continue;
-        if (tcg) {
-            if ((rc = launch_dense_tc(b.X_hi + (size_t)s0 * M * K, b.X_lo + (size_t)s0 * M * K, b.Wcat_hi[phase],
-                                      b.Wcat_lo[phase], m->bg[phase], b.GP + (size_t)s0 * M * G4, nullptr, nullptr, ns * Mi,
-                                      K, G4, 0, st)))
-                return rc;
-            continue;
-        }
-        if ((rc = gemm_nn(b.X + (size_t)s0 * M * K, K, m->WgT[phase], G4, b.GP + (size_t)s0 * M * G4, G4,
-                          ns * Mi, G4, K, m->bg[phase], st)))
-            return rc;
-    }
+    if ((rc = gate_preactivations(m, b, Mi, S, S_enc, tcg ? &b : nullptr, st))) return rc;
     // (C) reverse time: cell -> input gradient -> grid MLP -> scatter to the neighbours' hidden states
     const size_t place_smem = (size_t)l->n_max * nm1 * sizeof(short);
     TB2_REQUIRE(place_smem <= 200 * 1024 && cells < 32768, "scene too large for the social backward");
@@ -1626,27 +1580,7 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
         if ((rc = colsum(b.DXIN + E, EP, S * Mi, P, g->pool_embedding_bias1, nullptr, b.scratch, b.scratch_floats, st))) return rc;
     }
     // (D) parameter gradients: one reduction over all (step, row) records per tensor
-    for (int phase = 0; phase < 2; ++phase) {
-        const int s0 = phase == TB2_PHASE_ENCODER ? 0 : S_enc;
-        const int ns = phase == TB2_PHASE_ENCODER ? S_enc : S - S_enc;
-        if (ns <= 0) continue;
-        const float* DG = b.DG + (size_t)s0 * M * G4;
-        const float* X = b.X + (size_t)s0 * M * K;
-        const int rows = ns * Mi;
-        float* gWih = phase == TB2_PHASE_ENCODER ? g->encoder_weight_ih : g->decoder_weight_ih;
-        float* gWhh = phase == TB2_PHASE_ENCODER ? g->encoder_weight_hh : g->decoder_weight_hh;
-        float* gbih = phase == TB2_PHASE_ENCODER ? g->encoder_bias_ih : g->decoder_bias_ih;
-        float* gbhh = phase == TB2_PHASE_ENCODER ? g->encoder_bias_hh : g->decoder_bias_hh;
-        if ((rc = gemm_tn(DG, G4, X, K, gWih, EP, rows, G4, EP, b.scratch, b.scratch_floats, st))) return rc;
-        if ((rc = gemm_tn(DG, G4, X + EP, K, gWhh, H, rows, G4, H, b.scratch, b.scratch_floats, st))) return rc;
-        if ((rc = colsum(DG, G4, rows, G4, gbih, gbhh, b.scratch, b.scratch_floats, st))) return rc;
-    }
-    if ((rc = gemm_tn(b.DN, 8, b.HS, H, g->hidden2normal_weight, H, S * Mi, 5, H, b.scratch, b.scratch_floats, st)))
-        return rc;
-    if ((rc = colsum(b.DN, 8, S * Mi, 5, g->hidden2normal_bias, nullptr, b.scratch, b.scratch_floats, st))) return rc;
-    bwd_embed_kernel<<<E - 2, 256, 0, st>>>(b.X, K, b.DXIN, EP, b.VEL, S * Mi, g->input_embedding_weight,
-                                            g->input_embedding_bias);
-    TB2_LAUNCH_CHECK();
+    if ((rc = lstm_weight_grads(m, w, g, b, Mi, S, S_enc, false, st))) return rc;
     untranspose_add_kernel<<<2048, 256, 0, st>>>(b.dWt1, g->pool_embedding_weight0, cells, C, d1);
     TB2_LAUNCH_CHECK();
     // lat_j = W_enc h_j + b_enc (gridbased_pooling.py:160-167): h of step s-1 is states[s-1]
@@ -1762,15 +1696,7 @@ static int sequence_backward_impl(const tb2_lstm* m, const tb2_layout* l, const 
         }
         TB2_LAUNCH_CHECK();
     }
-    // (B) gate pre-activations of all steps: one GEMM per cell (encoder / decoder weights)
-    for (int phase = 0; phase < 2; ++phase) {
-        const int s0 = phase == TB2_PHASE_ENCODER ? 0 : S_enc;
-        const int ns = phase == TB2_PHASE_ENCODER ? S_enc : S - S_enc;
-        if (ns <= 0) continue;
-        if ((rc = gemm_nn(b.X + (size_t)s0 * R * K, K, m->WgT[phase], G4, b.GP + (size_t)s0 * R * G4, G4, ns * R,
-                          G4, K, m->bg[phase], st)))
-            return rc;
-    }
+    if ((rc = gate_preactivations(m, b, R, S, S_enc, nullptr, st))) return rc;
     // (C) the sequential chain: one kernel per step
     int cur = 0;
     for (int s = S - 1; s >= 0; --s, cur ^= 1) {
@@ -1789,30 +1715,7 @@ static int sequence_backward_impl(const tb2_lstm* m, const tb2_layout* l, const 
         if (rc) return rc;
     }
     // (D) + (E) input gradients of all steps and the parameter gradients: one reduction per tensor
-    for (int phase = 0; phase < 2; ++phase) {
-        const int s0 = phase == TB2_PHASE_ENCODER ? 0 : S_enc;
-        const int ns = phase == TB2_PHASE_ENCODER ? S_enc : S - S_enc;
-        if (ns <= 0) continue;
-        const float* DG = b.DG + (size_t)s0 * R * G4;
-        const float* X = b.X + (size_t)s0 * R * K;
-        const int rows = ns * R;
-        float* gWih = phase == TB2_PHASE_ENCODER ? g->encoder_weight_ih : g->decoder_weight_ih;
-        float* gWhh = phase == TB2_PHASE_ENCODER ? g->encoder_weight_hh : g->decoder_weight_hh;
-        float* gbih = phase == TB2_PHASE_ENCODER ? g->encoder_bias_ih : g->decoder_bias_ih;
-        float* gbhh = phase == TB2_PHASE_ENCODER ? g->encoder_bias_hh : g->decoder_bias_hh;
-        const float* Wih = phase == TB2_PHASE_ENCODER ? w->encoder_weight_ih : w->decoder_weight_ih;
-        // dX_in = dgates . W_ih   (torch layout [4H, E+P] is the [K = 4H, N = E+P] operand as it stands)
-        if ((rc = gemm_nn(DG, G4, Wih, EP, b.DXIN + (size_t)s0 * R * EP, EP, rows, EP, G4, nullptr, st))) return rc;
-        if ((rc = gemm_tn(DG, G4, X, K, gWih, EP, rows, G4, EP, b.scratch, b.scratch_floats, st))) return rc;
-        if ((rc = gemm_tn(DG, G4, X + EP, K, gWhh, H, rows, G4, H, b.scratch, b.scratch_floats, st))) return rc;
-        if ((rc = colsum(DG, G4, rows, G4, gbih, gbhh, b.scratch, b.scratch_floats, st))) return rc;
-    }
-    if ((rc = gemm_tn(b.DN, 8, b.HS, H, g->hidden2normal_weight, H, S * R, 5, H, b.scratch, b.scratch_floats, st)))
-        return rc;
-    if ((rc = colsum(b.DN, 8, S * R, 5, g->hidden2normal_bias, nullptr, b.scratch, b.scratch_floats, st))) return rc;
-    bwd_embed_kernel<<<E - 2, 256, 0, st>>>(b.X, K, b.DXIN, EP, b.VEL, S * R, g->input_embedding_weight,
-                                            g->input_embedding_bias);
-    TB2_LAUNCH_CHECK();
+    if ((rc = lstm_weight_grads(m, w, g, b, R, S, S_enc, true, st))) return rc;
     if (pooled) {
         relu_mask_kernel<<<(unsigned)(((size_t)S * R * P + 255) / 256), 256, 0, st>>>(b.X, K, b.DXIN, EP, S * R, E, P);
         TB2_LAUNCH_CHECK();
