@@ -160,6 +160,23 @@ int resolve_step_inputs(const tb2_layout* l, const float* observed, int obs_leng
     return TB2_OK;
 }
 
+// Non-grid interaction module (pool types from TB2_POOL_HIDDEN_MLP on), one kernel per scene -> out [M, pool_out].
+// nn_lstm / Trajectron also advance the interaction-encoder LSTM state kept in the workspace.
+static int launch_nongrid_pool(const tb2_lstm* m, const tb2_layout* l, const float* hidden, const float* obs1,
+                               const float* obs2, const Workspace* ws, float* out, cudaStream_t st) {
+    int rc;
+    switch (m->cfg.pool_type) {
+        case TB2_POOL_HIDDEN_MLP: return launch_hidden_mlp_pool(m, l, hidden, obs1, obs2, out, st);
+        case TB2_POOL_ATTN_MLP: return launch_attn_mlp_pool(m, l, hidden, obs1, obs2, out, st);
+        case TB2_POOL_NN_MLP: return launch_nn_mlp_pool(m, l, obs1, obs2, out, st);
+        case TB2_POOL_NN_LSTM: rc = launch_nn_mlp_pool(m, l, obs1, obs2, ws->pool_feat, st); break;
+        case TB2_POOL_TRAJECTRON: rc = launch_trajectron_feat(m, l, obs1, obs2, ws->scene_sum, ws->pool_feat, st); break;
+        default: TB2_REQUIRE(false, "model has no non-grid interaction pooling");
+    }
+    if (rc) return rc;
+    return launch_pool_lstm_cell(m, l, ws->pool_feat, ws->pool_h, ws->pool_c, out, st);
+}
+
 }  // namespace tb2
 
 using namespace tb2;
@@ -205,104 +222,72 @@ int tb2_profile_end(char* json_out, size_t capacity) {
     return TB2_OK;
 }
 
-int tb2_lstm_create(const tb2_lstm_config* cfg, tb2_lstm** out) {
-    TB2_REQUIRE(cfg && out, "null argument");
-    *out = nullptr;
-    if (!hidden_dim_supported(cfg->hidden_dim)) {
-        set_error(kHiddenDimMessage);
-        return TB2_ERR_UNSUPPORTED;
+// Pool widths of the configuration (C, cells, n_mlp, mlp_dims, pool_out, P), each pool type's own checks first.
+static int configure_pool(const tb2_lstm_config& c, tb2_lstm* m) {
+    switch (c.pool_type) {
+        case TB2_POOL_NONE:
+            return TB2_OK;
+        case TB2_POOL_OCCUPANCY:
+        case TB2_POOL_DIRECTIONAL:
+        case TB2_POOL_SOCIAL:
+            if (c.pool_size != 1 || c.blur_size != 1) {
+                set_error("pool_size / blur_size != 1 are not built (the reference CLI never sets them)");
+                return TB2_ERR_UNSUPPORTED;
+            }
+            TB2_REQUIRE(c.n >= 1 && c.n <= 64 && c.cell_side > 0.f, "grid size");
+            TB2_REQUIRE(c.num_layers >= 0 && c.num_layers <= kMaxMlpLayers, "num_layers");
+            m->C = c.pool_type == TB2_POOL_OCCUPANCY ? 1 : c.pool_type == TB2_POOL_DIRECTIONAL ? 2 : c.latent_dim;
+            if (c.pool_type == TB2_POOL_SOCIAL && !(m->C == 4 || m->C == 8 || m->C == 16 || m->C == 32)) {
+                set_error("social latent_dim must be 4, 8, 16 or 32");
+                return TB2_ERR_UNSUPPORTED;
+            }
+            m->cells = c.n * c.n;
+            m->n_mlp = c.num_layers;
+            m->mlp_dims[0] = m->C * m->cells;
+            for (int i = 1; i <= m->n_mlp; ++i) {
+                m->mlp_dims[i] = (i == m->n_mlp) ? c.out_dim : c.layer_dims[i - 1];
+                TB2_REQUIRE(m->mlp_dims[i] >= 1, "MLP width");
+            }
+            m->pool_out = m->n_mlp == 0 ? m->mlp_dims[0] : c.out_dim;
+            break;
+        case TB2_POOL_NN_LSTM:
+            TB2_REQUIRE(c.mlp_dim_hidden >= 1 && c.mlp_dim_hidden <= 512 && c.out_dim <= 1024 && c.mlp_dim_vel != 0,
+                        "nearest-neighbour LSTM pooling needs 1 <= hidden_dim <= 512, out_dim <= 1024 and velocities");
+            [[fallthrough]];
+        case TB2_POOL_NN_MLP:
+            TB2_REQUIRE(c.n >= 1 && c.n <= 32 && c.mlp_dim_spatial >= 1 && c.out_dim == c.n * c.mlp_dim_spatial,
+                        "nearest-neighbour pooling needs 1 <= n <= 32 and out_dim == n * mlp_dim_spatial");
+            m->pool_out = c.out_dim;
+            break;
+        case TB2_POOL_TRAJECTRON:
+            TB2_REQUIRE(c.mlp_dim_hidden >= 1 && c.mlp_dim_hidden <= 512 && c.out_dim >= 1 && c.out_dim <= 1024,
+                        "Trajectron pooling needs 1 <= hidden_dim <= 512 and out_dim <= 1024");
+            m->pool_out = c.out_dim;
+            break;
+        case TB2_POOL_ATTN_MLP:
+            TB2_REQUIRE(c.mlp_dim_spatial >= 1 && c.mlp_dim_vel >= 0 && c.mlp_dim_hidden >= 0 && c.out_dim >= 1 &&
+                            c.mlp_dim_spatial + c.mlp_dim_vel + c.mlp_dim_hidden <= 128,
+                        "attention pooling needs mlp_dim <= 128 (kernel specialisation)");
+            m->pool_out = c.out_dim;
+            break;
+        case TB2_POOL_HIDDEN_MLP:
+            TB2_REQUIRE(c.mlp_dim_spatial >= 1 && c.mlp_dim_vel >= 0 && c.mlp_dim_hidden >= 0 && c.out_dim >= 1 &&
+                            c.mlp_dim_spatial + c.mlp_dim_vel + c.mlp_dim_hidden <= 4096,
+                        "hidden-state MLP pooling widths");
+            m->pool_out = c.out_dim;
+            break;
     }
-    TB2_REQUIRE(cfg->embedding_dim >= 4 && cfg->embedding_dim <= 1024, "embedding_dim out of range");
-    TB2_REQUIRE(cfg->pool_type >= TB2_POOL_NONE && cfg->pool_type <= TB2_POOL_TRAJECTRON, "bad pool_type");
-    tb2_lstm* m = new (std::nothrow) tb2_lstm();
-    TB2_REQUIRE(m, "out of host memory");
-    m->cfg = *cfg;
-    m->H = cfg->hidden_dim;
-    m->E = cfg->embedding_dim;
-    m->weights_set = false;
-    m->tc_disabled = tensor_cores_disabled();
-    m->C = 0; m->cells = 0; m->n_mlp = 0; m->P = 0; m->pool_out = 0;
-    m->We = m->be = m->Wn = m->bn = m->WencT = m->benc = m->Wt1 = m->base1 = nullptr;
-    m->Wt1_hi = m->Wt1_lo = nullptr;
-    for (int i = 0; i < 2; ++i) { m->WgT[i] = m->bg[i] = nullptr; m->Wg_hi[i] = m->Wg_lo[i] = nullptr; }
-    for (int i = 0; i < kMaxMlpLayers; ++i) { m->WT[i] = m->bl[i] = nullptr; m->W_hi[i] = m->W_lo[i] = nullptr; }
-    m->mp_Ws = m->mp_bs = m->mp_Wv = m->mp_bv = m->mp_WhT = m->mp_bh = m->mp_WoT = m->mp_bo = nullptr;
-    m->at_AqT = m->at_Ak = m->at_AvT = m->at_bqkv = m->at_WoT = m->at_bo = nullptr;
-    m->pl_WihT = m->pl_WhhT = m->pl_b = nullptr;
-    auto fail = [&](int rc) { tb2_lstm_destroy(m); return rc; };
-    if (cfg->pool_type == TB2_POOL_TRAJECTRON) {
-        if (!(cfg->mlp_dim_hidden >= 1 && cfg->mlp_dim_hidden <= 512 && cfg->out_dim >= 1 && cfg->out_dim <= 1024)) {
-            set_error("invalid argument: Trajectron pooling needs 1 <= hidden_dim <= 512 and out_dim <= 1024");
-            return fail(TB2_ERR_INVALID);
-        }
-        m->pool_out = cfg->out_dim;
-        if (cfg->pool_to_input) m->P = m->pool_out;
-        else if (m->pool_out != m->H) { set_error("invalid argument: pool_to_input=0 needs out_dim == hidden_dim"); return fail(TB2_ERR_INVALID); }
-    }
-    if (cfg->pool_type == TB2_POOL_NN_LSTM &&
-        !(cfg->mlp_dim_hidden >= 1 && cfg->mlp_dim_hidden <= 512 && cfg->out_dim <= 1024 && cfg->mlp_dim_vel != 0)) {
-        set_error("invalid argument: nearest-neighbour LSTM pooling needs 1 <= hidden_dim <= 512, out_dim <= 1024 and velocities");
-        return fail(TB2_ERR_INVALID);
-    }
-    if (cfg->pool_type == TB2_POOL_TRAJECTRON) {
-        // validated above
-    } else
-    if (cfg->pool_type == TB2_POOL_NN_MLP || cfg->pool_type == TB2_POOL_NN_LSTM) {
-        if (!(cfg->n >= 1 && cfg->n <= 32 && cfg->mlp_dim_spatial >= 1 && cfg->out_dim == cfg->n * cfg->mlp_dim_spatial)) {
-            set_error("invalid argument: nearest-neighbour pooling needs 1 <= n <= 32 and out_dim == n * mlp_dim_spatial");
-            return fail(TB2_ERR_INVALID);
-        }
-        m->pool_out = cfg->out_dim;
-        if (cfg->pool_to_input) m->P = m->pool_out;
-        else if (m->pool_out != m->H) { set_error("invalid argument: pool_to_input=0 needs out_dim == hidden_dim"); return fail(TB2_ERR_INVALID); }
-    } else
-    if (cfg->pool_type == TB2_POOL_ATTN_MLP) {
-        const int Ea = cfg->mlp_dim_spatial + cfg->mlp_dim_vel + cfg->mlp_dim_hidden;
-        if (!(cfg->mlp_dim_spatial >= 1 && cfg->mlp_dim_vel >= 0 && cfg->mlp_dim_hidden >= 0 && cfg->out_dim >= 1 && Ea <= 128)) {
-            set_error("invalid argument: attention pooling needs mlp_dim <= 128 (kernel specialisation)");
-            return fail(TB2_ERR_INVALID);
-        }
-        m->pool_out = cfg->out_dim;
-        if (cfg->pool_to_input) m->P = m->pool_out;
-        else if (m->pool_out != m->H) { set_error("invalid argument: pool_to_input=0 needs out_dim == hidden_dim"); return fail(TB2_ERR_INVALID); }
-    } else
-    if (cfg->pool_type == TB2_POOL_HIDDEN_MLP) {
-        if (!(cfg->mlp_dim_spatial >= 1 && cfg->mlp_dim_vel >= 0 && cfg->mlp_dim_hidden >= 0 && cfg->out_dim >= 1 &&
-              cfg->mlp_dim_spatial + cfg->mlp_dim_vel + cfg->mlp_dim_hidden <= 4096)) {
-            set_error("invalid argument: hidden-state MLP pooling widths");
-            return fail(TB2_ERR_INVALID);
-        }
-        m->pool_out = cfg->out_dim;
-        if (cfg->pool_to_input) m->P = m->pool_out;
-        else if (m->pool_out != m->H) { set_error("invalid argument: pool_to_input=0 needs out_dim == hidden_dim"); return fail(TB2_ERR_INVALID); }
-    } else
-    if (cfg->pool_type != TB2_POOL_NONE) {
-        if (cfg->pool_size != 1 || cfg->blur_size != 1) {
-            set_error("pool_size / blur_size != 1 are not built (the reference CLI never sets them)");
-            return fail(TB2_ERR_UNSUPPORTED);
-        }
-        if (!(cfg->n >= 1 && cfg->n <= 64 && cfg->cell_side > 0.f)) { set_error("invalid argument: grid size"); return fail(TB2_ERR_INVALID); }
-        if (!(cfg->num_layers >= 0 && cfg->num_layers <= kMaxMlpLayers)) { set_error("invalid argument: num_layers"); return fail(TB2_ERR_INVALID); }
-        m->C = cfg->pool_type == TB2_POOL_OCCUPANCY ? 1 : cfg->pool_type == TB2_POOL_DIRECTIONAL ? 2 : cfg->latent_dim;
-        if (cfg->pool_type == TB2_POOL_SOCIAL && !(m->C == 4 || m->C == 8 || m->C == 16 || m->C == 32)) {
-            set_error("social latent_dim must be 4, 8, 16 or 32");
-            return fail(TB2_ERR_UNSUPPORTED);
-        }
-        m->cells = cfg->n * cfg->n;
-        m->n_mlp = cfg->num_layers;
-        m->mlp_dims[0] = m->C * m->cells;
-        for (int i = 1; i <= m->n_mlp; ++i)
-            m->mlp_dims[i] = (i == m->n_mlp) ? cfg->out_dim : cfg->layer_dims[i - 1];
-        m->pool_out = m->n_mlp == 0 ? m->mlp_dims[0] : cfg->out_dim;
-        for (int i = 1; i <= m->n_mlp; ++i)
-            if (m->mlp_dims[i] < 1) { set_error("invalid argument: MLP width"); return fail(TB2_ERR_INVALID); }
-        if (cfg->pool_to_input) m->P = m->pool_out;
-        else if (m->pool_out != m->H) { set_error("invalid argument: pool_to_input=0 needs out_dim == hidden_dim"); return fail(TB2_ERR_INVALID); }
-    }
-    m->K_gate = m->E + m->P + m->H;
-    m->K_gate_pad = (m->K_gate + kGateBK - 1) / kGateBK * kGateBK;
+    // the pool output is concatenated to the LSTM input, or added to the hidden state (lstm.py:151)
+    TB2_REQUIRE(c.pool_to_input || m->pool_out == m->H, "pool_to_input=0 needs out_dim == hidden_dim");
+    m->P = c.pool_to_input ? m->pool_out : 0;
+    return TB2_OK;
+}
+
+// Device buffers of the model: input embedding, gates and head, then those of its pool type.
+static int alloc_buffers(tb2_lstm* m) {
+    const tb2_lstm_config& c = m->cfg;
     int rc;
-#define ALLOC(ptr, count) if ((rc = dev_alloc(m->owned, (void**)&(ptr), (size_t)(count) * sizeof(float)))) return fail(rc)
+#define ALLOC(ptr, count) if ((rc = dev_alloc(m->owned, (void**)&(ptr), (size_t)(count) * sizeof(float)))) return rc
     ALLOC(m->We, (m->E - 2) * 2);
     ALLOC(m->be, m->E - 2);
     ALLOC(m->Wn, 5 * m->H);
@@ -322,71 +307,108 @@ int tb2_lstm_create(const tb2_lstm_config* cfg, tb2_lstm** out) {
             m->Wg_lo[ph] = lo;
         }
     }
-    if (cfg->pool_type == TB2_POOL_SOCIAL) {
-        ALLOC(m->WencT, m->H * m->C);
-        ALLOC(m->benc, m->C);
-    }
-    if (cfg->pool_type == TB2_POOL_TRAJECTRON) {
-        ALLOC(m->mp_Ws, (size_t)cfg->out_dim * 8);
-        ALLOC(m->mp_bs, cfg->out_dim);
-    }
-    if (cfg->pool_type == TB2_POOL_NN_LSTM || cfg->pool_type == TB2_POOL_TRAJECTRON) {
-        const size_t Hp = (size_t)cfg->mlp_dim_hidden;
-        ALLOC(m->pl_WihT, (size_t)cfg->out_dim * 4 * Hp);
+    const size_t Hp = (size_t)c.mlp_dim_hidden, D = (size_t)(c.mlp_dim_spatial + c.mlp_dim_vel + c.mlp_dim_hidden);
+    auto encoder_lstm = [&]() {         // interaction-encoder LSTMCell + hidden2pool (nn_lstm, Trajectron)
+        ALLOC(m->pl_WihT, (size_t)c.out_dim * 4 * Hp);
         ALLOC(m->pl_WhhT, Hp * 4 * Hp);
         ALLOC(m->pl_b, 4 * Hp);
-        ALLOC(m->mp_WoT, Hp * (size_t)cfg->out_dim);
-        ALLOC(m->mp_bo, cfg->out_dim);
-    }
-    if (cfg->pool_type == TB2_POOL_NN_MLP || cfg->pool_type == TB2_POOL_NN_LSTM) {
-        ALLOC(m->mp_Ws, cfg->mlp_dim_spatial * 4);
-        ALLOC(m->mp_bs, cfg->mlp_dim_spatial);
-    } else
-    if (cfg->pool_type == TB2_POOL_ATTN_MLP) {
-        const size_t Ea = (size_t)(cfg->mlp_dim_spatial + cfg->mlp_dim_vel + cfg->mlp_dim_hidden);
-        ALLOC(m->at_AqT, Ea * Ea);
-        ALLOC(m->at_Ak, Ea * Ea);
-        ALLOC(m->at_AvT, Ea * Ea);
-        ALLOC(m->at_bqkv, 3 * Ea);
-        ALLOC(m->at_WoT, Ea * Ea);
-        ALLOC(m->at_bo, Ea);
-    }
-    if (cfg->pool_type == TB2_POOL_HIDDEN_MLP || cfg->pool_type == TB2_POOL_ATTN_MLP) {
-        const int D = cfg->mlp_dim_spatial + cfg->mlp_dim_vel + cfg->mlp_dim_hidden;
-        ALLOC(m->mp_Ws, cfg->mlp_dim_spatial * 2);
-        ALLOC(m->mp_bs, cfg->mlp_dim_spatial);
-        ALLOC(m->mp_Wv, std::max(cfg->mlp_dim_vel, 1) * 2);
-        ALLOC(m->mp_bv, std::max(cfg->mlp_dim_vel, 1));
-        ALLOC(m->mp_WhT, (size_t)m->H * std::max(cfg->mlp_dim_hidden, 1));
-        ALLOC(m->mp_bh, std::max(cfg->mlp_dim_hidden, 1));
-        ALLOC(m->mp_WoT, (size_t)D * cfg->out_dim);
-        ALLOC(m->mp_bo, cfg->out_dim);
-    }
-    if (m->n_mlp >= 1) {
-        ALLOC(m->Wt1, (size_t)m->cells * m->C * m->mlp_dims[1]);
-        ALLOC(m->base1, m->mlp_dims[1]);
-        if (cfg->pool_type == TB2_POOL_SOCIAL && m->C == 16 && !no_tc) {
-            const size_t half = ((size_t)m->cells * 16 * m->mlp_dims[1] + 1) / 2;
-            float *hi, *lo;
-            ALLOC(hi, 2 * half);      // interleaved (hi | lo) slabs
-            ALLOC(lo, 4);
-            m->Wt1_hi = hi;
-            m->Wt1_lo = lo;
-        }
-        for (int layer = 1; layer < m->n_mlp; ++layer) {
-            ALLOC(m->WT[layer], (size_t)m->mlp_dims[layer] * m->mlp_dims[layer + 1]);
-            ALLOC(m->bl[layer], m->mlp_dims[layer + 1]);
-            if (layer == 1 && !no_tc && dense_tc_supported(m->mlp_dims[1], m->mlp_dims[2])) {
-                const size_t half = ((size_t)m->mlp_dims[1] * m->mlp_dims[2] + 1) / 2;   // bf16 pairs in float units
+        ALLOC(m->mp_WoT, Hp * (size_t)c.out_dim);
+        ALLOC(m->mp_bo, c.out_dim);
+        return TB2_OK;
+    };
+    switch (c.pool_type) {
+        case TB2_POOL_NONE:
+            break;
+        case TB2_POOL_SOCIAL:
+            ALLOC(m->WencT, m->H * m->C);
+            ALLOC(m->benc, m->C);
+            [[fallthrough]];
+        case TB2_POOL_OCCUPANCY:
+        case TB2_POOL_DIRECTIONAL:
+            if (m->n_mlp == 0) break;
+            ALLOC(m->Wt1, (size_t)m->cells * m->C * m->mlp_dims[1]);
+            ALLOC(m->base1, m->mlp_dims[1]);
+            if (c.pool_type == TB2_POOL_SOCIAL && m->C == 16 && !no_tc) {
+                const size_t half = ((size_t)m->cells * 16 * m->mlp_dims[1] + 1) / 2;
                 float *hi, *lo;
-                ALLOC(hi, half);
-                ALLOC(lo, half);
-                m->W_hi[1] = hi;
-                m->W_lo[1] = lo;
+                ALLOC(hi, 2 * half);      // interleaved (hi | lo) slabs
+                ALLOC(lo, 4);
+                m->Wt1_hi = hi;
+                m->Wt1_lo = lo;
             }
-        }
+            for (int layer = 1; layer < m->n_mlp; ++layer) {
+                ALLOC(m->WT[layer], (size_t)m->mlp_dims[layer] * m->mlp_dims[layer + 1]);
+                ALLOC(m->bl[layer], m->mlp_dims[layer + 1]);
+                if (layer == 1 && !no_tc && dense_tc_supported(m->mlp_dims[1], m->mlp_dims[2])) {
+                    const size_t half = ((size_t)m->mlp_dims[1] * m->mlp_dims[2] + 1) / 2;   // bf16 pairs in float units
+                    float *hi, *lo;
+                    ALLOC(hi, half);
+                    ALLOC(lo, half);
+                    m->W_hi[1] = hi;
+                    m->W_lo[1] = lo;
+                }
+            }
+            break;
+        case TB2_POOL_NN_LSTM:
+            if ((rc = encoder_lstm())) return rc;
+            [[fallthrough]];
+        case TB2_POOL_NN_MLP:
+            ALLOC(m->mp_Ws, c.mlp_dim_spatial * 4);
+            ALLOC(m->mp_bs, c.mlp_dim_spatial);
+            break;
+        case TB2_POOL_TRAJECTRON:
+            ALLOC(m->mp_Ws, (size_t)c.out_dim * 8);
+            ALLOC(m->mp_bs, c.out_dim);
+            if ((rc = encoder_lstm())) return rc;
+            break;
+        case TB2_POOL_ATTN_MLP:
+            ALLOC(m->at_AqT, D * D);
+            ALLOC(m->at_Ak, D * D);
+            ALLOC(m->at_AvT, D * D);
+            ALLOC(m->at_bqkv, 3 * D);
+            ALLOC(m->at_WoT, D * D);
+            ALLOC(m->at_bo, D);
+            [[fallthrough]];
+        case TB2_POOL_HIDDEN_MLP:      // spatial / velocity / hidden embeddings + out projection
+            ALLOC(m->mp_Ws, c.mlp_dim_spatial * 2);
+            ALLOC(m->mp_bs, c.mlp_dim_spatial);
+            ALLOC(m->mp_Wv, std::max(c.mlp_dim_vel, 1) * 2);
+            ALLOC(m->mp_bv, std::max(c.mlp_dim_vel, 1));
+            ALLOC(m->mp_WhT, (size_t)m->H * std::max(c.mlp_dim_hidden, 1));
+            ALLOC(m->mp_bh, std::max(c.mlp_dim_hidden, 1));
+            ALLOC(m->mp_WoT, D * c.out_dim);
+            ALLOC(m->mp_bo, c.out_dim);
+            break;
     }
 #undef ALLOC
+    return TB2_OK;
+}
+
+int tb2_lstm_create(const tb2_lstm_config* cfg, tb2_lstm** out) {
+    TB2_REQUIRE(cfg && out, "null argument");
+    *out = nullptr;
+    if (!hidden_dim_supported(cfg->hidden_dim)) {
+        set_error(kHiddenDimMessage);
+        return TB2_ERR_UNSUPPORTED;
+    }
+    TB2_REQUIRE(cfg->embedding_dim >= 4 && cfg->embedding_dim <= 1024, "embedding_dim out of range");
+    TB2_REQUIRE(cfg->pool_type >= TB2_POOL_NONE && cfg->pool_type <= TB2_POOL_TRAJECTRON, "bad pool_type");
+    tb2_lstm* m = new (std::nothrow) tb2_lstm();
+    TB2_REQUIRE(m, "out of host memory");
+    m->cfg = *cfg;
+    m->H = cfg->hidden_dim;
+    m->E = cfg->embedding_dim;
+    m->tc_disabled = tensor_cores_disabled();
+    int rc = configure_pool(*cfg, m);
+    if (rc == TB2_OK) {
+        m->K_gate = m->E + m->P + m->H;
+        m->K_gate_pad = (m->K_gate + kGateBK - 1) / kGateBK * kGateBK;
+        rc = alloc_buffers(m);
+    }
+    if (rc != TB2_OK) {
+        tb2_lstm_destroy(m);
+        return rc;
+    }
     *out = m;
     return TB2_OK;
 }
@@ -527,15 +549,7 @@ int tb2_pool_forward(const tb2_lstm* m, const tb2_layout* l, const float* hidden
     Workspace ws;
     carve_workspace(m, l, workspace, &ws);
     cudaStream_t st = (cudaStream_t)stream;
-    if (m->cfg.pool_type == TB2_POOL_HIDDEN_MLP) return launch_hidden_mlp_pool(m, l, hidden, obs1, obs2, pooled_out, st);
-    if (m->cfg.pool_type == TB2_POOL_NN_MLP) return launch_nn_mlp_pool(m, l, obs1, obs2, pooled_out, st);
-    if (m->cfg.pool_type == TB2_POOL_NN_LSTM || m->cfg.pool_type == TB2_POOL_TRAJECTRON) {      // stateful: advances the LSTM state kept in the workspace
-        if (m->cfg.pool_type == TB2_POOL_NN_LSTM) rc = launch_nn_mlp_pool(m, l, obs1, obs2, ws.pool_feat, st);
-        else rc = launch_trajectron_feat(m, l, obs1, obs2, ws.scene_sum, ws.pool_feat, st);
-        if (rc) return rc;
-        return launch_pool_lstm_cell(m, l, ws.pool_feat, ws.pool_h, ws.pool_c, pooled_out, st);
-    }
-    if (m->cfg.pool_type == TB2_POOL_ATTN_MLP) return launch_attn_mlp_pool(m, l, hidden, obs1, obs2, pooled_out, st);
+    if (m->cfg.pool_type >= TB2_POOL_HIDDEN_MLP) return launch_nongrid_pool(m, l, hidden, obs1, obs2, &ws, pooled_out, st);
     if ((rc = launch_pool_prepare(m, l, hidden, obs1, obs2, 0, 0, 0, &ws, st))) return rc;
     return launch_pool_mlp(m, l, &ws, pooled_out, nullptr, nullptr, st);
 }
@@ -549,16 +563,8 @@ static int step_impl(const tb2_lstm* m, const tb2_layout* l, int phase, const fl
     const bool tc = m->Wg_hi[0] != nullptr;
     const float* pooled = nullptr;
     if (m->cfg.pool_type >= TB2_POOL_HIDDEN_MLP) {
-        // non-grid interaction module: one kernel per scene -> pooled fp32, split for the tensor-core gate kernel
-        if (m->cfg.pool_type == TB2_POOL_NN_MLP) rc = launch_nn_mlp_pool(m, l, obs1, obs2, ws->pooled, st);
-        else if (m->cfg.pool_type == TB2_POOL_NN_LSTM || m->cfg.pool_type == TB2_POOL_TRAJECTRON) {
-            if (m->cfg.pool_type == TB2_POOL_NN_LSTM) rc = launch_nn_mlp_pool(m, l, obs1, obs2, ws->pool_feat, st);
-            else rc = launch_trajectron_feat(m, l, obs1, obs2, ws->scene_sum, ws->pool_feat, st);
-            if (!rc) rc = launch_pool_lstm_cell(m, l, ws->pool_feat, ws->pool_h, ws->pool_c, ws->pooled, st);
-        }
-        else if (m->cfg.pool_type == TB2_POOL_ATTN_MLP) rc = launch_attn_mlp_pool(m, l, h_in, obs1, obs2, ws->pooled, st);
-        else rc = launch_hidden_mlp_pool(m, l, h_in, obs1, obs2, ws->pooled, st);
-        if (rc) return rc;
+        // pooled fp32, split for the tensor-core gate kernel
+        if ((rc = launch_nongrid_pool(m, l, h_in, obs1, obs2, ws, ws->pooled, st))) return rc;
         if (tc && (rc = launch_split_bf16(ws->pooled, ws->pool_hi, ws->pool_lo, (size_t)l->M * m->P, st))) return rc;
         pooled = ws->pooled;
     } else

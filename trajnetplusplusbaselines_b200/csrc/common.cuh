@@ -133,41 +133,42 @@ constexpr int kGateBK = 16;        // K-chunk of the gate GEMM; weight rows are 
 
 // Opaque handle bodies ---------------------------------------------------------------------
 struct tb2_lstm {
-    tb2_lstm_config cfg;
-    int H, E, C, cells, n_mlp;
-    int P;                 // pooled width fed to the LSTM input (0 if none / pool_to_input == 0)
-    int pool_out;          // width of the pool output (grid width when n_mlp == 0)
-    int mlp_dims[tb2::kMaxMlpLayers + 1];  // [grid_dim, d1, ..]
-    int K_gate, K_gate_pad;
-    bool weights_set;
-    bool tc_disabled;      // TB2_DISABLE_TC=1 at creation: every kernel choice takes the fp32 FFMA version
+    tb2_lstm_config cfg = {};
+    int H = 0, E = 0, C = 0, cells = 0, n_mlp = 0;
+    int P = 0;             // pooled width fed to the LSTM input (0 if none / pool_to_input == 0)
+    int pool_out = 0;      // width of the pool output (grid width when n_mlp == 0)
+    int mlp_dims[tb2::kMaxMlpLayers + 1] = {};  // [grid_dim, d1, ..]
+    int K_gate = 0, K_gate_pad = 0;
+    bool weights_set = false;
+    bool tc_disabled = false;   // TB2_DISABLE_TC=1 at creation: every kernel choice takes the fp32 FFMA version
     // device buffers (owned)
-    float* We;             // [E-2, 2]
-    float* be;             // [E-2]
-    float* WgT[2];         // [K_gate_pad, 4H]  rows: emb | pooled | h
-    float* bg[2];          // [4H] = b_ih + b_hh
-    float* Wn;             // [5, H]
-    float* bn;             // [5]
-    float* WencT;          // [H, C]
-    float* benc;           // [C]
-    float* Wt1;            // [cells, C, d1]  cell-major slabs of pool.embedding.0.weight
-    float* base1;          // [d1] = b1 + constant * rowsum(W1)
-    void* Wt1_hi;          // social, C == 16: bf16 [cells, d1, 16] (hi, lo) slabs for sparse_layer1_mma
-    void* Wt1_lo;
-    float* WT[tb2::kMaxMlpLayers];   // layers >= 2: [K, N] transposed
-    float* bl[tb2::kMaxMlpLayers];   // biases of layers >= 2
-    void* W_hi[tb2::kMaxMlpLayers];  // [1] only (second Linear): bf16 [N, K] (hi, lo) split for the wgmma path (null: FFMA path)
-    void* W_lo[tb2::kMaxMlpLayers];
+    float* We = nullptr;        // [E-2, 2]
+    float* be = nullptr;        // [E-2]
+    float* WgT[2] = {};         // [K_gate_pad, 4H]  rows: emb | pooled | h
+    float* bg[2] = {};          // [4H] = b_ih + b_hh
+    float* Wn = nullptr;        // [5, H]
+    float* bn = nullptr;        // [5]
+    float* WencT = nullptr;     // [H, C]
+    float* benc = nullptr;      // [C]
+    float* Wt1 = nullptr;       // [cells, C, d1]  cell-major slabs of pool.embedding.0.weight
+    float* base1 = nullptr;     // [d1] = b1 + constant * rowsum(W1)
+    void* Wt1_hi = nullptr;     // social, C == 16: bf16 [cells, d1, 16] (hi, lo) slabs for sparse_layer1_mma
+    void* Wt1_lo = nullptr;
+    float* WT[tb2::kMaxMlpLayers] = {};   // layers >= 2: [K, N] transposed
+    float* bl[tb2::kMaxMlpLayers] = {};   // biases of layers >= 2
+    void* W_hi[tb2::kMaxMlpLayers] = {};  // [1] only (second Linear): bf16 [N, K] (hi, lo) split for the wgmma path (null: FFMA path)
+    void* W_lo[tb2::kMaxMlpLayers] = {};
     std::vector<cudaEvent_t> step_events;     // tb2_lstm_forward_sequence_host: one event per recurrence step
     // HiddenStateMLPPooling (TB2_POOL_HIDDEN_MLP)
-    float *mp_Ws, *mp_bs, *mp_Wv, *mp_bv, *mp_WhT, *mp_bh, *mp_WoT, *mp_bo;
+    float *mp_Ws = nullptr, *mp_bs = nullptr, *mp_Wv = nullptr, *mp_bv = nullptr, *mp_WhT = nullptr, *mp_bh = nullptr,
+          *mp_WoT = nullptr, *mp_bo = nullptr;
     // AttentionMLPPooling (TB2_POOL_ATTN_MLP): in-projection . wq / wk / wv combined, q and v transposed [E in][E out],
     // k [E out][E in]; biases, out-projection transposed
-    float *at_AqT, *at_Ak, *at_AvT, *at_bqkv, *at_WoT, *at_bo;
+    float *at_AqT = nullptr, *at_Ak = nullptr, *at_AvT = nullptr, *at_bqkv = nullptr, *at_WoT = nullptr, *at_bo = nullptr;
     // NearestNeighborLSTM (TB2_POOL_NN_LSTM): interaction-encoder LSTMCell, weights transposed [in][4 Hp], fused bias
-    float *pl_WihT, *pl_WhhT, *pl_b;
-    void* Wg_hi[2];        // gate weights [4H (rank, gate, unit), K_gate] bf16 split (null: FFMA gates)
-    void* Wg_lo[2];
+    float *pl_WihT = nullptr, *pl_WhhT = nullptr, *pl_b = nullptr;
+    void* Wg_hi[2] = {};        // gate weights [4H (rank, gate, unit), K_gate] bf16 split (null: FFMA gates)
+    void* Wg_lo[2] = {};
     std::vector<void*> owned;
 };
 

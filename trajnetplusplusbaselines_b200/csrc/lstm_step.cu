@@ -394,6 +394,48 @@ static int copy_dev(const float* src, float* dst, size_t n, cudaStream_t st) {
     return TB2_OK;
 }
 
+// Interaction-encoder LSTMCell and hidden2pool of NearestNeighborLSTM / TrajectronPooling
+static int upload_encoder_lstm(tb2_lstm* m, const tb2_lstm_weights* w, cudaStream_t st) {
+    const tb2_lstm_config& c = m->cfg;
+    const int Hp = c.mlp_dim_hidden;
+    TB2_REQUIRE(w->pool_lstm_weight_ih && w->pool_lstm_weight_hh && w->pool_lstm_bias_ih && w->pool_lstm_bias_hh &&
+                w->pool_out_weight && w->pool_out_bias, "pool.pool_lstm / pool.hidden2pool parameters missing");
+    transpose_kernel<<<256, 256, 0, st>>>(w->pool_lstm_weight_ih, m->pl_WihT, 4 * Hp, c.out_dim);
+    TB2_LAUNCH_CHECK();
+    transpose_kernel<<<256, 256, 0, st>>>(w->pool_lstm_weight_hh, m->pl_WhhT, 4 * Hp, Hp);
+    TB2_LAUNCH_CHECK();
+    add_bias_kernel<<<(4 * Hp + 255) / 256, 256, 0, st>>>(w->pool_lstm_bias_ih, w->pool_lstm_bias_hh, m->pl_b, 4 * Hp);
+    TB2_LAUNCH_CHECK();
+    transpose_kernel<<<128, 256, 0, st>>>(w->pool_out_weight, m->mp_WoT, c.out_dim, Hp);
+    TB2_LAUNCH_CHECK();
+    return copy_dev(w->pool_out_bias, m->mp_bo, (size_t)c.out_dim, st);
+}
+
+// Spatial / velocity / hidden-state embeddings and out projection of HiddenStateMLPPooling / AttentionMLPPooling
+static int upload_embeddings(tb2_lstm* m, const tb2_lstm_weights* w, cudaStream_t st) {
+    const tb2_lstm_config& c = m->cfg;
+    const int D = c.mlp_dim_spatial + c.mlp_dim_vel + c.mlp_dim_hidden;
+    TB2_REQUIRE(w->pool_spatial_weight && w->pool_spatial_bias && w->pool_out_weight && w->pool_out_bias,
+                "pool.spatial_embedding / pool.out_projection missing");
+    TB2_REQUIRE(c.mlp_dim_vel == 0 || (w->pool_vel_weight && w->pool_vel_bias), "pool.vel_embedding missing");
+    TB2_REQUIRE(c.mlp_dim_hidden == 0 || (w->pool_hidden_weight && w->pool_hidden_bias), "pool.hidden_embedding missing");
+    int rc;
+    if ((rc = copy_dev(w->pool_spatial_weight, m->mp_Ws, (size_t)c.mlp_dim_spatial * 2, st))) return rc;
+    if ((rc = copy_dev(w->pool_spatial_bias, m->mp_bs, (size_t)c.mlp_dim_spatial, st))) return rc;
+    if (c.mlp_dim_vel) {
+        if ((rc = copy_dev(w->pool_vel_weight, m->mp_Wv, (size_t)c.mlp_dim_vel * 2, st))) return rc;
+        if ((rc = copy_dev(w->pool_vel_bias, m->mp_bv, (size_t)c.mlp_dim_vel, st))) return rc;
+    }
+    if (c.mlp_dim_hidden) {
+        transpose_kernel<<<64, 256, 0, st>>>(w->pool_hidden_weight, m->mp_WhT, c.mlp_dim_hidden, m->H);
+        TB2_LAUNCH_CHECK();
+        if ((rc = copy_dev(w->pool_hidden_bias, m->mp_bh, (size_t)c.mlp_dim_hidden, st))) return rc;
+    }
+    transpose_kernel<<<128, 256, 0, st>>>(w->pool_out_weight, m->mp_WoT, c.out_dim, D);
+    TB2_LAUNCH_CHECK();
+    return copy_dev(w->pool_out_bias, m->mp_bo, (size_t)c.out_dim, st);
+}
+
 int launch_repack(tb2_lstm* m, const tb2_lstm_weights* w, cudaStream_t st) {
     TB2_REQUIRE(w->input_embedding_weight && w->input_embedding_bias, "input embedding weights missing");
     TB2_REQUIRE(w->encoder_weight_ih && w->encoder_weight_hh && w->encoder_bias_ih && w->encoder_bias_hh,
@@ -418,99 +460,76 @@ int launch_repack(tb2_lstm* m, const tb2_lstm_weights* w, cudaStream_t st) {
             (rc = launch_repack_gates_tc(wih[ph], whh[ph], m->Wg_hi[ph], m->Wg_lo[ph], m->E + m->P, m->H, st)))
             return rc;
     }
-    if (m->cfg.pool_type == TB2_POOL_TRAJECTRON) {
-        TB2_REQUIRE(w->pool_spatial_weight && w->pool_spatial_bias, "pool.embedding.0 (Trajectron pooling) missing");
-        if ((rc = copy_dev(w->pool_spatial_weight, m->mp_Ws, (size_t)m->cfg.out_dim * 8, st))) return rc;
-        if ((rc = copy_dev(w->pool_spatial_bias, m->mp_bs, (size_t)m->cfg.out_dim, st))) return rc;
-    }
-    if (m->cfg.pool_type == TB2_POOL_NN_LSTM || m->cfg.pool_type == TB2_POOL_TRAJECTRON) {
-        const tb2_lstm_config& c = m->cfg;
-        const int Hp = c.mlp_dim_hidden;
-        TB2_REQUIRE(w->pool_lstm_weight_ih && w->pool_lstm_weight_hh && w->pool_lstm_bias_ih && w->pool_lstm_bias_hh &&
-                    w->pool_out_weight && w->pool_out_bias, "pool.pool_lstm / pool.hidden2pool parameters missing");
-        transpose_kernel<<<256, 256, 0, st>>>(w->pool_lstm_weight_ih, m->pl_WihT, 4 * Hp, c.out_dim);
-        TB2_LAUNCH_CHECK();
-        transpose_kernel<<<256, 256, 0, st>>>(w->pool_lstm_weight_hh, m->pl_WhhT, 4 * Hp, Hp);
-        TB2_LAUNCH_CHECK();
-        add_bias_kernel<<<(4 * Hp + 255) / 256, 256, 0, st>>>(w->pool_lstm_bias_ih, w->pool_lstm_bias_hh, m->pl_b, 4 * Hp);
-        TB2_LAUNCH_CHECK();
-        transpose_kernel<<<128, 256, 0, st>>>(w->pool_out_weight, m->mp_WoT, c.out_dim, Hp);
-        TB2_LAUNCH_CHECK();
-        if ((rc = copy_dev(w->pool_out_bias, m->mp_bo, (size_t)c.out_dim, st))) return rc;
-    }
-    if (m->cfg.pool_type == TB2_POOL_NN_MLP || m->cfg.pool_type == TB2_POOL_NN_LSTM) {
-        const tb2_lstm_config& c = m->cfg;
-        TB2_REQUIRE(w->pool_spatial_weight && w->pool_spatial_bias, "pool.embedding.0 (nearest-neighbour pooling) missing");
-        if ((rc = copy_dev(w->pool_spatial_weight, m->mp_Ws, (size_t)c.mlp_dim_spatial * (c.mlp_dim_vel ? 4 : 2), st))) return rc;
-        if ((rc = copy_dev(w->pool_spatial_bias, m->mp_bs, (size_t)c.mlp_dim_spatial, st))) return rc;
-    }
-    if (m->cfg.pool_type == TB2_POOL_ATTN_MLP) {
-        const int Ea = m->cfg.mlp_dim_spatial + m->cfg.mlp_dim_vel + m->cfg.mlp_dim_hidden;
-        TB2_REQUIRE(w->pool_attn_wq && w->pool_attn_wk && w->pool_attn_wv && w->pool_attn_in_proj_weight &&
-                    w->pool_attn_in_proj_bias && w->pool_attn_out_proj_weight && w->pool_attn_out_proj_bias,
-                    "pool.wq / wk / wv / multihead_attn parameters missing");
-        // in-projection . w{q,k,v}: A[o][c] = sum_m Win[o][m] w[m][c], stored transposed [c][o] for q and v, [o][c] for k
-        // (attn_mlp_pool_kernel reads Ak^T q with a lane per c)
-        const float* wqkv[3] = {w->pool_attn_wq, w->pool_attn_wk, w->pool_attn_wv};
-        float* outA[3] = {m->at_AqT, m->at_Ak, m->at_AvT};
-        for (int i = 0; i < 3; ++i) {
-            combine_proj_kernel<<<(Ea * Ea + 255) / 256, 256, 0, st>>>(w->pool_attn_in_proj_weight + (size_t)i * Ea * Ea, wqkv[i],
-                                                                     outA[i], Ea, i == 1);
+    const tb2_lstm_config& c = m->cfg;
+    switch (c.pool_type) {
+        case TB2_POOL_NONE:
+            break;
+        case TB2_POOL_SOCIAL:
+            TB2_REQUIRE(w->pool_encoding_weight && w->pool_encoding_bias, "pool.hidden_dim_encoding missing");
+            transpose_kernel<<<64, 256, 0, st>>>(w->pool_encoding_weight, m->WencT, m->C, m->H);
             TB2_LAUNCH_CHECK();
-        }
-        if ((rc = copy_dev(w->pool_attn_in_proj_bias, m->at_bqkv, (size_t)3 * Ea, st))) return rc;
-        transpose_kernel<<<64, 256, 0, st>>>(w->pool_attn_out_proj_weight, m->at_WoT, Ea, Ea);
-        TB2_LAUNCH_CHECK();
-        if ((rc = copy_dev(w->pool_attn_out_proj_bias, m->at_bo, (size_t)Ea, st))) return rc;
-    }
-    if (m->cfg.pool_type == TB2_POOL_HIDDEN_MLP || m->cfg.pool_type == TB2_POOL_ATTN_MLP) {
-        const tb2_lstm_config& c = m->cfg;
-        const int D = c.mlp_dim_spatial + c.mlp_dim_vel + c.mlp_dim_hidden;
-        TB2_REQUIRE(w->pool_spatial_weight && w->pool_spatial_bias && w->pool_out_weight && w->pool_out_bias,
-                    "pool.spatial_embedding / pool.out_projection missing");
-        TB2_REQUIRE(c.mlp_dim_vel == 0 || (w->pool_vel_weight && w->pool_vel_bias), "pool.vel_embedding missing");
-        TB2_REQUIRE(c.mlp_dim_hidden == 0 || (w->pool_hidden_weight && w->pool_hidden_bias), "pool.hidden_embedding missing");
-        if ((rc = copy_dev(w->pool_spatial_weight, m->mp_Ws, (size_t)c.mlp_dim_spatial * 2, st))) return rc;
-        if ((rc = copy_dev(w->pool_spatial_bias, m->mp_bs, (size_t)c.mlp_dim_spatial, st))) return rc;
-        if (c.mlp_dim_vel) {
-            if ((rc = copy_dev(w->pool_vel_weight, m->mp_Wv, (size_t)c.mlp_dim_vel * 2, st))) return rc;
-            if ((rc = copy_dev(w->pool_vel_bias, m->mp_bv, (size_t)c.mlp_dim_vel, st))) return rc;
-        }
-        if (c.mlp_dim_hidden) {
-            transpose_kernel<<<64, 256, 0, st>>>(w->pool_hidden_weight, m->mp_WhT, c.mlp_dim_hidden, m->H);
+            if ((rc = copy_dev(w->pool_encoding_bias, m->benc, (size_t)m->C, st))) return rc;
+            [[fallthrough]];
+        case TB2_POOL_OCCUPANCY:
+        case TB2_POOL_DIRECTIONAL:
+            if (m->n_mlp == 0) break;
+            TB2_REQUIRE(w->pool_embedding_weight[0] && w->pool_embedding_bias[0], "pool.embedding.0 missing");
+            repack_layer1_kernel<<<1024, 256, 0, st>>>(w->pool_embedding_weight[0], w->pool_embedding_bias[0],
+                                                       m->Wt1, m->base1, m->mlp_dims[1], m->C, m->cells, c.constant);
             TB2_LAUNCH_CHECK();
-            if ((rc = copy_dev(w->pool_hidden_bias, m->mp_bh, (size_t)c.mlp_dim_hidden, st))) return rc;
-        }
-        transpose_kernel<<<128, 256, 0, st>>>(w->pool_out_weight, m->mp_WoT, c.out_dim, D);
-        TB2_LAUNCH_CHECK();
-        if ((rc = copy_dev(w->pool_out_bias, m->mp_bo, (size_t)c.out_dim, st))) return rc;
-    }
-    if (m->cfg.pool_type == TB2_POOL_SOCIAL) {
-        TB2_REQUIRE(w->pool_encoding_weight && w->pool_encoding_bias, "pool.hidden_dim_encoding missing");
-        transpose_kernel<<<64, 256, 0, st>>>(w->pool_encoding_weight, m->WencT, m->C, m->H);
-        TB2_LAUNCH_CHECK();
-        if ((rc = copy_dev(w->pool_encoding_bias, m->benc, (size_t)m->C, st))) return rc;
-    }
-    if (m->cfg.pool_type != TB2_POOL_NONE && m->cfg.pool_type < TB2_POOL_HIDDEN_MLP && m->n_mlp >= 1) {
-        TB2_REQUIRE(w->pool_embedding_weight[0] && w->pool_embedding_bias[0], "pool.embedding.0 missing");
-        repack_layer1_kernel<<<1024, 256, 0, st>>>(w->pool_embedding_weight[0], w->pool_embedding_bias[0],
-                                                   m->Wt1, m->base1, m->mlp_dims[1], m->C, m->cells,
-                                                   m->cfg.constant);
-        TB2_LAUNCH_CHECK();
-        if (m->Wt1_hi &&
-            (rc = launch_repack_layer1_mma(w->pool_embedding_weight[0], m->Wt1_hi, m->Wt1_lo, m->mlp_dims[1], m->cells, st)))
-            return rc;
-        for (int layer = 1; layer < m->n_mlp; ++layer) {
-            TB2_REQUIRE(w->pool_embedding_weight[layer] && w->pool_embedding_bias[layer], "pool.embedding layer missing");
-            transpose_kernel<<<512, 256, 0, st>>>(w->pool_embedding_weight[layer], m->WT[layer],
-                                                  m->mlp_dims[layer + 1], m->mlp_dims[layer]);
-            TB2_LAUNCH_CHECK();
-            if ((rc = copy_dev(w->pool_embedding_bias[layer], m->bl[layer], (size_t)m->mlp_dims[layer + 1], st))) return rc;
-            if (m->W_hi[layer] &&
-                (rc = launch_split_bf16(w->pool_embedding_weight[layer], m->W_hi[layer], m->W_lo[layer],
-                                        (size_t)m->mlp_dims[layer] * m->mlp_dims[layer + 1], st)))
+            if (m->Wt1_hi &&
+                (rc = launch_repack_layer1_mma(w->pool_embedding_weight[0], m->Wt1_hi, m->Wt1_lo, m->mlp_dims[1], m->cells, st)))
                 return rc;
+            for (int layer = 1; layer < m->n_mlp; ++layer) {
+                TB2_REQUIRE(w->pool_embedding_weight[layer] && w->pool_embedding_bias[layer], "pool.embedding layer missing");
+                transpose_kernel<<<512, 256, 0, st>>>(w->pool_embedding_weight[layer], m->WT[layer],
+                                                      m->mlp_dims[layer + 1], m->mlp_dims[layer]);
+                TB2_LAUNCH_CHECK();
+                if ((rc = copy_dev(w->pool_embedding_bias[layer], m->bl[layer], (size_t)m->mlp_dims[layer + 1], st))) return rc;
+                if (m->W_hi[layer] &&
+                    (rc = launch_split_bf16(w->pool_embedding_weight[layer], m->W_hi[layer], m->W_lo[layer],
+                                            (size_t)m->mlp_dims[layer] * m->mlp_dims[layer + 1], st)))
+                    return rc;
+            }
+            break;
+        case TB2_POOL_NN_LSTM:
+            if ((rc = upload_encoder_lstm(m, w, st))) return rc;
+            [[fallthrough]];
+        case TB2_POOL_NN_MLP:
+            TB2_REQUIRE(w->pool_spatial_weight && w->pool_spatial_bias, "pool.embedding.0 (nearest-neighbour pooling) missing");
+            if ((rc = copy_dev(w->pool_spatial_weight, m->mp_Ws, (size_t)c.mlp_dim_spatial * (c.mlp_dim_vel ? 4 : 2), st))) return rc;
+            if ((rc = copy_dev(w->pool_spatial_bias, m->mp_bs, (size_t)c.mlp_dim_spatial, st))) return rc;
+            break;
+        case TB2_POOL_TRAJECTRON:
+            TB2_REQUIRE(w->pool_spatial_weight && w->pool_spatial_bias, "pool.embedding.0 (Trajectron pooling) missing");
+            if ((rc = copy_dev(w->pool_spatial_weight, m->mp_Ws, (size_t)c.out_dim * 8, st))) return rc;
+            if ((rc = copy_dev(w->pool_spatial_bias, m->mp_bs, (size_t)c.out_dim, st))) return rc;
+            if ((rc = upload_encoder_lstm(m, w, st))) return rc;
+            break;
+        case TB2_POOL_ATTN_MLP: {
+            const int Ea = c.mlp_dim_spatial + c.mlp_dim_vel + c.mlp_dim_hidden;
+            TB2_REQUIRE(w->pool_attn_wq && w->pool_attn_wk && w->pool_attn_wv && w->pool_attn_in_proj_weight &&
+                        w->pool_attn_in_proj_bias && w->pool_attn_out_proj_weight && w->pool_attn_out_proj_bias,
+                        "pool.wq / wk / wv / multihead_attn parameters missing");
+            // in-projection . w{q,k,v}: A[o][c] = sum_m Win[o][m] w[m][c], stored transposed [c][o] for q and v, [o][c] for k
+            // (attn_mlp_pool_kernel reads Ak^T q with a lane per c)
+            const float* wqkv[3] = {w->pool_attn_wq, w->pool_attn_wk, w->pool_attn_wv};
+            float* outA[3] = {m->at_AqT, m->at_Ak, m->at_AvT};
+            for (int i = 0; i < 3; ++i) {
+                combine_proj_kernel<<<(Ea * Ea + 255) / 256, 256, 0, st>>>(w->pool_attn_in_proj_weight + (size_t)i * Ea * Ea,
+                                                                         wqkv[i], outA[i], Ea, i == 1);
+                TB2_LAUNCH_CHECK();
+            }
+            if ((rc = copy_dev(w->pool_attn_in_proj_bias, m->at_bqkv, (size_t)3 * Ea, st))) return rc;
+            transpose_kernel<<<64, 256, 0, st>>>(w->pool_attn_out_proj_weight, m->at_WoT, Ea, Ea);
+            TB2_LAUNCH_CHECK();
+            if ((rc = copy_dev(w->pool_attn_out_proj_bias, m->at_bo, (size_t)Ea, st))) return rc;
+            if ((rc = upload_embeddings(m, w, st))) return rc;
+            break;
         }
+        case TB2_POOL_HIDDEN_MLP:
+            if ((rc = upload_embeddings(m, w, st))) return rc;
+            break;
     }
     m->weights_set = true;
     return TB2_OK;

@@ -96,21 +96,111 @@ class LayoutCache:
         return item
 
 
-def plug_getstate(module):
-    """`__getstate__` of the pooling modules: the per-process device handles of the stand-alone plug path (model
-    handle, layouts, zero LSTM-cell weights, interaction-encoder state bookkeeping) are never pickled
-    (LSTMPredictor.save pickles the whole model, lstm.py:270-277); they are rebuilt lazily after loading."""
-    state = module.__dict__.copy()
-    state.pop('_compiled_call_impl', None)         # like torch.nn.Module.__getstate__
-    if '_handle' in state:
+def lstm_config(hidden_dim, embedding_dim, pool_to_input, pool):
+    """tb2_lstm_config of an LSTM of these widths around the interaction module `pool` (None: no pooling)."""
+    cfg = _lib.LstmConfig()
+    cfg.hidden_dim = int(hidden_dim)
+    cfg.embedding_dim = int(embedding_dim)
+    cfg.pool_to_input = int(bool(pool_to_input))
+    cfg.pool_type = _lib.POOL_NONE
+    cfg.pool_size = cfg.blur_size = 1
+    if pool is not None:
+        pool.fill_config(cfg)
+    return cfg
+
+
+class PoolPlug(torch.nn.Module):
+    """Base of the interaction modules (GridBasedPooling and the non-grid modules).
+
+    Inside `LSTM.forward` a module is not called: the fused sequence entry point reads its configuration
+    (`fill_config`) and parameters (`weight_fields`).  Called on its own, the module is the reference's pool plug,
+    `(hidden_states [B, N, H], obs1 [B, N, 2], obs2 [B, N, 2]) -> [B * N, width]`, run through a model handle of its
+    own (tb2_pool_forward) whose LSTM-cell slots hold zeros: tb2_lstm_set_weights requires them, the pool never
+    reads them."""
+    _reads_hidden = False       # the plug reads hidden states (and its handle's LSTM width is theirs)
+    stateful = False            # carries an LSTM state of its own through the time loop, kept in the engine's workspace
+
+    def __init__(self):
+        super().__init__()
+        self._handle = None
+        self._layouts = LayoutCache()
+
+    def __getstate__(self):
+        """The per-process device handles of the plug (model handle, layouts, zero LSTM-cell weights,
+        interaction-encoder state bookkeeping) are never pickled (LSTMPredictor.save pickles the whole model,
+        lstm.py:270-277); they are rebuilt lazily after loading."""
+        state = self.__dict__.copy()
+        state.pop('_compiled_call_impl', None)         # like torch.nn.Module.__getstate__
         state['_handle'] = None
-    if '_layouts' in state:
         state['_layouts'] = LayoutCache()
-    state.pop('_standalone_dummy', None)
-    state.pop('_state_tracks', None)
-    if '_reset_pending' in state:
-        state['_reset_pending'] = True
-    return state
+        state.pop('_standalone_dummy', None)
+        state.pop('_state_tracks', None)
+        if '_reset_pending' in state:
+            state['_reset_pending'] = True
+        return state
+
+    def weights_version(self):
+        return weights_key(self)
+
+    def reset(self, num_tracks, max_num_neigh, device):
+        """The reference resets per-call pool state here; a stateless module keeps none."""
+        self.track_mask = None
+
+    def _plug_width(self):
+        """LSTM width of the plug's handle: that of the hidden states it reads, else any supported width."""
+        return int(self.hidden_dim) if self._reads_hidden else 128
+
+    def _plug_out_dim(self):
+        """Width of the plug's output."""
+        return int(self.out_dim)
+
+    def _plug_device(self, obs1):
+        device = next(self.parameters()).device
+        if device.type != 'cuda':
+            raise RuntimeError("%s runs on CUDA only: move the module to the GPU (module.cuda())" % type(self).__name__)
+        return device
+
+    def _plug_state(self, handle, layout):
+        """Bookkeeping of a stateful module before a plug call."""
+
+    def _plug_handle(self, device):
+        """The plug's model handle on `device` with the module's current weights."""
+        if self._handle is None or self._handle.device != device:
+            self._handle = ModelHandle(lstm_config(self._plug_width(), 64, True, self), device)
+            self._standalone_dummy = None
+        if getattr(self, '_standalone_dummy', None) is None:
+            z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=device)
+            H, in_dim = self._plug_width(), 64 + self._plug_out_dim()
+            self._standalone_dummy = dict(
+                input_embedding_weight=z(62, 2), input_embedding_bias=z(62),
+                encoder_weight_ih=z(4 * H, in_dim), encoder_weight_hh=z(4 * H, H),
+                encoder_bias_ih=z(4 * H), encoder_bias_hh=z(4 * H),
+                decoder_weight_ih=z(4 * H, in_dim), decoder_weight_hh=z(4 * H, H),
+                decoder_bias_ih=z(4 * H), decoder_bias_hh=z(4 * H),
+                hidden2normal_weight=z(5, H), hidden2normal_bias=z(5))
+        fields = dict(self._standalone_dummy)
+        fields.update(self.weight_fields())
+        self._handle.set_weights(fields, key=self.weights_version())
+        return self._handle
+
+    def forward(self, hidden_states, obs1, obs2):
+        """[B, N, H], [B, N, 2], [B, N, 2] -> [B * N, width] on the device of obs1."""
+        _lib.require_cuda()
+        batch_size, num_tracks = obs1.size(0), obs1.size(1)
+        device = self._plug_device(obs1)
+        if self._reads_hidden and hidden_states.size(-1) != self.hidden_dim:
+            raise ValueError("hidden_states width != hidden_dim")
+        handle = self._plug_handle(device)
+        layout = self._layouts.get(range(0, batch_size * num_tracks + 1, num_tracks), device=device)
+        self._plug_state(handle, layout)
+        f32 = dict(device=device, dtype=torch.float32)
+        o1 = obs1.detach().to(**f32).reshape(-1, 2).contiguous()
+        o2 = obs2.detach().to(**f32).reshape(-1, 2).contiguous()
+        hid = None
+        if self._reads_hidden:
+            hid = hidden_states.detach().to(**f32).reshape(batch_size * num_tracks, -1).contiguous()
+        out = handle.pool_forward(layout, hid, o1, o2, self._plug_out_dim())
+        return out.to(obs1.device) if obs1.device != device else out
 
 
 class ModelHandle:
@@ -152,20 +242,7 @@ class ModelHandle:
         if not force and key is not None and key == self._weights_key:
             return
         lib = _lib.load()
-        w = _lib.LstmWeights()
-        keep = []
-        for field, value in named.items():
-            if isinstance(value, (list, tuple)):
-                arr = getattr(w, field)
-                for i, t in enumerate(value):
-                    if t is not None:
-                        t = self._prep(t)
-                        keep.append(t)
-                        arr[i] = t.data_ptr()
-            elif value is not None:
-                t = self._prep(value)
-                keep.append(t)
-                setattr(w, field, t.data_ptr())
+        w, keep = self.weights_struct(named)
         with torch.cuda.device(self.device):
             _lib.check(lib.tb2_lstm_set_weights(self.handle, ctypes.byref(w), _stream(self.device)))
         # the repack kernels read `keep` asynchronously on the current stream; record usage

@@ -9,14 +9,14 @@ pool is not even called -- the fused sequence entry point consumes its parameter
 import torch
 
 from .. import _lib
-from ..engine import LayoutCache, ModelHandle, plug_getstate, weights_key
+from ..engine import PoolPlug
 
 _TYPES = {'occupancy': _lib.POOL_OCCUPANCY, 'directional': _lib.POOL_DIRECTIONAL,
           'social': _lib.POOL_SOCIAL}
 _ARCH_LAYERS = {'None': 0, None: 0, 'one_layer': 1, 'two_layer': 2, 'three_layer': 3}
 
 
-class GridBasedPooling(torch.nn.Module):
+class GridBasedPooling(PoolPlug):
     def __init__(self, cell_side=2.0, n=4, hidden_dim=128, out_dim=None,
                  type_='occupancy', pool_size=1, blur_size=1, front=False,
                  embedding_arch='one_layer', pretrained_pool_encoder=None,
@@ -74,13 +74,7 @@ class GridBasedPooling(torch.nn.Module):
                 mods += [torch.nn.Linear(dims[i], dims[i + 1]), torch.nn.ReLU()]
             self.embedding = torch.nn.Sequential(*mods)
 
-        self._handle = None
-        self._layouts = LayoutCache()
-
     # -- configuration shared with LSTM ---------------------------------------------------------
-    def __getstate__(self):
-        return plug_getstate(self)
-
     def fill_config(self, cfg):
         """Write the pooling fields of a tb2_lstm_config."""
         cfg.pool_type = _TYPES[self.type_]
@@ -108,18 +102,15 @@ class GridBasedPooling(torch.nn.Module):
             fields['pool_embedding_bias'] = [l.bias for l in linears]
         return fields
 
-    def weights_version(self):
-        return weights_key(self)
+    # -- the plug (gridbased_pooling.py:94-110; reset: the reference resets its dead pool-LSTM state, :345-351) -------
+    @property
+    def _reads_hidden(self):
+        return self.type_ == 'social'
 
-    # -- the plug --------------------------------------------------------------------------------
-    def reset(self, num_tracks, max_num_neigh, device):
-        """Reference resets the (dead) pool-LSTM state here (gridbased_pooling.py:345-351)."""
-        self.track_mask = None
+    def _plug_out_dim(self):
+        return int(self.out_dim if self.embedding is not None else self.n * self.n * self.pooling_dim)
 
-    def forward(self, hidden_state, obs1, obs2):
-        """[B, N, H], [B, N, 2], [B, N, 2] -> [B * N, out_dim] (gridbased_pooling.py:94-110)."""
-        _lib.require_cuda()
-        batch_size, num_tracks = obs1.size(0), obs1.size(1)
+    def _plug_device(self, obs1):
         params = list(self.parameters())
         device = params[0].device if params else obs1.device
         if device.type != 'cuda':
@@ -129,45 +120,4 @@ class GridBasedPooling(torch.nn.Module):
                 device = torch.device('cuda', torch.cuda.current_device())
             else:
                 raise RuntimeError("GridBasedPooling runs on CUDA only: move the module (or inputs) to the GPU")
-        if self._handle is None or self._handle.device != device:
-            cfg = _lib.LstmConfig()
-            cfg.hidden_dim = self._plug_width()
-            cfg.embedding_dim = 64
-            cfg.pool_to_input = 1
-            self.fill_config(cfg)
-            self._handle = ModelHandle(cfg, device)
-            self._standalone_dummy = None
-        self._set_plug_weights(device)
-        layout = self._layouts.get(range(0, batch_size * num_tracks + 1, num_tracks), device=device)
-        f32 = dict(device=device, dtype=torch.float32)
-        o1 = obs1.detach().to(**f32).reshape(-1, 2).contiguous()
-        o2 = obs2.detach().to(**f32).reshape(-1, 2).contiguous()
-        hid = None
-        if self.type_ == 'social':
-            if hidden_state.size(-1) != self.hidden_dim:
-                raise ValueError("hidden_state width != hidden_dim")
-            hid = hidden_state.detach().to(**f32).reshape(batch_size * num_tracks, -1).contiguous()
-        width = self.out_dim if self.embedding is not None else self.n * self.n * self.pooling_dim
-        out = self._handle.pool_forward(layout, hid, o1, o2, width)
-        return out.to(obs1.device) if obs1.device != device else out
-
-    def _plug_width(self):
-        # social pooling reads the hidden states; the other grids leave the handle's LSTM width unused
-        return int(self.hidden_dim) if self.type_ == 'social' else 128
-
-    def _set_plug_weights(self, device):
-        # the LSTM-cell slots of the handle are never read by tb2_pool_forward; feed zeros once
-        if getattr(self, '_standalone_dummy', None) is None:
-            z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=device)
-            H = self._plug_width()
-            in_dim = 64 + (self.out_dim if self.embedding is not None else self.n * self.n * self.pooling_dim)
-            self._standalone_dummy = dict(
-                input_embedding_weight=z(62, 2), input_embedding_bias=z(62),
-                encoder_weight_ih=z(4 * H, in_dim), encoder_weight_hh=z(4 * H, H),
-                encoder_bias_ih=z(4 * H), encoder_bias_hh=z(4 * H),
-                decoder_weight_ih=z(4 * H, in_dim), decoder_weight_hh=z(4 * H, H),
-                decoder_bias_ih=z(4 * H), decoder_bias_hh=z(4 * H),
-                hidden2normal_weight=z(5, H), hidden2normal_bias=z(5))
-        fields = dict(self._standalone_dummy)
-        fields.update(self.weight_fields())
-        self._handle.set_weights(fields, key=self.weights_version())
+        return device

@@ -14,7 +14,7 @@ import torch
 
 from .. import _lib
 from ..data import paths_to_xy
-from ..engine import LayoutCache, ModelHandle, weights_key
+from ..engine import LayoutCache, ModelHandle, lstm_config, weights_key
 from .modules import Hidden2Normal, InputEmbedding
 
 NAN = float('nan')
@@ -105,16 +105,9 @@ class LSTM(torch.nn.Module):
             raise RuntimeError("LSTM parameters are on %s: move the model to a CUDA device (model.to('cuda')); "
                                "there is no CPU path" % device)
         if self._handle is None or self._handle.device != device:
-            cfg = _lib.LstmConfig()
-            cfg.hidden_dim = int(self.hidden_dim)
-            cfg.embedding_dim = int(self.embedding_dim)
-            cfg.pool_to_input = int(bool(self.pool_to_input))
-            cfg.pool_type = _lib.POOL_NONE
-            cfg.pool_size = cfg.blur_size = 1
-            if self.pool is not None:
-                if not hasattr(self.pool, 'fill_config'):
-                    raise NotImplementedError("only GridBasedPooling and the HiddenStateMLPPooling / NearestNeighborMLP / AttentionMLPPooling / NearestNeighborLSTM / TrajectronPooling interaction modules are built")
-                self.pool.fill_config(cfg)
+            if self.pool is not None and not hasattr(self.pool, 'fill_config'):
+                raise NotImplementedError("only GridBasedPooling and the HiddenStateMLPPooling / NearestNeighborMLP / AttentionMLPPooling / NearestNeighborLSTM / TrajectronPooling interaction modules are built")
+            cfg = lstm_config(self.hidden_dim, self.embedding_dim, self.pool_to_input, self.pool)
             self._handle = ModelHandle(cfg, device)
         key = weights_key(self)
         if force_repack or key != self._handle._weights_key:

@@ -24,43 +24,10 @@ the same per-track LSTMCell / hidden2pool (traj_scene_sum_kernel + traj_feat_ker
 import torch
 
 from .. import _lib
-from ..engine import LayoutCache, ModelHandle, plug_getstate, weights_key
+from ..engine import PoolPlug
 
 
-class _StandalonePlug:
-    """Shared stand-alone path of the non-grid plugs: a model handle whose LSTM-cell slots hold zeros."""
-    _reads_hidden = False           # True: the handle's LSTM width is the width of the hidden states the plug reads
-
-    def _plug_width(self):
-        return int(self.hidden_dim) if self._reads_hidden else 128
-
-    def _plug_handle(self, device):
-        if self._handle is None or self._handle.device != device:
-            cfg = _lib.LstmConfig()
-            cfg.hidden_dim = self._plug_width()
-            cfg.embedding_dim = 64
-            cfg.pool_to_input = 1
-            self.fill_config(cfg)
-            self._handle = ModelHandle(cfg, device)
-            self._standalone_dummy = None
-        if getattr(self, '_standalone_dummy', None) is None:
-            z = lambda *s: torch.zeros(*s, dtype=torch.float32, device=device)
-            H = self._plug_width()
-            in_dim = 64 + self.out_dim
-            self._standalone_dummy = dict(
-                input_embedding_weight=z(62, 2), input_embedding_bias=z(62),
-                encoder_weight_ih=z(4 * H, in_dim), encoder_weight_hh=z(4 * H, H),
-                encoder_bias_ih=z(4 * H), encoder_bias_hh=z(4 * H),
-                decoder_weight_ih=z(4 * H, in_dim), decoder_weight_hh=z(4 * H, H),
-                decoder_bias_ih=z(4 * H), decoder_bias_hh=z(4 * H),
-                hidden2normal_weight=z(5, H), hidden2normal_bias=z(5))
-        fields = dict(self._standalone_dummy)
-        fields.update(self.weight_fields())
-        self._handle.set_weights(fields, key=self.weights_version())
-        return self._handle
-
-
-class HiddenStateMLPPooling(torch.nn.Module, _StandalonePlug):
+class HiddenStateMLPPooling(PoolPlug):
     _reads_hidden = True
 
     def __init__(self, hidden_dim=128, mlp_dim=128, mlp_dim_spatial=32, mlp_dim_vel=32, out_dim=None):
@@ -80,20 +47,14 @@ class HiddenStateMLPPooling(torch.nn.Module, _StandalonePlug):
         if self.mlp_dim_hidden:
             self.hidden_embedding = torch.nn.Sequential(torch.nn.Linear(self.hidden_dim, self.mlp_dim_hidden), torch.nn.ReLU())
         self.out_projection = torch.nn.Linear(self.mlp_dim, self.out_dim)
-        self._handle = None
-        self._layouts = LayoutCache()
 
     # -- configuration shared with LSTM ---------------------------------------------------------
-    def __getstate__(self):
-        return plug_getstate(self)
-
     def fill_config(self, cfg):
         cfg.pool_type = _lib.POOL_HIDDEN_MLP
         cfg.out_dim = int(self.out_dim)
         cfg.mlp_dim_spatial = int(self.mlp_dim_spatial)
         cfg.mlp_dim_vel = int(self.mlp_dim_vel)
         cfg.mlp_dim_hidden = int(self.mlp_dim_hidden)
-        cfg.pool_size = cfg.blur_size = 1
 
     def weight_fields(self):
         fields = dict(pool_spatial_weight=self.spatial_embedding[0].weight, pool_spatial_bias=self.spatial_embedding[0].bias,
@@ -104,33 +65,8 @@ class HiddenStateMLPPooling(torch.nn.Module, _StandalonePlug):
             fields.update(pool_hidden_weight=self.hidden_embedding[0].weight, pool_hidden_bias=self.hidden_embedding[0].bias)
         return fields
 
-    def weights_version(self):
-        return weights_key(self)
 
-    # -- the plug --------------------------------------------------------------------------------
-    def reset(self, num_tracks, max_num_neigh, device):
-        self.track_mask = None
-
-    def forward(self, hidden_states, obs1, obs2):
-        """[B, N, H], [B, N, 2], [B, N, 2] -> [B * N, out_dim] (non_gridbased_pooling.py:197-239)."""
-        _lib.require_cuda()
-        batch_size, num_tracks = obs2.size(0), obs2.size(1)
-        device = self.out_projection.weight.device
-        if device.type != 'cuda':
-            raise RuntimeError("HiddenStateMLPPooling runs on CUDA only: move the module to the GPU (module.cuda())")
-        if hidden_states.size(-1) != self.hidden_dim:
-            raise ValueError("hidden_states width != hidden_dim")
-        handle = self._plug_handle(device)
-        layout = self._layouts.get(range(0, batch_size * num_tracks + 1, num_tracks), device=device)
-        f32 = dict(device=device, dtype=torch.float32)
-        o1 = obs1.detach().to(**f32).reshape(-1, 2).contiguous()
-        o2 = obs2.detach().to(**f32).reshape(-1, 2).contiguous()
-        hid = hidden_states.detach().to(**f32).reshape(batch_size * num_tracks, -1).contiguous()
-        out = handle.pool_forward(layout, hid, o1, o2, self.out_dim)
-        return out.to(obs2.device) if obs2.device != device else out
-
-
-class NearestNeighborMLP(torch.nn.Module, _StandalonePlug):
+class NearestNeighborMLP(PoolPlug):
     def __init__(self, n=4, out_dim=32, no_vel=False):
         """Same arguments and sub-module names as the reference (non_gridbased_pooling.py:78-91)."""
         super().__init__()
@@ -141,11 +77,6 @@ class NearestNeighborMLP(torch.nn.Module, _StandalonePlug):
         self.no_velocity = no_vel
         self.input_dim = 2 if self.no_velocity else 4
         self.embedding = torch.nn.Sequential(torch.nn.Linear(self.input_dim, int(out_dim / self.n)), torch.nn.ReLU())
-        self._handle = None
-        self._layouts = LayoutCache()
-
-    def __getstate__(self):
-        return plug_getstate(self)
 
     def fill_config(self, cfg):
         cfg.pool_type = _lib.POOL_NN_MLP
@@ -154,34 +85,12 @@ class NearestNeighborMLP(torch.nn.Module, _StandalonePlug):
         cfg.mlp_dim_spatial = int(self.out_dim // self.n)
         cfg.mlp_dim_vel = 0 if self.no_velocity else 1
         cfg.mlp_dim_hidden = 0
-        cfg.pool_size = cfg.blur_size = 1
 
     def weight_fields(self):
         return dict(pool_spatial_weight=self.embedding[0].weight, pool_spatial_bias=self.embedding[0].bias)
 
-    def weights_version(self):
-        return weights_key(self)
 
-    def reset(self, num_tracks, max_num_neigh, device):
-        self.track_mask = None
-
-    def forward(self, _, obs1, obs2):
-        """_, [B, N, 2], [B, N, 2] -> [B * N, out_dim] (non_gridbased_pooling.py:96-147)."""
-        _lib.require_cuda()
-        batch_size, num_tracks = obs2.size(0), obs2.size(1)
-        device = self.embedding[0].weight.device
-        if device.type != 'cuda':
-            raise RuntimeError("NearestNeighborMLP runs on CUDA only: move the module to the GPU (module.cuda())")
-        handle = self._plug_handle(device)
-        layout = self._layouts.get(range(0, batch_size * num_tracks + 1, num_tracks), device=device)
-        f32 = dict(device=device, dtype=torch.float32)
-        o1 = obs1.detach().to(**f32).reshape(-1, 2).contiguous()
-        o2 = obs2.detach().to(**f32).reshape(-1, 2).contiguous()
-        out = handle.pool_forward(layout, None, o1, o2, self.out_dim)
-        return out.to(obs2.device) if obs2.device != device else out
-
-
-class AttentionMLPPooling(torch.nn.Module, _StandalonePlug):
+class AttentionMLPPooling(PoolPlug):
     _reads_hidden = True
 
     def __init__(self, hidden_dim=128, mlp_dim=128, mlp_dim_spatial=32, mlp_dim_vel=32, out_dim=None, fill_value=-10):
@@ -206,11 +115,6 @@ class AttentionMLPPooling(torch.nn.Module, _StandalonePlug):
         self.wv = torch.nn.Linear(self.mlp_dim, self.mlp_dim, bias=False)
         self.multihead_attn = torch.nn.MultiheadAttention(embed_dim=self.mlp_dim, num_heads=1)
         self.out_projection = torch.nn.Linear(self.mlp_dim, self.out_dim)
-        self._handle = None
-        self._layouts = LayoutCache()
-
-    def __getstate__(self):
-        return plug_getstate(self)
 
     def fill_config(self, cfg):
         cfg.pool_type = _lib.POOL_ATTN_MLP
@@ -219,7 +123,6 @@ class AttentionMLPPooling(torch.nn.Module, _StandalonePlug):
         cfg.mlp_dim_vel = int(self.mlp_dim_vel)
         cfg.mlp_dim_hidden = int(self.mlp_dim_hidden)
         cfg.attn_fill = float(self.fill_value)
-        cfg.pool_size = cfg.blur_size = 1
 
     def weight_fields(self):
         fields = dict(pool_spatial_weight=self.spatial_embedding[0].weight, pool_spatial_bias=self.spatial_embedding[0].bias,
@@ -235,32 +138,10 @@ class AttentionMLPPooling(torch.nn.Module, _StandalonePlug):
             fields.update(pool_hidden_weight=self.hidden_embedding[0].weight, pool_hidden_bias=self.hidden_embedding[0].bias)
         return fields
 
-    def weights_version(self):
-        return weights_key(self)
 
-    def reset(self, num_tracks, max_num_neigh, device):
-        self.track_mask = None
+class NearestNeighborLSTM(PoolPlug):
+    stateful = True
 
-    def forward(self, hidden_states, obs1, obs2):
-        """[B, N, H], [B, N, 2], [B, N, 2] -> [B * N, out_dim] (non_gridbased_pooling.py:297-351)."""
-        _lib.require_cuda()
-        batch_size, num_tracks = obs2.size(0), obs2.size(1)
-        device = self.out_projection.weight.device
-        if device.type != 'cuda':
-            raise RuntimeError("AttentionMLPPooling runs on CUDA only: move the module to the GPU (module.cuda())")
-        if hidden_states.size(-1) != self.hidden_dim:
-            raise ValueError("hidden_states width != hidden_dim")
-        handle = self._plug_handle(device)
-        layout = self._layouts.get(range(0, batch_size * num_tracks + 1, num_tracks), device=device)
-        f32 = dict(device=device, dtype=torch.float32)
-        o1 = obs1.detach().to(**f32).reshape(-1, 2).contiguous()
-        o2 = obs2.detach().to(**f32).reshape(-1, 2).contiguous()
-        hid = hidden_states.detach().to(**f32).reshape(batch_size * num_tracks, -1).contiguous()
-        out = handle.pool_forward(layout, hid, o1, o2, self.out_dim)
-        return out.to(obs2.device) if obs2.device != device else out
-
-
-class NearestNeighborLSTM(torch.nn.Module, _StandalonePlug):
     def __init__(self, n=4, hidden_dim=256, out_dim=32):
         """Same arguments and sub-module names as the reference (non_gridbased_pooling.py:371-383)."""
         super().__init__()
@@ -273,12 +154,7 @@ class NearestNeighborLSTM(torch.nn.Module, _StandalonePlug):
         self.hidden_dim = hidden_dim
         self.pool_lstm = torch.nn.LSTMCell(out_dim, hidden_dim)
         self.hidden2pool = torch.nn.Linear(hidden_dim, out_dim)
-        self._handle = None
-        self._layouts = LayoutCache()
         self._reset_pending = True
-
-    def __getstate__(self):
-        return plug_getstate(self)
 
     def fill_config(self, cfg):
         cfg.pool_type = _lib.POOL_NN_LSTM
@@ -287,7 +163,6 @@ class NearestNeighborLSTM(torch.nn.Module, _StandalonePlug):
         cfg.mlp_dim_spatial = int(self.out_dim // self.n)
         cfg.mlp_dim_vel = 1
         cfg.mlp_dim_hidden = int(self.hidden_dim)
-        cfg.pool_size = cfg.blur_size = 1
 
     def weight_fields(self):
         return dict(pool_spatial_weight=self.embedding[0].weight, pool_spatial_bias=self.embedding[0].bias,
@@ -295,42 +170,27 @@ class NearestNeighborLSTM(torch.nn.Module, _StandalonePlug):
                     pool_lstm_bias_ih=self.pool_lstm.bias_ih, pool_lstm_bias_hh=self.pool_lstm.bias_hh,
                     pool_out_weight=self.hidden2pool.weight, pool_out_bias=self.hidden2pool.bias)
 
-    def weights_version(self):
-        return weights_key(self)
-
     def reset(self, num_tracks, max_num_neigh, device):
         """Reference: fresh zero state per track (non_gridbased_pooling.py:385-389); here the state of the stand-alone plug
         lives in the handle's workspace and is zeroed before the next call (LSTM.forward zeroes its own)."""
         self._reset_pending = True
 
-    def forward(self, _, obs1, obs2):
-        """_, [B, N, 2], [B, N, 2] -> [B * N, out_dim]; advances the interaction-encoder state (non_gridbased_pooling.py:391-451)."""
-        _lib.require_cuda()
-        batch_size, num_tracks = obs2.size(0), obs2.size(1)
-        device = self.hidden2pool.weight.device
-        if device.type != 'cuda':
-            raise RuntimeError("NearestNeighborLSTM runs on CUDA only: move the module to the GPU (module.cuda())")
-        handle = self._plug_handle(device)
-        layout = self._layouts.get(range(0, batch_size * num_tracks + 1, num_tracks), device=device)
+    def _plug_state(self, handle, layout):
+        """A plug call advances the interaction-encoder state (non_gridbased_pooling.py:391-451)."""
         if self._reset_pending:
             handle.pool_state_reset(layout)
             self._reset_pending = False
-            self._state_tracks = batch_size * num_tracks
-        elif getattr(self, '_state_tracks', None) != batch_size * num_tracks:
+            self._state_tracks = layout.num_tracks
+        elif getattr(self, '_state_tracks', None) != layout.num_tracks:
             # the reference stacks `num_tracks` state rows from reset() against B * N feature rows and fails the same way
             raise RuntimeError("the interaction-encoder state holds %s tracks, this call has %d: call reset(num_tracks, ...)"
-                               % (getattr(self, '_state_tracks', None), batch_size * num_tracks))
-        f32 = dict(device=device, dtype=torch.float32)
-        o1 = obs1.detach().to(**f32).reshape(-1, 2).contiguous()
-        o2 = obs2.detach().to(**f32).reshape(-1, 2).contiguous()
-        out = handle.pool_forward(layout, None, o1, o2, self.out_dim)
-        return out.to(obs2.device) if obs2.device != device else out
+                               % (getattr(self, '_state_tracks', None), layout.num_tracks))
 
 
 class TrajectronPooling(NearestNeighborLSTM):
     def __init__(self, n=4, hidden_dim=256, out_dim=32, track_mask=None):
         """Same arguments and sub-module names as the reference (non_gridbased_pooling.py:468-479; `n` is unused there)."""
-        torch.nn.Module.__init__(self)
+        PoolPlug.__init__(self)
         if hidden_dim > 512 or out_dim > 1024:
             raise ValueError("TrajectronPooling needs hidden_dim <= 512 and out_dim <= 1024")
         self.n = n
@@ -340,8 +200,6 @@ class TrajectronPooling(NearestNeighborLSTM):
         self.pool_lstm = torch.nn.LSTMCell(out_dim, hidden_dim)
         self.hidden2pool = torch.nn.Linear(hidden_dim, out_dim)
         self.track_mask = track_mask
-        self._handle = None
-        self._layouts = LayoutCache()
         self._reset_pending = True
 
     def fill_config(self, cfg):
@@ -351,4 +209,3 @@ class TrajectronPooling(NearestNeighborLSTM):
         cfg.mlp_dim_spatial = int(self.out_dim)
         cfg.mlp_dim_vel = 1
         cfg.mlp_dim_hidden = int(self.hidden_dim)
-        cfg.pool_size = cfg.blur_size = 1

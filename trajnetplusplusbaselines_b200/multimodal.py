@@ -26,12 +26,7 @@ DECODE_BYTES = 2 << 30
 def stateful_pool(body):
     """True for interaction modules that carry an LSTM state of their own through the time loop (NearestNeighborLSTM,
     TrajectronPooling): that state lives in the engine's workspace and is not replicated per mode."""
-    pool = body.pool
-    if pool is None or not hasattr(pool, 'fill_config'):
-        return False
-    cfg = _lib.LstmConfig()
-    pool.fill_config(cfg)
-    return cfg.pool_type in (_lib.POOL_NN_LSTM, _lib.POOL_TRAJECTRON)
+    return bool(getattr(body.pool, 'stateful', False))
 
 
 def replicated_split(split, k):
