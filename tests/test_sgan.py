@@ -120,6 +120,16 @@ def test_sgan_modes_and_predictor():
 
 
 @pytest.mark.gpu
+def test_discriminator_refuses_more_tracks_than_batch_split():
+    """A batch_split that covers fewer tracks than observed is refused, as LSTM.forward refuses it."""
+    name, kind, xy, bs, Wg, Wd, noise = _inputs(SGAN_CASES[0])
+    _, dis = _models(kind, Wg, Wd, noise)
+    scene = torch.from_numpy(np.concatenate([xy, xy[:, :1]], axis=1))         # one track more than bs[-1]
+    with torch.no_grad(), pytest.raises(ValueError, match=r"batch_split\[-1\] != number of tracks"):
+        dis(scene[:9], scene[9:21], torch.zeros(scene.shape[1], 2), torch.from_numpy(bs))
+
+
+@pytest.mark.gpu
 def test_sgan_training_fails_loudly():
     name, kind, xy, bs, Wg, Wd, noise = _inputs(SGAN_CASES[0])
     gen, _ = _models(kind, Wg, Wd, noise)

@@ -59,6 +59,17 @@ def test_cuda_vae_matches_reference(case):
 
 
 @pytest.mark.gpu
+def test_vae_refuses_more_tracks_than_batch_split():
+    """A batch_split that covers fewer tracks than observed is refused, as LSTM.forward refuses it."""
+    from trajnetplusplusbaselines_b200.vae import VAE
+    xy, bs = O.synthetic_scenes(3, 5, seed=9)
+    scene = torch.from_numpy(np.concatenate([xy, xy[:, :1]], axis=1))         # one track more than bs[-1]
+    model = VAE().cuda().eval()
+    with torch.no_grad(), pytest.raises(ValueError, match=r"batch_split\[-1\] != number of tracks"):
+        model(scene[:9], torch.zeros(scene.shape[1], 2), torch.from_numpy(bs), n_predict=12)
+
+
+@pytest.mark.gpu
 def test_vae_predictor_and_training_guard():
     from trajnetplusplusbaselines_b200.data import TrackRow
     from trajnetplusplusbaselines_b200.vae import VAE, VAEPredictor

@@ -42,6 +42,11 @@ def _stream(device):
     return ctypes.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
+def linear_on(linear, device):
+    """(weight, bias) of a torch.nn.Linear as fp32 contiguous tensors on `device`, for a kernel that reads them."""
+    return tuple(t.detach().to(device=device, dtype=torch.float32).contiguous() for t in (linear.weight, linear.bias))
+
+
 def _device_of(device):
     """Resolved CUDA device (the current one when `device` is None or an index-less 'cuda')."""
     device = torch.device('cuda' if device is None else device)
@@ -83,7 +88,10 @@ class LayoutCache:
         self._items = OrderedDict()
 
     def get(self, batch_split, pad_to_batch_max=True, device=None):
+        """batch_split: a sequence, tensor or array of offsets."""
         device = _device_of(device)
+        if hasattr(batch_split, 'tolist'):       # one conversion instead of a 0-d tensor per element
+            batch_split = batch_split.tolist()
         key = tuple(int(v) for v in batch_split) + (bool(pad_to_batch_max), device.index)
         item = self._items.get(key)
         if item is None:
@@ -329,21 +337,22 @@ class ModelHandle:
         return int(_lib.load().tb2_lstm_train_cache_bytes(self.handle, layout.handle, int(num_steps)))
 
     def forward_sequence_train(self, layout, observed, truth, n_decode, normals, positions, h, c, states, cache):
-        """tb2_lstm_forward_sequence_train: per-step forward quantities of the social pooling stay in `cache`
-        (uint8 device tensor of train_cache_bytes) for tb2_lstm_sequence_backward_cached."""
+        """tb2_lstm_forward_sequence_train: the per-step states go to `states` [S, 2, M, H]; per-step forward
+        quantities of the social pooling stay in `cache` (uint8 device tensor of train_cache_bytes, None when that is
+        0) for tb2_lstm_sequence_backward_cached."""
         lib = _lib.load()
         ws, need = self.workspace(layout)
         with torch.cuda.device(self.device):
             _lib.check(lib.tb2_lstm_forward_sequence_train(
                 self.handle, layout.handle, _ptr(observed), int(observed.shape[0]), _ptr(truth), int(n_decode),
-                _ptr(normals), _ptr(positions), _ptr(h), _ptr(c), _ptr(states), _ptr(cache), int(cache.numel()),
-                _ptr(ws), need, _stream(self.device)))
+                _ptr(normals), _ptr(positions), _ptr(h), _ptr(c), _ptr(states), _ptr(cache),
+                0 if cache is None else int(cache.numel()), _ptr(ws), need, _stream(self.device)))
 
-    def forward_sequence(self, layout, observed, truth, n_decode, normals, positions, h, c, states=None):
+    def forward_sequence(self, layout, observed, truth, n_decode, normals, positions, h, c):
         lib = _lib.load()
         ws, need = self.workspace(layout)
         with torch.cuda.device(self.device):
             _lib.check(lib.tb2_lstm_forward_sequence(
                 self.handle, layout.handle, _ptr(observed), int(observed.shape[0]), _ptr(truth),
-                int(n_decode), _ptr(normals), _ptr(positions), _ptr(h), _ptr(c), _ptr(states),
+                int(n_decode), _ptr(normals), _ptr(positions), _ptr(h), _ptr(c), _ptr(None),
                 _ptr(ws), need, _stream(self.device)))

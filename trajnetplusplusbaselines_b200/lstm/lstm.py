@@ -8,6 +8,7 @@ tb2_lstm_forward_sequence (csrc/capi.cu).  There is no torch or CPU implementati
 step in this package: without the CUDA library the calls raise.
 """
 import math
+from collections import namedtuple
 
 import numpy as np
 import torch
@@ -18,6 +19,9 @@ from ..engine import LayoutCache, ModelHandle, lstm_config, weights_key
 from .modules import Hidden2Normal, InputEmbedding
 
 NAN = float('nan')
+
+# one forward set up by LSTM._sequence
+Sequence = namedtuple('Sequence', 'handle layout obs truth n_decode S_enc S normals positions h c out_device')
 
 
 def drop_distant(xy, r=6.0):
@@ -161,7 +165,7 @@ class LSTM(torch.nn.Module):
             h, c = torch.stack(list(h)), torch.stack(list(c))
         h = h.detach().to(device=device, dtype=torch.float32).contiguous().clone()
         c = c.detach().to(device=device, dtype=torch.float32).contiguous().clone()
-        layout = self._layouts.get(batch_split.tolist() if torch.is_tensor(batch_split) else batch_split, device=device)
+        layout = self._layouts.get(batch_split, device=device)
         o1 = self._to_device(obs1, device)
         o2 = self._to_device(obs2, device)
         normal, _ = handle.step_forward(layout, phase, o1, o2, h, c)
@@ -182,18 +186,18 @@ class LSTM(torch.nn.Module):
             return sequence_with_grad(self, observed, batch_split, prediction_truth, n_predict)
         return self._forward_nograd(observed, batch_split, prediction_truth, n_predict)
 
-    def _forward_nograd(self, observed, batch_split, prediction_truth, n_predict, want_states=False,
-                        pad_to_batch_max=True, force_repack=False):
+    def _sequence(self, observed, batch_split, prediction_truth, n_predict, pad_to_batch_max=True, force_repack=False):
+        """A forward of `observed` [obs_length, M, 2] set up on the model's device: the inputs there and empty outputs
+        and (h, c) state.  Launches nothing.  The steps are [0, S_enc) for the encoder and [S_enc, S) for the decoder;
+        truth is None when there is no teacher forcing."""
         handle = self._engine(force_repack)
         device = handle.device
-        out_device = observed.device
-        layout = self._layouts.get(batch_split.tolist() if torch.is_tensor(batch_split) else batch_split,
-                                   pad_to_batch_max, device=device)
+        layout = self._layouts.get(batch_split, pad_to_batch_max, device=device)
         M = layout.num_tracks
         if observed.shape[1] != M:
             raise ValueError("batch_split[-1] != number of tracks")
         obs = self._to_device(observed, device)
-        obs_length = int(obs.shape[0])
+        truth = None
         if prediction_truth is not None:
             if isinstance(prediction_truth, (list, tuple)):
                 prediction_truth = torch.stack(list(prediction_truth))
@@ -202,40 +206,64 @@ class LSTM(torch.nn.Module):
             if n_decode == 0:
                 truth = None
         else:
-            truth = None
             n_decode = int(n_predict) - 1
-        S = obs_length - 1 + n_decode
+        S_enc = int(obs.shape[0]) - 1
+        S = S_enc + n_decode
         f32 = dict(dtype=torch.float32, device=device)
-        normals = torch.empty((S, M, 5), **f32)
-        positions = torch.empty((S, M, 2), **f32)
-        h = torch.empty((M, self.hidden_dim), **f32)
-        c = torch.empty((M, self.hidden_dim), **f32)
-        states = torch.empty((S, 2, M, self.hidden_dim), **f32) if want_states else None
-        cache = None
-        if want_states:        # training forward: keep what the social backward would recompute (0 bytes: no cache)
-            cache_bytes = handle.train_cache_bytes(layout, S)
-            if cache_bytes > 0:
-                cache = torch.empty(cache_bytes, dtype=torch.uint8, device=device)
-        if out_device != device and not want_states and obs_length > 2:
-            # host caller: every step's slice of the results is copied to pinned host memory on a second stream
-            # while the later steps compute; one synchronisation of that stream at the end
-            normals_h, positions_h = self._host_buffers(normals, positions)
-            copy_stream = self._copy_stream(device)
-            handle.forward_sequence_host(layout, obs, truth, n_decode, normals, positions, h, c, normals_h, positions_h,
-                                         copy_stream)
-            copy_stream.synchronize()
-            return normals_h.view(normals_h.shape), positions_h.view(positions_h.shape)
-        if cache is not None:
-            handle.forward_sequence_train(layout, obs, truth, n_decode, normals, positions, h, c, states, cache)
-        else:
-            handle.forward_sequence(layout, obs, truth, n_decode, normals, positions, h, c, states)
-        if obs_length == 2:                      # lstm.py:222-223: positions seeded with observed[-1]
-            positions = torch.cat([obs[-1:].clone(), positions], dim=0)
-        if want_states:
-            return normals, positions, states, (obs, truth, layout, cache)
-        if out_device != device:
+        return Sequence(handle, layout, obs, truth, n_decode, S_enc, S,
+                        normals=torch.empty((S, M, 5), **f32), positions=torch.empty((S, M, 2), **f32),
+                        h=torch.empty((M, self.hidden_dim), **f32), c=torch.empty((M, self.hidden_dim), **f32),
+                        out_device=observed.device)
+
+    def _encode(self, seq):
+        """The encoder steps [0, S_enc) of `seq`, into its own outputs and state."""
+        seq.handle.forward_steps(seq.layout, seq.obs, seq.truth, seq.n_decode, 0, seq.S_enc, seq.normals,
+                                 seq.positions, seq.h, seq.c)
+        return seq
+
+    def _decode(self, seq, context, seed=True):
+        """One decode from a copy of the encoder state and outputs of `seq`: context(h, c) edits the copied state, then
+        the decoder steps [S_enc, S) run.  Returns the outputs as _results does."""
+        h, c = seq.h.clone(), seq.c.clone()
+        normals, positions = seq.normals.clone(), seq.positions.clone()
+        context(h, c)
+        seq.handle.forward_steps(seq.layout, seq.obs, seq.truth, seq.n_decode, seq.S_enc, seq.S, normals, positions,
+                                 h, c)
+        return self._results(seq, normals, positions, seed)
+
+    def _results(self, seq, normals, positions, seed=True):
+        """(normals, positions) on the device `observed` came from.  seed: at obs_length 2 the positions start with
+        observed[-1] (lstm.py:222-223, sgan.py:353-354; the VAE has no such rule)."""
+        if seed and seq.obs.shape[0] == 2:
+            positions = torch.cat([seq.obs[-1:].clone(), positions], dim=0)
+        if seq.out_device != seq.handle.device:
             normals, positions = self._to_host(normals, positions)
         return normals, positions
+
+    def _forward_nograd(self, observed, batch_split, prediction_truth, n_predict, want_states=False,
+                        pad_to_batch_max=True, force_repack=False):
+        seq = self._sequence(observed, batch_split, prediction_truth, n_predict, pad_to_batch_max, force_repack)
+        handle, layout, device = seq.handle, seq.layout, seq.handle.device
+        inputs = (layout, seq.obs, seq.truth, seq.n_decode, seq.normals, seq.positions, seq.h, seq.c)
+        if want_states:
+            # training forward: the outputs stay on the device; the per-step states are kept for the backward, and
+            # so is what the social backward would otherwise recompute (0 bytes: no cache)
+            states = torch.empty((seq.S, 2, layout.num_tracks, self.hidden_dim), dtype=torch.float32, device=device)
+            cache_bytes = handle.train_cache_bytes(layout, seq.S)
+            cache = torch.empty(cache_bytes, dtype=torch.uint8, device=device) if cache_bytes > 0 else None
+            handle.forward_sequence_train(*inputs, states, cache)
+            normals, positions = self._results(seq._replace(out_device=device), seq.normals, seq.positions)
+            return normals, positions, states, (seq.obs, seq.truth, layout, cache)
+        if seq.out_device != device and seq.obs.shape[0] > 2:
+            # host caller: every step's slice of the results is copied to pinned host memory on a second stream
+            # while the later steps compute; one synchronisation of that stream at the end
+            normals_h, positions_h = self._host_buffers(seq.normals, seq.positions)
+            copy_stream = self._copy_stream(device)
+            handle.forward_sequence_host(*inputs, normals_h, positions_h, copy_stream)
+            copy_stream.synchronize()
+            return normals_h.view(normals_h.shape), positions_h.view(positions_h.shape)
+        handle.forward_sequence(*inputs)
+        return self._results(seq, seq.normals, seq.positions)
 
     def _host_buffers(self, *tensors):
         """Pinned host buffers shaped like `tensors`, from a pool (no per-call allocation: fresh host
@@ -282,8 +310,11 @@ class LSTM(torch.nn.Module):
         return state
 
 
-class LSTMPredictor(object):
-    """Reference lstm.py:266-313."""
+class Predictor(object):
+    """What the LSTM, S-GAN and VAE predictors share (reference lstm.py:266-313, sgan.py:583-630, vae.py:347-398):
+    save / load and the per-scene call.  A subclass supplies `_mode_scenes` and the two class attributes below."""
+    start_length_applies = True      # the model is fed xy[start_length:obs_length], else xy[:obs_length]
+    neighbours_every_mode = True     # every mode returns the neighbours' predictions, else mode 0 only
 
     def __init__(self, model):
         self.model = model
@@ -299,30 +330,42 @@ class LSTMPredictor(object):
         with open(filename, 'rb') as f:
             return torch.load(f, weights_only=False)   # torch >= 2.6 default would reject the pickle
 
-    def __call__(self, paths, scene_goal, n_predict=12, modes=1, predict_all=True, obs_length=9, start_length=0, args=None):
+    def _mode_scenes(self, observed, scene_goal, batch_split, n_predict, modes):
+        """The predicted positions [S, N, 2] of every mode, in order (an iterable)."""
+        raise NotImplementedError
+
+    def __call__(self, paths, scene_goal, n_predict=12, modes=1, predict_all=True, obs_length=9, start_length=0,
+                 args=None):
         self.model.eval()
         with torch.no_grad():
             xy = paths_to_xy(paths)
             batch_split = [0, xy.shape[1]]
-
             normalize = bool(getattr(args, 'normalize_scene', False))
             if normalize:
                 xy, rotation, center, scene_goal = center_scene(xy, obs_length, goals=np.asarray(scene_goal))
-
             xy = torch.Tensor(xy)
             scene_goal = torch.Tensor(np.asarray(scene_goal))
             batch_split = torch.Tensor(batch_split).long()
-
+            first = start_length if self.start_length_applies else 0
             multimodal_outputs = {}
-            for num_p in range(modes):
-                _, output_scenes = self.model(xy[start_length:obs_length], scene_goal, batch_split, n_predict=n_predict)
+            for num_p, output_scenes in enumerate(self._mode_scenes(xy[first:obs_length], scene_goal, batch_split,
+                                                                    n_predict, modes)):
                 output_scenes = output_scenes.cpu().numpy()
                 if normalize:
                     output_scenes = inverse_scene(output_scenes, rotation, center)
                 output_primary = output_scenes[-n_predict:, 0]
                 output_neighs = output_scenes[-n_predict:, 1:]
-                multimodal_outputs[num_p] = [output_primary, output_neighs]
+                multimodal_outputs[num_p] = [output_primary,
+                                             output_neighs if num_p == 0 or self.neighbours_every_mode else []]
         return multimodal_outputs
+
+
+class LSTMPredictor(Predictor):
+    """Reference lstm.py:266-313."""
+
+    def _mode_scenes(self, observed, scene_goal, batch_split, n_predict, modes):
+        for _ in range(modes):        # one forward per mode, each mode's outputs handled before the next forward
+            yield self.model(observed, scene_goal, batch_split, n_predict=n_predict)[1]
 
     def predict_batch(self, scenes, scene_goals=None, n_predict=12, obs_length=9, start_length=0, args=None):
         """Many scenes in ONE forward call (SURVEY.md 8f rank 1: replaces the evaluator's

@@ -18,6 +18,7 @@ import torch
 
 from . import _lib
 from .engine import _ptr, _stream
+from .lstm.lstm import Predictor
 
 # device memory one decode may take: the engine's workspace for its rows plus their replicated state
 DECODE_BYTES = 2 << 30
@@ -71,35 +72,63 @@ def predict_modes(body, observed, split, n_predict, modes, context, max_rows=Non
     context(h_enc, c_enc, q0, q1, h_out, c_out) writes the decoder starting state of modes [q0, q1) into
     h_out / c_out [(q1 - q0) * M, H].  Returns the positions of the last n_predict steps, float32 [n_predict,
     modes * M, 2] on the device, mode-major."""
-    handle = body._engine()
-    device = handle.device
-    layout = body._layouts.get(split.tolist(), False, device=device)
-    M = layout.num_tracks
-    obs_length = int(observed.shape[0])
-    n_decode = int(n_predict) - 1
-    S_enc = obs_length - 1
-    S = S_enc + n_decode
+    enc = body._encode(body._sequence(observed, split, None, n_predict, pad_to_batch_max=False))
+    handle, device, M, S_enc, S = enc.handle, enc.handle.device, enc.layout.num_tracks, enc.S_enc, enc.S
     H = int(body.hidden_dim)
     f32 = dict(dtype=torch.float32, device=device)
-    normals0, positions0 = torch.empty((S, M, 5), **f32), torch.empty((S, M, 2), **f32)
-    h0, c0 = torch.empty((M, H), **f32), torch.empty((M, H), **f32)
-    handle.forward_steps(layout, observed, None, n_decode, 0, S_enc, normals0, positions0, h0, c0)
-    cap = rows_per_decode(handle, layout, S, obs_length) if max_rows is None else int(max_rows)
+    cap = rows_per_decode(handle, enc.layout, S, int(enc.obs.shape[0])) if max_rows is None else int(max_rows)
     per_group = max(1, min(modes, cap // max(M, 1)))
     out = torch.empty((n_predict, modes * M, 2), **f32)
     for q0 in range(0, modes, per_group):
         q1 = min(q0 + per_group, modes)
         kq = q1 - q0
         rows = kq * M
-        rep = body._layouts.get(replicated_split(split, kq).tolist(), False, device=device)
-        obs_rep = observed.repeat(1, kq, 1)
+        rep = body._layouts.get(replicated_split(split, kq), False, device=device)
+        obs_rep = enc.obs.repeat(1, kq, 1)
         normals, positions = torch.empty((S, rows, 5), **f32), torch.empty((S, rows, 2), **f32)
-        positions[:S_enc] = positions0[:S_enc].repeat(1, kq, 1)      # the decoder's first inputs
+        positions[:S_enc] = enc.positions[:S_enc].repeat(1, kq, 1)      # the decoder's first inputs
         h, c = torch.empty((rows, H), **f32), torch.empty((rows, H), **f32)
-        context(h0, c0, q0, q1, h, c)
-        handle.forward_steps(rep, obs_rep, None, n_decode, S_enc, S, normals, positions, h, c)
+        context(enc.h, enc.c, q0, q1, h, c)
+        handle.forward_steps(rep, obs_rep, None, enc.n_decode, S_enc, S, normals, positions, h, c)
         out[:, q0 * M:q1 * M] = positions[S - n_predict:]
     return out
+
+
+class ModesPredictor(Predictor):
+    """Base of the multi-modal predictors (SGANPredictor, VAEPredictor): the per-scene call returns the neighbours in
+    mode 0 only, and predict_batch_xy decodes every mode of many scenes at once through _predict_batch_xy."""
+    neighbours_every_mode = False
+    _model_noun = 'model'       # what the refusal of batched decoding calls the model
+
+    def _lstm_model(self):
+        """The LSTM whose engine runs the model."""
+        raise NotImplementedError
+
+    def batch_decode_supported(self):
+        """predict_batch_xy serves every model except those whose interaction module carries its own LSTM state
+        (NearestNeighborLSTM, TrajectronPooling): that state is not replicated per mode."""
+        return not stateful_pool(self._lstm_model())
+
+    def _predict_batch_xy(self, xys, n_predict, obs_length, start_length, args, modes, max_rows, make_context):
+        """predict_batch_xy: make_context(device, split, modes) draws the random inputs of every mode and returns the
+        context() of predict_modes."""
+        body = self._lstm_model()
+        if not self.batch_decode_supported():
+            raise NotImplementedError("batched decoding of a %s whose interaction module keeps an LSTM state is not "
+                                      "built; call the predictor scene by scene" % self._model_noun)
+        self.model.eval()
+        modes = int(modes)
+        if modes < 1:
+            raise ValueError("modes must be >= 1")
+        if not xys:
+            return []
+        normalize = bool(getattr(args, 'normalize_scene', False))
+        first = start_length if self.start_length_applies else 0
+        with torch.no_grad():
+            observed, split, rotation, center = observed_batch(body, xys, obs_length, first, normalize)
+            context = make_context(observed.device, split, modes)
+            pred = predict_modes(body, observed, split, n_predict, modes, context, max_rows)
+            return scene_results(pred, split, modes, n_predict, normalize, rotation, center)
 
 
 def scene_results(pred, split, modes, n_predict, normalize, rotation=None, center=None):

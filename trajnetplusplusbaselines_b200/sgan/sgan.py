@@ -11,15 +11,11 @@ state_dict keys (reference checkpoints load verbatim).  GAN training (variety lo
 steps) is not built: forward under grad mode raises.  SGANPredictor.predict_batch_xy decodes every mode
 of many scenes at once (the evaluator's path, ../multimodal.py).
 """
-import ctypes
-
-import numpy as np
 import torch
 from torch import nn
 
 from .. import _lib, multimodal
-from ..data import paths_to_xy
-from ..engine import _ptr, _stream
+from ..engine import _ptr, _stream, linear_on
 from ..lstm.lstm import LSTM, center_scene, drop_distant, inverse_scene  # noqa: F401
 
 
@@ -64,58 +60,26 @@ class LSTMGenerator(LSTM):
         return get_noise((self.noise_dim,), self.noise_type, device=device).float().contiguous()
 
     def encode(self, observed, batch_split, prediction_truth, n_predict):
-        """Encoder steps only; returns the context every mode's decoder starts from."""
-        handle = self._engine()
-        device = handle.device
-        layout = self._layouts.get(batch_split.tolist() if torch.is_tensor(batch_split) else batch_split,
-                                   device=self._device())
-        M = layout.num_tracks
-        if observed.shape[1] != M:
-            raise ValueError("batch_split[-1] != number of tracks")
-        obs = self._to_device(observed, device)
-        obs_length = int(obs.shape[0])
-        truth = None
+        """Encoder steps only; returns the sequence every mode's decoder starts from."""
         if prediction_truth is not None:
-            if isinstance(prediction_truth, (list, tuple)):
-                prediction_truth = torch.stack(list(prediction_truth))
             # sgan.py:367-369 chains (observed[-1:], prediction_truth[:-1]): the last frame is unused
-            truth = self._to_device(prediction_truth, device)[:-1].contiguous()
-            n_decode = int(truth.shape[0])
-            if n_decode == 0:
-                truth = None
-        else:
-            n_decode = int(n_predict) - 1
-        S = obs_length - 1 + n_decode
-        f32 = dict(dtype=torch.float32, device=device)
-        ctx = dict(handle=handle, layout=layout, obs=obs, truth=truth, n_decode=n_decode, S=S, S_enc=obs_length - 1,
-                   normals=torch.empty((S, M, 5), **f32), positions=torch.empty((S, M, 2), **f32),
-                   h=torch.empty((M, self.hidden_dim), **f32), c=torch.empty((M, self.hidden_dim), **f32),
-                   out_device=observed.device)
-        handle.forward_steps(layout, obs, truth, n_decode, 0, ctx['S_enc'], ctx['normals'], ctx['positions'],
-                             ctx['h'], ctx['c'])
-        return ctx
+            prediction_truth = prediction_truth[:-1]
+        return self._encode(self._sequence(observed, batch_split, prediction_truth, n_predict))
 
-    def decode(self, ctx):
+    def decode(self, seq):
         """One mode: noise into a copy of the encoder state, then the decoder steps."""
-        handle, device = ctx['handle'], ctx['handle'].device
-        h, c = ctx['h'].clone(), ctx['c'].clone()
-        normals, positions = ctx['normals'].clone(), ctx['positions'].clone()
-        if not self.no_noise:
-            lin = self.mlp_decoder_context[0]
-            noise = self._draw_noise(device)
-            lib = _lib.load()
-            w = lin.weight.detach().to(device=device, dtype=torch.float32).contiguous()
-            b = lin.bias.detach().to(device=device, dtype=torch.float32).contiguous()
-            with torch.cuda.device(device):
-                _lib.check(lib.tb2_sgan_add_noise(_ptr(w), _ptr(b), _ptr(noise), _ptr(h), int(h.shape[0]),
-                                                  int(self.hidden_dim), int(self.noise_dim), _stream(device)))
-        handle.forward_steps(ctx['layout'], ctx['obs'], ctx['truth'], ctx['n_decode'], ctx['S_enc'], ctx['S'],
-                             normals, positions, h, c)
-        if int(ctx['obs'].shape[0]) == 2:        # sgan.py:353-354: positions seeded with observed[-1]
-            positions = torch.cat([ctx['obs'][-1:].clone(), positions], dim=0)
-        if ctx['out_device'] != device:
-            normals, positions = self._to_host(normals, positions)
-        return normals, positions
+        return self._decode(seq, self._add_noise)
+
+    def _add_noise(self, h, c):
+        """h <- [ReLU(mlp_decoder_context(h)), noise] in place, one noise draw for every track (sgan.py:200-221)."""
+        if self.no_noise:
+            return
+        device = h.device
+        noise = self._draw_noise(device)
+        w, b = linear_on(self.mlp_decoder_context[0], device)
+        with torch.cuda.device(device):
+            _lib.check(_lib.load().tb2_sgan_add_noise(_ptr(w), _ptr(b), _ptr(noise), _ptr(h), int(h.shape[0]),
+                                                      int(self.hidden_dim), int(self.noise_dim), _stream(device)))
 
     def forward(self, observed, goals, batch_split, prediction_truth=None, n_predict=None):
         """sgan.py:301-394: (rel_pred_scene [S, M, 5], pred_scene [S, M, 2])."""
@@ -158,19 +122,11 @@ class LSTMDiscriminator(torch.nn.Module):
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             raise NotImplementedError("S-GAN training is not built; score under torch.no_grad()")
         body = self._lstm[0]
-        handle = body._engine()
-        device = handle.device
-        seq = torch.cat([body._to_device(observed, device), body._to_device(prediction, device)], dim=0)
-        layout = body._layouts.get(batch_split.tolist() if torch.is_tensor(batch_split) else batch_split,
-                                   device=body._device())
-        M = layout.num_tracks
-        S = int(seq.shape[0]) - 1
-        f32 = dict(dtype=torch.float32, device=device)
-        normals, positions = torch.empty((S, M, 5), **f32), torch.empty((S, M, 2), **f32)
-        h, c = torch.empty((M, self.hidden_dim), **f32), torch.empty((M, self.hidden_dim), **f32)
-        handle.forward_steps(layout, seq, None, 0, 0, S, normals, positions, h, c)
-        prim = torch.as_tensor(layout.offsets[:-1], device=device)
-        scores = self.real_classifier(h[prim])
+        # n_predict = 1: no decoder step, every frame of [observed; prediction] goes through the encoder
+        seq = body._encode(body._sequence(torch.cat([observed, prediction], dim=0), batch_split, None, 1))
+        device = seq.handle.device
+        prim = torch.as_tensor(seq.layout.offsets[:-1], device=device)
+        scores = self.real_classifier(seq.h[prim])
         return scores if observed.device == device else scores.to(observed.device)
 
 
@@ -191,9 +147,9 @@ class SGAN(torch.nn.Module):
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             raise NotImplementedError("S-GAN training is not built; call under torch.no_grad()")
         rel_pred_list, pred_list = [], []
-        ctx = self.generator.encode(observed, batch_split, prediction_truth, n_predict)   # shared by all modes
+        seq = self.generator.encode(observed, batch_split, prediction_truth, n_predict)   # shared by all modes
         for _ in range(self.k):
-            rel_pred_scene, pred_scene = self.generator.decode(ctx)
+            rel_pred_scene, pred_scene = self.generator.decode(seq)
             rel_pred_list.append(rel_pred_scene)
             pred_list.append(pred_scene)
             if step_type == 'd':
@@ -205,53 +161,19 @@ class SGAN(torch.nn.Module):
         return rel_pred_list, pred_list, None, None
 
 
-class SGANPredictor(object):
+class SGANPredictor(multimodal.ModesPredictor):
     """sgan.py:583-630."""
+    start_length_applies = False     # sgan.py:603 feeds xy[:obs_length]
+    _model_noun = 'generator'
 
-    def __init__(self, model):
-        self.model = model
+    def _lstm_model(self):
+        return self.model.generator
 
-    def save(self, state, filename):
-        with open(filename, 'wb') as f:
-            torch.save(self, f)
-        with open(filename + '.state', 'wb') as f:
-            torch.save(state, f)
-
-    @staticmethod
-    def load(filename):
-        with open(filename, 'rb') as f:
-            return torch.load(f, weights_only=False)
-
-    def __call__(self, paths, scene_goal, n_predict=12, modes=1, predict_all=True, obs_length=9, start_length=0,
-                 args=None):
-        self.model.eval()
+    def _mode_scenes(self, observed, scene_goal, batch_split, n_predict, modes):
         self.model.d_steps = 0
         if modes is not None:
             self.model.k = modes
-        with torch.no_grad():
-            xy = paths_to_xy(paths)
-            batch_split = [0, xy.shape[1]]
-            normalize = bool(getattr(args, 'normalize_scene', False))
-            if normalize:
-                xy, rotation, center, scene_goal = center_scene(xy, obs_length, goals=np.asarray(scene_goal))
-            xy = torch.Tensor(xy)
-            scene_goal = torch.Tensor(np.asarray(scene_goal))
-            batch_split = torch.Tensor(batch_split).long()
-            multimodal_outputs = {}
-            _, output_scenes_list, _, _ = self.model(xy[:obs_length], scene_goal, batch_split, n_predict=n_predict)
-            for num_p, output_scenes in enumerate(output_scenes_list):
-                output_scenes = output_scenes.cpu().numpy()
-                if normalize:
-                    output_scenes = inverse_scene(output_scenes, rotation, center)
-                output_primary = output_scenes[-n_predict:, 0]
-                output_neighs = output_scenes[-n_predict:, 1:]
-                multimodal_outputs[num_p] = [output_primary, output_neighs if num_p == 0 else []]
-        return multimodal_outputs
-
-    def batch_decode_supported(self):
-        """predict_batch_xy serves every generator except those whose interaction module carries its own LSTM state
-        (NearestNeighborLSTM, TrajectronPooling): that state is not replicated per mode."""
-        return not multimodal.stateful_pool(self.model.generator)
+        return self.model(observed, scene_goal, batch_split, n_predict=n_predict)[1]
 
     def predict_batch_xy(self, xys, scene_goals=None, n_predict=12, obs_length=9, start_length=0, args=None, modes=1,
                          noise=None, max_rows=None):
@@ -263,33 +185,18 @@ class SGANPredictor(object):
         of the generator apply as in __call__.  noise: explicit [modes, B, noise_dim] vectors instead of the draw.
         max_rows: rows of one decode (default: multimodal.rows_per_decode); more modes are decoded in groups."""
         gen = self.model.generator
-        if not self.batch_decode_supported():
-            raise NotImplementedError("batched decoding of a generator whose interaction module keeps an LSTM state "
-                                      "is not built; call the predictor scene by scene")
-        self.model.eval()
-        modes = int(modes)
-        if modes < 1:
-            raise ValueError("modes must be >= 1")
-        if not xys:
-            return []
-        normalize = bool(getattr(args, 'normalize_scene', False))
-        with torch.no_grad():
-            # sgan.py:603 feeds xy[:obs_length]: start_length does not apply to the generator
-            observed, split, rotation, center = multimodal.observed_batch(gen, xys, obs_length, 0, normalize)
-            device = observed.device
-            B, nd = len(xys), int(gen.noise_dim)
+
+        def context(device, split, modes):
+            B, nd = len(split) - 1, int(gen.noise_dim)
             if gen.no_noise:
-                noise = None
+                draws = None
             elif noise is not None:
-                noise = torch.as_tensor(noise, dtype=torch.float32).to(device).reshape(modes, B, nd).contiguous()
+                draws = torch.as_tensor(noise, dtype=torch.float32).to(device).reshape(modes, B, nd).contiguous()
             elif gen.fixed_noise is not None:
                 fixed = torch.as_tensor(gen.fixed_noise, dtype=torch.float32).to(device).reshape(1, 1, nd)
-                noise = fixed.expand(modes, B, nd).contiguous()
+                draws = fixed.expand(modes, B, nd).contiguous()
             else:
-                noise = get_noise((modes, B, nd), gen.noise_type, device=device).float().contiguous()
-            lin = gen.mlp_decoder_context[0]
-            w = lin.weight.detach().to(device=device, dtype=torch.float32).contiguous()
-            b = lin.bias.detach().to(device=device, dtype=torch.float32).contiguous()
-            context = multimodal.sgan_context(w, b, noise, multimodal.group_of_rows(split, device), B, nd)
-            pred = multimodal.predict_modes(gen, observed, split, n_predict, modes, context, max_rows)
-            return multimodal.scene_results(pred, split, modes, n_predict, normalize, rotation, center)
+                draws = get_noise((modes, B, nd), gen.noise_type, device=device).float().contiguous()
+            w, b = linear_on(gen.mlp_decoder_context[0], device)
+            return multimodal.sgan_context(w, b, draws, multimodal.group_of_rows(split, device), B, nd)
+        return self._predict_batch_xy(xys, n_predict, obs_length, start_length, args, modes, max_rows, context)

@@ -9,14 +9,11 @@ constructor arguments and state_dict keys.  Training (prediction encoder, KL ter
 model.train() + forward raises.  VAEPredictor.predict_batch_xy decodes every mode of many scenes at
 once (the evaluator's path, ../multimodal.py).
 """
-import ctypes
-
 import numpy as np
 import torch
 
 from .. import _lib, multimodal
-from ..data import paths_to_xy
-from ..engine import _ptr, _stream
+from ..engine import _ptr, _stream, linear_on
 from ..lstm.lstm import LSTM, center_scene, drop_distant, inverse_scene  # noqa: F401
 from ..lstm.modules import Hidden2Normal, InputEmbedding
 
@@ -95,31 +92,10 @@ class VAE(torch.nn.Module):
         if not self.desire:
             raise NotImplementedError("desire=False (latent prior from vae_encoder_x) is not built")
         body = self._body[0]
-        handle = body._engine()
-        device = handle.device
-        layout = body._layouts.get(batch_split.tolist() if torch.is_tensor(batch_split) else batch_split,
-                                   device=body._device())
-        M = layout.num_tracks
-        obs = body._to_device(observed, device)
-        obs_length = int(obs.shape[0])
-        truth = None
-        if prediction_truth is not None:
-            if isinstance(prediction_truth, (list, tuple)):
-                prediction_truth = torch.stack(list(prediction_truth))
-            truth = body._to_device(prediction_truth, device)
-            n_decode = int(truth.shape[0])
-            if n_decode == 0:
-                truth = None
-        else:
-            n_decode = int(n_predict) - 1
-        S, S_enc = obs_length - 1 + n_decode, obs_length - 1
-        f32 = dict(dtype=torch.float32, device=device)
-        normals0, positions0 = torch.empty((S, M, 5), **f32), torch.empty((S, M, 2), **f32)
-        h0, c0 = torch.empty((M, self.hidden_dim), **f32), torch.empty((M, self.hidden_dim), **f32)
-        handle.forward_steps(layout, obs, truth, n_decode, 0, S_enc, normals0, positions0, h0, c0)
+        seq = body._encode(body._sequence(observed, batch_split, prediction_truth, n_predict))
+        device, M = seq.handle.device, seq.layout.num_tracks
         lib = _lib.load()
-        w = self.vae_decoder.fc.weight.detach().to(device=device, dtype=torch.float32).contiguous()
-        b = self.vae_decoder.fc.bias.detach().to(device=device, dtype=torch.float32).contiguous()
+        w, b = linear_on(self.vae_decoder.fc, device)
         rel_list, pred_list = [], []
         for k in range(self.num_modes):
             if self.fixed_z is not None:
@@ -127,65 +103,26 @@ class VAE(torch.nn.Module):
             else:      # prior N(0, exp(1) I): z_mu_obs = 0, z_var_log_obs = 1 (vae.py:277-278)
                 z = sample_multivariate_distribution(torch.zeros(M, self.latent_dim), torch.ones(M, self.latent_dim))
             z = z.to(device).contiguous()
-            h, c = h0.clone(), c0.clone()
-            normals, positions = normals0.clone(), positions0.clone()
-            with torch.cuda.device(device):
-                _lib.check(lib.tb2_vae_scale_hidden(_ptr(w), _ptr(b), _ptr(z), _ptr(h), M, int(self.hidden_dim),
-                                                    int(self.latent_dim), _stream(device)))
-            handle.forward_steps(layout, obs, truth, n_decode, S_enc, S, normals, positions, h, c)
-            if observed.device != device:
-                normals, positions = body._to_host(normals, positions)
+
+            def scale_hidden(h, c):
+                with torch.cuda.device(device):
+                    _lib.check(lib.tb2_vae_scale_hidden(_ptr(w), _ptr(b), _ptr(z), _ptr(h), M, int(self.hidden_dim),
+                                                        int(self.latent_dim), _stream(device)))
+            normals, positions = body._decode(seq, scale_hidden, seed=False)
             rel_list.append(normals)
             pred_list.append(positions)
         return rel_list, pred_list, None, None
 
 
-class VAEPredictor(object):
+class VAEPredictor(multimodal.ModesPredictor):
     """vae.py:347-398."""
 
-    def __init__(self, model):
-        self.model = model
+    def _lstm_model(self):
+        return self.model._body[0]
 
-    def save(self, state, filename):
-        with open(filename, 'wb') as f:
-            torch.save(self, f)
-        with open(filename + '.state', 'wb') as f:
-            torch.save(state, f)
-
-    @staticmethod
-    def load(filename):
-        with open(filename, 'rb') as f:
-            return torch.load(f, weights_only=False)
-
-    def __call__(self, paths, scene_goal, n_predict=12, modes=1, predict_all=True, obs_length=9, start_length=0,
-                 args=None):
-        self.model.eval()
+    def _mode_scenes(self, observed, scene_goal, batch_split, n_predict, modes):
         self.model.num_modes = modes
-        with torch.no_grad():
-            xy = paths_to_xy(paths)
-            batch_split = [0, xy.shape[1]]
-            normalize = bool(getattr(args, 'normalize_scene', False))
-            if normalize:
-                xy, rotation, center, scene_goal = center_scene(xy, obs_length, goals=np.asarray(scene_goal))
-            xy = torch.Tensor(xy)
-            scene_goal = torch.Tensor(np.asarray(scene_goal))
-            batch_split = torch.Tensor(batch_split).long()
-            multimodal_outputs = {}
-            _, output_scenes_list, _, _ = self.model(xy[start_length:obs_length], scene_goal, batch_split,
-                                                     n_predict=n_predict)
-            for num_p, output_scenes in enumerate(output_scenes_list):
-                output_scenes = output_scenes.cpu().numpy()
-                if normalize:
-                    output_scenes = inverse_scene(output_scenes, rotation, center)
-                output_primary = output_scenes[-n_predict:, 0]
-                output_neighs = output_scenes[-n_predict:, 1:]
-                multimodal_outputs[num_p] = [output_primary, output_neighs if num_p == 0 else []]
-        return multimodal_outputs
-
-    def batch_decode_supported(self):
-        """predict_batch_xy serves every model except those whose interaction module carries its own LSTM state
-        (NearestNeighborLSTM, TrajectronPooling): that state is not replicated per mode."""
-        return not multimodal.stateful_pool(self.model._body[0])
+        return self.model(observed, scene_goal, batch_split, n_predict=n_predict)[1]
 
     def predict_batch_xy(self, xys, scene_goals=None, n_predict=12, obs_length=9, start_length=0, args=None, modes=1,
                          z=None, max_rows=None):
@@ -196,33 +133,16 @@ class VAEPredictor(object):
         per call, on the device, one per (mode, track) from the prior N(0, e I) as in __call__; the model's `fixed_z`
         ([modes, M, latent_dim] over the M tracks of all scenes) replaces the draw, and so does z (same shape).
         max_rows: rows of one decode (default: multimodal.rows_per_decode); more modes are decoded in groups."""
-        body = self.model._body[0]
-        if not self.batch_decode_supported():
-            raise NotImplementedError("batched decoding of a model whose interaction module keeps an LSTM state "
-                                      "is not built; call the predictor scene by scene")
-        self.model.eval()
         if not self.model.desire:
             raise NotImplementedError("desire=False (latent prior from vae_encoder_x) is not built")
-        modes = int(modes)
-        if modes < 1:
-            raise ValueError("modes must be >= 1")
-        if not xys:
-            return []
-        normalize = bool(getattr(args, 'normalize_scene', False))
-        with torch.no_grad():
-            observed, split, rotation, center = multimodal.observed_batch(body, xys, obs_length, start_length,
-                                                                          normalize)
-            device = observed.device
+
+        def context(device, split, modes):
             M, L = int(split[-1]), int(self.model.latent_dim)
-            if z is None:
-                z = self.model.fixed_z
-            if z is not None:
-                z = torch.as_tensor(z, dtype=torch.float32).to(device).reshape(modes, M, L).contiguous()
+            draws = self.model.fixed_z if z is None else z
+            if draws is not None:
+                draws = torch.as_tensor(draws, dtype=torch.float32).to(device).reshape(modes, M, L).contiguous()
             else:      # prior N(0, exp(1) I): z_mu_obs = 0, z_var_log_obs = 1 (vae.py:277-278)
-                z = torch.randn((modes, M, L), device=device).mul_(float(np.exp(0.5)))
-            fc = self.model.vae_decoder.fc
-            w = fc.weight.detach().to(device=device, dtype=torch.float32).contiguous()
-            b = fc.bias.detach().to(device=device, dtype=torch.float32).contiguous()
-            pred = multimodal.predict_modes(body, observed, split, n_predict, modes,
-                                            multimodal.vae_context(w, b, z, L), max_rows)
-            return multimodal.scene_results(pred, split, modes, n_predict, normalize, rotation, center)
+                draws = torch.randn((modes, M, L), device=device).mul_(float(np.exp(0.5)))
+            w, b = linear_on(self.model.vae_decoder.fc, device)
+            return multimodal.vae_context(w, b, draws, L)
+        return self._predict_batch_xy(xys, n_predict, obs_length, start_length, args, modes, max_rows, context)
