@@ -651,6 +651,15 @@ MODEL_SPECS = {
                             embedding_arch="one_layer"),
     "directional_p29": dict(type_="directional", hidden_dim=128, cell_side=0.6, n=12, out_dim=29,
                             embedding_arch="one_layer"),
+    # grids whose first Linear each first-layer kernel of the forward takes (tests/test_step_forward.py): the row
+    # kernel's 64-column chunk (n = 16), weights too large for it (cells x C > 1280), no embedding (the grid itself)
+    "directional_n16": dict(type_="directional", hidden_dim=128, cell_side=0.6, n=16, out_dim=256,
+                            embedding_arch="one_layer"),
+    "occupancy_n36": dict(type_="occupancy", hidden_dim=128, cell_side=0.3, n=36, out_dim=64,
+                          embedding_arch="one_layer"),
+    "directional_n26": dict(type_="directional", hidden_dim=128, cell_side=0.4, n=26, out_dim=64,
+                            embedding_arch="one_layer"),
+    "occupancy_raw": dict(type_="occupancy", hidden_dim=128, cell_side=0.6, n=8, out_dim=64, embedding_arch="None"),
 }
 
 
@@ -705,16 +714,22 @@ def pool_config(kind):
     return None if spec is None else PoolConfig(**spec)
 
 
-def random_weights(kind, seed=0, scale=1.0, embedding_dim=64, hidden_dim=128, relu_bias=None):
+def random_weights(kind, seed=0, scale=1.0, embedding_dim=64, hidden_dim=128, relu_bias=None, out_dim=None,
+                   pool_to_input=True):
     """Seeded weights in the reference's state_dict layout (uniform(-1/sqrt(fan_in), ..) like
     torch's default init, times `scale`).  numpy RandomState => identical on every machine.
 
     relu_bias = beta: the biases of the grid embedding's Linears (pool.embedding.*.bias) become +beta
     (even units) and -beta (odd units).  The pre-activations of those ReLUs then stay far from 0, so
     rounding differences between implementations cannot flip a ReLU mask, and half of the units are
-    still dead, so a backward that ignores the mask is still caught.  The other weights are unchanged."""
+    still dead, so a backward that ignores the mask is still caught.  The other weights are unchanged.
+
+    out_dim: the interaction module's out_dim instead of the kind's.  pool_to_input=False: the LSTM input is
+    the embedding alone (the pooled vector is added to h, lstm.py:151), so weight_ih has embedding_dim columns."""
     rng = np.random.RandomState(seed)
     cfg = pool_config(kind)
+    if cfg is not None and out_dim is not None:
+        cfg.out_dim = out_dim
     W = {}
 
     def lin(name_w, name_b, out_f, in_f):
@@ -773,6 +788,8 @@ def random_weights(kind, seed=0, scale=1.0, embedding_dim=64, hidden_dim=128, re
     lin("input_embedding.input_embeddings.0.weight", "input_embedding.input_embeddings.0.bias", E - 2, 2)
     lin("goal_embedding.input_embeddings.0.weight", "goal_embedding.input_embeddings.0.bias", E - 2, 2)
     k = scale / math.sqrt(H)
+    if not pool_to_input:
+        pool_dim = 0
     for ph in ("encoder", "decoder"):
         W[ph + ".weight_ih"] = rng.uniform(-k, k, size=(4 * H, E + pool_dim)).astype(F32)
         W[ph + ".weight_hh"] = rng.uniform(-k, k, size=(4 * H, H)).astype(F32)

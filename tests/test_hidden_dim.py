@@ -5,11 +5,11 @@ H = 64 and 256 (tests/golden/hidden_dim_golden.npz, oracle/make_hidden_dim_golde
 before it reads any file.
 
 GPU:
-  * forwards of every interaction module at H = 32, 64, 96, 192, 256, with the tensor cores on and with TB2_DISABLE_TC=1,
+  * forwards of every interaction module at every width 32 .. 256, with the tensor cores on and with TB2_DISABLE_TC=1,
     against the oracle, asserting which gate kernel ran (`lstm_gates_tc` at H = 64, 128, 192, 256); the cluster of one
     (H = 64) against the two-CTA kernel on the zero-padded H = 128 model, bit for bit;
   * one Trainer.train_batch step of vanilla / occupancy (with a collision term) / directional / social (one_layer and
-    two_layer) at H = 64, 96, 256 against the float64 restatement, with bit-identical reruns;
+    two_layer) at every width but 128 against the float64 restatement, with bit-identical reruns;
   * the reference's own Trainer.train_batch, Trainer.loop and predict_scene driving this package's model and
     predictor, evaluate_file and the trainer CLI file to file (also continuing a reference checkpoint);
   * S-GAN and VAE: batched multi-mode predictions bit-identical to the per-scene call, and the oracle;
@@ -161,7 +161,7 @@ def test_cli_refuses_width_before_reading_data(H, tmp_path, monkeypatch):
 # ---------------------------------------------------------------------------------------------------------------------
 # GPU: forwards of every interaction module against the oracle
 # ---------------------------------------------------------------------------------------------------------------------
-GPU_WIDTHS = [32, 64, 96, 192, 256]
+GPU_WIDTHS = list(range(32, 257, 32))
 POOL_KINDS = ["vanilla", "occupancy", "directional", "social", "hiddenstatemlp", "attentionmlp", "nn", "nn_lstm",
               "traj_pool"]
 NONGRID = {"hiddenstatemlp", "attentionmlp", "nn", "nn_lstm", "traj_pool"}
@@ -281,7 +281,7 @@ TRAIN_CASES = [
     ("social_default", "social_default", "pred", 0.0, 0.2, 5),
     ("social_two_layer", "social_d96", "pred", 0.0, 0.2, 7),
 ]
-TRAIN_WIDTHS = [64, 96, 256]
+TRAIN_WIDTHS = [32, 64, 96, 160, 192, 224, 256]      # 128: test_training.py and the others
 # The one case above 1e-4: occupancy with a collision term at H = 64 on the tensor cores measures up to 8e-4 (its fp32
 # path: 5.9e-6).  The zero-padded H = 128 copy of the model, run by the two-CTA kernel of the H = 128 build, gives the
 # same bits in the forward and the same error (test_cluster_of_one_training_step_equals_two_cta_kernel), so the error
@@ -289,10 +289,16 @@ TRAIN_WIDTHS = [64, 96, 256]
 CASE_GATES = {("occupancy_col", 64, True): 1e-3}
 
 
+# (case, H) -> weight seed where the default H + 9 puts a fed-back primary within 1e-5 cells of a cell edge
+# (directional at H = 32: 1.4e-6 cells)
+WEIGHT_SEEDS = {("directional", 32): 42}
+
+
 def _train_inputs(case, H):
     _, kind, _, _, _, dseed = case
     xy, bs = O.synthetic_scenes(10, 12, seed=dseed, ragged=True, nan_tracks=True)
-    return xy, bs, O.random_weights(kind, seed=H + 9, hidden_dim=H, relu_bias=3.0)
+    seed = WEIGHT_SEEDS.get((case[0], H), H + 9)
+    return xy, bs, O.random_weights(kind, seed=seed, hidden_dim=H, relu_bias=3.0)
 
 
 def _check_margins(case, stats):

@@ -17,9 +17,32 @@ import torch.nn.functional as F
 NAN = float("nan")
 
 
-def _grid(pool_cfg, W, obs1, obs2, hidden, dtype, stats, primary_edges):
+def _mm(x, w, kernel=None):
+    """x @ w.T, or kernel.mm(x, w) when a kernel emulation (see bf16_product) is given."""
+    mm = getattr(kernel, "mm", None)
+    return x @ w.T if mm is None else mm(x, w)
+
+
+def bf16_product(passes=3):
+    """x @ w.T as the tensor-core kernels compute it from fp32 operands: hi = bf16(v), lo = bf16(v - hi) of both,
+    then hi.hi + hi.lo + lo.hi summed in float64 (passes=3); passes=2 drops lo.hi."""
+    def split(v):
+        hi = v.to(torch.bfloat16).to(v.dtype)
+        return hi, (v - hi).to(torch.bfloat16).to(v.dtype)
+
+    def mm(x, w):
+        (xh, xl), (wh, wl) = split(x), split(w)
+        out = xh @ wh.T + xh @ wl.T
+        return out + xl @ wh.T if passes == 3 else out
+    return mm
+
+
+def _grid(pool_cfg, W, obs1, obs2, hidden, dtype, stats, primary_edges, kernel=None):
     """[B, N, ...] padded -> pooled [B*N, out] (gridbased_pooling.py:112-170,227-305,308-335), cf.
-    oracle.lstm_oracle.occupancy_grid / pool_forward.
+    oracle.lstm_oracle.occupancy_grid / pool_forward.  embedding_arch None / 'None': the grid itself.
+
+    kernel: an emulation of a kernel's arithmetic: kernel.mm(x, w) replaces the embedding's products and
+    kernel.grid(grid [B*N, C, n, n]) edits the grid before the embedding (either may be absent).
 
     The cells are binned in fp32 on the fp32 positions, like the reference, whatever `dtype` the
     arithmetic runs in.  The reference writes the grid with ONE index_put (gridbased_pooling.py:293): in
@@ -84,10 +107,12 @@ def _grid(pool_cfg, W, obs1, obs2, hidden, dtype, stats, primary_edges):
     # where a cell holds exactly 0: the writers of a cell that an out-of-range pair (value `constant` = 0)
     # overwrote last receive no gradient
     grid = F.lp_pool2d(grid.transpose(1, 2).reshape(B * N, C, n, n), 1, 1)
+    if getattr(kernel, "grid", None) is not None:
+        grid = kernel.grid(grid)
     x = grid.reshape(B * N, -1)
-    n_layers = {"one_layer": 1, "two_layer": 2, "three_layer": 3}[pool_cfg.embedding_arch]
+    n_layers = {None: 0, "None": 0, "one_layer": 1, "two_layer": 2, "three_layer": 3}[pool_cfg.embedding_arch]
     for l in range(n_layers):
-        z = x @ W["pool.embedding.%d.weight" % (2 * l)].T + W["pool.embedding.%d.bias" % (2 * l)]
+        z = _mm(x, W["pool.embedding.%d.weight" % (2 * l)], kernel) + W["pool.embedding.%d.bias" % (2 * l)]
         _note(stats, "relu_pool%d" % l, float(z.detach().abs().min()))
         x = torch.relu(z)
     return x
@@ -277,8 +302,68 @@ def nongrid_pool_ragged(pool_cfg, W, h, obs1, obs2, bs, pad_to_batch_max=True, d
     return _pool_lstm(Wp, out, pool_state) if pool_cfg.type_ == "nn_lstm" else out
 
 
+def _pad(x, bs, fill):
+    """ragged [M, ...] -> padded [B, Nmax, ...] (generate_pooling_inputs, lstm.py:25-42)."""
+    B = len(bs) - 1
+    n_max = max(bs[b + 1] - bs[b] for b in range(B))
+    out = torch.full((B, n_max) + tuple(x.shape[1:]), fill, dtype=x.dtype)
+    for b in range(B):
+        out[b, :bs[b + 1] - bs[b]] = x[bs[b]:bs[b + 1]]
+    return out
+
+
+def pool_state_zeros(pool_cfg, M, dtype):
+    """The interaction-encoder state of nn_lstm / traj_pool after pool.reset (lstm.py:213-216), else None."""
+    if getattr(pool_cfg, "type_", None) in ("nn_lstm", "traj_pool"):
+        return {"h": torch.zeros(M, pool_cfg.hidden_dim, dtype=dtype), "c": torch.zeros(M, pool_cfg.hidden_dim, dtype=dtype)}
+    return None
+
+
+def step(W, pool_cfg, phase, h, c, obs1, obs2, batch_split, hidden_dim, dtype, pool_to_input=True, stats=None,
+         pad_to_batch_max=True, pool_state=None, kernel=None):
+    """LSTM.step (lstm.py:91-168): h, c [M, H] `dtype`, obs1 / obs2 [M, 2] fp32 (NaN = absent) -> (h', c', normal
+    [M, 5]); rows absent at obs1 or obs2 keep h, c and get normal = NaN.
+
+    pool_to_input=False: the pooled vector of the present rows is added to their h before the W_hh product
+    (lstm.py:151), and the LSTM input is the embedding alone.  pool_state: see pool_state_zeros (advanced in place).
+    kernel: see _grid; kernel.mm also replaces the gate product."""
+    bs = [int(v) for v in batch_split]
+    M = obs2.shape[0]
+    mask = ~torch.isnan(obs1[:, 0]) & ~torch.isnan(obs2[:, 0])
+    vel = (obs2 - obs1)[mask].to(dtype)
+    e = torch.relu((vel * 4.0) @ W["input_embedding.input_embeddings.0.weight"].T +
+                   W["input_embedding.input_embeddings.0.bias"])
+    x = torch.cat([e, torch.zeros(e.shape[0], 2, dtype=dtype)], dim=1)
+    hm = h[mask]
+    if getattr(pool_cfg, "type_", None) in NONGRID:
+        pooled = nongrid_pool_ragged(pool_cfg, W, h.detach(), obs1, obs2, bs, pad_to_batch_max, dtype, pool_state,
+                                     stats)[mask]
+    elif pool_cfg is not None:
+        pooled = _grid(pool_cfg, W, _pad(obs1, bs, NAN), _pad(obs2, bs, NAN), _pad(h, bs, NAN), dtype, stats,
+                       primary_edges=phase == "decoder", kernel=kernel)[_pad(mask, bs, False).reshape(-1)]
+    if pool_cfg is not None:
+        if pool_to_input:
+            x = torch.cat([x, pooled], dim=1)
+        else:
+            hm = hm + pooled
+    gates = (_mm(x, W[phase + ".weight_ih"], kernel) + W[phase + ".bias_ih"] + _mm(hm, W[phase + ".weight_hh"], kernel)
+             + W[phase + ".bias_hh"])
+    H = hidden_dim
+    i, f = torch.sigmoid(gates[:, :H]), torch.sigmoid(gates[:, H:2 * H])
+    g, o = torch.tanh(gates[:, 2 * H:3 * H]), torch.sigmoid(gates[:, 3 * H:])
+    c2 = f * c[mask] + i * g
+    h2 = o * torch.tanh(c2)
+    raw = h2 @ W["hidden2normal.linear.weight"].T + W["hidden2normal.linear.bias"]
+    nrm = torch.cat([raw[:, :2], 0.01 + 0.2 * torch.sigmoid(raw[:, 2:4]), 0.7 * torch.sigmoid(raw[:, 4:5])], dim=1)
+    idx = mask.nonzero().flatten()
+    h_out = h.index_copy(0, idx, h2)
+    c_out = c.index_copy(0, idx, c2)
+    normal = torch.full((M, 5), NAN, dtype=dtype).index_copy(0, idx, nrm)
+    return h_out, c_out, normal
+
+
 def forward(W, pool_cfg, observed, batch_split, prediction_truth=None, n_predict=None, hidden_dim=128,
-            dtype=torch.float32, stats=None, feed_back=None, pad_to_batch_max=True):
+            dtype=torch.float32, stats=None, feed_back=None, pad_to_batch_max=True, pool_to_input=True, kernel=None):
     """W: dict of `dtype` tensors (requires_grad as wanted).  Returns rel [S, M, 5] (`dtype`), pred [S, M, 2]
     (fp32: the positions the model feeds back are fp32 data, as in the reference).  stats: see _grid.
 
@@ -287,53 +372,18 @@ def forward(W, pool_cfg, observed, batch_split, prediction_truth=None, n_predict
     exact for that implementation's trajectory and no fed-back position can be binned differently.
 
     pad_to_batch_max: with a non-grid pool, False gives each scene its own slots (the per-scene layout): the
-    attention keys stop at the scene's tracks and Trajectron's sums at its scene."""
+    attention keys stop at the scene's tracks and Trajectron's sums at its scene.  pool_to_input, kernel: see step."""
     bs = [int(v) for v in batch_split]
-    B = len(bs) - 1
     M = observed.shape[1]
-    n_max = max(bs[i + 1] - bs[i] for i in range(B))
     prim = torch.tensor(bs[:-1])
     h = torch.zeros(M, hidden_dim, dtype=dtype)
     c = torch.zeros(M, hidden_dim, dtype=dtype)
     truth = [None] * (n_predict - 1) if n_predict is not None else [t.clone() for t in prediction_truth]
-    nongrid = getattr(pool_cfg, "type_", None) in NONGRID
-    pool_state = None
-    if nongrid and pool_cfg.type_ in ("nn_lstm", "traj_pool"):      # pool.reset(...) at the start (lstm.py:213-216)
-        pool_state = {"h": torch.zeros(M, pool_cfg.hidden_dim, dtype=dtype),
-                      "c": torch.zeros(M, pool_cfg.hidden_dim, dtype=dtype)}
+    pool_state = pool_state_zeros(pool_cfg, M, dtype)
 
-    def pad(x, fill):
-        out = torch.full((B, n_max) + tuple(x.shape[1:]), fill, dtype=x.dtype)
-        for b in range(B):
-            out[b, :bs[b + 1] - bs[b]] = x[bs[b]:bs[b + 1]]
-        return out
-
-    def step(phase, h, c, obs1, obs2):
-        mask = ~torch.isnan(obs1[:, 0]) & ~torch.isnan(obs2[:, 0])
-        vel = (obs2 - obs1)[mask].to(dtype)
-        e = torch.relu((vel * 4.0) @ W["input_embedding.input_embeddings.0.weight"].T +
-                       W["input_embedding.input_embeddings.0.bias"])
-        x = torch.cat([e, torch.zeros(e.shape[0], 2, dtype=dtype)], dim=1)
-        if nongrid:
-            pooled = nongrid_pool_ragged(pool_cfg, W, h.detach(), obs1, obs2, bs, pad_to_batch_max, dtype, pool_state, stats)
-            x = torch.cat([x, pooled[mask]], dim=1)
-        elif pool_cfg is not None:
-            pooled = _grid(pool_cfg, W, pad(obs1, NAN), pad(obs2, NAN), pad(h, NAN), dtype, stats,
-                           primary_edges=phase == "decoder")
-            x = torch.cat([x, pooled[pad(mask, False).reshape(-1)]], dim=1)
-        gates = x @ W[phase + ".weight_ih"].T + W[phase + ".bias_ih"] + h[mask] @ W[phase + ".weight_hh"].T + W[phase + ".bias_hh"]
-        H = hidden_dim
-        i, f = torch.sigmoid(gates[:, :H]), torch.sigmoid(gates[:, H:2 * H])
-        g, o = torch.tanh(gates[:, 2 * H:3 * H]), torch.sigmoid(gates[:, 3 * H:])
-        c2 = f * c[mask] + i * g
-        h2 = o * torch.tanh(c2)
-        raw = h2 @ W["hidden2normal.linear.weight"].T + W["hidden2normal.linear.bias"]
-        nrm = torch.cat([raw[:, :2], 0.01 + 0.2 * torch.sigmoid(raw[:, 2:4]), 0.7 * torch.sigmoid(raw[:, 4:5])], dim=1)
-        idx = mask.nonzero().flatten()
-        h_out = h.index_copy(0, idx, h2)
-        c_out = c.index_copy(0, idx, c2)
-        normal = torch.full((M, 5), NAN, dtype=dtype).index_copy(0, idx, nrm)
-        return h_out, c_out, normal
+    def step_(phase, h, c, obs1, obs2):
+        return step(W, pool_cfg, phase, h, c, obs1, obs2, bs, hidden_dim, dtype, pool_to_input, stats,
+                    pad_to_batch_max, pool_state, kernel)
 
     normals, positions = [], []
     if observed.shape[0] == 2:
@@ -344,7 +394,7 @@ def forward(W, pool_cfg, observed, batch_split, prediction_truth=None, n_predict
         return feed_back[i] if feed_back is not None else positions[i].detach()
 
     for t in range(observed.shape[0] - 1):
-        h, c, normal = step("encoder", h, c, observed[t], observed[t + 1])
+        h, c, normal = step_("encoder", h, c, observed[t], observed[t + 1])
         normals.append(normal)
         positions.append(observed[t + 1] + normal[:, :2].to(observed.dtype))
     seq = [observed[-1].clone()] + truth
@@ -361,7 +411,7 @@ def forward(W, pool_cfg, observed, batch_split, prediction_truth=None, n_predict
             obs2 = obs2.clone()
             obs2[prim] = fed(-1)[prim]
             seq[k + 1] = obs2
-        h, c, normal = step("decoder", h, c, obs1, obs2)
+        h, c, normal = step_("decoder", h, c, obs1, obs2)
         normals.append(normal)
         positions.append(obs2 + normal[:, :2].to(obs2.dtype))
     return torch.stack(normals), torch.stack(positions)

@@ -1103,9 +1103,12 @@ int launch_pool_mlp(const tb2_lstm* m, const tb2_layout* l, Workspace* ws, float
     if (want_split && !direct_split && pooled_out == nullptr) pooled_out = ws->pooled;
     int rc_all = TB2_OK;
     if (m->n_mlp == 0) {
-        dense_grid_kernel<<<l->M, 128, 0, st>>>(ws->win_count, ws->win_ent, ws->win_val, ws->lat,
-                                                l->row_scene, l->scene_off, m->benc, pooled_out, m->C,
-                                                m->cells, nm1, m->cfg.constant, m->cfg.pool_type);
+        {
+            KernelTimer kt("dense_grid", st);
+            dense_grid_kernel<<<l->M, 128, 0, st>>>(ws->win_count, ws->win_ent, ws->win_val, ws->lat,
+                                                    l->row_scene, l->scene_off, m->benc, pooled_out, m->C,
+                                                    m->cells, nm1, m->cfg.constant, m->cfg.pool_type);
+        }
         TB2_LAUNCH_CHECK();
         if (want_split) rc_all = launch_split_bf16(pooled_out, pool_hi, pool_lo, (size_t)l->M * m->pool_out, st);
         return rc_all;
