@@ -9,6 +9,8 @@ kernels compute wrong results; only their times mean anything:
   1  accumulators summed in registers: no shared-memory accumulator loads or stores
   2  every tile reads cell 0's weights: the same requests, always L2 hits on one slab per column chunk
   3  no mma.sync: the products replaced by a few integer operations on the same fragments
+  4  every tile reads cell 0's weights from a copy each warp makes in shared memory before the loop: no L2 weight
+     traffic at all (2 keeps the same L2 requests in flight)
 Prints one JSON line per run and a summary line with the range of each variant.
 """
 import argparse
@@ -21,7 +23,7 @@ import tempfile
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-VARIANTS = {1: "no accumulator traffic", 2: "weights from cell 0", 3: "no mma"}
+VARIANTS = {1: "no accumulator traffic", 2: "weights from cell 0", 3: "no mma", 4: "weights from shared memory"}
 
 
 def build_variant(n, out_dir):

@@ -16,7 +16,7 @@ does, computed from the shapes:
     padded row slots of those tiles;
   * a model (not a measurement) of the shared-memory wavefronts of one CTA's tile loop, from the same winners.  A warp
     access costs, per group of lanes the hardware serves together, the larger of the distinct 4-byte words over 32 and
-    the most distinct words in one bank; times 16 warps.  "before_tile_list" and "tile_list" take all 32 lanes as one
+    the most distinct words in one bank; times the warps of a CTA (16, or 8 for the 32-column layouts).  "before_tile_list" and "tile_list" take all 32 lanes as one
     group (the tile layout before the flat tile list: padding rows load the zero latent row and read-modify-write
     dummy accumulator rows, 32-bit A loads from separate hi / lo rows; and the flat tile list: padding rows touch no
     accumulator, one 128-bit (hi, lo) A load per row, two 32-bit slot words, two 64-bit loads and stores per
@@ -24,7 +24,9 @@ does, computed from the shapes:
     a 128-bit access a quarter-warp (rows 2q, 2q + 1) at a time, which is where two accumulator rows of a tile collide:
     "tile_list_64bit_stride264" is the flat tile list again, "packed_128bit_stride<S>" the current layout (one slot
     word, one 128-bit load and store per accumulator row, the warp's 16 columns of a row contiguous) at row strides of
-    264, 272 (the kernel's) and 280 floats;
+    264, 272 and 280 floats, "warp32_128bit_stride<S>" the kernel's layout (8 warps of 32 columns: a tile's slot word
+    and A rows loaded once per warp, two adjacent 128-bit words per accumulator row and lane) at strides of 256 to 280
+    floats (the kernel's is 260);
   * CTAs per SM (cudaOccupancyMaxActiveBlocksPerMultiprocessor), hence the number of waves.
 Prints one JSON line with the GPU's name and power limit.
 """
@@ -137,6 +139,7 @@ def wavefronts_per_cta(xy_frames, bs, cfg):
 
 
 ACC_STRIDES = (264, 272, 280)
+ACC_STRIDES_32 = (256, 260, 264, 268, 272, 276, 280)
 
 
 def phased_wavefronts_per_cta(xy_frames, bs, cfg):
@@ -144,7 +147,11 @@ def phased_wavefronts_per_cta(xy_frames, bs, cfg):
     accesses per quarter-warp (see the module docstring): {layout: wavefronts}."""
     cap, cells = GROUP_CAP, cfg.n * cfg.n
     rows_per_group = GROUP_CAP // PEDS * PEDS
-    names = ["tile_list_64bit_stride264"] + ["packed_128bit_stride%d" % s for s in ACC_STRIDES]
+    names = (["tile_list_64bit_stride264"] + ["packed_128bit_stride%d" % s for s in ACC_STRIDES] +
+             ["warp32_128bit_stride%d" % s for s in ACC_STRIDES_32])
+    n16 = 1 + len(ACC_STRIDES)
+    warps = np.array([16] * n16 + [8] * len(ACC_STRIDES_32))      # warps of a CTA walking the whole tile list
+    slot_words = np.array([2] + [1] * (len(names) - 1))
     tot = np.zeros(len(names))
     n = 0
     for xy in xy_frames:
@@ -170,14 +177,18 @@ def phased_wavefronts_per_cta(xy_frames, bs, cfg):
                             r4 = [e[0] for e in s8[4 * h:4 * h + 4] if e is not None]
                             acc[0] += 2 * 2 * _wavefronts([r * 264 + 2 * t + c for r in r4
                                                            for t in range(4) for c in (0, 1)])
-                        for i, stride in enumerate(ACC_STRIDES):
-                            for q in range(4):                  # 128-bit: rows 2q, 2q + 1, load + store
-                                r2 = [e[0] for e in s8[2 * q:2 * q + 2] if e is not None]
+                        for q in range(4):                      # 128-bit: rows 2q, 2q + 1, load + store
+                            r2 = [e[0] for e in s8[2 * q:2 * q + 2] if e is not None]
+                            for i, stride in enumerate(ACC_STRIDES):
                                 acc[1 + i] += 2 * _wavefronts([r * stride + 4 * t + c for r in r2
                                                                for t in range(4) for c in range(4)])
-                    tot += a + acc + np.array([2] + [1] * len(ACC_STRIDES))      # slot words
+                            for i, stride in enumerate(ACC_STRIDES_32):     # 32 columns: words 8t and 8t + 4
+                                for h in (0, 1):
+                                    acc[n16 + i] += 2 * _wavefronts([r * stride + 8 * t + 4 * h + c for r in r2
+                                                                     for t in range(4) for c in range(4)])
+                    tot += warps * (a + acc + slot_words)
             n += 1
-    return {k: float(v) * 16 / n for k, v in zip(names, tot)}
+    return {k: float(v) / n for k, v in zip(names, tot)}
 
 
 def main():

@@ -331,7 +331,7 @@ static int alloc_buffers(tb2_lstm* m) {
             if (c.pool_type == TB2_POOL_SOCIAL && m->C == 16 && !no_tc) {
                 const size_t half = ((size_t)m->cells * 16 * m->mlp_dims[1] + 1) / 2;
                 float *hi, *lo;
-                ALLOC(hi, 2 * half);      // interleaved (hi | lo) slabs
+                ALLOC(hi, 2 * half + (size_t)kLayer1MmaTailCols * 16);      // interleaved (hi | lo) slabs, zero tail
                 ALLOC(lo, 4);
                 m->Wt1_hi = hi;
                 m->Wt1_lo = lo;

@@ -128,6 +128,9 @@ constexpr int kMaxHidden = 256;
 inline bool hidden_dim_supported(int H) { return H >= 32 && H <= kMaxHidden && H % 32 == 0; }
 constexpr const char* kHiddenDimMessage = "hidden_dim must be a multiple of 32 from 32 to 256 (32, 64, 96, ..., 256)";
 constexpr int kGateBK = 16;        // K-chunk of the gate GEMM; weight rows are padded to it
+// Zero columns after the last cell of sparse_layer1_mma's weight image: the kernel loads whole 256-column chunks
+// without bounds checks, and the columns past d1 (never written out) of the last cell fall into this tail.
+constexpr int kLayer1MmaTailCols = 256;
 
 }  // namespace tb2
 

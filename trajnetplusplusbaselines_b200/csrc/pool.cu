@@ -86,6 +86,9 @@ struct PrepParams {
 __device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
     asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"((uint32_t)__cvta_generic_to_shared(smem)), "l"(gmem) : "memory");
 }
+__device__ __forceinline__ void cp_async4(void* smem, const void* gmem) {
+    asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((uint32_t)__cvta_generic_to_shared(smem)), "l"(gmem) : "memory");
+}
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
 
@@ -576,31 +579,34 @@ __global__ void __launch_bounds__(kL1Threads, 1) sparse_layer1_kernel(L1Params p
 //   neighbours) and the cell's weight slab is B [16 x 256]; pairs-per-cell is ~10, far below the
 //   64-row minimum of wgmma, so this irregular piece uses warp-level
 //   mma.sync.m16n8k16 (bf16 inputs, fp32 accumulate) with the same 3-pass (hi, lo) split as the
-//   dense layers.  Warp w owns output columns [16w, 16w+16) of the chunk (two n-tiles) for ALL
+//   dense layers.  Warp w owns output columns [32w, 32w+32) of the chunk (four n-tiles) for ALL
 //   pedestrians of the scene group, so accumulator rows are never shared between warps: no
-//   atomics, no barriers inside the cell loop, deterministic ascending-cell summation.
+//   atomics, no barriers inside the cell loop, deterministic ascending-cell summation.  A tile's
+//   slot word and A fragments are loaded once per warp and serve 12 mma (4 n-tiles x 3 passes).
 //   The bucketing pass lays the pairs out as one flat list of 16-row tiles in ascending cell
 //   order: every cell's run starts on a multiple of 16 and its padding slots hold a padding word, so
 //   each tile carries one cell and the cell loop is a fixed-stride loop over the CTA's tiles.
 //   Padding rows read the zero latent row and never touch the accumulators.  The loop
-//   is software-pipelined one tile ahead: tile k+1's slot words and A fragments (read-only in
-//   the loop) are requested before tile k's mma, and tile k's accumulator loads are issued
-//   before its mma results are needed (see DESIGN §8 for what bounds the kernel).
-//   An accumulator row keeps a warp's 16 columns in the order [t][n-tile][2], so the four values a lane
-//   holds of a row (columns 2t, 2t+1 of both n-tiles) are one 128-bit word; a slot is 16 bits (latent row, accumulator
-//   row) and one 32-bit word carries rows g and g + 8 of a tile.
-//   smem: acc[cap][272] fp32 | lat[cap+2][4 t][hi.x, hi.y, lo.x, lo.y] bf16 pairs | buckets |
+//   is software-pipelined: tile k+1's mma are issued before tile k's accumulators are added and
+//   stored (the mma operands never alias the accumulators); meanwhile tile k+2's A fragments
+//   and tile k+3's slot word (read-only in the loop) are requested, and the cell of the tile whose
+//   weights are requested next is read a tile early (see DESIGN §8 for what bounds the kernel).
+//   An accumulator row keeps a warp's 32 columns in the order [t][n-tile][2], so the eight values a lane
+//   holds of a row (columns 2t, 2t+1 of the four n-tiles) are two adjacent 128-bit words; a slot is 16 bits (latent
+//   row, accumulator row) and one 32-bit word carries rows g and g + 8 of a tile.
+//   smem: acc[cap][260] fp32 | lat[cap+2][4 t][hi.x, hi.y, lo.x, lo.y] bf16 pairs | buckets |
 //         tiles' cells | padded entries | raw winner lists
 //   Weights: Wt_hi / Wt_lo [cell][OUT][16] bf16, k permuted so a lane's B fragment is one 8-byte
 //   load (position 4t..4t+3 = k {2t, 2t+1, 2t+8, 2t+9}).
 // ------------------------------------------------------------------------------------------
 // Accumulator row stride in floats.  A 128-bit access is served a quarter-warp (rows g = 2q, 2q + 1 of a tile) at a
-// time and a row's 16 floats span 16 banks starting at 16 (row + warp) mod 32: two rows collide only when they agree
-// mod 2 (scripts/layer1_bench.py models the strides).
-constexpr int kMmaAccStride = kL1Cols + 16;
+// time; one of a lane's two words of a row covers the banks {0-3, 8-11, 16-19, 24-27} + 4 h + row * 260 mod 32, so
+// two rows collide only when they agree mod 2 (scripts/layer1_bench.py models the strides).
+constexpr int kMmaAccStride = kL1Cols + 4;
 
 // TB2_L1_ABLATE (scripts/layer1_ablate.py, timing only, results wrong): 1 = accumulators summed in registers instead of
-// shared memory, 2 = every tile reads cell 0's weights, 3 = no mma.  Unset in the library.
+// shared memory, 2 = every tile reads cell 0's weights, 3 = no mma, 4 = every tile reads cell 0's weights from a copy
+// in shared memory (no L2 weight traffic in the loop).  Unset in the library.
 #ifndef TB2_L1_ABLATE
 #define TB2_L1_ABLATE 0
 #endif
@@ -624,16 +630,21 @@ struct L1MmaParams {
     float constant;
 };
 
-constexpr int kMmaThreads = 512;          // 16 warps x 16 output columns
-constexpr int kMmaDepth = 8;              // tiles of B fragments a lane has requested ahead of use
+constexpr int kMmaThreads = 256;          // 8 warps x 32 output columns
+constexpr int kMmaDepth = 8;              // ring of B fragment sets: tile k + kMmaDepth's is requested as tile k is stored
 constexpr int kMmaMaxCap = 254;           // 8-bit slot fields: latent rows [0, cap + 1], accumulator rows [0, cap), 0xff = none
 
 // Tiles a scene group can need: every cell's run of pairs is rounded up to 16 rows, and the pairs of a group number at
 // most cap * nm1, so the padded list holds at most cap * nm1 + 15 * cells slots.
 __host__ __device__ inline size_t l1_mma_max_tiles(int cap, int cells, int nm1) { return ((size_t)cap * nm1 + (size_t)15 * cells) / 16; }
 
-// 16-bit slots of the whole tile list, the look-ahead tiles included
-__host__ __device__ inline size_t l1_mma_slots(size_t max_tiles) { return 16 * max_tiles + 16 * kMmaDepth; }
+// 16-bit slots of the whole tile list and the all-padding tiles after it: the loop runs in rounds of kMmaDepth tiles
+// and reads slot words three tiles ahead
+__host__ __device__ inline size_t l1_mma_slots(size_t max_tiles) { return 16 * max_tiles + 16 * (kMmaDepth + 2); }
+
+#if TB2_L1_ABLATE == 4
+constexpr size_t kMmaAblateSlab = (size_t)kL1Cols * 32 * sizeof(__nv_bfloat16);    // cell 0's (hi, lo) slab of a chunk
+#endif
 
 __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1MmaParams p) {
     extern __shared__ __align__(16) unsigned char smem_l1m[];
@@ -647,7 +658,7 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
 
     // lat rows [0, cap) real, cap = NaN-padded slot (b_enc), cap + 1 = zeros (padding slots); a row is 4 x 16 bytes,
     // lane t's (hi, lo) fragments of k {2t, 2t+1, 2t+8, 2t+9} together, the order of the weight image
-    float* acc = reinterpret_cast<float*>(smem_l1m);                                       // [cap][272]
+    float* acc = reinterpret_cast<float*>(smem_l1m);                                       // [cap][260]
     __nv_bfloat16* lat = reinterpret_cast<__nv_bfloat16*>(acc + (size_t)p.cap * kMmaAccStride);   // [cap+2][32]
     int* start = reinterpret_cast<int*>(lat + (size_t)(p.cap + 2) * 32);                   // [cells+1] padded slot offsets
     int* cursor = start + p.cells + 1;                                                     // [cells]
@@ -670,9 +681,11 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
         uint32_t* ent2 = reinterpret_cast<uint32_t*>(ent);
         for (int idx = tid; idx < (int)(l1_mma_slots(max_tiles) / 2); idx += kMmaThreads) ent2[idx] = pad | (pad << 16);
     }
-    // this thread's 128-bit word of every accumulator row: warp ew's lane-t word, columns {2 et, 2 et + 1} of both n-tiles
-    const int ew = (tid >> 2) & 15, et = tid & 3;
-    const int ecol = chunk0 + ew * 16 + 2 * et;
+    // this thread's 128-bit word of every accumulator row: word eh of warp ew's lane et, columns {2 et, 2 et + 1} of
+    // n-tiles 2 eh and 2 eh + 1
+    const int ew = (tid >> 3) & 7, eh = (tid >> 2) & 1, et = tid & 3;
+    const int ecol = chunk0 + ew * 32 + eh * 16 + 2 * et;
+    const int eword = ew * 32 + 8 * et + 4 * eh;
     {
         float4 b4;
         b4.x = ecol < p.OUT ? p.base[ecol] : 0.f;
@@ -680,30 +693,40 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
         b4.z = ecol + 8 < p.OUT ? p.base[ecol + 8] : 0.f;
         b4.w = ecol + 9 < p.OUT ? p.base[ecol + 9] : 0.f;
         for (int r = tid >> 6; r < P; r += kMmaThreads / 64)
-            *reinterpret_cast<float4*>(acc + r * kMmaAccStride + ew * 16 + 4 * et) = b4;
+            *reinterpret_cast<float4*>(acc + r * kMmaAccStride + eword) = b4;
     }
     // win_count / win_ent / lat come from pool_prepare.  The outputs written below are read by the previous step's
     // dense_layer_tc: that kernel has completed once this wait returns, because every kernel between it and this one
     // waits for its own predecessor to complete before it can complete.
     grid_dep_wait();
     grid_dep_launch();
-    // one coalesced pass over the group's winner lists (rows of a group are contiguous in memory)
-    for (int r = tid; r < P; r += kMmaThreads) cnt_s[r] = p.win_count[row0 + r];
+    // one coalesced pass over the group's winner lists (rows of a group are contiguous in memory), every request in
+    // flight at once: a thread copies ~P * nm1 / 256 words
+    for (int r = tid; r < P; r += kMmaThreads) cp_async4(cnt_s + r, p.win_count + row0 + r);
     {
         const uint32_t* src = p.win_ent + (size_t)row0 * p.nm1;
-        for (int idx = tid; idx < P * p.nm1; idx += kMmaThreads) raw[idx] = src[idx];
+        for (int idx = tid; idx < P * p.nm1; idx += kMmaThreads) cp_async4(raw + idx, src + idx);
     }
-    for (int idx = tid; idx < (P + 2) * 16; idx += kMmaThreads) {
-        const int r = idx >> 4, k = idx & 15;
-        float v = 0.f;
-        if (r < P) v = p.lat[(size_t)(row0 + r) * 16 + k] - p.constant;
-        else if (r == P) v = p.benc[k] - p.constant;
-        const __nv_bfloat16 h = __float2bfloat16_rn(v);
-        const int kp = kperm16(k);                                    // = 4 t + i
-        const int dst = (r < P ? r : p.cap + (r - P)) * 32 + (kp >> 2) * 8 + (kp & 3);
-        lat[dst] = h;
-        lat[dst + 4] = __float2bfloat16_rn(v - __bfloat162float(h));
+    cp_async_commit();
+    // latent rows, four channels per thread
+    for (int idx = tid; idx < (P + 2) * 4; idx += kMmaThreads) {
+        const int r = idx >> 2, k0 = (idx & 3) * 4;
+        float4 v4 = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (r < P) v4 = *reinterpret_cast<const float4*>(p.lat + (size_t)(row0 + r) * 16 + k0);
+        else if (r == P) v4 = *reinterpret_cast<const float4*>(p.benc + k0);
+        const float vk[4] = {v4.x, v4.y, v4.z, v4.w};
+        const int row = r < P ? r : p.cap + (r - P);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+            const float v = r <= P ? vk[i] - p.constant : 0.f;
+            const __nv_bfloat16 h = __float2bfloat16_rn(v);
+            const int kp = kperm16(k0 + i);                           // = 4 t + i
+            const int dst = row * 32 + (kp >> 2) * 8 + (kp & 3);
+            lat[dst] = h;
+            lat[dst + 4] = __float2bfloat16_rn(v - __bfloat162float(h));
+        }
     }
+    cp_async_wait_all();
     __syncthreads();
     const int total = P * p.nm1;
     for (int idx = tid; idx < total; idx += kMmaThreads) {
@@ -731,7 +754,7 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
             run += padded;
         }
         // beyond the last cell the list runs on in all-padding tiles: the loop works in rounds of kMmaDepth tiles and
-        // looks one tile ahead
+        // looks ahead
         if (tid == 31) start[p.cells] = incl;
     }
     __syncthreads();
@@ -748,14 +771,20 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
     __syncthreads();
 
     const int tiles = start[p.cells] >> 4;
-    // this lane loads, for n-tile j (j = 0, 1), column chunk0 + 16 warp + 8 j + g
-    const int ncol0 = chunk0 + warp * 16 + g;
+    // this lane loads, for n-tile j (j = 0 .. 3), column chunk0 + 32 warp + 8 j + g
+    const int ncol0 = chunk0 + warp * 32 + g;
     const uint32_t cell_stride = (uint32_t)p.OUT * 32;   // bf16 elements per cell (hi + lo interleaved)
     const __nv_bfloat16* wh = p.Wt_hi + (size_t)ncol0 * 32 + 8 * t;
-    bool okc[2];
-#pragma unroll
-    for (int j = 0; j < 2; ++j) okc[j] = ncol0 + 8 * j < p.OUT;
-    struct BFrag { uint2 h[2], l[2]; };
+#if TB2_L1_ABLATE == 4
+    // cell 0's slab of the warp's 32 columns, copied once: 32 x 64 bytes, [column][t][hi.x, hi.y, lo.x, lo.y]
+    uint4* wslab = reinterpret_cast<uint4*>((reinterpret_cast<uintptr_t>(sbase + p.cap) + 15) & ~(uintptr_t)15) + warp * 128;
+    for (int i = lane; i < 128; i += 32) {
+        const int c = chunk0 + warp * 32 + (i >> 2);
+        wslab[i] = c < p.OUT ? __ldcg(reinterpret_cast<const uint4*>(p.Wt_hi + (size_t)c * 32) + (i & 3)) : make_uint4(0u, 0u, 0u, 0u);
+    }
+    __syncwarp();
+#endif
+    struct BFrag { uint2 h[4], l[4]; };
     auto load_b = [&](int cell) -> BFrag {      // this lane's fragments of one cell
 #if TB2_L1_ABLATE == 2
         cell = 0;
@@ -763,10 +792,15 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
         const __nv_bfloat16* w = wh + (uint32_t)cell * cell_stride;
         BFrag f;
 #pragma unroll
-        for (int j = 0; j < 2; ++j) {
-            // one 16-byte L2 load per n-tile: (hi.x, hi.y, lo.x, lo.y) fragments of column ncol0 + 8 j
-            const uint4 v = okc[j] ? __ldcg(reinterpret_cast<const uint4*>(w + j * 8 * 32))
-                                   : make_uint4(0u, 0u, 0u, 0u);
+        for (int j = 0; j < 4; ++j) {
+            // one 16-byte L2 load per n-tile: (hi.x, hi.y, lo.x, lo.y) fragments of column ncol0 + 8 j.  A column
+            // past OUT reads the next cell's slab or the image's zero tail; its accumulators are never written out.
+#if TB2_L1_ABLATE == 4
+            (void)w;
+            const uint4 v = wslab[(8 * j + g) * 4 + t];
+#else
+            const uint4 v = __ldcg(reinterpret_cast<const uint4*>(w + j * 8 * 32));
+#endif
             f.h[j] = make_uint2(v.x, v.y);
             f.l[j] = make_uint2(v.z, v.w);
         }
@@ -776,22 +810,45 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
     struct Tile { uint32_t e; uint4 a0, a1; };
     const uint4* latT = reinterpret_cast<const uint4*>(lat) + t;
     const uint32_t* ent2 = reinterpret_cast<const uint32_t*>(ent);
-    auto fetch = [&](int k) -> Tile {
+    auto a_rows = [&](uint32_t e) -> Tile {
         Tile f;
-        f.e = ent2[8 * k + g];
-        f.a0 = latT[((f.e >> 8) & 0xffu) * 4];
-        f.a1 = latT[(f.e >> 24) * 4];
+        f.e = e;
+        f.a0 = latT[((e >> 8) & 0xffu) * 4];
+        f.a1 = latT[(e >> 24) * 4];
         return f;
     };
-    float* accw = acc + warp * 16 + 4 * t;
-    // register ring of kMmaDepth fragment sets: the slab of tile k + kMmaDepth is requested right after tile k is
-    // consumed (a cell of several tiles requests its slab once per tile)
+    // rows g and g + 8 of a tile: d[j][0, 1] and d[j][2, 3] of n-tile j, each summed from +0 in three passes
+    auto tile_mma = [&](const Tile& a, const BFrag& bf, float (&d)[4][4]) {
+        const uint32_t ah[4] = {a.a0.x, a.a1.x, a.a0.y, a.a1.y};
+        const uint32_t al[4] = {a.a0.z, a.a1.z, a.a0.w, a.a1.w};
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+#if TB2_L1_ABLATE == 3
+#pragma unroll
+            for (int x = 0; x < 4; ++x)
+                d[j][x] = __uint_as_float((ah[x] ^ bf.h[j].x ^ bf.l[j].y) + (al[x] ^ bf.h[j].y ^ bf.l[j].x));
+#else
+            d[j][0] = d[j][1] = d[j][2] = d[j][3] = 0.f;
+            mma_bf16_16816(d[j], ah, bf.h[j].x, bf.h[j].y);
+            mma_bf16_16816(d[j], ah, bf.l[j].x, bf.l[j].y);
+            mma_bf16_16816(d[j], al, bf.h[j].x, bf.h[j].y);
+#endif
+        }
+    };
+    float* accw = acc + warp * 32 + 8 * t;
+    // register ring of kMmaDepth fragment sets: slot k mod kMmaDepth holds tile k's slab until tile k's mma has been
+    // issued (one tile ahead of its store), then the slab of tile k + kMmaDepth is requested into it (a cell of several
+    // tiles requests its slab once per tile)
     BFrag b[kMmaDepth];
 #pragma unroll
     for (int i = 0; i < kMmaDepth; ++i) b[i] = load_b(i < tiles ? tcell[i] : 0);
-    Tile cur = fetch(0);
+    Tile cur = a_rows(ent2[g]), nxt = a_rows(ent2[8 + g]);
+    uint32_t e2 = ent2[16 + g];                                      // slot word of tile k + 2
+    int cell_ahead = kMmaDepth < tiles ? tcell[kMmaDepth] : 0;     // cell of tile k + kMmaDepth
+    float d[4][4];
+    tile_mma(cur, b[0], d);
 #if TB2_L1_ABLATE == 1
-    float4 s0a = make_float4(0.f, 0.f, 0.f, 0.f), s1a = s0a;
+    float4 s0a = make_float4(0.f, 0.f, 0.f, 0.f), s0b = s0a, s1a = s0a, s1b = s0a;
 #endif
     for (int k0 = 0; k0 < tiles; k0 += kMmaDepth) {
 #pragma unroll
@@ -801,61 +858,60 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
             const bool v0 = r0 != 0xffu, v1 = r1 != 0xffu;
             float4* q0 = reinterpret_cast<float4*>(accw + r0 * kMmaAccStride);
             float4* q1 = reinterpret_cast<float4*>(accw + r1 * kMmaAccStride);
-            // Accumulators of tile k, both loaded before either is stored: a row occurs at most once per cell, so rows
-            // g and g + 8 of a tile are different rows.  They come after tile k - 1's stores, which may hold the same
+            // Accumulators of tile k, all loaded before any is stored: a row occurs at most once per cell, so rows g
+            // and g + 8 of a tile are different rows.  They come after tile k - 1's stores, which may hold the same
             // rows.
-            float4 u0, u1;
+            float4 u0a, u0b, u1a, u1b;
 #if TB2_L1_ABLATE == 1
-            u0 = s0a; u1 = s1a;
+            u0a = s0a; u0b = s0b; u1a = s1a; u1b = s1b;
 #else
-            if (v0) u0 = *q0;
-            if (v1) u1 = *q1;
+            if (v0) { u0a = q0[0]; u0b = q0[1]; }
+            if (v1) { u1a = q1[0]; u1b = q1[1]; }
 #endif
-            const Tile nxt = fetch(k + 1);
-            const uint32_t ah[4] = {cur.a0.x, cur.a1.x, cur.a0.y, cur.a1.y};
-            const uint32_t al[4] = {cur.a0.z, cur.a1.z, cur.a0.w, cur.a1.w};
-            float d[2][4];
-#pragma unroll
-            for (int j = 0; j < 2; ++j) {
-#if TB2_L1_ABLATE == 3
-#pragma unroll
-                for (int x = 0; x < 4; ++x)
-                    d[j][x] = __uint_as_float((ah[x] ^ b[i].h[j].x ^ b[i].l[j].y) + (al[x] ^ b[i].h[j].y ^ b[i].l[j].x));
-#else
-                d[j][0] = d[j][1] = d[j][2] = d[j][3] = 0.f;
-                mma_bf16_16816(d[j], ah, b[i].h[j].x, b[i].h[j].y);
-                mma_bf16_16816(d[j], ah, b[i].l[j].x, b[i].l[j].y);
-                mma_bf16_16816(d[j], al, b[i].h[j].x, b[i].h[j].y);
-#endif
-            }
-            u0 = make_float4(u0.x + d[0][0], u0.y + d[0][1], u0.z + d[1][0], u0.w + d[1][1]);
-            u1 = make_float4(u1.x + d[0][2], u1.y + d[0][3], u1.z + d[1][2], u1.w + d[1][3]);
+            // tile k + 1's products while tile k's accumulators are in flight; tile k + 2's A rows (its slot word
+            // arrived during tile k - 1) and tile k + 3's slot word behind them
+            float dn[4][4];
+            tile_mma(nxt, b[(i + 1) % kMmaDepth], dn);
+            const Tile nn = a_rows(e2);
+            e2 = ent2[8 * (k + 3) + g];
+            u0a = make_float4(u0a.x + d[0][0], u0a.y + d[0][1], u0a.z + d[1][0], u0a.w + d[1][1]);
+            u0b = make_float4(u0b.x + d[2][0], u0b.y + d[2][1], u0b.z + d[3][0], u0b.w + d[3][1]);
+            u1a = make_float4(u1a.x + d[0][2], u1a.y + d[0][3], u1a.z + d[1][2], u1a.w + d[1][3]);
+            u1b = make_float4(u1b.x + d[2][2], u1b.y + d[2][3], u1b.z + d[3][2], u1b.w + d[3][3]);
 #if TB2_L1_ABLATE == 1
-            if (v0) s0a = u0;
-            if (v1) s1a = u1;
+            if (v0) { s0a = u0a; s0b = u0b; }
+            if (v1) { s1a = u1a; s1b = u1b; }
 #else
-            if (v0) *q0 = u0;
-            if (v1) *q1 = u1;
+            if (v0) { q0[0] = u0a; q0[1] = u0b; }
+            if (v1) { q1[0] = u1a; q1[1] = u1b; }
 #endif
-            if (k + kMmaDepth < tiles) b[i] = load_b(tcell[k + kMmaDepth]);
+            if (k + kMmaDepth < tiles) b[i] = load_b(cell_ahead);
+            cell_ahead = k + kMmaDepth + 1 < tiles ? tcell[k + kMmaDepth + 1] : 0;
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+#pragma unroll
+                for (int x = 0; x < 4; ++x) d[j][x] = dn[j][x];
             cur = nxt;
+            nxt = nn;
         }
     }
 #if TB2_L1_ABLATE == 1
     if (P > 0) {
-        *reinterpret_cast<float4*>(accw + (g % P) * kMmaAccStride) = s0a;
+        float4* q0 = reinterpret_cast<float4*>(accw + (g % P) * kMmaAccStride);
+        q0[0] = s0a; q0[1] = s0b;
         __syncwarp();
-        *reinterpret_cast<float4*>(accw + ((g + 8) % P) * kMmaAccStride) = s1a;
+        float4* q1 = reinterpret_cast<float4*>(accw + ((g + 8) % P) * kMmaAccStride);
+        q1[0] = s1a; q1[1] = s1b;
     }
 #endif
     __syncthreads();
-    // Lanes et and et ^ 1 swap a column pair, so the even lane holds columns [2 et, 2 et + 4) of n-tile 0 and the odd
-    // lane columns [2 et - 2, 2 et + 2) of n-tile 1: four adjacent outputs per thread.
+    // Lanes et and et ^ 1 swap a column pair, so the even lane holds columns [2 et, 2 et + 4) of n-tile 2 eh and the
+    // odd lane columns [2 et - 2, 2 et + 2) of n-tile 2 eh + 1: four adjacent outputs per thread.
     const bool odd = et & 1;
     const int ocol = odd ? ecol + 6 : ecol;
     const bool vec = (p.OUT & 3) == 0;              // then ocol < OUT covers all four, and the rows stay aligned
     for (int r = tid >> 6; r < P; r += kMmaThreads / 64) {
-        const float4 a = *reinterpret_cast<const float4*>(acc + r * kMmaAccStride + ew * 16 + 4 * et);
+        const float4 a = *reinterpret_cast<const float4*>(acc + r * kMmaAccStride + eword);
         const float sx = __shfl_xor_sync(0xffffffffu, odd ? a.x : a.z, 1);
         const float sy = __shfl_xor_sync(0xffffffffu, odd ? a.y : a.w, 1);
         float v[4] = {odd ? sx : a.x, odd ? sy : a.y, odd ? a.z : sx, odd ? a.w : sy};
@@ -900,6 +956,9 @@ static size_t l1_mma_smem_bytes(int cap, int cells, int nm1) {
     b += l1_mma_slots(tiles) * sizeof(uint16_t);                      // padded entries + all-padding tiles
     b += (size_t)cap * nm1 * sizeof(uint32_t);                        // raw winner lists
     b += (size_t)cap * 2 * sizeof(int);                               // winners per row, scene base per row
+#if TB2_L1_ABLATE == 4
+    b += 16 + kMmaAblateSlab;
+#endif
     return b + 16;
 }
 
@@ -937,8 +996,11 @@ __global__ void repack_layer1_mma_kernel(const float* __restrict__ W1, __nv_bflo
 }
 
 int launch_repack_layer1_mma(const float* W1, void* hi, void* lo, int OUT, int cells, cudaStream_t st) {
+    static_assert(kLayer1MmaTailCols >= kL1Cols, "a chunk's columns past OUT must stay inside the weight image");
     repack_layer1_mma_kernel<<<1024, 256, 0, st>>>(W1, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo, OUT, cells);
     TB2_LAUNCH_CHECK();
+    TB2_CHECK_CUDA(cudaMemsetAsync((__nv_bfloat16*)hi + (size_t)cells * OUT * 32, 0,
+                                   (size_t)kLayer1MmaTailCols * 32 * sizeof(__nv_bfloat16), st));
     return TB2_OK;
 }
 
