@@ -3,7 +3,7 @@ classical/trajnet_evaluator.py (kf, sf, sf_opt, orca, orca_opt, cv) with `predic
 
 The reference calls each model's `predict(paths, ...)` once per scene under joblib (classical/trajnet_evaluator.py:91).
 Here a chunk of scenes goes through one call: social force and ORCA simulate every pedestrian of the chunk in one
-`simulate_batch` launch, the Kalman filter fits every track of the chunk in one device launch
+`simulate_batch` launch (their `rollout`), the Kalman filter fits every track of the chunk in one device launch
 (kalman.predict_concat_device), constant velocity is one NumPy expression.  Per scene the result equals the
 per-scene `predict` on the preprocessed paths (kalman.predict(..., n_samples=0) for kf without noise), so
 evaluator.evaluate_file writes the bytes the row pipeline writes from those per-scene results.
@@ -16,47 +16,39 @@ import numpy as np
 from . import kalman, orca, socialforce
 from .common import initial_states_xy
 
-FPS = 20
-SAMPLING_RATE = int(FPS / 2.5)             # socialforce.py / orca.py: one sample every 8 simulation steps
-
 
 def _split(out, offsets):
     """[T, A, 2] positions of all pedestrians -> per scene {0: (primary [T, 2], neighbours [T, K, 2])}."""
     return [{0: (out[:, lo, 0:2], out[:, lo + 1:hi, 0:2])} for lo, hi in zip(offsets[:-1], offsets[1:])]
 
 
-class SocialForceBatch:
-    """socialforce.predict(paths, sf_params=...) for every scene of a chunk: one simulate_batch launch."""
+class SimulatorBatch:
+    """simulator.predict(paths, params) for every scene of a chunk, `simulator` the socialforce or orca module: one
+    simulator.rollout launch."""
 
-    def __init__(self, sf_params=(0.5, 2.1, 0.3), device=None):
-        self.sf_params = [float(v) for v in sf_params]
-        self.device = device
-
-    def predict_batch_xy(self, xys, n_predict=12, obs_length=9, args=None, modes=1):
-        if not xys:
-            return []
-        state, _, offsets, _ = initial_states_xy([(None, xy) for xy in xys], obs_length, n_predict, truth=False)
-        out = socialforce.simulate_batch(state, offsets, self.sf_params, n_steps=n_predict * SAMPLING_RATE,
-                                         sample_every=SAMPLING_RATE, fps=FPS, device=self.device)
-        return _split(out.cpu().numpy(), offsets)
-
-
-class OrcaBatch:
-    """orca.predict(paths, orca_params=...) for every scene of a chunk: one simulate_batch launch of
-    SAMPLING_RATE * n_predict + 1 steps (orca.py:99)."""
-
-    def __init__(self, orca_params=(1.5, 1.5, 0.4), device=None):
-        self.orca_params = [float(v) for v in orca_params]
+    def __init__(self, simulator, params, device=None):
+        self.simulator = simulator
+        self.params = [float(v) for v in params]
         self.device = device
 
     def predict_batch_xy(self, xys, n_predict=12, obs_length=9, args=None, modes=1):
         if not xys:
             return []
         state, speeds, offsets, _ = initial_states_xy([(None, xy) for xy in xys], obs_length, n_predict, truth=False)
-        out = orca.simulate_batch(state[:, 0:2], state[:, 2:4], state[:, 4:6], speeds, offsets, self.orca_params,
-                                  n_steps=SAMPLING_RATE * n_predict + 1, sample_every=SAMPLING_RATE, fps=FPS,
-                                  device=self.device)
-        return _split(out.cpu().numpy().astype(np.float64), offsets)
+        out = self.simulator.rollout(state, speeds, offsets, self.params, n_predict, device=self.device)
+        return _split(out, offsets)
+
+
+class SocialForceBatch(SimulatorBatch):
+    def __init__(self, sf_params=(0.5, 2.1, 0.3), device=None):
+        super().__init__(socialforce, sf_params, device)
+        self.sf_params = self.params
+
+
+class OrcaBatch(SimulatorBatch):
+    def __init__(self, orca_params=(1.5, 1.5, 0.4), device=None):
+        super().__init__(orca, orca_params, device)
+        self.orca_params = self.params
 
 
 def kalman_tracks_xy(xy, obs_length):
@@ -84,10 +76,8 @@ class KalmanBatch:
     def predict_batch_xy(self, xys, n_predict=12, obs_length=9, args=None, modes=1):
         per_scene = [kalman_tracks_xy(xy, obs_length) for xy in xys]
         counts = np.array([len(c) for c, _, _ in per_scene], dtype=np.int64)
-        lengths = np.concatenate([n for _, _, n in per_scene]) if per_scene else np.zeros(0, dtype=np.int64)
-        offsets = np.zeros(len(lengths) + 1, dtype=np.int64)
-        offsets[1:] = np.cumsum(lengths)
-        obs = np.concatenate([r for _, r, _ in per_scene]) if per_scene else np.zeros((0, 2))
+        tracks = [t for _, rows, n in per_scene if len(n) for t in np.split(rows, np.cumsum(n)[:-1])]
+        obs, offsets = kalman.concat_tracks(tracks)
         pred = kalman.predict_concat_device(obs, offsets, n_predict=n_predict, n_samples=self.n_samples,
                                             em_iterations=self.em_iterations, generator=self.generator,
                                             device=self.device)[0].cpu().numpy()

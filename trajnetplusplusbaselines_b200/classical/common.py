@@ -5,15 +5,20 @@ Mirrors the adapter code around the third-party simulators in the reference
 simulated, their initial velocity (stride-3 finite difference) and their destination (linear
 extrapolation of the observed path).
 """
+import ctypes
 from collections import namedtuple
 
 import numpy as np
 
+FPS = 20                                   # simulation steps per second (socialforce.py:71, orca.py:86)
 
-def split_paths(paths, obs_length):
-    primary = paths[0]
-    start_frame = primary[obs_length - 1].frame
-    return start_frame
+
+def sampling_rate(fps):
+    """Simulation steps per observed frame: the scenes are sampled at 2.5 Hz (socialforce.py:72, orca.py:87)."""
+    return int(fps / 2.5)
+
+
+SAMPLING_RATE = sampling_rate(FPS)
 
 
 def _velocity(cx, cy, px, py, stride):
@@ -192,3 +197,65 @@ def sweep_params(params, dtype, names, positive, B):
         if not (arr[:, c] > 0).all():
             raise ValueError("%s must be > 0" % names[c])
     return np.ascontiguousarray(arr)
+
+
+# ---- the one driver of tb2_sf_* / tb2_orca_* (socialforce.py and orca.py state what is their own) -------------------
+def simulate(sim, params, inputs, batch_split, n_samples, out_dtype, device=None):
+    """One tb2_<sim>_simulate launch over every scene of batch_split.  inputs: [(array, torch dtype)] in the entry
+    point's order, one row per pedestrian; params: the ctypes parameter struct.  -> sampled positions
+    [n_samples, A, 2] of out_dtype on `device` (default: the current CUDA device)."""
+    import torch
+    from .. import _lib
+    from ..engine import SceneLayout, _device_of, _ptr, _stream
+    _lib.require_cuda()
+    lib = _lib.load()
+    device = _device_of(device)
+    tensors = [torch.as_tensor(x, dtype=dtype).to(device).contiguous() for x, dtype in inputs]
+    layout = SceneLayout(batch_split, device=device)
+    if layout.num_tracks != tensors[0].shape[0]:
+        raise ValueError("batch_split[-1] != number of pedestrians")
+    out = torch.empty((n_samples, tensors[0].shape[0], 2), dtype=out_dtype, device=device)
+    with torch.cuda.device(device):
+        _lib.check(getattr(lib, "tb2_%s_simulate" % sim)(layout.handle, ctypes.byref(params), *map(_ptr, tensors),
+                                                          _ptr(out), _stream(device)))
+    return out
+
+
+def sweep(sim, prepared, settings, params, inputs):
+    """One tb2_<sim>_sweep launch: settings [P, 3] (checked by sweep_params), params the ctypes struct of the fields
+    the settings leave alone, inputs the device tensors of prepared in the entry point's order -> (ade, fde) CUDA
+    float64 [P, B]."""
+    import torch
+    from .. import _lib
+    from ..engine import _ptr, _stream
+    _lib.require_cuda()
+    lib = _lib.load()
+    B, T = int(prepared.truth.shape[0]), int(prepared.truth.shape[1])
+    device = prepared.state.device
+    prm = torch.from_numpy(settings).to(device)
+    ade = torch.empty((len(settings), B), dtype=torch.float64, device=device)
+    fde = torch.empty_like(ade)
+    with torch.cuda.device(device):
+        _lib.check(getattr(lib, "tb2_%s_sweep" % sim)(prepared.layout.handle, ctypes.byref(params), _ptr(prm),
+                                                       len(settings), *map(_ptr, inputs), _ptr(prepared.truth), T,
+                                                       _ptr(ade), _ptr(fde), _stream(device)))
+    return ade, fde
+
+
+def predict(rollout, input_paths, dest_dict, dest_type, predict_all, n_predict, obs_length, stationary=False):
+    """The reference adapters' `predict` around a simulator (socialforce.py:74-111, orca.py:84-134).  rollout(state,
+    speeds, offsets, pred_length) -> positions [pred_length, K, 2] float64 (host) of the K pedestrians present at the
+    last observed frame, primary first.  stationary: with none present, the primary stays where it was last seen
+    (socialforce.py:96-99; the ORCA adapter has no such case)."""
+    start_frame = input_paths[0][obs_length - 1].frame
+    state, speeds = initial_states(input_paths, start_frame, n_predict, dest_dict, dest_type)
+    if stationary and len(state) == 0:
+        past_path = [t for t in input_paths[0] if t.frame == start_frame]
+        states = np.stack([[[past_path[0].x, past_path[0].y]] for _ in range(n_predict)])
+    else:
+        states = rollout(state, speeds, [0, len(state)], n_predict)
+    primary_track = states[:, 0, 0:2]
+    neighbours_tracks = states[:, 1:, 0:2]
+    if not predict_all:
+        neighbours_tracks = []
+    return {0: (primary_track, neighbours_tracks)}

@@ -18,14 +18,19 @@ _A = np.array([[1, 1, 0, 0], [0, 1, 0, 0], [0, 0, 1, 1], [0, 0, 0, 1]], dtype=np
 _C = np.array([[1, 0, 0, 0], [0, 0, 1, 0]], dtype=np.float64)
 
 
+def concat_tracks(tracks):
+    """Tracks [T_i, 2] -> (obs [sum T_i, 2] float64, offsets [n + 1] int64): the layout of the Kalman entry points."""
+    tracks = [np.asarray(t, dtype=np.float64).reshape(-1, 2) for t in tracks]
+    offsets = np.zeros(len(tracks) + 1, dtype=np.int64)
+    offsets[1:] = np.cumsum([len(t) for t in tracks])
+    return (np.ascontiguousarray(np.concatenate(tracks)) if tracks else np.zeros((0, 2))), offsets
+
+
 def predict_tracks(tracks, n_predict=12, n_samples=5, em_iterations=10):
     """tracks: list of [T_i, 2] arrays -> [n_tracks, n_predict, 2] float64."""
     lib = _lib.load()
-    tracks = [np.ascontiguousarray(t, dtype=np.float64) for t in tracks]
-    n = len(tracks)
-    offs = np.zeros(n + 1, dtype=np.int64)
-    offs[1:] = np.cumsum([len(t) for t in tracks])
-    obs = np.ascontiguousarray(np.concatenate(tracks, axis=0)) if n else np.zeros((0, 2))
+    obs, offs = concat_tracks(tracks)
+    n = len(offs) - 1
     pred = np.zeros((n, n_predict, 2), dtype=np.float64)
     q = np.zeros((n, 4, 4), dtype=np.float64)
     r = np.zeros((n, 2, 2), dtype=np.float64)
@@ -80,10 +85,7 @@ def predict_tracks_device(tracks, n_predict=12, n_samples=5, em_iterations=10, g
     n_samples >= 1: the mean of n_samples sampled rollouts, drawn as one rollout driven by Q / n_samples and
     R / n_samples from eps [n_tracks, n_predict, 6] standard normals (default: torch.randn on the device from
     `generator`).  The random stream is torch's, not NumPy's global one (DESIGN §8)."""
-    tracks = [np.asarray(t, dtype=np.float64).reshape(-1, 2) for t in tracks]
-    offs = np.zeros(len(tracks) + 1, dtype=np.int64)
-    offs[1:] = np.cumsum([len(t) for t in tracks])
-    obs = np.concatenate(tracks, axis=0) if tracks else np.zeros((0, 2))
+    obs, offs = concat_tracks(tracks)
     return predict_concat_device(obs, offs, n_predict=n_predict, n_samples=n_samples, em_iterations=em_iterations,
                                  generator=generator, eps=eps, device=device)[0]
 

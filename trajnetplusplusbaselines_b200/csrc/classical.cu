@@ -1,4 +1,4 @@
-// Classical crowd simulators: social force and ORCA, one persistent kernel each.
+// Classical crowd simulators: social force and ORCA, one persistent rollout kernel and one sweep kernel for both.
 //
 // The reference builds ONE simulator per scene and crosses Python -> third-party code every
 // step (classical/socialforce.py:89-95: 96 x socialforce.Simulator.step(); classical/orca.py:
@@ -36,17 +36,6 @@ __device__ __forceinline__ double sf_potential(double rx, double ry, double sb, 
     const double in_sqrt = s * s - (dt * sb) * (dt * sb);
     const double b = 0.5 * sqrt(in_sqrt);
     return v0 * exp(-b / sigma);
-}
-
-// kWarpScenes: every scene has at most 32 pedestrians -> one WARP per scene, 4 scenes per CTA, __syncwarp instead
-// of __syncthreads (a CTA of one warp caps an SM at 32 resident warps; the arithmetic per pedestrian is unchanged,
-// results are bit-identical to the one-scene-per-CTA form).
-constexpr int kScenesPerCta = 4;
-
-template <bool kWarpScenes>
-__device__ __forceinline__ void scene_sync() {
-    if (kWarpScenes) __syncwarp();
-    else __syncthreads();
 }
 
 // One pedestrian of a social-force rollout: position, velocity, destination, initial and maximum speed
@@ -103,140 +92,6 @@ __device__ __forceinline__ void sf_advance(SfAgent& g, const SfScene& sc, int a,
     const double factor = isnan(q) ? q : (q < 1.0 ? q : 1.0);       // numpy.minimum(1, q)
     g.ux = wx * factor; g.uy = wy * factor;
     g.x = g.x + g.ux * dt; g.y = g.y + g.uy * dt;
-}
-
-template <bool kWarpScenes>
-__global__ void sf_simulate_kernel(const int* __restrict__ scene_off, const double* __restrict__ state,
-                                   double* __restrict__ out, int A, int B, int n_max, tb2_sf_params p) {
-    extern __shared__ double smem_sf[];
-    const int scene = kWarpScenes ? blockIdx.x * kScenesPerCta + (int)(threadIdx.x >> 5) : (int)blockIdx.x;
-    if (scene >= B) return;                                  // whole warp (kWarpScenes): no block-wide barrier below
-    const int row0 = scene_off[scene];
-    const int n = scene_off[scene + 1] - row0;
-    const int a = kWarpScenes ? (int)(threadIdx.x & 31) : (int)threadIdx.x;
-    double* px = smem_sf + (kWarpScenes ? (size_t)(threadIdx.x >> 5) * n_max * 7 : 0);
-    const SfScene sc{px, px + n, px + 2 * n, px + 3 * n, px + 4 * n, px + 5 * n, px + 6 * n};
-
-    const double dt = (double)p.delta_t, tau = (double)p.tau, v0 = (double)p.v0, sigma = (double)p.sigma;
-    const double cosphi = sf_cosphi();
-    SfAgent g = {};
-    if (a < n) g = sf_agent_init(state + (size_t)(row0 + a) * 6);
-    int sample = 0;
-    for (int k = 0; k < p.n_steps; ++k) {
-        double eax = 0, eay = 0;
-        if (a < n) sf_publish(g, sc, a, eax, eay);
-        scene_sync<kWarpScenes>();
-        if (a < n) {
-            sf_advance(g, sc, a, n, eax, eay, dt, tau, v0, sigma, cosphi);
-            if (k % p.sample_every == 0) {
-                double* o = out + ((size_t)sample * A + row0 + a) * 2;
-                o[0] = g.x; o[1] = g.y;
-            }
-        }
-        if (k % p.sample_every == 0) ++sample;
-        scene_sync<kWarpScenes>();
-    }
-}
-
-// -----------------------------------------------------------------------------------------
-// Parameter sweeps: a work item is (scene, setting); only the primary's ADE / FDE leave the chip.
-// One CTA per scene runs every setting of it.  kPacked (scene of n <= 32): lane segments of W = next power of two >= n,
-// each segment its own setting with its own scene arrays, 32 / W settings per warp in lockstep under __syncwarp.
-// Otherwise the whole CTA is one item, looping over the settings.  Each thread keeps its pedestrian's initial state in
-// registers (the lane -> pedestrian map is fixed for the scene); the primary's truth sits in shared memory.  The primary
-// (pedestrian 0) accumulates |truth - position| in float64, sequentially over the samples: ADE = sum / n_samples,
-// FDE = the last distance.  No atomics: reruns are bit-identical.
-// -----------------------------------------------------------------------------------------
-constexpr int kSweepWarps = 4;
-
-__device__ __forceinline__ int sweep_width(int n) {
-    int w = 1;
-    while (w < n) w <<= 1;
-    return w;
-}
-
-// Lane geometry of one item: pedestrian index a, first setting `slot`, settings per round `nslots`, array stride.
-struct SweepLane { int a, slot, nslots, stride, warp_first; };
-
-template <bool kPacked>
-__device__ __forceinline__ SweepLane sweep_lane(int n) {
-    SweepLane L;
-    if (kPacked) {
-        const int W = sweep_width(n), per_warp = 32 / W, lane = (int)(threadIdx.x & 31), warp = (int)(threadIdx.x >> 5);
-        L.a = lane & (W - 1);
-        L.warp_first = warp * per_warp;
-        L.slot = L.warp_first + lane / W;
-        L.nslots = (int)(blockDim.x >> 5) * per_warp;
-        L.stride = W;
-    } else {
-        L.a = (int)threadIdx.x;
-        L.warp_first = L.slot = 0;
-        L.nslots = 1;
-        L.stride = n;
-    }
-    return L;
-}
-
-// Loads the primary's last n_samples truth rows into shared memory; returns false when the CTA's scene is not of
-// this form (packed: n <= 32; CTA: n > 32).
-template <bool kPacked>
-__device__ __forceinline__ bool sweep_scene(const int* scene_off, const double* truth, int T, int n_samples,
-                                            double* tr, int& row0, int& n) {
-    row0 = scene_off[blockIdx.x];
-    n = scene_off[blockIdx.x + 1] - row0;
-    if (kPacked ? n > 32 : n <= 32) return false;            // whole CTA
-    const double* src = truth + ((size_t)blockIdx.x * T + (T - n_samples)) * 2;
-    for (int i = (int)threadIdx.x; i < 2 * n_samples; i += (int)blockDim.x) tr[i] = src[i];
-    __syncthreads();
-    return true;
-}
-
-template <bool kPacked>
-__global__ void sf_sweep_kernel(const int* __restrict__ scene_off, const double* __restrict__ state,
-                                const double* __restrict__ params, int P, const double* __restrict__ truth, int T,
-                                double* __restrict__ ade, double* __restrict__ fde, int B, tb2_sf_params p) {
-    extern __shared__ double smem_sfs[];
-    const int n_samples = (p.n_steps + p.sample_every - 1) / p.sample_every;
-    double* tr = smem_sfs;
-    int row0, n;
-    if (!sweep_scene<kPacked>(scene_off, truth, T, n_samples, tr, row0, n)) return;
-    const SweepLane L = sweep_lane<kPacked>(n);
-    double* px = tr + 2 * n_samples + (kPacked ? (size_t)(threadIdx.x - L.a) * 7 : 0);    // this segment's arrays
-    const SfScene sc{px, px + L.stride, px + 2 * L.stride, px + 3 * L.stride, px + 4 * L.stride, px + 5 * L.stride,
-                     px + 6 * L.stride};
-    const double dt = (double)p.delta_t;
-    const double cosphi = sf_cosphi();
-    SfAgent g0 = {};
-    if (L.a < n) g0 = sf_agent_init(state + (size_t)(row0 + L.a) * 6);
-    for (int base = 0; base < P; base += L.nslots) {
-        if (kPacked && base + L.warp_first >= P) break;     // warp-uniform: no setting left for this warp
-        const int s = base + L.slot;
-        const bool on = L.a < n && s < P;
-        double tau = 1.0, v0 = 0.0, sigma = 1.0;
-        if (on) { tau = params[(size_t)s * 3]; v0 = params[(size_t)s * 3 + 1]; sigma = params[(size_t)s * 3 + 2]; }
-        SfAgent g = g0;
-        double sum = 0.0, last = 0.0;
-        int sample = 0;
-        for (int k = 0; k < p.n_steps; ++k) {
-            double eax = 0, eay = 0;
-            if (on) sf_publish(g, sc, L.a, eax, eay);
-            scene_sync<kPacked>();
-            if (on) {
-                sf_advance(g, sc, L.a, n, eax, eay, dt, tau, v0, sigma, cosphi);
-                if (L.a == 0 && k % p.sample_every == 0) {
-                    const double ex = tr[2 * sample] - g.x, ey = tr[2 * sample + 1] - g.y;
-                    last = sqrt(ex * ex + ey * ey);
-                    sum += last;
-                }
-            }
-            if (k % p.sample_every == 0) ++sample;
-            scene_sync<kPacked>();
-        }
-        if (on && L.a == 0) {
-            ade[(size_t)s * B + blockIdx.x] = sum / (double)n_samples;
-            fde[(size_t)s * B + blockIdx.x] = last;
-        }
-    }
 }
 
 // =========================================================================================
@@ -434,94 +289,260 @@ __device__ __forceinline__ void orca_advance(OrcaAgent& g, float2 newv, float ti
     else g.pref = f2((float)gx, (float)gy);
 }
 
-template <bool kWarpScenes>
-__global__ void orca_simulate_kernel(const int* __restrict__ scene_off, const float2* __restrict__ pos_in,
-                                     const float2* __restrict__ vel_in, const double2* __restrict__ goal_in,
-                                     const double* __restrict__ speed_in, float2* __restrict__ out, int A, int B,
-                                     int n_max, tb2_orca_params p) {
-    extern __shared__ float2 smem_orca[];
-    const int scene = kWarpScenes ? blockIdx.x * kScenesPerCta + (int)(threadIdx.x >> 5) : (int)blockIdx.x;
-    if (scene >= B) return;
-    const int row0 = scene_off[scene];
-    const int n = scene_off[scene + 1] - row0;
-    const int a = kWarpScenes ? (int)(threadIdx.x & 31) : (int)threadIdx.x;
-    float2* pos = smem_orca + (kWarpScenes ? (size_t)(threadIdx.x >> 5) * n_max * 2 : 0);
-    float2* vel = pos + n;
+// =========================================================================================
+// One rollout for both simulators
+// =========================================================================================
+// A simulator trait holds what differs between social force and ORCA: the agent and its initial state, the constants
+// of a setting (the params struct, or a sweep's [3] settings row in place of its three swept fields), the scene arrays
+// in shared memory, a prologue before the first step, the two phases of a step around the scene barrier (phase 1 reads
+// the scene, phase 2 moves the agent), which step counts take a sample, and the host-side checks of its parameters.
 
-    OrcaAgent g = {};
-    if (a < n) {
-        g = orca_agent_init(pos_in[row0 + a], vel_in[row0 + a], goal_in[row0 + a], speed_in[row0 + a]);
-        pos[a] = g.pos;
-        vel[a] = g.vel;
+// kWarpScenes: every scene has at most 32 pedestrians -> one WARP per scene, 4 scenes per CTA, __syncwarp instead
+// of __syncthreads (a CTA of one warp caps an SM at 32 resident warps; the arithmetic per pedestrian is unchanged,
+// results are bit-identical to the one-scene-per-CTA form).
+constexpr int kScenesPerCta = 4;
+
+template <bool kWarpScenes>
+__device__ __forceinline__ void scene_sync() {
+    if (kWarpScenes) __syncwarp();
+    else __syncthreads();
+}
+
+struct SfSim {
+    using Params = tb2_sf_params;
+    using Setting = double;                    // tau, v0, sigma
+    using Agent = SfAgent;
+    using Scene = SfScene;
+    using Handoff = double2;                   // phase 1 -> phase 2: the desired direction
+    using Pos = double2;
+    struct Inputs { const double* state; };
+    struct Consts { double dt, tau, v0, sigma, cosphi; };
+    static constexpr size_t kPedBytes = 7 * sizeof(double);
+    static constexpr int kSampleOffset = 0;    // sample after step k = 0 .. n_steps - 1 when k % sample_every == 0
+
+    __device__ static Agent agent(const Inputs& in, int row) { return sf_agent_init(in.state + (size_t)row * 6); }
+    __device__ static Consts consts(const Params& p, const Setting* row) {
+        return {(double)p.delta_t, row ? row[0] : (double)p.tau, row ? row[1] : (double)p.v0,
+                row ? row[2] : (double)p.sigma, sf_cosphi()};
     }
-    scene_sync<kWarpScenes>();
-    const OrcaStep c = orca_step_consts(p.time_step, p.neighbor_dist, p.time_horizon, p.radius, p.max_neighbors);
+    // The scene arrays from pedestrian slot `first` on, each `stride` long.
+    __device__ static Scene scene(void* arrays, size_t first, int stride) {
+        double* px = static_cast<double*>(arrays) + first * 7;
+        return {px, px + stride, px + 2 * stride, px + 3 * stride, px + 4 * stride, px + 5 * stride, px + 6 * stride};
+    }
+    template <bool kWarp>
+    __device__ static void prologue(const Agent&, const Scene&, int, bool) {}
+    __device__ static Handoff phase1(const Agent& g, const Consts&, const Scene& sc, int a, int) {
+        double2 e;
+        sf_publish(g, sc, a, e.x, e.y);
+        return e;
+    }
+    __device__ static void phase2(Agent& g, const Consts& c, const Scene& sc, int a, int n, Handoff e) {
+        sf_advance(g, sc, a, n, e.x, e.y, c.dt, c.tau, c.v0, c.sigma, c.cosphi);
+    }
+    __device__ static Pos position(const Agent& g) { return make_double2(g.x, g.y); }
+
+    static int check(const Params&) { return TB2_OK; }
+    static int check_setting(const Setting* s) {
+        TB2_REQUIRE(s[0] > 0.0 && s[2] > 0.0, "tau and sigma must be > 0");
+        return TB2_OK;
+    }
+};
+
+struct OrcaSim {
+    using Params = tb2_orca_params;
+    using Setting = float;                     // neighbor_dist, time_horizon, radius
+    using Agent = OrcaAgent;
+    struct Scene { float2* pos; float2* vel; };
+    using Handoff = float2;                    // phase 1 -> phase 2: the new velocity
+    using Pos = float2;
+    struct Inputs { const float2* pos; const float2* vel; const double2* goal; const double* speed; };
+    struct Consts { OrcaStep step; float time_step; double end_range; };
+    static constexpr size_t kPedBytes = 2 * sizeof(float2);
+    static constexpr int kSampleOffset = 1;    // sample after step count = 1 .. n_steps when count % sample_every == 0
+
+    __device__ static Agent agent(const Inputs& in, int row) {
+        return orca_agent_init(in.pos[row], in.vel[row], in.goal[row], in.speed[row]);
+    }
+    __device__ static Consts consts(const Params& p, const Setting* row) {
+        return {orca_step_consts(p.time_step, row ? row[0] : p.neighbor_dist, row ? row[1] : p.time_horizon,
+                                 row ? row[2] : p.radius, p.max_neighbors),
+                p.time_step, p.end_range};
+    }
+    __device__ static Scene scene(void* arrays, size_t first, int stride) {
+        float2* pos = static_cast<float2*>(arrays) + first * 2;
+        return {pos, pos + stride};
+    }
+    // The first step reads every agent's initial position / velocity.
+    template <bool kWarp>
+    __device__ static void prologue(const Agent& g, const Scene& sc, int a, bool on) {
+        if (on) { sc.pos[a] = g.pos; sc.vel[a] = g.vel; }
+        scene_sync<kWarp>();
+    }
+    __device__ static Handoff phase1(const Agent& g, const Consts& c, const Scene& sc, int a, int n) {
+        return orca_new_velocity(sc.pos, sc.vel, a, n, g, c.step);
+    }
+    __device__ static void phase2(Agent& g, const Consts& c, const Scene& sc, int a, int, Handoff v) {
+        orca_advance(g, v, c.time_step, c.end_range);
+        sc.pos[a] = g.pos;
+        sc.vel[a] = g.vel;
+    }
+    __device__ static Pos position(const Agent& g) { return g.pos; }
+
+    static int check(const Params& p) {
+        TB2_REQUIRE(p.max_neighbors >= 1 && p.max_neighbors <= kOrcaMaxNeigh, "max_neighbors must be in [1, 16]");
+        return TB2_OK;
+    }
+    static int check_setting(const Setting* s) {
+        TB2_REQUIRE(s[1] > 0.0f && s[2] > 0.0f, "time_horizon and radius must be > 0");
+        return TB2_OK;
+    }
+};
+
+// Samples of an n_steps rollout: the step counts k = kSampleOffset .. n_steps - 1 + kSampleOffset that `every` divides.
+template <class Sim>
+__host__ __device__ __forceinline__ int sample_count(int n_steps, int every) {
+    return (n_steps - 1 + Sim::kSampleOffset) / every + 1 - Sim::kSampleOffset;
+}
+
+// The rollout of agent a of a scene of n under one setting.  Lanes with on == false (no pedestrian, or no setting)
+// take only the barriers.  sink(sample, position) receives, in sample order, the samples of the lanes it takes.
+template <class Sim, bool kWarp, class Sink>
+__device__ __forceinline__ void rollout(typename Sim::Agent g, const typename Sim::Consts& c,
+                                        const typename Sim::Scene& sc, int a, int n, bool on, int n_steps, int every,
+                                        Sink& sink) {
+    Sim::template prologue<kWarp>(g, sc, a, on);
     int sample = 0;
-    for (int count = 1; count <= p.n_steps; ++count) {
-        float2 newv = g.vel;
-        if (a < n) newv = orca_new_velocity(pos, vel, a, n, g, c);
-        scene_sync<kWarpScenes>();                       // every agent has read the old positions / velocities
-        if (a < n) {
-            orca_advance(g, newv, p.time_step, p.end_range);
-            pos[a] = g.pos;
-            vel[a] = g.vel;
-            if (count % p.sample_every == 0) out[(size_t)sample * A + row0 + a] = g.pos;
+    for (int k = Sim::kSampleOffset; k < n_steps + Sim::kSampleOffset; ++k) {
+        typename Sim::Handoff h = {};
+        if (on) h = Sim::phase1(g, c, sc, a, n);
+        scene_sync<kWarp>();                       // every agent has read the scene before any agent moves
+        if (on) Sim::phase2(g, c, sc, a, n, h);
+        if (k % every == 0) {
+            if (on && sink.takes(a)) sink(sample, Sim::position(g));
+            ++sample;
         }
-        if (count % p.sample_every == 0) ++sample;
-        scene_sync<kWarpScenes>();
+        scene_sync<kWarp>();
     }
 }
 
-// Parameter sweep of ORCA (see sf_sweep_kernel): params [P, 3] = neighbor_dist, time_horizon, radius.  The primary's
-// float positions are widened to double before the difference with the truth (the adapter's astype(np.float64)).
+// Sample j of every pedestrian -> out[j * A + row].
+template <class Pos>
+struct PositionSink {
+    __device__ static bool takes(int) { return true; }
+    Pos* out;
+    int A, row;
+    __device__ void operator()(int sample, Pos pos) const { out[(size_t)sample * A + row] = pos; }
+};
+
+// The primary's (pedestrian 0's) score against the truth rows tr: |truth - position| in float64 (ORCA's float position
+// widened first, the adapter's astype(np.float64)), summed in sample order; `last` is the final distance.
+struct ScoreSink {
+    __device__ static bool takes(int a) { return a == 0; }
+    const double* tr;
+    double sum = 0.0, last = 0.0;
+    template <class Pos>
+    __device__ void operator()(int sample, Pos pos) {
+        const double ex = tr[2 * sample] - (double)pos.x, ey = tr[2 * sample + 1] - (double)pos.y;
+        last = sqrt(ex * ex + ey * ey);
+        sum += last;
+    }
+};
+
+template <class Sim, bool kWarpScenes>
+__global__ void simulate_kernel(const int* __restrict__ scene_off, typename Sim::Inputs in,
+                                typename Sim::Pos* __restrict__ out, int A, int B, int n_max, typename Sim::Params p) {
+    extern __shared__ double smem_classical[];
+    const int scene = kWarpScenes ? blockIdx.x * kScenesPerCta + (int)(threadIdx.x >> 5) : (int)blockIdx.x;
+    if (scene >= B) return;                                  // whole warp (kWarpScenes): no block-wide barrier below
+    const int row0 = scene_off[scene];
+    const int n = scene_off[scene + 1] - row0;
+    const int a = kWarpScenes ? (int)(threadIdx.x & 31) : (int)threadIdx.x;
+    const typename Sim::Scene sc = Sim::scene(smem_classical, kWarpScenes ? (size_t)(threadIdx.x >> 5) * n_max : 0, n);
+    typename Sim::Agent g = {};
+    if (a < n) g = Sim::agent(in, row0 + a);
+    PositionSink<typename Sim::Pos> sink{out, A, row0 + a};
+    rollout<Sim, kWarpScenes>(g, Sim::consts(p, nullptr), sc, a, n, a < n, p.n_steps, p.sample_every, sink);
+}
+
+// -----------------------------------------------------------------------------------------
+// Parameter sweeps: a work item is (scene, setting); only the primary's ADE / FDE leave the chip.
+// One CTA per scene runs every setting of it.  kPacked (scene of n <= 32): lane segments of W = next power of two >= n,
+// each segment its own setting with its own scene arrays, 32 / W settings per warp in lockstep under __syncwarp.
+// Otherwise the whole CTA is one item, looping over the settings.  Each thread keeps its pedestrian's initial state in
+// registers (the lane -> pedestrian map is fixed for the scene); the primary's truth sits in shared memory.  The primary
+// (pedestrian 0) accumulates |truth - position| in float64, sequentially over the samples: ADE = sum / n_samples,
+// FDE = the last distance.  No atomics: reruns are bit-identical.
+// -----------------------------------------------------------------------------------------
+constexpr int kSweepWarps = 4;
+
+__device__ __forceinline__ int sweep_width(int n) {
+    int w = 1;
+    while (w < n) w <<= 1;
+    return w;
+}
+
+// Lane geometry of one item: pedestrian index a, first setting `slot`, settings per round `nslots`, array stride.
+struct SweepLane { int a, slot, nslots, stride, warp_first; };
+
 template <bool kPacked>
-__global__ void orca_sweep_kernel(const int* __restrict__ scene_off, const float2* __restrict__ pos_in,
-                                  const float2* __restrict__ vel_in, const double2* __restrict__ goal_in,
-                                  const double* __restrict__ speed_in, const float* __restrict__ params, int P,
-                                  const double* __restrict__ truth, int T, double* __restrict__ ade,
-                                  double* __restrict__ fde, int B, tb2_orca_params p) {
-    extern __shared__ double smem_os[];
-    const int n_samples = p.n_steps / p.sample_every;
-    double* tr = smem_os;
+__device__ __forceinline__ SweepLane sweep_lane(int n) {
+    SweepLane L;
+    if (kPacked) {
+        const int W = sweep_width(n), per_warp = 32 / W, lane = (int)(threadIdx.x & 31), warp = (int)(threadIdx.x >> 5);
+        L.a = lane & (W - 1);
+        L.warp_first = warp * per_warp;
+        L.slot = L.warp_first + lane / W;
+        L.nslots = (int)(blockDim.x >> 5) * per_warp;
+        L.stride = W;
+    } else {
+        L.a = (int)threadIdx.x;
+        L.warp_first = L.slot = 0;
+        L.nslots = 1;
+        L.stride = n;
+    }
+    return L;
+}
+
+// Loads the primary's last n_samples truth rows into shared memory; returns false when the CTA's scene is not of
+// this form (packed: n <= 32; CTA: n > 32).
+template <bool kPacked>
+__device__ __forceinline__ bool sweep_scene(const int* scene_off, const double* truth, int T, int n_samples,
+                                            double* tr, int& row0, int& n) {
+    row0 = scene_off[blockIdx.x];
+    n = scene_off[blockIdx.x + 1] - row0;
+    if (kPacked ? n > 32 : n <= 32) return false;            // whole CTA
+    const double* src = truth + ((size_t)blockIdx.x * T + (T - n_samples)) * 2;
+    for (int i = (int)threadIdx.x; i < 2 * n_samples; i += (int)blockDim.x) tr[i] = src[i];
+    __syncthreads();
+    return true;
+}
+
+// params [P, 3]: row s replaces the three swept fields of p (SfSim / OrcaSim::Setting).
+template <class Sim, bool kPacked>
+__global__ void sweep_kernel(const int* __restrict__ scene_off, typename Sim::Inputs in,
+                             const typename Sim::Setting* __restrict__ params, int P, const double* __restrict__ truth,
+                             int T, double* __restrict__ ade, double* __restrict__ fde, int B, typename Sim::Params p) {
+    extern __shared__ double smem_classical[];
+    const int n_samples = sample_count<Sim>(p.n_steps, p.sample_every);
+    double* tr = smem_classical;
     int row0, n;
     if (!sweep_scene<kPacked>(scene_off, truth, T, n_samples, tr, row0, n)) return;
     const SweepLane L = sweep_lane<kPacked>(n);
-    float2* pos = reinterpret_cast<float2*>(tr + 2 * n_samples) + (kPacked ? (size_t)(threadIdx.x - L.a) * 2 : 0);
-    float2* vel = pos + L.stride;
-    OrcaAgent g0 = {};
-    if (L.a < n) g0 = orca_agent_init(pos_in[row0 + L.a], vel_in[row0 + L.a], goal_in[row0 + L.a], speed_in[row0 + L.a]);
+    // this segment's arrays: packed, the segment's first lane is its first pedestrian
+    const typename Sim::Scene sc = Sim::scene(tr + 2 * n_samples, kPacked ? threadIdx.x - L.a : 0, L.stride);
+    typename Sim::Agent g0 = {};
+    if (L.a < n) g0 = Sim::agent(in, row0 + L.a);
     for (int base = 0; base < P; base += L.nslots) {
         if (kPacked && base + L.warp_first >= P) break;     // warp-uniform: no setting left for this warp
         const int s = base + L.slot;
         const bool on = L.a < n && s < P;
-        OrcaStep c = {};
-        if (on) c = orca_step_consts(p.time_step, params[(size_t)s * 3], params[(size_t)s * 3 + 1],
-                                     params[(size_t)s * 3 + 2], p.max_neighbors);
-        OrcaAgent g = g0;
-        if (on) { pos[L.a] = g.pos; vel[L.a] = g.vel; }
-        scene_sync<kPacked>();
-        double sum = 0.0, last = 0.0;
-        int sample = 0;
-        for (int count = 1; count <= p.n_steps; ++count) {
-            float2 newv = g.vel;
-            if (on) newv = orca_new_velocity(pos, vel, L.a, n, g, c);
-            scene_sync<kPacked>();
-            if (on) {
-                orca_advance(g, newv, p.time_step, p.end_range);
-                pos[L.a] = g.pos;
-                vel[L.a] = g.vel;
-                if (L.a == 0 && count % p.sample_every == 0) {
-                    const double ex = tr[2 * sample] - (double)g.pos.x, ey = tr[2 * sample + 1] - (double)g.pos.y;
-                    last = sqrt(ex * ex + ey * ey);
-                    sum += last;
-                }
-            }
-            if (count % p.sample_every == 0) ++sample;
-            scene_sync<kPacked>();
-        }
+        ScoreSink sink{tr};
+        rollout<Sim, kPacked>(g0, Sim::consts(p, on ? params + (size_t)s * 3 : nullptr), sc, L.a, n, on, p.n_steps,
+                              p.sample_every, sink);
         if (on && L.a == 0) {
-            ade[(size_t)s * B + blockIdx.x] = sum / (double)n_samples;
-            fde[(size_t)s * B + blockIdx.x] = last;
+            ade[(size_t)s * B + blockIdx.x] = sink.sum / (double)n_samples;
+            fde[(size_t)s * B + blockIdx.x] = sink.last;
         }
     }
 }
@@ -529,6 +550,37 @@ __global__ void orca_sweep_kernel(const int* __restrict__ scene_off, const float
 }  // namespace tb2
 
 using namespace tb2;
+
+template <class Sim>
+static int check_rollout(const typename Sim::Params& p) {
+    TB2_REQUIRE(p.n_steps >= 1 && p.sample_every >= 1, "bad step counts");
+    return Sim::check(p);
+}
+
+// Warp form (4 scenes per 128-thread CTA) when every scene has at most 32 pedestrians, else one CTA per scene.
+template <class Sim>
+static int simulate_launch(const char* name, const tb2_layout* l, const typename Sim::Params& p,
+                           typename Sim::Inputs in, typename Sim::Pos* out, void* stream) {
+    int rc = check_rollout<Sim>(p);
+    if (rc != TB2_OK) return rc;
+    TB2_REQUIRE(l->n_max <= 1024, "scene larger than 1024 pedestrians");
+    cudaStream_t st = (cudaStream_t)stream;
+    const size_t smem = (size_t)l->n_max * Sim::kPedBytes;
+    {
+        KernelTimer kt(name, st);
+        if (l->n_max <= 32)
+            simulate_kernel<Sim, true><<<(l->B + kScenesPerCta - 1) / kScenesPerCta, 32 * kScenesPerCta,
+                                         smem * kScenesPerCta, st>>>(l->scene_off, in, out, l->M, l->B, l->n_max, p);
+        else {
+            static DynSmemConfig configured;
+            TB2_CHECK_CUDA(configured.ensure(simulate_kernel<Sim, false>, smem, 48 * 1024));
+            simulate_kernel<Sim, false><<<l->B, (l->n_max + 31) / 32 * 32, smem, st>>>(l->scene_off, in, out, l->M,
+                                                                                      l->B, l->n_max, p);
+        }
+    }
+    TB2_LAUNCH_CHECK();
+    return TB2_OK;
+}
 
 // Host-side checks shared by the sweeps: counts, then the parameters read back from the device (P x 3 values).
 template <typename T>
@@ -550,23 +602,37 @@ static int sweep_counts(const tb2_layout* l, int P, int T, int n_samples) {
     return TB2_OK;
 }
 
-// Launches both forms over every scene; each CTA keeps only the scenes of its form (packed: n <= 32, CTA: n > 32).
-template <typename KPacked, typename KCta, typename... Args>
-static int sweep_launch(const char* name, KPacked kp, KCta kc, const tb2_layout* l, int P, int n_samples,
-                        size_t per_thread, cudaStream_t st, Args... args) {
+// Checks the call, then launches both forms over every scene; each CTA keeps only the scenes of its form (packed:
+// n <= 32, CTA: n > 32).
+template <class Sim>
+static int sweep_launch(const char* name, const tb2_layout* l, const typename Sim::Params& p,
+                        const typename Sim::Setting* params, int P, typename Sim::Inputs in, const double* truth, int T,
+                        double* ade, double* fde, void* stream) {
+    int rc = check_rollout<Sim>(p);
+    if (rc != TB2_OK) return rc;
+    const int n_samples = sample_count<Sim>(p.n_steps, p.sample_every);
+    rc = sweep_counts(l, P, T, n_samples);
+    if (rc != TB2_OK) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    std::vector<typename Sim::Setting> h;
+    rc = sweep_params_host(params, P, h, st);
+    for (int s = 0; rc == TB2_OK && s < P; ++s) rc = Sim::check_setting(&h[(size_t)s * 3]);
+    if (rc != TB2_OK) return rc;
+
     const size_t truth_bytes = (size_t)n_samples * 2 * sizeof(double);
     const int w_max = l->n_max >= 32 ? 32 : (l->n_max <= 1 ? 1 : 1 << (32 - __builtin_clz(l->n_max - 1)));
     const int64_t want = ((int64_t)P * w_max + 31) / 32;
     const int warps = (int)(want < kSweepWarps ? want : kSweepWarps);
     KernelTimer kt(name, st);
-    kp<<<l->B, 32 * warps, truth_bytes + (size_t)32 * warps * per_thread, st>>>(args...);
+    sweep_kernel<Sim, true><<<l->B, 32 * warps, truth_bytes + (size_t)32 * warps * Sim::kPedBytes, st>>>(
+        l->scene_off, in, params, P, truth, T, ade, fde, l->B, p);
     TB2_LAUNCH_CHECK();
     if (l->n_max > 32) {
         const int threads = (l->n_max + 31) / 32 * 32;
-        const size_t smem = truth_bytes + (size_t)l->n_max * per_thread;
+        const size_t smem = truth_bytes + (size_t)l->n_max * Sim::kPedBytes;
         static DynSmemConfig configured;
-        TB2_CHECK_CUDA(configured.ensure(kc, smem, 48 * 1024));
-        kc<<<l->B, threads, smem, st>>>(args...);
+        TB2_CHECK_CUDA(configured.ensure(sweep_kernel<Sim, false>, smem, 48 * 1024));
+        sweep_kernel<Sim, false><<<l->B, threads, smem, st>>>(l->scene_off, in, params, P, truth, T, ade, fde, l->B, p);
         TB2_LAUNCH_CHECK();
     }
     return TB2_OK;
@@ -576,84 +642,28 @@ extern "C" {
 
 int tb2_sf_simulate(const tb2_layout* l, const tb2_sf_params* p, const double* state, double* out, void* stream) {
     TB2_REQUIRE(l && p && state && out, "null argument");
-    TB2_REQUIRE(p->n_steps >= 1 && p->sample_every >= 1, "bad step counts");
-    TB2_REQUIRE(l->n_max <= 1024, "scene larger than 1024 pedestrians");
-    cudaStream_t st = (cudaStream_t)stream;
-    int threads = (l->n_max + 31) / 32 * 32;
-    size_t smem = (size_t)l->n_max * 7 * sizeof(double);
-    {
-        KernelTimer kt("sf_simulate", st);
-        if (l->n_max <= 32)
-            sf_simulate_kernel<true><<<(l->B + kScenesPerCta - 1) / kScenesPerCta, 32 * kScenesPerCta, smem * kScenesPerCta, st>>>(
-                l->scene_off, state, out, l->M, l->B, l->n_max, *p);
-        else {
-            static DynSmemConfig configured;
-            TB2_CHECK_CUDA(configured.ensure(sf_simulate_kernel<false>, smem, 48 * 1024));
-            sf_simulate_kernel<false><<<l->B, threads, smem, st>>>(l->scene_off, state, out, l->M, l->B, l->n_max, *p);
-        }
-    }
-    TB2_LAUNCH_CHECK();
-    return TB2_OK;
+    return simulate_launch<SfSim>("sf_simulate", l, *p, {state}, (double2*)out, stream);
 }
 
 int tb2_orca_simulate(const tb2_layout* l, const tb2_orca_params* p, const float* pos, const float* vel,
                       const double* goal, const double* speed, float* out, void* stream) {
     TB2_REQUIRE(l && p && pos && vel && goal && speed && out, "null argument");
-    TB2_REQUIRE(p->n_steps >= 1 && p->sample_every >= 1, "bad step counts");
-    TB2_REQUIRE(p->max_neighbors >= 1 && p->max_neighbors <= kOrcaMaxNeigh, "max_neighbors must be in [1, 16]");
-    TB2_REQUIRE(l->n_max <= 1024, "scene larger than 1024 pedestrians");
-    cudaStream_t st = (cudaStream_t)stream;
-    int threads = (l->n_max + 31) / 32 * 32;
-    size_t smem = (size_t)l->n_max * 2 * sizeof(float2);
-    {
-        KernelTimer kt("orca_simulate", st);
-        if (l->n_max <= 32)
-            orca_simulate_kernel<true><<<(l->B + kScenesPerCta - 1) / kScenesPerCta, 32 * kScenesPerCta, smem * kScenesPerCta, st>>>(
-                l->scene_off, (const float2*)pos, (const float2*)vel, (const double2*)goal, speed, (float2*)out, l->M, l->B,
-                l->n_max, *p);
-        else
-            orca_simulate_kernel<false><<<l->B, threads, smem, st>>>(l->scene_off, (const float2*)pos, (const float2*)vel,
-                                                                    (const double2*)goal, speed, (float2*)out, l->M, l->B,
-                                                                    l->n_max, *p);
-    }
-    TB2_LAUNCH_CHECK();
-    return TB2_OK;
+    return simulate_launch<OrcaSim>("orca_simulate", l, *p, {(const float2*)pos, (const float2*)vel,
+                                    (const double2*)goal, speed}, (float2*)out, stream);
 }
 
 int tb2_sf_sweep(const tb2_layout* l, const tb2_sf_params* p, const double* params, int32_t P, const double* state,
                  const double* truth, int32_t truth_len, double* ade_out, double* fde_out, void* stream) {
     TB2_REQUIRE(l && p && params && state && truth && ade_out && fde_out, "null argument");
-    TB2_REQUIRE(p->n_steps >= 1 && p->sample_every >= 1, "bad step counts");
-    const int n_samples = (p->n_steps + p->sample_every - 1) / p->sample_every;
-    int rc = sweep_counts(l, P, truth_len, n_samples);
-    if (rc != TB2_OK) return rc;
-    cudaStream_t st = (cudaStream_t)stream;
-    std::vector<double> h;
-    rc = sweep_params_host(params, P, h, st);
-    if (rc != TB2_OK) return rc;
-    for (int s = 0; s < P; ++s) TB2_REQUIRE(h[s * 3] > 0.0 && h[s * 3 + 2] > 0.0, "tau and sigma must be > 0");
-    return sweep_launch("sf_sweep", sf_sweep_kernel<true>, sf_sweep_kernel<false>, l, P, n_samples, 7 * sizeof(double), st,
-                        (const int*)l->scene_off, state, params, (int)P, truth, (int)truth_len, ade_out, fde_out, l->B, *p);
+    return sweep_launch<SfSim>("sf_sweep", l, *p, params, P, {state}, truth, truth_len, ade_out, fde_out, stream);
 }
 
 int tb2_orca_sweep(const tb2_layout* l, const tb2_orca_params* p, const float* params, int32_t P, const float* pos,
                    const float* vel, const double* goal, const double* speed, const double* truth, int32_t truth_len,
                    double* ade_out, double* fde_out, void* stream) {
     TB2_REQUIRE(l && p && params && pos && vel && goal && speed && truth && ade_out && fde_out, "null argument");
-    TB2_REQUIRE(p->n_steps >= 1 && p->sample_every >= 1, "bad step counts");
-    TB2_REQUIRE(p->max_neighbors >= 1 && p->max_neighbors <= kOrcaMaxNeigh, "max_neighbors must be in [1, 16]");
-    const int n_samples = p->n_steps / p->sample_every;
-    int rc = sweep_counts(l, P, truth_len, n_samples);
-    if (rc != TB2_OK) return rc;
-    cudaStream_t st = (cudaStream_t)stream;
-    std::vector<float> h;
-    rc = sweep_params_host(params, P, h, st);
-    if (rc != TB2_OK) return rc;
-    for (int s = 0; s < P; ++s)
-        TB2_REQUIRE(h[s * 3 + 1] > 0.0f && h[s * 3 + 2] > 0.0f, "time_horizon and radius must be > 0");
-    return sweep_launch("orca_sweep", orca_sweep_kernel<true>, orca_sweep_kernel<false>, l, P, n_samples,
-                        2 * sizeof(float2), st, (const int*)l->scene_off, (const float2*)pos, (const float2*)vel,
-                        (const double2*)goal, speed, params, (int)P, truth, (int)truth_len, ade_out, fde_out, l->B, *p);
+    return sweep_launch<OrcaSim>("orca_sweep", l, *p, params, P, {(const float2*)pos, (const float2*)vel,
+                                 (const double2*)goal, speed}, truth, truth_len, ade_out, fde_out, stream);
 }
 
 }  // extern "C"
