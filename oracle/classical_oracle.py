@@ -35,8 +35,10 @@ def _sf_value(r_ab, speeds, e, delta_t, v0, sigma):
 
 
 def sf_step(state, initial_speeds, max_speeds, delta_t, v0, sigma, fd_delta=1e-3,
-            twophi=200.0, out_of_view_factor=0.5):
-    """One Simulator.step().  state [N,7] float64 (x,y,vx,vy,dx,dy,tau), updated in place."""
+            twophi=200.0, out_of_view_factor=0.5, counters=None):
+    """One Simulator.step().  state [N,7] float64 (x,y,vx,vy,dx,dy,tau), updated in place.
+    counters: None, or a dict that gets SF_COUNTERS added to it (pairs a != b weighted out of view; pedestrians
+    whose speed is clipped to max_speeds)."""
     pos = state[:, 0:2]
     vel = state[:, 2:4]
     dest = state[:, 4:6]
@@ -62,20 +64,35 @@ def sf_step(state, initial_speeds, max_speeds, delta_t, v0, sigma, fd_delta=1e-3
     w = out_of_view_factor * np.ones_like(in_sight, dtype=np.float64)
     w[in_sight] = 1.0
     np.fill_diagonal(w, 0.0)
-    F = F0 + np.sum(w[..., None] * f_ab, axis=1)
+    # sum over b = 0 .. N-1 in index order, then F0 + sum: one rounding order, the one the CUDA kernel uses
+    wf = w[..., None] * f_ab
+    total = np.zeros_like(F0)
+    for b in range(len(state)):
+        total += wf[:, b]
+    F = F0 + total
     wv = vel + delta_t * F
     desired = np.linalg.norm(wv, axis=-1)
     with np.errstate(divide='ignore', invalid='ignore'):
-        factor = np.minimum(1.0, max_speeds / desired)
+        q = max_speeds / desired
+        factor = np.minimum(1.0, q)
+    if counters is not None:
+        off_diagonal = ~np.eye(len(state), dtype=bool)
+        counters['out_of_view'] = counters.get('out_of_view', 0) + int((~in_sight & off_diagonal).sum())
+        counters['speed_clip'] = counters.get('speed_clip', 0) + int((q < 1.0).sum())
     v_new = wv * factor[:, None]
     state[:, 0:2] = pos + v_new * delta_t
     state[:, 2:4] = v_new
     return state
 
 
-def sf_simulate(initial_state, delta_t=0.05, tau=0.5, v0=2.1, sigma=0.3, n_steps=96, sample_every=8):
+SF_COUNTERS = ('out_of_view', 'speed_clip')
+
+
+def sf_simulate(initial_state, delta_t=0.05, tau=0.5, v0=2.1, sigma=0.3, n_steps=96, sample_every=8,
+                counters=None):
     """classical/socialforce.py:89-95: n_steps x step(), keep the states whose index % 8 == 0
-    (i.e. after sim steps 1, 9, 17, ...).  initial_state [N,6] -> [n_samples, N, 2]."""
+    (i.e. after sim steps 1, 9, 17, ...).  initial_state [N,6] -> [n_samples, N, 2].
+    counters: None, or a dict that sums sf_step's counters over the steps."""
     state = np.concatenate([np.asarray(initial_state, dtype=np.float64),
                             np.full((len(initial_state), 1), tau)], axis=1)
     initial_speeds = np.linalg.norm(state[:, 2:4], axis=-1)
@@ -83,7 +100,7 @@ def sf_simulate(initial_state, delta_t=0.05, tau=0.5, v0=2.1, sigma=0.3, n_steps
     out = []
     with np.errstate(divide='ignore', invalid='ignore'):
         for k in range(n_steps):
-            sf_step(state, initial_speeds, max_speeds, delta_t, v0, sigma)
+            sf_step(state, initial_speeds, max_speeds, delta_t, v0, sigma, counters=counters)
             if k % sample_every == 0:
                 out.append(state[:, 0:2].copy())
     return np.stack(out)

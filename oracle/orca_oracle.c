@@ -111,11 +111,15 @@ static void lp3(const line_t* lines, int n, int begin, float radius, v2* result)
  *   pos, vel   [n][2] float  (initial position / velocity)
  *   goal       [n][2] double, speed [n] double (initial speed; maxSpeed = 1.3 * speed)
  *   out        [n_steps / sample_every][n][2] float
+ *   counters   NULL, or [4] int64 counts added to: (agent, step) pairs whose neighbour list is full
+ *              (max_neighbors); ORCA lines built by the collision branch (distance <= 2 radius);
+ *              linearProgram3 calls; (agent, step) pairs whose preferred velocity is zeroed within
+ *              end_range of the goal
  */
 int orca_simulate_scene(int n, const float* pos_in, const float* vel_in, const double* goal,
                         const double* speed, float time_step, float neighbor_dist, int max_neighbors,
                         float time_horizon, float radius, double end_range, int n_steps,
-                        int sample_every, float* out) {
+                        int sample_every, float* out, long long* counters) {
     if (max_neighbors > ORCA_MAX_NEIGH) return -1;
     v2* pos = (v2*)malloc(sizeof(v2) * n);
     v2* vel = (v2*)malloc(sizeof(v2) * n);
@@ -149,6 +153,7 @@ int orca_simulate_scene(int n, const float* pos_in, const float* vel_in, const d
                     if (nn == max_neighbors) range_sq = nd[nn - 1];
                 }
             }
+            if (counters && nn == max_neighbors) ++counters[0];
             line_t lines[ORCA_MAX_NEIGH];
             for (int k = 0; k < nn; ++k) {
                 const int b = nb[k];
@@ -179,6 +184,7 @@ int orca_simulate_scene(int n, const float* pos_in, const float* vel_in, const d
                         u = sub(mul(dp2, l.dir), rv);
                     }
                 } else {
+                    if (counters) ++counters[1];
                     const v2 w = sub(rv, mul(inv_ts, rp));
                     const float wl = sqrtf(abssq(w));
                     const v2 uw = mk(w.x / wl, w.y / wl);
@@ -190,7 +196,10 @@ int orca_simulate_scene(int n, const float* pos_in, const float* vel_in, const d
             }
             v2 res;
             const int fail = lp2(lines, nn, maxsp[a], pref[a], 0, &res);
-            if (fail < nn) lp3(lines, nn, fail, maxsp[a], &res);
+            if (fail < nn) {
+                if (counters) ++counters[2];
+                lp3(lines, nn, fail, maxsp[a], &res);
+            }
             newv[a] = res;
         }
         for (int a = 0; a < n; ++a) {
@@ -209,6 +218,7 @@ int orca_simulate_scene(int n, const float* pos_in, const float* vel_in, const d
             const double dx = goal[2 * a] - (double)pos[a].x, dy = goal[2 * a + 1] - (double)pos[a].y;
             const double dist = sqrt(dx * dx + dy * dy);
             if (dist < end_range) {
+                if (counters) ++counters[3];
                 pref[a] = mk(0.0f, 0.0f);
             } else if (dist > speed[a]) {
                 pref[a] = mk((float)(speed[a] * dx / dist), (float)(speed[a] * dy / dist));

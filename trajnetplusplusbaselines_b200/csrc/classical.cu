@@ -449,9 +449,14 @@ struct ScoreSink {
     }
 };
 
+// Launch bounds: the CTA form takes scenes of up to 1024 pedestrians, one thread each, so it must compile to at most 64
+// registers a thread (65 536 / 1024); unbounded, ptxas gave social force 80 and the device refused blocks above 768
+// threads.  The warp form keeps its fixed 128-thread CTA.  minBlocks = 1 leaves the warp form's register budget where
+// it was (with 128 alone it spilled).
 template <class Sim, bool kWarpScenes>
-__global__ void simulate_kernel(const int* __restrict__ scene_off, typename Sim::Inputs in,
-                                typename Sim::Pos* __restrict__ out, int A, int B, int n_max, typename Sim::Params p) {
+__global__ void __launch_bounds__(kWarpScenes ? 32 * kScenesPerCta : 1024, 1)
+simulate_kernel(const int* __restrict__ scene_off, typename Sim::Inputs in, typename Sim::Pos* __restrict__ out, int A,
+                int B, int n_max, typename Sim::Params p) {
     extern __shared__ double smem_classical[];
     const int scene = kWarpScenes ? blockIdx.x * kScenesPerCta + (int)(threadIdx.x >> 5) : (int)blockIdx.x;
     if (scene >= B) return;                                  // whole warp (kWarpScenes): no block-wide barrier below
@@ -518,11 +523,13 @@ __device__ __forceinline__ bool sweep_scene(const int* scene_off, const double* 
     return true;
 }
 
-// params [P, 3]: row s replaces the three swept fields of p (SfSim / OrcaSim::Setting).
+// params [P, 3]: row s replaces the three swept fields of p (SfSim / OrcaSim::Setting).  Launch bounds as for
+// simulate_kernel: the CTA form up to 1024 threads, the packed form at most kSweepWarps warps.
 template <class Sim, bool kPacked>
-__global__ void sweep_kernel(const int* __restrict__ scene_off, typename Sim::Inputs in,
-                             const typename Sim::Setting* __restrict__ params, int P, const double* __restrict__ truth,
-                             int T, double* __restrict__ ade, double* __restrict__ fde, int B, typename Sim::Params p) {
+__global__ void __launch_bounds__(kPacked ? 32 * kSweepWarps : 1024, 1)
+sweep_kernel(const int* __restrict__ scene_off, typename Sim::Inputs in, const typename Sim::Setting* __restrict__ params,
+             int P, const double* __restrict__ truth, int T, double* __restrict__ ade, double* __restrict__ fde, int B,
+             typename Sim::Params p) {
     extern __shared__ double smem_classical[];
     const int n_samples = sample_count<Sim>(p.n_steps, p.sample_every);
     double* tr = smem_classical;
