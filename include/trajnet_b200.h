@@ -95,6 +95,9 @@ typedef struct tb2_lstm_config {
     int32_t mlp_dim_vel;     /* Linear(2, .) on 4 (v_j - v_i); may be 0            */
     int32_t mlp_dim_hidden;  /* Linear(H, .) on h_j; may be 0                      */
     float attn_fill;         /* TB2_POOL_ATTN_MLP: fill_value of embed_with_masking (-10) */
+    int32_t goal_dim;        /* LSTM(goal_flag=True): goal_dim, the width of the goal embedding appended to the
+                              * input embedding (lstm.py:72-85,131-139); 0 = no goal input.  Inference only:
+                              * the training forward and the backward return TB2_ERR_UNSUPPORTED when it is set */
 } tb2_lstm_config;
 
 /* Device pointers to the parameters in the reference's state_dict layout (row-major
@@ -139,6 +142,9 @@ typedef struct tb2_lstm_weights {
     const float* pool_lstm_weight_hh;     /* pool.pool_lstm.weight_hh [4 Hp, Hp] */
     const float* pool_lstm_bias_ih;       /* [4 Hp] */
     const float* pool_lstm_bias_hh;       /* [4 Hp] */
+    /* goal_dim > 0 (NULL otherwise); encoder / decoder weight_ih columns are then [emb | goal | pooled] */
+    const float* goal_embedding_weight;   /* goal_embedding.input_embeddings.0.weight [goal_dim-2, 2] */
+    const float* goal_embedding_bias;     /* [goal_dim-2] */
 } tb2_lstm_weights;
 
 typedef struct tb2_lstm tb2_lstm;          /* opaque: config + repacked weights on the device */
@@ -242,6 +248,35 @@ int tb2_lstm_forward_steps(const tb2_lstm* model, const tb2_layout* layout,
                            float* normals_out_dev, float* positions_out_dev,
                            float* h_dev, float* c_dev, float* states_out_dev,
                            void* workspace_dev, size_t workspace_bytes, void* stream);
+
+/* Goal-conditioned variants of the three calls above (LSTM(goal_flag=True), lstm.py:131-139).
+ *   goals_dev [M, 2]  every track's goal, constant over the sequence.  Each step feeds the LSTM
+ *                     [emb(velocity) | goal_emb | pooled] with goal_emb = cat(ReLU(W_g . 4 d + b_g), 0, 0),
+ *                     d = (obs2 - goal) / |obs2 - goal| (0 where that norm is 0).
+ * A model with goal_dim > 0 needs goals_dev: NULL returns TB2_ERR_INVALID (the reference never
+ * substitutes zero goals), and so do the goal-less calls above, which forward here with NULL.
+ * With goal_dim == 0 goals_dev is ignored. */
+int tb2_lstm_step_forward_goals(const tb2_lstm* model, const tb2_layout* layout, int32_t phase,
+                                const float* obs1_dev, const float* obs2_dev, const float* goals_dev,
+                                const float* h_in_dev, const float* c_in_dev,
+                                float* h_out_dev, float* c_out_dev,
+                                float* normal_out_dev, float* pos_out_dev,
+                                void* workspace_dev, size_t workspace_bytes, void* stream);
+int tb2_lstm_forward_steps_goals(const tb2_lstm* model, const tb2_layout* layout,
+                                 const float* observed_dev, int32_t obs_length,
+                                 const float* truth_dev, int32_t n_decode, const float* goals_dev,
+                                 int32_t first_step, int32_t last_step,
+                                 float* normals_out_dev, float* positions_out_dev,
+                                 float* h_dev, float* c_dev, float* states_out_dev,
+                                 void* workspace_dev, size_t workspace_bytes, void* stream);
+int tb2_lstm_forward_sequence_host_goals(tb2_lstm* model, const tb2_layout* layout,
+                                         const float* observed_dev, int32_t obs_length,
+                                         const float* truth_dev, int32_t n_decode, const float* goals_dev,
+                                         float* normals_out_dev, float* positions_out_dev,
+                                         float* h_dev, float* c_dev,
+                                         void* workspace_dev, size_t workspace_bytes,
+                                         float* normals_host, float* positions_host,
+                                         void* stream, void* copy_stream);
 
 /* LSTMGenerator.adding_noise (sgan/sgan.py:200-221), in place on the hidden state of all tracks:
  *   h[m] <- cat(ReLU(weight . h[m] + bias), noise)   weight [H - noise_dim, H] (mlp_decoder_context.0),

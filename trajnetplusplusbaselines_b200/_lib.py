@@ -40,6 +40,7 @@ class LstmConfig(ctypes.Structure):
         ("mlp_dim_vel", ctypes.c_int32),
         ("mlp_dim_hidden", ctypes.c_int32),
         ("attn_fill", ctypes.c_float),
+        ("goal_dim", ctypes.c_int32),
     ]
 
 
@@ -80,6 +81,8 @@ class LstmWeights(ctypes.Structure):
         ("pool_lstm_weight_hh", ctypes.c_void_p),
         ("pool_lstm_bias_ih", ctypes.c_void_p),
         ("pool_lstm_bias_hh", ctypes.c_void_p),
+        ("goal_embedding_weight", ctypes.c_void_p),
+        ("goal_embedding_bias", ctypes.c_void_p),
     ]
 
 
@@ -143,6 +146,12 @@ PROTOTYPES = {
     "tb2_lstm_forward_sequence": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
     "tb2_lstm_forward_sequence_host": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp]),
     "tb2_lstm_forward_steps": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
+    "tb2_lstm_step_forward_goals": (ctypes.c_int, [_vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz,
+                                                   _vp]),
+    "tb2_lstm_forward_steps_goals": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _i32, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp,
+                                                    _vp, _sz, _vp]),
+    "tb2_lstm_forward_sequence_host_goals": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp,
+                                                            _sz, _vp, _vp, _vp, _vp]),
     "tb2_lstm_backward_workspace_bytes": (_sz, [_vp, _vp, _i32, _i32]),
     "tb2_lstm_sequence_backward": (ctypes.c_int, [_vp, _vp, ctypes.POINTER(LstmWeights), _vp, _i32, _vp, _i32,
                                                   _vp, _vp, _vp, _vp, _i32, ctypes.POINTER(LstmGrads),

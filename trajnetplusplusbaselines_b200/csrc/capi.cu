@@ -73,8 +73,8 @@ size_t carve_workspace(const tb2_lstm* m, const tb2_layout* l, void* base, Works
     w.act[1] = (float*)take(M * wmax * sizeof(float));
     w.act2 = (float*)take(m->n_mlp > 2 ? M * wmax * sizeof(float) : 16);
     w.pooled = (float*)take(M * (size_t)std::max(m->pool_out, 1) * sizeof(float));
-    w.emb_hi = take(M * 64 * 2);
-    w.emb_lo = take(M * 64 * 2);
+    w.emb_hi = take(M * (64 + (size_t)m->G) * 2);
+    w.emb_lo = take(M * (64 + (size_t)m->G) * 2);
     w.pool_hi = take(M * (size_t)std::max(m->P, 1) * 2);
     w.pool_lo = take(M * (size_t)std::max(m->P, 1) * 2);
     for (int i = 0; i < 2; ++i) {
@@ -184,7 +184,7 @@ using namespace tb2;
 extern "C" {
 
 const char* tb2_last_error(void) { return g_error.c_str(); }
-int tb2_version(void) { return 100; }
+int tb2_version(void) { return 101; }
 uint64_t tb2_launch_count(void) { return g_launch_count.load(); }
 
 int tb2_profile_begin(void) {
@@ -292,6 +292,10 @@ static int alloc_buffers(tb2_lstm* m) {
     ALLOC(m->be, m->E - 2);
     ALLOC(m->Wn, 5 * m->H);
     ALLOC(m->bn, 5);
+    if (m->G > 0) {
+        ALLOC(m->Wgl, (m->G - 2) * 2);
+        ALLOC(m->bgl, m->G - 2);
+    }
     for (int ph = 0; ph < 2; ++ph) {
         ALLOC(m->WgT[ph], (size_t)m->K_gate_pad * 4 * m->H);
         ALLOC(m->bg[ph], 4 * m->H);
@@ -392,16 +396,18 @@ int tb2_lstm_create(const tb2_lstm_config* cfg, tb2_lstm** out) {
         return TB2_ERR_UNSUPPORTED;
     }
     TB2_REQUIRE(cfg->embedding_dim >= 4 && cfg->embedding_dim <= 1024, "embedding_dim out of range");
+    TB2_REQUIRE(cfg->goal_dim == 0 || (cfg->goal_dim >= 4 && cfg->goal_dim <= 1024), "goal_dim out of range (0 = no goals)");
     TB2_REQUIRE(cfg->pool_type >= TB2_POOL_NONE && cfg->pool_type <= TB2_POOL_TRAJECTRON, "bad pool_type");
     tb2_lstm* m = new (std::nothrow) tb2_lstm();
     TB2_REQUIRE(m, "out of host memory");
     m->cfg = *cfg;
     m->H = cfg->hidden_dim;
     m->E = cfg->embedding_dim;
+    m->G = cfg->goal_dim;
     m->tc_disabled = tensor_cores_disabled();
     int rc = configure_pool(*cfg, m);
     if (rc == TB2_OK) {
-        m->K_gate = m->E + m->P + m->H;
+        m->K_gate = m->E + m->G + m->P + m->H;
         m->K_gate_pad = (m->K_gate + kGateBK - 1) / kGateBK * kGateBK;
         rc = alloc_buffers(m);
     }
@@ -556,7 +562,7 @@ int tb2_pool_forward(const tb2_lstm* m, const tb2_layout* l, const float* hidden
 
 // hs_cur: index (0/1) of the ping-pong buffer holding the bf16 split of h_in (tensor-core gates)
 static int step_impl(const tb2_lstm* m, const tb2_layout* l, int phase, const float* obs1,
-                     const float* obs2, const float* h_in, const float* c_in, float* h_out,
+                     const float* obs2, const float* goals, const float* h_in, const float* c_in, float* h_out,
                      float* c_out, float* normal_out, float* pos_out, Workspace* ws, int hs_cur,
                      cudaStream_t st) {
     int rc;
@@ -569,7 +575,8 @@ static int step_impl(const tb2_lstm* m, const tb2_layout* l, int phase, const fl
         pooled = ws->pooled;
     } else
     if (m->cfg.pool_type != TB2_POOL_NONE) {
-        if ((rc = launch_pool_prepare(m, l, h_in, obs1, obs2, 1, ws->write_pairs, tc ? 1 : 0, ws, st))) return rc;
+        // on the tensor-core path pool_prepare also writes the emb ([emb | goal_emb]) operand of the gate GEMM
+        if ((rc = launch_pool_prepare(m, l, h_in, obs1, obs2, 1, ws->write_pairs, tc ? 1 : 0, ws, st, goals))) return rc;
         if (tc) rc = launch_pool_mlp(m, l, ws, nullptr, ws->pool_hi, ws->pool_lo, st);
         else rc = launch_pool_mlp(m, l, ws, ws->pooled, nullptr, nullptr, st);
         if (rc) return rc;
@@ -577,21 +584,40 @@ static int step_impl(const tb2_lstm* m, const tb2_layout* l, int phase, const fl
     }
     if (tc) {
         if ((m->cfg.pool_type == TB2_POOL_NONE || m->cfg.pool_type >= TB2_POOL_HIDDEN_MLP) &&     // grid pools: pool_prepare already wrote emb
-            (rc = launch_embed_split(m, l->M, obs1, obs2, ws->emb_hi, ws->emb_lo, st)))
+            (rc = launch_embed_split(m, l->M, obs1, obs2, goals, ws->emb_hi, ws->emb_lo, st)))
             return rc;
         return launch_gates_tc(m, l, phase, obs1, obs2, ws->emb_hi, ws->emb_lo, ws->pool_hi, ws->pool_lo,
                                ws->hs_hi[hs_cur], ws->hs_lo[hs_cur], ws->hs_hi[hs_cur ^ 1], ws->hs_lo[hs_cur ^ 1],
                                h_in, c_in, h_out, c_out, normal_out, pos_out, st);
     }
-    return launch_gates(m, l, phase, obs1, obs2, pooled, h_in, c_in, h_out, c_out, normal_out, pos_out, st);
+    return launch_gates(m, l, phase, obs1, obs2, goals, pooled, h_in, c_in, h_out, c_out, normal_out, pos_out, st);
+}
+
+// The goals a call hands to the kernels: required by a goal-conditioned model, ignored by any other (lstm.py:131)
+static int resolve_goals(const tb2_lstm* m, const float** goals) {
+    if (m->G == 0) {
+        *goals = nullptr;
+        return TB2_OK;
+    }
+    TB2_REQUIRE(*goals, "the model has a goal embedding (goal_dim > 0): pass goals_dev [M, 2] through a *_goals call");
+    return TB2_OK;
 }
 
 int tb2_lstm_step_forward(const tb2_lstm* m, const tb2_layout* l, int32_t phase, const float* obs1,
                           const float* obs2, const float* h_in, const float* c_in, float* h_out,
                           float* c_out, float* normal_out, float* pos_out, void* workspace,
                           size_t workspace_bytes, void* stream) {
+    return tb2_lstm_step_forward_goals(m, l, phase, obs1, obs2, nullptr, h_in, c_in, h_out, c_out, normal_out, pos_out,
+                                       workspace, workspace_bytes, stream);
+}
+
+int tb2_lstm_step_forward_goals(const tb2_lstm* m, const tb2_layout* l, int32_t phase, const float* obs1,
+                                const float* obs2, const float* goals, const float* h_in, const float* c_in, float* h_out,
+                                float* c_out, float* normal_out, float* pos_out, void* workspace,
+                                size_t workspace_bytes, void* stream) {
     int rc = check_ready(m, l, workspace, workspace_bytes);
     if (rc) return rc;
+    if ((rc = resolve_goals(m, &goals))) return rc;
     TB2_REQUIRE(phase == TB2_PHASE_ENCODER || phase == TB2_PHASE_DECODER, "bad phase");
     TB2_REQUIRE(obs1 && obs2 && h_in && c_in && h_out && c_out && normal_out, "null argument");
     Workspace ws;
@@ -600,7 +626,7 @@ int tb2_lstm_step_forward(const tb2_lstm* m, const tb2_layout* l, int32_t phase,
     if (m->Wg_hi[0] &&
         (rc = launch_split_bf16(h_in, ws.hs_hi[0], ws.hs_lo[0], (size_t)l->M * m->H, st)))
         return rc;
-    return step_impl(m, l, phase, obs1, obs2, h_in, c_in, h_out, c_out, normal_out, pos_out, &ws, 0, st);
+    return step_impl(m, l, phase, obs1, obs2, goals, h_in, c_in, h_out, c_out, normal_out, pos_out, &ws, 0, st);
 }
 
 // Steps [first_step, last_step) of the time loop.  first_step == 0 starts from the zero state
@@ -615,12 +641,13 @@ struct HostSink {              // optional: per-step device-to-host streaming of
 };
 
 static int forward_steps_impl(const tb2_lstm* m, const tb2_layout* l, const float* observed,
-                              int32_t obs_length, const float* truth, int32_t n_decode, int32_t first_step,
-                              int32_t last_step, float* normals_out, float* positions_out, float* h, float* c,
-                              float* states_out, void* workspace, size_t workspace_bytes, void* stream,
+                              int32_t obs_length, const float* truth, int32_t n_decode, const float* goals,
+                              int32_t first_step, int32_t last_step, float* normals_out, float* positions_out, float* h,
+                              float* c, float* states_out, void* workspace, size_t workspace_bytes, void* stream,
                               const HostSink* sink, const TrainCache* cache = nullptr) {
     int rc = check_ready(m, l, workspace, workspace_bytes);
     if (rc) return rc;
+    if ((rc = resolve_goals(m, &goals))) return rc;
     TB2_REQUIRE(observed && normals_out && positions_out && h && c, "null argument");
     TB2_REQUIRE(obs_length >= 2 && n_decode >= 0, "need obs_length >= 2 and n_decode >= 0");
     const int S = obs_length - 1 + n_decode;
@@ -670,7 +697,7 @@ static int forward_steps_impl(const tb2_lstm* m, const tb2_layout* l, const floa
             wstep.pool_lo = (char*)cache->pool_lo + us * M * (size_t)m->P * 2;
             wstep.write_pairs = 1;
         }
-        if ((rc = step_impl(m, l, phase, o1, o2, h_prev, c_prev, h_next, c_next,
+        if ((rc = step_impl(m, l, phase, o1, o2, goals, h_prev, c_prev, h_next, c_next,
                             normals_out + (size_t)s * M * 5, positions_out + (size_t)s * frame, &wstep, s & 1, st)))
             return rc;
         h_prev = h_next;
@@ -696,7 +723,15 @@ int tb2_lstm_forward_steps(const tb2_lstm* m, const tb2_layout* l, const float* 
                            int32_t obs_length, const float* truth, int32_t n_decode, int32_t first_step,
                            int32_t last_step, float* normals_out, float* positions_out, float* h, float* c,
                            float* states_out, void* workspace, size_t workspace_bytes, void* stream) {
-    return forward_steps_impl(m, l, observed, obs_length, truth, n_decode, first_step, last_step, normals_out,
+    return forward_steps_impl(m, l, observed, obs_length, truth, n_decode, nullptr, first_step, last_step, normals_out,
+                              positions_out, h, c, states_out, workspace, workspace_bytes, stream, nullptr);
+}
+
+int tb2_lstm_forward_steps_goals(const tb2_lstm* m, const tb2_layout* l, const float* observed,
+                                 int32_t obs_length, const float* truth, int32_t n_decode, const float* goals,
+                                 int32_t first_step, int32_t last_step, float* normals_out, float* positions_out, float* h,
+                                 float* c, float* states_out, void* workspace, size_t workspace_bytes, void* stream) {
+    return forward_steps_impl(m, l, observed, obs_length, truth, n_decode, goals, first_step, last_step, normals_out,
                               positions_out, h, c, states_out, workspace, workspace_bytes, stream, nullptr);
 }
 
@@ -704,6 +739,16 @@ int tb2_lstm_forward_sequence_host(tb2_lstm* m, const tb2_layout* l, const float
                                    const float* truth, int32_t n_decode, float* normals_out, float* positions_out,
                                    float* h, float* c, void* workspace, size_t workspace_bytes,
                                    float* normals_host, float* positions_host, void* stream, void* copy_stream) {
+    return tb2_lstm_forward_sequence_host_goals(m, l, observed, obs_length, truth, n_decode, nullptr, normals_out,
+                                                positions_out, h, c, workspace, workspace_bytes, normals_host,
+                                                positions_host, stream, copy_stream);
+}
+
+int tb2_lstm_forward_sequence_host_goals(tb2_lstm* m, const tb2_layout* l, const float* observed, int32_t obs_length,
+                                         const float* truth, int32_t n_decode, const float* goals, float* normals_out,
+                                         float* positions_out, float* h, float* c, void* workspace,
+                                         size_t workspace_bytes, float* normals_host, float* positions_host, void* stream,
+                                         void* copy_stream) {
     TB2_REQUIRE(m && normals_host && positions_host && copy_stream, "null argument");
     TB2_REQUIRE(obs_length >= 2 && n_decode >= 0, "need obs_length >= 2 and n_decode >= 0");
     const int S = obs_length - 1 + n_decode;
@@ -713,7 +758,7 @@ int tb2_lstm_forward_sequence_host(tb2_lstm* m, const tb2_layout* l, const float
         m->step_events.push_back(ev);
     }
     HostSink sink{normals_host, positions_host, (cudaStream_t)copy_stream, &m->step_events};
-    return forward_steps_impl(m, l, observed, obs_length, truth, n_decode, 0, S, normals_out, positions_out, h, c,
+    return forward_steps_impl(m, l, observed, obs_length, truth, n_decode, goals, 0, S, normals_out, positions_out, h, c,
                               nullptr, workspace, workspace_bytes, stream, &sink);
 }
 
@@ -742,11 +787,15 @@ int tb2_lstm_forward_sequence_train(const tb2_lstm* m, const tb2_layout* l, cons
     TB2_REQUIRE(m && l, "null handle");
     TB2_REQUIRE(obs_length >= 2 && n_decode >= 0, "need obs_length >= 2 and n_decode >= 0");
     TB2_REQUIRE(states_out, "a training forward keeps the per-step states");
+    if (m->G > 0) {
+        set_error("training a goal-conditioned model (goal_dim > 0) is not built");
+        return TB2_ERR_UNSUPPORTED;
+    }
     const int S = obs_length - 1 + n_decode;
     TrainCache tc;
     const size_t need = carve_train_cache(m, l, (size_t)S, cache, &tc);
     TB2_REQUIRE(!cache || (need > 0 && cache_bytes >= need), "training cache too small (tb2_lstm_train_cache_bytes)");
-    return forward_steps_impl(m, l, observed, obs_length, truth, n_decode, 0, S, normals_out, positions_out, h, c,
+    return forward_steps_impl(m, l, observed, obs_length, truth, n_decode, nullptr, 0, S, normals_out, positions_out, h, c,
                               states_out, workspace, workspace_bytes, stream, nullptr, cache ? &tc : nullptr);
 }
 

@@ -138,6 +138,7 @@ constexpr int kLayer1MmaTailCols = 256;
 struct tb2_lstm {
     tb2_lstm_config cfg = {};
     int H = 0, E = 0, C = 0, cells = 0, n_mlp = 0;
+    int G = 0;             // goal embedding width (cfg.goal_dim; 0: no goal input)
     int P = 0;             // pooled width fed to the LSTM input (0 if none / pool_to_input == 0)
     int pool_out = 0;      // width of the pool output (grid width when n_mlp == 0)
     int mlp_dims[tb2::kMaxMlpLayers + 1] = {};  // [grid_dim, d1, ..]
@@ -147,7 +148,9 @@ struct tb2_lstm {
     // device buffers (owned)
     float* We = nullptr;        // [E-2, 2]
     float* be = nullptr;        // [E-2]
-    float* WgT[2] = {};         // [K_gate_pad, 4H]  rows: emb | pooled | h
+    float* Wgl = nullptr;       // [G-2, 2] goal embedding (G > 0)
+    float* bgl = nullptr;       // [G-2]
+    float* WgT[2] = {};         // [K_gate_pad, 4H]  rows: emb | goal | pooled | h
     float* bg[2] = {};          // [4H] = b_ih + b_hh
     float* Wn = nullptr;        // [5, H]
     float* bn = nullptr;        // [5]
@@ -203,7 +206,7 @@ struct Workspace {
     float* act[2];         // ping-pong MLP activations [M, max width]
     float* act2;           // third scratch (three_layer with a tensor-core second layer)
     float* pooled;         // [M, pool_out]
-    void* emb_hi;          // [M, 64] bf16 split operands of the tensor-core gate kernel
+    void* emb_hi;          // [M, 64 + G] bf16 split operands of the tensor-core gate kernel ([emb | goal_emb]; E == 64 there)
     void* emb_lo;
     void* pool_hi;         // [M, P]
     void* pool_lo;
@@ -240,12 +243,13 @@ int launch_resolve_obs(const tb2_layout* l, const float* base, const float* pred
                        cudaStream_t st);
 int launch_pool_prepare(const tb2_lstm* m, const tb2_layout* l, const float* hidden,
                         const float* obs1, const float* obs2, int skip_masked, int write_pairs,
-                        int write_emb, Workspace* ws, cudaStream_t st);
+                        int write_emb, Workspace* ws, cudaStream_t st, const float* goals = nullptr);
 // pooled_out fp32 and/or (pool_hi, pool_lo) bf16 split (either may be null, not both)
 int launch_pool_mlp(const tb2_lstm* m, const tb2_layout* l, Workspace* ws, float* pooled_out,
                     void* pool_hi, void* pool_lo, cudaStream_t st);
+// goals [M, 2]: null unless m->G > 0
 int launch_gates(const tb2_lstm* m, const tb2_layout* l, int phase, const float* obs1,
-                 const float* obs2, const float* pooled, const float* h_in, const float* c_in,
+                 const float* obs2, const float* goals, const float* pooled, const float* h_in, const float* c_in,
                  float* h_out, float* c_out, float* normal_out, float* pos_out, cudaStream_t st);
 int launch_repack(tb2_lstm* m, const tb2_lstm_weights* w, cudaStream_t st);
 int launch_repack_layer1_mma(const float* W1, void* hi, void* lo, int OUT, int cells, cudaStream_t st);
@@ -267,7 +271,8 @@ int launch_dense_tc(const void* a_hi, const void* a_lo, const void* w_hi, const 
                     float* Y, void* Y_hi, void* Y_lo, int M, int K, int N, int relu, cudaStream_t st);
 bool gates_tc_supported(const tb2_lstm* m);
 int launch_repack_gates_tc(const float* w_ih, const float* w_hh, void* hi, void* lo, int in_dim, int H, cudaStream_t st);
-int launch_embed_split(const tb2_lstm* m, int M, const float* obs1, const float* obs2, void* hi, void* lo, cudaStream_t st);
+int launch_embed_split(const tb2_lstm* m, int M, const float* obs1, const float* obs2, const float* goals, void* hi, void* lo,
+                       cudaStream_t st);
 int launch_gates_tc(const tb2_lstm* m, const tb2_layout* l, int phase, const float* obs1, const float* obs2,
                     const void* emb_hi, const void* emb_lo, const void* pool_hi, const void* pool_lo,
                     const void* hs_in_hi, const void* hs_in_lo, void* hs_out_hi, void* hs_out_lo,

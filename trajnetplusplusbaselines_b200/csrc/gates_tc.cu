@@ -3,7 +3,9 @@
 //
 // Same contract as lstm_gates_kernel (csrc/lstm_step.cu; reference LSTM.step lstm.py:118-168,
 // torch.nn.LSTMCell, Hidden2Normal modules.py:56-64), specialised for E = 64, H = 64, 128, 192 or 256,
-// pool_to_input: gates[M, 4H] = [emb | pooled | h][M, K] . [W_ih | W_hh]^T, K = 64 + P + H.
+// pool_to_input: gates[M, 4H] = [emb | pooled | h][M, K] . [W_ih | W_hh]^T, K = 64 + P + H.  A goal-conditioned
+// model (kGoal) has the goal embedding after emb: [emb | goal_emb | pooled | h], K = 64 + G + P + H, 64 + G a
+// multiple of 64, and embed_split writes both embeddings as one [M, 64 + G] operand.
 //
 // All three K segments arrive as bf16 (hi, lo) pairs written by their producers (embed_split,
 // the grid-embedding layer's epilogue, the previous step's epilogue) and the product is the
@@ -62,10 +64,11 @@ struct GateTcParams {
     const float* Wn;            // [5, H]
     const float* bn;            // [5]
     int M, P;
+    int G;                      // goal embedding width (kGoal instances only)
 };
 
 // R = cluster size = H / 64 (1 to 4; a cluster of one at H = 64): the strides and the rank loop of the epilogue are compile-time constants
-template <int R>
+template <int R, bool kGoal>
 __global__ void __launch_bounds__(kGtThreads, 1)
 lstm_gates_tc_kernel(const __grid_constant__ CUtensorMap map_emb_hi, const __grid_constant__ CUtensorMap map_emb_lo,
                      const __grid_constant__ CUtensorMap map_pool_hi, const __grid_constant__ CUtensorMap map_pool_lo,
@@ -83,8 +86,9 @@ lstm_gates_tc_kernel(const __grid_constant__ CUtensorMap map_emb_hi, const __gri
     const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int rank = blockIdx.x;           // cluster rank == n-tile: units [64 rank, 64 rank + 64)
     const int m0 = blockIdx.y * kGtBM;
-    const int kb_pool = p.P / kGtBK;       // k-blocks: [emb | pooled x kb_pool | h x H / 64]
-    const int num_kb = 1 + kb_pool + H / kGtBK;
+    const int kb_pool = p.P / kGtBK;       // k-blocks: [emb (+ goal_emb) x kb_emb | pooled x kb_pool | h x H / 64]
+    const int kb_emb = kGoal ? (64 + p.G) / kGtBK : 1;
+    const int num_kb = kb_emb + kb_pool + H / kGtBK;
     const uint32_t ring = (smem_u32(smem_gt) + 1023u) & ~1023u;
 
     for (int i = threadIdx.x; i < 5 * 64; i += kGtThreads) wn_s[i / 64][i % 64] = p.Wn[(i / 64) * H + rank * 64 + (i % 64)];
@@ -120,9 +124,15 @@ lstm_gates_tc_kernel(const __grid_constant__ CUtensorMap map_emb_hi, const __gri
                 mbar_expect_tx(bar, kGtStageBytes);
                 const CUtensorMap *ahi, *alo;
                 int ka;
-                if (kb == 0) { ahi = &map_emb_hi; alo = &map_emb_lo; ka = 0; }
-                else if (kb <= kb_pool) { ahi = &map_pool_hi; alo = &map_pool_lo; ka = (kb - 1) * kGtBK; }
-                else { ahi = &map_h_hi; alo = &map_h_lo; ka = (kb - 1 - kb_pool) * kGtBK; }
+                if constexpr (kGoal) {
+                    if (kb < kb_emb) { ahi = &map_emb_hi; alo = &map_emb_lo; ka = kb * kGtBK; }
+                    else if (kb < kb_emb + kb_pool) { ahi = &map_pool_hi; alo = &map_pool_lo; ka = (kb - kb_emb) * kGtBK; }
+                    else { ahi = &map_h_hi; alo = &map_h_lo; ka = (kb - kb_emb - kb_pool) * kGtBK; }
+                } else {
+                    if (kb == 0) { ahi = &map_emb_hi; alo = &map_emb_lo; ka = 0; }
+                    else if (kb <= kb_pool) { ahi = &map_pool_hi; alo = &map_pool_lo; ka = (kb - 1) * kGtBK; }
+                    else { ahi = &map_h_hi; alo = &map_h_lo; ka = (kb - 1 - kb_pool) * kGtBK; }
+                }
                 tma_load_2d(base, ahi, bar, ka, m0);
                 tma_load_2d(base + kGtABytes, alo, bar, ka, m0);
                 tma_load_2d(base + 2 * kGtABytes, &map_w_hi, bar, kb * kGtBK, rank * kGtBN);
@@ -266,20 +276,38 @@ lstm_gates_tc_kernel(const __grid_constant__ CUtensorMap map_emb_hi, const __gri
 // ------------------------------------------------------------------------------------------
 // producers of the split operands
 // ------------------------------------------------------------------------------------------
-// emb[M, 64] = cat(relu(W_e . (4 v) + b_e), 0, 0) as bf16 (hi, lo)   (modules.py:24-30)
+// emb[M, 64] = cat(relu(W_e . (4 v) + b_e), 0, 0) as bf16 (hi, lo)   (modules.py:24-30); kGoal: [M, E + G] rows
+// [emb | cat(relu(W_g . (4 d) + b_g), 0, 0)], d = (obs2 - goal) / |obs2 - goal|, 0 at norm 0 (lstm.py:131-139)
+struct GoalEmbed {
+    const float2* goals;
+    const float* Wg;
+    const float* bg;
+    int G;
+};
+
+template <bool kGoal>
 __global__ void embed_split_kernel(const float2* __restrict__ obs1, const float2* __restrict__ obs2,
                                    const float* __restrict__ We, const float* __restrict__ be,
-                                   __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo, int M, int E) {
+                                   __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo, int M, int E,
+                                   GoalEmbed ge) {
     grid_dep_wait();
     grid_dep_launch();
     const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-    if (idx >= M * E) return;
-    const int m = idx / E, k = idx - m * E;
+    const int W = kGoal ? E + ge.G : E;
+    if (idx >= M * W) return;
+    const int m = idx / W, k = idx - m * W;
     const float2 a = obs1[m], b = obs2[m];
     float v = 0.f;
     if (k < E - 2 && !(isnan(a.x) || isnan(b.x))) {
         const float vx = (b.x - a.x) * 4.0f, vy = (b.y - a.y) * 4.0f;
         v = fmaxf(fmaf(We[2 * k + 1], vy, fmaf(We[2 * k], vx, be[k])), 0.f);
+    } else if (kGoal && k >= E && k < W - 2 && !(isnan(a.x) || isnan(b.x))) {
+        const int kg = k - E;
+        const float2 g = ge.goals[m];
+        const float dx = b.x - g.x, dy = b.y - g.y;
+        const float n = sqrtf(dx * dx + dy * dy);
+        const float gx = n != 0.f ? dx / n : 0.f, gy = n != 0.f ? dy / n : 0.f;
+        v = fmaxf(fmaf(ge.Wg[2 * kg + 1], gy * 4.0f, fmaf(ge.Wg[2 * kg], gx * 4.0f, ge.bg[kg])), 0.f);
     }
     const __nv_bfloat16 h = __float2bfloat16_rn(v);
     hi[idx] = h;
@@ -308,7 +336,7 @@ __global__ void repack_gates_tc_kernel(const float* __restrict__ w_ih, const flo
 int make_bf16_tile_map(CUtensorMap* map, const void* base, int rows, int cols, int box_rows);
 
 bool gates_tc_supported(const tb2_lstm* m) {
-    if (m->H % 64 != 0 || m->E != 64) return false;
+    if (m->H % 64 != 0 || m->E != 64 || (m->E + m->G) % kGtBK != 0) return false;
     if (m->cfg.pool_type != TB2_POOL_NONE && !m->cfg.pool_to_input) return false;
     if (m->P % kGtBK != 0) return false;
     return true;
@@ -321,14 +349,32 @@ int launch_repack_gates_tc(const float* w_ih, const float* w_hh, void* hi, void*
     return TB2_OK;
 }
 
-int launch_embed_split(const tb2_lstm* m, int M, const float* obs1, const float* obs2, void* hi, void* lo,
-                       cudaStream_t st) {
-    const int total = M * m->E;
+int launch_embed_split(const tb2_lstm* m, int M, const float* obs1, const float* obs2, const float* goals, void* hi,
+                       void* lo, cudaStream_t st) {
+    const int total = M * (m->E + m->G);
+    const GoalEmbed ge{(const float2*)goals, m->Wgl, m->bgl, m->G};
     {
         KernelTimer kt("embed_split", st);
-        launch_pdl(embed_split_kernel, dim3((total + 255) / 256), dim3(256), 0, st, (const float2*)obs1,
-                   (const float2*)obs2, (const float*)m->We, (const float*)m->be, (__nv_bfloat16*)hi,
-                   (__nv_bfloat16*)lo, M, m->E);
+        launch_pdl(m->G > 0 ? embed_split_kernel<true> : embed_split_kernel<false>, dim3((total + 255) / 256), dim3(256), 0,
+                   st, (const float2*)obs1, (const float2*)obs2, (const float*)m->We, (const float*)m->be,
+                   (__nv_bfloat16*)hi, (__nv_bfloat16*)lo, M, m->E, ge);
+    }
+    TB2_LAUNCH_CHECK();
+    return TB2_OK;
+}
+
+template <int R, bool kGoal>
+static int launch_gates_tc_k(const CUtensorMap& me_hi, const CUtensorMap& me_lo, const CUtensorMap& mp_hi,
+                             const CUtensorMap& mp_lo, const CUtensorMap& mh_hi, const CUtensorMap& mh_lo,
+                             const CUtensorMap& mw_hi, const CUtensorMap& mw_lo, const GateTcParams& p, cudaStream_t st) {
+    const size_t smem = (size_t)kGtStages * kGtStageBytes + 1024;
+    static DynSmemConfig configured;
+    TB2_CHECK_CUDA(configured.ensure(lstm_gates_tc_kernel<R, kGoal>, smem));
+    dim3 grid(R, (p.M + kGtBM - 1) / kGtBM);
+    {
+        KernelTimer kt("lstm_gates_tc", st);
+        launch_pdl_cluster(lstm_gates_tc_kernel<R, kGoal>, grid, dim3(kGtThreads), smem, st, (unsigned)R, me_hi, me_lo,
+                           mp_hi, mp_lo, mh_hi, mh_lo, mw_hi, mw_lo, p);
     }
     TB2_LAUNCH_CHECK();
     return TB2_OK;
@@ -338,17 +384,8 @@ template <int R>
 static int launch_gates_tc_t(const CUtensorMap& me_hi, const CUtensorMap& me_lo, const CUtensorMap& mp_hi,
                              const CUtensorMap& mp_lo, const CUtensorMap& mh_hi, const CUtensorMap& mh_lo,
                              const CUtensorMap& mw_hi, const CUtensorMap& mw_lo, const GateTcParams& p, cudaStream_t st) {
-    const size_t smem = (size_t)kGtStages * kGtStageBytes + 1024;
-    static DynSmemConfig configured;
-    TB2_CHECK_CUDA(configured.ensure(lstm_gates_tc_kernel<R>, smem));
-    dim3 grid(R, (p.M + kGtBM - 1) / kGtBM);
-    {
-        KernelTimer kt("lstm_gates_tc", st);
-        launch_pdl_cluster(lstm_gates_tc_kernel<R>, grid, dim3(kGtThreads), smem, st, (unsigned)R, me_hi, me_lo, mp_hi,
-                           mp_lo, mh_hi, mh_lo, mw_hi, mw_lo, p);
-    }
-    TB2_LAUNCH_CHECK();
-    return TB2_OK;
+    return p.G > 0 ? launch_gates_tc_k<R, true>(me_hi, me_lo, mp_hi, mp_lo, mh_hi, mh_lo, mw_hi, mw_lo, p, st)
+                   : launch_gates_tc_k<R, false>(me_hi, me_lo, mp_hi, mp_lo, mh_hi, mh_lo, mw_hi, mw_lo, p, st);
 }
 
 int launch_gates_tc(const tb2_lstm* m, const tb2_layout* l, int phase, const float* obs1, const float* obs2,
@@ -359,8 +396,8 @@ int launch_gates_tc(const tb2_lstm* m, const tb2_layout* l, int phase, const flo
     const int M = l->M;
     CUtensorMap me_hi, me_lo, mp_hi, mp_lo, mh_hi, mh_lo, mw_hi, mw_lo;
     int rc;
-    if ((rc = make_bf16_tile_map(&me_hi, emb_hi, M, 64, kGtBM))) return rc;
-    if ((rc = make_bf16_tile_map(&me_lo, emb_lo, M, 64, kGtBM))) return rc;
+    if ((rc = make_bf16_tile_map(&me_hi, emb_hi, M, 64 + m->G, kGtBM))) return rc;
+    if ((rc = make_bf16_tile_map(&me_lo, emb_lo, M, 64 + m->G, kGtBM))) return rc;
     if (m->P > 0) {
         if ((rc = make_bf16_tile_map(&mp_hi, pool_hi, M, m->P, kGtBM))) return rc;
         if ((rc = make_bf16_tile_map(&mp_lo, pool_lo, M, m->P, kGtBM))) return rc;
@@ -384,6 +421,7 @@ int launch_gates_tc(const tb2_lstm* m, const tb2_layout* l, int phase, const flo
     p.bn = m->bn;
     p.M = M;
     p.P = m->P;
+    p.G = m->G;
     switch (m->H) {
         case 64: return launch_gates_tc_t<1>(me_hi, me_lo, mp_hi, mp_lo, mh_hi, mh_lo, mw_hi, mw_lo, p, st);
         case 128: return launch_gates_tc_t<2>(me_hi, me_lo, mp_hi, mp_lo, mh_hi, mh_lo, mw_hi, mw_lo, p, st);

@@ -10,9 +10,10 @@
 // Tiling: CTA = 32 tracks x all 4H gate columns, 256 threads; thread (warp w, lane l) owns
 // rows 4w..4w+3 and hidden units U l..U l+U-1 (U = H / 32) of all four gates, so the LSTM pointwise
 // math needs no exchange and the 5-wide Gaussian head is a warp-shuffle reduction.  The A operand
-// [emb | pooled | h] is assembled on the fly in shared memory (the embedding is recomputed
-// from the 2-float velocity, never stored); W^T streams from L2 through a cp.async
-// double buffer (16 x 4H floats per stage: 128 KB in all at H = 256).
+// [emb | goal_emb | pooled | h] is assembled on the fly in shared memory (the embeddings are recomputed
+// from the 2-float velocity and goal direction, never stored; goal_emb only in the kGoal instances, the
+// goal-conditioned models); W^T streams from L2 through a cp.async double buffer (16 x 4H floats per
+// stage: 128 KB in all at H = 256).
 #include <math_constants.h>
 
 #include "common.cuh"
@@ -39,6 +40,10 @@ struct GateParams {
     const float* Wn;       // [5, H]
     const float* bn;
     int M, E, P, K, K_pad, add_pooled_to_h;
+    const float2* goals;   // [M] (kGoal instances only)
+    const float* Wgl;      // [G-2, 2] goal embedding
+    const float* bgl;
+    int G;
 };
 
 __device__ __forceinline__ float sigmoidf_(float x) { return 1.f / (1.f + expf(-x)); }
@@ -86,8 +91,8 @@ __device__ __forceinline__ void st_units(float* dst, const float (&v)[U]) {
     }
 }
 
-// U = hidden units per lane (H = 32 U)
-template <int U>
+// U = hidden units per lane (H = 32 U); kGoal: the input carries the goal embedding (p.G columns after emb)
+template <int U, bool kGoal>
 __global__ void __launch_bounds__(kGThreads, U <= 4 ? 2 : 1) lstm_gates_kernel(GateParams p) {
     constexpr int H = 32 * U, N = 4 * H;
     extern __shared__ __align__(16) float smem_gates[];
@@ -95,6 +100,7 @@ __global__ void __launch_bounds__(kGThreads, U <= 4 ? 2 : 1) lstm_gates_kernel(G
     float (*As)[kGateBK][kGM] = reinterpret_cast<float (*)[kGateBK][kGM]>(smem_gates + 2 * kGateBK * N);  // 4 KB
     __shared__ float2 vel4[kGM];                            // 4 * (obs2 - obs1)
     __shared__ float2 obs2s[kGM];
+    __shared__ float2 goal4[kGM];                           // 4 * (obs2 - goal) / |obs2 - goal| (kGoal)
     __shared__ int maskS[kGM];
 
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
@@ -110,6 +116,16 @@ __global__ void __launch_bounds__(kGThreads, U <= 4 ? 2 : 1) lstm_gates_kernel(G
         maskS[tid] = !(isnan(a.x) || isnan(b.x));                           // lstm.py:118
         vel4[tid] = make_float2((b.x - a.x) * 4.0f, (b.y - a.y) * 4.0f);   // modules.py:27 (scale)
         obs2s[tid] = b;
+        if constexpr (kGoal) {                               // lstm.py:133-136: direction from the goal to the track
+            float2 d = make_float2(0.f, 0.f);
+            if (m < p.M) {
+                const float2 g = p.goals[m];
+                const float dx = b.x - g.x, dy = b.y - g.y;
+                const float n = sqrtf(dx * dx + dy * dy);
+                if (n != 0.f) d = make_float2(dx / n, dy / n);
+            }
+            goal4[tid] = make_float2(d.x * 4.0f, d.y * 4.0f);               // InputEmbedding scale
+        }
     }
     __syncthreads();
 
@@ -133,6 +149,7 @@ __global__ void __launch_bounds__(kGThreads, U <= 4 ? 2 : 1) lstm_gates_kernel(G
             cp_async16(dst + idx, src + idx);
         }
     };
+    const int EG = p.E + (kGoal ? p.G : 0);                  // end of the [emb | goal_emb] columns
     auto load_a = [&](int buf, int chunk) {
         // 16 k x 32 rows = 512 values, 2 per thread; thread -> (kk = idx / 32, r = idx % 32)
 #pragma unroll
@@ -149,10 +166,16 @@ __global__ void __launch_bounds__(kGThreads, U <= 4 ? 2 : 1) lstm_gates_kernel(G
                         float e = fmaf(p.We[2 * k + 1], vv.y, fmaf(p.We[2 * k], vv.x, p.be[k]));
                         v = fmaxf(e, 0.f);
                     }
-                } else if (k < p.E + p.P) {
-                    v = p.pooled[(size_t)m * p.P + (k - p.E)];
+                } else if (kGoal && k < EG) {
+                    const int kg = k - p.E;
+                    if (kg < p.G - 2) {
+                        float2 gd = goal4[r];
+                        v = fmaxf(fmaf(p.Wgl[2 * kg + 1], gd.y, fmaf(p.Wgl[2 * kg], gd.x, p.bgl[kg])), 0.f);
+                    }
+                } else if (k < EG + p.P) {
+                    v = p.pooled[(size_t)m * p.P + (k - EG)];
                 } else if (k < p.K) {
-                    int u = k - p.E - p.P;
+                    int u = k - EG - p.P;
                     v = p.h_in[(size_t)m * H + u];
                     if (p.add_pooled_to_h) v += p.pooled[(size_t)m * H + u];   // lstm.py:151
                 }
@@ -257,22 +280,27 @@ __global__ void __launch_bounds__(kGThreads, U <= 4 ? 2 : 1) lstm_gates_kernel(G
     }
 }
 
-template <int U>
-static int launch_gates_t(const GateParams& p, cudaStream_t st) {
+template <int U, bool kGoal>
+static int launch_gates_k(const GateParams& p, cudaStream_t st) {
     const size_t smem = (size_t)2 * kGateBK * (4 * 32 * U + kGM) * sizeof(float);
     static DynSmemConfig configured;
-    TB2_CHECK_CUDA(configured.ensure(lstm_gates_kernel<U>, smem));
+    TB2_CHECK_CUDA(configured.ensure(lstm_gates_kernel<U, kGoal>, smem));
     const int blocks = (p.M + kGM - 1) / kGM;
     {
         KernelTimer kt("lstm_gates", st);
-        lstm_gates_kernel<U><<<blocks, kGThreads, smem, st>>>(p);
+        lstm_gates_kernel<U, kGoal><<<blocks, kGThreads, smem, st>>>(p);
     }
     TB2_LAUNCH_CHECK();
     return TB2_OK;
 }
 
+template <int U>
+static int launch_gates_t(const GateParams& p, cudaStream_t st) {
+    return p.G > 0 ? launch_gates_k<U, true>(p, st) : launch_gates_k<U, false>(p, st);
+}
+
 int launch_gates(const tb2_lstm* m, const tb2_layout* l, int phase, const float* obs1,
-                 const float* obs2, const float* pooled, const float* h_in, const float* c_in,
+                 const float* obs2, const float* goals, const float* pooled, const float* h_in, const float* c_in,
                  float* h_out, float* c_out, float* normal_out, float* pos_out, cudaStream_t st) {
     GateParams p;
     p.obs1 = (const float2*)obs1;
@@ -296,6 +324,10 @@ int launch_gates(const tb2_lstm* m, const tb2_layout* l, int phase, const float*
     p.K = m->K_gate;
     p.K_pad = m->K_gate_pad;
     p.add_pooled_to_h = (m->cfg.pool_type != TB2_POOL_NONE && !m->cfg.pool_to_input) ? 1 : 0;
+    p.goals = (const float2*)goals;
+    p.Wgl = m->Wgl;
+    p.bgl = m->bgl;
+    p.G = m->G;
     switch (m->H) {
         case 32: return launch_gates_t<1>(p, st);
         case 64: return launch_gates_t<2>(p, st);
@@ -448,16 +480,21 @@ int launch_repack(tb2_lstm* m, const tb2_lstm_weights* w, cudaStream_t st) {
     if ((rc = copy_dev(w->input_embedding_bias, m->be, (size_t)(m->E - 2), st))) return rc;
     if ((rc = copy_dev(w->hidden2normal_weight, m->Wn, (size_t)5 * m->H, st))) return rc;
     if ((rc = copy_dev(w->hidden2normal_bias, m->bn, 5, st))) return rc;
+    if (m->G > 0) {
+        TB2_REQUIRE(w->goal_embedding_weight && w->goal_embedding_bias, "goal embedding weights missing (goal_dim > 0)");
+        if ((rc = copy_dev(w->goal_embedding_weight, m->Wgl, (size_t)(m->G - 2) * 2, st))) return rc;
+        if ((rc = copy_dev(w->goal_embedding_bias, m->bgl, (size_t)(m->G - 2), st))) return rc;
+    }
     const float* wih[2] = {w->encoder_weight_ih, w->decoder_weight_ih};
     const float* whh[2] = {w->encoder_weight_hh, w->decoder_weight_hh};
     const float* bih[2] = {w->encoder_bias_ih, w->decoder_bias_ih};
     const float* bhh[2] = {w->encoder_bias_hh, w->decoder_bias_hh};
     for (int ph = 0; ph < 2; ++ph) {
         repack_gates_kernel<<<512, 256, 0, st>>>(wih[ph], whh[ph], bih[ph], bhh[ph], m->WgT[ph], m->bg[ph],
-                                                 m->E + m->P, m->H, m->K_gate_pad);
+                                                 m->E + m->G + m->P, m->H, m->K_gate_pad);
         TB2_LAUNCH_CHECK();
         if (m->Wg_hi[ph] &&
-            (rc = launch_repack_gates_tc(wih[ph], whh[ph], m->Wg_hi[ph], m->Wg_lo[ph], m->E + m->P, m->H, st)))
+            (rc = launch_repack_gates_tc(wih[ph], whh[ph], m->Wg_hi[ph], m->Wg_lo[ph], m->E + m->G + m->P, m->H, st)))
             return rc;
     }
     const tb2_lstm_config& c = m->cfg;

@@ -81,6 +81,10 @@ struct PrepParams {
     int E;
     int n_max, H, C, n, pool_type, front, skip_masked, write_pairs, pad_to_max;
     float side, width;
+    const float2* goals;      // goal-conditioned model (kGoal): the emb operand is [M, E + G] rows [emb | goal_emb]
+    const float* Wg;          // goal embedding [G-2, 2]
+    const float* bg;
+    int G;
 };
 
 __device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
@@ -98,6 +102,7 @@ __device__ __forceinline__ float nan_to_num_f(float x) {
     return x;
 }
 
+template <bool kGoal>
 __global__ void __launch_bounds__(kPrepMaxThreads, 2) pool_prepare_kernel(PrepParams p) {
     const int kPrepThreads = (int)blockDim.x, kPrepWarps = kPrepThreads >> 5;
     extern __shared__ __align__(16) float smem_prep[];
@@ -155,17 +160,27 @@ __global__ void __launch_bounds__(kPrepMaxThreads, 2) pool_prepare_kernel(PrepPa
     cp_async_wait_all();
     __syncthreads();
     if (p.emb_hi != nullptr) {
-        // emb = cat(relu(W_e . (4 v) + b_e), 0, 0) (modules.py:24-30) as bf16 (hi, lo) for the gate GEMM
-        const int e_shift = (p.E & (p.E - 1)) == 0 ? 31 - __clz(p.E) : -1;       // E = 64: no integer division per element
-        for (int idx = tid; idx < n_s * p.E; idx += kPrepThreads) {
-            const int j = e_shift >= 0 ? idx >> e_shift : idx / p.E, k = idx - j * p.E;
+        // emb = cat(relu(W_e . (4 v) + b_e), 0, 0) (modules.py:24-30) as bf16 (hi, lo) for the gate GEMM; kGoal: followed
+        // in the row by cat(relu(W_g . (4 d) + b_g), 0, 0), d = (obs2 - goal) / |obs2 - goal|, 0 at norm 0 (lstm.py:131-139)
+        const int EW = kGoal ? p.E + p.G : p.E;                                     // row width of the operand
+        const int e_shift = (EW & (EW - 1)) == 0 ? 31 - __clz(EW) : -1;           // E = 64: no integer division per element
+        for (int idx = tid; idx < n_s * EW; idx += kPrepThreads) {
+            const int j = e_shift >= 0 ? idx >> e_shift : idx / EW, k = idx - j * EW;
             const float2 v = vel[j];
             float e = 0.f;
-            if (k < p.E - 2 && !isnan(v.x))
+            if (k < p.E - 2 && !isnan(v.x)) {
                 e = fmaxf(fmaf(p.We[2 * k + 1], v.y * 4.0f, fmaf(p.We[2 * k], v.x * 4.0f, p.be[k])), 0.f);
+            } else if (kGoal && k >= p.E && k < EW - 2 && !isnan(v.x)) {
+                const int kg = k - p.E;
+                const float2 b = p.obs2[row0 + j], g = p.goals[row0 + j];
+                const float dx = b.x - g.x, dy = b.y - g.y;
+                const float n = sqrtf(dx * dx + dy * dy);
+                const float gx = n != 0.f ? dx / n : 0.f, gy = n != 0.f ? dy / n : 0.f;
+                e = fmaxf(fmaf(p.Wg[2 * kg + 1], gy * 4.0f, fmaf(p.Wg[2 * kg], gx * 4.0f, p.bg[kg])), 0.f);
+            }
             const __nv_bfloat16 h = __float2bfloat16_rn(e);
-            p.emb_hi[(size_t)(row0 + j) * p.E + k] = h;
-            p.emb_lo[(size_t)(row0 + j) * p.E + k] = __float2bfloat16_rn(e - __bfloat162float(h));
+            p.emb_hi[(size_t)(row0 + j) * EW + k] = h;
+            p.emb_lo[(size_t)(row0 + j) * EW + k] = __float2bfloat16_rn(e - __bfloat162float(h));
         }
     }
     if (fast_lat) {
@@ -308,8 +323,9 @@ __global__ void __launch_bounds__(kPrepMaxThreads, 2) pool_prepare_kernel(PrepPa
 
 int launch_pool_prepare(const tb2_lstm* m, const tb2_layout* l, const float* hidden,
                         const float* obs1, const float* obs2, int skip_masked, int write_pairs,
-                        int write_emb, Workspace* ws, cudaStream_t st) {
+                        int write_emb, Workspace* ws, cudaStream_t st, const float* goals) {
     TB2_REQUIRE(l->n_max <= kMaxSceneForPrep, "scene larger than 256 pedestrians");
+    const bool goal_emb = write_emb && m->G > 0;
     PrepParams p;
     p.obs1 = (const float2*)obs1;
     p.obs2 = (const float2*)obs2;
@@ -337,6 +353,10 @@ int launch_pool_prepare(const tb2_lstm* m, const tb2_layout* l, const float* hid
     p.E = m->E;
     p.emb_hi = write_emb ? (__nv_bfloat16*)ws->emb_hi : nullptr;
     p.emb_lo = write_emb ? (__nv_bfloat16*)ws->emb_lo : nullptr;
+    p.goals = (const float2*)goals;
+    p.Wg = m->Wgl;
+    p.bg = m->bgl;
+    p.G = m->G;
     p.side = m->cfg.cell_side;        // pool_size == 1
     p.width = (float)m->cfg.n;
     int nm1 = l->n_max > 1 ? l->n_max - 1 : 1;
@@ -344,12 +364,14 @@ int launch_pool_prepare(const tb2_lstm* m, const tb2_layout* l, const float* hid
     size_t smem = (size_t)l->n_max * 2 * sizeof(float2) + (size_t)(((nthreads / 32) * nm1 + 3) & ~3) * sizeof(int);
     if (m->cfg.pool_type == TB2_POOL_SOCIAL) smem += ((size_t)(m->H + 8) * m->C + (size_t)l->n_max * m->H) * sizeof(float);
     smem = (smem + 15) & ~(size_t)15;
-    static DynSmemConfig configured;
+    static DynSmemConfig configured[2];
     TB2_REQUIRE(smem <= 227 * 1024, "scene too large for pool_prepare shared memory");
-    TB2_CHECK_CUDA(configured.ensure(pool_prepare_kernel, smem, 48 * 1024));
+    TB2_REQUIRE(!goal_emb || goals, "goals missing");
+    auto kernel = goal_emb ? pool_prepare_kernel<true> : pool_prepare_kernel<false>;
+    TB2_CHECK_CUDA(configured[goal_emb].ensure(kernel, smem, 48 * 1024));
     {
         KernelTimer kt("pool_prepare", st);
-        launch_pdl(pool_prepare_kernel, dim3(l->B), dim3(nthreads), smem, st, p);
+        launch_pdl(kernel, dim3(l->B), dim3(nthreads), smem, st, p);
     }
     TB2_LAUNCH_CHECK();
     return TB2_OK;

@@ -1644,6 +1644,10 @@ static int sequence_backward_impl(const tb2_lstm* m, const tb2_layout* l, const 
     TB2_REQUIRE(m->weights_set, "tb2_lstm_set_weights has not been called");
     TB2_REQUIRE(observed && positions && states && d_normals && active_rows, "null argument");
     TB2_REQUIRE(obs_length >= 2 && n_decode >= 0, "need obs_length >= 2 and n_decode >= 0");
+    if (m->G > 0) {
+        set_error("training a goal-conditioned model (goal_dim > 0) is not built");
+        return TB2_ERR_UNSUPPORTED;
+    }
     const bool social = m->cfg.pool_type == TB2_POOL_SOCIAL;
     if (social && (m->n_mlp < 1 || m->n_mlp > 2 || !m->cfg.pool_to_input || m->cfg.constant != 0.f)) {
         set_error("social training backward supports one_layer / two_layer embeddings with constant = 0");

@@ -5,6 +5,8 @@ The reference imports `trajnetplusplustools` (not vendored, absent from this ima
 visible in the reference's DATA_BLOCK/*.ndjson; these helpers implement just that.
 """
 import json
+import os
+import pickle
 from collections import namedtuple, defaultdict
 
 import numpy as np
@@ -78,6 +80,61 @@ def preprocess_test(scene, obs_len):
     last_obs_frame = obs_frames[-1]
     return [[row for row in ped if row.frame <= last_obs_frame]
             for ped in scene if ped[0].frame <= last_obs_frame]
+
+
+def goal_file(dataset_file):
+    """Where the reference's evaluator reads the goals of a test file (evaluator/write_utils.py:21-25): relative to the
+    working directory, goal_files/test_private/<file stem>.pkl."""
+    stem = os.path.splitext(os.path.basename(dataset_file))[0]
+    return os.path.join('goal_files', 'test_private', stem + '.pkl')
+
+
+def load_goal_file(path):
+    """The goals of a test file: dict pedestrian id -> (x, y), as written by the reference's get_dest.py."""
+    if not os.path.exists(path):
+        raise FileNotFoundError("goal file %s not found (a goal-conditioned model reads the goals of every test file "
+                                "from goal_files/test_private/<file>.pkl)" % path)
+    with open(path, 'rb') as f:
+        return pickle.load(f)
+
+
+def scene_pedestrians(filename):
+    """The pedestrian ids with a row inside some scene of an ndjson file (the scenes read_ndjson_scenes yields, before
+    preprocess_test): the ids whose goals the reference's evaluator looks up (evaluator/write_utils.py:21-25)."""
+    cols = parse_ndjson_columns(filename)
+    if cols is None:                                        # the row pipeline is the definition
+        return {path[0].pedestrian for _, paths in read_ndjson_scenes(filename) for path in paths}
+    order = np.argsort(cols['frame'], kind='stable')
+    f, p = cols['frame'][order], cols['ped'][order]
+    los = np.searchsorted(f, cols['scene_start'], side='left')
+    his = np.searchsorted(f, cols['scene_end'], side='right')
+    ids = set()
+    for lo, hi, primary in zip(los, his, cols['scene_ped']):
+        peds = np.unique(p[lo:hi])
+        if primary in peds:                                 # read_ndjson_scenes skips a scene without its primary
+            ids.update(peds.tolist())
+    return ids
+
+
+def check_goal_ids(goals, filename, path='goal file'):
+    """Raise KeyError naming the first pedestrian of a scene of `filename` that has no goal in `goals`.  Like the
+    reference, every track of a scene needs one, including the tracks preprocess_test then drops."""
+    missing = sorted(ped for ped in scene_pedestrians(filename) if ped not in goals)
+    if missing:
+        raise KeyError("%s has no goal for pedestrian %s (%d pedestrian(s) of %s without a goal)"
+                       % (path, missing[0], len(missing), filename))
+
+
+def scene_goals(goals, ped_ids, path='goal file'):
+    """float64 [len(ped_ids), 2]: the goals of a scene's tracks in track order (primary first), looked up by pedestrian
+    id.  The tracks are those the predictor gets, so a track preprocess_test drops has no goal row."""
+    out = np.empty((len(ped_ids), 2), dtype=np.float64)
+    for i, ped in enumerate(ped_ids):
+        g = goals.get(ped, goals.get(int(ped))) if hasattr(goals, 'get') else None
+        if g is None:
+            raise KeyError("%s has no goal for pedestrian %s" % (path, ped))
+        out[i] = (float(g[0]), float(g[1]))
+    return out
 
 
 def trajnet_line(row):

@@ -104,11 +104,13 @@ class LayoutCache:
         return item
 
 
-def lstm_config(hidden_dim, embedding_dim, pool_to_input, pool):
-    """tb2_lstm_config of an LSTM of these widths around the interaction module `pool` (None: no pooling)."""
+def lstm_config(hidden_dim, embedding_dim, pool_to_input, pool, goal_dim=0):
+    """tb2_lstm_config of an LSTM of these widths around the interaction module `pool` (None: no pooling); goal_dim > 0:
+    the LSTM input carries a goal embedding of that width (LSTM(goal_flag=True))."""
     cfg = _lib.LstmConfig()
     cfg.hidden_dim = int(hidden_dim)
     cfg.embedding_dim = int(embedding_dim)
+    cfg.goal_dim = int(goal_dim)
     cfg.pool_to_input = int(bool(pool_to_input))
     cfg.pool_type = _lib.POOL_NONE
     cfg.pool_size = cfg.blur_size = 1
@@ -298,7 +300,9 @@ class ModelHandle:
         with torch.cuda.device(self.device):
             _lib.check(lib.tb2_pool_state_reset(self.handle, layout.handle, _ptr(ws), need, _stream(self.device)))
 
-    def step_forward(self, layout, phase, obs1, obs2, h, c):
+    # goals: [M, 2] fp32 device tensor of a goal-conditioned model (None for any other; the library refuses a goal model
+    # without them)
+    def step_forward(self, layout, phase, obs1, obs2, h, c, goals=None):
         """One step; h, c updated in place.  Returns (normal [M,5], pos [M,2])."""
         lib = _lib.load()
         ws, need = self.workspace(layout)
@@ -306,31 +310,32 @@ class ModelHandle:
         normal = torch.empty((M, 5), dtype=torch.float32, device=self.device)
         pos = torch.empty((M, 2), dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
-            _lib.check(lib.tb2_lstm_step_forward(self.handle, layout.handle, phase, _ptr(obs1), _ptr(obs2),
-                                                 _ptr(h), _ptr(c), _ptr(h), _ptr(c), _ptr(normal),
-                                                 _ptr(pos), _ptr(ws), need, _stream(self.device)))
+            _lib.check(lib.tb2_lstm_step_forward_goals(self.handle, layout.handle, phase, _ptr(obs1), _ptr(obs2),
+                                                       _ptr(goals), _ptr(h), _ptr(c), _ptr(h), _ptr(c), _ptr(normal),
+                                                       _ptr(pos), _ptr(ws), need, _stream(self.device)))
         return normal, pos
 
-    def forward_steps(self, layout, observed, truth, n_decode, first_step, last_step, normals, positions, h, c):
+    def forward_steps(self, layout, observed, truth, n_decode, first_step, last_step, normals, positions, h, c,
+                      goals=None):
         """Steps [first_step, last_step) of the time loop on caller-owned state (tb2_lstm_forward_steps)."""
         lib = _lib.load()
         ws, need = self.workspace(layout)
         with torch.cuda.device(self.device):
-            _lib.check(lib.tb2_lstm_forward_steps(
+            _lib.check(lib.tb2_lstm_forward_steps_goals(
                 self.handle, layout.handle, _ptr(observed), int(observed.shape[0]), _ptr(truth),
-                int(n_decode), int(first_step), int(last_step), _ptr(normals), _ptr(positions), _ptr(h), _ptr(c),
-                _ptr(None), _ptr(ws), need, _stream(self.device)))
+                int(n_decode), _ptr(goals), int(first_step), int(last_step), _ptr(normals), _ptr(positions), _ptr(h),
+                _ptr(c), _ptr(None), _ptr(ws), need, _stream(self.device)))
 
     def forward_sequence_host(self, layout, observed, truth, n_decode, normals, positions, h, c, normals_host,
-                              positions_host, copy_stream):
+                              positions_host, copy_stream, goals=None):
         """tb2_lstm_forward_sequence_host: per-step device-to-host copies on `copy_stream`; the caller
         synchronises that stream before reading the pinned host tensors."""
         lib = _lib.load()
         ws, need = self.workspace(layout)
         with torch.cuda.device(self.device):
-            _lib.check(lib.tb2_lstm_forward_sequence_host(
+            _lib.check(lib.tb2_lstm_forward_sequence_host_goals(
                 self.handle, layout.handle, _ptr(observed), int(observed.shape[0]), _ptr(truth), int(n_decode),
-                _ptr(normals), _ptr(positions), _ptr(h), _ptr(c), _ptr(ws), need, _ptr(normals_host),
+                _ptr(goals), _ptr(normals), _ptr(positions), _ptr(h), _ptr(c), _ptr(ws), need, _ptr(normals_host),
                 _ptr(positions_host), _stream(self.device), ctypes.c_void_p(copy_stream.cuda_stream)))
 
     def train_cache_bytes(self, layout, num_steps):
@@ -348,11 +353,7 @@ class ModelHandle:
                 _ptr(normals), _ptr(positions), _ptr(h), _ptr(c), _ptr(states), _ptr(cache),
                 0 if cache is None else int(cache.numel()), _ptr(ws), need, _stream(self.device)))
 
-    def forward_sequence(self, layout, observed, truth, n_decode, normals, positions, h, c):
-        lib = _lib.load()
-        ws, need = self.workspace(layout)
-        with torch.cuda.device(self.device):
-            _lib.check(lib.tb2_lstm_forward_sequence(
-                self.handle, layout.handle, _ptr(observed), int(observed.shape[0]), _ptr(truth),
-                int(n_decode), _ptr(normals), _ptr(positions), _ptr(h), _ptr(c), _ptr(None),
-                _ptr(ws), need, _stream(self.device)))
+    def forward_sequence(self, layout, observed, truth, n_decode, normals, positions, h, c, goals=None):
+        """The whole time loop (tb2_lstm_forward_sequence, i.e. forward_steps over [0, S))."""
+        self.forward_steps(layout, observed, truth, n_decode, 0, int(observed.shape[0]) - 1 + int(n_decode), normals,
+                           positions, h, c, goals)

@@ -12,8 +12,8 @@ import inspect
 import os
 import shutil
 
-from .data import (load_test_scenes_xy, paths_to_xy, preprocess_test, read_ndjson_scenes, write_predictions,
-                   write_predictions_xy)
+from .data import (check_goal_ids, goal_file, load_goal_file, load_test_scenes_xy, paths_to_xy, preprocess_test,
+                   read_ndjson_scenes, scene_goals, write_predictions, write_predictions_xy)
 
 
 def load_test_scenes(filename, obs_length=9):
@@ -47,17 +47,20 @@ def batches_modes(predictor):
     return _takes_modes(predictor) and (supported is None or bool(supported()))
 
 
-def _predict_xy(predictor, xys, pred_length, obs_length, modes, args):
+def _predict_xy(predictor, xys, pred_length, obs_length, modes, args, goals=None):
     if batches_modes(predictor):
         return predictor.predict_batch_xy(xys, n_predict=pred_length, obs_length=obs_length, args=args, modes=modes)
+    if goals is not None:
+        return predictor.predict_batch_xy(xys, goals, n_predict=pred_length, obs_length=obs_length, args=args)
     return predictor.predict_batch_xy(xys, n_predict=pred_length, obs_length=obs_length, args=args)
 
 
-def predict_scenes(predictor, scenes, obs_length=9, pred_length=12, modes=1, chunk=1024, args=None):
+def predict_scenes(predictor, scenes, obs_length=9, pred_length=12, modes=1, chunk=1024, args=None, goals=None):
     """Predictions for a list of (filename, scene_id, paths), in order.  A predictor with
     predict_batch (LSTMPredictor) gets `chunk` scenes per forward at modes 1, one whose predict_batch_xy takes `modes`
     (S-GAN / VAE) `chunk` scenes per decode of all modes; any other predictor of the reference's call signature
-    (classical, LSTM at modes > 1) is called scene by scene."""
+    (classical, LSTM at modes > 1) is called scene by scene.  goals: per scene the goals [N, 2] of its tracks (a
+    goal-conditioned model), else None (the predictor gets zeros, like the reference's)."""
     out = []
     if batches_modes(predictor):
         for i in range(0, len(scenes), chunk):
@@ -67,12 +70,16 @@ def predict_scenes(predictor, scenes, obs_length=9, pred_length=12, modes=1, chu
     if hasattr(predictor, 'predict_batch') and modes == 1:
         for i in range(0, len(scenes), chunk):
             part = [paths for _, _, paths in scenes[i:i + chunk]]
-            out.extend(predictor.predict_batch(part, n_predict=pred_length, obs_length=obs_length, args=args))
+            if goals is not None:
+                out.extend(predictor.predict_batch(part, goals[i:i + chunk], n_predict=pred_length, obs_length=obs_length,
+                                                   args=args))
+            else:
+                out.extend(predictor.predict_batch(part, n_predict=pred_length, obs_length=obs_length, args=args))
         return out
     import numpy as np
-    for _, _, paths in scenes:
-        out.append(predictor(paths, np.zeros((len(paths), 2)), n_predict=pred_length, obs_length=obs_length,
-                             modes=modes, args=args))
+    for i, (_, _, paths) in enumerate(scenes):
+        goal = goals[i] if goals is not None else np.zeros((len(paths), 2))
+        out.append(predictor(paths, goal, n_predict=pred_length, obs_length=obs_length, modes=modes, args=args))
     return out
 
 
@@ -108,27 +115,36 @@ def _column_pipeline(predictor, modes):
 
 
 def evaluate_file(predictor, infile, outfile, obs_length=9, pred_length=12, modes=1, chunk=1024, args=None,
-                  rank=None, world_size=None):
+                  rank=None, world_size=None, goals=None, goals_path='goal file'):
     """ndjson in -> ndjson out (the records evaluator/write_utils.write_predictions appends).
     Returns the number of scenes of the file.  With world_size > 1 (arguments or the initialised process group) the
-    scenes are sharded over the ranks; rank 0 assembles `outfile` from the per-rank parts."""
+    scenes are sharded over the ranks; rank 0 assembles `outfile` from the per-rank parts.
+
+    goals: for a goal-conditioned model the goals of the file (dict pedestrian id -> (x, y), read from goals_path).
+    Every scene gets the goals of the tracks it keeps, in track order; a missing id raises before anything is written.
+    Deliberate deviation: the reference passes the goals of the unfiltered scene, so a scene with a track that
+    preprocess_test drops fails there on mismatched shapes."""
     columns = _column_pipeline(predictor, modes)
     if columns:
         scenes = load_test_scenes_xy(infile, obs_length)                 # [(xy, SceneMeta)]
         sizes = [xy.shape[1] for xy, _ in scenes]
+        if goals is not None:
+            goals = [scene_goals(goals, [meta.pedestrian] + list(meta.neigh_ids), goals_path) for _, meta in scenes]
 
-        def run(part, filename):
+        def run(part, part_goals, filename):
             preds = []
             for i in range(0, len(part), chunk):
                 preds.extend(_predict_xy(predictor, [xy for xy, _ in part[i:i + chunk]], pred_length, obs_length, modes,
-                                         args))
+                                         args, None if part_goals is None else part_goals[i:i + chunk]))
             write_predictions_xy(preds, [meta for _, meta in part], filename, obs_length=obs_length, pred_length=pred_length)
     else:
         scenes = load_test_scenes(infile, obs_length)                    # [(filename, scene_id, paths)]
         sizes = [len(paths) for _, _, paths in scenes]
+        if goals is not None:
+            goals = [scene_goals(goals, [path[0].pedestrian for path in paths], goals_path) for _, _, paths in scenes]
 
-        def run(part, filename):
-            preds = predict_scenes(predictor, part, obs_length, pred_length, modes, chunk, args)
+        def run(part, part_goals, filename):
+            preds = predict_scenes(predictor, part, obs_length, pred_length, modes, chunk, args, part_goals)
             write_predictions(preds, part, filename, obs_length=obs_length, pred_length=pred_length)
     rank, world = _rank_world(rank, world_size)
     if world == 1:
@@ -136,7 +152,7 @@ def evaluate_file(predictor, infile, outfile, obs_length=9, pred_length=12, mode
             os.remove(outfile)
         open(outfile, "w").close()
         if scenes:
-            run(scenes, outfile)
+            run(scenes, goals, outfile)
         return len(scenes)
     from .parallel import shard_scenes
     split = [0]
@@ -149,7 +165,7 @@ def evaluate_file(predictor, infile, outfile, obs_length=9, pred_length=12, mode
         os.remove(part)
     open(part, "w").close()                                # an empty shard still leaves its (empty) part
     if mine:
-        run(mine, part)
+        run(mine, None if goals is None else goals[lo:hi], part)
     _barrier()                                              # every part is complete
     if rank == 0:
         with open(outfile, "wb") as out:
@@ -165,7 +181,11 @@ def evaluate_file(predictor, infile, outfile, obs_length=9, pred_length=12, mode
 def get_predictions(args, load_predictor=None):
     """The write side of lstm/trajnet_evaluator.get_predictions (:28-64): for every model in args.output
     and every `*.ndjson` of the test folder, write `<path>/test_pred/<model>_modes<k>/<dataset>.ndjson`.
-    Existing model folders are skipped, like the reference does.  Returns {model_name: scenes written}."""
+    Existing model folders are skipped, like the reference does.  A goal-conditioned model (predictor.model.goal_flag)
+    reads the goals of every test file from goal_files/test_private/<file>.pkl under the working directory, like the
+    reference's evaluator.  Every goal file is loaded, and every pedestrian of every scene checked to have a goal, before
+    the model folder is created: a missing file or id leaves nothing behind that a re-run would take for finished
+    predictions.  Returns {model_name: scenes written}."""
     if load_predictor is None:
         def load_predictor(filename):
             from .lstm import LSTMPredictor
@@ -186,14 +206,19 @@ def get_predictions(args, load_predictor=None):
             if rank == 0:
                 print('Predictions corresponding to {} already exist.'.format(model_name))
             continue
+        predictor = load_predictor(model)
+        goals = {}
+        if getattr(getattr(predictor, 'model', None), 'goal_flag', False):
+            for dataset in datasets:
+                goals[dataset] = load_goal_file(goal_file(dataset))
+                check_goal_ids(goals[dataset], os.path.join(test_dir, dataset), goal_file(dataset))
         if rank == 0:
             os.makedirs(out_dir)
         _barrier()
-        predictor = load_predictor(model)
         written[model_name] = sum(
             evaluate_file(predictor, os.path.join(test_dir, dataset), os.path.join(out_dir, dataset),
                           obs_length=args.obs_length, pred_length=args.pred_length, modes=args.modes,
-                          chunk=args.chunk, args=args)
+                          chunk=args.chunk, args=args, goals=goals.get(dataset), goals_path=goal_file(dataset))
             for dataset in datasets)
     return written
 

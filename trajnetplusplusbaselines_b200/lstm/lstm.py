@@ -21,7 +21,7 @@ from .modules import Hidden2Normal, InputEmbedding
 NAN = float('nan')
 
 # one forward set up by LSTM._sequence
-Sequence = namedtuple('Sequence', 'handle layout obs truth n_decode S_enc S normals positions h c out_device')
+Sequence = namedtuple('Sequence', 'handle layout obs truth n_decode S_enc S normals positions h c out_device goals')
 
 
 def drop_distant(xy, r=6.0):
@@ -78,7 +78,7 @@ class LSTM(torch.nn.Module):
 
         self.goal_flag = goal_flag
         self.goal_dim = goal_dim or embedding_dim
-        self.goal_embedding = InputEmbedding(2, self.goal_dim, scale)   # kept for state_dict parity
+        self.goal_embedding = InputEmbedding(2, self.goal_dim, scale)
         goal_rep_dim = self.goal_dim if self.goal_flag else 0
 
         pooling_dim = 0
@@ -101,8 +101,6 @@ class LSTM(torch.nn.Module):
         """force_repack: re-upload / repack the weights even if (data_ptr, _version, optimizer epoch) did
         not change.  The training forward passes True: updates through `p.data` (manual SGD, EMA,
         `.data.clamp_`) change none of the three."""
-        if self.goal_flag:
-            raise NotImplementedError("goal_flag=True is not built (off in every BASELINE config)")
         device = self._device()
         if device.type != 'cuda':
             _lib.require_cuda()
@@ -111,7 +109,8 @@ class LSTM(torch.nn.Module):
         if self._handle is None or self._handle.device != device:
             if self.pool is not None and not hasattr(self.pool, 'fill_config'):
                 raise NotImplementedError("only GridBasedPooling and the HiddenStateMLPPooling / NearestNeighborMLP / AttentionMLPPooling / NearestNeighborLSTM / TrajectronPooling interaction modules are built")
-            cfg = lstm_config(self.hidden_dim, self.embedding_dim, self.pool_to_input, self.pool)
+            cfg = lstm_config(self.hidden_dim, self.embedding_dim, self.pool_to_input, self.pool,
+                              self.goal_dim if self.goal_flag else 0)
             self._handle = ModelHandle(cfg, device)
         key = weights_key(self)
         if force_repack or key != self._handle._weights_key:
@@ -128,12 +127,30 @@ class LSTM(torch.nn.Module):
             decoder_bias_ih=self.decoder.bias_ih, decoder_bias_hh=self.decoder.bias_hh,
             hidden2normal_weight=self.hidden2normal.linear.weight,
             hidden2normal_bias=self.hidden2normal.linear.bias)
+        if self.goal_flag:
+            goal = self.goal_embedding.input_embeddings[0]
+            fields.update(goal_embedding_weight=goal.weight, goal_embedding_bias=goal.bias)
         if self.pool is not None:
             fields.update(self.pool.weight_fields())
         return fields
 
-    def _to_device(self, t, device):
-        """Host tensors go through pinned staging (H2D inside the caller's timed region)."""
+    def _goals_on(self, goals, num_tracks, device):
+        """The goals [M, 2] a goal-conditioned model reads, fp32 on `device`; None for a model without goal input (which
+        ignores them, like the reference)."""
+        if not self.goal_flag:
+            return None
+        if goals is None:
+            raise ValueError("goal_flag=True: the model needs the goals of the tracks ([M, 2])")
+        if not torch.is_tensor(goals):
+            goals = torch.as_tensor(np.asarray(goals, dtype=np.float64))
+        if tuple(goals.shape) != (num_tracks, 2):
+            raise ValueError("goals must be [%d, 2] (one per track), got %s" % (num_tracks, list(goals.shape)))
+        return self._to_device(goals, device, 'goals')
+
+    def _to_device(self, t, device, slot):
+        """Host tensors go through pinned staging (H2D inside the caller's timed region).  slot names the argument: each
+        argument of a call has its own staging buffer, and a buffer is refilled only once its previous asynchronous copy
+        to the device has completed."""
         if t is None:
             return None
         t = t.detach()
@@ -142,15 +159,19 @@ class LSTM(torch.nn.Module):
         t = t.to(dtype=torch.float32).contiguous()
         if t.is_pinned():
             return t.to(device, non_blocking=True)
-        key = (tuple(t.shape), 'in')
-        buf = self._pinned.get(key)
-        if buf is None:
-            buf = torch.empty(t.shape, dtype=torch.float32, pin_memory=True)
-            self._pinned[key] = buf
+        key = (tuple(t.shape), 'in', slot)
+        staged = self._pinned.get(key)
+        if staged is None:
+            staged = (torch.empty(t.shape, dtype=torch.float32, pin_memory=True), torch.cuda.Event())
+            self._pinned[key] = staged
+        buf, copied = staged
+        copied.synchronize()              # the previous copy out of this buffer has been read (no-op before the first)
         # plain single-threaded memcpy: torch's CPU copy_ may go through the intra-op thread pool,
         # whose wake-up latency showed rare 10-50 ms tails on the (virtualised) GPU hosts
         np.copyto(buf.numpy(), t.numpy())
-        return buf.to(device, non_blocking=True)
+        out = buf.to(device, non_blocking=True)
+        copied.record(torch.cuda.current_stream(device))
+        return out
 
     # -- reference API -----------------------------------------------------------------------
     def step(self, lstm, hidden_cell_state, obs1, obs2, goals, batch_split):
@@ -166,9 +187,10 @@ class LSTM(torch.nn.Module):
         h = h.detach().to(device=device, dtype=torch.float32).contiguous().clone()
         c = c.detach().to(device=device, dtype=torch.float32).contiguous().clone()
         layout = self._layouts.get(batch_split, device=device)
-        o1 = self._to_device(obs1, device)
-        o2 = self._to_device(obs2, device)
-        normal, _ = handle.step_forward(layout, phase, o1, o2, h, c)
+        o1 = self._to_device(obs1, device, 'obs1')
+        o2 = self._to_device(obs2, device, 'obs2')
+        g = self._goals_on(goals, layout.num_tracks, device)
+        normal, _ = handle.step_forward(layout, phase, o1, o2, h, c, g)
         if was_list:
             return (list(h), list(c)), normal
         return (h, c), normal
@@ -184,24 +206,26 @@ class LSTM(torch.nn.Module):
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             from .training import sequence_with_grad
             return sequence_with_grad(self, observed, batch_split, prediction_truth, n_predict)
-        return self._forward_nograd(observed, batch_split, prediction_truth, n_predict)
+        return self._forward_nograd(observed, batch_split, prediction_truth, n_predict, goals=goals)
 
-    def _sequence(self, observed, batch_split, prediction_truth, n_predict, pad_to_batch_max=True, force_repack=False):
+    def _sequence(self, observed, batch_split, prediction_truth, n_predict, pad_to_batch_max=True, force_repack=False,
+                  goals=None):
         """A forward of `observed` [obs_length, M, 2] set up on the model's device: the inputs there and empty outputs
         and (h, c) state.  Launches nothing.  The steps are [0, S_enc) for the encoder and [S_enc, S) for the decoder;
-        truth is None when there is no teacher forcing."""
+        truth is None when there is no teacher forcing.  goals [M, 2]: read by a goal-conditioned model only."""
         handle = self._engine(force_repack)
         device = handle.device
         layout = self._layouts.get(batch_split, pad_to_batch_max, device=device)
         M = layout.num_tracks
         if observed.shape[1] != M:
             raise ValueError("batch_split[-1] != number of tracks")
-        obs = self._to_device(observed, device)
+        obs = self._to_device(observed, device, 'observed')
+        goals = self._goals_on(goals, M, device)
         truth = None
         if prediction_truth is not None:
             if isinstance(prediction_truth, (list, tuple)):
                 prediction_truth = torch.stack(list(prediction_truth))
-            truth = self._to_device(prediction_truth, device)
+            truth = self._to_device(prediction_truth, device, 'truth')
             n_decode = int(truth.shape[0])
             if n_decode == 0:
                 truth = None
@@ -213,12 +237,12 @@ class LSTM(torch.nn.Module):
         return Sequence(handle, layout, obs, truth, n_decode, S_enc, S,
                         normals=torch.empty((S, M, 5), **f32), positions=torch.empty((S, M, 2), **f32),
                         h=torch.empty((M, self.hidden_dim), **f32), c=torch.empty((M, self.hidden_dim), **f32),
-                        out_device=observed.device)
+                        out_device=observed.device, goals=goals)
 
     def _encode(self, seq):
         """The encoder steps [0, S_enc) of `seq`, into its own outputs and state."""
         seq.handle.forward_steps(seq.layout, seq.obs, seq.truth, seq.n_decode, 0, seq.S_enc, seq.normals,
-                                 seq.positions, seq.h, seq.c)
+                                 seq.positions, seq.h, seq.c, seq.goals)
         return seq
 
     def _decode(self, seq, context, seed=True):
@@ -228,7 +252,7 @@ class LSTM(torch.nn.Module):
         normals, positions = seq.normals.clone(), seq.positions.clone()
         context(h, c)
         seq.handle.forward_steps(seq.layout, seq.obs, seq.truth, seq.n_decode, seq.S_enc, seq.S, normals, positions,
-                                 h, c)
+                                 h, c, seq.goals)
         return self._results(seq, normals, positions, seed)
 
     def _results(self, seq, normals, positions, seed=True):
@@ -241,8 +265,8 @@ class LSTM(torch.nn.Module):
         return normals, positions
 
     def _forward_nograd(self, observed, batch_split, prediction_truth, n_predict, want_states=False,
-                        pad_to_batch_max=True, force_repack=False):
-        seq = self._sequence(observed, batch_split, prediction_truth, n_predict, pad_to_batch_max, force_repack)
+                        pad_to_batch_max=True, force_repack=False, goals=None):
+        seq = self._sequence(observed, batch_split, prediction_truth, n_predict, pad_to_batch_max, force_repack, goals)
         handle, layout, device = seq.handle, seq.layout, seq.handle.device
         inputs = (layout, seq.obs, seq.truth, seq.n_decode, seq.normals, seq.positions, seq.h, seq.c)
         if want_states:
@@ -259,10 +283,10 @@ class LSTM(torch.nn.Module):
             # while the later steps compute; one synchronisation of that stream at the end
             normals_h, positions_h = self._host_buffers(seq.normals, seq.positions)
             copy_stream = self._copy_stream(device)
-            handle.forward_sequence_host(*inputs, normals_h, positions_h, copy_stream)
+            handle.forward_sequence_host(*inputs, normals_h, positions_h, copy_stream, seq.goals)
             copy_stream.synchronize()
             return normals_h.view(normals_h.shape), positions_h.view(positions_h.shape)
-        handle.forward_sequence(*inputs)
+        handle.forward_sequence(*inputs, seq.goals)
         return self._results(seq, seq.normals, seq.positions)
 
     def _host_buffers(self, *tensors):
@@ -380,22 +404,31 @@ class LSTMPredictor(Predictor):
 
     def predict_batch_xy(self, xys, scene_goals=None, n_predict=12, obs_length=9, start_length=0, args=None):
         """predict_batch on arrays: xys = list of float64 [n_frames, N_i, 2] as paths_to_xy returns them (the column
-        pipeline of the evaluator, data.load_test_scenes_xy, builds them without TrackRow objects)."""
+        pipeline of the evaluator, data.load_test_scenes_xy, builds them without TrackRow objects).  scene_goals: per
+        scene the goals [N_i, 2] of its tracks, read by a goal-conditioned model (goal_flag=True) only."""
         self.model.eval()
         normalize = bool(getattr(args, 'normalize_scene', False))
         split = np.zeros(len(xys) + 1, dtype=np.int64)
         split[1:] = np.cumsum([xy.shape[1] for xy in xys])
+        goals = None
+        if self.model.goal_flag:
+            if scene_goals is None or len(scene_goals) != len(xys):
+                raise ValueError("goal_flag=True: predict_batch_xy needs one goal array per scene (scene_goals)")
+            goals = np.concatenate([np.asarray(g, dtype=np.float64).reshape(-1, 2) for g in scene_goals], axis=0)
         with torch.no_grad():
             if normalize:
                 # center_scene / inverse_scene of every scene on the device (lstm/scene_ops.py, SURVEY.md 8f rank 3)
                 from .scene_ops import inverse_scenes, preprocess_scenes
-                observed, _, _, rotation, center = preprocess_scenes([xy[:obs_length] for xy in xys], device=self.model._device(),
-                                                                     normalize_scene=True, obs_length=obs_length)
+                prepared = preprocess_scenes([xy[:obs_length] for xy in xys], device=self.model._device(),
+                                             normalize_scene=True, obs_length=obs_length, goals=goals)
+                observed, _, _, rotation, center = prepared[:5]
+                goals = prepared[5] if goals is not None else None
                 observed = observed[start_length:]
             else:
                 observed = torch.Tensor(np.concatenate([xy[start_length:obs_length] for xy in xys], axis=1))
+                goals = torch.Tensor(goals) if goals is not None else None
             _, output_scenes = self.model._forward_nograd(observed, torch.from_numpy(split), None, n_predict,
-                                                          pad_to_batch_max=False)
+                                                          pad_to_batch_max=False, goals=goals)
             if normalize:
                 output_scenes = inverse_scenes(output_scenes, split, rotation, center)
             else:

@@ -42,7 +42,7 @@ def _frame_table(center, angle):
     return table
 
 
-def preprocess_scenes(scenes, device=None, r=None, normalize_scene=False, obs_length=9, thetas=None):
+def preprocess_scenes(scenes, device=None, r=None, normalize_scene=False, obs_length=9, thetas=None, goals=None):
     """Build one model batch from `scenes` (list of float64 arrays [T, N_i, 2], primary first, as Reader.paths_to_xy
     returns them), doing per scene what the reference's trainer loop does (lstm/trainer.py:107-116):
 
@@ -51,7 +51,11 @@ def preprocess_scenes(scenes, device=None, r=None, normalize_scene=False, obs_le
       thetas [B]     -> random_rotation with these angles (the caller draws them: `random.random() * 2 * pi`)
 
     Returns (xy float32 CUDA tensor [T, M', 2], batch_split int64 CPU tensor [B + 1], keep mask bool ndarray [M],
-    rotation ndarray [B], centre ndarray [B, 2]); rotation / centre are zeros without normalize_scene."""
+    rotation ndarray [B], centre ndarray [B, 2]); rotation / centre are zeros without normalize_scene.
+
+    goals: float64 [M, 2], one goal per track of the concatenated scenes.  They go through the same transform as the
+    positions (center_scene / random_rotation with goals, lstm/utils.py:10-51), a track that drop_distant removes takes
+    its goal with it, and float32 goals [M', 2] on the device are appended to the returned tuple."""
     _lib.require_cuda()
     lib = _lib.load()
     device = _device_of(device)
@@ -87,6 +91,15 @@ def preprocess_scenes(scenes, device=None, r=None, normalize_scene=False, obs_le
         out = torch.empty((T, M_out, 2), dtype=torch.float32, device=device)
         _lib.check(lib.tb2_scenes_transform(_ptr(xy), _ptr(off), _ptr(keep_dev), _ptr(out_off), T, M, M_out, B, _ptr(frame),
                                             _ptr(aug), _ptr(out), st))
+        if goals is not None:           # one more "frame" of points through the same per-point transform
+            goals = np.ascontiguousarray(goals, dtype=np.float64)
+            if goals.shape != (M, 2):
+                raise ValueError("goals must be [%d, 2] (one per track), got %s" % (M, list(goals.shape)))
+            goals_in = torch.from_numpy(goals).to(device)
+            goals_out = torch.empty((M_out, 2), dtype=torch.float32, device=device)
+            _lib.check(lib.tb2_scenes_transform(_ptr(goals_in), _ptr(off), _ptr(keep_dev), _ptr(out_off), 1, M, M_out, B,
+                                                _ptr(frame), _ptr(aug), _ptr(goals_out), st))
+            return out, torch.from_numpy(new_split), keep, rotation, center, goals_out
     return out, torch.from_numpy(new_split), keep, rotation, center
 
 

@@ -29,8 +29,15 @@ _GRAD_FIELDS = {
 }
 
 
+def _refuse_goals(model):
+    if model.goal_flag:       # goal-conditioned models are built for inference only
+        from .trainer import GOALS_MESSAGE
+        raise NotImplementedError(GOALS_MESSAGE)
+
+
 def _grad_targets(model):
     """field name -> parameter, for every parameter the backward kernel produces a gradient for."""
+    _refuse_goals(model)
     out = {k: f(model) for k, f in _GRAD_FIELDS.items()}
     pool = model.pool
     if pool is not None and not hasattr(pool, 'embedding_arch'):        # only GridBasedPooling has a backward
@@ -120,5 +127,6 @@ class _SequenceFn(torch.autograd.Function):
 
 
 def sequence_with_grad(model, observed, batch_split, prediction_truth, n_predict):
+    _refuse_goals(model)
     params = tuple(model.parameters())
     return _SequenceFn.apply(model, observed, batch_split, prediction_truth, n_predict, *params)

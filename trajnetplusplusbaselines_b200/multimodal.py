@@ -66,12 +66,22 @@ def observed_batch(body, xys, obs_length, start_length, normalize):
     return torch.from_numpy(host.astype(np.float32)).to(device), split, None, None
 
 
+GOALS_MESSAGE = "S-GAN / VAE with goal_flag=True are not built (goal-conditioned decoding); goal_flag=True is built for LSTM"
+
+
+def refuse_goals(model):
+    """S-GAN / VAE decode without goals: a goal-conditioned one is refused rather than run on missing inputs."""
+    if getattr(model, 'goal_flag', False):
+        raise NotImplementedError(GOALS_MESSAGE)
+
+
 def predict_modes(body, observed, split, n_predict, modes, context, max_rows=None):
     """Encoder once over the scenes of `split`, then the decoders of all `modes` modes.
 
     context(h_enc, c_enc, q0, q1, h_out, c_out) writes the decoder starting state of modes [q0, q1) into
     h_out / c_out [(q1 - q0) * M, H].  Returns the positions of the last n_predict steps, float32 [n_predict,
     modes * M, 2] on the device, mode-major."""
+    refuse_goals(body)
     enc = body._encode(body._sequence(observed, split, None, n_predict, pad_to_batch_max=False))
     handle, device, M, S_enc, S = enc.handle, enc.handle.device, enc.layout.num_tracks, enc.S_enc, enc.S
     H = int(body.hidden_dim)

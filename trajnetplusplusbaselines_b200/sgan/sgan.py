@@ -61,6 +61,7 @@ class LSTMGenerator(LSTM):
 
     def encode(self, observed, batch_split, prediction_truth, n_predict):
         """Encoder steps only; returns the sequence every mode's decoder starts from."""
+        multimodal.refuse_goals(self)
         if prediction_truth is not None:
             # sgan.py:367-369 chains (observed[-1:], prediction_truth[:-1]): the last frame is unused
             prediction_truth = prediction_truth[:-1]
@@ -119,6 +120,7 @@ class LSTMDiscriminator(torch.nn.Module):
 
     def forward(self, observed, prediction, goals, batch_split):
         """scores [batch_size, 1] of the primary tracks (sgan.py:524-581)."""
+        multimodal.refuse_goals(self)
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             raise NotImplementedError("S-GAN training is not built; score under torch.no_grad()")
         body = self._lstm[0]

@@ -86,6 +86,7 @@ class VAE(torch.nn.Module):
     def forward(self, observed, goals, batch_split, prediction_truth=None, n_predict=None):
         """(rel_pred_scene list, pred_scene list, z_distr_xy, z_distr_x), vae.py:188-315 in eval mode."""
         assert ((prediction_truth is None) + (n_predict is None)) == 1
+        multimodal.refuse_goals(self)
         if self.training or (torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())):
             raise NotImplementedError("VAE training (prediction encoder, KL term) is not built; use "
                                       "model.eval() under torch.no_grad()")
