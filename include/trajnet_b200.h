@@ -566,6 +566,17 @@ int tb2_orca_sweep(const tb2_layout* layout, const tb2_orca_params* p, const flo
                    const float* pos_dev, const float* vel_dev, const double* goal_dev, const double* speed_dev,
                    const double* truth_dev, int32_t truth_len, double* ade_out_dev, double* fde_out_dev, void* stream);
 
+/* tb2_sf_sweep with the derivatives of every item's ADE / FDE with respect to its setting (forward mode: each quantity
+ * of the rollout carries its partials d/d(tau, v0, sigma) as float64 duals).  Same arguments as tb2_sf_sweep, plus
+ *   dade_out_dev [P, B, 3], dfde_out_dev [P, B, 3] double: d/d(tau, v0, sigma) of ade_out[s * B + b] / fde_out[s * B + b]
+ * ade_out / fde_out equal tb2_sf_sweep's bit for bit (the values are the same operations in the same order).  The
+ * field-of-view weight and the speed clip are piecewise: their tangent is that of the branch the value takes.  A
+ * non-finite ADE has non-finite derivatives.  No atomics: reruns are bit-identical.  TB2_ERR_INVALID as tb2_sf_sweep,
+ * and for a scene of more than 256 pedestrians (the tangent rollout's register budget), before any launch. */
+int tb2_sf_sweep_grad(const tb2_layout* layout, const tb2_sf_params* p, const double* params_dev, int32_t P,
+                      const double* state_dev, const double* truth_dev, int32_t truth_len, double* ade_out_dev,
+                      double* fde_out_dev, double* dade_out_dev, double* dfde_out_dev, void* stream);
+
 /* Kalman predictor, HOST code (BASELINE configs[0] is CPU-only), float64.  Replaces
  * pykalman.KalmanFilter(...).em / .smooth / expected .sample rollout (classical/kalman.py:40-60).
  *   obs_host            [total_obs, 2] observed positions of all tracks, concatenated

@@ -185,6 +185,7 @@ PROTOTYPES = {
                                                  _sz, _vp]),
     "tb2_orca_simulate": (ctypes.c_int, [_vp, ctypes.POINTER(OrcaParams), _vp, _vp, _vp, _vp, _vp, _vp]),
     "tb2_sf_sweep": (ctypes.c_int, [_vp, ctypes.POINTER(SfParams), _vp, _i32, _vp, _vp, _i32, _vp, _vp, _vp]),
+    "tb2_sf_sweep_grad": (ctypes.c_int, [_vp, ctypes.POINTER(SfParams), _vp, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp]),
     "tb2_orca_sweep": (ctypes.c_int, [_vp, ctypes.POINTER(OrcaParams), _vp, _i32, _vp, _vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp]),
 }
 

@@ -221,10 +221,11 @@ def simulate(sim, params, inputs, batch_split, n_samples, out_dtype, device=None
     return out
 
 
-def sweep(sim, prepared, settings, params, inputs):
+def sweep(sim, prepared, settings, params, inputs, grad=False):
     """One tb2_<sim>_sweep launch: settings [P, 3] (checked by sweep_params), params the ctypes struct of the fields
     the settings leave alone, inputs the device tensors of prepared in the entry point's order -> (ade, fde) CUDA
-    float64 [P, B]."""
+    float64 [P, B].  grad: tb2_<sim>_sweep_grad instead -> (ade, fde, dade, dfde), the derivatives [P, B, 3] with
+    respect to the three settings."""
     import torch
     from .. import _lib
     from ..engine import _ptr, _stream
@@ -233,13 +234,14 @@ def sweep(sim, prepared, settings, params, inputs):
     B, T = int(prepared.truth.shape[0]), int(prepared.truth.shape[1])
     device = prepared.state.device
     prm = torch.from_numpy(settings).to(device)
-    ade = torch.empty((len(settings), B), dtype=torch.float64, device=device)
-    fde = torch.empty_like(ade)
+    outs = [torch.empty((len(settings), B), dtype=torch.float64, device=device) for _ in range(2)]
+    if grad:
+        outs += [torch.empty((len(settings), B, 3), dtype=torch.float64, device=device) for _ in range(2)]
     with torch.cuda.device(device):
-        _lib.check(getattr(lib, "tb2_%s_sweep" % sim)(prepared.layout.handle, ctypes.byref(params), _ptr(prm),
-                                                       len(settings), *map(_ptr, inputs), _ptr(prepared.truth), T,
-                                                       _ptr(ade), _ptr(fde), _stream(device)))
-    return ade, fde
+        _lib.check(getattr(lib, "tb2_%s_sweep%s" % (sim, "_grad" if grad else ""))(
+            prepared.layout.handle, ctypes.byref(params), _ptr(prm), len(settings), *map(_ptr, inputs),
+            _ptr(prepared.truth), T, *map(_ptr, outs), _stream(device)))
+    return tuple(outs)
 
 
 def predict(rollout, input_paths, dest_dict, dest_type, predict_all, n_predict, obs_length, stationary=False):

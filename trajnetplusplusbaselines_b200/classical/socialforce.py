@@ -13,6 +13,9 @@ from . import common
 from .common import FPS, SAMPLING_RATE, sampling_rate, sweep_params
 
 
+MAX_GRAD_SCENE = 256         # tb2_sf_sweep_grad's largest scene (kSfGradMaxScene, csrc/classical.cu)
+
+
 def steps_for(pred_length, rate=SAMPLING_RATE):
     """Simulation steps for pred_length observed frames (socialforce.py:93)."""
     return pred_length * rate
@@ -39,16 +42,29 @@ def rollout(state, speeds, batch_split, sf_params, pred_length, device=None):
     return simulate_batch(state, batch_split, sf_params, n_steps=steps_for(pred_length), device=device).cpu().numpy()
 
 
+def _sweep(prepared, params, fps, grad):
+    prm = sweep_params(params, np.float64, ("tau", "v0", "sigma"), (0, 2), int(prepared.truth.shape[0]))
+    rate = sampling_rate(fps)
+    p = _params(prm[0], steps_for(int(prepared.truth.shape[1]), rate), rate, fps)
+    return common.sweep("sf", prepared, prm, p, [prepared.state], grad=grad)
+
+
 def sweep(prepared, params, fps=FPS):
     """ADE / FDE of the primary of every scene of `prepared` (common.PreparedScenes) under every setting of params
     [P, 3] (tau, v0, sigma) -> (ade, fde) CUDA float64 [P, B], one launch (tb2_sf_sweep).  Row s equals
     simulate_batch(state, agent_offsets, params[s], n_steps=steps_for(pred_length, rate), sample_every=rate) with
     rate = sampling_rate(fps), scored against prepared.truth: distances in sample order summed in float64,
     ADE = sum / pred_length, FDE = the last distance.  The trajectories never reach device memory."""
-    prm = sweep_params(params, np.float64, ("tau", "v0", "sigma"), (0, 2), int(prepared.truth.shape[0]))
-    rate = sampling_rate(fps)
-    p = _params(prm[0], steps_for(int(prepared.truth.shape[1]), rate), rate, fps)
-    return common.sweep("sf", prepared, prm, p, [prepared.state])
+    return _sweep(prepared, params, fps, False)
+
+
+def sweep_grad(prepared, params, fps=FPS):
+    """sweep with derivatives -> (ade, fde, dade, dfde) CUDA float64; ade / fde [P, B] equal sweep's bit for bit,
+    dade / dfde [P, B, 3] are d/d(tau, v0, sigma) of them, carried through the rollout in forward mode
+    (tb2_sf_sweep_grad).  The field-of-view weight and the speed clip are piecewise: the derivative is that of the
+    branch taken.  The library refuses a scene of more than MAX_GRAD_SCENE pedestrians before any launch; the
+    parameters are checked as in sweep."""
+    return _sweep(prepared, params, fps, True)
 
 
 def predict(input_paths, dest_dict=None, dest_type='interp', sf_params=[0.5, 2.1, 0.3],

@@ -14,6 +14,7 @@
 #include <math_constants.h>
 
 #include <cmath>
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -22,30 +23,137 @@ namespace tb2 {
 // =========================================================================================
 // social force (double precision like upstream numpy)
 // =========================================================================================
+// The social-force code is written once over its scalar type T: double for the rollout itself, Dual for the rollout
+// that also carries d/d(tau, v0, sigma) (tb2_sf_sweep_grad).
+
+// Forward-mode dual number: a float64 value and its partials with respect to (tau, v0, sigma).  The value of every
+// operation is the double operation on the values, so a Dual rollout's values equal the double rollout's bit for bit.
+// Branches are taken by the caller on val(); their tangent is the taken branch's.
+struct Dual {
+    double v, d[3];
+    Dual() = default;
+    __device__ __forceinline__ Dual(double x) : v(x), d{0.0, 0.0, 0.0} {}
+
+    __device__ __forceinline__ friend Dual operator+(const Dual& a, const Dual& b) {
+        Dual r(a.v + b.v);
+#pragma unroll
+        for (int i = 0; i < 3; ++i) r.d[i] = a.d[i] + b.d[i];
+        return r;
+    }
+    __device__ __forceinline__ friend Dual operator+(const Dual& a, double b) {
+        Dual r = a;
+        r.v = a.v + b;
+        return r;
+    }
+    __device__ __forceinline__ friend Dual operator-(const Dual& a, const Dual& b) {
+        Dual r(a.v - b.v);
+#pragma unroll
+        for (int i = 0; i < 3; ++i) r.d[i] = a.d[i] - b.d[i];
+        return r;
+    }
+    __device__ __forceinline__ friend Dual operator-(double a, const Dual& b) {
+        Dual r(a - b.v);
+#pragma unroll
+        for (int i = 0; i < 3; ++i) r.d[i] = -b.d[i];
+        return r;
+    }
+    __device__ __forceinline__ friend Dual operator-(const Dual& a) {
+        Dual r(-a.v);
+#pragma unroll
+        for (int i = 0; i < 3; ++i) r.d[i] = -a.d[i];
+        return r;
+    }
+    __device__ __forceinline__ friend Dual operator*(const Dual& a, const Dual& b) {
+        Dual r(a.v * b.v);
+#pragma unroll
+        for (int i = 0; i < 3; ++i) r.d[i] = a.d[i] * b.v + a.v * b.d[i];
+        return r;
+    }
+    __device__ __forceinline__ friend Dual operator*(double a, const Dual& b) {
+        Dual r(a * b.v);
+#pragma unroll
+        for (int i = 0; i < 3; ++i) r.d[i] = a * b.d[i];
+        return r;
+    }
+    __device__ __forceinline__ friend Dual operator*(const Dual& a, double b) {
+        Dual r(a.v * b);
+#pragma unroll
+        for (int i = 0; i < 3; ++i) r.d[i] = a.d[i] * b;
+        return r;
+    }
+    __device__ __forceinline__ friend Dual operator/(const Dual& a, const Dual& b) {
+        Dual r(a.v / b.v);
+#pragma unroll
+        for (int i = 0; i < 3; ++i) r.d[i] = (a.d[i] - r.v * b.d[i]) / b.v;
+        return r;
+    }
+    __device__ __forceinline__ friend Dual operator/(double a, const Dual& b) {
+        Dual r(a / b.v);
+#pragma unroll
+        for (int i = 0; i < 3; ++i) r.d[i] = -(r.v * b.d[i]) / b.v;
+        return r;
+    }
+    __device__ __forceinline__ friend Dual operator/(const Dual& a, double b) {
+        Dual r(a.v / b);
+#pragma unroll
+        for (int i = 0; i < 3; ++i) r.d[i] = a.d[i] / b;
+        return r;
+    }
+    __device__ __forceinline__ Dual& operator+=(const Dual& b) { return *this = *this + b; }
+    // sqrt(0) occurs only as the norm of a zero vector, whose tangent is zero too: d = 0 there
+    __device__ __forceinline__ friend Dual sqrt(const Dual& a) {
+        Dual r(sqrt(a.v));
+        const double k = r.v == 0.0 ? 0.0 : 0.5 / r.v;
+#pragma unroll
+        for (int i = 0; i < 3; ++i) r.d[i] = a.d[i] * k;
+        return r;
+    }
+    __device__ __forceinline__ friend Dual exp(const Dual& a) {
+        Dual r(exp(a.v));
+#pragma unroll
+        for (int i = 0; i < 3; ++i) r.d[i] = r.v * a.d[i];
+        return r;
+    }
+};
+struct Dual2 { Dual x, y; };
+
+__device__ __forceinline__ double val(double x) { return x; }
+__device__ __forceinline__ double val(const Dual& x) { return x.v; }
+
+// A swept parameter's unit tangent: parameter i of (tau, v0, sigma); nothing to seed in a double.
+__device__ __forceinline__ void seed(double&, int) {}
+__device__ __forceinline__ void seed(Dual& x, int i) { x.d[i] = 1.0; }
+
+template <class T> struct Vec2Of { using type = double2; };
+template <> struct Vec2Of<Dual> { using type = Dual2; };
+
+template <class T>
 struct SfScene {
-    double* px; double* py; double* vx; double* vy; double* ex; double* ey; double* sp;
+    T* px; T* py; T* vx; T* vy; T* ex; T* ey; T* sp;
 };
 
-__device__ __forceinline__ double sf_potential(double rx, double ry, double sb, double ebx, double eby,
-                                               double dt, double v0, double sigma) {
+template <class T>
+__device__ __forceinline__ T sf_potential(T rx, T ry, T sb, T ebx, T eby, double dt, T v0, T sigma) {
     // V(r_ab) = v0 exp(-b / sigma), b = 0.5 sqrt((|r| + |r - dt s_b e_b|)^2 - (dt s_b)^2)
-    const double n1 = sqrt(rx * rx + ry * ry);
-    const double qx = rx - dt * sb * ebx, qy = ry - dt * sb * eby;
-    const double n2 = sqrt(qx * qx + qy * qy);
-    const double s = n1 + n2;
-    const double in_sqrt = s * s - (dt * sb) * (dt * sb);
-    const double b = 0.5 * sqrt(in_sqrt);
+    const T n1 = sqrt(rx * rx + ry * ry);
+    const T qx = rx - dt * sb * ebx, qy = ry - dt * sb * eby;
+    const T n2 = sqrt(qx * qx + qy * qy);
+    const T s = n1 + n2;
+    const T in_sqrt = s * s - (dt * sb) * (dt * sb);
+    const T b = 0.5 * sqrt(in_sqrt);
     return v0 * exp(-b / sigma);
 }
 
 // One pedestrian of a social-force rollout: position, velocity, destination, initial and maximum speed
-// (Simulator.__init__: initial_speeds, max_speeds = 1.3 x).
-struct SfAgent { double x, y, ux, uy, dx, dy, s0, smax; };
+// (Simulator.__init__: initial_speeds, max_speeds = 1.3 x).  Destination and speeds do not depend on the parameters.
+template <class T>
+struct SfAgent { T x, y, ux, uy; double dx, dy, s0, smax; };
 
-__device__ __forceinline__ SfAgent sf_agent_init(const double* st) {
-    SfAgent g;
+template <class T>
+__device__ __forceinline__ SfAgent<T> sf_agent_init(const double* st) {
+    SfAgent<T> g;
     g.x = st[0]; g.y = st[1]; g.ux = st[2]; g.uy = st[3]; g.dx = st[4]; g.dy = st[5];
-    g.s0 = sqrt(g.ux * g.ux + g.uy * g.uy);
+    g.s0 = sqrt(val(g.ux) * val(g.ux) + val(g.uy) * val(g.uy));
     g.smax = 1.3 * g.s0;
     return g;
 }
@@ -54,42 +162,46 @@ __device__ __forceinline__ double sf_cosphi() { return cos(200.0 / 2.0 / 180.0 *
 
 // First half of a step: the desired direction (NaN at the destination, as upstream), published with the state for the
 // neighbour loop of every pedestrian of the scene.
-__device__ __forceinline__ void sf_publish(const SfAgent& g, const SfScene& sc, int a, double& eax, double& eay) {
-    const double gx = g.dx - g.x, gy = g.dy - g.y;
-    const double gn = sqrt(gx * gx + gy * gy);
+template <class T>
+__device__ __forceinline__ void sf_publish(const SfAgent<T>& g, const SfScene<T>& sc, int a, T& eax, T& eay) {
+    const T gx = g.dx - g.x, gy = g.dy - g.y;
+    const T gn = sqrt(gx * gx + gy * gy);
     eax = gx / gn; eay = gy / gn;
     sc.px[a] = g.x; sc.py[a] = g.y; sc.vx[a] = g.ux; sc.vy[a] = g.uy; sc.ex[a] = eax; sc.ey[a] = eay;
     sc.sp[a] = sqrt(g.ux * g.ux + g.uy * g.uy);
 }
 
 // Second half: driving force + pairwise repulsion over b = 0 .. n-1 in index order, speed clip, position update.
-__device__ __forceinline__ void sf_advance(SfAgent& g, const SfScene& sc, int a, int n, double eax, double eay,
-                                           double dt, double tau, double v0, double sigma, double cosphi) {
+// The field-of-view test and the clip take their branch from the value.
+template <class T>
+__device__ __forceinline__ void sf_advance(SfAgent<T>& g, const SfScene<T>& sc, int a, int n, T eax, T eay, double dt,
+                                           T tau, T v0, T sigma, double cosphi) {
     const double fd = 1e-3;
-    double Fx = 1.0 / tau * (g.s0 * eax - g.ux);
-    double Fy = 1.0 / tau * (g.s0 * eay - g.uy);
-    double sumx = 0.0, sumy = 0.0;
+    T Fx = 1.0 / tau * (g.s0 * eax - g.ux);
+    T Fy = 1.0 / tau * (g.s0 * eay - g.uy);
+    T sumx = 0.0, sumy = 0.0;
     for (int b = 0; b < n; ++b) {
-        double fx = 0.0, fy = 0.0, w = 0.0;
+        T fx = 0.0, fy = 0.0;
+        double w = 0.0;
         if (b != a) {
-            const double rx = g.x - sc.px[b], ry = g.y - sc.py[b];
-            const double sb = sc.sp[b], ebx = sc.ex[b], eby = sc.ey[b];
-            const double v = sf_potential(rx, ry, sb, ebx, eby, dt, v0, sigma);
-            const double dvdx = (sf_potential(rx + fd, ry, sb, ebx, eby, dt, v0, sigma) - v) / fd;
-            const double dvdy = (sf_potential(rx, ry + fd, sb, ebx, eby, dt, v0, sigma) - v) / fd;
+            const T rx = g.x - sc.px[b], ry = g.y - sc.py[b];
+            const T sb = sc.sp[b], ebx = sc.ex[b], eby = sc.ey[b];
+            const T v = sf_potential(rx, ry, sb, ebx, eby, dt, v0, sigma);
+            const T dvdx = (sf_potential(rx + fd, ry, sb, ebx, eby, dt, v0, sigma) - v) / fd;
+            const T dvdy = (sf_potential(rx, ry + fd, sb, ebx, eby, dt, v0, sigma) - v) / fd;
             fx = -1.0 * dvdx; fy = -1.0 * dvdy;               // f_ab = -grad V
-            const double gx = -fx, gy = -fy;                  // w(e, -f_ab)
-            const bool in_sight = (eax * gx + eay * gy) > sqrt(gx * gx + gy * gy) * cosphi;
+            const T gx = -fx, gy = -fy;                       // w(e, -f_ab)
+            const bool in_sight = val(eax * gx + eay * gy) > val(sqrt(gx * gx + gy * gy) * cosphi);
             w = in_sight ? 1.0 : 0.5;
         }
         sumx += w * fx;
         sumy += w * fy;
     }
     Fx += sumx; Fy += sumy;
-    const double wx = g.ux + dt * Fx, wy = g.uy + dt * Fy;
-    const double wn = sqrt(wx * wx + wy * wy);
-    const double q = g.smax / wn;
-    const double factor = isnan(q) ? q : (q < 1.0 ? q : 1.0);       // numpy.minimum(1, q)
+    const T wx = g.ux + dt * Fx, wy = g.uy + dt * Fy;
+    const T wn = sqrt(wx * wx + wy * wy);
+    const T q = g.smax / wn;
+    const T factor = isnan(val(q)) ? q : (val(q) < 1.0 ? q : T(1.0));      // numpy.minimum(1, q)
     g.ux = wx * factor; g.uy = wy * factor;
     g.x = g.x + g.ux * dt; g.y = g.y + g.uy * dt;
 }
@@ -308,39 +420,44 @@ __device__ __forceinline__ void scene_sync() {
     else __syncthreads();
 }
 
-struct SfSim {
+// Social force over scalar type T; SfSim (double) is the rollout, SfGradSim (Dual) the rollout with its tangents.
+template <class T>
+struct SfRollout {
     using Params = tb2_sf_params;
     using Setting = double;                    // tau, v0, sigma
-    using Agent = SfAgent;
-    using Scene = SfScene;
-    using Handoff = double2;                   // phase 1 -> phase 2: the desired direction
-    using Pos = double2;
+    using Agent = SfAgent<T>;
+    using Scene = SfScene<T>;
+    using Handoff = typename Vec2Of<T>::type;  // phase 1 -> phase 2: the desired direction
+    using Pos = typename Vec2Of<T>::type;
     struct Inputs { const double* state; };
-    struct Consts { double dt, tau, v0, sigma, cosphi; };
-    static constexpr size_t kPedBytes = 7 * sizeof(double);
+    struct Consts { double dt; T tau, v0, sigma; double cosphi; };
+    static constexpr size_t kPedBytes = 7 * sizeof(T);
     static constexpr int kSampleOffset = 0;    // sample after step k = 0 .. n_steps - 1 when k % sample_every == 0
 
-    __device__ static Agent agent(const Inputs& in, int row) { return sf_agent_init(in.state + (size_t)row * 6); }
+    __device__ static Agent agent(const Inputs& in, int row) { return sf_agent_init<T>(in.state + (size_t)row * 6); }
+    // The swept parameters seeded with unit tangents (for T = Dual).
     __device__ static Consts consts(const Params& p, const Setting* row) {
-        return {(double)p.delta_t, row ? row[0] : (double)p.tau, row ? row[1] : (double)p.v0,
-                row ? row[2] : (double)p.sigma, sf_cosphi()};
+        Consts c = {(double)p.delta_t, row ? row[0] : (double)p.tau, row ? row[1] : (double)p.v0,
+                    row ? row[2] : (double)p.sigma, sf_cosphi()};
+        seed(c.tau, 0); seed(c.v0, 1); seed(c.sigma, 2);
+        return c;
     }
     // The scene arrays from pedestrian slot `first` on, each `stride` long.
     __device__ static Scene scene(void* arrays, size_t first, int stride) {
-        double* px = static_cast<double*>(arrays) + first * 7;
+        T* px = static_cast<T*>(arrays) + first * 7;
         return {px, px + stride, px + 2 * stride, px + 3 * stride, px + 4 * stride, px + 5 * stride, px + 6 * stride};
     }
     template <bool kWarp>
     __device__ static void prologue(const Agent&, const Scene&, int, bool) {}
     __device__ static Handoff phase1(const Agent& g, const Consts&, const Scene& sc, int a, int) {
-        double2 e;
+        Handoff e;
         sf_publish(g, sc, a, e.x, e.y);
         return e;
     }
     __device__ static void phase2(Agent& g, const Consts& c, const Scene& sc, int a, int n, Handoff e) {
         sf_advance(g, sc, a, n, e.x, e.y, c.dt, c.tau, c.v0, c.sigma, c.cosphi);
     }
-    __device__ static Pos position(const Agent& g) { return make_double2(g.x, g.y); }
+    __device__ static Pos position(const Agent& g) { return {g.x, g.y}; }
 
     static int check(const Params&) { return TB2_OK; }
     static int check_setting(const Setting* s) {
@@ -348,6 +465,9 @@ struct SfSim {
         return TB2_OK;
     }
 };
+
+struct SfSim : SfRollout<double> {};
+struct SfGradSim : SfRollout<Dual> {};
 
 struct OrcaSim {
     using Params = tb2_orca_params;
@@ -444,6 +564,18 @@ struct ScoreSink {
     template <class Pos>
     __device__ void operator()(int sample, Pos pos) {
         const double ex = tr[2 * sample] - (double)pos.x, ey = tr[2 * sample + 1] - (double)pos.y;
+        last = sqrt(ex * ex + ey * ey);
+        sum += last;
+    }
+};
+
+// ScoreSink for a Dual rollout: the same values, and d|truth - position| with them, in sample order.
+struct GradScoreSink {
+    __device__ static bool takes(int a) { return a == 0; }
+    const double* tr;
+    Dual sum = 0.0, last = 0.0;
+    __device__ void operator()(int sample, const Dual2& pos) {
+        const Dual ex = tr[2 * sample] - pos.x, ey = tr[2 * sample + 1] - pos.y;
         last = sqrt(ex * ex + ey * ey);
         sum += last;
     }
@@ -554,6 +686,47 @@ sweep_kernel(const int* __restrict__ scene_off, typename Sim::Inputs in, const t
     }
 }
 
+// The tangent sweep: sweep_kernel<SfGradSim> with GradScoreSink, writing dade / dfde [P, B, 3] (d/d(tau, v0, sigma) of
+// each item's ADE / FDE) beside ade / fde.  Its own kernel rather than an output policy of sweep_kernel, which would
+// change the value kernels' register schedule.  A Dual rollout needs about four times the registers of the double one:
+// the CTA form is bounded at kSfGradMaxScene threads, which ptxas fits in 255 registers without spills.
+constexpr int kSfGradMaxScene = 256;
+
+template <bool kPacked>
+__global__ void __launch_bounds__(kPacked ? 32 * kSweepWarps : kSfGradMaxScene, 1)
+sf_sweep_grad_kernel(const int* __restrict__ scene_off, SfGradSim::Inputs in, const double* __restrict__ params, int P,
+                     const double* __restrict__ truth, int T, double* __restrict__ ade, double* __restrict__ fde,
+                     double* __restrict__ dade, double* __restrict__ dfde, int B, SfGradSim::Params p) {
+    extern __shared__ double smem_classical[];
+    const int n_samples = sample_count<SfGradSim>(p.n_steps, p.sample_every);
+    double* tr = smem_classical;
+    int row0, n;
+    if (!sweep_scene<kPacked>(scene_off, truth, T, n_samples, tr, row0, n)) return;
+    const SweepLane L = sweep_lane<kPacked>(n);
+    const SfGradSim::Scene sc = SfGradSim::scene(tr + 2 * n_samples, kPacked ? threadIdx.x - L.a : 0, L.stride);
+    SfGradSim::Agent g0 = {};
+    if (L.a < n) g0 = SfGradSim::agent(in, row0 + L.a);
+    for (int base = 0; base < P; base += L.nslots) {
+        if (kPacked && base + L.warp_first >= P) break;
+        const int s = base + L.slot;
+        const bool on = L.a < n && s < P;
+        GradScoreSink sink{tr};
+        rollout<SfGradSim, kPacked>(g0, SfGradSim::consts(p, on ? params + (size_t)s * 3 : nullptr), sc, L.a, n, on,
+                                    p.n_steps, p.sample_every, sink);
+        if (on && L.a == 0) {
+            const size_t i = (size_t)s * B + blockIdx.x;
+            const Dual m = sink.sum / (double)n_samples;
+            ade[i] = m.v;
+            fde[i] = sink.last.v;
+#pragma unroll
+            for (int j = 0; j < 3; ++j) {
+                dade[i * 3 + j] = m.d[j];
+                dfde[i * 3 + j] = sink.last.d[j];
+            }
+        }
+    }
+}
+
 }  // namespace tb2
 
 using namespace tb2;
@@ -599,26 +772,26 @@ static int sweep_params_host(const T* params_dev, int P, std::vector<T>& h, cuda
     return TB2_OK;
 }
 
-static int sweep_counts(const tb2_layout* l, int P, int T, int n_samples) {
+static int sweep_counts(const tb2_layout* l, int P, int T, int n_samples, int max_scene) {
     TB2_REQUIRE(l->B >= 1, "no scenes");
     TB2_REQUIRE(P >= 1, "P < 1 settings");
     TB2_REQUIRE((int64_t)P * l->B < ((int64_t)1 << 31), "P x B >= 2^31");
-    TB2_REQUIRE(l->n_max <= 1024, "scene larger than 1024 pedestrians");
+    TB2_REQUIRE(l->n_max <= max_scene, "scene larger than " + std::to_string(max_scene) + " pedestrians");
     TB2_REQUIRE(n_samples >= 1 && n_samples <= 1024, "sample count must be in [1, 1024]");
     TB2_REQUIRE(T >= n_samples, "truth shorter than the sample count");
     return TB2_OK;
 }
 
 // Checks the call, then launches both forms over every scene; each CTA keeps only the scenes of its form (packed:
-// n <= 32, CTA: n > 32).
-template <class Sim>
+// n <= 32, CTA: n > 32).  launch(form, threads, smem) launches the kernel of form std::true_type (packed) or
+// std::false_type (CTA) on B CTAs.
+template <class Sim, class Launch>
 static int sweep_launch(const char* name, const tb2_layout* l, const typename Sim::Params& p,
-                        const typename Sim::Setting* params, int P, typename Sim::Inputs in, const double* truth, int T,
-                        double* ade, double* fde, void* stream) {
+                        const typename Sim::Setting* params, int P, int T, int max_scene, void* stream, Launch launch) {
     int rc = check_rollout<Sim>(p);
     if (rc != TB2_OK) return rc;
     const int n_samples = sample_count<Sim>(p.n_steps, p.sample_every);
-    rc = sweep_counts(l, P, T, n_samples);
+    rc = sweep_counts(l, P, T, n_samples, max_scene);
     if (rc != TB2_OK) return rc;
     cudaStream_t st = (cudaStream_t)stream;
     std::vector<typename Sim::Setting> h;
@@ -631,18 +804,33 @@ static int sweep_launch(const char* name, const tb2_layout* l, const typename Si
     const int64_t want = ((int64_t)P * w_max + 31) / 32;
     const int warps = (int)(want < kSweepWarps ? want : kSweepWarps);
     KernelTimer kt(name, st);
-    sweep_kernel<Sim, true><<<l->B, 32 * warps, truth_bytes + (size_t)32 * warps * Sim::kPedBytes, st>>>(
-        l->scene_off, in, params, P, truth, T, ade, fde, l->B, p);
+    rc = launch(std::true_type(), 32 * warps, truth_bytes + (size_t)32 * warps * Sim::kPedBytes, st);
+    if (rc != TB2_OK) return rc;
+    if (l->n_max > 32)
+        rc = launch(std::false_type(), (l->n_max + 31) / 32 * 32, truth_bytes + (size_t)l->n_max * Sim::kPedBytes, st);
+    return rc;
+}
+
+// One sweep kernel form: dynamic shared memory above 48 KB opted into once per kernel and device.
+template <class Kernel, class... Args>
+static int sweep_form(Kernel kernel, DynSmemConfig& configured, int B, int threads, size_t smem, cudaStream_t st,
+                      Args... args) {
+    TB2_CHECK_CUDA(configured.ensure(kernel, smem, 48 * 1024));
+    kernel<<<B, threads, smem, st>>>(args...);
     TB2_LAUNCH_CHECK();
-    if (l->n_max > 32) {
-        const int threads = (l->n_max + 31) / 32 * 32;
-        const size_t smem = truth_bytes + (size_t)l->n_max * Sim::kPedBytes;
-        static DynSmemConfig configured;
-        TB2_CHECK_CUDA(configured.ensure(sweep_kernel<Sim, false>, smem, 48 * 1024));
-        sweep_kernel<Sim, false><<<l->B, threads, smem, st>>>(l->scene_off, in, params, P, truth, T, ade, fde, l->B, p);
-        TB2_LAUNCH_CHECK();
-    }
     return TB2_OK;
+}
+
+template <class Sim>
+static int sweep_values(const char* name, const tb2_layout* l, const typename Sim::Params& p,
+                        const typename Sim::Setting* params, int P, typename Sim::Inputs in, const double* truth, int T,
+                        double* ade, double* fde, void* stream) {
+    return sweep_launch<Sim>(name, l, p, params, P, T, 1024, stream, [&](auto packed, int threads, size_t smem,
+                                                                            cudaStream_t st) {
+        static DynSmemConfig configured;
+        return sweep_form(sweep_kernel<Sim, decltype(packed)::value>, configured, l->B, threads, smem, st, l->scene_off,
+                          in, params, P, truth, T, ade, fde, l->B, p);
+    });
 }
 
 extern "C" {
@@ -662,14 +850,27 @@ int tb2_orca_simulate(const tb2_layout* l, const tb2_orca_params* p, const float
 int tb2_sf_sweep(const tb2_layout* l, const tb2_sf_params* p, const double* params, int32_t P, const double* state,
                  const double* truth, int32_t truth_len, double* ade_out, double* fde_out, void* stream) {
     TB2_REQUIRE(l && p && params && state && truth && ade_out && fde_out, "null argument");
-    return sweep_launch<SfSim>("sf_sweep", l, *p, params, P, {state}, truth, truth_len, ade_out, fde_out, stream);
+    return sweep_values<SfSim>("sf_sweep", l, *p, params, P, {state}, truth, truth_len, ade_out, fde_out, stream);
+}
+
+int tb2_sf_sweep_grad(const tb2_layout* l, const tb2_sf_params* p, const double* params, int32_t P, const double* state,
+                      const double* truth, int32_t truth_len, double* ade_out, double* fde_out, double* dade_out,
+                      double* dfde_out, void* stream) {
+    TB2_REQUIRE(l && p && params && state && truth && ade_out && fde_out && dade_out && dfde_out, "null argument");
+    return sweep_launch<SfGradSim>("sf_sweep_grad", l, *p, params, P, truth_len, kSfGradMaxScene, stream,
+                                   [&](auto packed, int threads, size_t smem, cudaStream_t st) {
+        static DynSmemConfig configured;
+        return sweep_form(sf_sweep_grad_kernel<decltype(packed)::value>, configured, l->B, threads, smem, st,
+                          l->scene_off, SfGradSim::Inputs{state}, params, P, truth, truth_len, ade_out, fde_out, dade_out,
+                          dfde_out, l->B, *p);
+    });
 }
 
 int tb2_orca_sweep(const tb2_layout* l, const tb2_orca_params* p, const float* params, int32_t P, const float* pos,
                    const float* vel, const double* goal, const double* speed, const double* truth, int32_t truth_len,
                    double* ade_out, double* fde_out, void* stream) {
     TB2_REQUIRE(l && p && params && pos && vel && goal && speed && truth && ade_out && fde_out, "null argument");
-    return sweep_launch<OrcaSim>("orca_sweep", l, *p, params, P, {(const float2*)pos, (const float2*)vel,
+    return sweep_values<OrcaSim>("orca_sweep", l, *p, params, P, {(const float2*)pos, (const float2*)vel,
                                  (const double2*)goal, speed}, truth, truth_len, ade_out, fde_out, stream);
 }
 
