@@ -352,13 +352,16 @@ size_t tb2_lstm_backward_workspace_bytes(const tb2_lstm* model, const tb2_layout
  * training config), and social pooling with a one_layer / two_layer embedding (constant = 0).
  * Social pooling couples all tracks of a scene through the hidden-state scatter (the reference
  * does not detach hidden_states_to_pool, lstm.py:26): the backward then runs on all M rows and
- * active_rows is ignored. */
+ * active_rows is ignored.
+ *   cache_dev        the training cache tb2_lstm_forward_sequence_train filled (social pooling; without it
+ *                    the call returns TB2_ERR_INVALID).  Other models have none: NULL / 0. */
 int tb2_lstm_sequence_backward(const tb2_lstm* model, const tb2_layout* layout, const tb2_lstm_weights* weights,
                                const float* observed_dev, int32_t obs_length, const float* truth_dev,
                                int32_t n_decode, const float* positions_dev, const float* states_dev,
                                const float* d_normals_dev, const int32_t* active_rows_dev, int32_t num_active,
                                const tb2_lstm_grads* grads, void* workspace_dev, size_t workspace_bytes,
-                               void* bwd_workspace_dev, size_t bwd_workspace_bytes, void* stream);
+                               void* bwd_workspace_dev, size_t bwd_workspace_bytes, const void* cache_dev,
+                               size_t cache_bytes, void* stream);
 
 /* TB2_POOL_NN_LSTM / TB2_POOL_TRAJECTRON: zero the interaction-encoder LSTM state kept in `workspace`
  * (NearestNeighborLSTM.reset, non_gridbased_pooling.py:385-389; TrajectronPooling.reset, :481-485).  tb2_lstm_forward_sequence / _steps(first_step = 0) do this themselves; the
@@ -367,24 +370,17 @@ int tb2_lstm_sequence_backward(const tb2_lstm* model, const tb2_layout* layout, 
 int tb2_pool_state_reset(const tb2_lstm* model, const tb2_layout* layout, void* workspace_dev, size_t workspace_bytes,
                          void* stream);
 
-/* Training forward that keeps, per step, what the social backward would otherwise recompute (winners, latent vectors,
- * hidden1 and the pooled vector of the grid embedding; reference: everything autograd saves inside
- * GridBasedPooling.forward, lstm/gridbased_pooling.py:94-170,308-335).  tb2_lstm_train_cache_bytes returns 0 for
- * configurations without a cache (then use tb2_lstm_forward_sequence / tb2_lstm_sequence_backward); `cache` is a
- * caller-owned device buffer that must stay untouched until tb2_lstm_sequence_backward_cached has run. */
+/* Training forward: keeps, per step, the grid-embedding records the social backward reads (winners, latent vectors,
+ * hidden1 and the pooled vector; reference: everything autograd saves inside GridBasedPooling.forward,
+ * lstm/gridbased_pooling.py:94-170,308-335).  tb2_lstm_train_cache_bytes is > 0 for every social model the backward
+ * supports and 0 for the other models, which keep no cache (pass NULL / 0); `cache` is a caller-owned device buffer
+ * that must stay untouched until tb2_lstm_sequence_backward has run. */
 size_t tb2_lstm_train_cache_bytes(const tb2_lstm* model, const tb2_layout* layout, int32_t num_steps);
 int tb2_lstm_forward_sequence_train(const tb2_lstm* model, const tb2_layout* layout, const float* observed_dev,
                                     int32_t obs_length, const float* truth_dev, int32_t n_decode, float* normals_out_dev,
                                     float* positions_out_dev, float* h_dev, float* c_dev, float* states_out_dev,
                                     void* cache_dev, size_t cache_bytes, void* workspace_dev, size_t workspace_bytes,
                                     void* stream);
-int tb2_lstm_sequence_backward_cached(const tb2_lstm* model, const tb2_layout* layout, const tb2_lstm_weights* weights,
-                                      const float* observed_dev, int32_t obs_length, const float* truth_dev,
-                                      int32_t n_decode, const float* positions_dev, const float* states_dev,
-                                      const float* d_normals_dev, const int32_t* active_rows_dev, int32_t num_active,
-                                      const tb2_lstm_grads* grads, void* workspace_dev, size_t workspace_bytes,
-                                      void* bwd_workspace_dev, size_t bwd_workspace_bytes, const void* cache_dev,
-                                      size_t cache_bytes, void* stream);
 
 /* PredictionLoss on the device (lstm/loss.py:52-91, gaussian_2d :24-50): per (frame, scene)
  *   values_out  [T, B]    = -log(0.01 + bg N(x|mu,3,3,0) + (0.99-bg) N(x|mu,s1,s2,rho)) of the primary

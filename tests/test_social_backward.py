@@ -4,8 +4,8 @@ to different kernels, against a float64 autograd restatement (tests/torch_ref.py
 The restatement is pinned on the CPU to gradients of the unmodified reference at tiny shapes
 (tests/golden/social_train_golden.npz, oracle/make_social_train_golden.py).  On the GPU each case runs a
 teacher-forced training step with the tensor cores on and with TB2_DISABLE_TC=1, checks that the step
-took the kernels the case is meant to cover (cached / uncached backward, kernel names from
-tb2_profile_begin / end), and compares the loss and every parameter gradient with the float64
+took the kernels the case is meant to cover (kernel names from tb2_profile_begin / end) with the
+forward's training cache, and compares the loss and every parameter gradient with the float64
 restatement at realistic shapes.
 
 Preconditions, asserted before comparing: the grid embedding's biases are +-3 (random_weights
@@ -73,28 +73,28 @@ def test_torch_restatement_matches_social_reference(social_golden, case):
 TC_KERNELS = {"sparse_layer1_mma", "social_dgrid_mma", "social_dw1_mma", "dense_layer_tc"}
 FFMA_KERNELS = {"sparse_layer1", "social_dgrid", "social_dw1"}
 
-# (id, kind, data, obs_length, pred_length, data seed, weight seed, train cache with the tensor cores on,
-#  kernels the step runs with the tensor cores on).  data: (scenes, max peds, ragged) or a list of scene sizes.
-# With TB2_DISABLE_TC=1 every case runs uncached on FFMA_KERNELS and none of TC_KERNELS.
+# (id, kind, data, obs_length, pred_length, data seed, weight seed, kernels the step runs with the tensor cores on).
+# data: (scenes, max peds, ragged) or a list of scene sizes.
+# With TB2_DISABLE_TC=1 every case runs on FFMA_KERNELS and none of TC_KERNELS.
 GPU_CASES = [
     # the reference trainer's --type social: one_layer, the first Linear writes the gates' operand directly
-    ("reference_default", "social_default", (16, 20, True), 9, 12, 2, 102, True,
+    ("reference_default", "social_default", (16, 20, True), 9, 12, 2, 102,
      {"sparse_layer1_mma", "social_dgrid_mma", "social_dw1_mma", "dense_layer_tc"}),
-    ("latent4", "social_c4", (16, 20, True), 9, 12, 1, 101, True,
+    ("latent4", "social_c4", (16, 20, True), 9, 12, 1, 101,
      {"sparse_layer1", "social_dgrid", "social_dw1", "dense_layer_tc"}),
-    ("latent32", "social_c32", (16, 20, True), 9, 12, 1, 101, True,
+    ("latent32", "social_c32", (16, 20, True), 9, 12, 1, 101,
      {"sparse_layer1", "social_dgrid", "social_dw1", "dense_layer_tc"}),
-    # d1 % 32 == 0 but < 256: a partial 256-column chunk; no wgmma second layer, so uncached + fp32 row GEMMs
-    ("latent16_d96", "social_d96", (16, 20, True), 9, 12, 1, 101, False,
+    # d1 % 32 == 0 but < 256: a partial 256-column chunk; no wgmma second layer, so fp32 records + fp32 row GEMMs
+    ("latent16_d96", "social_d96", (16, 20, True), 9, 12, 1, 101,
      {"sparse_layer1_mma", "social_dgrid_mma", "social_dw1_mma"}),
     # d1 % 32 != 0: FFMA dgrid / dW1 after a tensor-core forward
-    ("latent16_d200", "social_d200", (16, 20, True), 9, 12, 1, 101, False,
+    ("latent16_d200", "social_d200", (16, 20, True), 9, 12, 1, 101,
      {"sparse_layer1_mma", "social_dgrid", "social_dw1"}),
-    ("baseline", "social", (16, 20, False), 9, 12, 3, 103, True,
+    ("baseline", "social", (16, 20, False), 9, 12, 3, 103,
      {"sparse_layer1_mma", "social_dgrid_mma", "social_dw1_mma", "dense_layer_tc"}),
-    ("large_scene", "social", [70, 2, 25], 9, 12, 3, 103, True,
+    ("large_scene", "social", [70, 2, 25], 9, 12, 3, 103,
      {"sparse_layer1_mma", "social_dgrid_mma", "social_dw1_mma", "dense_layer_tc"}),
-    ("short_sequence", "social_default", (16, 20, True), 2, 3, 1, 101, True,
+    ("short_sequence", "social_default", (16, 20, True), 2, 3, 1, 101,
      {"sparse_layer1_mma", "social_dgrid_mma", "social_dw1_mma", "dense_layer_tc"}),
 ]
 
@@ -159,7 +159,7 @@ def _train_step(kind, W, xy, bs, obs_length, pred_length):
 @pytest.mark.parametrize("tc", [True, False], ids=["tc", "no_tc"])
 @pytest.mark.parametrize("case", GPU_CASES, ids=[c[0] for c in GPU_CASES])
 def test_cuda_social_backward_matches_float64_restatement(restated, monkeypatch, case, tc):
-    name, kind, _, obs_length, pred_length, _, _, cached, tc_kernels = case
+    name, kind, _, obs_length, pred_length, _, _, tc_kernels = case
     if not tc:
         monkeypatch.setenv("TB2_DISABLE_TC", "1")     # read when the model's handle is created
     else:
@@ -168,8 +168,8 @@ def test_cuda_social_backward_matches_float64_restatement(restated, monkeypatch,
     xy, bs, W = _case_inputs(case)
     model, loss, kernels, cache_bytes = _train_step(kind, W, xy, bs, obs_length, pred_length)
 
-    # the branch this case exists for
-    assert (cache_bytes > 0) == (cached and tc), (name, cache_bytes)
+    # the branch this case exists for, trained from the forward's cache
+    assert cache_bytes > 0, (name, cache_bytes)
     want = tc_kernels if tc else FFMA_KERNELS
     unwanted = (TC_KERNELS | FFMA_KERNELS) - want
     assert want <= kernels and not (unwanted & kernels), (name, sorted(kernels & (TC_KERNELS | FFMA_KERNELS)))
@@ -197,6 +197,33 @@ def test_cuda_social_backward_matches_float64_restatement(restated, monkeypatch,
         assert (p1.grad is None) == (p2.grad is None), n1
         if p1.grad is not None:
             assert torch.equal(p1.grad, p2.grad), n1
+
+
+@pytest.mark.gpu
+def test_social_backward_without_cache_is_refused(monkeypatch):
+    """The social backward reads its grid-embedding records from the training forward's cache only: a backward
+    handed no cache is refused, naming the call that fills it."""
+    case = GPU_CASES[0]
+    _, kind, _, obs_length, pred_length = case[:5]
+    xy, bs, W = _case_inputs(case)
+    from trajnetplusplusbaselines_b200.lstm import LSTM, GridBasedPooling, PredictionLoss
+    model = LSTM(pool=GridBasedPooling(**O.MODEL_SPECS[kind]))
+    model.load_state_dict({k: torch.from_numpy(v.copy()) for k, v in W.items()})
+    model = model.cuda().train()
+    forward = model._forward_nograd
+
+    def forward_dropping_cache(*args, **kwargs):
+        normals, positions, states, (obs, truth, layout, cache) = forward(*args, **kwargs)
+        assert cache is not None
+        return normals, positions, states, (obs, truth, layout, None)
+    monkeypatch.setattr(model, "_forward_nograd", forward_dropping_cache)
+    scene = torch.from_numpy(xy).cuda()
+    batch_split = torch.from_numpy(bs)
+    rel, _ = model(scene[:obs_length], torch.zeros(xy.shape[1], 2), batch_split, scene[obs_length:-1].clone())
+    targets = scene[obs_length:obs_length + pred_length] - scene[obs_length - 1:obs_length + pred_length - 1]
+    loss = PredictionLoss()(rel[-pred_length:], targets, batch_split)
+    with pytest.raises(RuntimeError, match=r"error -1: .*tb2_lstm_forward_sequence_train"):
+        loss.backward()
 
 
 # ---------------------------------------------------------------------------------------------

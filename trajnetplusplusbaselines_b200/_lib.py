@@ -155,13 +155,10 @@ PROTOTYPES = {
     "tb2_lstm_backward_workspace_bytes": (_sz, [_vp, _vp, _i32, _i32]),
     "tb2_lstm_sequence_backward": (ctypes.c_int, [_vp, _vp, ctypes.POINTER(LstmWeights), _vp, _i32, _vp, _i32,
                                                   _vp, _vp, _vp, _vp, _i32, ctypes.POINTER(LstmGrads),
-                                                  _vp, _sz, _vp, _sz, _vp]),
+                                                  _vp, _sz, _vp, _sz, _vp, _sz, _vp]),
     "tb2_pool_state_reset": (ctypes.c_int, [_vp, _vp, _vp, _sz, _vp]),
     "tb2_lstm_train_cache_bytes": (_sz, [_vp, _vp, _i32]),
     "tb2_lstm_forward_sequence_train": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _sz, _vp]),
-    "tb2_lstm_sequence_backward_cached": (ctypes.c_int, [_vp, _vp, ctypes.POINTER(LstmWeights), _vp, _i32, _vp, _i32,
-                                                         _vp, _vp, _vp, _vp, _i32, ctypes.POINTER(LstmGrads),
-                                                         _vp, _sz, _vp, _sz, _vp, _sz, _vp]),
     "tb2_sgan_add_noise": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp]),
     "tb2_vae_scale_hidden": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp]),
     "tb2_sgan_decoder_context": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),

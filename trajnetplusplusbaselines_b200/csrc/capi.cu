@@ -95,10 +95,8 @@ size_t carve_workspace(const tb2_lstm* m, const tb2_layout* l, void* base, Works
 }
 
 size_t carve_train_cache(const tb2_lstm* m, const tb2_layout* l, size_t S, void* base, TrainCache* out) {
+    if (!social_trainable(m)) return 0;
     const bool two = m->n_mlp == 2;
-    if (m->cfg.pool_type != TB2_POOL_SOCIAL || m->Wg_hi[0] == nullptr || m->n_mlp < 1 || m->n_mlp > 2 || !m->cfg.pool_to_input ||
-        (two && m->W_hi[1] == nullptr))
-        return 0;
     const size_t M = (size_t)l->M, C = (size_t)m->C, nm1 = (size_t)(l->n_max > 1 ? l->n_max - 1 : 1);
     const size_t d1 = (size_t)m->mlp_dims[1], P = (size_t)m->P;
     size_t off = 0;
@@ -113,10 +111,10 @@ size_t carve_train_cache(const tb2_lstm* m, const tb2_layout* l, size_t S, void*
     c.win_ent = (uint32_t*)take(S * M * nm1 * sizeof(uint32_t));
     c.pair_cell = (int*)take(S * M * nm1 * sizeof(int));
     c.pair_flag = (uint8_t*)take(S * M * nm1);
-    c.h1_hi = two ? take(S * M * d1 * 2) : nullptr;
-    c.h1_lo = two ? take(S * M * d1 * 2) : nullptr;
-    c.pool_hi = take(S * M * P * 2);
-    c.pool_lo = take(S * M * P * 2);
+    c.h1_step = two ? 2 * align_up(M * d1 * 2, 256) : 0;      // 4 bytes per element: fp32, or bf16 hi + lo
+    c.pooled_step = 2 * align_up(M * P * 2, 256);
+    c.h1 = two ? (char*)take(S * c.h1_step) : nullptr;
+    c.pooled = (char*)take(S * c.pooled_step);
     if (out) *out = c;
     return off;
 }
@@ -184,7 +182,7 @@ using namespace tb2;
 extern "C" {
 
 const char* tb2_last_error(void) { return g_error.c_str(); }
-int tb2_version(void) { return 101; }
+int tb2_version(void) { return 102; }
 uint64_t tb2_launch_count(void) { return g_launch_count.load(); }
 
 int tb2_profile_begin(void) {
@@ -684,17 +682,24 @@ static int forward_steps_impl(const tb2_lstm* m, const tb2_layout* l, const floa
         Workspace wstep = ws;
         if (cache) {        // this step's winners, latent vectors, hidden1 and pooled vector stay where the backward reads them
             const size_t nm1 = (size_t)(l->n_max > 1 ? l->n_max - 1 : 1), us = (size_t)s;
+            const PoolFormats f = pool_formats(m);
             wstep.lat = cache->lat + us * M * m->C;
             wstep.win_count = cache->win_count + us * M;
             wstep.win_ent = cache->win_ent + us * M * nm1;
             wstep.pair_cell = cache->pair_cell + us * M * nm1;
             wstep.pair_flag = cache->pair_flag + us * M * nm1;
-            if (cache->h1_hi) {
-                wstep.act[0] = (float*)((char*)cache->h1_hi + us * M * (size_t)m->mlp_dims[1] * 2);
-                wstep.act[1] = (float*)((char*)cache->h1_lo + us * M * (size_t)m->mlp_dims[1] * 2);
+            if (cache->h1) {
+                char* h1 = cache->h1 + us * cache->h1_step;
+                wstep.act[0] = (float*)h1;
+                if (f.h1_pair) wstep.act[1] = (float*)(h1 + cache->h1_step / 2);
             }
-            wstep.pool_hi = (char*)cache->pool_hi + us * M * (size_t)m->P * 2;
-            wstep.pool_lo = (char*)cache->pool_lo + us * M * (size_t)m->P * 2;
+            char* pooled = cache->pooled + us * cache->pooled_step;
+            if (f.pooled_pair) {
+                wstep.pool_hi = pooled;
+                wstep.pool_lo = pooled + cache->pooled_step / 2;
+            } else {
+                wstep.pooled = (float*)pooled;
+            }
             wstep.write_pairs = 1;
         }
         if ((rc = step_impl(m, l, phase, o1, o2, goals, h_prev, c_prev, h_next, c_next,

@@ -220,21 +220,41 @@ struct Workspace {
     float* scene_sum;      // [B, 4] TrajectronPooling: sum of (pos, vel) over the visible tracks of every scene
 };
 
-// Per-step forward quantities a training forward keeps for the social backward (tb2_lstm_forward_sequence_train):
-// the backward then skips its own pool_prepare / grid-embedding recomputation.  Layouts match the backward's
-// own per-step arrays ([S][M][...]).
+// How a forward step hands on hidden1 (the grid embedding's first Linear output, read by the second Linear) and the
+// pooled vector (read by the gate kernel): as a bf16 (hi, lo) pair only where the producing kernel writes the pair
+// itself, as fp32 wherever an fp32 tensor is made (also when that fp32 tensor is split afterwards).  hidden1 is a pair
+// for the wgmma second Linear; the pooled vector is a pair when the tensor-core gates read it from a last layer that
+// writes the split (the first Linear, or the wgmma second Linear).  The training cache keeps both in this format.
+struct PoolFormats {
+    bool h1_pair;
+    bool pooled_pair;
+};
+inline PoolFormats pool_formats(const tb2_lstm* m) {
+    const bool tc2 = m->n_mlp >= 2 && m->W_hi[1] != nullptr;
+    return {tc2, m->Wg_hi[0] != nullptr && (m->n_mlp == 1 || (m->n_mlp == 2 && tc2))};
+}
+
+// The social models the training backward supports; exactly these keep a training cache
+inline bool social_trainable(const tb2_lstm* m) {
+    return m->cfg.pool_type == TB2_POOL_SOCIAL && m->n_mlp >= 1 && m->n_mlp <= 2 && m->cfg.pool_to_input &&
+           m->cfg.constant == 0.f && m->G == 0;
+}
+
+// Per-step forward quantities the training forward (tb2_lstm_forward_sequence_train) keeps for the social backward,
+// which reads its grid-embedding records from here only.  Step s of hidden1 / the pooled vector is a slot of
+// h1_step / pooled_step bytes at h1 / pooled + s * step: fp32 [M][n], or bf16 hi [M][n] followed by lo [M][n] at
+// step / 2 (pool_formats).  Every slot and half is 256-byte aligned, like the workspace buffers it stands in for.
 struct TrainCache {
     float* lat;            // [S][M][C]
     int* win_count;        // [S][M]
     uint32_t* win_ent;     // [S][M][nm1]
     int* pair_cell;        // [S][M][nm1]
     uint8_t* pair_flag;    // [S][M * nm1]
-    void* h1_hi;           // [S][M][d1] bf16 (two_layer) or null
-    void* h1_lo;
-    void* pool_hi;         // [S][M][P] bf16
-    void* pool_lo;
+    char* h1;              // two_layer: [S] slots of [M][d1]; null otherwise
+    char* pooled;          // [S] slots of [M][P]
+    size_t h1_step, pooled_step;
 };
-// 0 when the configuration keeps no cache (anything but social pooling on the tensor-core path)
+// 0 for models without a cache (all but social_trainable ones)
 size_t carve_train_cache(const tb2_lstm* m, const tb2_layout* l, size_t S, void* base, TrainCache* out);
 size_t carve_workspace(const tb2_lstm* m, const tb2_layout* l, void* base, Workspace* ws);
 

@@ -1181,9 +1181,8 @@ int launch_pool_mlp(const tb2_lstm* m, const tb2_layout* l, Workspace* ws, float
     const int nm1 = l->n_max > 1 ? l->n_max - 1 : 1;
     // producers that cannot write the bf16 split themselves go through fp32 scratch + launch_split_bf16
     const bool want_split = pool_hi != nullptr;
-    const bool last_is_l1 = m->n_mlp == 1;
-    const bool last_is_tc = m->n_mlp == 2 && m->W_hi[1] != nullptr;
-    const bool direct_split = want_split && (last_is_l1 || last_is_tc);
+    const PoolFormats formats = pool_formats(m);
+    const bool direct_split = want_split && formats.pooled_pair;
     if (want_split && !direct_split && pooled_out == nullptr) pooled_out = ws->pooled;
     int rc_all = TB2_OK;
     if (m->n_mlp == 0) {
@@ -1226,11 +1225,11 @@ int launch_pool_mlp(const tb2_lstm* m, const tb2_layout* l, Workspace* ws, float
     p.constant = m->cfg.constant;
     float* l1_out = (m->n_mlp == 1) ? pooled_out : ws->act[0];
     // second Linear on the tensor cores: layer 1 hands its activations over as bf16 (hi, lo)
-    const bool tc2 = m->n_mlp >= 2 && m->W_hi[1] != nullptr;
+    const bool tc2 = formats.h1_pair;
     p.out = tc2 ? nullptr : l1_out;
     p.out_hi = tc2 ? reinterpret_cast<__nv_bfloat16*>(ws->act[0]) : nullptr;
     p.out_lo = tc2 ? reinterpret_cast<__nv_bfloat16*>(ws->act[1]) : nullptr;
-    if (last_is_l1 && direct_split) {      // one_layer embedding feeding the tensor-core gates
+    if (m->n_mlp == 1 && direct_split) {      // one_layer embedding feeding the tensor-core gates
         p.out = pooled_out;                // may be null
         p.out_hi = reinterpret_cast<__nv_bfloat16*>(pool_hi);
         p.out_lo = reinterpret_cast<__nv_bfloat16*>(pool_lo);

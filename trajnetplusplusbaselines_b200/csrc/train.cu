@@ -18,7 +18,7 @@
 //       fixed order.  No floating-point atomics: results are bit-identical from run to run.
 // Social pooling couples the tracks of a scene through lat_j = W_enc h_j: every track receives
 // gradient, so social_backward (further down) runs on all M rows, with its own (A) (this step's
-// forward records, from the training cache or recomputed) and its own (C), which adds the
+// forward records, from the training cache) and its own (C), which adds the
 // backward of the grid MLP and of the hidden-state scatter to the chain.  Both drivers keep the
 // same per-(step, row) records (RowRecords) and share phase (B) (gate_preactivations) and the
 // LSTM / head / input-embedding weight gradients (lstm_weight_grads).
@@ -934,7 +934,7 @@ __global__ void untranspose_add_kernel(const float* __restrict__ dWt1, float* __
     }
 }
 
-// hidden1 of a step as fp32: from the bf16 (hi, lo) pair the tensor-core layer consumed, or a copy
+// a forward record (hidden1 or the pooled vector of a step) as fp32: from the bf16 (hi, lo) pair, or a copy
 __global__ void merge_split_kernel(const __nv_bfloat16* __restrict__ hi, const __nv_bfloat16* __restrict__ lo,
                                    const float* __restrict__ src, float* __restrict__ dst, size_t n) {
     for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x)
@@ -1210,11 +1210,9 @@ static int split2d(const float* src, int ld_src, size_t rows, int cols, __nv_bfl
 }
 
 struct SocBuffers : RowRecords {
-    float *H1, *DH1, *LAT, *DLAT, *DGRID, *dWt1, *zero_h;
-    int *rows, *winc, *counts, *base, *start, *pcell;
+    float *H1, *DH1, *DLAT, *DGRID, *dWt1;
+    int *rows, *counts, *base, *start;
     unsigned* sorted;
-    uint8_t* pflag;
-    uint32_t* wine;
     __nv_bfloat16 *Wt1_hi, *Wt1_lo;                       // bf16 split of the cell-major first-layer weights (dgrid on mma.sync)
     // 3-pass wgmma versions of the row GEMMs (dense_layer_tc_kernel): bf16 (hi, lo) operands
     __nv_bfloat16 *X_hi, *X_lo;                           // [S][M][K]
@@ -1238,17 +1236,11 @@ static size_t carve_social(const tb2_lstm* m, const tb2_layout* l, size_t S, voi
     carve_records(m, M, S, P * d1, c, o);
     o->H1 = c.take(m->n_mlp == 2 ? S * M * d1 : 4);
     o->DH1 = c.take(M * (d1 > H ? d1 : H));     // also holds the [M,H] recurrent d h of a step
-    o->LAT = c.take(S * M * C);
     o->DLAT = c.take(S * M * C);
     o->DGRID = c.take(M * nm1 * C);
     o->dWt1 = c.take(cells * C * d1);
-    o->zero_h = c.take(M * H);
     o->rows = reinterpret_cast<int*>(c.take(M));
-    o->winc = reinterpret_cast<int*>(c.take(S * M));
-    o->wine = reinterpret_cast<uint32_t*>(c.take(S * M * nm1));
     o->sorted = reinterpret_cast<unsigned*>(c.take(M * nm1));
-    o->pcell = reinterpret_cast<int*>(c.take(S * M * nm1));
-    o->pflag = reinterpret_cast<uint8_t*>(c.take((S * M * nm1 + 3) / 4));
     o->counts = reinterpret_cast<int*>(c.take((size_t)l->B * cells));
     o->base = reinterpret_cast<int*>(c.take((size_t)l->B * cells));
     o->start = reinterpret_cast<int*>(c.take(cells + 1));
@@ -1363,44 +1355,23 @@ static int social_pair_kernels(const tb2_lstm* m, const tb2_layout* l, const Soc
     return TB2_OK;
 }
 
-// (A) this step's forward records: winners and pair tables, latent vectors (b.LAT), hidden1 (b.H1, two_layer) and the
-// pooled vector (ws.pooled).  With a training cache the forward kept them; otherwise they are recomputed from h_prev.
+// (A) this step's hidden1 (b.H1, two_layer) and pooled vector (ws.pooled) as fp32, from the training cache: hi + lo
+// where the forward kept the bf16 pair, a copy where it kept fp32 (pool_formats)
 static int social_step_records(const tb2_lstm* m, const tb2_layout* l, const SocBuffers& b, const Workspace& ws,
-                               const TrainCache* cache, int s, const float* h_prev, const float* o1, const float* o2,
-                               cudaStream_t st) {
-    const size_t M = (size_t)l->M, P = (size_t)m->P, d1 = (size_t)m->mlp_dims[1], C = (size_t)m->C;
-    const size_t nm1 = (size_t)(l->n_max > 1 ? l->n_max - 1 : 1);
-    const bool two = m->n_mlp == 2;
-    float* H1 = b.H1 + (size_t)s * M * d1;
-    if (cache) {
-        // hidden1 and the pooled vector of the forward, as fp32 (hi + lo of the bf16 pair the next kernel consumed)
-        if (two) {
-            merge_split_kernel<<<1024, 256, 0, st>>>((const __nv_bfloat16*)cache->h1_hi + (size_t)s * M * d1,
-                                                     (const __nv_bfloat16*)cache->h1_lo + (size_t)s * M * d1, nullptr,
-                                                     H1, M * d1);
-            TB2_LAUNCH_CHECK();
-        }
-        merge_split_kernel<<<512, 256, 0, st>>>((const __nv_bfloat16*)cache->pool_hi + (size_t)s * M * P,
-                                                (const __nv_bfloat16*)cache->pool_lo + (size_t)s * M * P, nullptr, ws.pooled,
-                                                M * P);
-        TB2_LAUNCH_CHECK();
-        return TB2_OK;
-    }
-    Workspace w2 = ws;
-    w2.lat = b.LAT + (size_t)s * M * C;
-    w2.win_count = b.winc + (size_t)s * M;
-    w2.win_ent = b.wine + (size_t)s * M * nm1;
-    w2.pair_cell = b.pcell + (size_t)s * M * nm1;
-    w2.pair_flag = b.pflag + (size_t)s * M * nm1;
-    int rc;
-    if ((rc = launch_pool_prepare(m, l, h_prev ? h_prev : b.zero_h, o1, o2, 1, 1, 0, &w2, st))) return rc;
-    if ((rc = launch_pool_mlp(m, l, &w2, ws.pooled, nullptr, nullptr, st))) return rc;
-    if (two) {      // a tensor-core second Linear read hidden1 as the bf16 (hi, lo) pair in act[0] / act[1]
-        const bool tc2 = m->W_hi[1] != nullptr;
-        merge_split_kernel<<<1024, 256, 0, st>>>(tc2 ? (const __nv_bfloat16*)ws.act[0] : nullptr,
-                                                 tc2 ? (const __nv_bfloat16*)ws.act[1] : nullptr, ws.act[0], H1, M * d1);
+                               const TrainCache& cache, int s, cudaStream_t st) {
+    const size_t M = (size_t)l->M, P = (size_t)m->P, d1 = (size_t)m->mlp_dims[1];
+    const PoolFormats f = pool_formats(m);
+    auto merge = [&](const char* slot, size_t step, bool pair, float* dst, size_t n, int blocks) {
+        const __nv_bfloat16* hi = pair ? (const __nv_bfloat16*)slot : nullptr;
+        const __nv_bfloat16* lo = pair ? (const __nv_bfloat16*)(slot + step / 2) : nullptr;
+        merge_split_kernel<<<blocks, 256, 0, st>>>(hi, lo, pair ? nullptr : (const float*)slot, dst, n);
+    };
+    if (m->n_mlp == 2) {
+        merge(cache.h1 + (size_t)s * cache.h1_step, cache.h1_step, f.h1_pair, b.H1 + (size_t)s * M * d1, M * d1, 1024);
         TB2_LAUNCH_CHECK();
     }
+    merge(cache.pooled + (size_t)s * cache.pooled_step, cache.pooled_step, f.pooled_pair, ws.pooled, M * P, 512);
+    TB2_LAUNCH_CHECK();
     return TB2_OK;
 }
 
@@ -1409,8 +1380,8 @@ static int social_step_records(const tb2_lstm* m, const tb2_layout* l, const Soc
 static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lstm_weights* w,
                            const float* observed, int obs_length, const float* truth, int n_decode,
                            const float* positions, const float* states, const float* d_normals,
-                           const tb2_lstm_grads* g, Workspace& ws, void* bwd_workspace, cudaStream_t st,
-                           const TrainCache* cache = nullptr) {
+                           const tb2_lstm_grads* g, Workspace& ws, void* bwd_workspace, const TrainCache& cache,
+                           cudaStream_t st) {
     const int S = obs_length - 1 + n_decode, S_enc = obs_length - 1;
     const int Mi = l->M, K = m->K_gate, E = m->E, P = m->P, EP = E + P, C = m->C, cells = m->cells;
     const int H = m->H, G4 = 4 * H;
@@ -1423,27 +1394,19 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
                 "social backward needs gradient buffers for pool.hidden_dim_encoding and pool.embedding");
     SocBuffers b;
     carve_social(m, l, (size_t)S, bwd_workspace, &b);
-    if (cache) {      // the forward kept its per-step winners / latent vectors: same [S][M][...] layouts
-        b.LAT = cache->lat;
-        b.winc = cache->win_count;
-        b.wine = cache->win_ent;
-        b.pcell = cache->pair_cell;
-        b.pflag = cache->pair_flag;
-    }
     TB2_CHECK_CUDA(cudaMemsetAsync(b.dc, 0, M * H * sizeof(float), st));
     TB2_CHECK_CUDA(cudaMemsetAsync(b.dWt1, 0, (size_t)cells * C * d1 * sizeof(float), st));
-    TB2_CHECK_CUDA(cudaMemsetAsync(b.zero_h, 0, M * H * sizeof(float), st));      // state before step 0
     iota_kernel<<<(Mi + 255) / 256, 256, 0, st>>>(b.rows, Mi);
     TB2_LAUNCH_CHECK();
     int rc;
     if ((rc = launch_split_bf16(m->Wt1, b.Wt1_hi, b.Wt1_lo, (size_t)cells * C * d1, st))) return rc;
-    // (A) forward quantities of every step: winners + lat, hidden1, X = [emb | pooled | h_prev]
+    // (A) forward quantities of every step: hidden1, X = [emb | pooled | h_prev]
     for (int s = 0; s < S; ++s) {
         const float *o1, *o2;
         int phase;
         if ((rc = resolve_step_inputs(l, observed, obs_length, truth, positions, s, &ws, &o1, &o2, &phase, st))) return rc;
         const float* h_prev = s > 0 ? states + ((size_t)(s - 1) * 2 + 0) * M * H : nullptr;
-        if ((rc = social_step_records(m, l, b, ws, cache, s, h_prev, o1, o2, st))) return rc;
+        if ((rc = social_step_records(m, l, b, ws, cache, s, st))) return rc;
         {
             KernelTimer kt("bwd_gather", st);
             bwd_gather_kernel<<<Mi, 256, 0, st>>>(b.rows, Mi, (const float2*)o1, (const float2*)o2, m->We, m->be,
@@ -1543,12 +1506,12 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
             TB2_LAUNCH_CHECK();
         }
         if ((rc = colsum(b.DH1, d1, Mi, d1, g->pool_embedding_bias0, nullptr, b.scratch, b.scratch_floats, st))) return rc;
-        const int* winc = b.winc + (size_t)s * M;
-        const uint32_t* wine = b.wine + (size_t)s * M * nm1;
-        const int* pcell = b.pcell + (size_t)s * M * nm1;
-        const uint8_t* pflag = b.pflag + (size_t)s * M * nm1;
+        const int* winc = cache.win_count + (size_t)s * M;
+        const uint32_t* wine = cache.win_ent + (size_t)s * M * nm1;
+        const int* pcell = cache.pair_cell + (size_t)s * M * nm1;
+        const uint8_t* pflag = cache.pair_flag + (size_t)s * M * nm1;
         const int* msk = b.masked + (size_t)s * M;
-        const float* lat = b.LAT + (size_t)s * M * C;
+        const float* lat = cache.lat + (size_t)s * M * C;
         {
             KernelTimer kt("social_pair_sort", st);
             pair_count_kernel<<<l->B, 256, cells * sizeof(int), st>>>(l->scene_off, msk, pcell, pflag, nm1, cells,
@@ -1606,40 +1569,12 @@ size_t tb2_lstm_backward_workspace_bytes(const tb2_lstm* m, const tb2_layout* l,
                      nullptr, nullptr);
 }
 
-static int sequence_backward_impl(const tb2_lstm* m, const tb2_layout* l, const tb2_lstm_weights* w,
-                               const float* observed, int32_t obs_length, const float* truth, int32_t n_decode,
-                               const float* positions, const float* states, const float* d_normals,
-                               const int32_t* active_rows, int32_t num_active, const tb2_lstm_grads* g,
-                               void* workspace, size_t workspace_bytes, void* bwd_workspace,
-                               size_t bwd_workspace_bytes, void* stream, const void* cache, size_t cache_bytes);
-
 int tb2_lstm_sequence_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lstm_weights* w,
                                const float* observed, int32_t obs_length, const float* truth, int32_t n_decode,
                                const float* positions, const float* states, const float* d_normals,
                                const int32_t* active_rows, int32_t num_active, const tb2_lstm_grads* g,
                                void* workspace, size_t workspace_bytes, void* bwd_workspace,
-                               size_t bwd_workspace_bytes, void* stream) {
-    return sequence_backward_impl(m, l, w, observed, obs_length, truth, n_decode, positions, states, d_normals, active_rows,
-                                  num_active, g, workspace, workspace_bytes, bwd_workspace, bwd_workspace_bytes, stream, nullptr, 0);
-}
-
-int tb2_lstm_sequence_backward_cached(const tb2_lstm* m, const tb2_layout* l, const tb2_lstm_weights* w,
-                                      const float* observed, int32_t obs_length, const float* truth, int32_t n_decode,
-                                      const float* positions, const float* states, const float* d_normals,
-                                      const int32_t* active_rows, int32_t num_active, const tb2_lstm_grads* g,
-                                      void* workspace, size_t workspace_bytes, void* bwd_workspace,
-                                      size_t bwd_workspace_bytes, const void* cache, size_t cache_bytes, void* stream) {
-    return sequence_backward_impl(m, l, w, observed, obs_length, truth, n_decode, positions, states, d_normals, active_rows,
-                                  num_active, g, workspace, workspace_bytes, bwd_workspace, bwd_workspace_bytes, stream, cache,
-                                  cache_bytes);
-}
-
-static int sequence_backward_impl(const tb2_lstm* m, const tb2_layout* l, const tb2_lstm_weights* w,
-                               const float* observed, int32_t obs_length, const float* truth, int32_t n_decode,
-                               const float* positions, const float* states, const float* d_normals,
-                               const int32_t* active_rows, int32_t num_active, const tb2_lstm_grads* g,
-                               void* workspace, size_t workspace_bytes, void* bwd_workspace,
-                               size_t bwd_workspace_bytes, void* stream, const void* cache, size_t cache_bytes) {
+                               size_t bwd_workspace_bytes, const void* cache, size_t cache_bytes, void* stream) {
     TB2_REQUIRE(m && l && w && g, "null handle");
     TB2_REQUIRE(m->weights_set, "tb2_lstm_set_weights has not been called");
     TB2_REQUIRE(observed && positions && states && d_normals && active_rows, "null argument");
@@ -1649,7 +1584,7 @@ static int sequence_backward_impl(const tb2_lstm* m, const tb2_layout* l, const 
         return TB2_ERR_UNSUPPORTED;
     }
     const bool social = m->cfg.pool_type == TB2_POOL_SOCIAL;
-    if (social && (m->n_mlp < 1 || m->n_mlp > 2 || !m->cfg.pool_to_input || m->cfg.constant != 0.f)) {
+    if (social && !social_trainable(m)) {
         set_error("social training backward supports one_layer / two_layer embeddings with constant = 0");
         return TB2_ERR_UNSUPPORTED;
     }
@@ -1662,17 +1597,17 @@ static int sequence_backward_impl(const tb2_lstm* m, const tb2_layout* l, const 
     TB2_REQUIRE(workspace && workspace_bytes >= carve_workspace(m, l, nullptr, nullptr), "workspace too small");
     TB2_REQUIRE(bwd_workspace && bwd_workspace_bytes >= tb2_lstm_backward_workspace_bytes(m, l, num_active, S),
                 "backward workspace too small");
+    TrainCache tc;
+    const size_t cache_need = carve_train_cache(m, l, (size_t)S, const_cast<void*>(cache), &tc);
+    TB2_REQUIRE(!social || cache, "a social model trains from the cache its tb2_lstm_forward_sequence_train call filled");
+    TB2_REQUIRE(cache_bytes >= cache_need, "training cache too small (tb2_lstm_train_cache_bytes)");
     if (num_active == 0) return TB2_OK;
     cudaStream_t st = (cudaStream_t)stream;
     Workspace ws;
     carve_workspace(m, l, workspace, &ws);
-    if (social) {    // every track of a scene receives gradient: all rows, active_rows is ignored
-        TrainCache tc;
-        const size_t need = cache ? carve_train_cache(m, l, (size_t)S, const_cast<void*>(cache), &tc) : 0;
-        TB2_REQUIRE(!cache || (need > 0 && cache_bytes >= need), "training cache too small (tb2_lstm_train_cache_bytes)");
+    if (social)      // every track of a scene receives gradient: all rows, active_rows is ignored
         return social_backward(m, l, w, observed, obs_length, truth, n_decode, positions, states, d_normals, g, ws,
-                               bwd_workspace, st, cache ? &tc : nullptr);
-    }
+                               bwd_workspace, tc, st);
     const int R = num_active, K = m->K_gate, E = m->E, P = m->P, EP = E + P, H = m->H, G4 = 4 * H;
     const size_t M = (size_t)l->M;
     BwdBuffers b;

@@ -344,7 +344,7 @@ class ModelHandle:
     def forward_sequence_train(self, layout, observed, truth, n_decode, normals, positions, h, c, states, cache):
         """tb2_lstm_forward_sequence_train: the per-step states go to `states` [S, 2, M, H]; per-step forward
         quantities of the social pooling stay in `cache` (uint8 device tensor of train_cache_bytes, None when that is
-        0) for tb2_lstm_sequence_backward_cached."""
+        0) for tb2_lstm_sequence_backward."""
         lib = _lib.load()
         ws, need = self.workspace(layout)
         with torch.cuda.device(self.device):

@@ -271,7 +271,7 @@ class LSTM(torch.nn.Module):
         inputs = (layout, seq.obs, seq.truth, seq.n_decode, seq.normals, seq.positions, seq.h, seq.c)
         if want_states:
             # training forward: the outputs stay on the device; the per-step states are kept for the backward, and
-            # so is what the social backward would otherwise recompute (0 bytes: no cache)
+            # so are the grid-embedding records the social backward reads (0 bytes: not a social model, no cache)
             states = torch.empty((seq.S, 2, layout.num_tracks, self.hidden_dim), dtype=torch.float32, device=device)
             cache_bytes = handle.train_cache_bytes(layout, seq.S)
             cache = torch.empty(cache_bytes, dtype=torch.uint8, device=device) if cache_bytes > 0 else None

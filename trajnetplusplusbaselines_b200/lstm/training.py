@@ -1,7 +1,7 @@
 """Autograd bridge for training: LSTM.forward under grad mode.
 
 The forward is the same fused CUDA time loop as inference (with the per-step states kept);
-the backward is tb2_lstm_sequence_backward_cached (csrc/train.cu): BPTT restricted to the tracks that
+the backward is tb2_lstm_sequence_backward (csrc/train.cu): BPTT restricted to the tracks that
 actually receive gradient (all tracks for social pooling, whose hidden-state scatter couples the
 tracks of a scene).  Mirrors what autograd computes for the reference's
 Trainer.train_batch (trajnetbaselines/lstm/trainer.py:229-269).
@@ -108,9 +108,9 @@ class _SequenceFn(torch.autograd.Function):
             bws = torch.empty(bneed, dtype=torch.uint8, device=device)
             pos_steps = positions[-S:].contiguous()
             n_decode = S - (int(ctx.obs.shape[0]) - 1)
-            cache_bytes = 0 if ctx.cache is None else int(ctx.cache.numel())      # no cache: the backward recomputes
+            cache_bytes = 0 if ctx.cache is None else int(ctx.cache.numel())      # no cache: not a social model
             with torch.cuda.device(device):
-                _lib.check(lib.tb2_lstm_sequence_backward_cached(
+                _lib.check(lib.tb2_lstm_sequence_backward(
                     handle.handle, layout.handle, ctypes.byref(w), _ptr(ctx.obs), int(ctx.obs.shape[0]),
                     _ptr(ctx.truth), n_decode, _ptr(pos_steps), _ptr(ctx.states), _ptr(dn), _ptr(active), R,
                     ctypes.byref(g), _ptr(ws), need, _ptr(bws), bneed, _ptr(ctx.cache), cache_bytes, _stream(device)))
