@@ -278,6 +278,28 @@ int tb2_lstm_forward_sequence_host_goals(tb2_lstm* model, const tb2_layout* layo
                                          float* normals_host, float* positions_host,
                                          void* stream, void* copy_stream);
 
+/* Sampled forward (no reference counterpart: the reference feeds back the mean of every step's bivariate normal,
+ * lstm/lstm.py:232,255).  tb2_lstm_forward_steps, and after every step s >= obs_length - 2 of the range (the last
+ * encoder step's output and every decoder step: the n_decode + 1 predicted positions) the step's position is replaced
+ * by a draw of its normal before anything reads it, so the draw is what the following steps are fed back:
+ *   pos[s, m] += (sx e1, sy (rho e1 + sqrt(1 - rho^2) e2)),   (sx, sy, rho) = normals[s, m, 2:5],
+ *   (e1, e2) = eps_dev[s - (obs_length - 2), m]
+ * eps_dev [n_decode + 1, M, 2] holds standard normal pairs aligned with the last n_decode + 1 steps.  A pair of exactly
+ * (0, 0) leaves the position bit-unchanged (all zeros: the bits of tb2_lstm_forward_steps); rows with NaN normals stay
+ * NaN.  NULL eps_dev returns TB2_ERR_INVALID, a goal-conditioned model TB2_ERR_UNSUPPORTED. */
+int tb2_lstm_forward_steps_sampled(const tb2_lstm* model, const tb2_layout* layout,
+                                   const float* observed_dev, int32_t obs_length,
+                                   const float* truth_dev, int32_t n_decode, int32_t first_step, int32_t last_step,
+                                   const float* eps_dev, float* normals_out_dev, float* positions_out_dev,
+                                   float* h_dev, float* c_dev, float* states_out_dev,
+                                   void* workspace_dev, size_t workspace_bytes, void* stream);
+
+/* The sampling of tb2_lstm_forward_steps_sampled on one step's rows: positions [rows, 2] += the offset above from
+ * normals [rows, 5] and eps [rows, 2], in place.  The batched multi-mode decode applies it to the replicated output of
+ * the last encoder step before the decoder steps run. */
+int tb2_lstm_sample_positions(const float* normals_dev, float* positions_dev, const float* eps_dev, int32_t rows,
+                              void* stream);
+
 /* LSTMGenerator.adding_noise (sgan/sgan.py:200-221), in place on the hidden state of all tracks:
  *   h[m] <- cat(ReLU(weight . h[m] + bias), noise)   weight [H - noise_dim, H] (mlp_decoder_context.0),
  * noise [noise_dim] is one vector shared by all tracks.  Called between the encoder steps and the

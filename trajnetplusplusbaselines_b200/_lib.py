@@ -152,6 +152,9 @@ PROTOTYPES = {
                                                     _vp, _sz, _vp]),
     "tb2_lstm_forward_sequence_host_goals": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp,
                                                             _sz, _vp, _vp, _vp, _vp]),
+    "tb2_lstm_forward_steps_sampled": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp,
+                                                      _vp, _vp, _sz, _vp]),
+    "tb2_lstm_sample_positions": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp]),
     "tb2_lstm_backward_workspace_bytes": (_sz, [_vp, _vp, _i32, _i32]),
     "tb2_lstm_sequence_backward": (ctypes.c_int, [_vp, _vp, ctypes.POINTER(LstmWeights), _vp, _i32, _vp, _i32,
                                                   _vp, _vp, _vp, _vp, _i32, ctypes.POINTER(LstmGrads),

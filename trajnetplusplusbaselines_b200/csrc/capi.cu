@@ -182,7 +182,7 @@ using namespace tb2;
 extern "C" {
 
 const char* tb2_last_error(void) { return g_error.c_str(); }
-int tb2_version(void) { return 102; }
+int tb2_version(void) { return 103; }
 uint64_t tb2_launch_count(void) { return g_launch_count.load(); }
 
 int tb2_profile_begin(void) {
@@ -642,7 +642,7 @@ static int forward_steps_impl(const tb2_lstm* m, const tb2_layout* l, const floa
                               int32_t obs_length, const float* truth, int32_t n_decode, const float* goals,
                               int32_t first_step, int32_t last_step, float* normals_out, float* positions_out, float* h,
                               float* c, float* states_out, void* workspace, size_t workspace_bytes, void* stream,
-                              const HostSink* sink, const TrainCache* cache = nullptr) {
+                              const HostSink* sink, const TrainCache* cache = nullptr, const float* eps = nullptr) {
     int rc = check_ready(m, l, workspace, workspace_bytes);
     if (rc) return rc;
     if ((rc = resolve_goals(m, &goals))) return rc;
@@ -705,6 +705,11 @@ static int forward_steps_impl(const tb2_lstm* m, const tb2_layout* l, const floa
         if ((rc = step_impl(m, l, phase, o1, o2, goals, h_prev, c_prev, h_next, c_next,
                             normals_out + (size_t)s * M * 5, positions_out + (size_t)s * frame, &wstep, s & 1, st)))
             return rc;
+        // sampled forward: the predicted steps (the last encoder step's output on) feed back a draw instead of the mean
+        if (eps && s >= obs_length - 2 &&
+            (rc = launch_sample_positions(normals_out + (size_t)s * M * 5, positions_out + (size_t)s * frame,
+                                          eps + (size_t)(s - (obs_length - 2)) * frame, (int)M, st)))
+            return rc;
         h_prev = h_next;
         c_prev = c_next;
         if (sink) {     // this step's results -> host, behind the step, beside the following steps
@@ -738,6 +743,21 @@ int tb2_lstm_forward_steps_goals(const tb2_lstm* m, const tb2_layout* l, const f
                                  float* c, float* states_out, void* workspace, size_t workspace_bytes, void* stream) {
     return forward_steps_impl(m, l, observed, obs_length, truth, n_decode, goals, first_step, last_step, normals_out,
                               positions_out, h, c, states_out, workspace, workspace_bytes, stream, nullptr);
+}
+
+int tb2_lstm_forward_steps_sampled(const tb2_lstm* m, const tb2_layout* l, const float* observed,
+                                   int32_t obs_length, const float* truth, int32_t n_decode, int32_t first_step,
+                                   int32_t last_step, const float* eps, float* normals_out, float* positions_out,
+                                   float* h, float* c, float* states_out, void* workspace, size_t workspace_bytes,
+                                   void* stream) {
+    TB2_REQUIRE(m, "null handle");
+    if (m->G > 0) {
+        set_error("sampled forwards of a goal-conditioned model (goal_dim > 0) are not built");
+        return TB2_ERR_UNSUPPORTED;
+    }
+    TB2_REQUIRE(eps, "eps_dev [n_decode + 1, M, 2] is required (all zeros for the mean trajectory)");
+    return forward_steps_impl(m, l, observed, obs_length, truth, n_decode, nullptr, first_step, last_step, normals_out,
+                              positions_out, h, c, states_out, workspace, workspace_bytes, stream, nullptr, nullptr, eps);
 }
 
 int tb2_lstm_forward_sequence_host(tb2_lstm* m, const tb2_layout* l, const float* observed, int32_t obs_length,

@@ -299,6 +299,8 @@ int launch_gates_tc(const tb2_lstm* m, const tb2_layout* l, int phase, const flo
                     const float* h_in, const float* c_in, float* h_out, float* c_out, float* normal_out,
                     float* pos_out, cudaStream_t st);
 int launch_split_bf16(const float* src, void* hi, void* lo, size_t n, cudaStream_t st);
+// pos [rows, 2] += the offset of the bivariate normal normals [rows, 5] at the standard normal pairs eps [rows, 2]
+int launch_sample_positions(const float* normals, float* pos, const float* eps, int rows, cudaStream_t st);
 int launch_grid_indices_copy(const tb2_layout* l, const Workspace* ws, int32_t* cell_out,
                              uint8_t* flag_out, cudaStream_t st);
 

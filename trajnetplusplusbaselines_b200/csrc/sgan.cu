@@ -129,9 +129,50 @@ __global__ void __launch_bounds__(128) vae_decoder_context_kernel(const float* _
     }
 }
 
+// Sampled LSTM positions (no reference counterpart: the reference feeds back the mean, lstm/lstm.py:232,255): row r of
+// one step moves from obs2 + mu to a draw of the step's bivariate normal,
+//   pos[r] += (sx e1, sy (rho e1 + sqrt(1 - rho^2) e2)),   (sx, sy, rho) = normals[r, 2:5], (e1, e2) = eps[r],
+// the Cholesky factor of [[sx^2, rho sx sy], [rho sx sy, sy^2]] applied to a standard normal pair.  A pair of exactly
+// (0, 0) leaves the row's bits untouched (the mean mode keeps its signed zeros); a NaN normal leaves a NaN position.
+// Launched inside the PDL step chain: the step's gate kernel wrote normals / pos, the next step's kernels read pos.
+__global__ void __launch_bounds__(256) sample_positions_kernel(const float* __restrict__ normals,
+                                                               float* __restrict__ pos,
+                                                               const float* __restrict__ eps, int rows) {
+    grid_dep_wait();          // normals / positions come from the step's gate kernel
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r < rows) {
+        const float e1 = eps[2 * (size_t)r], e2 = eps[2 * (size_t)r + 1];
+        if (e1 != 0.f || e2 != 0.f) {
+            const float* n = normals + (size_t)r * 5;
+            const float sx = n[2], sy = n[3], rho = n[4];
+            const float a = sqrtf(1.f - rho * rho);
+            pos[2 * (size_t)r] += sx * e1;
+            pos[2 * (size_t)r + 1] += sy * (rho * e1 + a * e2);
+        }
+    }
+    grid_dep_launch();        // after the writes: the next step reads the sampled positions
+}
+
+int launch_sample_positions(const float* normals, float* pos, const float* eps, int rows, cudaStream_t st) {
+    if (rows <= 0) return TB2_OK;
+    {
+        KernelTimer kt("sample_positions", st);
+        launch_pdl(sample_positions_kernel, dim3((rows + 255) / 256), dim3(256), 0, st, normals, pos, eps, rows);
+    }
+    TB2_LAUNCH_CHECK();
+    return TB2_OK;
+}
+
 }  // namespace tb2
 
 using namespace tb2;
+
+extern "C" int tb2_lstm_sample_positions(const float* normals, float* positions, const float* eps, int32_t rows,
+                                         void* stream) {
+    TB2_REQUIRE(normals && positions && eps, "null argument (normals, positions and eps are required)");
+    TB2_REQUIRE(rows >= 0, "bad sizes");
+    return launch_sample_positions(normals, positions, eps, rows, (cudaStream_t)stream);
+}
 
 extern "C" int tb2_vae_scale_hidden(const float* weight, const float* bias, const float* z, float* h, int32_t M,
                                     int32_t H, int32_t latent_dim, void* stream) {

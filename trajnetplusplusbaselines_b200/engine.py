@@ -326,6 +326,18 @@ class ModelHandle:
                 int(n_decode), _ptr(goals), int(first_step), int(last_step), _ptr(normals), _ptr(positions), _ptr(h),
                 _ptr(c), _ptr(None), _ptr(ws), need, _stream(self.device)))
 
+    def forward_steps_sampled(self, layout, observed, truth, n_decode, first_step, last_step, eps, normals, positions, h,
+                              c):
+        """forward_steps with every predicted position drawn from its step's normal at the standard normal pairs
+        eps [n_decode + 1, M, 2] (tb2_lstm_forward_steps_sampled)."""
+        lib = _lib.load()
+        ws, need = self.workspace(layout)
+        with torch.cuda.device(self.device):
+            _lib.check(lib.tb2_lstm_forward_steps_sampled(
+                self.handle, layout.handle, _ptr(observed), int(observed.shape[0]), _ptr(truth), int(n_decode),
+                int(first_step), int(last_step), _ptr(eps), _ptr(normals), _ptr(positions), _ptr(h), _ptr(c),
+                _ptr(None), _ptr(ws), need, _stream(self.device)))
+
     def forward_sequence_host(self, layout, observed, truth, n_decode, normals, positions, h, c, normals_host,
                               positions_host, copy_stream, goals=None):
         """tb2_lstm_forward_sequence_host: per-step device-to-host copies on `copy_stream`; the caller

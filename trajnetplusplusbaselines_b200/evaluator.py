@@ -178,9 +178,32 @@ def evaluate_file(predictor, infile, outfile, obs_length=9, pred_length=12, mode
     return len(scenes)
 
 
+def prediction_folder(model, args):
+    """Folder of a model's predictions under test_pred: `<model>_modes<k>`, or `<model>_sample_modes<k>` for the
+    sampled predictions of args.sample (so that they never mix with the mean-trajectory files)."""
+    sample = '_sample' if getattr(args, 'sample', False) else ''
+    return os.path.basename(model).replace('.pkl', '') + sample + '_modes' + str(args.modes)
+
+
+def _sampled_predictor(predictor):
+    """--sample: the loaded LSTMPredictor's model in a SampledLSTMPredictor; any other predictor exits with a message."""
+    from .lstm import LSTMPredictor
+    if not isinstance(predictor, LSTMPredictor):
+        raise SystemExit("--sample draws the modes of an LSTM model (LSTMPredictor); %s has no per-step normal to "
+                         "sample: run it without --sample" % type(predictor).__name__)
+    from .lstm.sampling import SampledLSTMPredictor
+    try:
+        return SampledLSTMPredictor(predictor.model)
+    except NotImplementedError as e:
+        raise SystemExit("--sample: %s" % e)
+
+
 def get_predictions(args, load_predictor=None):
     """The write side of lstm/trajnet_evaluator.get_predictions (:28-64): for every model in args.output
     and every `*.ndjson` of the test folder, write `<path>/test_pred/<model>_modes<k>/<dataset>.ndjson`.
+    With args.sample the predictor is a SampledLSTMPredictor of the loaded LSTM model (mode 0 the mean, the others drawn
+    from the model's per-step normals) writing `<model>_sample_modes<k>`; a predictor that is not an LSTMPredictor exits
+    with a message before anything is written.
     Existing model folders are skipped, like the reference does.  A goal-conditioned model (predictor.model.goal_flag)
     reads the goals of every test file from goal_files/test_private/<file>.pkl under the working directory, like the
     reference's evaluator.  Every goal file is loaded, and every pedestrian of every scene checked to have a goal, before
@@ -198,7 +221,7 @@ def get_predictions(args, load_predictor=None):
     datasets = sorted(f for f in os.listdir(test_dir) if not f.startswith('.') and f.endswith('.ndjson'))
     written = {}
     for model in args.output:
-        model_name = os.path.basename(model).replace('.pkl', '') + '_modes' + str(args.modes)
+        model_name = prediction_folder(model, args)
         out_dir = os.path.join(args.path, model_name)
         exists = os.path.exists(out_dir)
         _barrier()                                          # every rank has looked before rank 0 creates the folder
@@ -207,6 +230,8 @@ def get_predictions(args, load_predictor=None):
                 print('Predictions corresponding to {} already exist.'.format(model_name))
             continue
         predictor = load_predictor(model)
+        if getattr(args, 'sample', False):
+            predictor = _sampled_predictor(predictor)
         goals = {}
         if getattr(getattr(predictor, 'model', None), 'goal_flag', False):
             for dataset in datasets:
@@ -237,6 +262,9 @@ def main(argv=None):
     parser.add_argument('--normalize_scene', action='store_true')
     parser.add_argument('--modes', default=1, type=int)
     parser.add_argument('--chunk', default=1024, type=int, help='scenes per batched forward')
+    parser.add_argument('--sample', action='store_true',
+                        help='LSTM models: draw modes 1..k-1 from the per-step normals (mode 0 is the mean) into '
+                             '<model>_sample_modes<k>')
     parser.add_argument('--evaluate', action='store_true',
                         help='after writing the predictions, score them against test_private and print the table')
     # the reference's scoring flags: they take effect with --evaluate (without it this tool only writes)

@@ -1,4 +1,5 @@
-"""Every mode of every scene in one batched decode: the evaluator path of the multi-modal predictors (S-GAN, VAE).
+"""Every mode of every scene in one batched decode: the evaluator path of the multi-modal predictors (S-GAN, VAE, and the
+sampled LSTM modes of lstm/sampling.py, whose decode draws every predicted position from its step's normal).
 
 The per-scene predictors (SGANPredictor / VAEPredictor.__call__) run one encoder pass and then k decoder passes of
 pred_length - 1 steps each over the 5-50 tracks of one scene.  Here the encoder runs once over the B scenes of a chunk
@@ -75,12 +76,23 @@ def refuse_goals(model):
         raise NotImplementedError(GOALS_MESSAGE)
 
 
-def predict_modes(body, observed, split, n_predict, modes, context, max_rows=None):
+def sample_positions(normals, positions, eps):
+    """positions [rows, 2] += the offset of the normals [rows, 5] at the standard normal pairs eps [rows, 2], in place on
+    the device (tb2_lstm_sample_positions)."""
+    device = positions.device
+    with torch.cuda.device(device):
+        _lib.check(_lib.load().tb2_lstm_sample_positions(_ptr(normals), _ptr(positions), _ptr(eps),
+                                                         int(positions.shape[0]), _stream(device)))
+
+
+def predict_modes(body, observed, split, n_predict, modes, context, max_rows=None, eps=None):
     """Encoder once over the scenes of `split`, then the decoders of all `modes` modes.
 
     context(h_enc, c_enc, q0, q1, h_out, c_out) writes the decoder starting state of modes [q0, q1) into
-    h_out / c_out [(q1 - q0) * M, H].  Returns the positions of the last n_predict steps, float32 [n_predict,
-    modes * M, 2] on the device, mode-major."""
+    h_out / c_out [(q1 - q0) * M, H].  eps: float32 [n_predict, modes * M, 2] on the device, mode-major: every predicted
+    position of the decode is drawn from its step's normal (tb2_lstm_forward_steps_sampled), the first one, the
+    encoder's last output, on the replicated rows before the decoder starts.  Returns the positions of the last
+    n_predict steps, float32 [n_predict, modes * M, 2] on the device, mode-major."""
     refuse_goals(body)
     enc = body._encode(body._sequence(observed, split, None, n_predict, pad_to_batch_max=False))
     handle, device, M, S_enc, S = enc.handle, enc.handle.device, enc.layout.num_tracks, enc.S_enc, enc.S
@@ -99,7 +111,12 @@ def predict_modes(body, observed, split, n_predict, modes, context, max_rows=Non
         positions[:S_enc] = enc.positions[:S_enc].repeat(1, kq, 1)      # the decoder's first inputs
         h, c = torch.empty((rows, H), **f32), torch.empty((rows, H), **f32)
         context(enc.h, enc.c, q0, q1, h, c)
-        handle.forward_steps(rep, obs_rep, None, enc.n_decode, S_enc, S, normals, positions, h, c)
+        if eps is None:
+            handle.forward_steps(rep, obs_rep, None, enc.n_decode, S_enc, S, normals, positions, h, c)
+        else:
+            part = eps[:, q0 * M:q1 * M].contiguous()
+            sample_positions(enc.normals[S_enc - 1].repeat(kq, 1), positions[S_enc - 1], part[0])
+            handle.forward_steps_sampled(rep, obs_rep, None, enc.n_decode, S_enc, S, part, normals, positions, h, c)
         out[:, q0 * M:q1 * M] = positions[S - n_predict:]
     return out
 
@@ -119,9 +136,10 @@ class ModesPredictor(Predictor):
         (NearestNeighborLSTM, TrajectronPooling): that state is not replicated per mode."""
         return not stateful_pool(self._lstm_model())
 
-    def _predict_batch_xy(self, xys, n_predict, obs_length, start_length, args, modes, max_rows, make_context):
+    def _predict_batch_xy(self, xys, n_predict, obs_length, start_length, args, modes, max_rows, make_context,
+                          make_eps=None):
         """predict_batch_xy: make_context(device, split, modes) draws the random inputs of every mode and returns the
-        context() of predict_modes."""
+        context() of predict_modes; make_eps(device, M, modes), if given, returns its eps."""
         body = self._lstm_model()
         if not self.batch_decode_supported():
             raise NotImplementedError("batched decoding of a %s whose interaction module keeps an LSTM state is not "
@@ -137,7 +155,8 @@ class ModesPredictor(Predictor):
         with torch.no_grad():
             observed, split, rotation, center = observed_batch(body, xys, obs_length, first, normalize)
             context = make_context(observed.device, split, modes)
-            pred = predict_modes(body, observed, split, n_predict, modes, context, max_rows)
+            eps = make_eps(observed.device, int(split[-1]), modes) if make_eps is not None else None
+            pred = predict_modes(body, observed, split, n_predict, modes, context, max_rows, eps)
             return scene_results(pred, split, modes, n_predict, normalize, rotation, center)
 
 
@@ -168,6 +187,12 @@ def group_of_rows(split, device):
     return torch.from_numpy(np.repeat(np.arange(len(split) - 1, dtype=np.int32), np.diff(split))).to(device)
 
 
+def replicated_context(h_enc, c_enc, q0, q1, h_out, c_out):
+    """context() of predict_modes where every mode's decoder starts from the encoder state itself."""
+    h_out.copy_(h_enc.repeat(q1 - q0, 1))
+    c_out.copy_(c_enc.repeat(q1 - q0, 1))
+
+
 def sgan_context(weight, bias, noise, groups, num_groups, noise_dim):
     """context() of predict_modes for the S-GAN generator: noise [k, num_groups, noise_dim] (None: no noise)."""
     lib = _lib.load()
@@ -175,8 +200,7 @@ def sgan_context(weight, bias, noise, groups, num_groups, noise_dim):
     def run(h_enc, c_enc, q0, q1, h_out, c_out):
         kq = q1 - q0
         if noise is None:                      # no_noise: the decoder starts from the encoder state (sgan.py:200-204)
-            h_out.copy_(h_enc.repeat(kq, 1))
-            c_out.copy_(c_enc.repeat(kq, 1))
+            replicated_context(h_enc, c_enc, q0, q1, h_out, c_out)
             return
         part = noise[q0:q1].contiguous()
         device = h_enc.device

@@ -457,11 +457,13 @@ def format_table(label, results, col_result):
 
 
 def trajnet_evaluate(args, out=print):
-    """Scores <args.path>/<model>_modes<k>/*.ndjson against the ground truth in the sibling test_private folder and prints
+    """Scores <args.path>/<model>_modes<k>/*.ndjson (<model>_sample_modes<k> with args.sample) against the ground truth
+    in the sibling test_private folder and prints
     one table per model.  Returns {label: {dataset: (metrics, categories, sub_categories)}}."""
     pred_root = args.path.rstrip(os.sep)
     private_root = (pred_root[:-len('_pred')] if pred_root.endswith('_pred') else pred_root) + '_private'
-    model_names = [os.path.basename(model).replace('.pkl', '') + '_modes' + str(args.modes) for model in args.output]
+    from .evaluator import prediction_folder
+    model_names = [prediction_folder(model, args) for model in args.output]
     labels = args.labels if getattr(args, 'labels', None) is not None else model_names
     disable_collision = getattr(args, 'disable_collision', False)
     everything = {}
