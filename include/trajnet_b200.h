@@ -55,6 +55,14 @@ extern "C" {
                                    * [out_dim, 8]; the sum runs over the whole batch in the padded (trainer) layout and over
                                    * the scene in the per-scene layout; then the LSTMCell / hidden2pool of TB2_POOL_NN_LSTM */
 
+#define TB2_POOL_EXTERNAL 16      /* any other interaction module (a torch.nn.Module with the reference's pool plug,
+                                   * lstm.py:25-42,141-151): the caller runs it between the step's kernels.  out_dim = its
+                                   * width; the library keeps no pool weights; pool_to_input 0 (out_dim == hidden_dim) or 1.
+                                   * Only the step calls below serve it: tb2_pool_inputs_padded, the module,
+                                   * tb2_lstm_step_forward_pooled (tb2_lstm_step_backward for training).  tb2_pool_forward,
+                                   * tb2_lstm_step_forward(_goals), the sequence / steps calls and
+                                   * tb2_lstm_sequence_backward return TB2_ERR_INVALID; goals are not built with it */
+
 #define TB2_PHASE_ENCODER 0
 #define TB2_PHASE_DECODER 1
 
@@ -333,6 +341,30 @@ int tb2_vae_decoder_context(const float* weight_dev, const float* bias_dev, cons
                             int32_t latent_dim, int32_t k, float* h_out_dev, float* c_out_dev, void* stream);
 
 /* ---------------------------------------------------------------------------------------
+ * External interaction modules (TB2_POOL_EXTERNAL): one recurrence step with the module run by the caller.
+ * n_pad = tb2_layout_max_scene(layout); slot (b, j) of the padded layout [B, n_pad] is track scene_offsets[b] + j
+ * when j < the size of scene b, padding otherwise.
+ * ------------------------------------------------------------------------------------- */
+/* generate_pooling_inputs (lstm.py:25-42): obs1 / obs2 [M, 2] and h [M, H] of the ragged layout ->
+ * obs1_pad / obs2_pad [B, n_pad, 2] and h_pad [B, n_pad, H], NaN in the padding slots.  Every track's hidden state goes
+ * in, absent tracks included.  The module is then called as pool(h_pad, obs1_pad, obs2_pad) -> [B * n_pad, out_dim]. */
+int tb2_pool_inputs_padded(const tb2_layout* layout, const float* obs1_dev, const float* obs2_dev, const float* h_dev,
+                           int32_t H, float* obs1_pad_out_dev, float* obs2_pad_out_dev, float* h_pad_out_dev,
+                           void* stream);
+/* Its backward: d_h_dev [M, H] += the rows of d_h_pad_dev [B, n_pad, H] at every track's slot (padding is dropped). */
+int tb2_pool_inputs_padded_backward(const tb2_layout* layout, const float* d_h_pad_dev, int32_t H, float* d_h_dev,
+                                    void* stream);
+/* tb2_lstm_step_forward with the module's output pooled_padded_dev [B * n_pad, out_dim]: the row of every present track
+ * (pool_sample[track_mask_positions], lstm.py:148) is concatenated to the LSTM input (pool_to_input) or added to its
+ * hidden state (lstm.py:151); absent tracks keep their state as in tb2_lstm_step_forward.  h_out / c_out may alias
+ * h_in / c_in. */
+int tb2_lstm_step_forward_pooled(const tb2_lstm* model, const tb2_layout* layout, int32_t phase,
+                                 const float* obs1_dev, const float* obs2_dev, const float* pooled_padded_dev,
+                                 const float* h_in_dev, const float* c_in_dev, float* h_out_dev, float* c_out_dev,
+                                 float* normal_out_dev, float* pos_out_dev, void* workspace_dev, size_t workspace_bytes,
+                                 void* stream);
+
+/* ---------------------------------------------------------------------------------------
  * Training: backward of the whole time loop (what autograd does for Trainer.train_batch,
  * lstm/trainer.py:229-269, through LSTM.forward).  Gradient accumulators are fp32 device
  * buffers in the reference's parameter layout (+=, caller zeroes them).
@@ -384,6 +416,22 @@ int tb2_lstm_sequence_backward(const tb2_lstm* model, const tb2_layout* layout, 
                                const tb2_lstm_grads* grads, void* workspace_dev, size_t workspace_bytes,
                                void* bwd_workspace_dev, size_t bwd_workspace_bytes, const void* cache_dev,
                                size_t cache_bytes, void* stream);
+
+/* Backward of one tb2_lstm_step_forward_pooled step (TB2_POOL_EXTERNAL), from the step's inputs: the gate
+ * pre-activations are recomputed (one GEMM), then
+ *   d_h_in_dev, d_c_in_dev  [M, H]                gradient wrt h_in / c_in (absent tracks: d_h_out / d_c_out unchanged)
+ *   d_pooled_padded_dev     [B * n_pad, out_dim]  gradient wrt pooled_padded (0 for absent tracks and padding slots)
+ * and the step's gradients are ADDED to `grads`: input embedding, the phase's LSTMCell and hidden2normal (those fields
+ * must be set; the other phase's may be NULL).  d_normal_dev [M, 5] is the upstream gradient wrt the step's normals
+ * with that wrt pos already added to its first two columns (pos = obs2 + mu); NaN entries count as 0.  d_c_in may alias
+ * d_c_out.  Fed-back positions are inputs (detached, lstm.py:242-250): no gradient flows into obs1 / obs2. */
+size_t tb2_lstm_step_backward_workspace_bytes(const tb2_lstm* model, const tb2_layout* layout);
+int tb2_lstm_step_backward(const tb2_lstm* model, const tb2_layout* layout, const tb2_lstm_weights* weights,
+                           int32_t phase, const float* obs1_dev, const float* obs2_dev, const float* pooled_padded_dev,
+                           const float* h_in_dev, const float* c_in_dev, const float* d_h_out_dev,
+                           const float* d_c_out_dev, const float* d_normal_dev, float* d_h_in_dev, float* d_c_in_dev,
+                           float* d_pooled_padded_dev, const tb2_lstm_grads* grads, void* bwd_workspace_dev,
+                           size_t bwd_workspace_bytes, void* stream);
 
 /* TB2_POOL_NN_LSTM / TB2_POOL_TRAJECTRON: zero the interaction-encoder LSTM state kept in `workspace`
  * (NearestNeighborLSTM.reset, non_gridbased_pooling.py:385-389; TrajectronPooling.reset, :481-485).  tb2_lstm_forward_sequence / _steps(first_step = 0) do this themselves; the

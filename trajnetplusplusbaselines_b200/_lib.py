@@ -11,6 +11,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libtrajnet_b200.so")
 
 POOL_NONE, POOL_OCCUPANCY, POOL_DIRECTIONAL, POOL_SOCIAL, POOL_HIDDEN_MLP, POOL_NN_MLP, POOL_ATTN_MLP, POOL_NN_LSTM, POOL_TRAJECTRON = 0, 1, 2, 3, 4, 5, 6, 7, 8
+POOL_EXTERNAL = 16      # any other interaction module: torch runs it between the step's kernels (lstm/external.py)
 PHASE_ENCODER, PHASE_DECODER = 0, 1
 # LSTM widths the kernels are built for, and tb2_lstm_create's refusal of any other (kHiddenDimMessage, csrc/common.cuh)
 HIDDEN_DIMS = tuple(range(32, 257, 32))
@@ -160,6 +161,13 @@ PROTOTYPES = {
                                                   _vp, _vp, _vp, _vp, _i32, ctypes.POINTER(LstmGrads),
                                                   _vp, _sz, _vp, _sz, _vp, _sz, _vp]),
     "tb2_pool_state_reset": (ctypes.c_int, [_vp, _vp, _vp, _sz, _vp]),
+    "tb2_pool_inputs_padded": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp]),
+    "tb2_pool_inputs_padded_backward": (ctypes.c_int, [_vp, _vp, _i32, _vp, _vp]),
+    "tb2_lstm_step_forward_pooled": (ctypes.c_int, [_vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz,
+                                                    _vp]),
+    "tb2_lstm_step_backward_workspace_bytes": (_sz, [_vp, _vp]),
+    "tb2_lstm_step_backward": (ctypes.c_int, [_vp, _vp, ctypes.POINTER(LstmWeights), _i32, _vp, _vp, _vp, _vp, _vp, _vp,
+                                              _vp, _vp, _vp, _vp, _vp, ctypes.POINTER(LstmGrads), _vp, _sz, _vp]),
     "tb2_lstm_train_cache_bytes": (_sz, [_vp, _vp, _i32]),
     "tb2_lstm_forward_sequence_train": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _sz, _vp]),
     "tb2_sgan_add_noise": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp]),

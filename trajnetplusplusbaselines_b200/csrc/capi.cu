@@ -182,7 +182,7 @@ using namespace tb2;
 extern "C" {
 
 const char* tb2_last_error(void) { return g_error.c_str(); }
-int tb2_version(void) { return 103; }
+int tb2_version(void) { return 104; }
 uint64_t tb2_launch_count(void) { return g_launch_count.load(); }
 
 int tb2_profile_begin(void) {
@@ -274,6 +274,10 @@ static int configure_pool(const tb2_lstm_config& c, tb2_lstm* m) {
                         "hidden-state MLP pooling widths");
             m->pool_out = c.out_dim;
             break;
+        case TB2_POOL_EXTERNAL:       // the caller's module: only its width matters here
+            TB2_REQUIRE(c.out_dim >= 1 && c.out_dim <= 4096, "external interaction module: 1 <= out_dim <= 4096");
+            m->pool_out = c.out_dim;
+            break;
     }
     // the pool output is concatenated to the LSTM input, or added to the hidden state (lstm.py:151)
     TB2_REQUIRE(c.pool_to_input || m->pool_out == m->H, "pool_to_input=0 needs out_dim == hidden_dim");
@@ -320,6 +324,7 @@ static int alloc_buffers(tb2_lstm* m) {
     };
     switch (c.pool_type) {
         case TB2_POOL_NONE:
+        case TB2_POOL_EXTERNAL:       // no pool weights: the caller's module owns them
             break;
         case TB2_POOL_SOCIAL:
             ALLOC(m->WencT, m->H * m->C);
@@ -395,7 +400,9 @@ int tb2_lstm_create(const tb2_lstm_config* cfg, tb2_lstm** out) {
     }
     TB2_REQUIRE(cfg->embedding_dim >= 4 && cfg->embedding_dim <= 1024, "embedding_dim out of range");
     TB2_REQUIRE(cfg->goal_dim == 0 || (cfg->goal_dim >= 4 && cfg->goal_dim <= 1024), "goal_dim out of range (0 = no goals)");
-    TB2_REQUIRE(cfg->pool_type >= TB2_POOL_NONE && cfg->pool_type <= TB2_POOL_TRAJECTRON, "bad pool_type");
+    TB2_REQUIRE((cfg->pool_type >= TB2_POOL_NONE && cfg->pool_type <= TB2_POOL_TRAJECTRON) ||
+                    cfg->pool_type == TB2_POOL_EXTERNAL,
+                "bad pool_type");
     tb2_lstm* m = new (std::nothrow) tb2_lstm();
     TB2_REQUIRE(m, "out of host memory");
     m->cfg = *cfg;
@@ -546,6 +553,7 @@ int tb2_pool_forward(const tb2_lstm* m, const tb2_layout* l, const float* hidden
     int rc = check_ready(m, l, workspace, workspace_bytes);
     if (rc) return rc;
     TB2_REQUIRE(m->cfg.pool_type != TB2_POOL_NONE, "model has no interaction pooling");
+    TB2_REQUIRE(m->cfg.pool_type != TB2_POOL_EXTERNAL, kExternalPoolMessage);
     TB2_REQUIRE(obs1 && obs2 && pooled_out, "null argument");
     TB2_REQUIRE((m->cfg.pool_type != TB2_POOL_SOCIAL && m->cfg.pool_type != TB2_POOL_HIDDEN_MLP &&
                  m->cfg.pool_type != TB2_POOL_ATTN_MLP) || hidden,
@@ -558,15 +566,22 @@ int tb2_pool_forward(const tb2_lstm* m, const tb2_layout* l, const float* hidden
     return launch_pool_mlp(m, l, &ws, pooled_out, nullptr, nullptr, st);
 }
 
-// hs_cur: index (0/1) of the ping-pong buffer holding the bf16 split of h_in (tensor-core gates)
+// hs_cur: index (0/1) of the ping-pong buffer holding the bf16 split of h_in (tensor-core gates); pooled_pad: the
+// external module's output [B * n_max, pool_out] (TB2_POOL_EXTERNAL only)
 static int step_impl(const tb2_lstm* m, const tb2_layout* l, int phase, const float* obs1,
                      const float* obs2, const float* goals, const float* h_in, const float* c_in, float* h_out,
                      float* c_out, float* normal_out, float* pos_out, Workspace* ws, int hs_cur,
-                     cudaStream_t st) {
+                     cudaStream_t st, const float* pooled_pad = nullptr) {
     int rc;
     const bool tc = m->Wg_hi[0] != nullptr;
     const float* pooled = nullptr;
-    if (m->cfg.pool_type >= TB2_POOL_HIDDEN_MLP) {
+    if (m->cfg.pool_type == TB2_POOL_EXTERNAL) {
+        // the module's row of every present track: fp32, or the split the tensor-core gate kernel reads
+        if ((rc = launch_external_pooled(m, l, obs1, obs2, pooled_pad, nullptr, tc ? nullptr : ws->pooled,
+                                         tc ? ws->pool_hi : nullptr, tc ? ws->pool_lo : nullptr, st)))
+            return rc;
+        pooled = ws->pooled;
+    } else if (m->cfg.pool_type >= TB2_POOL_HIDDEN_MLP) {
         // pooled fp32, split for the tensor-core gate kernel
         if ((rc = launch_nongrid_pool(m, l, h_in, obs1, obs2, ws, ws->pooled, st))) return rc;
         if (tc && (rc = launch_split_bf16(ws->pooled, ws->pool_hi, ws->pool_lo, (size_t)l->M * m->P, st))) return rc;
@@ -615,6 +630,7 @@ int tb2_lstm_step_forward_goals(const tb2_lstm* m, const tb2_layout* l, int32_t 
                                 size_t workspace_bytes, void* stream) {
     int rc = check_ready(m, l, workspace, workspace_bytes);
     if (rc) return rc;
+    TB2_REQUIRE(m->cfg.pool_type != TB2_POOL_EXTERNAL, kExternalPoolMessage);
     if ((rc = resolve_goals(m, &goals))) return rc;
     TB2_REQUIRE(phase == TB2_PHASE_ENCODER || phase == TB2_PHASE_DECODER, "bad phase");
     TB2_REQUIRE(obs1 && obs2 && h_in && c_in && h_out && c_out && normal_out, "null argument");
@@ -625,6 +641,30 @@ int tb2_lstm_step_forward_goals(const tb2_lstm* m, const tb2_layout* l, int32_t 
         (rc = launch_split_bf16(h_in, ws.hs_hi[0], ws.hs_lo[0], (size_t)l->M * m->H, st)))
         return rc;
     return step_impl(m, l, phase, obs1, obs2, goals, h_in, c_in, h_out, c_out, normal_out, pos_out, &ws, 0, st);
+}
+
+int tb2_lstm_step_forward_pooled(const tb2_lstm* m, const tb2_layout* l, int32_t phase, const float* obs1,
+                                 const float* obs2, const float* pooled_pad, const float* h_in, const float* c_in,
+                                 float* h_out, float* c_out, float* normal_out, float* pos_out, void* workspace,
+                                 size_t workspace_bytes, void* stream) {
+    int rc = check_ready(m, l, workspace, workspace_bytes);
+    if (rc) return rc;
+    TB2_REQUIRE(m->cfg.pool_type == TB2_POOL_EXTERNAL,
+                "tb2_lstm_step_forward_pooled serves external interaction modules (TB2_POOL_EXTERNAL)");
+    if (m->G > 0) {
+        set_error("goals with an external interaction module are not built");
+        return TB2_ERR_UNSUPPORTED;
+    }
+    TB2_REQUIRE(phase == TB2_PHASE_ENCODER || phase == TB2_PHASE_DECODER, "bad phase");
+    TB2_REQUIRE(obs1 && obs2 && pooled_pad && h_in && c_in && h_out && c_out && normal_out, "null argument");
+    Workspace ws;
+    carve_workspace(m, l, workspace, &ws);
+    cudaStream_t st = (cudaStream_t)stream;
+    if (m->Wg_hi[0] &&
+        (rc = launch_split_bf16(h_in, ws.hs_hi[0], ws.hs_lo[0], (size_t)l->M * m->H, st)))
+        return rc;
+    return step_impl(m, l, phase, obs1, obs2, nullptr, h_in, c_in, h_out, c_out, normal_out, pos_out, &ws, 0, st,
+                     pooled_pad);
 }
 
 // Steps [first_step, last_step) of the time loop.  first_step == 0 starts from the zero state
@@ -645,6 +685,7 @@ static int forward_steps_impl(const tb2_lstm* m, const tb2_layout* l, const floa
                               const HostSink* sink, const TrainCache* cache = nullptr, const float* eps = nullptr) {
     int rc = check_ready(m, l, workspace, workspace_bytes);
     if (rc) return rc;
+    TB2_REQUIRE(m->cfg.pool_type != TB2_POOL_EXTERNAL, kExternalPoolMessage);
     if ((rc = resolve_goals(m, &goals))) return rc;
     TB2_REQUIRE(observed && normals_out && positions_out && h && c, "null argument");
     TB2_REQUIRE(obs_length >= 2 && n_decode >= 0, "need obs_length >= 2 and n_decode >= 0");

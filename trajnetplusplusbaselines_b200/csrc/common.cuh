@@ -131,6 +131,10 @@ constexpr int kGateBK = 16;        // K-chunk of the gate GEMM; weight rows are 
 // Zero columns after the last cell of sparse_layer1_mma's weight image: the kernel loads whole 256-column chunks
 // without bounds checks, and the columns past d1 (never written out) of the last cell fall into this tail.
 constexpr int kLayer1MmaTailCols = 256;
+// Refusal of the fused calls for a model whose interaction module the caller runs (TB2_POOL_EXTERNAL)
+constexpr const char* kExternalPoolMessage =
+    "an external interaction module (TB2_POOL_EXTERNAL) runs step by step: tb2_pool_inputs_padded, the module, "
+    "tb2_lstm_step_forward_pooled, and tb2_lstm_step_backward for training";
 
 }  // namespace tb2
 
@@ -301,6 +305,14 @@ int launch_gates_tc(const tb2_lstm* m, const tb2_layout* l, int phase, const flo
 int launch_split_bf16(const float* src, void* hi, void* lo, size_t n, cudaStream_t st);
 // pos [rows, 2] += the offset of the bivariate normal normals [rows, 5] at the standard normal pairs eps [rows, 2]
 int launch_sample_positions(const float* normals, float* pos, const float* eps, int rows, cudaStream_t st);
+// TB2_POOL_EXTERNAL: the caller's pooled_pad [B * n_max, pool_out] row of every present track (0 for absent ones,
+// + base when given) as fp32 `out` and / or the bf16 (hi, lo) split
+int launch_external_pooled(const tb2_lstm* m, const tb2_layout* l, const float* obs1, const float* obs2,
+                           const float* pooled_pad, const float* base, float* out, void* hi, void* lo, cudaStream_t st);
+// d pooled_pad [B * n_max, P] from src[m, col .. col + P) of the present tracks; d_h_in = pass + dh_rec on the M rows
+int launch_external_step_grads(const tb2_layout* l, const int* masked, const float* src, int ld_src, int col, int P,
+                               const float* pass, const float* dh_rec, int H, float* d_pooled_pad, float* d_h_in,
+                               cudaStream_t st);
 int launch_grid_indices_copy(const tb2_layout* l, const Workspace* ws, int32_t* cell_out,
                              uint8_t* flag_out, cudaStream_t st);
 

@@ -500,6 +500,7 @@ int launch_repack(tb2_lstm* m, const tb2_lstm_weights* w, cudaStream_t st) {
     const tb2_lstm_config& c = m->cfg;
     switch (c.pool_type) {
         case TB2_POOL_NONE:
+        case TB2_POOL_EXTERNAL:       // the caller's module owns its weights
             break;
         case TB2_POOL_SOCIAL:
             TB2_REQUIRE(w->pool_encoding_weight && w->pool_encoding_bias, "pool.hidden_dim_encoding missing");

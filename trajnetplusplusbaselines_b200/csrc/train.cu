@@ -1326,6 +1326,27 @@ static int lstm_weight_grads(const tb2_lstm* m, const tb2_lstm_weights* w, const
     return TB2_OK;
 }
 
+// Buffers of tb2_lstm_step_backward (external interaction module): the records of one step over all M rows
+struct StepBwdBuffers : RowRecords {
+    float* pooled;     // [M, pool_out] the module's rows as the gate operand (pool_to_input)
+    float* h_eff;      // [M, H] h_in + pooled (pool_to_input = 0)
+    float* DH;         // [M, H] dgates . W_hh
+    int* rows;         // [M] 0 .. M - 1
+};
+
+static size_t carve_step_bwd(const tb2_lstm* m, const tb2_layout* l, void* base, StepBwdBuffers* b) {
+    const size_t M = (size_t)l->M, H = (size_t)m->H;
+    StepBwdBuffers tmp;
+    StepBwdBuffers* o = b ? b : &tmp;
+    Carve c{base};
+    carve_records(m, M, 1, 0, c, o);
+    o->pooled = c.take(m->cfg.pool_to_input ? M * (size_t)m->pool_out : 4);
+    o->h_eff = c.take(m->cfg.pool_to_input ? 4 : M * H);
+    o->DH = c.take(M * H);
+    o->rows = reinterpret_cast<int*>(c.take(M));
+    return c.bytes();
+}
+
 template <int C>
 static int social_pair_kernels(const tb2_lstm* m, const tb2_layout* l, const SocBuffers& b, const float* lat,
                                int nm1, int d1, cudaStream_t st) {
@@ -1583,6 +1604,7 @@ int tb2_lstm_sequence_backward(const tb2_lstm* m, const tb2_layout* l, const tb2
         set_error("training a goal-conditioned model (goal_dim > 0) is not built");
         return TB2_ERR_UNSUPPORTED;
     }
+    TB2_REQUIRE(m->cfg.pool_type != TB2_POOL_EXTERNAL, kExternalPoolMessage);
     const bool social = m->cfg.pool_type == TB2_POOL_SOCIAL;
     if (social && !social_trainable(m)) {
         set_error("social training backward supports one_layer / two_layer embeddings with constant = 0");
@@ -1665,6 +1687,83 @@ int tb2_lstm_sequence_backward(const tb2_lstm* m, const tb2_layout* l, const tb2
             return rc;
     }
     return TB2_OK;
+}
+
+size_t tb2_lstm_step_backward_workspace_bytes(const tb2_lstm* m, const tb2_layout* l) {
+    if (!m || !l) return 0;
+    return carve_step_bwd(m, l, nullptr, nullptr);
+}
+
+// One step of the external-module LSTM backward, on all M rows (the module couples the tracks of a scene through their
+// hidden states): the gather (bwd_gather_kernel) and gate GEMM of phases (A) / (B), the cell / head kernel of (C) with
+// the incoming d h as its recurrent input, and the weight reductions of (D) / (E) over the step's M records.
+int tb2_lstm_step_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lstm_weights* w, int32_t phase,
+                           const float* obs1, const float* obs2, const float* pooled_pad, const float* h_in,
+                           const float* c_in, const float* d_h_out, const float* d_c_out, const float* d_normal,
+                           float* d_h_in, float* d_c_in, float* d_pooled_pad, const tb2_lstm_grads* g,
+                           void* bwd_workspace, size_t bwd_workspace_bytes, void* stream) {
+    TB2_REQUIRE(m && l && w && g, "null handle");
+    TB2_REQUIRE(m->weights_set, "tb2_lstm_set_weights has not been called");
+    TB2_REQUIRE(m->cfg.pool_type == TB2_POOL_EXTERNAL,
+                "tb2_lstm_step_backward serves external interaction modules (TB2_POOL_EXTERNAL); the built-in models "
+                "train through tb2_lstm_sequence_backward");
+    if (m->G > 0) {
+        set_error("training a goal-conditioned model (goal_dim > 0) is not built");
+        return TB2_ERR_UNSUPPORTED;
+    }
+    TB2_REQUIRE(phase == TB2_PHASE_ENCODER || phase == TB2_PHASE_DECODER, "bad phase");
+    TB2_REQUIRE(obs1 && obs2 && pooled_pad && h_in && c_in && d_h_out && d_c_out && d_normal && d_h_in && d_c_in &&
+                    d_pooled_pad, "null argument");
+    const bool enc = phase == TB2_PHASE_ENCODER;
+    TB2_REQUIRE(w->input_embedding_weight && w->input_embedding_bias && w->hidden2normal_weight && w->hidden2normal_bias &&
+                    (enc ? w->encoder_weight_ih && w->encoder_weight_hh : w->decoder_weight_ih && w->decoder_weight_hh),
+                "weights of the input embedding, the phase's LSTMCell and hidden2normal are required");
+    TB2_REQUIRE(g->input_embedding_weight && g->input_embedding_bias && g->hidden2normal_weight && g->hidden2normal_bias &&
+                    (enc ? g->encoder_weight_ih && g->encoder_weight_hh && g->encoder_bias_ih && g->encoder_bias_hh
+                         : g->decoder_weight_ih && g->decoder_weight_hh && g->decoder_bias_ih && g->decoder_bias_hh),
+                "gradients of the input embedding, the phase's LSTMCell and hidden2normal are required");
+    TB2_REQUIRE(bwd_workspace && bwd_workspace_bytes >= carve_step_bwd(m, l, nullptr, nullptr),
+                "backward workspace too small (tb2_lstm_step_backward_workspace_bytes)");
+    TB2_REQUIRE(((uintptr_t)bwd_workspace & 15) == 0, "backward workspace must be 16-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    const int M = l->M, K = m->K_gate, E = m->E, P = m->P, EP = E + P, H = m->H, G4 = 4 * H;
+    const bool to_input = m->cfg.pool_to_input != 0;
+    StepBwdBuffers b;
+    carve_step_bwd(m, l, bwd_workspace, &b);
+    int rc;
+    iota_kernel<<<(M + 255) / 256, 256, 0, st>>>(b.rows, M);
+    TB2_LAUNCH_CHECK();
+    // (A) X = [emb | pooled | h_in] (pool_to_input) or [emb | h_in + pooled]: the operand the forward's gate kernel read
+    if ((rc = launch_external_pooled(m, l, obs1, obs2, pooled_pad, to_input ? nullptr : h_in,
+                                     to_input ? b.pooled : b.h_eff, nullptr, nullptr, st)))
+        return rc;
+    {
+        KernelTimer kt("bwd_gather", st);
+        bwd_gather_kernel<<<M, 256, 0, st>>>(b.rows, M, (const float2*)obs1, (const float2*)obs2, m->We, m->be,
+                                             to_input ? h_in : b.h_eff, nullptr, nullptr, nullptr, nullptr, nullptr, 1,
+                                             m->C, m->cells, to_input ? b.pooled : nullptr, b.X, nullptr, b.VEL,
+                                             b.masked, E, P, K, H);
+    }
+    TB2_LAUNCH_CHECK();
+    // (B) gate pre-activations
+    if ((rc = gemm_nn(b.X, K, m->WgT[phase], G4, b.GP, G4, M, G4, K, m->bg[phase], st))) return rc;
+    // (C) cell + head backward: d h_out enters as the recurrent input, d c_out is updated in place into d c_in
+    TB2_CHECK_CUDA(cudaMemsetAsync(b.pass[1], 0, (size_t)M * H * sizeof(float), st));
+    if (d_c_in != d_c_out)
+        TB2_CHECK_CUDA(cudaMemcpyAsync(d_c_in, d_c_out, (size_t)M * H * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    {
+        KernelTimer kt("bwd_cell_head", st);
+        rc = launch_cell_head(H, M, st, b.rows, b.masked, b.GP, c_in, nullptr, nullptr, d_h_out, b.pass[1], b.pass[0],
+                              d_c_in, d_normal, m->Wn, m->bn, b.DG, b.HS, b.DN, M);
+    }
+    if (rc) return rc;
+    // (D) + (E) dX_in = dgates . W_ih and the step's weight gradients; d h_in through W_hh
+    if ((rc = lstm_weight_grads(m, w, g, b, M, 1, enc ? 1 : 0, true, st))) return rc;
+    if ((rc = gemm_nn(b.DG, G4, enc ? w->encoder_weight_hh : w->decoder_weight_hh, H, b.DH, H, M, H, G4, nullptr, st)))
+        return rc;
+    // d pooled: the pooled columns of dX_in, or d (h_in + pooled) = d h_in's recurrent part (pool_to_input = 0)
+    return launch_external_step_grads(l, b.masked, to_input ? b.DXIN : b.DH, to_input ? EP : H, to_input ? E : 0,
+                                      m->pool_out, b.pass[0], b.DH, H, d_pooled_pad, d_h_in, st);
 }
 
 }  // extern "C"

@@ -114,8 +114,11 @@ def lstm_config(hidden_dim, embedding_dim, pool_to_input, pool, goal_dim=0):
     cfg.pool_to_input = int(bool(pool_to_input))
     cfg.pool_type = _lib.POOL_NONE
     cfg.pool_size = cfg.blur_size = 1
-    if pool is not None:
+    if pool is not None and hasattr(pool, 'fill_config'):
         pool.fill_config(cfg)
+    elif pool is not None:       # a module of the caller's, run in torch between the step's kernels (lstm/external.py)
+        cfg.pool_type = _lib.POOL_EXTERNAL
+        cfg.out_dim = int(pool.out_dim)
     return cfg
 
 

@@ -16,9 +16,15 @@ import torch
 from .. import _lib
 from ..data import paths_to_xy
 from ..engine import LayoutCache, ModelHandle, lstm_config, weights_key
+from .external import EXTERNAL_GOALS_MESSAGE, external_forward, external_step, is_external, scene_size_groups
 from .modules import Hidden2Normal, InputEmbedding
 
 NAN = float('nan')
+
+# the fused sequence calls (S-GAN / VAE decoding, sampled modes) read a built-in module's configuration; a module of the
+# caller's runs only through LSTM.forward / LSTM.step
+EXTERNAL_FUSED_MESSAGE = ("%s is an external interaction module (it has no fill_config): LSTM.forward, LSTM.step and "
+                          "LSTMPredictor run it; S-GAN / VAE and sampled predictions with it are not built")
 
 # one forward set up by LSTM._sequence
 Sequence = namedtuple('Sequence', 'handle layout obs truth n_decode S_enc S normals positions h c out_device goals')
@@ -107,8 +113,6 @@ class LSTM(torch.nn.Module):
             raise RuntimeError("LSTM parameters are on %s: move the model to a CUDA device (model.to('cuda')); "
                                "there is no CPU path" % device)
         if self._handle is None or self._handle.device != device:
-            if self.pool is not None and not hasattr(self.pool, 'fill_config'):
-                raise NotImplementedError("only GridBasedPooling and the HiddenStateMLPPooling / NearestNeighborMLP / AttentionMLPPooling / NearestNeighborLSTM / TrajectronPooling interaction modules are built")
             cfg = lstm_config(self.hidden_dim, self.embedding_dim, self.pool_to_input, self.pool,
                               self.goal_dim if self.goal_flag else 0)
             self._handle = ModelHandle(cfg, device)
@@ -130,7 +134,7 @@ class LSTM(torch.nn.Module):
         if self.goal_flag:
             goal = self.goal_embedding.input_embeddings[0]
             fields.update(goal_embedding_weight=goal.weight, goal_embedding_bias=goal.bias)
-        if self.pool is not None:
+        if self.pool is not None and not is_external(self.pool):      # an external module's weights stay in torch
             fields.update(self.pool.weight_fields())
         return fields
 
@@ -177,9 +181,11 @@ class LSTM(torch.nn.Module):
     def step(self, lstm, hidden_cell_state, obs1, obs2, goals, batch_split):
         """One step (lstm.py:91-168).  hidden_cell_state = (h [M, H], c [M, H]) flat CUDA tensors
         (the reference's per-track Python lists are also accepted and converted)."""
+        phase = _lib.PHASE_ENCODER if lstm is self.encoder else _lib.PHASE_DECODER
+        if is_external(self.pool):
+            return external_step(self, hidden_cell_state, phase, obs1, obs2, batch_split)
         handle = self._engine()
         device = handle.device
-        phase = _lib.PHASE_ENCODER if lstm is self.encoder else _lib.PHASE_DECODER
         h, c = hidden_cell_state
         was_list = isinstance(h, (list, tuple))
         if was_list:
@@ -203,6 +209,8 @@ class LSTM(torch.nn.Module):
         on the device `observed` came from.
         """
         assert ((prediction_truth is None) + (n_predict is None)) == 1
+        if is_external(self.pool):        # the module runs in torch between the step's kernels (lstm/external.py)
+            return external_forward(self, observed, goals, batch_split, prediction_truth, n_predict)
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             from .training import sequence_with_grad
             return sequence_with_grad(self, observed, batch_split, prediction_truth, n_predict)
@@ -213,6 +221,8 @@ class LSTM(torch.nn.Module):
         """A forward of `observed` [obs_length, M, 2] set up on the model's device: the inputs there and empty outputs
         and (h, c) state.  Launches nothing.  The steps are [0, S_enc) for the encoder and [S_enc, S) for the decoder;
         truth is None when there is no teacher forcing.  goals [M, 2]: read by a goal-conditioned model only."""
+        if is_external(self.pool):
+            raise NotImplementedError(EXTERNAL_FUSED_MESSAGE % type(self.pool).__name__)
         handle = self._engine(force_repack)
         device = handle.device
         layout = self._layouts.get(batch_split, pad_to_batch_max, device=device)
@@ -405,7 +415,24 @@ class LSTMPredictor(Predictor):
     def predict_batch_xy(self, xys, scene_goals=None, n_predict=12, obs_length=9, start_length=0, args=None):
         """predict_batch on arrays: xys = list of float64 [n_frames, N_i, 2] as paths_to_xy returns them (the column
         pipeline of the evaluator, data.load_test_scenes_xy, builds them without TrackRow objects).  scene_goals: per
-        scene the goals [N_i, 2] of its tracks, read by a goal-conditioned model (goal_flag=True) only."""
+        scene the goals [N_i, 2] of its tracks, read by a goal-conditioned model (goal_flag=True) only.
+
+        With an external interaction module (lstm/external.py) the scenes run in one padded forward per distinct
+        scene size: a group has no padding, so each scene is seen as in a per-scene call by any module whose batch
+        entries do not interact, and a stateful module keeps one state per forward.  A module that mixes the entries of
+        its batch (a sum over the whole batch, like TrajectronPooling's) matches per-scene calls only in __call__."""
+        if is_external(self.model.pool):
+            if self.model.goal_flag:
+                raise NotImplementedError(EXTERNAL_GOALS_MESSAGE)
+            results = [None] * len(xys)
+            for idx in scene_size_groups(xys):
+                part = self._predict_batch_xy([xys[i] for i in idx], None, n_predict, obs_length, start_length, args)
+                for i, r in zip(idx, part):
+                    results[i] = r
+            return results
+        return self._predict_batch_xy(xys, scene_goals, n_predict, obs_length, start_length, args)
+
+    def _predict_batch_xy(self, xys, scene_goals, n_predict, obs_length, start_length, args):
         self.model.eval()
         normalize = bool(getattr(args, 'normalize_scene', False))
         split = np.zeros(len(xys) + 1, dtype=np.int64)
@@ -427,8 +454,11 @@ class LSTMPredictor(Predictor):
             else:
                 observed = torch.Tensor(np.concatenate([xy[start_length:obs_length] for xy in xys], axis=1))
                 goals = torch.Tensor(goals) if goals is not None else None
-            _, output_scenes = self.model._forward_nograd(observed, torch.from_numpy(split), None, n_predict,
-                                                          pad_to_batch_max=False, goals=goals)
+            if is_external(self.model.pool):
+                _, output_scenes = self.model(observed, goals, torch.from_numpy(split), n_predict=n_predict)
+            else:
+                _, output_scenes = self.model._forward_nograd(observed, torch.from_numpy(split), None, n_predict,
+                                                              pad_to_batch_max=False, goals=goals)
             if normalize:
                 output_scenes = inverse_scenes(output_scenes, split, rotation, center)
             else:

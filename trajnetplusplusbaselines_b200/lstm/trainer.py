@@ -228,7 +228,7 @@ def check_trainable(model):
     if model.hidden_dim not in _lib.HIDDEN_DIMS:
         raise RuntimeError(_lib.HIDDEN_DIM_MESSAGE)
     pool = model.pool
-    if pool is None:
+    if pool is None or not hasattr(pool, 'fill_config'):       # none, or an external module (trained through autograd)
         return
     layers = 0 if pool.embedding is None else sum(isinstance(m, torch.nn.Linear) for m in pool.embedding)
     width = pool.out_dim if layers else pool.n * pool.n * pool.pooling_dim

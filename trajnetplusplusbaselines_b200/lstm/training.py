@@ -40,6 +40,8 @@ def _grad_targets(model):
     _refuse_goals(model)
     out = {k: f(model) for k, f in _GRAD_FIELDS.items()}
     pool = model.pool
+    if pool is not None and not hasattr(pool, 'fill_config'):
+        return out         # an external module: autograd carries its own gradients (lstm/external.py)
     if pool is not None and not hasattr(pool, 'embedding_arch'):        # only GridBasedPooling has a backward
         raise NotImplementedError("training of %s is not built (inference only); use torch.no_grad()" % type(pool).__name__)
     if pool is not None and pool.embedding is not None:
