@@ -367,7 +367,9 @@ int tb2_lstm_step_forward_pooled(const tb2_lstm* model, const tb2_layout* layout
 /* ---------------------------------------------------------------------------------------
  * Training: backward of the whole time loop (what autograd does for Trainer.train_batch,
  * lstm/trainer.py:229-269, through LSTM.forward).  Gradient accumulators are fp32 device
- * buffers in the reference's parameter layout (+=, caller zeroes them).
+ * buffers in the reference's parameter layout (+=, caller zeroes them).  Zero the whole struct
+ * before filling it (memset / `= {0}`): a NULL field is a gradient the call does not compute, and
+ * fields appended by later versions then stay NULL.
  * ------------------------------------------------------------------------------------- */
 typedef struct tb2_lstm_grads {
     float* input_embedding_weight;   /* [E-2, 2] */
@@ -388,6 +390,14 @@ typedef struct tb2_lstm_grads {
     float* pool_embedding_bias1;     /* [out_dim] or NULL */
     float* pool_encoding_weight;     /* pool.hidden_dim_encoding.weight grad [latent, H] (social) or NULL */
     float* pool_encoding_bias;       /* [latent] or NULL */
+    /* Gradient wrt the observed positions (version 105), NULL = not computed.  It flows through the encoder steps'
+     * velocity inputs (vel = obs2 - obs1), the directional grid's relative velocities and, with social pooling, the
+     * hidden states the grid reads.  Decoder inputs are detached: fed-back positions, teacher-forced truth and the
+     * copy of observed[-1] (lstm.py:235-250).  The head term pred = obs2 + mu is the caller's: the call cannot tell
+     * d pred from d mu in d_normals. */
+    float* d_observed;               /* [obs_length, M, 2] (+=), tb2_lstm_sequence_backward */
+    float* d_obs1;                   /* [M, 2] (+=), tb2_lstm_step_backward; set both or neither */
+    float* d_obs2;                   /* [M, 2] (+=), tb2_lstm_step_backward */
 } tb2_lstm_grads;
 
 /* scratch for tb2_lstm_sequence_backward: per (step, active row) records + per-step buffers */
@@ -424,7 +434,8 @@ int tb2_lstm_sequence_backward(const tb2_lstm* model, const tb2_layout* layout, 
  * and the step's gradients are ADDED to `grads`: input embedding, the phase's LSTMCell and hidden2normal (those fields
  * must be set; the other phase's may be NULL).  d_normal_dev [M, 5] is the upstream gradient wrt the step's normals
  * with that wrt pos already added to its first two columns (pos = obs2 + mu); NaN entries count as 0.  d_c_in may alias
- * d_c_out.  Fed-back positions are inputs (detached, lstm.py:242-250): no gradient flows into obs1 / obs2. */
+ * d_c_out.  grads->d_obs1 / d_obs2 (optional) receive the gradient through the step's velocity input; the term of
+ * pos = obs2 + mu is the caller's. */
 size_t tb2_lstm_step_backward_workspace_bytes(const tb2_lstm* model, const tb2_layout* layout);
 int tb2_lstm_step_backward(const tb2_lstm* model, const tb2_layout* layout, const tb2_lstm_weights* weights,
                            int32_t phase, const float* obs1_dev, const float* obs2_dev, const float* pooled_padded_dev,

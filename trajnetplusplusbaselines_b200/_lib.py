@@ -94,7 +94,7 @@ class LstmGrads(ctypes.Structure):
         "decoder_weight_ih", "decoder_weight_hh", "decoder_bias_ih", "decoder_bias_hh",
         "hidden2normal_weight", "hidden2normal_bias",
         "pool_embedding_weight0", "pool_embedding_bias0", "pool_embedding_weight1", "pool_embedding_bias1",
-        "pool_encoding_weight", "pool_encoding_bias")]
+        "pool_encoding_weight", "pool_encoding_bias", "d_observed", "d_obs1", "d_obs2")]
 
 
 class SfParams(ctypes.Structure):

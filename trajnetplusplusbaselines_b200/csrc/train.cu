@@ -946,6 +946,107 @@ __global__ void iota_kernel(int* __restrict__ p, int n) {
     if (i < n) p[i] = i;
 }
 
+// row_of[rows[r]] = r (the caller fills row_of with -1 first)
+__global__ void row_of_kernel(const int* __restrict__ rows, int R, int* __restrict__ row_of) {
+    const int r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r < R) row_of[rows[r]] = r;
+}
+
+__device__ __forceinline__ float warp_sum(float v) {
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+    return v;
+}
+
+// Gradient wrt the positions of one step's inputs, vel = obs2 - obs1 (lstm.py:123-125): one CTA per scene, one warp per
+// track t, every sum in a fixed order (no atomics: run-to-run identical).
+//   d vel_t  = 4 We^T (relu mask (.) dX_emb[t])            the input embedding (modules.py:24-30), record row of t
+//   PAIRS (directional grid, gridbased_pooling.py:118-140): rel_ij = vel_j - vel_i of every IN-RANGE pair (i, j) of an
+//   observer i with a record receives d grid_i[cell(i, j), c] = Wt1[cell][c]^T dz_i, like index_put_'s backward gives
+//   it to every writer, overwritten ones included.  Nothing reaches a channel whose cell holds exactly 0 (lp_pool2d's
+//   sign(0)^2 = 0, :304: an out-of-range pair wrote the cell last, or the winner's value is 0) or a component of rel
+//   that is not finite (nan_to_num, :140).  Track t collects + d rel_it as neighbour and - d rel_tj as observer, in
+//   ascending observer order.
+//   d obs2[t] += d vel_t,  d obs1[t] -= d vel_t
+// X / DXIN / G are the step's records (row r = row_of[track]), DXIN's pooled columns already ReLU-masked (dz).
+template <bool PAIRS>
+__global__ void __launch_bounds__(256) input_grad_kernel(
+    const int* __restrict__ scene_off, const int* __restrict__ row_of, const float2* __restrict__ obs1,
+    const float2* __restrict__ obs2, const float* __restrict__ X, int ldx, const float* __restrict__ DXIN, int EP, int E,
+    const float* __restrict__ We, const int* __restrict__ pair_cell, const uint8_t* __restrict__ pair_flag, int nm1,
+    const float* __restrict__ G, int cells, const float* __restrict__ Wt1, float* __restrict__ d_obs1,
+    float* __restrict__ d_obs2) {
+    const int b = blockIdx.x, row0 = scene_off[b], n_s = scene_off[b + 1] - row0;
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int P = EP - E;
+    for (int t = warp; t < n_s; t += blockDim.x >> 5) {
+        const int mt = row0 + t, rt = row_of[mt];
+        float ax = 0.f, ay = 0.f;
+        if (rt >= 0) {
+            for (int k = lane; k < E - 2; k += 32) {
+                if (X[(size_t)rt * ldx + k] > 0.f) {
+                    const float d = DXIN[(size_t)rt * EP + k];
+                    ax = fmaf(We[2 * k], d, ax);
+                    ay = fmaf(We[2 * k + 1], d, ay);
+                }
+            }
+            ax = 4.f * warp_sum(ax);
+            ay = 4.f * warp_sum(ay);
+        }
+        if (PAIRS) {
+            float px = 0.f, py = 0.f;
+            const float2 at = obs1[mt], bt = obs2[mt];
+            const float vtx = bt.x - at.x, vty = bt.y - at.y;
+            for (int i = 0; i < n_s; ++i) {
+                const int ri = row_of[row0 + i];
+                if (ri < 0) continue;
+                const float2 ai = obs1[row0 + i], bi = obs2[row0 + i];
+                const float vix = bi.x - ai.x, viy = bi.y - ai.y;
+                const float* dz = DXIN + (size_t)ri * EP + E;
+                const float* gi = G + (size_t)ri * 2 * cells;
+                const int jj0 = i == t ? 0 : t - (t > i), jj1 = i == t ? n_s - 1 : jj0 + 1;
+                for (int jj = jj0; jj < jj1; ++jj) {
+                    const size_t slot = (size_t)(row0 + i) * nm1 + jj;
+                    if (!pair_flag[slot]) continue;
+                    const int j = jj + (jj >= i), cell = pair_cell[slot];
+                    float vjx = vtx, vjy = vty;
+                    if (i == t) {
+                        const float2 aj = obs1[row0 + j], bj = obs2[row0 + j];
+                        vjx = bj.x - aj.x;
+                        vjy = bj.y - aj.y;
+                    }
+                    const bool live_x = gi[cell] != 0.f && isfinite(vjx - vix);
+                    const bool live_y = gi[cells + cell] != 0.f && isfinite(vjy - viy);
+                    if (!live_x && !live_y) continue;
+                    const float* w0 = Wt1 + (size_t)cell * 2 * P;
+                    float sx = 0.f, sy = 0.f;
+                    for (int o = lane; o < P; o += 32) {
+                        sx = fmaf(w0[o], dz[o], sx);
+                        sy = fmaf(w0[P + o], dz[o], sy);
+                    }
+                    sx = live_x ? warp_sum(sx) : 0.f;
+                    sy = live_y ? warp_sum(sy) : 0.f;
+                    if (i == t) {
+                        px -= sx;
+                        py -= sy;
+                    } else {
+                        px += sx;
+                        py += sy;
+                    }
+                }
+            }
+            ax += px;
+            ay += py;
+        }
+        if (lane == 0) {
+            d_obs2[2 * (size_t)mt] += ax;
+            d_obs2[2 * (size_t)mt + 1] += ay;
+            d_obs1[2 * (size_t)mt] -= ax;
+            d_obs1[2 * (size_t)mt + 1] -= ay;
+        }
+    }
+}
+
 }  // namespace tb2
 
 using namespace tb2;
@@ -1160,15 +1261,17 @@ static void carve_records(const tb2_lstm* m, size_t rows, size_t S, size_t extra
 
 struct BwdBuffers : RowRecords {
     float* G;                                      // [S][R][C n n] grid rows
+    int* row_of;                                   // [M] record row of each track, -1: none (d observed)
 };
 
-static size_t carve_bwd(const tb2_lstm* m, size_t R, size_t S, void* base, BwdBuffers* b) {
+static size_t carve_bwd(const tb2_lstm* m, size_t R, size_t S, size_t M, void* base, BwdBuffers* b) {
     const size_t P = (size_t)m->P, CG = (size_t)m->C * (size_t)m->cells;
     BwdBuffers tmp;
     BwdBuffers* o = b ? b : &tmp;
     Carve c{base};
     carve_records(m, R, S, P * CG, c, o);
     o->G = c.take(P ? S * R * CG : 4);
+    o->row_of = reinterpret_cast<int*>(c.take(M));
     return c.bytes();
 }
 
@@ -1323,6 +1426,43 @@ static int lstm_weight_grads(const tb2_lstm* m, const tb2_lstm_weights* w, const
     bwd_embed_kernel<<<E - 2, 256, 0, st>>>(b.X, K, b.DXIN, EP, b.VEL, S * rows, g->input_embedding_weight,
                                             g->input_embedding_bias);
     TB2_LAUNCH_CHECK();
+    return TB2_OK;
+}
+
+// d observed of the encoder steps [0, S_enc) (g->d_observed, [obs_length, M, 2], +=): input_grad_kernel per step over
+// the step's records (rows: record row -> track, row_of: track -> record row or -1).  Directional grids first rebuild
+// the step's pair table (pool_prepare, the winners the gather read, plus cells and range flags).  Steps in ascending
+// order: each frame's two contributions are added in a fixed order.
+static int observed_grads(const tb2_lstm* m, const tb2_layout* l, const RowRecords& b, const float* G, int rows,
+                          const int* row_of, const float* observed, const float* states, int S_enc, Workspace& ws,
+                          float* d_observed, cudaStream_t st) {
+    const int K = m->K_gate, E = m->E, EP = E + m->P, H = m->H;
+    const size_t M = (size_t)l->M, CG = (size_t)m->C * (size_t)m->cells;
+    const int nm1 = l->n_max > 1 ? l->n_max - 1 : 1;
+    const bool pairs = m->cfg.pool_type == TB2_POOL_DIRECTIONAL;
+    int rc;
+    for (int s = 0; s < S_enc; ++s) {
+        const float* o1 = observed + (size_t)s * M * 2;
+        const float* o2 = observed + (size_t)(s + 1) * M * 2;
+        const float* Xs = b.X + (size_t)s * rows * K;
+        const float* DXs = b.DXIN + (size_t)s * rows * EP;
+        float* d1 = d_observed + (size_t)s * M * 2;
+        float* d2 = d_observed + (size_t)(s + 1) * M * 2;
+        if (pairs) {
+            const float* h_prev = s > 0 ? states + ((size_t)(s - 1) * 2 + 0) * M * H : nullptr;
+            if ((rc = launch_pool_prepare(m, l, h_prev, o1, o2, 1, 1, 0, &ws, st))) return rc;
+            KernelTimer kt("bwd_input_dir_pairs", st);
+            input_grad_kernel<true><<<l->B, 256, 0, st>>>(l->scene_off, row_of, (const float2*)o1, (const float2*)o2, Xs, K,
+                                                          DXs, EP, E, m->We, ws.pair_cell, ws.pair_flag, nm1,
+                                                          G + (size_t)s * rows * CG, m->cells, m->Wt1, d1, d2);
+        } else {
+            KernelTimer kt("bwd_input_vel", st);
+            input_grad_kernel<false><<<l->B, 256, 0, st>>>(l->scene_off, row_of, (const float2*)o1, (const float2*)o2, Xs,
+                                                           K, DXs, EP, E, m->We, nullptr, nullptr, nm1, nullptr, 0,
+                                                           nullptr, d1, d2);
+        }
+        TB2_LAUNCH_CHECK();
+    }
     return TB2_OK;
 }
 
@@ -1575,6 +1715,11 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
             return rc;
     }
     if ((rc = colsum(b.DLAT, C, S * Mi, C, g->pool_encoding_bias, nullptr, b.scratch, b.scratch_floats, st))) return rc;
+    // d observed: every track has its record row (rows = row_of = 0 .. M - 1); the grid values are hidden states, whose
+    // gradient the chain above already carried into each neighbour's own inputs
+    if (g->d_observed &&
+        (rc = observed_grads(m, l, b, nullptr, Mi, b.rows, observed, states, S_enc, ws, g->d_observed, st)))
+        return rc;
     return TB2_OK;
 }
 }  // namespace tb2
@@ -1587,7 +1732,7 @@ size_t tb2_lstm_backward_workspace_bytes(const tb2_lstm* m, const tb2_layout* l,
     if (m->cfg.pool_type == TB2_POOL_SOCIAL)
         return carve_social(m, l, (size_t)(num_steps > 0 ? num_steps : 1), nullptr, nullptr);
     return carve_bwd(m, (size_t)(num_active > 0 ? num_active : 1), (size_t)(num_steps > 0 ? num_steps : 1),
-                     nullptr, nullptr);
+                     (size_t)l->M, nullptr, nullptr);
 }
 
 int tb2_lstm_sequence_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lstm_weights* w,
@@ -1633,7 +1778,7 @@ int tb2_lstm_sequence_backward(const tb2_lstm* m, const tb2_layout* l, const tb2
     const int R = num_active, K = m->K_gate, E = m->E, P = m->P, EP = E + P, H = m->H, G4 = 4 * H;
     const size_t M = (size_t)l->M;
     BwdBuffers b;
-    carve_bwd(m, (size_t)R, (size_t)S, bwd_workspace, &b);
+    carve_bwd(m, (size_t)R, (size_t)S, M, bwd_workspace, &b);
     TB2_CHECK_CUDA(cudaMemsetAsync(b.dc, 0, (size_t)R * H * sizeof(float), st));
     const int nm1 = l->n_max > 1 ? l->n_max - 1 : 1;
     const bool pooled = m->cfg.pool_type != TB2_POOL_NONE;
@@ -1685,6 +1830,12 @@ int tb2_lstm_sequence_backward(const tb2_lstm* m, const tb2_layout* l, const tb2
             return rc;
         if ((rc = colsum(b.DXIN + E, EP, S * R, P, g->pool_embedding_bias0, nullptr, b.scratch, b.scratch_floats, st)))
             return rc;
+    }
+    if (g->d_observed) {     // the active rows' inputs, and through the directional pairs their neighbours'
+        TB2_CHECK_CUDA(cudaMemsetAsync(b.row_of, 0xff, M * sizeof(int), st));
+        row_of_kernel<<<(R + 255) / 256, 256, 0, st>>>(active_rows, R, b.row_of);
+        TB2_LAUNCH_CHECK();
+        if ((rc = observed_grads(m, l, b, b.G, R, b.row_of, observed, states, S_enc, ws, g->d_observed, st))) return rc;
     }
     return TB2_OK;
 }
@@ -1761,6 +1912,14 @@ int tb2_lstm_step_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
     if ((rc = lstm_weight_grads(m, w, g, b, M, 1, enc ? 1 : 0, true, st))) return rc;
     if ((rc = gemm_nn(b.DG, G4, enc ? w->encoder_weight_hh : w->decoder_weight_hh, H, b.DH, H, M, H, G4, nullptr, st)))
         return rc;
+    if (g->d_obs1 || g->d_obs2) {     // d obs1 / d obs2 through the step's velocity input
+        TB2_REQUIRE(g->d_obs1 && g->d_obs2, "d_obs1 and d_obs2 are set together");
+        KernelTimer kt("bwd_input_vel", st);
+        input_grad_kernel<false><<<l->B, 256, 0, st>>>(l->scene_off, b.rows, (const float2*)obs1, (const float2*)obs2, b.X,
+                                                       K, b.DXIN, EP, E, m->We, nullptr, nullptr, 1, nullptr, 0, nullptr,
+                                                       g->d_obs1, g->d_obs2);
+        TB2_LAUNCH_CHECK();
+    }
     // d pooled: the pooled columns of dX_in, or d (h_in + pooled) = d h_in's recurrent part (pool_to_input = 0)
     return launch_external_step_grads(l, b.masked, to_input ? b.DXIN : b.DH, to_input ? EP : H, to_input ? E : 0,
                                       m->pool_out, b.pass[0], b.DH, H, d_pooled_pad, d_h_in, st);

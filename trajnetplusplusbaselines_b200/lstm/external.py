@@ -17,7 +17,8 @@ current stream, with no host synchronisation in between.  Per step:
 n_pad is the largest scene of the batch, and every track's hidden state goes in, absent tracks included, as in the
 reference.  Under grad mode each of the two library calls is a torch.autograd.Function (backward:
 tb2_pool_inputs_padded_backward and tb2_lstm_step_backward), so autograd carries the gradient through the user's
-module into its parameters and into every track's hidden state.
+module into its parameters and into every track's hidden state, and, when `observed` requires grad, into the
+positions the encoder steps read (the velocity input, the module's position inputs and pos = obs2 + mu).
 """
 import ctypes
 
@@ -62,19 +63,27 @@ class _PaddedInputs(torch.autograd.Function):
                                                           _ptr(o2p), _ptr(hp), _stream(h.device)))
         ctx.layout = layout
         ctx.shape = tuple(h.shape)
-        ctx.mark_non_differentiable(o1p, o2p)
+        if not (ctx.needs_input_grad[1] or ctx.needs_input_grad[2]):
+            ctx.mark_non_differentiable(o1p, o2p)
         return o1p, o2p, hp
 
     @staticmethod
+    def _unpad(layout, d_pad, width, device):
+        """[M, width] += the track slots of d_pad [B, n_pad, width]; None when nothing flowed back."""
+        d = torch.zeros((layout.num_tracks, width), dtype=torch.float32, device=device)
+        if d_pad is not None:
+            with torch.cuda.device(device):
+                _lib.check(_lib.load().tb2_pool_inputs_padded_backward(layout.handle, _ptr(_f32(d_pad)), width, _ptr(d),
+                                                                       _stream(device)))
+        return d
+
+    @staticmethod
     def backward(ctx, d_o1p, d_o2p, d_hp):
-        if d_hp is None:
-            return None, None, None, None
-        d_hp = _f32(d_hp)
-        d_h = torch.zeros(ctx.shape, dtype=torch.float32, device=d_hp.device)
-        with torch.cuda.device(d_hp.device):
-            _lib.check(_lib.load().tb2_pool_inputs_padded_backward(ctx.layout.handle, _ptr(d_hp), ctx.shape[1], _ptr(d_h),
-                                                                   _stream(d_hp.device)))
-        return None, None, None, d_h
+        device = next(t.device for t in (d_hp, d_o1p, d_o2p) if t is not None)
+        d_o1 = _PaddedInputs._unpad(ctx.layout, d_o1p, 2, device) if ctx.needs_input_grad[1] else None
+        d_o2 = _PaddedInputs._unpad(ctx.layout, d_o2p, 2, device) if ctx.needs_input_grad[2] else None
+        d_h = _PaddedInputs._unpad(ctx.layout, d_hp, ctx.shape[1], device) if d_hp is not None else None
+        return None, d_o1, d_o2, d_h
 
 
 def _lstm_params(model):
@@ -114,12 +123,17 @@ class _PooledStep(torch.autograd.Function):
         if d_pos is not None:            # pos = obs2 + mu (lstm.py:232,255); obs2 is data / detached
             dn[:, :2] += torch.nan_to_num(d_pos.to(torch.float32))
         d_h_in, d_c_in, d_pooled = torch.empty((M, H), **f32), torch.empty((M, H), **f32), torch.empty_like(pooled)
+        want_obs = ctx.needs_input_grad[4] or ctx.needs_input_grad[5]
+        d_obs1 = torch.zeros((M, 2), **f32) if want_obs else None
+        d_obs2 = torch.zeros((M, 2), **f32) if want_obs else None
         cell = "encoder_" if phase == _lib.PHASE_ENCODER else "decoder_"
         fields = [k for k in _GRAD_FIELDS if not k.startswith(("encoder_", "decoder_")) or k.startswith(cell)]
         grads = {k: torch.zeros(tuple(_GRAD_FIELDS[k](model).shape), **f32) for k in fields}
         g = _lib.LstmGrads()
         for k, t in grads.items():
             setattr(g, k, t.data_ptr())
+        if want_obs:
+            g.d_obs1, g.d_obs2 = d_obs1.data_ptr(), d_obs2.data_ptr()
         w, keep = handle.weights_struct(model._weight_fields())
         lib = _lib.load()
         need = int(lib.tb2_lstm_step_backward_workspace_bytes(handle.handle, layout.handle))
@@ -130,11 +144,13 @@ class _PooledStep(torch.autograd.Function):
                 _ptr(c), _ptr(d_h_out), _ptr(d_c_out), _ptr(dn), _ptr(d_h_in), _ptr(d_c_in), _ptr(d_pooled),
                 ctypes.byref(g), _ptr(bws), need, _stream(device)))
         del keep
+        if want_obs and d_pos is not None:      # pos = obs2 + mu
+            d_obs2 += torch.nan_to_num(d_pos.to(torch.float32))
         out = []
         for k, p in zip(_GRAD_FIELDS, ctx.params):
             gr = grads.get(k)
             out.append(gr.to(p.dtype) if (gr is not None and p.requires_grad) else None)
-        return (None, None, None, None, None, None, d_pooled, d_h_in, d_c_in) + tuple(out)
+        return (None, None, None, None, d_obs1, d_obs2, d_pooled, d_h_in, d_c_in) + tuple(out)
 
 
 def pooled_step(model, handle, layout, phase, obs1, obs2, h, c):
@@ -173,7 +189,10 @@ def external_forward(model, observed, goals, batch_split, prediction_truth=None,
     M = layout.num_tracks
     if observed.shape[1] != M:
         raise ValueError("batch_split[-1] != number of tracks")
-    obs = model._to_device(observed, device, 'observed')
+    if grad and torch.is_tensor(observed) and observed.requires_grad:      # d observed flows back through the copy
+        obs = observed.to(device=device, dtype=torch.float32).contiguous()
+    else:
+        obs = model._to_device(observed, device, 'observed')
     truth = _truth_frames(model, prediction_truth, device)
     n_decode = int(truth.shape[0]) if truth is not None else int(n_predict) - 1
     H = int(model.hidden_dim)
@@ -189,8 +208,9 @@ def external_forward(model, observed, goals, batch_split, prediction_truth=None,
         normals.append(normal)
         positions.append(pos)
     primaries = _primaries(layout) if n_decode > 0 else None
-    # seq[0] = observed[-1] is a tensor in every forward: its primary rows take the fed-back position too
-    seq = [obs[-1]] + ([truth[k] for k in range(n_decode)] if truth is not None else [None] * n_decode)
+    # seq[0] = observed[-1] is a tensor in every forward: its primary rows take the fed-back position too.  It is the
+    # reference's deep copy (lstm.py:235): no gradient flows back through it
+    seq = [obs[-1].detach()] + ([truth[k] for k in range(n_decode)] if truth is not None else [None] * n_decode)
     for k in range(n_decode):                                         # decoder: the feedback rule of lstm.py:240-250
         o1, o2 = seq[k], seq[k + 1]
         if o1 is None:

@@ -26,7 +26,8 @@ def _require_cuda_f32(t, what):
 
 class _PrimaryLossFn(torch.autograd.Function):
     """values [T, B] of the primaries; backward scatters d value / d inputs into [T, M, 5].
-    kind 0: PredictionLoss (bivariate Gaussian + background), kind 1: L2Loss."""
+    kind 0: PredictionLoss (bivariate Gaussian + background), kind 1: L2Loss.  Both depend on targets - mu only, so
+    d targets = -d mu of the primaries (the Trainer's first target, xy[obs] - xy[obs - 1], depends on observed)."""
 
     @staticmethod
     def forward(ctx, inputs, targets, prim, background_rate, kind):
@@ -55,7 +56,8 @@ class _PrimaryLossFn(torch.autograd.Function):
         T, M = ctx.shape
         grad = torch.zeros((T, M, 5), dtype=torch.float32, device=dinputs.device)
         grad[:, prim.long()] = dinputs * grad_values.unsqueeze(-1)
-        return grad, None, None, None, None
+        d_targets = -grad[..., :2] if ctx.needs_input_grad[1] else None
+        return grad, d_targets, None, None, None
 
 
 class _CollisionLossFn(torch.autograd.Function):

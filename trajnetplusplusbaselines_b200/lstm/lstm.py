@@ -211,7 +211,9 @@ class LSTM(torch.nn.Module):
         assert ((prediction_truth is None) + (n_predict is None)) == 1
         if is_external(self.pool):        # the module runs in torch between the step's kernels (lstm/external.py)
             return external_forward(self, observed, goals, batch_split, prediction_truth, n_predict)
-        if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
+        # the graph path: parameter gradients, and / or d observed (a model with frozen parameters serves input gradients)
+        if torch.is_grad_enabled() and ((torch.is_tensor(observed) and observed.requires_grad) or
+                                        any(p.requires_grad for p in self.parameters())):
             from .training import sequence_with_grad
             return sequence_with_grad(self, observed, batch_split, prediction_truth, n_predict)
         return self._forward_nograd(observed, batch_split, prediction_truth, n_predict, goals=goals)

@@ -5,6 +5,11 @@ the backward is tb2_lstm_sequence_backward (csrc/train.cu): BPTT restricted to t
 actually receive gradient (all tracks for social pooling, whose hidden-state scatter couples the
 tracks of a scene).  Mirrors what autograd computes for the reference's
 Trainer.train_batch (trajnetbaselines/lstm/trainer.py:229-269).
+
+When `observed` requires grad, the same backward also returns d observed: through the encoder steps'
+velocity inputs, the directional grid's relative velocities and the hidden states social pooling
+reads, plus pred = obs2 + mu of the encoder steps.  The decoder's inputs are detached, as in the
+reference (its deep copy of observed[-1] and prediction_truth, and the fed-back positions).
 """
 import ctypes
 
@@ -72,6 +77,7 @@ class _SequenceFn(torch.autograd.Function):
         ctx.states = states
         ctx.cache = cache
         ctx.num_steps = normals.shape[0]
+        ctx.observed_meta = (observed.device, observed.dtype) if torch.is_tensor(observed) else None
         ctx.params = params
         ctx.save_for_backward(positions)
         return normals, positions
@@ -85,12 +91,21 @@ class _SequenceFn(torch.autograd.Function):
         lib = _lib.load()
         S = ctx.num_steps
         M = layout.num_tracks
+        obs_length = int(ctx.obs.shape[0])
         dn = torch.zeros((S, M, 5), dtype=torch.float32, device=device)
         if d_normals is not None:
             dn += torch.nan_to_num(d_normals.to(device=device, dtype=torch.float32))
-        if d_positions is not None:       # pred = obs2 + mu (lstm.py:232,255); obs2 is data / detached
-            dp = torch.nan_to_num(d_positions.to(device=device, dtype=torch.float32))[-S:]
+        d_obs = None
+        if ctx.needs_input_grad[1]:
+            d_obs = torch.zeros((obs_length, M, 2), dtype=torch.float32, device=device)
+        if d_positions is not None:       # pred = obs2 + mu (lstm.py:232,255)
+            dp_all = torch.nan_to_num(d_positions.to(device=device, dtype=torch.float32))
+            dp = dp_all[-S:]
             dn[:, :, :2] += dp
+            if d_obs is not None:         # obs2 of the encoder steps is observed[s + 1]; the decoder's are detached
+                if dp_all.shape[0] > S:   # obs_length 2: positions[0] is observed[-1] itself (lstm.py:222-223)
+                    d_obs[-1] += dp_all[0]
+                d_obs[1:obs_length] += dp[:obs_length - 1]
         dn = dn.contiguous()
         social = model.pool is not None and getattr(model.pool, 'type_', None) == 'social'
         if social:      # the hidden-state scatter couples all tracks of a scene: every row is active
@@ -104,6 +119,8 @@ class _SequenceFn(torch.autograd.Function):
             g = _lib.LstmGrads()
             for k, t in grads.items():
                 setattr(g, k, t.data_ptr())
+            if d_obs is not None:
+                g.d_observed = d_obs.data_ptr()
             w, keep = handle.weights_struct(model._weight_fields())
             ws, need = handle.workspace(layout)
             bneed = int(lib.tb2_lstm_backward_workspace_bytes(handle.handle, layout.handle, R, S))
@@ -125,10 +142,15 @@ class _SequenceFn(torch.autograd.Function):
         for p in ctx.params:
             gr = by_param.get(id(p))
             out.append(gr.to(p.dtype) if (gr is not None and p.requires_grad) else None)
-        return (None, None, None, None, None) + tuple(out)
+        if d_obs is not None:
+            device_in, dtype_in = ctx.observed_meta
+            d_obs = d_obs.to(device=device_in, dtype=dtype_in)
+        return (None, d_obs, None, None, None) + tuple(out)
 
 
 def sequence_with_grad(model, observed, batch_split, prediction_truth, n_predict):
     _refuse_goals(model)
+    if torch.is_tensor(observed) and observed.requires_grad:
+        _grad_targets(model)          # refuses the modules without a backward before anything runs
     params = tuple(model.parameters())
     return _SequenceFn.apply(model, observed, batch_split, prediction_truth, n_predict, *params)

@@ -76,6 +76,13 @@ def refuse_goals(model):
         raise NotImplementedError(GOALS_MESSAGE)
 
 
+def refuse_input_grad(model, *inputs):
+    """S-GAN / VAE have no backward: an input that asks for a gradient is refused rather than left without one."""
+    if torch.is_grad_enabled() and any(torch.is_tensor(t) and t.requires_grad for t in inputs):
+        raise NotImplementedError("gradients wrt the inputs of %s are not built (it has no backward); call it under "
+                                  "torch.no_grad() or detach the inputs" % type(model).__name__)
+
+
 def sample_positions(normals, positions, eps):
     """positions [rows, 2] += the offset of the normals [rows, 5] at the standard normal pairs eps [rows, 2], in place on
     the device (tb2_lstm_sample_positions)."""

@@ -88,6 +88,7 @@ class LSTMGenerator(LSTM):
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             raise NotImplementedError("S-GAN training (variety loss / discriminator steps) is not built; "
                                       "call the generator under torch.no_grad()")
+        multimodal.refuse_input_grad(self, observed, prediction_truth)
         return self.decode(self.encode(observed, batch_split, prediction_truth, n_predict))
 
 
@@ -123,6 +124,7 @@ class LSTMDiscriminator(torch.nn.Module):
         multimodal.refuse_goals(self)
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             raise NotImplementedError("S-GAN training is not built; score under torch.no_grad()")
+        multimodal.refuse_input_grad(self, observed, prediction)
         body = self._lstm[0]
         # n_predict = 1: no decoder step, every frame of [observed; prediction] goes through the encoder
         seq = body._encode(body._sequence(torch.cat([observed, prediction], dim=0), batch_split, None, 1))
@@ -148,6 +150,7 @@ class SGAN(torch.nn.Module):
         assert ((prediction_truth is None) + (n_predict is None)) == 1
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters()):
             raise NotImplementedError("S-GAN training is not built; call under torch.no_grad()")
+        multimodal.refuse_input_grad(self, observed, prediction_truth)
         rel_pred_list, pred_list = [], []
         seq = self.generator.encode(observed, batch_split, prediction_truth, n_predict)   # shared by all modes
         for _ in range(self.k):

@@ -90,6 +90,7 @@ class VAE(torch.nn.Module):
         if self.training or (torch.is_grad_enabled() and any(p.requires_grad for p in self.parameters())):
             raise NotImplementedError("VAE training (prediction encoder, KL term) is not built; use "
                                       "model.eval() under torch.no_grad()")
+        multimodal.refuse_input_grad(self, observed, prediction_truth)
         if not self.desire:
             raise NotImplementedError("desire=False (latent prior from vae_encoder_x) is not built")
         body = self._body[0]
