@@ -35,13 +35,16 @@ namespace tb2 {
 
 constexpr int kGtBM = 128;
 constexpr int kGtBN = 256;          // 64 units x 4 gates
-constexpr int kGtBK = 64;
-constexpr int kGtStages = 2;
+// 32-wide k-blocks (64-byte rows, 64B swizzle): 48 KB a stage, so a 3-stage ring fits beside the epilogue's shared
+// memory (the cell state it reads is staged there too) and two stages' loads can be in flight behind the one being
+// multiplied
+constexpr int kGtBK = 32;
+constexpr int kGtStages = 3;
 constexpr int kGtThreads = 384;     // two MMA + epilogue warpgroups, one producer warpgroup
 constexpr int kGtConsumerWarps = 8;
-constexpr uint32_t kGtABytes = kGtBM * kGtBK * 2;      // 16 KB
-constexpr uint32_t kGtBBytes = kGtBN * kGtBK * 2;      // 32 KB
-constexpr uint32_t kGtStageBytes = 2 * kGtABytes + 2 * kGtBBytes;   // 96 KB
+constexpr uint32_t kGtABytes = kGtBM * kGtBK * 2;      // 8 KB
+constexpr uint32_t kGtBBytes = kGtBN * kGtBK * 2;      // 16 KB
+constexpr uint32_t kGtStageBytes = 2 * kGtABytes + 2 * kGtBBytes;   // 48 KB
 
 // Gate non-linearities on the SFU (ex2.approx, ~2 ulp) -- the epilogue was bound by the ~200
 // instructions per hidden unit of the libm-accurate expf / tanhf.  Absolute error ~1e-7 per
@@ -82,12 +85,16 @@ lstm_gates_tc_kernel(const __grid_constant__ CUtensorMap map_emb_hi, const __gri
     __shared__ float bg_s[4][64];          // fused gate bias of this CTA's units
     constexpr int H = 64 * R;
     __shared__ float peer_part[R > 1 ? R - 1 : 1][kGtBM][5];  // rank 0: partial head sums of ranks 1, 2, ..
+    // c_in of each consumer thread's 16 (row, unit pair) slots, [slot][thread], copied during the mainloop: read from
+    // global memory in the epilogue, each load would wait behind the previous slot's stores (possible aliasing)
+    __shared__ float2 c_s[16][256];
+    __shared__ float2 obs_s[kGtBM][2];     // obs1, obs2 of the tile's rows, copied with c_s
 
     const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int rank = blockIdx.x;           // cluster rank == n-tile: units [64 rank, 64 rank + 64)
     const int m0 = blockIdx.y * kGtBM;
-    const int kb_pool = p.P / kGtBK;       // k-blocks: [emb (+ goal_emb) x kb_emb | pooled x kb_pool | h x H / 64]
-    const int kb_emb = kGoal ? (64 + p.G) / kGtBK : 1;
+    const int kb_pool = p.P / kGtBK;       // k-blocks: [emb (+ goal_emb) x kb_emb | pooled x kb_pool | h x H / 32]
+    const int kb_emb = (64 + (kGoal ? p.G : 0)) / kGtBK;
     const int num_kb = kb_emb + kb_pool + H / kGtBK;
     const uint32_t ring = (smem_u32(smem_gt) + 1023u) & ~1023u;
 
@@ -111,11 +118,30 @@ lstm_gates_tc_kernel(const __grid_constant__ CUtensorMap map_emb_hi, const __gri
 
     // rows (rl, rl + 8) of the tile and their quarter-row share of the head sums (consumer threads)
     const int rl = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    if (wg < 2) {
+#pragma unroll
+        for (int hr = 0; hr < 2; ++hr) {
+            const int row = m0 + rl + 8 * hr;
+            if (row >= p.M) continue;
+            if ((lane & 3) == 0) {
+                asm volatile("cp.async.ca.shared.global [%0], [%1], 8;"
+                             ::"r"(smem_u32(&obs_s[rl + 8 * hr][0])), "l"(p.obs1 + row) : "memory");
+                asm volatile("cp.async.ca.shared.global [%0], [%1], 8;"
+                             ::"r"(smem_u32(&obs_s[rl + 8 * hr][1])), "l"(p.obs2 + row) : "memory");
+            }
+#pragma unroll
+            for (int n8 = 0; n8 < 8; ++n8)
+                asm volatile("cp.async.ca.shared.global [%0], [%1], 8;"
+                             ::"r"(smem_u32(&c_s[8 * hr + n8][threadIdx.x])),
+                               "l"(p.c_in + (size_t)row * H + rank * 64 + 8 * n8 + 2 * (lane & 3)) : "memory");
+        }
+        asm volatile("cp.async.commit_group;" ::: "memory");
+    }
     float part[2][5] = {{0.f, 0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f, 0.f}};
 
     if (wg == 2) {
         if (threadIdx.x == 256) {
-            for (int kb = 0; kb < num_kb; ++kb) {
+            for (int kb = 0; kb < (TB2_GEMM_ABLATE == 2 ? 1 : num_kb); ++kb) {
                 const int s = kb % kGtStages;
                 const uint32_t phase = (kb / kGtStages) & 1;
                 mbar_wait(smem_u32(&empty_bar[s]), phase ^ 1);
@@ -124,15 +150,9 @@ lstm_gates_tc_kernel(const __grid_constant__ CUtensorMap map_emb_hi, const __gri
                 mbar_expect_tx(bar, kGtStageBytes);
                 const CUtensorMap *ahi, *alo;
                 int ka;
-                if constexpr (kGoal) {
-                    if (kb < kb_emb) { ahi = &map_emb_hi; alo = &map_emb_lo; ka = kb * kGtBK; }
-                    else if (kb < kb_emb + kb_pool) { ahi = &map_pool_hi; alo = &map_pool_lo; ka = (kb - kb_emb) * kGtBK; }
-                    else { ahi = &map_h_hi; alo = &map_h_lo; ka = (kb - kb_emb - kb_pool) * kGtBK; }
-                } else {
-                    if (kb == 0) { ahi = &map_emb_hi; alo = &map_emb_lo; ka = 0; }
-                    else if (kb <= kb_pool) { ahi = &map_pool_hi; alo = &map_pool_lo; ka = (kb - 1) * kGtBK; }
-                    else { ahi = &map_h_hi; alo = &map_h_lo; ka = (kb - 1 - kb_pool) * kGtBK; }
-                }
+                if (kb < kb_emb) { ahi = &map_emb_hi; alo = &map_emb_lo; ka = kb * kGtBK; }
+                else if (kb < kb_emb + kb_pool) { ahi = &map_pool_hi; alo = &map_pool_lo; ka = (kb - kb_emb) * kGtBK; }
+                else { ahi = &map_h_hi; alo = &map_h_lo; ka = (kb - kb_emb - kb_pool) * kGtBK; }
                 tma_load_2d(base, ahi, bar, ka, m0);
                 tma_load_2d(base + kGtABytes, alo, bar, ka, m0);
                 tma_load_2d(base + 2 * kGtABytes, &map_w_hi, bar, kb * kGtBK, rank * kGtBN);
@@ -144,40 +164,48 @@ lstm_gates_tc_kernel(const __grid_constant__ CUtensorMap map_emb_hi, const __gri
         float acc[kGtBN / 2];
 #pragma unroll
         for (int i = 0; i < kGtBN / 2; ++i) acc[i] = 0.f;
-        const uint32_t a_off = (uint32_t)wg * 64 * 128;
+        const uint32_t a_off = (uint32_t)wg * 64 * 2 * kGtBK;    // this warpgroup's 64 rows of the A tiles
         for (int kb = 0; kb < num_kb; ++kb) {
-            const int s = kb % kGtStages;
-            const uint32_t phase = (kb / kGtStages) & 1;
+            const int s = TB2_GEMM_ABLATE == 2 ? 0 : kb % kGtStages;
+            const uint32_t phase = TB2_GEMM_ABLATE == 2 ? 0 : (kb / kGtStages) & 1;
             mbar_wait(smem_u32(&full_bar[s]), phase);
             const uint32_t base = ring + s * kGtStageBytes;
-            const uint64_t a_hi = wgmma_desc(base + a_off);
-            const uint64_t a_lo = wgmma_desc(base + kGtABytes + a_off);
-            const uint64_t b_hi = wgmma_desc(base + 2 * kGtABytes);
-            const uint64_t b_lo = wgmma_desc(base + 2 * kGtABytes + kGtBBytes);
+            const uint64_t a_hi = wgmma_desc<2 * kGtBK>(base + a_off);
+            const uint64_t a_lo = wgmma_desc<2 * kGtBK>(base + kGtABytes + a_off);
+            const uint64_t b_hi = wgmma_desc<2 * kGtBK>(base + 2 * kGtABytes);
+            const uint64_t b_lo = wgmma_desc<2 * kGtBK>(base + 2 * kGtABytes + kGtBBytes);
             wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < kGtBK / 16; ++k) {
+            for (int k = 0; k < (TB2_GEMM_ABLATE == 1 ? 0 : kGtBK / 16); ++k) {
                 const uint64_t adv = (uint64_t)((k * 16 * 2) >> 4);
                 wgmma_bf16(acc, a_hi + adv, b_hi + adv, (kb | k) != 0);
                 wgmma_bf16(acc, a_hi + adv, b_lo + adv, 1u);
                 wgmma_bf16(acc, a_lo + adv, b_hi + adv, 1u);
             }
             wgmma_commit();
-            wgmma_wait_all();
+#if TB2_GEMM_ABLATE == 4
+            wgmma_wait<1>();
+            if (kb > 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[(kb - 1) % kGtStages]));
+#else
+            wgmma_wait<0>();
             if (lane == 0) mbar_arrive(smem_u32(&empty_bar[s]));
+#endif
         }
+        wgmma_wait<0>();
+        asm volatile("cp.async.wait_group 0;" ::: "memory");       // this thread's c_s slots and its rows' obs_s
+        asm volatile("bar.sync 1, 256;" ::: "memory");             // obs_s rows copied by the other threads of a quad
         // gate g of unit u = 8 n8 + 2 (lane % 4) + j, row rl + 8 hr: acc[4 (8 g + n8) + 2 hr + j]
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
             const int row = m0 + rl + 8 * hr;
-            if (row >= p.M) continue;
-            const float2 o1 = p.obs1[row], o2 = p.obs2[row];
+            if (row >= p.M || (TB2_GEMM_ABLATE == 3 && p.M > 0)) continue;
+            const float2 o1 = obs_s[rl + 8 * hr][0], o2 = obs_s[rl + 8 * hr][1];
             const bool masked = isnan(o1.x) || isnan(o2.x);                  // lstm.py:118
 #pragma unroll
             for (int n8 = 0; n8 < 8; ++n8) {
                 const int u = 8 * n8 + 2 * (lane & 3);
                 const size_t o = (size_t)row * H + rank * 64 + u;
-                float2 c = *reinterpret_cast<const float2*>(p.c_in + o);
+                float2 c = c_s[8 * hr + n8][threadIdx.x];
                 float2 h;
                 if (!masked) {
                     float cn[2], hn[2];
@@ -245,9 +273,9 @@ lstm_gates_tc_kernel(const __grid_constant__ CUtensorMap map_emb_hi, const __gri
 #pragma unroll
         for (int hr = 0; hr < 2; ++hr) {
             const int row = m0 + rl + 8 * hr;
-            if (row >= p.M) continue;
+            if (row >= p.M || (TB2_GEMM_ABLATE == 3 && p.M > 0)) continue;
             float* no = p.normal_out + (size_t)row * 5;
-            const float2 o1 = p.obs1[row], o2 = p.obs2[row];
+            const float2 o1 = obs_s[rl + 8 * hr][0], o2 = obs_s[rl + 8 * hr][1];
             if (isnan(o1.x) || isnan(o2.x)) {
 #pragma unroll
                 for (int q = 0; q < 5; ++q) no[q] = CUDART_NAN_F;
@@ -333,12 +361,13 @@ __global__ void repack_gates_tc_kernel(const float* __restrict__ w_ih, const flo
     }
 }
 
-int make_bf16_tile_map(CUtensorMap* map, const void* base, int rows, int cols, int box_rows);
+int make_bf16_tile_map(CUtensorMap* map, const void* base, int rows, int cols, int box_rows, int box_cols);
 
+// the segments are whole multiples of 64 columns (two k-blocks), the widths the kernel has always taken
 bool gates_tc_supported(const tb2_lstm* m) {
-    if (m->H % 64 != 0 || m->E != 64 || (m->E + m->G) % kGtBK != 0) return false;
+    if (m->H % 64 != 0 || m->E != 64 || (m->E + m->G) % 64 != 0) return false;
     if (m->cfg.pool_type != TB2_POOL_NONE && !m->cfg.pool_to_input) return false;
-    if (m->P % kGtBK != 0) return false;
+    if (m->P % 64 != 0) return false;
     return true;
 }
 
@@ -396,19 +425,19 @@ int launch_gates_tc(const tb2_lstm* m, const tb2_layout* l, int phase, const flo
     const int M = l->M;
     CUtensorMap me_hi, me_lo, mp_hi, mp_lo, mh_hi, mh_lo, mw_hi, mw_lo;
     int rc;
-    if ((rc = make_bf16_tile_map(&me_hi, emb_hi, M, 64 + m->G, kGtBM))) return rc;
-    if ((rc = make_bf16_tile_map(&me_lo, emb_lo, M, 64 + m->G, kGtBM))) return rc;
+    if ((rc = make_bf16_tile_map(&me_hi, emb_hi, M, 64 + m->G, kGtBM, kGtBK))) return rc;
+    if ((rc = make_bf16_tile_map(&me_lo, emb_lo, M, 64 + m->G, kGtBM, kGtBK))) return rc;
     if (m->P > 0) {
-        if ((rc = make_bf16_tile_map(&mp_hi, pool_hi, M, m->P, kGtBM))) return rc;
-        if ((rc = make_bf16_tile_map(&mp_lo, pool_lo, M, m->P, kGtBM))) return rc;
+        if ((rc = make_bf16_tile_map(&mp_hi, pool_hi, M, m->P, kGtBM, kGtBK))) return rc;
+        if ((rc = make_bf16_tile_map(&mp_lo, pool_lo, M, m->P, kGtBM, kGtBK))) return rc;
     } else {
         mp_hi = me_hi;
         mp_lo = me_lo;
     }
-    if ((rc = make_bf16_tile_map(&mh_hi, hs_in_hi, M, m->H, kGtBM))) return rc;
-    if ((rc = make_bf16_tile_map(&mh_lo, hs_in_lo, M, m->H, kGtBM))) return rc;
-    if ((rc = make_bf16_tile_map(&mw_hi, m->Wg_hi[phase], 4 * m->H, m->K_gate, kGtBN))) return rc;
-    if ((rc = make_bf16_tile_map(&mw_lo, m->Wg_lo[phase], 4 * m->H, m->K_gate, kGtBN))) return rc;
+    if ((rc = make_bf16_tile_map(&mh_hi, hs_in_hi, M, m->H, kGtBM, kGtBK))) return rc;
+    if ((rc = make_bf16_tile_map(&mh_lo, hs_in_lo, M, m->H, kGtBM, kGtBK))) return rc;
+    if ((rc = make_bf16_tile_map(&mw_hi, m->Wg_hi[phase], 4 * m->H, m->K_gate, kGtBN, kGtBK))) return rc;
+    if ((rc = make_bf16_tile_map(&mw_lo, m->Wg_lo[phase], 4 * m->H, m->K_gate, kGtBN, kGtBK))) return rc;
     GateTcParams p;
     p.obs1 = (const float2*)obs1;
     p.obs2 = (const float2*)obs2;

@@ -55,6 +55,7 @@ dense_layer_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid
     extern __shared__ __align__(1024) unsigned char smem_tc[];
     __shared__ __align__(8) uint64_t full_bar[kTcStages];
     __shared__ __align__(8) uint64_t empty_bar[kTcStages];
+    __shared__ float bias_s[kTcBN];
 
     const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int m0 = blockIdx.y * kTcBM, n0 = blockIdx.x * kTcBN;
@@ -79,7 +80,7 @@ dense_layer_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid
 
     if (wg == 2) {
         if (threadIdx.x == 256) {
-            for (int kb = 0; kb < num_kb; ++kb) {
+            for (int kb = 0; kb < (TB2_GEMM_ABLATE == 2 ? 1 : num_kb); ++kb) {
                 const int s = kb % kTcStages;
                 const uint32_t phase = (kb / kTcStages) & 1;
                 mbar_wait(smem_u32(&empty_bar[s]), phase ^ 1);
@@ -94,13 +95,16 @@ dense_layer_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid
         }
         return;
     }
+    // the bias tile in shared memory: a global load in the epilogue waits its latency (it was issued after stores the
+    // compiler cannot rule out that it aliases)
+    if (threadIdx.x < kTcBN) bias_s[threadIdx.x] = p.bias[n0 + threadIdx.x];
     float acc[kTcBN / 2];
 #pragma unroll
     for (int i = 0; i < kTcBN / 2; ++i) acc[i] = 0.f;
     const uint32_t a_off = (uint32_t)wg * 64 * 128;        // this warpgroup's 64 rows of the A tiles
     for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = kb % kTcStages;
-        const uint32_t phase = (kb / kTcStages) & 1;
+        const int s = TB2_GEMM_ABLATE == 2 ? 0 : kb % kTcStages;
+        const uint32_t phase = TB2_GEMM_ABLATE == 2 ? 0 : (kb / kTcStages) & 1;
         mbar_wait(smem_u32(&full_bar[s]), phase);
         const uint32_t base = ring + s * kTcStageBytes;
         const uint64_t a_hi = wgmma_desc(base + a_off);
@@ -109,34 +113,67 @@ dense_layer_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid
         const uint64_t b_lo = wgmma_desc(base + 2 * kTcABytes + kTcBBytes);
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < kTcBK / 16; ++k) {
+        for (int k = 0; k < (TB2_GEMM_ABLATE == 1 ? 0 : kTcBK / 16); ++k) {
             const uint64_t adv = (uint64_t)((k * 16 * 2) >> 4);      // 32 bytes per K step
             wgmma_bf16(acc, a_hi + adv, b_hi + adv, (kb | k) != 0);
             wgmma_bf16(acc, a_hi + adv, b_lo + adv, 1u);
             wgmma_bf16(acc, a_lo + adv, b_hi + adv, 1u);
         }
         wgmma_commit();
-        wgmma_wait_all();
+#if TB2_GEMM_ABLATE == 4
+        wgmma_wait<1>();
+        if (kb > 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[(kb - 1) % kTcStages]));
+#else
+        wgmma_wait<0>();
         if (lane == 0) mbar_arrive(smem_u32(&empty_bar[s]));        // this warp no longer reads the stage
+#endif
     }
-    // epilogue from the accumulator fragment: per register pair, one row and two adjacent columns
-    const int row0 = m0 + wg * 64 + (warp & 3) * 16 + (lane >> 2);
-    const int col0 = n0 + 2 * (lane & 3);
+    wgmma_wait<0>();
+    asm volatile("bar.sync 1, 256;" ::: "memory");     // bias_s written, and every consumer is done with the ring
+    // epilogue: bias + ReLU (+ bf16 split) from the accumulator fragment (per register pair, one row and two adjacent
+    // columns) into row-major tiles in the ring, then whole rows out in 16-byte stores.  Stored from the fragment
+    // directly, a warp's store covers 16 or 32 bytes of each of 8 rows.  Row strides are padded by 32 bytes so that
+    // the 8 rows of a fragment store fall in different banks.
+    constexpr int kYStride = kTcBN + 8;                 // floats
+    constexpr int kHStride = kTcBN + 16;                // bf16
+    static_assert(kTcBM * (kYStride * 4 + 2 * kHStride * 2) <= kTcStages * kTcStageBytes, "output tiles fit the ring");
+    float* y_s = reinterpret_cast<float*>(smem_tc + (ring - smem_u32(smem_tc)));
+    uint32_t* hi_s = reinterpret_cast<uint32_t*>(y_s + kTcBM * kYStride);
+    uint32_t* lo_s = hi_s + kTcBM * kHStride / 2;
+    const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int c0 = 2 * (lane & 3);
 #pragma unroll
     for (int i = 0; i < kTcBN / 2; i += 2) {
-        const int gr = row0 + 8 * ((i >> 1) & 1);
-        const int gc = col0 + 8 * (i >> 2);
-        float v0 = acc[i] + p.bias[gc], v1 = acc[i + 1] + p.bias[gc + 1];
+        const int r = r0 + 8 * ((i >> 1) & 1);
+        const int c = c0 + 8 * (i >> 2);
+        float v0 = acc[i] + bias_s[c], v1 = acc[i + 1] + bias_s[c + 1];
         if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
-        if (gr >= p.M) continue;
-        const size_t yoff = (size_t)gr * p.N + gc;
-        if (p.Y) *reinterpret_cast<float2*>(p.Y + yoff) = make_float2(v0, v1);
-        if (p.Y_hi) {
-            const __nv_bfloat16 h0 = __float2bfloat16_rn(v0), h1 = __float2bfloat16_rn(v1);
-            *reinterpret_cast<uint32_t*>(p.Y_hi + yoff) = pack_bf16x2(__bfloat16_as_ushort(h0), __bfloat16_as_ushort(h1));
-            *reinterpret_cast<uint32_t*>(p.Y_lo + yoff) =
-                pack_bf16x2(__bfloat16_as_ushort(__float2bfloat16_rn(v0 - __bfloat162float(h0))),
-                            __bfloat16_as_ushort(__float2bfloat16_rn(v1 - __bfloat162float(h1))));
+        *reinterpret_cast<float2*>(y_s + r * kYStride + c) = make_float2(v0, v1);
+        const __nv_bfloat16 h0 = __float2bfloat16_rn(v0), h1 = __float2bfloat16_rn(v1);
+        hi_s[(r * kHStride + c) / 2] = pack_bf16x2(__bfloat16_as_ushort(h0), __bfloat16_as_ushort(h1));
+        lo_s[(r * kHStride + c) / 2] = pack_bf16x2(__bfloat16_as_ushort(__float2bfloat16_rn(v0 - __bfloat162float(h0))),
+                                                   __bfloat16_as_ushort(__float2bfloat16_rn(v1 - __bfloat162float(h1))));
+    }
+    asm volatile("bar.sync 1, 256;" ::: "memory");
+    if (TB2_GEMM_ABLATE == 3 && p.M > 0) return;
+    if (p.Y) {
+        constexpr int kChunks = kTcBN / 4;              // 16-byte chunks of a fp32 row
+        for (int q = threadIdx.x; q < kTcBM * kChunks; q += 256) {
+            const int r = q / kChunks, c = 4 * (q % kChunks);
+            if (m0 + r < p.M)
+                *reinterpret_cast<float4*>(p.Y + (size_t)(m0 + r) * p.N + n0 + c) =
+                    *reinterpret_cast<const float4*>(y_s + r * kYStride + c);
+        }
+    }
+    if (p.Y_hi) {
+        constexpr int kChunks = kTcBN / 8;              // 16-byte chunks of a bf16 row
+        for (int q = threadIdx.x; q < kTcBM * kChunks; q += 256) {
+            const int r = q / kChunks, c = 8 * (q % kChunks);
+            if (m0 + r < p.M) {
+                const size_t o = (size_t)(m0 + r) * p.N + n0 + c;
+                *reinterpret_cast<uint4*>(p.Y_hi + o) = *reinterpret_cast<const uint4*>(hi_s + (r * kHStride + c) / 2);
+                *reinterpret_cast<uint4*>(p.Y_lo + o) = *reinterpret_cast<const uint4*>(lo_s + (r * kHStride + c) / 2);
+            }
         }
     }
 }
@@ -161,16 +198,17 @@ static EncodeTiledFn encode_fn() {
     return fn;
 }
 
-// bf16 row-major [rows, cols] matrix, box = [box_rows, 64 cols], 128B swizzle
+// bf16 row-major [rows, cols] matrix, box = [box_rows, box_cols], box_cols = 64 (128B swizzle) or 32 (64B swizzle)
 // A descriptor depends on (address, shape, box) only, and the step kernels are launched with the same few operand
 // buffers over and over: a small per-thread direct-mapped cache keeps the driver's encode call (a few microseconds,
 // 12 per recurrence step) off the launch path.
-int make_bf16_tile_map(CUtensorMap* map, const void* base, int rows, int cols, int box_rows) {
-    struct Entry { const void* base; int rows, cols, box_rows; bool valid; CUtensorMap map; };
+int make_bf16_tile_map(CUtensorMap* map, const void* base, int rows, int cols, int box_rows, int box_cols) {
+    struct Entry { const void* base; int rows, cols, box_rows, box_cols; bool valid; CUtensorMap map; };
     static thread_local Entry cache[256] = {};
     const uintptr_t key = reinterpret_cast<uintptr_t>(base);
-    Entry& e = cache[((key >> 8) ^ (key >> 17) ^ (uintptr_t)(rows * 131 + cols * 7 + box_rows)) & 255];
-    if (e.valid && e.base == base && e.rows == rows && e.cols == cols && e.box_rows == box_rows) {
+    Entry& e = cache[((key >> 8) ^ (key >> 17) ^ (uintptr_t)(rows * 131 + cols * 7 + box_rows + box_cols)) & 255];
+    if (e.valid && e.base == base && e.rows == rows && e.cols == cols && e.box_rows == box_rows &&
+        e.box_cols == box_cols) {
         *map = e.map;
         return TB2_OK;
     }
@@ -178,13 +216,15 @@ int make_bf16_tile_map(CUtensorMap* map, const void* base, int rows, int cols, i
     if (!fn) { set_error("cuTensorMapEncodeTiled unavailable"); return TB2_ERR_CUDA; }
     cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
     cuuint64_t strides[1] = {(cuuint64_t)cols * 2};
-    cuuint32_t box[2] = {(cuuint32_t)kTcBK, (cuuint32_t)box_rows};
+    cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
     cuuint32_t estr[2] = {1, 1};
     CUresult r = fn(map, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                    CU_TENSOR_MAP_INTERLEAVE_NONE, box_cols == 64 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B,
+                    CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled failed (" + std::to_string((int)r) + ")"); return TB2_ERR_CUDA; }
-    e.base = base; e.rows = rows; e.cols = cols; e.box_rows = box_rows; e.map = *map; e.valid = true;
+    e.base = base; e.rows = rows; e.cols = cols; e.box_rows = box_rows; e.box_cols = box_cols; e.map = *map;
+    e.valid = true;
     return TB2_OK;
 }
 
@@ -210,11 +250,11 @@ int launch_dense_tc(const void* a_hi, const void* a_lo, const void* w_hi, const 
     TB2_REQUIRE(dense_tc_supported(K, N), "tensor-core dense layer needs K % 64 == 0 and N % 64 == 0");
     CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
     int rc;
-    if ((rc = make_bf16_tile_map(&ma_hi, a_hi, M, K, kTcBM))) return rc;
-    if ((rc = make_bf16_tile_map(&ma_lo, a_lo, M, K, kTcBM))) return rc;
+    if ((rc = make_bf16_tile_map(&ma_hi, a_hi, M, K, kTcBM, kTcBK))) return rc;
+    if ((rc = make_bf16_tile_map(&ma_lo, a_lo, M, K, kTcBM, kTcBK))) return rc;
     const int bn = (N % 128 == 0) ? 128 : 64;
-    if ((rc = make_bf16_tile_map(&mb_hi, w_hi, N, K, bn))) return rc;
-    if ((rc = make_bf16_tile_map(&mb_lo, w_lo, N, K, bn))) return rc;
+    if ((rc = make_bf16_tile_map(&mb_hi, w_hi, N, K, bn, kTcBK))) return rc;
+    if ((rc = make_bf16_tile_map(&mb_lo, w_lo, N, K, bn, kTcBK))) return rc;
     TcParams p;
     p.bias = bias;
     p.Y = Y;

@@ -2,14 +2,24 @@
 // warpgroup MMA (wgmma) on bf16 operands in 128-byte-swizzled, K-major shared-memory tiles.
 //
 // Tile layout (written by TMA with CU_TENSOR_MAP_SWIZZLE_128B): rows of 64 bf16 (128 bytes),
-// 8-row atoms of 1024 bytes, so a tile must start on a 1024-byte boundary.  One wgmma consumes
-// K = 16 (32 bytes of a row); the next K step advances the descriptor's start address by 32 bytes.
+// 8-row atoms of 1024 bytes, so a tile must start on a 1024-byte boundary (SWIZZLE_64B: rows of 32
+// bf16, 512-byte atoms).  One wgmma consumes K = 16 (32 bytes of a row); the next K step advances
+// the descriptor's start address by 32 bytes.
 //
 // Accumulator fragment of wgmma.m64nNk16 (f32), thread t of the warpgroup, register i < N / 2:
 //   row = 16 * (t / 32) + (t % 32) / 4 + 8 * ((i / 2) % 2),   col = 8 * (i / 4) + 2 * (t % 4) + i % 2
 #pragma once
 #include <cuda.h>
 #include <stdint.h>
+
+// TB2_GEMM_ABLATE (scripts/step_gemm_ablate.py, timing only, results wrong) takes one part out of the mainloops of
+// dense_layer_tc and lstm_gates_tc: 1 = no wgmma (loads and barriers only), 2 = one stage loaded, every k-block reads
+// it (wgmma issue without the L2 operand stream), 3 = no epilogue stores (nor the arithmetic that feeds them),
+// 4 = one wgmma group in flight: wait_group 1 after committing k-block kb, then kb - 1's stage released.  Unset in
+// the library, which waits for each k-block's group before releasing its stage: the variant was no faster (DESIGN §8).
+#ifndef TB2_GEMM_ABLATE
+#define TB2_GEMM_ABLATE 0
+#endif
 
 namespace tb2 {
 
@@ -41,19 +51,24 @@ __device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map
         ::"r"(dst), "l"(map), "r"(bar), "r"(c0), "r"(c1) : "memory");
 }
 
-// wgmma shared-memory matrix descriptor: K-major, SWIZZLE_128B, stride byte offset 1024 B between
-// 8-row atoms (the leading byte offset is unused for swizzled K-major tiles)
+// wgmma shared-memory matrix descriptor: K-major rows of kRowBytes (128: SWIZZLE_128B, 64 bf16 a row; 64:
+// SWIZZLE_64B, 32 bf16 a row), stride byte offset 8 rows between 8-row atoms (the leading byte offset is unused for
+// swizzled K-major tiles)
+template <int kRowBytes = 128>
 __device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr) {
+    static_assert(kRowBytes == 128 || kRowBytes == 64, "128- or 64-byte swizzled rows");
     uint64_t d = 0;
     d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);          // start address, bits [0,14)
     d |= (uint64_t)1 << 16;                               // leading byte offset (unused)
-    d |= (uint64_t)(1024 >> 4) << 32;                     // stride byte offset, bits [32,46)
-    d |= (uint64_t)1 << 62;                               // layout type SWIZZLE_128B
+    d |= (uint64_t)(8 * kRowBytes >> 4) << 32;            // stride byte offset, bits [32,46)
+    d |= (uint64_t)(kRowBytes == 128 ? 1 : 2) << 62;      // layout type SWIZZLE_128B / SWIZZLE_64B
     return d;
 }
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// wait until at most N committed groups are still in flight
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
 // D[64, N] (+)= A[64, 16] . B[N, 16]^T, both operands bf16 K-major in shared memory, fp32 accumulate;
 // accumulate == 0 overwrites D.  Overloaded on N through the accumulator array (N / 2 registers).
