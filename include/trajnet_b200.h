@@ -59,14 +59,16 @@ extern "C" {
                                    * lstm.py:25-42,141-151): the caller runs it between the step's kernels.  out_dim = its
                                    * width; the library keeps no pool weights; pool_to_input 0 (out_dim == hidden_dim) or 1.
                                    * Only the step calls below serve it: tb2_pool_inputs_padded, the module,
-                                   * tb2_lstm_step_forward_pooled (tb2_lstm_step_backward for training).  tb2_pool_forward,
-                                   * tb2_lstm_step_forward(_goals), the sequence / steps calls and
-                                   * tb2_lstm_sequence_backward return TB2_ERR_INVALID; goals are not built with it */
+                                   * tb2_lstm_step_forward with pooled_padded_dev (tb2_lstm_step_backward for training).
+                                   * tb2_pool_forward, tb2_lstm_forward_steps and tb2_lstm_sequence_backward return
+                                   * TB2_ERR_INVALID; goals are not built with it */
 
 #define TB2_PHASE_ENCODER 0
 #define TB2_PHASE_DECODER 1
 
 const char* tb2_last_error(void);
+/* 106: one step call (tb2_lstm_step_forward) and one step-range call (tb2_lstm_forward_steps) take the goal, external
+ * module, sampling, training-cache and host-output arguments that separate entry points took before. */
 int tb2_version(void);
 /* Number of library kernel launches issued by this process so far (bench "gpu_launches"). */
 uint64_t tb2_launch_count(void);
@@ -105,7 +107,7 @@ typedef struct tb2_lstm_config {
     float attn_fill;         /* TB2_POOL_ATTN_MLP: fill_value of embed_with_masking (-10) */
     int32_t goal_dim;        /* LSTM(goal_flag=True): goal_dim, the width of the goal embedding appended to the
                               * input embedding (lstm.py:72-85,131-139); 0 = no goal input.  Inference only:
-                              * the training forward and the backward return TB2_ERR_UNSUPPORTED when it is set */
+                              * the training forward (cache_dev) and the backward return TB2_ERR_UNSUPPORTED */
 } tb2_lstm_config;
 
 /* Device pointers to the parameters in the reference's state_dict layout (row-major
@@ -204,105 +206,75 @@ int tb2_pool_forward(const tb2_lstm* model, const tb2_layout* layout, const floa
 /* One recurrence step: replaces LSTM.step (lstm.py:91-168).
  *   phase            TB2_PHASE_ENCODER / TB2_PHASE_DECODER (which LSTMCell)
  *   obs1_dev/obs2_dev [M, 2]
+ *   goals_dev        [M, 2] every track's goal (LSTM(goal_flag=True), lstm.py:131-139): each step feeds the LSTM
+ *                    [emb(velocity) | goal_emb | pooled] with goal_emb = cat(ReLU(W_g . 4 d + b_g), 0, 0),
+ *                    d = (obs2 - goal) / |obs2 - goal| (0 where that norm is 0).  Required when goal_dim > 0 (NULL:
+ *                    TB2_ERR_INVALID, the reference never substitutes zero goals), ignored otherwise.
+ *   pooled_padded_dev [B * n_pad, out_dim] the output of the caller's interaction module (TB2_POOL_EXTERNAL, see the
+ *                    external-module section below): required by such a model, NULL for any other (TB2_ERR_INVALID).
+ *                    The row of every present track (pool_sample[track_mask_positions], lstm.py:148) is concatenated to
+ *                    the LSTM input (pool_to_input) or added to its hidden state (lstm.py:151).
  *   h_in/c_in -> h_out/c_out [M, H] (may alias); absent tracks keep their state
  *   normal_out_dev   [M, 5]  (mu_x, mu_y, sigma_x, sigma_y, rho), NaN rows for absent tracks
- *   pos_out_dev      [M, 2]  obs2 + mu (lstm.py:232,255), may be NULL */
+ *   pos_out_dev      [M, 2]  obs2 + mu (lstm.py:232,255), may be NULL
+ * An external model with goal_dim > 0 returns TB2_ERR_UNSUPPORTED. */
 int tb2_lstm_step_forward(const tb2_lstm* model, const tb2_layout* layout, int32_t phase,
-                          const float* obs1_dev, const float* obs2_dev,
-                          const float* h_in_dev, const float* c_in_dev,
-                          float* h_out_dev, float* c_out_dev,
+                          const float* obs1_dev, const float* obs2_dev, const float* goals_dev,
+                          const float* pooled_padded_dev,
+                          const float* h_in_dev, const float* c_in_dev, float* h_out_dev, float* c_out_dev,
                           float* normal_out_dev, float* pos_out_dev,
                           void* workspace_dev, size_t workspace_bytes, void* stream);
 
-/* Whole time loop: replaces LSTM.forward (lstm.py:170-264) including the decoder input rule
- * (lstm.py:240-250).
+/* Steps [first_step, last_step) of the time loop of LSTM.forward (lstm.py:170-264), including the decoder input rule
+ * (lstm.py:240-250); S = obs_length - 1 + n_decode steps in all, [0, S) is the whole forward.
  *   observed_dev  [obs_length, M, 2]
  *   truth_dev     [n_decode, M, 2] teacher-forcing positions (prediction_truth) or NULL for a
  *                 free-running rollout (n_predict = n_decode + 1)
- *   normals_out_dev   [S, M, 5],  S = obs_length - 1 + n_decode
- *   positions_out_dev [S, M, 2]
- *   h_dev, c_dev  [M, H] state buffers: zeroed by the call, hold the final state on return.
- *   states_out_dev optional [S, 2, M, H] (h, c after every step; training) or NULL. */
-int tb2_lstm_forward_sequence(const tb2_lstm* model, const tb2_layout* layout,
-                              const float* observed_dev, int32_t obs_length,
-                              const float* truth_dev, int32_t n_decode,
-                              float* normals_out_dev, float* positions_out_dev,
-                              float* h_dev, float* c_dev, float* states_out_dev,
-                              void* workspace_dev, size_t workspace_bytes, void* stream);
-
-/* The same time loop for callers whose results live in HOST memory (the reference's predictor / evaluator
- * boundary hands numpy arrays back): after every recurrence step the step's slices of normals / positions are
- * copied to the pinned host buffers on `copy_stream`, ordered behind the step by an event, while the later
- * steps compute -- the device-to-host traffic (S x M x 28 bytes) hides under the forward instead of following
- * it.  The call does not synchronise: results are complete once `copy_stream` is.  normals_host / positions_host
- * [S, M, 5] / [S, M, 2] must be page-locked; the device outputs are written as well. */
-int tb2_lstm_forward_sequence_host(tb2_lstm* model, const tb2_layout* layout,
-                                   const float* observed_dev, int32_t obs_length,
-                                   const float* truth_dev, int32_t n_decode,
-                                   float* normals_out_dev, float* positions_out_dev,
-                                   float* h_dev, float* c_dev,
-                                   void* workspace_dev, size_t workspace_bytes,
-                                   float* normals_host, float* positions_host,
-                                   void* stream, void* copy_stream);
-
-/* Steps [first_step, last_step) of the same time loop (S = obs_length - 1 + n_decode steps in all).
- * first_step = 0 starts from the zero state; otherwise h_dev / c_dev hold the state after step
- * first_step - 1 -- possibly edited by the caller in between, which is how the S-GAN generator
- * injects noise between encoder and decoder (sgan/sgan.py:200-221,373) -- and positions_out_dev
- * holds the positions of the earlier steps.  tb2_lstm_forward_sequence == steps [0, S). */
+ *   goals_dev     [M, 2] as in tb2_lstm_step_forward: required when goal_dim > 0, ignored otherwise
+ *   normals_out_dev   [S, M, 5],  positions_out_dev [S, M, 2]
+ *   h_dev, c_dev  [M, H] state buffers.  first_step = 0 zeroes them; otherwise they hold the state after step
+ *                 first_step - 1 -- possibly edited by the caller in between, which is how the S-GAN generator injects
+ *                 noise between encoder and decoder (sgan/sgan.py:200-221,373) -- and positions_out_dev holds the
+ *                 positions of the earlier steps.  They hold the final state on return.
+ *   states_out_dev optional [S, 2, M, H] (h, c after every step; training) or NULL.
+ * Options, each NULL when not used:
+ *   eps_dev       sampled forward (no reference counterpart: the reference feeds back the mean of every step's bivariate
+ *                 normal, lstm/lstm.py:232,255).  After every step s >= obs_length - 2 of the range (the last encoder
+ *                 step's output and every decoder step: the n_decode + 1 predicted positions) the step's position is
+ *                 replaced by a draw of its normal before anything reads it, so the draw is what the following steps
+ *                 are fed back:
+ *                   pos[s, m] += (sx e1, sy (rho e1 + sqrt(1 - rho^2) e2)),   (sx, sy, rho) = normals[s, m, 2:5],
+ *                   (e1, e2) = eps_dev[s - (obs_length - 2), m]
+ *                 eps_dev [n_decode + 1, M, 2] holds standard normal pairs aligned with the last n_decode + 1 steps.  A
+ *                 pair of exactly (0, 0) leaves the position bit-unchanged (all zeros: the bits of eps_dev = NULL);
+ *                 rows with NaN normals stay NaN.  A goal-conditioned model returns TB2_ERR_UNSUPPORTED.
+ *   cache_dev     training forward: keeps, per step, the grid-embedding records the social backward reads (winners,
+ *                 latent vectors, hidden1 and the pooled vector; reference: everything autograd saves inside
+ *                 GridBasedPooling.forward, lstm/gridbased_pooling.py:94-170,308-335).  Needs states_out_dev, the whole
+ *                 range [0, S) and cache_bytes >= tb2_lstm_train_cache_bytes(S) > 0 (TB2_ERR_INVALID otherwise); the
+ *                 buffer must stay untouched until tb2_lstm_sequence_backward has run.  A goal-conditioned model
+ *                 returns TB2_ERR_UNSUPPORTED.
+ *   normals_host, positions_host, copy_stream  (set together) host outputs, for callers whose results live in HOST
+ *                 memory (the reference's predictor / evaluator boundary hands numpy arrays back): after every step of
+ *                 the range the step's slices of normals / positions are copied to these page-locked buffers
+ *                 [S, M, 5] / [S, M, 2] on `copy_stream`, ordered behind the step by an event, while the later steps
+ *                 compute -- the device-to-host traffic (M x 28 bytes per step) hides under the forward instead of
+ *                 following it.  The call does not synchronise: results are complete once `copy_stream` is.  The
+ *                 device outputs are written as well.
+ * A TB2_POOL_EXTERNAL model returns TB2_ERR_INVALID: it runs step by step (tb2_lstm_step_forward). */
 int tb2_lstm_forward_steps(const tb2_lstm* model, const tb2_layout* layout,
-                           const float* observed_dev, int32_t obs_length,
-                           const float* truth_dev, int32_t n_decode, int32_t first_step, int32_t last_step,
-                           float* normals_out_dev, float* positions_out_dev,
-                           float* h_dev, float* c_dev, float* states_out_dev,
+                           const float* observed_dev, int32_t obs_length, const float* truth_dev, int32_t n_decode,
+                           const float* goals_dev, const float* eps_dev, int32_t first_step, int32_t last_step,
+                           float* normals_out_dev, float* positions_out_dev, float* h_dev, float* c_dev,
+                           float* states_out_dev, void* cache_dev, size_t cache_bytes,
+                           float* normals_host, float* positions_host, void* copy_stream,
                            void* workspace_dev, size_t workspace_bytes, void* stream);
 
-/* Goal-conditioned variants of the three calls above (LSTM(goal_flag=True), lstm.py:131-139).
- *   goals_dev [M, 2]  every track's goal, constant over the sequence.  Each step feeds the LSTM
- *                     [emb(velocity) | goal_emb | pooled] with goal_emb = cat(ReLU(W_g . 4 d + b_g), 0, 0),
- *                     d = (obs2 - goal) / |obs2 - goal| (0 where that norm is 0).
- * A model with goal_dim > 0 needs goals_dev: NULL returns TB2_ERR_INVALID (the reference never
- * substitutes zero goals), and so do the goal-less calls above, which forward here with NULL.
- * With goal_dim == 0 goals_dev is ignored. */
-int tb2_lstm_step_forward_goals(const tb2_lstm* model, const tb2_layout* layout, int32_t phase,
-                                const float* obs1_dev, const float* obs2_dev, const float* goals_dev,
-                                const float* h_in_dev, const float* c_in_dev,
-                                float* h_out_dev, float* c_out_dev,
-                                float* normal_out_dev, float* pos_out_dev,
-                                void* workspace_dev, size_t workspace_bytes, void* stream);
-int tb2_lstm_forward_steps_goals(const tb2_lstm* model, const tb2_layout* layout,
-                                 const float* observed_dev, int32_t obs_length,
-                                 const float* truth_dev, int32_t n_decode, const float* goals_dev,
-                                 int32_t first_step, int32_t last_step,
-                                 float* normals_out_dev, float* positions_out_dev,
-                                 float* h_dev, float* c_dev, float* states_out_dev,
-                                 void* workspace_dev, size_t workspace_bytes, void* stream);
-int tb2_lstm_forward_sequence_host_goals(tb2_lstm* model, const tb2_layout* layout,
-                                         const float* observed_dev, int32_t obs_length,
-                                         const float* truth_dev, int32_t n_decode, const float* goals_dev,
-                                         float* normals_out_dev, float* positions_out_dev,
-                                         float* h_dev, float* c_dev,
-                                         void* workspace_dev, size_t workspace_bytes,
-                                         float* normals_host, float* positions_host,
-                                         void* stream, void* copy_stream);
+/* Bytes of the training cache (cache_dev of tb2_lstm_forward_steps) for num_steps steps: > 0 for every social model
+ * the backward supports and 0 for the other models, which keep no cache (pass NULL / 0). */
+size_t tb2_lstm_train_cache_bytes(const tb2_lstm* model, const tb2_layout* layout, int32_t num_steps);
 
-/* Sampled forward (no reference counterpart: the reference feeds back the mean of every step's bivariate normal,
- * lstm/lstm.py:232,255).  tb2_lstm_forward_steps, and after every step s >= obs_length - 2 of the range (the last
- * encoder step's output and every decoder step: the n_decode + 1 predicted positions) the step's position is replaced
- * by a draw of its normal before anything reads it, so the draw is what the following steps are fed back:
- *   pos[s, m] += (sx e1, sy (rho e1 + sqrt(1 - rho^2) e2)),   (sx, sy, rho) = normals[s, m, 2:5],
- *   (e1, e2) = eps_dev[s - (obs_length - 2), m]
- * eps_dev [n_decode + 1, M, 2] holds standard normal pairs aligned with the last n_decode + 1 steps.  A pair of exactly
- * (0, 0) leaves the position bit-unchanged (all zeros: the bits of tb2_lstm_forward_steps); rows with NaN normals stay
- * NaN.  NULL eps_dev returns TB2_ERR_INVALID, a goal-conditioned model TB2_ERR_UNSUPPORTED. */
-int tb2_lstm_forward_steps_sampled(const tb2_lstm* model, const tb2_layout* layout,
-                                   const float* observed_dev, int32_t obs_length,
-                                   const float* truth_dev, int32_t n_decode, int32_t first_step, int32_t last_step,
-                                   const float* eps_dev, float* normals_out_dev, float* positions_out_dev,
-                                   float* h_dev, float* c_dev, float* states_out_dev,
-                                   void* workspace_dev, size_t workspace_bytes, void* stream);
-
-/* The sampling of tb2_lstm_forward_steps_sampled on one step's rows: positions [rows, 2] += the offset above from
+/* The sampling of tb2_lstm_forward_steps (eps_dev) on one step's rows: positions [rows, 2] += the offset above from
  * normals [rows, 5] and eps [rows, 2], in place.  The batched multi-mode decode applies it to the replicated output of
  * the last encoder step before the decoder steps run. */
 int tb2_lstm_sample_positions(const float* normals_dev, float* positions_dev, const float* eps_dev, int32_t rows,
@@ -354,16 +326,6 @@ int tb2_pool_inputs_padded(const tb2_layout* layout, const float* obs1_dev, cons
 /* Its backward: d_h_dev [M, H] += the rows of d_h_pad_dev [B, n_pad, H] at every track's slot (padding is dropped). */
 int tb2_pool_inputs_padded_backward(const tb2_layout* layout, const float* d_h_pad_dev, int32_t H, float* d_h_dev,
                                     void* stream);
-/* tb2_lstm_step_forward with the module's output pooled_padded_dev [B * n_pad, out_dim]: the row of every present track
- * (pool_sample[track_mask_positions], lstm.py:148) is concatenated to the LSTM input (pool_to_input) or added to its
- * hidden state (lstm.py:151); absent tracks keep their state as in tb2_lstm_step_forward.  h_out / c_out may alias
- * h_in / c_in. */
-int tb2_lstm_step_forward_pooled(const tb2_lstm* model, const tb2_layout* layout, int32_t phase,
-                                 const float* obs1_dev, const float* obs2_dev, const float* pooled_padded_dev,
-                                 const float* h_in_dev, const float* c_in_dev, float* h_out_dev, float* c_out_dev,
-                                 float* normal_out_dev, float* pos_out_dev, void* workspace_dev, size_t workspace_bytes,
-                                 void* stream);
-
 /* ---------------------------------------------------------------------------------------
  * Training: backward of the whole time loop (what autograd does for Trainer.train_batch,
  * lstm/trainer.py:229-269, through LSTM.forward).  Gradient accumulators are fp32 device
@@ -407,7 +369,7 @@ size_t tb2_lstm_backward_workspace_bytes(const tb2_lstm* model, const tb2_layout
 /* BPTT over the rows that receive gradient.
  *   weights          the same fp32 parameter pointers given to tb2_lstm_set_weights
  *   observed/truth   inputs of the forward call (truth: teacher forcing or NULL)
- *   positions_dev    [S, M, 2] and states_dev [S, 2, M, H]: outputs of tb2_lstm_forward_sequence
+ *   positions_dev    [S, M, 2] and states_dev [S, 2, M, H]: outputs of tb2_lstm_forward_steps
  *   d_normals_dev    [S, M, 5] upstream gradient wrt rel_pred_scene (d pred_scene already added to
  *                    its first two columns by the caller: pred = obs2 + mu, lstm.py:232,255)
  *   active_rows_dev  int32 [num_active]: tracks with a non-zero upstream gradient (PredictionLoss
@@ -417,7 +379,7 @@ size_t tb2_lstm_backward_workspace_bytes(const tb2_lstm* model, const tb2_layout
  * Social pooling couples all tracks of a scene through the hidden-state scatter (the reference
  * does not detach hidden_states_to_pool, lstm.py:26): the backward then runs on all M rows and
  * active_rows is ignored.
- *   cache_dev        the training cache tb2_lstm_forward_sequence_train filled (social pooling; without it
+ *   cache_dev        the training cache tb2_lstm_forward_steps filled (social pooling; without it
  *                    the call returns TB2_ERR_INVALID).  Other models have none: NULL / 0. */
 int tb2_lstm_sequence_backward(const tb2_lstm* model, const tb2_layout* layout, const tb2_lstm_weights* weights,
                                const float* observed_dev, int32_t obs_length, const float* truth_dev,
@@ -427,7 +389,7 @@ int tb2_lstm_sequence_backward(const tb2_lstm* model, const tb2_layout* layout, 
                                void* bwd_workspace_dev, size_t bwd_workspace_bytes, const void* cache_dev,
                                size_t cache_bytes, void* stream);
 
-/* Backward of one tb2_lstm_step_forward_pooled step (TB2_POOL_EXTERNAL), from the step's inputs: the gate
+/* Backward of one tb2_lstm_step_forward step of a TB2_POOL_EXTERNAL model, from the step's inputs: the gate
  * pre-activations are recomputed (one GEMM), then
  *   d_h_in_dev, d_c_in_dev  [M, H]                gradient wrt h_in / c_in (absent tracks: d_h_out / d_c_out unchanged)
  *   d_pooled_padded_dev     [B * n_pad, out_dim]  gradient wrt pooled_padded (0 for absent tracks and padding slots)
@@ -445,23 +407,11 @@ int tb2_lstm_step_backward(const tb2_lstm* model, const tb2_layout* layout, cons
                            size_t bwd_workspace_bytes, void* stream);
 
 /* TB2_POOL_NN_LSTM / TB2_POOL_TRAJECTRON: zero the interaction-encoder LSTM state kept in `workspace`
- * (NearestNeighborLSTM.reset, non_gridbased_pooling.py:385-389; TrajectronPooling.reset, :481-485).  tb2_lstm_forward_sequence / _steps(first_step = 0) do this themselves; the
+ * (NearestNeighborLSTM.reset, non_gridbased_pooling.py:385-389; TrajectronPooling.reset, :481-485).  tb2_lstm_forward_steps(first_step = 0) does this itself; the
  * stand-alone plug (tb2_pool_forward) advances the state on every call and needs it after a reset().  No-op for the
  * other pool types. */
 int tb2_pool_state_reset(const tb2_lstm* model, const tb2_layout* layout, void* workspace_dev, size_t workspace_bytes,
                          void* stream);
-
-/* Training forward: keeps, per step, the grid-embedding records the social backward reads (winners, latent vectors,
- * hidden1 and the pooled vector; reference: everything autograd saves inside GridBasedPooling.forward,
- * lstm/gridbased_pooling.py:94-170,308-335).  tb2_lstm_train_cache_bytes is > 0 for every social model the backward
- * supports and 0 for the other models, which keep no cache (pass NULL / 0); `cache` is a caller-owned device buffer
- * that must stay untouched until tb2_lstm_sequence_backward has run. */
-size_t tb2_lstm_train_cache_bytes(const tb2_lstm* model, const tb2_layout* layout, int32_t num_steps);
-int tb2_lstm_forward_sequence_train(const tb2_lstm* model, const tb2_layout* layout, const float* observed_dev,
-                                    int32_t obs_length, const float* truth_dev, int32_t n_decode, float* normals_out_dev,
-                                    float* positions_out_dev, float* h_dev, float* c_dev, float* states_out_dev,
-                                    void* cache_dev, size_t cache_bytes, void* workspace_dev, size_t workspace_bytes,
-                                    void* stream);
 
 /* PredictionLoss on the device (lstm/loss.py:52-91, gaussian_2d :24-50): per (frame, scene)
  *   values_out  [T, B]    = -log(0.01 + bg N(x|mu,3,3,0) + (0.99-bg) N(x|mu,s1,s2,rho)) of the primary

@@ -26,6 +26,45 @@ def test_library_builds_and_exports_header_symbols():
     assert lib.tb2_version() >= 100
 
 
+# size_t and uint64_t are the same 64-bit unsigned type on the platforms the library builds for (ctypes.c_size_t is
+# ctypes.c_uint64 there)
+_C_KINDS = {"int": "int32", "int32_t": "int32", "int64_t": "int64", "size_t": "size_t", "uint64_t": "size_t",
+            "float": "float", "double": "double"}
+
+
+def _c_kind(c_type):
+    return "pointer" if "*" in c_type else _C_KINDS[c_type.replace("const", "").strip()]
+
+
+def _ctypes_kind(t):
+    import ctypes
+    if t in (ctypes.c_void_p, ctypes.c_char_p) or issubclass(t, ctypes._Pointer):
+        return "pointer"
+    for kind, c in (("int32", ctypes.c_int32), ("int64", ctypes.c_int64), ("size_t", ctypes.c_size_t),
+                    ("float", ctypes.c_float), ("double", ctypes.c_double)):
+        if t is c:
+            return kind
+    return repr(t)
+
+
+def test_prototypes_match_header_declarations():
+    """Every ctypes prototype passes its function's arguments, and takes its result, as the header declares them: the
+    same number, and per position a pointer or a scalar of the same width and type.  A shifted argument would reach
+    the library as a garbage pointer."""
+    from trajnetplusplusbaselines_b200 import _lib
+    text = open(os.path.join(ROOT, "include", "trajnet_b200.h")).read()
+    text = re.sub(r"^#.*$", "", re.sub(r"/\*.*?\*/", "", text, flags=re.S), flags=re.M)
+    decls = re.findall(r"([^;{}()]*?)\b(tb2_[a-z0-9_]+)\s*\(([^()]*)\)\s*;", text)
+    assert sorted(name for _, name, _ in decls) == _declared()
+    for ret, name, params in decls:
+        params = [] if params.strip() == "void" else [re.sub(r"\w+\s*$", "", p) for p in params.split(",")]
+        restype, argtypes = _lib.PROTOTYPES[name]
+        assert len(argtypes) == len(params), (name, len(argtypes), len(params))
+        assert _ctypes_kind(restype) == _c_kind(ret), name
+        for i, (t, p) in enumerate(zip(argtypes, params)):
+            assert _ctypes_kind(t) == _c_kind(p), (name, i, p)
+
+
 def test_no_cpu_fallback_without_cuda():
     import torch
     if torch.cuda.is_available():

@@ -396,21 +396,17 @@ def test_goal_calls_without_goals_are_refused():
     h, c = torch.empty((M, 128), **f32), torch.empty((M, 128), **f32)
     normal = torch.empty((M, 5), **f32)
     stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    assert lib.tb2_lstm_step_forward_goals(handle.handle, layout.handle, 0, _ptr(obs[0]), _ptr(obs[1]), None, _ptr(h),
-                                           _ptr(c), _ptr(h), _ptr(c), _ptr(normal), None, _ptr(ws), need, stream) == -1
+    assert lib.tb2_lstm_step_forward(handle.handle, layout.handle, 0, _ptr(obs[0]), _ptr(obs[1]), None, None, _ptr(h),
+                                     _ptr(c), _ptr(h), _ptr(c), _ptr(normal), None, _ptr(ws), need, stream) == -1
     assert b"goals_dev" in lib.tb2_last_error()
-    assert lib.tb2_lstm_forward_steps_goals(handle.handle, layout.handle, _ptr(obs), 9, None, 11, None, 0, 19,
-                                            _ptr(normals), _ptr(positions), _ptr(h), _ptr(c), None, _ptr(ws), need,
-                                            stream) == -1
+    assert lib.tb2_lstm_forward_steps(handle.handle, layout.handle, _ptr(obs), 9, None, 11, None, None, 0, 19,
+                                      _ptr(normals), _ptr(positions), _ptr(h), _ptr(c), None, None, 0, None, None, None,
+                                      _ptr(ws), need, stream) == -1
     host_n, host_p = torch.empty((19, M, 5), pin_memory=True), torch.empty((19, M, 2), pin_memory=True)
     side = torch.cuda.Stream()
-    assert lib.tb2_lstm_forward_sequence_host_goals(handle.handle, layout.handle, _ptr(obs), 9, None, 11, None,
-                                                    _ptr(normals), _ptr(positions), _ptr(h), _ptr(c), _ptr(ws), need,
-                                                    _ptr(host_n), _ptr(host_p), stream,
-                                                    ctypes.c_void_p(side.cuda_stream)) == -1
-    # the goal-less entry points forward without goals: refused too
-    assert lib.tb2_lstm_forward_sequence(handle.handle, layout.handle, _ptr(obs), 9, None, 11, _ptr(normals),
-                                         _ptr(positions), _ptr(h), _ptr(c), None, _ptr(ws), need, stream) == -1
+    assert lib.tb2_lstm_forward_steps(handle.handle, layout.handle, _ptr(obs), 9, None, 11, None, None, 0, 19,
+                                      _ptr(normals), _ptr(positions), _ptr(h), _ptr(c), None, None, 0, _ptr(host_n),
+                                      _ptr(host_p), ctypes.c_void_p(side.cuda_stream), _ptr(ws), need, stream) == -1
     with pytest.raises(ValueError, match="needs the goals"):
         with torch.no_grad():
             model(obs.cpu(), None, torch.from_numpy(bs), n_predict=12)

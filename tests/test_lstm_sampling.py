@@ -1,5 +1,5 @@
 """Sampled multi-modal predictions of LSTM models (trajnetplusplusbaselines_b200/lstm/sampling.py, sample_positions_kernel
-in csrc/sgan.cu, tb2_lstm_forward_steps_sampled / tb2_lstm_sample_positions).
+in csrc/sgan.cu, tb2_lstm_forward_steps with eps_dev / tb2_lstm_sample_positions).
 
 Mode q >= 1 draws every predicted position from its step's bivariate normal,
 pos = obs2 + mu + (sx e1, sy (rho e1 + sqrt(1 - rho^2) e2)), and feeds that draw back; mode 0 (e = 0) is the mean.
@@ -247,7 +247,7 @@ def _edge_margin(cfg, pos, bs):
 @pytest.mark.parametrize("tc", [True, False], ids=["tc", "no_tc"])
 @pytest.mark.parametrize("kind", KINDS)
 def test_random_eps_matches_float64_restatement(monkeypatch, kind, tc):
-    """The sampled forward (tb2_lstm_forward_steps_sampled over a ragged per-scene layout) against torch_ref.forward
+    """The sampled forward (tb2_lstm_forward_steps with eps_dev over a ragged per-scene layout) against torch_ref.forward
     fed the GPU's positions, with the offset of its own float64 normals at the same eps added to every predicted
     position."""
     _set_tc(monkeypatch, tc)
@@ -299,7 +299,8 @@ def test_random_eps_matches_float64_restatement(monkeypatch, kind, tc):
 @pytest.mark.gpu
 def test_sample_positions_kernel_and_refusals():
     """tb2_lstm_sample_positions: the offset in place; a (0, 0) pair keeps the bits (signed zeros too); NaN normals stay
-    NaN.  NULL eps and a goal-conditioned model are refused."""
+    NaN.  A sampled forward of a goal-conditioned model is refused; NULL eps is the mean forward, bit for bit that of
+    all-zero eps."""
     from trajnetplusplusbaselines_b200 import _lib
     from trajnetplusplusbaselines_b200.engine import _ptr, _stream
     from trajnetplusplusbaselines_b200.lstm import LSTM
@@ -332,15 +333,19 @@ def test_sample_positions_kernel_and_refusals():
     ws, need = seq.handle.workspace(seq.layout)
 
     def call(e):
-        return lib.tb2_lstm_forward_steps_sampled(seq.handle.handle, seq.layout.handle, _ptr(seq.obs), 9, _ptr(None),
-                                                  11, 0, seq.S, _ptr(e), _ptr(seq.normals), _ptr(seq.positions),
-                                                  _ptr(seq.h), _ptr(seq.c), _ptr(None), _ptr(ws), need, stream)
+        return lib.tb2_lstm_forward_steps(seq.handle.handle, seq.layout.handle, _ptr(seq.obs), 9, _ptr(None), 11,
+                                          _ptr(None), _ptr(e), 0, seq.S, _ptr(seq.normals), _ptr(seq.positions),
+                                          _ptr(seq.h), _ptr(seq.c), _ptr(None), _ptr(None), 0, _ptr(None), _ptr(None),
+                                          _ptr(None), _ptr(ws), need, stream)
     assert call(eps) == -3 and b"goal" in lib.tb2_last_error()          # TB2_ERR_UNSUPPORTED
     plain, _ = _model("vanilla")
     seq = plain._sequence(xy, torch.tensor([0, 3]), None, 12)
     ws, need = seq.handle.workspace(seq.layout)
-    assert call(None) == -1 and b"eps" in lib.tb2_last_error()          # TB2_ERR_INVALID
+    assert call(None) == 0                                              # the mean forward
+    mean = seq.positions.clone(), seq.normals.clone()
     assert call(eps) == 0
+    for a, b in zip(mean, (seq.positions, seq.normals)):
+        assert np.array_equal(a.cpu().numpy().view(np.uint32), b.cpu().numpy().view(np.uint32))
 
 
 # ------------------------------------------------------------------------------------------------------------------

@@ -222,7 +222,7 @@ def test_social_backward_without_cache_is_refused(monkeypatch):
     rel, _ = model(scene[:obs_length], torch.zeros(xy.shape[1], 2), batch_split, scene[obs_length:-1].clone())
     targets = scene[obs_length:obs_length + pred_length] - scene[obs_length - 1:obs_length + pred_length - 1]
     loss = PredictionLoss()(rel[-pred_length:], targets, batch_split)
-    with pytest.raises(RuntimeError, match=r"error -1: .*tb2_lstm_forward_sequence_train"):
+    with pytest.raises(RuntimeError, match=r"error -1: .*tb2_lstm_forward_steps call \(cache_dev\)"):
         loss.backward()
 
 

@@ -143,18 +143,9 @@ PROTOTYPES = {
     "tb2_lstm_workspace_bytes": (_sz, [_vp, _vp]),
     "tb2_grid_indices": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp]),
     "tb2_pool_forward": (ctypes.c_int, [_vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
-    "tb2_lstm_step_forward": (ctypes.c_int, [_vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
-    "tb2_lstm_forward_sequence": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
-    "tb2_lstm_forward_sequence_host": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _vp, _vp, _vp]),
-    "tb2_lstm_forward_steps": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp]),
-    "tb2_lstm_step_forward_goals": (ctypes.c_int, [_vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz,
-                                                   _vp]),
-    "tb2_lstm_forward_steps_goals": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _i32, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp,
-                                                    _vp, _sz, _vp]),
-    "tb2_lstm_forward_sequence_host_goals": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp,
-                                                            _sz, _vp, _vp, _vp, _vp]),
-    "tb2_lstm_forward_steps_sampled": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _i32, _i32, _i32, _vp, _vp, _vp, _vp, _vp,
-                                                      _vp, _vp, _sz, _vp]),
+    "tb2_lstm_step_forward": (ctypes.c_int, [_vp, _vp, _i32] + [_vp] * 11 + [_sz, _vp]),
+    "tb2_lstm_forward_steps": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _i32, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp,
+                                              _vp, _sz, _vp, _vp, _vp, _vp, _sz, _vp]),
     "tb2_lstm_sample_positions": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp]),
     "tb2_lstm_backward_workspace_bytes": (_sz, [_vp, _vp, _i32, _i32]),
     "tb2_lstm_sequence_backward": (ctypes.c_int, [_vp, _vp, ctypes.POINTER(LstmWeights), _vp, _i32, _vp, _i32,
@@ -163,13 +154,10 @@ PROTOTYPES = {
     "tb2_pool_state_reset": (ctypes.c_int, [_vp, _vp, _vp, _sz, _vp]),
     "tb2_pool_inputs_padded": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _vp, _vp, _vp, _vp]),
     "tb2_pool_inputs_padded_backward": (ctypes.c_int, [_vp, _vp, _i32, _vp, _vp]),
-    "tb2_lstm_step_forward_pooled": (ctypes.c_int, [_vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _vp, _sz,
-                                                    _vp]),
     "tb2_lstm_step_backward_workspace_bytes": (_sz, [_vp, _vp]),
     "tb2_lstm_step_backward": (ctypes.c_int, [_vp, _vp, ctypes.POINTER(LstmWeights), _i32, _vp, _vp, _vp, _vp, _vp, _vp,
                                               _vp, _vp, _vp, _vp, _vp, ctypes.POINTER(LstmGrads), _vp, _sz, _vp]),
     "tb2_lstm_train_cache_bytes": (_sz, [_vp, _vp, _i32]),
-    "tb2_lstm_forward_sequence_train": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _i32, _vp, _vp, _vp, _vp, _vp, _vp, _sz, _vp, _sz, _vp]),
     "tb2_sgan_add_noise": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp]),
     "tb2_vae_scale_hidden": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _i32, _i32, _vp]),
     "tb2_sgan_decoder_context": (ctypes.c_int, [_vp, _vp, _vp, _vp, _i32, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp]),

@@ -182,7 +182,7 @@ using namespace tb2;
 extern "C" {
 
 const char* tb2_last_error(void) { return g_error.c_str(); }
-int tb2_version(void) { return 105; }
+int tb2_version(void) { return 106; }
 uint64_t tb2_launch_count(void) { return g_launch_count.load(); }
 
 int tb2_profile_begin(void) {
@@ -612,26 +612,25 @@ static int resolve_goals(const tb2_lstm* m, const float** goals) {
         *goals = nullptr;
         return TB2_OK;
     }
-    TB2_REQUIRE(*goals, "the model has a goal embedding (goal_dim > 0): pass goals_dev [M, 2] through a *_goals call");
+    TB2_REQUIRE(*goals, "the model has a goal embedding (goal_dim > 0): pass goals_dev [M, 2]");
     return TB2_OK;
 }
 
 int tb2_lstm_step_forward(const tb2_lstm* m, const tb2_layout* l, int32_t phase, const float* obs1,
-                          const float* obs2, const float* h_in, const float* c_in, float* h_out,
-                          float* c_out, float* normal_out, float* pos_out, void* workspace,
-                          size_t workspace_bytes, void* stream) {
-    return tb2_lstm_step_forward_goals(m, l, phase, obs1, obs2, nullptr, h_in, c_in, h_out, c_out, normal_out, pos_out,
-                                       workspace, workspace_bytes, stream);
-}
-
-int tb2_lstm_step_forward_goals(const tb2_lstm* m, const tb2_layout* l, int32_t phase, const float* obs1,
-                                const float* obs2, const float* goals, const float* h_in, const float* c_in, float* h_out,
-                                float* c_out, float* normal_out, float* pos_out, void* workspace,
-                                size_t workspace_bytes, void* stream) {
+                          const float* obs2, const float* goals, const float* pooled_pad, const float* h_in,
+                          const float* c_in, float* h_out, float* c_out, float* normal_out, float* pos_out,
+                          void* workspace, size_t workspace_bytes, void* stream) {
     int rc = check_ready(m, l, workspace, workspace_bytes);
     if (rc) return rc;
-    TB2_REQUIRE(m->cfg.pool_type != TB2_POOL_EXTERNAL, kExternalPoolMessage);
+    const bool external = m->cfg.pool_type == TB2_POOL_EXTERNAL;
+    if (external && m->G > 0) {
+        set_error("goals with an external interaction module are not built");
+        return TB2_ERR_UNSUPPORTED;
+    }
     if ((rc = resolve_goals(m, &goals))) return rc;
+    TB2_REQUIRE(!pooled_pad == !external,
+                "pooled_padded_dev is the output of an external interaction module: required by a TB2_POOL_EXTERNAL "
+                "model, NULL for any other");
     TB2_REQUIRE(phase == TB2_PHASE_ENCODER || phase == TB2_PHASE_DECODER, "bad phase");
     TB2_REQUIRE(obs1 && obs2 && h_in && c_in && h_out && c_out && normal_out, "null argument");
     Workspace ws;
@@ -640,30 +639,7 @@ int tb2_lstm_step_forward_goals(const tb2_lstm* m, const tb2_layout* l, int32_t 
     if (m->Wg_hi[0] &&
         (rc = launch_split_bf16(h_in, ws.hs_hi[0], ws.hs_lo[0], (size_t)l->M * m->H, st)))
         return rc;
-    return step_impl(m, l, phase, obs1, obs2, goals, h_in, c_in, h_out, c_out, normal_out, pos_out, &ws, 0, st);
-}
-
-int tb2_lstm_step_forward_pooled(const tb2_lstm* m, const tb2_layout* l, int32_t phase, const float* obs1,
-                                 const float* obs2, const float* pooled_pad, const float* h_in, const float* c_in,
-                                 float* h_out, float* c_out, float* normal_out, float* pos_out, void* workspace,
-                                 size_t workspace_bytes, void* stream) {
-    int rc = check_ready(m, l, workspace, workspace_bytes);
-    if (rc) return rc;
-    TB2_REQUIRE(m->cfg.pool_type == TB2_POOL_EXTERNAL,
-                "tb2_lstm_step_forward_pooled serves external interaction modules (TB2_POOL_EXTERNAL)");
-    if (m->G > 0) {
-        set_error("goals with an external interaction module are not built");
-        return TB2_ERR_UNSUPPORTED;
-    }
-    TB2_REQUIRE(phase == TB2_PHASE_ENCODER || phase == TB2_PHASE_DECODER, "bad phase");
-    TB2_REQUIRE(obs1 && obs2 && pooled_pad && h_in && c_in && h_out && c_out && normal_out, "null argument");
-    Workspace ws;
-    carve_workspace(m, l, workspace, &ws);
-    cudaStream_t st = (cudaStream_t)stream;
-    if (m->Wg_hi[0] &&
-        (rc = launch_split_bf16(h_in, ws.hs_hi[0], ws.hs_lo[0], (size_t)l->M * m->H, st)))
-        return rc;
-    return step_impl(m, l, phase, obs1, obs2, nullptr, h_in, c_in, h_out, c_out, normal_out, pos_out, &ws, 0, st,
+    return step_impl(m, l, phase, obs1, obs2, goals, h_in, c_in, h_out, c_out, normal_out, pos_out, &ws, 0, st,
                      pooled_pad);
 }
 
@@ -671,29 +647,46 @@ int tb2_lstm_step_forward_pooled(const tb2_lstm* m, const tb2_layout* l, int32_t
 // (lstm.py:207-210); otherwise h / c hold the state after step first_step - 1 (possibly edited by
 // the caller, e.g. the noise injection of the S-GAN generator between encoder and decoder,
 // sgan/sgan.py:200-221,373) and positions_out holds the positions of the earlier steps.
-struct HostSink {              // optional: per-step device-to-host streaming of the outputs
-    float* normals_host;
-    float* positions_host;
-    cudaStream_t copy_stream;
-    std::vector<cudaEvent_t>* events;
-};
-
-static int forward_steps_impl(const tb2_lstm* m, const tb2_layout* l, const float* observed,
-                              int32_t obs_length, const float* truth, int32_t n_decode, const float* goals,
-                              int32_t first_step, int32_t last_step, float* normals_out, float* positions_out, float* h,
-                              float* c, float* states_out, void* workspace, size_t workspace_bytes, void* stream,
-                              const HostSink* sink, const TrainCache* cache = nullptr, const float* eps = nullptr) {
+int tb2_lstm_forward_steps(const tb2_lstm* m, const tb2_layout* l, const float* observed, int32_t obs_length,
+                           const float* truth, int32_t n_decode, const float* goals, const float* eps,
+                           int32_t first_step, int32_t last_step, float* normals_out, float* positions_out, float* h,
+                           float* c, float* states_out, void* cache_dev, size_t cache_bytes, float* normals_host,
+                           float* positions_host, void* copy_stream, void* workspace, size_t workspace_bytes,
+                           void* stream) {
     int rc = check_ready(m, l, workspace, workspace_bytes);
     if (rc) return rc;
+    TB2_REQUIRE(obs_length >= 2 && n_decode >= 0, "need obs_length >= 2 and n_decode >= 0");
     TB2_REQUIRE(m->cfg.pool_type != TB2_POOL_EXTERNAL, kExternalPoolMessage);
+    if (m->G > 0 && eps) {
+        set_error("sampled forwards of a goal-conditioned model (goal_dim > 0) are not built");
+        return TB2_ERR_UNSUPPORTED;
+    }
+    if (m->G > 0 && cache_dev) {
+        set_error("training a goal-conditioned model (goal_dim > 0) is not built");
+        return TB2_ERR_UNSUPPORTED;
+    }
     if ((rc = resolve_goals(m, &goals))) return rc;
     TB2_REQUIRE(observed && normals_out && positions_out && h && c, "null argument");
-    TB2_REQUIRE(obs_length >= 2 && n_decode >= 0, "need obs_length >= 2 and n_decode >= 0");
     const int S = obs_length - 1 + n_decode;
     TB2_REQUIRE(first_step >= 0 && first_step <= last_step && last_step <= S, "bad step range");
+    TB2_REQUIRE(!normals_host == !positions_host && !normals_host == !copy_stream,
+                "normals_host, positions_host and copy_stream are set together");
+    TrainCache cache;
+    if (cache_dev) {
+        TB2_REQUIRE(states_out && first_step == 0 && last_step == S,
+                    "a training forward (cache_dev) runs steps [0, S) and keeps the per-step states (states_out_dev)");
+        const size_t need = carve_train_cache(m, l, (size_t)S, cache_dev, &cache);
+        TB2_REQUIRE(need > 0 && cache_bytes >= need, "training cache too small (tb2_lstm_train_cache_bytes)");
+    }
+    cudaStream_t st = (cudaStream_t)stream;
+    cudaStream_t copy_st = (cudaStream_t)copy_stream;
+    while (normals_host && (int)m->step_events.size() < last_step) {      // one event per step copied to the host
+        cudaEvent_t ev;
+        TB2_CHECK_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+        m->step_events.push_back(ev);
+    }
     Workspace ws;
     carve_workspace(m, l, workspace, &ws);
-    cudaStream_t st = (cudaStream_t)stream;
     const size_t M = (size_t)l->M, H = (size_t)m->H;
     const size_t frame = M * 2;
     if (first_step == 0 && ws.pool_h) {       // pool.reset(...) lstm.py:213-216
@@ -721,23 +714,23 @@ static int forward_steps_impl(const tb2_lstm* m, const tb2_layout* l, const floa
         float* h_next = states_out ? states_out + ((size_t)s * 2 + 0) * M * H : h;
         float* c_next = states_out ? states_out + ((size_t)s * 2 + 1) * M * H : c;
         Workspace wstep = ws;
-        if (cache) {        // this step's winners, latent vectors, hidden1 and pooled vector stay where the backward reads them
+        if (cache_dev) {        // this step's winners, latent vectors, hidden1 and pooled vector stay where the backward reads them
             const size_t nm1 = (size_t)(l->n_max > 1 ? l->n_max - 1 : 1), us = (size_t)s;
             const PoolFormats f = pool_formats(m);
-            wstep.lat = cache->lat + us * M * m->C;
-            wstep.win_count = cache->win_count + us * M;
-            wstep.win_ent = cache->win_ent + us * M * nm1;
-            wstep.pair_cell = cache->pair_cell + us * M * nm1;
-            wstep.pair_flag = cache->pair_flag + us * M * nm1;
-            if (cache->h1) {
-                char* h1 = cache->h1 + us * cache->h1_step;
+            wstep.lat = cache.lat + us * M * m->C;
+            wstep.win_count = cache.win_count + us * M;
+            wstep.win_ent = cache.win_ent + us * M * nm1;
+            wstep.pair_cell = cache.pair_cell + us * M * nm1;
+            wstep.pair_flag = cache.pair_flag + us * M * nm1;
+            if (cache.h1) {
+                char* h1 = cache.h1 + us * cache.h1_step;
                 wstep.act[0] = (float*)h1;
-                if (f.h1_pair) wstep.act[1] = (float*)(h1 + cache->h1_step / 2);
+                if (f.h1_pair) wstep.act[1] = (float*)(h1 + cache.h1_step / 2);
             }
-            char* pooled = cache->pooled + us * cache->pooled_step;
+            char* pooled = cache.pooled + us * cache.pooled_step;
             if (f.pooled_pair) {
                 wstep.pool_hi = pooled;
-                wstep.pool_lo = pooled + cache->pooled_step / 2;
+                wstep.pool_lo = pooled + cache.pooled_step / 2;
             } else {
                 wstep.pooled = (float*)pooled;
             }
@@ -753,14 +746,14 @@ static int forward_steps_impl(const tb2_lstm* m, const tb2_layout* l, const floa
             return rc;
         h_prev = h_next;
         c_prev = c_next;
-        if (sink) {     // this step's results -> host, behind the step, beside the following steps
-            cudaEvent_t ev = (*sink->events)[(size_t)s];
+        if (normals_host) {     // this step's results -> host, behind the step, beside the following steps
+            cudaEvent_t ev = m->step_events[(size_t)s];
             TB2_CHECK_CUDA(cudaEventRecord(ev, st));
-            TB2_CHECK_CUDA(cudaStreamWaitEvent(sink->copy_stream, ev, 0));
-            TB2_CHECK_CUDA(cudaMemcpyAsync(sink->normals_host + (size_t)s * M * 5, normals_out + (size_t)s * M * 5,
-                                           M * 5 * sizeof(float), cudaMemcpyDeviceToHost, sink->copy_stream));
-            TB2_CHECK_CUDA(cudaMemcpyAsync(sink->positions_host + (size_t)s * frame, positions_out + (size_t)s * frame,
-                                           frame * sizeof(float), cudaMemcpyDeviceToHost, sink->copy_stream));
+            TB2_CHECK_CUDA(cudaStreamWaitEvent(copy_st, ev, 0));
+            TB2_CHECK_CUDA(cudaMemcpyAsync(normals_host + (size_t)s * M * 5, normals_out + (size_t)s * M * 5,
+                                           M * 5 * sizeof(float), cudaMemcpyDeviceToHost, copy_st));
+            TB2_CHECK_CUDA(cudaMemcpyAsync(positions_host + (size_t)s * frame, positions_out + (size_t)s * frame,
+                                           frame * sizeof(float), cudaMemcpyDeviceToHost, copy_st));
         }
     }
     if (states_out && last_step > first_step) {
@@ -768,64 +761,6 @@ static int forward_steps_impl(const tb2_lstm* m, const tb2_layout* l, const floa
         TB2_CHECK_CUDA(cudaMemcpyAsync(c, c_prev, M * H * sizeof(float), cudaMemcpyDeviceToDevice, st));
     }
     return TB2_OK;
-}
-
-int tb2_lstm_forward_steps(const tb2_lstm* m, const tb2_layout* l, const float* observed,
-                           int32_t obs_length, const float* truth, int32_t n_decode, int32_t first_step,
-                           int32_t last_step, float* normals_out, float* positions_out, float* h, float* c,
-                           float* states_out, void* workspace, size_t workspace_bytes, void* stream) {
-    return forward_steps_impl(m, l, observed, obs_length, truth, n_decode, nullptr, first_step, last_step, normals_out,
-                              positions_out, h, c, states_out, workspace, workspace_bytes, stream, nullptr);
-}
-
-int tb2_lstm_forward_steps_goals(const tb2_lstm* m, const tb2_layout* l, const float* observed,
-                                 int32_t obs_length, const float* truth, int32_t n_decode, const float* goals,
-                                 int32_t first_step, int32_t last_step, float* normals_out, float* positions_out, float* h,
-                                 float* c, float* states_out, void* workspace, size_t workspace_bytes, void* stream) {
-    return forward_steps_impl(m, l, observed, obs_length, truth, n_decode, goals, first_step, last_step, normals_out,
-                              positions_out, h, c, states_out, workspace, workspace_bytes, stream, nullptr);
-}
-
-int tb2_lstm_forward_steps_sampled(const tb2_lstm* m, const tb2_layout* l, const float* observed,
-                                   int32_t obs_length, const float* truth, int32_t n_decode, int32_t first_step,
-                                   int32_t last_step, const float* eps, float* normals_out, float* positions_out,
-                                   float* h, float* c, float* states_out, void* workspace, size_t workspace_bytes,
-                                   void* stream) {
-    TB2_REQUIRE(m, "null handle");
-    if (m->G > 0) {
-        set_error("sampled forwards of a goal-conditioned model (goal_dim > 0) are not built");
-        return TB2_ERR_UNSUPPORTED;
-    }
-    TB2_REQUIRE(eps, "eps_dev [n_decode + 1, M, 2] is required (all zeros for the mean trajectory)");
-    return forward_steps_impl(m, l, observed, obs_length, truth, n_decode, nullptr, first_step, last_step, normals_out,
-                              positions_out, h, c, states_out, workspace, workspace_bytes, stream, nullptr, nullptr, eps);
-}
-
-int tb2_lstm_forward_sequence_host(tb2_lstm* m, const tb2_layout* l, const float* observed, int32_t obs_length,
-                                   const float* truth, int32_t n_decode, float* normals_out, float* positions_out,
-                                   float* h, float* c, void* workspace, size_t workspace_bytes,
-                                   float* normals_host, float* positions_host, void* stream, void* copy_stream) {
-    return tb2_lstm_forward_sequence_host_goals(m, l, observed, obs_length, truth, n_decode, nullptr, normals_out,
-                                                positions_out, h, c, workspace, workspace_bytes, normals_host,
-                                                positions_host, stream, copy_stream);
-}
-
-int tb2_lstm_forward_sequence_host_goals(tb2_lstm* m, const tb2_layout* l, const float* observed, int32_t obs_length,
-                                         const float* truth, int32_t n_decode, const float* goals, float* normals_out,
-                                         float* positions_out, float* h, float* c, void* workspace,
-                                         size_t workspace_bytes, float* normals_host, float* positions_host, void* stream,
-                                         void* copy_stream) {
-    TB2_REQUIRE(m && normals_host && positions_host && copy_stream, "null argument");
-    TB2_REQUIRE(obs_length >= 2 && n_decode >= 0, "need obs_length >= 2 and n_decode >= 0");
-    const int S = obs_length - 1 + n_decode;
-    while ((int)m->step_events.size() < S) {
-        cudaEvent_t ev;
-        TB2_CHECK_CUDA(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-        m->step_events.push_back(ev);
-    }
-    HostSink sink{normals_host, positions_host, (cudaStream_t)copy_stream, &m->step_events};
-    return forward_steps_impl(m, l, observed, obs_length, truth, n_decode, goals, 0, S, normals_out, positions_out, h, c,
-                              nullptr, workspace, workspace_bytes, stream, &sink);
 }
 
 int tb2_pool_state_reset(const tb2_lstm* m, const tb2_layout* l, void* workspace, size_t workspace_bytes, void* stream) {
@@ -844,34 +779,6 @@ int tb2_pool_state_reset(const tb2_lstm* m, const tb2_layout* l, void* workspace
 size_t tb2_lstm_train_cache_bytes(const tb2_lstm* m, const tb2_layout* l, int32_t num_steps) {
     if (!m || !l || num_steps < 1) return 0;
     return carve_train_cache(m, l, (size_t)num_steps, nullptr, nullptr);
-}
-
-int tb2_lstm_forward_sequence_train(const tb2_lstm* m, const tb2_layout* l, const float* observed, int32_t obs_length,
-                                    const float* truth, int32_t n_decode, float* normals_out, float* positions_out,
-                                    float* h, float* c, float* states_out, void* cache, size_t cache_bytes,
-                                    void* workspace, size_t workspace_bytes, void* stream) {
-    TB2_REQUIRE(m && l, "null handle");
-    TB2_REQUIRE(obs_length >= 2 && n_decode >= 0, "need obs_length >= 2 and n_decode >= 0");
-    TB2_REQUIRE(states_out, "a training forward keeps the per-step states");
-    if (m->G > 0) {
-        set_error("training a goal-conditioned model (goal_dim > 0) is not built");
-        return TB2_ERR_UNSUPPORTED;
-    }
-    const int S = obs_length - 1 + n_decode;
-    TrainCache tc;
-    const size_t need = carve_train_cache(m, l, (size_t)S, cache, &tc);
-    TB2_REQUIRE(!cache || (need > 0 && cache_bytes >= need), "training cache too small (tb2_lstm_train_cache_bytes)");
-    return forward_steps_impl(m, l, observed, obs_length, truth, n_decode, nullptr, 0, S, normals_out, positions_out, h, c,
-                              states_out, workspace, workspace_bytes, stream, nullptr, cache ? &tc : nullptr);
-}
-
-int tb2_lstm_forward_sequence(const tb2_lstm* m, const tb2_layout* l, const float* observed,
-                              int32_t obs_length, const float* truth, int32_t n_decode,
-                              float* normals_out, float* positions_out, float* h, float* c,
-                              float* states_out, void* workspace, size_t workspace_bytes, void* stream) {
-    TB2_REQUIRE(obs_length >= 2 && n_decode >= 0, "need obs_length >= 2 and n_decode >= 0");
-    return tb2_lstm_forward_steps(m, l, observed, obs_length, truth, n_decode, 0, obs_length - 1 + n_decode,
-                                  normals_out, positions_out, h, c, states_out, workspace, workspace_bytes, stream);
 }
 
 }  // extern "C"

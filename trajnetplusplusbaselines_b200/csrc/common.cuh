@@ -134,7 +134,7 @@ constexpr int kLayer1MmaTailCols = 256;
 // Refusal of the fused calls for a model whose interaction module the caller runs (TB2_POOL_EXTERNAL)
 constexpr const char* kExternalPoolMessage =
     "an external interaction module (TB2_POOL_EXTERNAL) runs step by step: tb2_pool_inputs_padded, the module, "
-    "tb2_lstm_step_forward_pooled, and tb2_lstm_step_backward for training";
+    "tb2_lstm_step_forward with pooled_padded_dev, and tb2_lstm_step_backward for training";
 
 }  // namespace tb2
 
@@ -168,7 +168,9 @@ struct tb2_lstm {
     float* bl[tb2::kMaxMlpLayers] = {};   // biases of layers >= 2
     void* W_hi[tb2::kMaxMlpLayers] = {};  // [1] only (second Linear): bf16 [N, K] (hi, lo) split for the wgmma path (null: FFMA path)
     void* W_lo[tb2::kMaxMlpLayers] = {};
-    std::vector<cudaEvent_t> step_events;     // tb2_lstm_forward_sequence_host: one event per recurrence step
+    // tb2_lstm_forward_steps with host outputs: one event per recurrence step, created on first use (hence mutable:
+    // the call takes a const model)
+    mutable std::vector<cudaEvent_t> step_events;
     // HiddenStateMLPPooling (TB2_POOL_HIDDEN_MLP)
     float *mp_Ws = nullptr, *mp_bs = nullptr, *mp_Wv = nullptr, *mp_bv = nullptr, *mp_WhT = nullptr, *mp_bh = nullptr,
           *mp_WoT = nullptr, *mp_bo = nullptr;
@@ -244,7 +246,7 @@ inline bool social_trainable(const tb2_lstm* m) {
            m->cfg.constant == 0.f && m->G == 0;
 }
 
-// Per-step forward quantities the training forward (tb2_lstm_forward_sequence_train) keeps for the social backward,
+// Per-step forward quantities the training forward (tb2_lstm_forward_steps with cache_dev) keeps for the social backward,
 // which reads its grid-embedding records from here only.  Step s of hidden1 / the pooled vector is a slot of
 // h1_step / pooled_step bytes at h1 / pooled + s * step: fp32 [M][n], or bf16 hi [M][n] followed by lo [M][n] at
 // step / 2 (pool_formats).  Every slot and half is 256-byte aligned, like the workspace buffers it stands in for.

@@ -1766,7 +1766,7 @@ int tb2_lstm_sequence_backward(const tb2_lstm* m, const tb2_layout* l, const tb2
                 "backward workspace too small");
     TrainCache tc;
     const size_t cache_need = carve_train_cache(m, l, (size_t)S, const_cast<void*>(cache), &tc);
-    TB2_REQUIRE(!social || cache, "a social model trains from the cache its tb2_lstm_forward_sequence_train call filled");
+    TB2_REQUIRE(!social || cache, "a social model trains from the cache its tb2_lstm_forward_steps call (cache_dev) filled");
     TB2_REQUIRE(cache_bytes >= cache_need, "training cache too small (tb2_lstm_train_cache_bytes)");
     if (num_active == 0) return TB2_OK;
     cudaStream_t st = (cudaStream_t)stream;

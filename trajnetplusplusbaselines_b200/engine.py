@@ -305,70 +305,47 @@ class ModelHandle:
 
     # goals: [M, 2] fp32 device tensor of a goal-conditioned model (None for any other; the library refuses a goal model
     # without them)
-    def step_forward(self, layout, phase, obs1, obs2, h, c, goals=None):
-        """One step; h, c updated in place.  Returns (normal [M,5], pos [M,2])."""
+    def step_forward(self, layout, phase, obs1, obs2, h, c, goals=None, pooled=None, h_out=None, c_out=None):
+        """One step (tb2_lstm_step_forward); without h_out / c_out, h and c are updated in place.  pooled: the external
+        interaction module's output [B * n_pad, out_dim] (TB2_POOL_EXTERNAL models only).  Returns (normal [M,5],
+        pos [M,2])."""
         lib = _lib.load()
         ws, need = self.workspace(layout)
         M = layout.num_tracks
         normal = torch.empty((M, 5), dtype=torch.float32, device=self.device)
         pos = torch.empty((M, 2), dtype=torch.float32, device=self.device)
+        h_out = h if h_out is None else h_out
+        c_out = c if c_out is None else c_out
         with torch.cuda.device(self.device):
-            _lib.check(lib.tb2_lstm_step_forward_goals(self.handle, layout.handle, phase, _ptr(obs1), _ptr(obs2),
-                                                       _ptr(goals), _ptr(h), _ptr(c), _ptr(h), _ptr(c), _ptr(normal),
-                                                       _ptr(pos), _ptr(ws), need, _stream(self.device)))
+            _lib.check(lib.tb2_lstm_step_forward(self.handle, layout.handle, phase, _ptr(obs1), _ptr(obs2), _ptr(goals),
+                                                 _ptr(pooled), _ptr(h), _ptr(c), _ptr(h_out), _ptr(c_out), _ptr(normal),
+                                                 _ptr(pos), _ptr(ws), need, _stream(self.device)))
         return normal, pos
 
     def forward_steps(self, layout, observed, truth, n_decode, first_step, last_step, normals, positions, h, c,
-                      goals=None):
-        """Steps [first_step, last_step) of the time loop on caller-owned state (tb2_lstm_forward_steps)."""
+                      goals=None, eps=None, states=None, cache=None, host=None):
+        """Steps [first_step, last_step) of the time loop on caller-owned state (tb2_lstm_forward_steps).
+        eps [n_decode + 1, M, 2]: every predicted position is drawn from its step's normal at these standard normal
+        pairs.  states [S, 2, M, H]: the state after every step.  cache: uint8 device tensor of train_cache_bytes,
+        where the social pooling keeps its per-step records for tb2_lstm_sequence_backward.  host = (normals_host,
+        positions_host, copy_stream): every step's results are copied to the pinned host tensors on copy_stream,
+        which the caller synchronises before reading them."""
         lib = _lib.load()
         ws, need = self.workspace(layout)
+        normals_host, positions_host, copy_stream = host if host is not None else (None, None, None)
         with torch.cuda.device(self.device):
-            _lib.check(lib.tb2_lstm_forward_steps_goals(
-                self.handle, layout.handle, _ptr(observed), int(observed.shape[0]), _ptr(truth),
-                int(n_decode), _ptr(goals), int(first_step), int(last_step), _ptr(normals), _ptr(positions), _ptr(h),
-                _ptr(c), _ptr(None), _ptr(ws), need, _stream(self.device)))
+            _lib.check(lib.tb2_lstm_forward_steps(
+                self.handle, layout.handle, _ptr(observed), int(observed.shape[0]), _ptr(truth), int(n_decode),
+                _ptr(goals), _ptr(eps), int(first_step), int(last_step), _ptr(normals), _ptr(positions), _ptr(h),
+                _ptr(c), _ptr(states), _ptr(cache), 0 if cache is None else int(cache.numel()), _ptr(normals_host),
+                _ptr(positions_host), ctypes.c_void_p(copy_stream.cuda_stream if copy_stream is not None else 0),
+                _ptr(ws), need, _stream(self.device)))
 
     def forward_steps_sampled(self, layout, observed, truth, n_decode, first_step, last_step, eps, normals, positions, h,
                               c):
         """forward_steps with every predicted position drawn from its step's normal at the standard normal pairs
-        eps [n_decode + 1, M, 2] (tb2_lstm_forward_steps_sampled)."""
-        lib = _lib.load()
-        ws, need = self.workspace(layout)
-        with torch.cuda.device(self.device):
-            _lib.check(lib.tb2_lstm_forward_steps_sampled(
-                self.handle, layout.handle, _ptr(observed), int(observed.shape[0]), _ptr(truth), int(n_decode),
-                int(first_step), int(last_step), _ptr(eps), _ptr(normals), _ptr(positions), _ptr(h), _ptr(c),
-                _ptr(None), _ptr(ws), need, _stream(self.device)))
-
-    def forward_sequence_host(self, layout, observed, truth, n_decode, normals, positions, h, c, normals_host,
-                              positions_host, copy_stream, goals=None):
-        """tb2_lstm_forward_sequence_host: per-step device-to-host copies on `copy_stream`; the caller
-        synchronises that stream before reading the pinned host tensors."""
-        lib = _lib.load()
-        ws, need = self.workspace(layout)
-        with torch.cuda.device(self.device):
-            _lib.check(lib.tb2_lstm_forward_sequence_host_goals(
-                self.handle, layout.handle, _ptr(observed), int(observed.shape[0]), _ptr(truth), int(n_decode),
-                _ptr(goals), _ptr(normals), _ptr(positions), _ptr(h), _ptr(c), _ptr(ws), need, _ptr(normals_host),
-                _ptr(positions_host), _stream(self.device), ctypes.c_void_p(copy_stream.cuda_stream)))
+        eps [n_decode + 1, M, 2]."""
+        self.forward_steps(layout, observed, truth, n_decode, first_step, last_step, normals, positions, h, c, eps=eps)
 
     def train_cache_bytes(self, layout, num_steps):
         return int(_lib.load().tb2_lstm_train_cache_bytes(self.handle, layout.handle, int(num_steps)))
-
-    def forward_sequence_train(self, layout, observed, truth, n_decode, normals, positions, h, c, states, cache):
-        """tb2_lstm_forward_sequence_train: the per-step states go to `states` [S, 2, M, H]; per-step forward
-        quantities of the social pooling stay in `cache` (uint8 device tensor of train_cache_bytes, None when that is
-        0) for tb2_lstm_sequence_backward."""
-        lib = _lib.load()
-        ws, need = self.workspace(layout)
-        with torch.cuda.device(self.device):
-            _lib.check(lib.tb2_lstm_forward_sequence_train(
-                self.handle, layout.handle, _ptr(observed), int(observed.shape[0]), _ptr(truth), int(n_decode),
-                _ptr(normals), _ptr(positions), _ptr(h), _ptr(c), _ptr(states), _ptr(cache),
-                0 if cache is None else int(cache.numel()), _ptr(ws), need, _stream(self.device)))
-
-    def forward_sequence(self, layout, observed, truth, n_decode, normals, positions, h, c, goals=None):
-        """The whole time loop (tb2_lstm_forward_sequence, i.e. forward_steps over [0, S))."""
-        self.forward_steps(layout, observed, truth, n_decode, 0, int(observed.shape[0]) - 1 + int(n_decode), normals,
-                           positions, h, c, goals)

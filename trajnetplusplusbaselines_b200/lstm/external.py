@@ -12,7 +12,8 @@ current stream, with no host synchronisation in between.  Per step:
 
     tb2_pool_inputs_padded        ragged obs1 / obs2 / h -> [B, n_pad, .], NaN padding (generate_pooling_inputs)
     pool(h_pad, obs1_pad, obs2_pad)
-    tb2_lstm_step_forward_pooled  the module's row of every present track into the gate operand, then the step
+    tb2_lstm_step_forward         with pooled_padded_dev: the module's row of every present track into the gate
+                                  operand, then the step
 
 n_pad is the largest scene of the batch, and every track's hidden state goes in, absent tracks included, as in the
 reference.  Under grad mode each of the two library calls is a torch.autograd.Function (backward:
@@ -94,15 +95,8 @@ def _lstm_params(model):
 class _PooledStep(torch.autograd.Function):
     @staticmethod
     def forward(ctx, model, handle, layout, phase, obs1, obs2, pooled, h, c, *params):
-        M, H = layout.num_tracks, int(h.shape[1])
-        f32 = dict(dtype=torch.float32, device=h.device)
-        h_out, c_out = torch.empty((M, H), **f32), torch.empty((M, H), **f32)
-        normal, pos = torch.empty((M, 5), **f32), torch.empty((M, 2), **f32)
-        ws, need = handle.workspace(layout)
-        with torch.cuda.device(h.device):
-            _lib.check(_lib.load().tb2_lstm_step_forward_pooled(
-                handle.handle, layout.handle, phase, _ptr(obs1), _ptr(obs2), _ptr(pooled), _ptr(h), _ptr(c), _ptr(h_out),
-                _ptr(c_out), _ptr(normal), _ptr(pos), _ptr(ws), need, _stream(h.device)))
+        h_out, c_out = torch.empty_like(h), torch.empty_like(c)
+        normal, pos = handle.step_forward(layout, phase, obs1, obs2, h, c, pooled=pooled, h_out=h_out, c_out=c_out)
         ctx.model, ctx.handle, ctx.layout, ctx.phase, ctx.params = model, handle, layout, phase, params
         ctx.save_for_backward(obs1, obs2, pooled, h, c)
         return h_out, c_out, normal, pos

@@ -4,7 +4,7 @@ Mirrors trajnetbaselines/lstm/lstm.py: drop_distant :16-22, LSTM :45-264, LSTMPr
 :266-313.  Same constructor arguments, same state_dict keys (SURVEY.md 8b/B2), same
 forward signature and return shapes; the time loop, the per-step mask / embed / pool /
 LSTMCell / Gaussian head and the decoder feedback rule all run on the GPU through
-tb2_lstm_forward_sequence (csrc/capi.cu).  There is no torch or CPU implementation of the
+tb2_lstm_forward_steps (csrc/capi.cu).  There is no torch or CPU implementation of the
 step in this package: without the CUDA library the calls raise.
 """
 import math
@@ -196,7 +196,7 @@ class LSTM(torch.nn.Module):
         o1 = self._to_device(obs1, device, 'obs1')
         o2 = self._to_device(obs2, device, 'obs2')
         g = self._goals_on(goals, layout.num_tracks, device)
-        normal, _ = handle.step_forward(layout, phase, o1, o2, h, c, g)
+        normal, _ = handle.step_forward(layout, phase, o1, o2, h, c, goals=g)
         if was_list:
             return (list(h), list(c)), normal
         return (h, c), normal
@@ -254,7 +254,7 @@ class LSTM(torch.nn.Module):
     def _encode(self, seq):
         """The encoder steps [0, S_enc) of `seq`, into its own outputs and state."""
         seq.handle.forward_steps(seq.layout, seq.obs, seq.truth, seq.n_decode, 0, seq.S_enc, seq.normals,
-                                 seq.positions, seq.h, seq.c, seq.goals)
+                                 seq.positions, seq.h, seq.c, goals=seq.goals)
         return seq
 
     def _decode(self, seq, context, seed=True):
@@ -264,7 +264,7 @@ class LSTM(torch.nn.Module):
         normals, positions = seq.normals.clone(), seq.positions.clone()
         context(h, c)
         seq.handle.forward_steps(seq.layout, seq.obs, seq.truth, seq.n_decode, seq.S_enc, seq.S, normals, positions,
-                                 h, c, seq.goals)
+                                 h, c, goals=seq.goals)
         return self._results(seq, normals, positions, seed)
 
     def _results(self, seq, normals, positions, seed=True):
@@ -280,14 +280,14 @@ class LSTM(torch.nn.Module):
                         pad_to_batch_max=True, force_repack=False, goals=None):
         seq = self._sequence(observed, batch_split, prediction_truth, n_predict, pad_to_batch_max, force_repack, goals)
         handle, layout, device = seq.handle, seq.layout, seq.handle.device
-        inputs = (layout, seq.obs, seq.truth, seq.n_decode, seq.normals, seq.positions, seq.h, seq.c)
+        inputs = (layout, seq.obs, seq.truth, seq.n_decode, 0, seq.S, seq.normals, seq.positions, seq.h, seq.c)
         if want_states:
             # training forward: the outputs stay on the device; the per-step states are kept for the backward, and
             # so are the grid-embedding records the social backward reads (0 bytes: not a social model, no cache)
             states = torch.empty((seq.S, 2, layout.num_tracks, self.hidden_dim), dtype=torch.float32, device=device)
             cache_bytes = handle.train_cache_bytes(layout, seq.S)
             cache = torch.empty(cache_bytes, dtype=torch.uint8, device=device) if cache_bytes > 0 else None
-            handle.forward_sequence_train(*inputs, states, cache)
+            handle.forward_steps(*inputs, goals=seq.goals, states=states, cache=cache)
             normals, positions = self._results(seq._replace(out_device=device), seq.normals, seq.positions)
             return normals, positions, states, (seq.obs, seq.truth, layout, cache)
         if seq.out_device != device and seq.obs.shape[0] > 2:
@@ -295,10 +295,10 @@ class LSTM(torch.nn.Module):
             # while the later steps compute; one synchronisation of that stream at the end
             normals_h, positions_h = self._host_buffers(seq.normals, seq.positions)
             copy_stream = self._copy_stream(device)
-            handle.forward_sequence_host(*inputs, normals_h, positions_h, copy_stream, seq.goals)
+            handle.forward_steps(*inputs, goals=seq.goals, host=(normals_h, positions_h, copy_stream))
             copy_stream.synchronize()
             return normals_h.view(normals_h.shape), positions_h.view(positions_h.shape)
-        handle.forward_sequence(*inputs, seq.goals)
+        handle.forward_steps(*inputs, goals=seq.goals)
         return self._results(seq, seq.normals, seq.positions)
 
     def _host_buffers(self, *tensors):

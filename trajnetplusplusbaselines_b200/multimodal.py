@@ -97,7 +97,7 @@ def predict_modes(body, observed, split, n_predict, modes, context, max_rows=Non
 
     context(h_enc, c_enc, q0, q1, h_out, c_out) writes the decoder starting state of modes [q0, q1) into
     h_out / c_out [(q1 - q0) * M, H].  eps: float32 [n_predict, modes * M, 2] on the device, mode-major: every predicted
-    position of the decode is drawn from its step's normal (tb2_lstm_forward_steps_sampled), the first one, the
+    position of the decode is drawn from its step's normal (tb2_lstm_forward_steps with eps_dev), the first one, the
     encoder's last output, on the replicated rows before the decoder starts.  Returns the positions of the last
     n_predict steps, float32 [n_predict, modes * M, 2] on the device, mode-major."""
     refuse_goals(body)
