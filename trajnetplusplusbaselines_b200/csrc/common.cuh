@@ -1,5 +1,7 @@
 // Shared host/device declarations of libtrajnet_b200 (sm_90a only).
 #pragma once
+#include <cuda.h>
+#include <cuda_bf16.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stddef.h>
@@ -46,6 +48,21 @@ extern std::atomic<uint64_t> g_launch_count;
 #ifdef __CUDACC__
 __device__ __forceinline__ void grid_dep_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 __device__ __forceinline__ void grid_dep_launch() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
+
+// The operand format of every 3-pass bf16 tensor-core product: an fp32 v is stored as hi = rn(v), lo = rn(v - hi),
+// and A.W ~= A_hi.W_hi + A_hi.W_lo + A_lo.W_hi (the dropped terms ~ 2^-17 relative)
+__device__ __forceinline__ void split_bf16(float v, __nv_bfloat16& hi, __nv_bfloat16& lo) {
+    const __nv_bfloat16 h = __float2bfloat16_rn(v);
+    hi = h;
+    lo = __float2bfloat16_rn(v - __bfloat162float(h));
+}
+// two adjacent values as packed bf16x2 words (v.x in the low half)
+__device__ __forceinline__ void split_bf16x2(float2 v, uint32_t& hi, uint32_t& lo) {
+    const __nv_bfloat162 h = __floats2bfloat162_rn(v.x, v.y);
+    const __nv_bfloat162 l = __floats2bfloat162_rn(v.x - __low2float(h), v.y - __high2float(h));
+    hi = *reinterpret_cast<const uint32_t*>(&h);
+    lo = *reinterpret_cast<const uint32_t*>(&l);
+}
 
 // Warp-level D += A . B, m16n8k16, bf16 inputs, fp32 accumulation (the 3-pass split kernels of pool.cu and train.cu)
 __device__ __forceinline__ void mma_bf16_16816(float (&d)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
@@ -304,6 +321,16 @@ int launch_gates_tc(const tb2_lstm* m, const tb2_layout* l, int phase, const flo
                     const void* hs_in_hi, const void* hs_in_lo, void* hs_out_hi, void* hs_out_lo,
                     const float* h_in, const float* c_in, float* h_out, float* c_out, float* normal_out,
                     float* pos_out, cudaStream_t st);
+// TMA maps of a bf16 (hi, lo) split operand, row-major [rows, cols], box [box_rows, box_cols]; box_cols = 64 (128-byte
+// swizzle) or 32 (64-byte swizzle)
+struct SplitMap {
+    CUtensorMap hi, lo;
+};
+int make_split_map(SplitMap* map, const void* hi, const void* lo, int rows, int cols, int box_rows, int box_cols);
+// fp32 [rows, cols] (leading dimension ld_src) -> bf16 (hi, lo) of leading dimension ld_dst, on at most max_blocks CTAs
+int launch_split_bf16_rows(const float* src, size_t ld_src, size_t rows, size_t cols, void* hi, void* lo, size_t ld_dst,
+                           unsigned max_blocks, cudaStream_t st);
+// flat array of n floats
 int launch_split_bf16(const float* src, void* hi, void* lo, size_t n, cudaStream_t st);
 // pos [rows, 2] += the offset of the bivariate normal normals [rows, 5] at the standard normal pairs eps [rows, 2]
 int launch_sample_positions(const float* normals, float* pos, const float* eps, int rows, cudaStream_t st);

@@ -67,11 +67,7 @@ __global__ void external_pooled_kernel(const int* __restrict__ scene_off, const 
         }
         if (base) v += base[idx];
         if (out) out[idx] = v;
-        if (hi) {
-            const __nv_bfloat16 h = __float2bfloat16_rn(v);
-            hi[idx] = h;
-            lo[idx] = __float2bfloat16_rn(v - __bfloat162float(h));
-        }
+        if (hi) split_bf16(v, hi[idx], lo[idx]);
     }
 }
 

@@ -13,8 +13,9 @@
 //
 // Grid: (H / 64, ceil(M / 128)) in clusters of H / 64 CTAs along x (set at launch).  The CTAs of a
 // cluster share a 128-row tile and rank r owns hidden units [64 r, 64 r + 64) x 4 gates (N = 256;
-// W rows are permuted at repack so a CTA's tile holds complete i/f/g/o quadruples).  Warpgroup 2 is the TMA producer; warpgroups 0
-// and 1 each run wgmma.m64n256k16 on 64 rows.  In the accumulator fragment (wgmma.cuh) the four
+// W rows are permuted at repack so a CTA's tile holds complete i/f/g/o quadruples).  The mainloop is TcRing (wgmma.cuh)
+// with 32-wide k-blocks, each taken from the segment (emb, pooled or h) it falls in: warpgroup 2 is the TMA producer,
+// warpgroups 0 and 1 each run wgmma.m64n256k16 on 64 rows.  In the accumulator fragment (wgmma.cuh) the four
 // gates of a unit sit in the same thread (columns u, 64 + u, 128 + u, 192 + u), so the epilogue
 // updates c / h (fp32 state + bf16 split for the next step) straight from registers and
 // accumulates its share of the 5-wide Hidden2Normal dot products; the four threads of a row add
@@ -39,12 +40,8 @@ constexpr int kGtBN = 256;          // 64 units x 4 gates
 // memory (the cell state it reads is staged there too) and two stages' loads can be in flight behind the one being
 // multiplied
 constexpr int kGtBK = 32;
-constexpr int kGtStages = 3;
+using GateRing = TcRing<kGtBM, kGtBN, kGtBK, 3>;
 constexpr int kGtThreads = 384;     // two MMA + epilogue warpgroups, one producer warpgroup
-constexpr int kGtConsumerWarps = 8;
-constexpr uint32_t kGtABytes = kGtBM * kGtBK * 2;      // 8 KB
-constexpr uint32_t kGtBBytes = kGtBN * kGtBK * 2;      // 16 KB
-constexpr uint32_t kGtStageBytes = 2 * kGtABytes + 2 * kGtBBytes;   // 48 KB
 
 // Gate non-linearities on the SFU (ex2.approx, ~2 ulp) -- the epilogue was bound by the ~200
 // instructions per hidden unit of the libm-accurate expf / tanhf.  Absolute error ~1e-7 per
@@ -53,6 +50,8 @@ __device__ __forceinline__ float g_sigmoid(float x) { return __fdividef(1.f, 1.f
 __device__ __forceinline__ float g_tanh(float x) { return 1.f - __fdividef(2.f, __expf(2.f * x) + 1.f); }
 
 struct GateTcParams {
+    SplitMap emb, pool, h;      // A segments [M, 64 + G], [M, P], [M, H]
+    SplitMap w;                 // [4H (rank, gate, unit), K]
     const float2* obs1;
     const float2* obs2;
     const float* h_in;          // [M, H] fp32 state before the step
@@ -73,14 +72,9 @@ struct GateTcParams {
 // R = cluster size = H / 64 (1 to 4; a cluster of one at H = 64): the strides and the rank loop of the epilogue are compile-time constants
 template <int R, bool kGoal>
 __global__ void __launch_bounds__(kGtThreads, 1)
-lstm_gates_tc_kernel(const __grid_constant__ CUtensorMap map_emb_hi, const __grid_constant__ CUtensorMap map_emb_lo,
-                     const __grid_constant__ CUtensorMap map_pool_hi, const __grid_constant__ CUtensorMap map_pool_lo,
-                     const __grid_constant__ CUtensorMap map_h_hi, const __grid_constant__ CUtensorMap map_h_lo,
-                     const __grid_constant__ CUtensorMap map_w_hi, const __grid_constant__ CUtensorMap map_w_lo,
-                     GateTcParams p) {
+lstm_gates_tc_kernel(const __grid_constant__ GateTcParams p) {
     extern __shared__ __align__(1024) unsigned char smem_gt[];
-    __shared__ __align__(8) uint64_t full_bar[kGtStages];
-    __shared__ __align__(8) uint64_t empty_bar[kGtStages];
+    __shared__ GateRing tc;
     __shared__ float wn_s[5][64];          // Hidden2Normal weights of this CTA's 64 units
     __shared__ float bg_s[4][64];          // fused gate bias of this CTA's units
     constexpr int H = 64 * R;
@@ -101,13 +95,7 @@ lstm_gates_tc_kernel(const __grid_constant__ CUtensorMap map_emb_hi, const __gri
     for (int i = threadIdx.x; i < 5 * 64; i += kGtThreads) wn_s[i / 64][i % 64] = p.Wn[(i / 64) * H + rank * 64 + (i % 64)];
     for (int i = threadIdx.x; i < 4 * 64; i += kGtThreads) bg_s[i / 64][i % 64] = p.bg[(i / 64) * H + rank * 64 + (i % 64)];
 
-    if (threadIdx.x == 0) {
-        for (int s = 0; s < kGtStages; ++s) {
-            mbar_init(smem_u32(&full_bar[s]), 1);
-            mbar_init(smem_u32(&empty_bar[s]), kGtConsumerWarps);
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
+    if (threadIdx.x == 0) tc.init();
     __syncthreads();
     grid_dep_wait();          // embedding / pooled / state operands come from the previous kernels
     grid_dep_launch();
@@ -139,59 +127,13 @@ lstm_gates_tc_kernel(const __grid_constant__ CUtensorMap map_emb_hi, const __gri
     }
     float part[2][5] = {{0.f, 0.f, 0.f, 0.f, 0.f}, {0.f, 0.f, 0.f, 0.f, 0.f}};
 
-    if (wg == 2) {
-        if (threadIdx.x == 256) {
-            for (int kb = 0; kb < (TB2_GEMM_ABLATE == 2 ? 1 : num_kb); ++kb) {
-                const int s = kb % kGtStages;
-                const uint32_t phase = (kb / kGtStages) & 1;
-                mbar_wait(smem_u32(&empty_bar[s]), phase ^ 1);
-                const uint32_t bar = smem_u32(&full_bar[s]);
-                const uint32_t base = ring + s * kGtStageBytes;
-                mbar_expect_tx(bar, kGtStageBytes);
-                const CUtensorMap *ahi, *alo;
-                int ka;
-                if (kb < kb_emb) { ahi = &map_emb_hi; alo = &map_emb_lo; ka = kb * kGtBK; }
-                else if (kb < kb_emb + kb_pool) { ahi = &map_pool_hi; alo = &map_pool_lo; ka = (kb - kb_emb) * kGtBK; }
-                else { ahi = &map_h_hi; alo = &map_h_lo; ka = (kb - kb_emb - kb_pool) * kGtBK; }
-                tma_load_2d(base, ahi, bar, ka, m0);
-                tma_load_2d(base + kGtABytes, alo, bar, ka, m0);
-                tma_load_2d(base + 2 * kGtABytes, &map_w_hi, bar, kb * kGtBK, rank * kGtBN);
-                tma_load_2d(base + 2 * kGtABytes + kGtBBytes, &map_w_lo, bar, kb * kGtBK, rank * kGtBN);
-            }
-        }
-        __syncwarp();
-    } else {
-        float acc[kGtBN / 2];
-#pragma unroll
-        for (int i = 0; i < kGtBN / 2; ++i) acc[i] = 0.f;
-        const uint32_t a_off = (uint32_t)wg * 64 * 2 * kGtBK;    // this warpgroup's 64 rows of the A tiles
-        for (int kb = 0; kb < num_kb; ++kb) {
-            const int s = TB2_GEMM_ABLATE == 2 ? 0 : kb % kGtStages;
-            const uint32_t phase = TB2_GEMM_ABLATE == 2 ? 0 : (kb / kGtStages) & 1;
-            mbar_wait(smem_u32(&full_bar[s]), phase);
-            const uint32_t base = ring + s * kGtStageBytes;
-            const uint64_t a_hi = wgmma_desc<2 * kGtBK>(base + a_off);
-            const uint64_t a_lo = wgmma_desc<2 * kGtBK>(base + kGtABytes + a_off);
-            const uint64_t b_hi = wgmma_desc<2 * kGtBK>(base + 2 * kGtABytes);
-            const uint64_t b_lo = wgmma_desc<2 * kGtBK>(base + 2 * kGtABytes + kGtBBytes);
-            wgmma_fence();
-#pragma unroll
-            for (int k = 0; k < (TB2_GEMM_ABLATE == 1 ? 0 : kGtBK / 16); ++k) {
-                const uint64_t adv = (uint64_t)((k * 16 * 2) >> 4);
-                wgmma_bf16(acc, a_hi + adv, b_hi + adv, (kb | k) != 0);
-                wgmma_bf16(acc, a_hi + adv, b_lo + adv, 1u);
-                wgmma_bf16(acc, a_lo + adv, b_hi + adv, 1u);
-            }
-            wgmma_commit();
-#if TB2_GEMM_ABLATE == 4
-            wgmma_wait<1>();
-            if (kb > 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[(kb - 1) % kGtStages]));
-#else
-            wgmma_wait<0>();
-            if (lane == 0) mbar_arrive(smem_u32(&empty_bar[s]));
-#endif
-        }
-        wgmma_wait<0>();
+    float acc[kGtBN / 2];
+    tc.run(ring, num_kb, m0, [&](int kb) {
+        if (kb < kb_emb) return TcATile{&p.emb, kb * kGtBK};
+        if (kb < kb_emb + kb_pool) return TcATile{&p.pool, (kb - kb_emb) * kGtBK};
+        return TcATile{&p.h, (kb - kb_emb - kb_pool) * kGtBK};
+    }, p.w, rank * kGtBN, acc);
+    if (wg < 2) {
         asm volatile("cp.async.wait_group 0;" ::: "memory");       // this thread's c_s slots and its rows' obs_s
         asm volatile("bar.sync 1, 256;" ::: "memory");             // obs_s rows copied by the other threads of a quad
         // gate g of unit u = 8 n8 + 2 (lane % 4) + j, row rl + 8 hr: acc[4 (8 g + n8) + 2 hr + j]
@@ -230,13 +172,8 @@ lstm_gates_tc_kernel(const __grid_constant__ CUtensorMap map_emb_hi, const __gri
                 }
                 *reinterpret_cast<float2*>(p.h_out + o) = h;
                 *reinterpret_cast<float2*>(p.c_out + o) = c;
-                const __nv_bfloat16 h0 = __float2bfloat16_rn(h.x), h1 = __float2bfloat16_rn(h.y);
-                const __nv_bfloat16 l0 = __float2bfloat16_rn(h.x - __bfloat162float(h0));
-                const __nv_bfloat16 l1 = __float2bfloat16_rn(h.y - __bfloat162float(h1));
-                *reinterpret_cast<uint32_t*>(p.hs_out_hi + o) =
-                    (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
-                *reinterpret_cast<uint32_t*>(p.hs_out_lo + o) =
-                    (uint32_t)__bfloat16_as_ushort(l0) | ((uint32_t)__bfloat16_as_ushort(l1) << 16);
+                split_bf16x2(h, *reinterpret_cast<uint32_t*>(p.hs_out_hi + o),
+                             *reinterpret_cast<uint32_t*>(p.hs_out_lo + o));
             }
         }
         // the four threads of a row add their shares (fixed order: deterministic)
@@ -337,9 +274,7 @@ __global__ void embed_split_kernel(const float2* __restrict__ obs1, const float2
         const float gx = n != 0.f ? dx / n : 0.f, gy = n != 0.f ? dy / n : 0.f;
         v = fmaxf(fmaf(ge.Wg[2 * kg + 1], gy * 4.0f, fmaf(ge.Wg[2 * kg], gx * 4.0f, ge.bg[kg])), 0.f);
     }
-    const __nv_bfloat16 h = __float2bfloat16_rn(v);
-    hi[idx] = h;
-    lo[idx] = __float2bfloat16_rn(v - __bfloat162float(h));
+    split_bf16(v, hi[idx], lo[idx]);
 }
 
 // W_cat[n][k] = [W_ih | W_hh] with rows permuted to (rank, gate, unit) order, as bf16 (hi, lo)
@@ -355,13 +290,9 @@ __global__ void repack_gates_tc_kernel(const float* __restrict__ w_ih, const flo
         const int rank = n / 256, gate = (n % 256) / 64, ul = n % 64;
         const int src = gate * H + rank * 64 + ul;    // original gate column
         const float v = k < in_dim ? w_ih[(size_t)src * in_dim + k] : w_hh[(size_t)src * H + (k - in_dim)];
-        const __nv_bfloat16 h = __float2bfloat16_rn(v);
-        hi[idx] = h;
-        lo[idx] = __float2bfloat16_rn(v - __bfloat162float(h));
+        split_bf16(v, hi[idx], lo[idx]);
     }
 }
-
-int make_bf16_tile_map(CUtensorMap* map, const void* base, int rows, int cols, int box_rows, int box_cols);
 
 // the segments are whole multiples of 64 columns (two k-blocks), the widths the kernel has always taken
 bool gates_tc_supported(const tb2_lstm* m) {
@@ -392,53 +323,22 @@ int launch_embed_split(const tb2_lstm* m, int M, const float* obs1, const float*
     return TB2_OK;
 }
 
-template <int R, bool kGoal>
-static int launch_gates_tc_k(const CUtensorMap& me_hi, const CUtensorMap& me_lo, const CUtensorMap& mp_hi,
-                             const CUtensorMap& mp_lo, const CUtensorMap& mh_hi, const CUtensorMap& mh_lo,
-                             const CUtensorMap& mw_hi, const CUtensorMap& mw_lo, const GateTcParams& p, cudaStream_t st) {
-    const size_t smem = (size_t)kGtStages * kGtStageBytes + 1024;
-    static DynSmemConfig configured;
-    TB2_CHECK_CUDA(configured.ensure(lstm_gates_tc_kernel<R, kGoal>, smem));
-    dim3 grid(R, (p.M + kGtBM - 1) / kGtBM);
-    {
-        KernelTimer kt("lstm_gates_tc", st);
-        launch_pdl_cluster(lstm_gates_tc_kernel<R, kGoal>, grid, dim3(kGtThreads), smem, st, (unsigned)R, me_hi, me_lo,
-                           mp_hi, mp_lo, mh_hi, mh_lo, mw_hi, mw_lo, p);
-    }
-    TB2_LAUNCH_CHECK();
-    return TB2_OK;
-}
-
-template <int R>
-static int launch_gates_tc_t(const CUtensorMap& me_hi, const CUtensorMap& me_lo, const CUtensorMap& mp_hi,
-                             const CUtensorMap& mp_lo, const CUtensorMap& mh_hi, const CUtensorMap& mh_lo,
-                             const CUtensorMap& mw_hi, const CUtensorMap& mw_lo, const GateTcParams& p, cudaStream_t st) {
-    return p.G > 0 ? launch_gates_tc_k<R, true>(me_hi, me_lo, mp_hi, mp_lo, mh_hi, mh_lo, mw_hi, mw_lo, p, st)
-                   : launch_gates_tc_k<R, false>(me_hi, me_lo, mp_hi, mp_lo, mh_hi, mh_lo, mw_hi, mw_lo, p, st);
-}
-
 int launch_gates_tc(const tb2_lstm* m, const tb2_layout* l, int phase, const float* obs1, const float* obs2,
                     const void* emb_hi, const void* emb_lo, const void* pool_hi, const void* pool_lo,
                     const void* hs_in_hi, const void* hs_in_lo, void* hs_out_hi, void* hs_out_lo,
                     const float* h_in, const float* c_in, float* h_out, float* c_out, float* normal_out,
                     float* pos_out, cudaStream_t st) {
     const int M = l->M;
-    CUtensorMap me_hi, me_lo, mp_hi, mp_lo, mh_hi, mh_lo, mw_hi, mw_lo;
-    int rc;
-    if ((rc = make_bf16_tile_map(&me_hi, emb_hi, M, 64 + m->G, kGtBM, kGtBK))) return rc;
-    if ((rc = make_bf16_tile_map(&me_lo, emb_lo, M, 64 + m->G, kGtBM, kGtBK))) return rc;
-    if (m->P > 0) {
-        if ((rc = make_bf16_tile_map(&mp_hi, pool_hi, M, m->P, kGtBM, kGtBK))) return rc;
-        if ((rc = make_bf16_tile_map(&mp_lo, pool_lo, M, m->P, kGtBM, kGtBK))) return rc;
-    } else {
-        mp_hi = me_hi;
-        mp_lo = me_lo;
-    }
-    if ((rc = make_bf16_tile_map(&mh_hi, hs_in_hi, M, m->H, kGtBM, kGtBK))) return rc;
-    if ((rc = make_bf16_tile_map(&mh_lo, hs_in_lo, M, m->H, kGtBM, kGtBK))) return rc;
-    if ((rc = make_bf16_tile_map(&mw_hi, m->Wg_hi[phase], 4 * m->H, m->K_gate, kGtBN, kGtBK))) return rc;
-    if ((rc = make_bf16_tile_map(&mw_lo, m->Wg_lo[phase], 4 * m->H, m->K_gate, kGtBN, kGtBK))) return rc;
     GateTcParams p;
+    int rc;
+    if ((rc = make_split_map(&p.emb, emb_hi, emb_lo, M, 64 + m->G, kGtBM, kGtBK))) return rc;
+    if (m->P > 0) {
+        if ((rc = make_split_map(&p.pool, pool_hi, pool_lo, M, m->P, kGtBM, kGtBK))) return rc;
+    } else {
+        p.pool = p.emb;
+    }
+    if ((rc = make_split_map(&p.h, hs_in_hi, hs_in_lo, M, m->H, kGtBM, kGtBK))) return rc;
+    if ((rc = make_split_map(&p.w, m->Wg_hi[phase], m->Wg_lo[phase], 4 * m->H, m->K_gate, kGtBN, kGtBK))) return rc;
     p.obs1 = (const float2*)obs1;
     p.obs2 = (const float2*)obs2;
     p.h_in = h_in; p.c_in = c_in; p.h_out = h_out; p.c_out = c_out;
@@ -451,15 +351,27 @@ int launch_gates_tc(const tb2_lstm* m, const tb2_layout* l, int phase, const flo
     p.M = M;
     p.P = m->P;
     p.G = m->G;
-    switch (m->H) {
-        case 64: return launch_gates_tc_t<1>(me_hi, me_lo, mp_hi, mp_lo, mh_hi, mh_lo, mw_hi, mw_lo, p, st);
-        case 128: return launch_gates_tc_t<2>(me_hi, me_lo, mp_hi, mp_lo, mh_hi, mh_lo, mw_hi, mw_lo, p, st);
-        case 192: return launch_gates_tc_t<3>(me_hi, me_lo, mp_hi, mp_lo, mh_hi, mh_lo, mw_hi, mw_lo, p, st);
-        case 256: return launch_gates_tc_t<4>(me_hi, me_lo, mp_hi, mp_lo, mh_hi, mh_lo, mw_hi, mw_lo, p, st);
-        default: break;
+    // one instance per cluster size R = H / 64 and goal input, each configured for its shared memory on its own
+    static void (*const kernels[4][2])(GateTcParams) = {
+        {lstm_gates_tc_kernel<1, false>, lstm_gates_tc_kernel<1, true>},
+        {lstm_gates_tc_kernel<2, false>, lstm_gates_tc_kernel<2, true>},
+        {lstm_gates_tc_kernel<3, false>, lstm_gates_tc_kernel<3, true>},
+        {lstm_gates_tc_kernel<4, false>, lstm_gates_tc_kernel<4, true>}};
+    static DynSmemConfig configured[4][2];
+    const int R = m->H / 64;
+    if (m->H % 64 != 0 || R < 1 || R > 4) {
+        set_error(kHiddenDimMessage);
+        return TB2_ERR_UNSUPPORTED;
     }
-    set_error(kHiddenDimMessage);
-    return TB2_ERR_UNSUPPORTED;
+    const int goal = p.G > 0;
+    TB2_CHECK_CUDA(configured[R - 1][goal].ensure(kernels[R - 1][goal], GateRing::kSmemBytes));
+    {
+        KernelTimer kt("lstm_gates_tc", st);
+        launch_pdl_cluster(kernels[R - 1][goal], dim3(R, (M + kGtBM - 1) / kGtBM), dim3(kGtThreads), GateRing::kSmemBytes,
+                           st, (unsigned)R, p);
+    }
+    TB2_LAUNCH_CHECK();
+    return TB2_OK;
 }
 
 }  // namespace tb2

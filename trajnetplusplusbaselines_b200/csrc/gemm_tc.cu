@@ -8,11 +8,10 @@
 // tensor-core passes:  A.W ~= A_hi.W_hi + A_hi.W_lo + A_lo.W_hi   (dropped terms ~ 2^-17 rel.).
 // A_hi / A_lo are written by the producing kernel (sparse_layer1), W_hi / W_lo at weight repack.
 //
-// Kernel shape (one 128 x BN output tile per CTA, 384 threads):
-//   warpgroup 2   TMA producer (one thread): 4 tiles per stage (A_hi, A_lo 128x64, W_hi, W_lo BNx64;
-//                 bf16, 128B-swizzled, K-major) into a shared-memory ring, mbarrier tx-counted
-//   warpgroups 0, 1  rows [64 wg, 64 wg + 64) of the tile: 12 wgmma.m64nBNk16 per stage into
-//                 fp32 register accumulators, then bias + ReLU and the stores straight from registers
+// Kernel shape (one 128 x BN output tile per CTA, 384 threads), mainloop TcRing (wgmma.cuh) with 64-wide k-blocks:
+//   warpgroup 2   TMA producer (one thread): A_hi, A_lo 128x64, W_hi, W_lo BNx64 per stage (128B-swizzled)
+//   warpgroups 0, 1  rows [64 wg, 64 wg + 64) of the tile: 12 wgmma.m64nBNk16 per stage into fp32 register
+//                 accumulators, then bias + ReLU (+ bf16 split) through shared memory and whole-row stores
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include <algorithm>
@@ -25,16 +24,12 @@ namespace tb2 {
 constexpr int kTcBM = 128;
 constexpr int kTcBK = 64;          // 64 bf16 = 128 bytes = one swizzle atom
 constexpr int kTcThreads = 384;
-constexpr int kTcConsumerWarps = 8;
-constexpr uint32_t kTcABytes = kTcBM * kTcBK * 2;     // 16 KB
 // BN = 128: 64 KB / stage, 3 stages;  BN = 64: 48 KB / stage, 4 stages (narrow layers)
-template <int BN> struct TcCfg {
-    static constexpr uint32_t kBBytes = BN * kTcBK * 2;
-    static constexpr uint32_t kStageBytes = 2 * kTcABytes + 2 * kBBytes;
-    static constexpr int kStages = BN == 128 ? 3 : 4;
-};
+template <int BN> using DenseRing = TcRing<kTcBM, BN, kTcBK, BN == 128 ? 3 : 4>;
 
 struct TcParams {
+    SplitMap a;                // A [M, K]
+    SplitMap w;                // W [N, K]
     const float* bias;
     float* Y;                  // fp32 output, or null
     __nv_bfloat16* Y_hi;       // bf16 (hi, lo) split output for a tensor-core consumer, or null
@@ -42,93 +37,33 @@ struct TcParams {
     int M, N, K, relu;
 };
 
-__device__ __forceinline__ uint32_t pack_bf16x2(unsigned short a, unsigned short b) { return (uint32_t)a | ((uint32_t)b << 16); }
-
 template <int kTcBN>
-__global__ void __launch_bounds__(kTcThreads, 1)
-dense_layer_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid_constant__ CUtensorMap map_a_lo,
-                      const __grid_constant__ CUtensorMap map_b_hi, const __grid_constant__ CUtensorMap map_b_lo,
-                      TcParams p) {
-    constexpr int kTcStages = TcCfg<kTcBN>::kStages;
-    constexpr uint32_t kTcBBytes = TcCfg<kTcBN>::kBBytes;
-    constexpr uint32_t kTcStageBytes = TcCfg<kTcBN>::kStageBytes;
+__global__ void __launch_bounds__(kTcThreads, 1) dense_layer_tc_kernel(const __grid_constant__ TcParams p) {
     extern __shared__ __align__(1024) unsigned char smem_tc[];
-    __shared__ __align__(8) uint64_t full_bar[kTcStages];
-    __shared__ __align__(8) uint64_t empty_bar[kTcStages];
+    __shared__ DenseRing<kTcBN> tc;
     __shared__ float bias_s[kTcBN];
 
     const int wg = threadIdx.x >> 7, warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int m0 = blockIdx.y * kTcBM, n0 = blockIdx.x * kTcBN;
-    const int num_kb = p.K / kTcBK;
     // 1024-byte aligned tile ring (dynamic smem base alignment is only guaranteed to 16 B)
     const uint32_t ring = (smem_u32(smem_tc) + 1023u) & ~1023u;
 
     if (threadIdx.x == 0) {
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a_hi) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_a_lo) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b_hi) : "memory");
-        asm volatile("prefetch.tensormap [%0];" ::"l"(&map_b_lo) : "memory");
-        for (int s = 0; s < kTcStages; ++s) {
-            mbar_init(smem_u32(&full_bar[s]), 1);
-            mbar_init(smem_u32(&empty_bar[s]), kTcConsumerWarps);
-        }
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&p.a.hi) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&p.a.lo) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&p.w.hi) : "memory");
+        asm volatile("prefetch.tensormap [%0];" ::"l"(&p.w.lo) : "memory");
+        tc.init();
     }
     __syncthreads();
     grid_dep_wait();          // the A operand is the previous kernel's output
     grid_dep_launch();
-
-    if (wg == 2) {
-        if (threadIdx.x == 256) {
-            for (int kb = 0; kb < (TB2_GEMM_ABLATE == 2 ? 1 : num_kb); ++kb) {
-                const int s = kb % kTcStages;
-                const uint32_t phase = (kb / kTcStages) & 1;
-                mbar_wait(smem_u32(&empty_bar[s]), phase ^ 1);
-                const uint32_t bar = smem_u32(&full_bar[s]);
-                const uint32_t base = ring + s * kTcStageBytes;
-                mbar_expect_tx(bar, kTcStageBytes);
-                tma_load_2d(base, &map_a_hi, bar, kb * kTcBK, m0);
-                tma_load_2d(base + kTcABytes, &map_a_lo, bar, kb * kTcBK, m0);
-                tma_load_2d(base + 2 * kTcABytes, &map_b_hi, bar, kb * kTcBK, n0);
-                tma_load_2d(base + 2 * kTcABytes + kTcBBytes, &map_b_lo, bar, kb * kTcBK, n0);
-            }
-        }
-        return;
-    }
     // the bias tile in shared memory: a global load in the epilogue waits its latency (it was issued after stores the
     // compiler cannot rule out that it aliases)
     if (threadIdx.x < kTcBN) bias_s[threadIdx.x] = p.bias[n0 + threadIdx.x];
     float acc[kTcBN / 2];
-#pragma unroll
-    for (int i = 0; i < kTcBN / 2; ++i) acc[i] = 0.f;
-    const uint32_t a_off = (uint32_t)wg * 64 * 128;        // this warpgroup's 64 rows of the A tiles
-    for (int kb = 0; kb < num_kb; ++kb) {
-        const int s = TB2_GEMM_ABLATE == 2 ? 0 : kb % kTcStages;
-        const uint32_t phase = TB2_GEMM_ABLATE == 2 ? 0 : (kb / kTcStages) & 1;
-        mbar_wait(smem_u32(&full_bar[s]), phase);
-        const uint32_t base = ring + s * kTcStageBytes;
-        const uint64_t a_hi = wgmma_desc(base + a_off);
-        const uint64_t a_lo = wgmma_desc(base + kTcABytes + a_off);
-        const uint64_t b_hi = wgmma_desc(base + 2 * kTcABytes);
-        const uint64_t b_lo = wgmma_desc(base + 2 * kTcABytes + kTcBBytes);
-        wgmma_fence();
-#pragma unroll
-        for (int k = 0; k < (TB2_GEMM_ABLATE == 1 ? 0 : kTcBK / 16); ++k) {
-            const uint64_t adv = (uint64_t)((k * 16 * 2) >> 4);      // 32 bytes per K step
-            wgmma_bf16(acc, a_hi + adv, b_hi + adv, (kb | k) != 0);
-            wgmma_bf16(acc, a_hi + adv, b_lo + adv, 1u);
-            wgmma_bf16(acc, a_lo + adv, b_hi + adv, 1u);
-        }
-        wgmma_commit();
-#if TB2_GEMM_ABLATE == 4
-        wgmma_wait<1>();
-        if (kb > 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[(kb - 1) % kTcStages]));
-#else
-        wgmma_wait<0>();
-        if (lane == 0) mbar_arrive(smem_u32(&empty_bar[s]));        // this warp no longer reads the stage
-#endif
-    }
-    wgmma_wait<0>();
+    tc.run(ring, p.K / kTcBK, m0, [&](int kb) { return TcATile{&p.a, kb * kTcBK}; }, p.w, n0, acc);
+    if (wg == 2) return;
     asm volatile("bar.sync 1, 256;" ::: "memory");     // bias_s written, and every consumer is done with the ring
     // epilogue: bias + ReLU (+ bf16 split) from the accumulator fragment (per register pair, one row and two adjacent
     // columns) into row-major tiles in the ring, then whole rows out in 16-byte stores.  Stored from the fragment
@@ -136,7 +71,7 @@ dense_layer_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid
     // the 8 rows of a fragment store fall in different banks.
     constexpr int kYStride = kTcBN + 8;                 // floats
     constexpr int kHStride = kTcBN + 16;                // bf16
-    static_assert(kTcBM * (kYStride * 4 + 2 * kHStride * 2) <= kTcStages * kTcStageBytes, "output tiles fit the ring");
+    static_assert(kTcBM * (kYStride * 4 + 2 * kHStride * 2) <= DenseRing<kTcBN>::kRingBytes, "output tiles fit the ring");
     float* y_s = reinterpret_cast<float*>(smem_tc + (ring - smem_u32(smem_tc)));
     uint32_t* hi_s = reinterpret_cast<uint32_t*>(y_s + kTcBM * kYStride);
     uint32_t* lo_s = hi_s + kTcBM * kHStride / 2;
@@ -149,10 +84,7 @@ dense_layer_tc_kernel(const __grid_constant__ CUtensorMap map_a_hi, const __grid
         float v0 = acc[i] + bias_s[c], v1 = acc[i + 1] + bias_s[c + 1];
         if (p.relu) { v0 = fmaxf(v0, 0.f); v1 = fmaxf(v1, 0.f); }
         *reinterpret_cast<float2*>(y_s + r * kYStride + c) = make_float2(v0, v1);
-        const __nv_bfloat16 h0 = __float2bfloat16_rn(v0), h1 = __float2bfloat16_rn(v1);
-        hi_s[(r * kHStride + c) / 2] = pack_bf16x2(__bfloat16_as_ushort(h0), __bfloat16_as_ushort(h1));
-        lo_s[(r * kHStride + c) / 2] = pack_bf16x2(__bfloat16_as_ushort(__float2bfloat16_rn(v0 - __bfloat162float(h0))),
-                                                   __bfloat16_as_ushort(__float2bfloat16_rn(v1 - __bfloat162float(h1))));
+        split_bf16x2(make_float2(v0, v1), hi_s[(r * kHStride + c) / 2], lo_s[(r * kHStride + c) / 2]);
     }
     asm volatile("bar.sync 1, 256;" ::: "memory");
     if (TB2_GEMM_ABLATE == 3 && p.M > 0) return;
@@ -202,7 +134,7 @@ static EncodeTiledFn encode_fn() {
 // A descriptor depends on (address, shape, box) only, and the step kernels are launched with the same few operand
 // buffers over and over: a small per-thread direct-mapped cache keeps the driver's encode call (a few microseconds,
 // 12 per recurrence step) off the launch path.
-int make_bf16_tile_map(CUtensorMap* map, const void* base, int rows, int cols, int box_rows, int box_cols) {
+static int make_bf16_tile_map(CUtensorMap* map, const void* base, int rows, int cols, int box_rows, int box_cols) {
     struct Entry { const void* base; int rows, cols, box_rows, box_cols; bool valid; CUtensorMap map; };
     static thread_local Entry cache[256] = {};
     const uintptr_t key = reinterpret_cast<uintptr_t>(base);
@@ -228,18 +160,22 @@ int make_bf16_tile_map(CUtensorMap* map, const void* base, int rows, int cols, i
     return TB2_OK;
 }
 
+int make_split_map(SplitMap* map, const void* hi, const void* lo, int rows, int cols, int box_rows, int box_cols) {
+    const int rc = make_bf16_tile_map(&map->hi, hi, rows, cols, box_rows, box_cols);
+    return rc ? rc : make_bf16_tile_map(&map->lo, lo, rows, cols, box_rows, box_cols);
+}
+
 bool dense_tc_supported(int K, int N) { return K >= kTcBK && K % kTcBK == 0 && N % 64 == 0; }
 
 template <int BN>
-static int launch_dense_tc_t(const CUtensorMap& ma_hi, const CUtensorMap& ma_lo, const CUtensorMap& mb_hi,
-                             const CUtensorMap& mb_lo, const TcParams& p, cudaStream_t st) {
-    const size_t smem = (size_t)TcCfg<BN>::kStages * TcCfg<BN>::kStageBytes + 1024;
+static int launch_dense_tc_t(const TcParams& p, cudaStream_t st) {
+    const size_t smem = DenseRing<BN>::kSmemBytes;
     static DynSmemConfig configured;
     TB2_CHECK_CUDA(configured.ensure(dense_layer_tc_kernel<BN>, smem));
     dim3 grid(p.N / BN, (p.M + kTcBM - 1) / kTcBM);
     {
         KernelTimer kt("dense_layer_tc", st);
-        launch_pdl(dense_layer_tc_kernel<BN>, grid, dim3(kTcThreads), smem, st, ma_hi, ma_lo, mb_hi, mb_lo, p);
+        launch_pdl(dense_layer_tc_kernel<BN>, grid, dim3(kTcThreads), smem, st, p);
     }
     TB2_LAUNCH_CHECK();
     return TB2_OK;
@@ -248,14 +184,11 @@ static int launch_dense_tc_t(const CUtensorMap& ma_hi, const CUtensorMap& ma_lo,
 int launch_dense_tc(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo, const float* bias,
                     float* Y, void* Y_hi, void* Y_lo, int M, int K, int N, int relu, cudaStream_t st) {
     TB2_REQUIRE(dense_tc_supported(K, N), "tensor-core dense layer needs K % 64 == 0 and N % 64 == 0");
-    CUtensorMap ma_hi, ma_lo, mb_hi, mb_lo;
-    int rc;
-    if ((rc = make_bf16_tile_map(&ma_hi, a_hi, M, K, kTcBM, kTcBK))) return rc;
-    if ((rc = make_bf16_tile_map(&ma_lo, a_lo, M, K, kTcBM, kTcBK))) return rc;
-    const int bn = (N % 128 == 0) ? 128 : 64;
-    if ((rc = make_bf16_tile_map(&mb_hi, w_hi, N, K, bn, kTcBK))) return rc;
-    if ((rc = make_bf16_tile_map(&mb_lo, w_lo, N, K, bn, kTcBK))) return rc;
     TcParams p;
+    int rc;
+    if ((rc = make_split_map(&p.a, a_hi, a_lo, M, K, kTcBM, kTcBK))) return rc;
+    const int bn = (N % 128 == 0) ? 128 : 64;
+    if ((rc = make_split_map(&p.w, w_hi, w_lo, N, K, bn, kTcBK))) return rc;
     p.bias = bias;
     p.Y = Y;
     p.Y_hi = (__nv_bfloat16*)Y_hi;
@@ -264,28 +197,32 @@ int launch_dense_tc(const void* a_hi, const void* a_lo, const void* w_hi, const 
     p.N = N;
     p.K = K;
     p.relu = relu;
-    return bn == 128 ? launch_dense_tc_t<128>(ma_hi, ma_lo, mb_hi, mb_lo, p, st)
-                     : launch_dense_tc_t<64>(ma_hi, ma_lo, mb_hi, mb_lo, p, st);
+    return bn == 128 ? launch_dense_tc_t<128>(p, st) : launch_dense_tc_t<64>(p, st);
 }
 
-// fp32 -> (hi, lo) bf16 split of a flat array: hi = rn(v), lo = rn(v - hi)
-__global__ void split_bf16_kernel(const float* __restrict__ src, __nv_bfloat16* __restrict__ hi,
-                                  __nv_bfloat16* __restrict__ lo, size_t n) {
-    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (size_t)gridDim.x * blockDim.x) {
-        const float v = src[i];
-        const __nv_bfloat16 h = __float2bfloat16_rn(v);
-        hi[i] = h;
-        lo[i] = __float2bfloat16_rn(v - __bfloat162float(h));
+// fp32 [rows, cols] (leading dimension ld_src) -> bf16 (hi, lo) of leading dimension ld_dst; a flat array is one row
+__global__ void split_bf16_kernel(const float* __restrict__ src, size_t ld_src, size_t rows, size_t cols,
+                                  __nv_bfloat16* __restrict__ hi, __nv_bfloat16* __restrict__ lo, size_t ld_dst) {
+    const size_t total = rows * cols;
+    for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const size_t r = rows == 1 ? 0 : i / cols;         // no 64-bit division for a flat array
+        const size_t c = i - r * cols;
+        split_bf16(src[r * ld_src + c], hi[r * ld_dst + c], lo[r * ld_dst + c]);
     }
 }
 
-int launch_split_bf16(const float* src, void* hi, void* lo, size_t n, cudaStream_t st) {
-    if (n == 0) return TB2_OK;
-    // grid-stride over at most 1184 CTAs of 256 threads (about 9 per SM of a 132-SM H100: one resident wave)
-    const unsigned blocks = (unsigned)std::min<size_t>((n + 255) / 256, 1184);
-    split_bf16_kernel<<<blocks, 256, 0, st>>>(src, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo, n);
+int launch_split_bf16_rows(const float* src, size_t ld_src, size_t rows, size_t cols, void* hi, void* lo, size_t ld_dst,
+                           unsigned max_blocks, cudaStream_t st) {
+    if (rows * cols == 0) return TB2_OK;
+    const unsigned blocks = (unsigned)std::min<size_t>((rows * cols + 255) / 256, max_blocks);
+    split_bf16_kernel<<<blocks, 256, 0, st>>>(src, ld_src, rows, cols, (__nv_bfloat16*)hi, (__nv_bfloat16*)lo, ld_dst);
     TB2_LAUNCH_CHECK();
     return TB2_OK;
+}
+
+int launch_split_bf16(const float* src, void* hi, void* lo, size_t n, cudaStream_t st) {
+    // at most 1184 CTAs of 256 threads (about 9 per SM of a 132-SM H100: one resident wave)
+    return launch_split_bf16_rows(src, n, 1, n, hi, lo, n, 1184, st);
 }
 
 }  // namespace tb2

@@ -178,9 +178,7 @@ __global__ void __launch_bounds__(kPrepMaxThreads, 2) pool_prepare_kernel(PrepPa
                 const float gx = n != 0.f ? dx / n : 0.f, gy = n != 0.f ? dy / n : 0.f;
                 e = fmaxf(fmaf(p.Wg[2 * kg + 1], gy * 4.0f, fmaf(p.Wg[2 * kg], gx * 4.0f, p.bg[kg])), 0.f);
             }
-            const __nv_bfloat16 h = __float2bfloat16_rn(e);
-            p.emb_hi[(size_t)(row0 + j) * EW + k] = h;
-            p.emb_lo[(size_t)(row0 + j) * EW + k] = __float2bfloat16_rn(e - __bfloat162float(h));
+            split_bf16(e, p.emb_hi[(size_t)(row0 + j) * EW + k], p.emb_lo[(size_t)(row0 + j) * EW + k]);
         }
     }
     if (fast_lat) {
@@ -585,9 +583,7 @@ __global__ void __launch_bounds__(kL1Threads, 1) sparse_layer1_kernel(L1Params p
             if (p.relu) v = fmaxf(v, 0.f);
             const size_t o = (size_t)(row0 + r) * p.OUT + col;
             if (p.out_hi) {
-                const __nv_bfloat16 h = __float2bfloat16_rn(v);
-                p.out_hi[o] = h;
-                p.out_lo[o] = __float2bfloat16_rn(v - __bfloat162float(h));
+                split_bf16(v, p.out_hi[o], p.out_lo[o]);
             } else {
                 p.out[o] = v;
             }
@@ -741,11 +737,9 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
 #pragma unroll
         for (int i = 0; i < 4; ++i) {
             const float v = r <= P ? vk[i] - p.constant : 0.f;
-            const __nv_bfloat16 h = __float2bfloat16_rn(v);
             const int kp = kperm16(k0 + i);                           // = 4 t + i
             const int dst = row * 32 + (kp >> 2) * 8 + (kp & 3);
-            lat[dst] = h;
-            lat[dst + 4] = __float2bfloat16_rn(v - __bfloat162float(h));
+            split_bf16(v, lat[dst], lat[dst + 4]);
         }
     }
     cp_async_wait_all();
@@ -945,10 +939,7 @@ __global__ void __launch_bounds__(kMmaThreads, 1) sparse_layer1_mma_kernel(L1Mma
         if (p.out_hi) {
             __align__(8) __nv_bfloat16 h[4], l[4];
 #pragma unroll
-            for (int x = 0; x < 4; ++x) {
-                h[x] = __float2bfloat16_rn(v[x]);
-                l[x] = __float2bfloat16_rn(v[x] - __bfloat162float(h[x]));
-            }
+            for (int x = 0; x < 4; ++x) split_bf16(v[x], h[x], l[x]);
             if (vec) {
                 if (ocol < p.OUT) {
                     *reinterpret_cast<uint2*>(p.out_hi + o) = *reinterpret_cast<const uint2*>(h);
@@ -1008,11 +999,9 @@ __global__ void repack_layer1_mma_kernel(const float* __restrict__ W1, __nv_bflo
         const size_t co = idx >> 4;
         const int o = (int)(co % OUT), cell = (int)(co / OUT);
         const float v = W1[(size_t)o * 16 * cells + (size_t)c * cells + cell];
-        const __nv_bfloat16 h = __float2bfloat16_rn(v);
         const int kp = kperm16(c);                      // = 4 t + i
         const size_t dst = (co << 5) + (size_t)(kp >> 2) * 8 + (kp & 3);
-        hi[dst] = h;                                    // `hi` holds the interleaved (hi | lo) slabs
-        hi[dst + 4] = __float2bfloat16_rn(v - __bfloat162float(h));
+        split_bf16(v, hi[dst], hi[dst + 4]);            // `hi` holds the interleaved (hi | lo) slabs
         (void)lo;
     }
 }
@@ -1112,11 +1101,7 @@ __global__ void __launch_bounds__(kRowsThreads, 1) pool_rows_kernel(RowsParams p
         }
         if (p.relu) acc = fmaxf(acc, 0.f);
         const size_t o = (size_t)(r0 + r) * p.OUT + col;
-        if (p.out_hi) {
-            const __nv_bfloat16 h = __float2bfloat16_rn(acc);
-            p.out_hi[o] = h;
-            p.out_lo[o] = __float2bfloat16_rn(acc - __bfloat162float(h));
-        }
+        if (p.out_hi) split_bf16(acc, p.out_hi[o], p.out_lo[o]);
         if (p.out) p.out[o] = acc;
     }
 }

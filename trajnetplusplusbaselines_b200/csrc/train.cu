@@ -671,13 +671,6 @@ __global__ void __launch_bounds__(256) social_dgrid_kernel(const unsigned* __res
 // contiguous bytes of a dz1 row per load) and are split into (hi, lo) in registers.  The FFMA version above needed
 // five shared-memory loads per 16 FMAs and ran at 8.6 TFLOP/s.
 // ------------------------------------------------------------------------------------------
-__device__ __forceinline__ void split2(const float2 v, uint32_t& hi, uint32_t& lo) {
-    const __nv_bfloat162 h = __floats2bfloat162_rn(v.x, v.y);
-    const __nv_bfloat162 l = __floats2bfloat162_rn(v.x - __low2float(h), v.y - __high2float(h));
-    hi = *reinterpret_cast<const uint32_t*>(&h);
-    lo = *reinterpret_cast<const uint32_t*>(&l);
-}
-
 constexpr int kDmPairs = 64, kDmYs = 8;
 static size_t dgrid_mma_smem(int d1) { return (size_t)2 * 16 * (d1 + 8) * sizeof(__nv_bfloat16) + 4 * 16 * 16 * sizeof(float) + kDmPairs * sizeof(int); }
 
@@ -722,7 +715,8 @@ __global__ void __launch_bounds__(256) social_dgrid_mma_kernel(const unsigned* _
             const float2 v01 = a0p ? *reinterpret_cast<const float2*>(a0p + k0 + 8) : z2;
             const float2 v11 = a1p ? *reinterpret_cast<const float2*>(a1p + k0 + 8) : z2;
             uint32_t ah[4], al[4];
-            split2(v00, ah[0], al[0]); split2(v10, ah[1], al[1]); split2(v01, ah[2], al[2]); split2(v11, ah[3], al[3]);
+            split_bf16x2(v00, ah[0], al[0]); split_bf16x2(v10, ah[1], al[1]);
+            split_bf16x2(v01, ah[2], al[2]); split_bf16x2(v11, ah[3], al[3]);
 #pragma unroll
             for (int nt = 0; nt < 2; ++nt) {
                 const uint32_t h0 = bh0[nt * ldw2 + k0 / 2], h1 = bh0[nt * ldw2 + k0 / 2 + 4];
@@ -842,10 +836,10 @@ __global__ void __launch_bounds__(256) social_dw1_mma_kernel(const unsigned* __r
             if (ks * 16 >= nb) break;
             const int kb = ks * 16;
             uint32_t ah[4], al[4];
-            split2(make_float2(lat_s[kb + 2 * t][g], lat_s[kb + 2 * t + 1][g]), ah[0], al[0]);
-            split2(make_float2(lat_s[kb + 2 * t][g + 8], lat_s[kb + 2 * t + 1][g + 8]), ah[1], al[1]);
-            split2(make_float2(lat_s[kb + 2 * t + 8][g], lat_s[kb + 2 * t + 9][g]), ah[2], al[2]);
-            split2(make_float2(lat_s[kb + 2 * t + 8][g + 8], lat_s[kb + 2 * t + 9][g + 8]), ah[3], al[3]);
+            split_bf16x2(make_float2(lat_s[kb + 2 * t][g], lat_s[kb + 2 * t + 1][g]), ah[0], al[0]);
+            split_bf16x2(make_float2(lat_s[kb + 2 * t][g + 8], lat_s[kb + 2 * t + 1][g + 8]), ah[1], al[1]);
+            split_bf16x2(make_float2(lat_s[kb + 2 * t + 8][g], lat_s[kb + 2 * t + 9][g]), ah[2], al[2]);
+            split_bf16x2(make_float2(lat_s[kb + 2 * t + 8][g + 8], lat_s[kb + 2 * t + 9][g + 8]), ah[3], al[3]);
             const float* r0 = dz1 + (size_t)row_s[kb + 2 * t] * d1 + obase + g;
             const float* r1 = dz1 + (size_t)row_s[kb + 2 * t + 1] * d1 + obase + g;
             const float* r2 = dz1 + (size_t)row_s[kb + 2 * t + 8] * d1 + obase + g;
@@ -853,8 +847,8 @@ __global__ void __launch_bounds__(256) social_dw1_mma_kernel(const unsigned* __r
 #pragma unroll
             for (int nt = 0; nt < 4; ++nt) {
                 uint32_t bh0, bl0, bh1, bl1;
-                split2(make_float2(__ldg(r0 + nt * 8), __ldg(r1 + nt * 8)), bh0, bl0);
-                split2(make_float2(__ldg(r2 + nt * 8), __ldg(r3 + nt * 8)), bh1, bl1);
+                split_bf16x2(make_float2(__ldg(r0 + nt * 8), __ldg(r1 + nt * 8)), bh0, bl0);
+                split_bf16x2(make_float2(__ldg(r2 + nt * 8), __ldg(r3 + nt * 8)), bh1, bl1);
                 mma_bf16_16816(acc[nt], ah, bh0, bh1);
                 mma_bf16_16816(acc[nt], al, bh0, bh1);
                 mma_bf16_16816(acc[nt], ah, bl0, bl1);
@@ -1276,19 +1270,6 @@ static size_t carve_bwd(const tb2_lstm* m, size_t R, size_t S, size_t M, void* b
 }
 
 
-// fp32 window [rows x cols] (leading dimension ld_src) -> bf16 (hi, lo) at column col_off of a [rows x ld_dst] matrix
-__global__ void split2d_kernel(const float* __restrict__ src, int ld_src, int rows, int cols, __nv_bfloat16* __restrict__ hi,
-                               __nv_bfloat16* __restrict__ lo, int ld_dst, int col_off) {
-    const size_t total = (size_t)rows * cols;
-    for (size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
-        const size_t r = idx / cols;
-        const int c = (int)(idx - r * cols);
-        const float v = src[r * ld_src + c];
-        const __nv_bfloat16 h = __float2bfloat16_rn(v);
-        hi[r * ld_dst + col_off + c] = h;
-        lo[r * ld_dst + col_off + c] = __float2bfloat16_rn(v - __bfloat162float(h));
-    }
-}
 // src [R x Cc] row-major -> bf16 (hi, lo) of its transpose [Cc x R] (weights: a few hundred KB, once per backward)
 __global__ void transpose_split_kernel(const float* __restrict__ src, int R, int Cc, __nv_bfloat16* __restrict__ hi,
                                        __nv_bfloat16* __restrict__ lo) {
@@ -1296,20 +1277,14 @@ __global__ void transpose_split_kernel(const float* __restrict__ src, int R, int
     for (size_t idx = (size_t)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
         const size_t c = idx / R;
         const int r = (int)(idx - c * R);
-        const float v = src[(size_t)r * Cc + c];
-        const __nv_bfloat16 h = __float2bfloat16_rn(v);
-        hi[idx] = h;
-        lo[idx] = __float2bfloat16_rn(v - __bfloat162float(h));
+        split_bf16(src[(size_t)r * Cc + c], hi[idx], lo[idx]);
     }
 }
+// fp32 window [rows x cols] (leading dimension ld_src) -> bf16 (hi, lo) at column col_off of a [rows x ld_dst] matrix
 static int split2d(const float* src, int ld_src, size_t rows, int cols, __nv_bfloat16* hi, __nv_bfloat16* lo, int ld_dst,
                    int col_off, cudaStream_t st) {
     KernelTimer kt("bwd_split", st);
-    const size_t total = rows * (size_t)cols;
-    const unsigned blocks = (unsigned)std::min<size_t>((total + 255) / 256, 148 * 16);
-    split2d_kernel<<<blocks, 256, 0, st>>>(src, ld_src, (int)rows, cols, hi, lo, ld_dst, col_off);
-    TB2_LAUNCH_CHECK();
-    return TB2_OK;
+    return launch_split_bf16_rows(src, ld_src, rows, cols, hi + col_off, lo + col_off, ld_dst, 148 * 16, st);
 }
 
 struct SocBuffers : RowRecords {

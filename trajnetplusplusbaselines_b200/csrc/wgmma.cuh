@@ -1,5 +1,6 @@
-// Hopper (sm_90a) building blocks of the tensor-core kernels: mbarrier, TMA tile loads and
-// warpgroup MMA (wgmma) on bf16 operands in 128-byte-swizzled, K-major shared-memory tiles.
+// Hopper (sm_90a) building blocks of the tensor-core kernels: mbarrier, TMA tile loads,
+// warpgroup MMA (wgmma) on bf16 operands in 128-byte-swizzled, K-major shared-memory tiles, and
+// TcRing, the 3-pass mainloop dense_layer_tc and lstm_gates_tc share.
 //
 // Tile layout (written by TMA with CU_TENSOR_MAP_SWIZZLE_128B): rows of 64 bf16 (128 bytes),
 // 8-row atoms of 1024 bytes, so a tile must start on a 1024-byte boundary (SWIZZLE_64B: rows of 32
@@ -12,11 +13,14 @@
 #include <cuda.h>
 #include <stdint.h>
 
-// TB2_GEMM_ABLATE (scripts/step_gemm_ablate.py, timing only, results wrong) takes one part out of the mainloops of
-// dense_layer_tc and lstm_gates_tc: 1 = no wgmma (loads and barriers only), 2 = one stage loaded, every k-block reads
-// it (wgmma issue without the L2 operand stream), 3 = no epilogue stores (nor the arithmetic that feeds them),
-// 4 = one wgmma group in flight: wait_group 1 after committing k-block kb, then kb - 1's stage released.  Unset in
-// the library, which waits for each k-block's group before releasing its stage: the variant was no faster (DESIGN §8).
+#include "common.cuh"
+
+// TB2_GEMM_ABLATE (scripts/step_gemm_ablate.py, timing only, results wrong) takes one part out of dense_layer_tc and
+// lstm_gates_tc: 1 = no wgmma (loads and barriers only), 2 = one stage loaded, every k-block reads it (wgmma issue
+// without the L2 operand stream), 3 = no epilogue stores (nor the arithmetic that feeds them), 4 = one wgmma group in
+// flight: wait_group 1 after committing k-block kb, then kb - 1's stage released.  1, 2 and 4 act in TcRing, 3 in the
+// kernels' epilogues.  Unset in the library, which waits for each k-block's group before releasing its stage: the
+// variant was no faster (DESIGN §8).
 #ifndef TB2_GEMM_ABLATE
 #define TB2_GEMM_ABLATE 0
 #endif
@@ -133,5 +137,95 @@ __device__ __forceinline__ void wgmma_bf16(float (&d)[128], uint64_t a, uint64_t
           "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
         : "l"(a), "l"(b), "r"(accumulate));
 }
+
+// k-block kb's A operand in TcRing: the tiles at (col, m0) of `map`
+struct TcATile {
+    const SplitMap* map;
+    int col;
+};
+
+// The 3-pass mainloop of dense_layer_tc and lstm_gates_tc, 384 threads.  Thread 256 (warpgroup 2) streams k-block kb's
+// tiles, A_hi / A_lo [BM, BK] and W_hi / W_lo [BN, BK] (bf16, K-major, 2 BK-byte swizzled rows), into a ring of kStages
+// stages, each guarded by a tx-counted full barrier and an empty barrier that every consumer warp arrives on.
+// Warpgroups 0 and 1 multiply rows [64 wg, 64 wg + 64) into acc: per k16 step A_hi.W_hi (overwriting acc at the first),
+// A_hi.W_lo, A_lo.W_hi, one commit per k-block, waited for before the stage is released.
+template <int BM, int BN, int BK, int kStages>
+struct TcRing {
+    static_assert(BM == 128, "two consumer warpgroups of 64 rows");
+    static constexpr uint32_t kABytes = BM * BK * 2;
+    static constexpr uint32_t kBBytes = BN * BK * 2;
+    static constexpr uint32_t kStageBytes = 2 * kABytes + 2 * kBBytes;
+    static constexpr uint32_t kRingBytes = kStages * kStageBytes;
+    static constexpr size_t kSmemBytes = kRingBytes + 1024;       // dynamic shared memory: + slack to align the ring
+
+    uint64_t full_bar[kStages];
+    uint64_t empty_bar[kStages];
+
+    // thread 0, before the __syncthreads that precedes run()
+    __device__ __forceinline__ void init() {
+        for (int s = 0; s < kStages; ++s) {
+            mbar_init(smem_u32(&full_bar[s]), 1);
+            mbar_init(smem_u32(&empty_bar[s]), 8);
+        }
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+
+    // every thread: a_tile(kb) is k-block kb's TcATile, W's tiles are at (kb * BK, n0).  Returns with the warps
+    // converged and, in warpgroups 0 and 1, the product in acc.
+    template <class ATileOf>
+    __device__ __forceinline__ void run(uint32_t ring, int num_kb, int m0, ATileOf a_tile, const SplitMap& w, int n0,
+                                        float (&acc)[BN / 2]) {
+        const int wg = threadIdx.x >> 7, lane = threadIdx.x & 31;
+        if (wg == 2) {
+            if (threadIdx.x == 256) {
+                for (int kb = 0; kb < (TB2_GEMM_ABLATE == 2 ? 1 : num_kb); ++kb) {
+                    const int s = kb % kStages;
+                    const uint32_t phase = (kb / kStages) & 1;
+                    mbar_wait(smem_u32(&empty_bar[s]), phase ^ 1);
+                    const uint32_t bar = smem_u32(&full_bar[s]);
+                    const uint32_t base = ring + s * kStageBytes;
+                    mbar_expect_tx(bar, kStageBytes);
+                    const TcATile a = a_tile(kb);
+                    tma_load_2d(base, &a.map->hi, bar, a.col, m0);
+                    tma_load_2d(base + kABytes, &a.map->lo, bar, a.col, m0);
+                    tma_load_2d(base + 2 * kABytes, &w.hi, bar, kb * BK, n0);
+                    tma_load_2d(base + 2 * kABytes + kBBytes, &w.lo, bar, kb * BK, n0);
+                }
+            }
+            __syncwarp();
+            return;
+        }
+#pragma unroll
+        for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+        const uint32_t a_off = (uint32_t)wg * 64 * 2 * BK;        // this warpgroup's 64 rows of the A tiles
+        for (int kb = 0; kb < num_kb; ++kb) {
+            const int s = TB2_GEMM_ABLATE == 2 ? 0 : kb % kStages;
+            const uint32_t phase = TB2_GEMM_ABLATE == 2 ? 0 : (kb / kStages) & 1;
+            mbar_wait(smem_u32(&full_bar[s]), phase);
+            const uint32_t base = ring + s * kStageBytes;
+            const uint64_t a_hi = wgmma_desc<2 * BK>(base + a_off);
+            const uint64_t a_lo = wgmma_desc<2 * BK>(base + kABytes + a_off);
+            const uint64_t b_hi = wgmma_desc<2 * BK>(base + 2 * kABytes);
+            const uint64_t b_lo = wgmma_desc<2 * BK>(base + 2 * kABytes + kBBytes);
+            wgmma_fence();
+#pragma unroll
+            for (int k = 0; k < (TB2_GEMM_ABLATE == 1 ? 0 : BK / 16); ++k) {
+                const uint64_t adv = (uint64_t)((k * 16 * 2) >> 4);      // 32 bytes per K step
+                wgmma_bf16(acc, a_hi + adv, b_hi + adv, (kb | k) != 0);
+                wgmma_bf16(acc, a_hi + adv, b_lo + adv, 1u);
+                wgmma_bf16(acc, a_lo + adv, b_hi + adv, 1u);
+            }
+            wgmma_commit();
+#if TB2_GEMM_ABLATE == 4
+            wgmma_wait<1>();
+            if (kb > 0 && lane == 0) mbar_arrive(smem_u32(&empty_bar[(kb - 1) % kStages]));
+#else
+            wgmma_wait<0>();
+            if (lane == 0) mbar_arrive(smem_u32(&empty_bar[s]));        // this warp no longer reads the stage
+#endif
+        }
+        wgmma_wait<0>();
+    }
+};
 
 }  // namespace tb2
