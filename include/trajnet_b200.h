@@ -68,7 +68,8 @@ extern "C" {
 
 const char* tb2_last_error(void);
 /* 106: one step call (tb2_lstm_step_forward) and one step-range call (tb2_lstm_forward_steps) take the goal, external
- * module, sampling, training-cache and host-output arguments that separate entry points took before. */
+ * module, sampling, training-cache and host-output arguments that separate entry points took before.
+ * 107: tb2_lstm_rollout_backward, tb2_attack_objective and tb2_attack_step. */
 int tb2_version(void);
 /* Number of library kernel launches issued by this process so far (bench "gpu_launches"). */
 uint64_t tb2_launch_count(void);
@@ -389,6 +390,28 @@ int tb2_lstm_sequence_backward(const tb2_lstm* model, const tb2_layout* layout, 
                                void* bwd_workspace_dev, size_t bwd_workspace_bytes, const void* cache_dev,
                                size_t cache_bytes, void* stream);
 
+/* Backward of a free-running forward (tb2_lstm_forward_steps with truth = NULL and a training cache for social pooling)
+ * on the graph where nothing is detached (version 107): the decoder's fed-back positions carry gradient.  Decoder step
+ * S_enc reads obs1 = observed[-1] (the scene primaries: positions[S_enc - 2], lstm.py:240-241) and
+ * obs2 = positions[S_enc - 1]; step S_enc + k (k >= 1) reads positions[S_enc + k - 2] and positions[S_enc + k - 1];
+ * every step outputs positions[s] = obs2 + mu.  A decoder input gets gradient through the same paths an encoder input
+ * does: the velocity input, the directional grid's relative velocities and pos = obs2 + mu (cell binning is piecewise
+ * constant: no gradient).  Same arguments as tb2_lstm_sequence_backward without truth, and:
+ *   d_normals_dev    [S, M, 5] gradient wrt rel_pred_scene alone (nothing added by the caller)
+ *   d_positions_dev  [S + (obs_length == 2), M, 2] gradient wrt LSTM.forward's pred_scene (at obs_length 2 it begins
+ *                    with observed[-1] itself)
+ *   grads->d_observed  required; the parameter gradients include the fed-back terms.
+ * active_rows: tracks with a non-zero d_normals or d_positions row; directional pooling couples the tracks of a scene
+ * through the relative velocities, so there every track must be listed (social pooling runs on all rows anyway).
+ * Workspace: tb2_lstm_backward_workspace_bytes.  Goal models: TB2_ERR_UNSUPPORTED. */
+int tb2_lstm_rollout_backward(const tb2_lstm* model, const tb2_layout* layout, const tb2_lstm_weights* weights,
+                              const float* observed_dev, int32_t obs_length, int32_t n_decode,
+                              const float* positions_dev, const float* states_dev, const float* d_normals_dev,
+                              const float* d_positions_dev, const int32_t* active_rows_dev, int32_t num_active,
+                              const tb2_lstm_grads* grads, void* workspace_dev, size_t workspace_bytes,
+                              void* bwd_workspace_dev, size_t bwd_workspace_bytes, const void* cache_dev,
+                              size_t cache_bytes, void* stream);
+
 /* Backward of one tb2_lstm_step_forward step of a TB2_POOL_EXTERNAL model, from the step's inputs: the gate
  * pre-activations are recomputed (one GEMM), then
  *   d_h_in_dev, d_c_in_dev  [M, H]                gradient wrt h_in / c_in (absent tracks: d_h_out / d_c_out unchanged)
@@ -434,6 +457,26 @@ int tb2_l2_loss(const float* inputs_dev, const float* targets_dev, const int32_t
  * (gradient wrt the primary's position, optional). */
 int tb2_collision_loss(const tb2_layout* layout, const float* positions_dev, int32_t T, float col_wt,
                        float col_distance, float* loss_out_dev, float* dprimary_out_dev, void* stream);
+
+/* Collision attack on free-running forecasts (attack.py), one launch each, no atomics.
+ * tb2_attack_objective -- per scene D_out [B] (double) = the smallest distance between the primary's and any neighbour's
+ *   positions at the points the scorer's Col-I test samples (tb2_score_scenes): frames [first_frame, num_frames) of
+ *   positions [num_frames, M, 2] where both tracks are finite, each segment between consecutive such frames sampled at
+ *   linspace(p_prev, p_t, 3) on both tracks.  D <= 0.2 m exactly when Col-I fires on the same values.  A scene without a
+ *   finite pair gets +inf.  d_positions_out [num_frames, M, 2] = the subgradient of D at the first minimiser in
+ *   (neighbour, frame, sample) order on the four segment endpoints (0 elsewhere, and for D = +inf or D = 0).
+ * tb2_attack_step -- per scene: when D [B] < best_D [B] (in/out; start at +inf) the iterate is recorded: best_D, the
+ *   primary's delta [obs_length, B, 2] into best_delta and the scene's rows of positions [num_frames, M, 2] into
+ *   best_positions.  Then with move != 0, unless best_D <= 0.2 m, every observed frame t of the primary whose position
+ *   and gradient g_t = d_observed[t, primary] are finite and g_t != 0 steps:
+ *   delta_t <- proj_eps(delta_t - alpha g_t / |g_t|) (L2 ball of radius eps per frame), and observed_adv
+ *   [obs_length, M, 2] gets observed + delta on the primary rows (its other rows are the caller's). */
+int tb2_attack_objective(const tb2_layout* layout, const float* positions_dev, int32_t num_frames, int32_t first_frame,
+                         double* D_out_dev, float* d_positions_out_dev, void* stream);
+int tb2_attack_step(const tb2_layout* layout, const float* d_observed_dev, const float* observed_dev, int32_t obs_length,
+                    float* delta_dev, const double* D_dev, int32_t num_frames, const float* positions_dev,
+                    double* best_D_dev, float* best_delta_dev, float* best_positions_dev, float* observed_adv_dev,
+                    float eps, float alpha, int32_t move, void* stream);
 
 /* ---------------------------------------------------------------------------------------
  * Scene preprocessing on the device (SURVEY.md 8f rank 3): the O(T * M) NumPy passes the reference runs scene by scene

@@ -1041,6 +1041,41 @@ __global__ void __launch_bounds__(256) input_grad_kernel(
     }
 }
 
+// ------------------------------------------------------------------------------------------
+// Position chain of the rollout backward (tb2_lstm_rollout_backward): step s outputs pos[s] = obs2_s + mu_s, and a
+// decoder step reads obs2_s = pos[s - 1] and obs1_s = pos[s - 2] (its first step: observed[-1], primaries pos[s - 2]).
+// dp [S][M][2] collects d pos[s] from the caller and from the later steps' inputs; dn [S][M][5] is the caller's
+// d_normals that the cell kernel of step s reads.
+// ------------------------------------------------------------------------------------------
+// before step s's cell kernel: d mu_s += d pos[s], and d obs2_s += d pos[s] (dp[s - 1] or observed[s + 1]: `up`)
+__global__ void rollout_fold_kernel(const float2* __restrict__ dp_s, float* __restrict__ dn_s, float2* __restrict__ up,
+                                    int M) {
+    const int m = blockIdx.x * blockDim.x + threadIdx.x;
+    if (m >= M) return;
+    const float2 d = dp_s[m];
+    dn_s[(size_t)m * 5] += d.x;
+    dn_s[(size_t)m * 5 + 1] += d.y;
+    up[m].x += d.x;
+    up[m].y += d.y;
+}
+
+// the first decoder step's d obs1 (`d1`): the primaries read pos[s - 2] (dp_m2; null when that is observed[-1]), every
+// other track observed[-1]
+__global__ void rollout_route_kernel(const float2* __restrict__ d1, const int* __restrict__ row_scene,
+                                     const int* __restrict__ scene_off, float2* __restrict__ dp_m2,
+                                     float2* __restrict__ d_last, int M) {
+    const int m = blockIdx.x * blockDim.x + threadIdx.x;
+    if (m >= M) return;
+    float2* t = (dp_m2 && scene_off[row_scene[m]] == m) ? dp_m2 + m : d_last + m;
+    t->x += d1[m].x;
+    t->y += d1[m].y;
+}
+
+__global__ void add_kernel(float* __restrict__ dst, const float* __restrict__ src, size_t n) {
+    const size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) dst[i] += src[i];
+}
+
 }  // namespace tb2
 
 using namespace tb2;
@@ -1253,9 +1288,21 @@ static void carve_records(const tb2_lstm* m, size_t rows, size_t S, size_t extra
     o->masked = reinterpret_cast<int*>(c.take(S * rows));
 }
 
+// The rollout backward's position chain (rollout_fold_kernel): dn [S][M][5], dp [S][M][2], d1 [M][2]
+struct RolloutBuffers {
+    float *dn, *dp, *d1;
+};
+
+static void carve_rollout(size_t S, size_t M, Carve& c, RolloutBuffers* o) {
+    o->dn = c.take(S * M * 5);
+    o->dp = c.take(S * M * 2);
+    o->d1 = c.take(M * 2);
+}
+
 struct BwdBuffers : RowRecords {
     float* G;                                      // [S][R][C n n] grid rows
     int* row_of;                                   // [M] record row of each track, -1: none (d observed)
+    RolloutBuffers ro;
 };
 
 static size_t carve_bwd(const tb2_lstm* m, size_t R, size_t S, size_t M, void* base, BwdBuffers* b) {
@@ -1266,6 +1313,7 @@ static size_t carve_bwd(const tb2_lstm* m, size_t R, size_t S, size_t M, void* b
     carve_records(m, R, S, P * CG, c, o);
     o->G = c.take(P ? S * R * CG : 4);
     o->row_of = reinterpret_cast<int*>(c.take(M));
+    carve_rollout(S, M, c, &o->ro);
     return c.bytes();
 }
 
@@ -1301,6 +1349,7 @@ struct SocBuffers : RowRecords {
     __nv_bfloat16 *WihT_hi[2], *WihT_lo[2];               // [E + P][G4]
     __nv_bfloat16 *W2T_hi, *W2T_lo;                       // [d1][P]
     float* zero_bias;                                     // [max(d1, G4)]
+    RolloutBuffers ro;
 };
 
 static size_t carve_social(const tb2_lstm* m, const tb2_layout* l, size_t S, void* basep, SocBuffers* b) {
@@ -1342,6 +1391,7 @@ static size_t carve_social(const tb2_lstm* m, const tb2_layout* l, size_t S, voi
     o->W2T_hi = take_bf16(d1 * P);
     o->W2T_lo = take_bf16(d1 * P);
     o->zero_bias = c.take(d1 > G4 ? d1 : G4);
+    carve_rollout(S, M, c, &o->ro);
     return c.bytes();
 }
 
@@ -1366,11 +1416,14 @@ static int gate_preactivations(const tb2_lstm* m, const RowRecords& b, int rows,
     return TB2_OK;
 }
 
+constexpr int kAllPhases = (1 << TB2_PHASE_ENCODER) | (1 << TB2_PHASE_DECODER);
+
 // LSTM, Hidden2Normal and InputEmbedding weight gradients: one reduction over all S * rows (step, row) records per
-// tensor.  input_grads: each cell first computes dX_in = dgates . W_ih of all its steps (the social backward computes
-// dX_in step by step inside its time loop instead, where the grid MLP's backward needs it).
+// tensor.  dxin_phases (bit 1 << phase): those cells first compute dX_in = dgates . W_ih of all their steps (the social
+// backward, and the rollout backward's decoder, compute dX_in step by step inside the time loop instead, where the grid
+// MLP's backward or the position chain needs it).
 static int lstm_weight_grads(const tb2_lstm* m, const tb2_lstm_weights* w, const tb2_lstm_grads* g, const RowRecords& b,
-                             int rows, int S, int S_enc, bool input_grads, cudaStream_t st) {
+                             int rows, int S, int S_enc, int dxin_phases, cudaStream_t st) {
     const int K = m->K_gate, E = m->E, EP = E + m->P, H = m->H, G4 = 4 * H;
     int rc;
     for (int phase = 0; phase < 2; ++phase) {
@@ -1382,7 +1435,7 @@ static int lstm_weight_grads(const tb2_lstm* m, const tb2_lstm_weights* w, const
         const float* X = b.X + (size_t)s0 * rows * K;
         const int n = ns * rows;
         // dX_in = dgates . W_ih   (torch layout [4H, E+P] is the [K = 4H, N = E+P] operand as it stands)
-        if (input_grads && (rc = gemm_nn(DG, G4, enc ? w->encoder_weight_ih : w->decoder_weight_ih, EP,
+        if ((dxin_phases >> phase & 1) && (rc = gemm_nn(DG, G4, enc ? w->encoder_weight_ih : w->decoder_weight_ih, EP,
                                          b.DXIN + (size_t)s0 * rows * EP, EP, n, EP, G4, nullptr, st)))
             return rc;
         if ((rc = gemm_tn(DG, G4, X, K, enc ? g->encoder_weight_ih : g->decoder_weight_ih, EP, n, G4, EP, b.scratch,
@@ -1436,6 +1489,80 @@ static int observed_grads(const tb2_lstm* m, const tb2_layout* l, const RowRecor
                                                            K, DXs, EP, E, m->We, nullptr, nullptr, nm1, nullptr, 0,
                                                            nullptr, d1, d2);
         }
+        TB2_LAUNCH_CHECK();
+    }
+    return TB2_OK;
+}
+
+// Rollout backward: the caller's d normals and d positions into the chain buffers.  At obs_length 2 the positions begin
+// with observed[-1] itself (lstm.py:222-223): that frame's gradient goes straight to d observed.
+static int rollout_begin(const tb2_layout* l, const RolloutBuffers& ro, const float* d_normals, const float* d_positions,
+                         int obs_length, int S, float* d_observed, cudaStream_t st) {
+    const size_t frame = (size_t)l->M * 2;
+    const size_t seed = obs_length == 2 ? 1 : 0;
+    TB2_CHECK_CUDA(cudaMemcpyAsync(ro.dn, d_normals, (size_t)S * l->M * 5 * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    TB2_CHECK_CUDA(cudaMemcpyAsync(ro.dp, d_positions + seed * frame, (size_t)S * frame * sizeof(float),
+                                   cudaMemcpyDeviceToDevice, st));
+    if (seed) {
+        add_kernel<<<(unsigned)((frame + 255) / 256), 256, 0, st>>>(d_observed + (size_t)(obs_length - 1) * frame,
+                                                                    d_positions, frame);
+        TB2_LAUNCH_CHECK();
+    }
+    return TB2_OK;
+}
+
+// Rollout backward, before step s's cell kernel: d pos[s] into d mu_s and into d obs2_s
+static int rollout_fold(const tb2_layout* l, const RolloutBuffers& ro, int s, int S_enc, float* d_observed,
+                        cudaStream_t st) {
+    const size_t M = (size_t)l->M;
+    float* up = s >= S_enc ? ro.dp + (size_t)(s - 1) * M * 2 : d_observed + (size_t)(s + 1) * M * 2;
+    {
+        KernelTimer kt("bwd_rollout_fold", st);
+        rollout_fold_kernel<<<(unsigned)((M + 255) / 256), 256, 0, st>>>((const float2*)(ro.dp + (size_t)s * M * 2),
+                                                                          ro.dn + (size_t)s * M * 5, (float2*)up, (int)M);
+    }
+    TB2_LAUNCH_CHECK();
+    return TB2_OK;
+}
+
+// Rollout backward, right after decoder step s's dX_in (records Xs / DXs / Gs of `rows` rows, row_of: track -> row):
+// d obs2_s into d pos[s - 1] and d obs1_s into d pos[s - 2] (the first decoder step: observed[-1], primaries
+// pos[s - 2]) through input_grad_kernel, which the encoder steps' d observed also uses.  Directional grids rebuild the
+// step's pair table and ReLU-mask the pooled columns of DXs in place first.
+static int rollout_inputs(const tb2_lstm* m, const tb2_layout* l, const RolloutBuffers& ro, const float* Xs, float* DXs,
+                          const float* Gs, int rows, const int* row_of, const float* observed, int obs_length,
+                          const float* positions, const float* states, int s, Workspace& ws, float* d_observed,
+                          cudaStream_t st) {
+    const int K = m->K_gate, E = m->E, P = m->P, EP = E + P;
+    const size_t M = (size_t)l->M;
+    const int nm1 = l->n_max > 1 ? l->n_max - 1 : 1;
+    const int first = s == obs_length - 1;
+    const float *o1, *o2;
+    int phase, rc;
+    if ((rc = resolve_step_inputs(l, observed, obs_length, nullptr, positions, s, &ws, &o1, &o2, &phase, st))) return rc;
+    float* d2 = ro.dp + (size_t)(s - 1) * M * 2;
+    float* d1 = first ? ro.d1 : ro.dp + (size_t)(s - 2) * M * 2;
+    if (first) TB2_CHECK_CUDA(cudaMemsetAsync(ro.d1, 0, M * 2 * sizeof(float), st));
+    if (m->cfg.pool_type == TB2_POOL_DIRECTIONAL) {
+        const float* h_prev = states + ((size_t)(s - 1) * 2 + 0) * M * m->H;
+        if ((rc = launch_pool_prepare(m, l, h_prev, o1, o2, 1, 1, 0, &ws, st))) return rc;
+        relu_mask_kernel<<<(unsigned)(((size_t)rows * P + 255) / 256), 256, 0, st>>>(Xs, K, DXs, EP, rows, E, P);
+        TB2_LAUNCH_CHECK();
+        KernelTimer kt("bwd_input_dir_pairs", st);
+        input_grad_kernel<true><<<l->B, 256, 0, st>>>(l->scene_off, row_of, (const float2*)o1, (const float2*)o2, Xs, K,
+                                                      DXs, EP, E, m->We, ws.pair_cell, ws.pair_flag, nm1, Gs, m->cells,
+                                                      m->Wt1, d1, d2);
+    } else {
+        KernelTimer kt("bwd_input_vel", st);
+        input_grad_kernel<false><<<l->B, 256, 0, st>>>(l->scene_off, row_of, (const float2*)o1, (const float2*)o2, Xs, K,
+                                                       DXs, EP, E, m->We, nullptr, nullptr, nm1, nullptr, 0, nullptr, d1,
+                                                       d2);
+    }
+    TB2_LAUNCH_CHECK();
+    if (first) {
+        rollout_route_kernel<<<(unsigned)((M + 255) / 256), 256, 0, st>>>(
+            (const float2*)ro.d1, l->row_scene, l->scene_off, s >= 2 ? (float2*)(ro.dp + (size_t)(s - 2) * M * 2) : nullptr,
+            (float2*)(d_observed + (size_t)(obs_length - 1) * M * 2), (int)M);
         TB2_LAUNCH_CHECK();
     }
     return TB2_OK;
@@ -1516,8 +1643,8 @@ static int social_step_records(const tb2_lstm* m, const tb2_layout* l, const Soc
 static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lstm_weights* w,
                            const float* observed, int obs_length, const float* truth, int n_decode,
                            const float* positions, const float* states, const float* d_normals,
-                           const tb2_lstm_grads* g, Workspace& ws, void* bwd_workspace, const TrainCache& cache,
-                           cudaStream_t st) {
+                           const float* d_positions, const tb2_lstm_grads* g, Workspace& ws, void* bwd_workspace,
+                           const TrainCache& cache, cudaStream_t st) {
     const int S = obs_length - 1 + n_decode, S_enc = obs_length - 1;
     const int Mi = l->M, K = m->K_gate, E = m->E, P = m->P, EP = E + P, C = m->C, cells = m->cells;
     const int H = m->H, G4 = 4 * H;
@@ -1536,6 +1663,9 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
     TB2_LAUNCH_CHECK();
     int rc;
     if ((rc = launch_split_bf16(m->Wt1, b.Wt1_hi, b.Wt1_lo, (size_t)cells * C * d1, st))) return rc;
+    const bool rollout = d_positions != nullptr;
+    if (rollout && (rc = rollout_begin(l, b.ro, d_normals, d_positions, obs_length, S, g->d_observed, st))) return rc;
+    const float* dnorm = rollout ? b.ro.dn : d_normals;
     // (A) forward quantities of every step: hidden1, X = [emb | pooled | h_prev]
     for (int s = 0; s < S; ++s) {
         const float *o1, *o2;
@@ -1607,12 +1737,13 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
                                      st)))
                 return rc;
         }
+        if (rollout && (rc = rollout_fold(l, b.ro, s, S_enc, g->d_observed, st))) return rc;
         {
             KernelTimer kt("bwd_cell_head", st);
             rc = launch_cell_head(H, Mi, st,
                 b.rows, b.masked + (size_t)s * M, b.GP + (size_t)s * M * G4, c_prev, nullptr, Whh_next, dh_rec,
                 b.pass[cur ^ 1], b.pass[cur], b.dc,
-                d_normals + (size_t)s * M * 5, m->Wn, m->bn, DGs, b.HS + (size_t)s * M * H,
+                dnorm + (size_t)s * M * 5, m->Wn, m->bn, DGs, b.HS + (size_t)s * M * H,
                 b.DN + (size_t)s * M * 8, Mi);
         }
         if (rc) return rc;
@@ -1622,6 +1753,10 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
                                       nullptr, nullptr, Mi, G4, EP, 0, st)))
                 return rc;
         } else if ((rc = gemm_nn(DGs, G4, Wih, EP, DXs, EP, Mi, EP, G4, nullptr, st))) return rc;
+        if (rollout && s >= S_enc &&
+            (rc = rollout_inputs(m, l, b.ro, Xs, DXs, nullptr, Mi, b.rows, observed, obs_length, positions, states, s, ws,
+                                 g->d_observed, st)))
+            return rc;
         const unsigned eb = (unsigned)((M * d1 + 255) / 256);
         if (two) {
             const float* H1s = b.H1 + (size_t)s * M * d1;
@@ -1679,7 +1814,7 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
         if ((rc = colsum(b.DXIN + E, EP, S * Mi, P, g->pool_embedding_bias1, nullptr, b.scratch, b.scratch_floats, st))) return rc;
     }
     // (D) parameter gradients: one reduction over all (step, row) records per tensor
-    if ((rc = lstm_weight_grads(m, w, g, b, Mi, S, S_enc, false, st))) return rc;
+    if ((rc = lstm_weight_grads(m, w, g, b, Mi, S, S_enc, 0, st))) return rc;
     untranspose_add_kernel<<<2048, 256, 0, st>>>(b.dWt1, g->pool_embedding_weight0, cells, C, d1);
     TB2_LAUNCH_CHECK();
     // lat_j = W_enc h_j + b_enc (gridbased_pooling.py:160-167): h of step s-1 is states[s-1]
@@ -1710,12 +1845,13 @@ size_t tb2_lstm_backward_workspace_bytes(const tb2_lstm* m, const tb2_layout* l,
                      (size_t)l->M, nullptr, nullptr);
 }
 
-int tb2_lstm_sequence_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lstm_weights* w,
-                               const float* observed, int32_t obs_length, const float* truth, int32_t n_decode,
-                               const float* positions, const float* states, const float* d_normals,
-                               const int32_t* active_rows, int32_t num_active, const tb2_lstm_grads* g,
-                               void* workspace, size_t workspace_bytes, void* bwd_workspace,
-                               size_t bwd_workspace_bytes, const void* cache, size_t cache_bytes, void* stream) {
+// tb2_lstm_sequence_backward (d_positions = NULL) and tb2_lstm_rollout_backward
+static int sequence_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lstm_weights* w, const float* observed,
+                             int32_t obs_length, const float* truth, int32_t n_decode, const float* positions,
+                             const float* states, const float* d_normals, const float* d_positions,
+                             const int32_t* active_rows, int32_t num_active, const tb2_lstm_grads* g, void* workspace,
+                             size_t workspace_bytes, void* bwd_workspace, size_t bwd_workspace_bytes, const void* cache,
+                             size_t cache_bytes, void* stream) {
     TB2_REQUIRE(m && l && w && g, "null handle");
     TB2_REQUIRE(m->weights_set, "tb2_lstm_set_weights has not been called");
     TB2_REQUIRE(observed && positions && states && d_normals && active_rows, "null argument");
@@ -1748,8 +1884,8 @@ int tb2_lstm_sequence_backward(const tb2_lstm* m, const tb2_layout* l, const tb2
     Workspace ws;
     carve_workspace(m, l, workspace, &ws);
     if (social)      // every track of a scene receives gradient: all rows, active_rows is ignored
-        return social_backward(m, l, w, observed, obs_length, truth, n_decode, positions, states, d_normals, g, ws,
-                               bwd_workspace, tc, st);
+        return social_backward(m, l, w, observed, obs_length, truth, n_decode, positions, states, d_normals, d_positions,
+                               g, ws, bwd_workspace, tc, st);
     const int R = num_active, K = m->K_gate, E = m->E, P = m->P, EP = E + P, H = m->H, G4 = 4 * H;
     const size_t M = (size_t)l->M;
     BwdBuffers b;
@@ -1778,25 +1914,43 @@ int tb2_lstm_sequence_backward(const tb2_lstm* m, const tb2_layout* l, const tb2
         TB2_LAUNCH_CHECK();
     }
     if ((rc = gate_preactivations(m, b, R, S, S_enc, nullptr, st))) return rc;
-    // (C) the sequential chain: one kernel per step
+    if (g->d_observed) {     // the active rows' inputs, and through the directional pairs their neighbours'
+        TB2_CHECK_CUDA(cudaMemsetAsync(b.row_of, 0xff, M * sizeof(int), st));
+        row_of_kernel<<<(R + 255) / 256, 256, 0, st>>>(active_rows, R, b.row_of);
+        TB2_LAUNCH_CHECK();
+    }
+    const bool rollout = d_positions != nullptr;
+    if (rollout && (rc = rollout_begin(l, b.ro, d_normals, d_positions, obs_length, S, g->d_observed, st))) return rc;
+    const float* dnorm = rollout ? b.ro.dn : d_normals;
+    // (C) the sequential chain: one kernel per step (the rollout backward adds its decoder steps' input gradients)
     int cur = 0;
     for (int s = S - 1; s >= 0; --s, cur ^= 1) {
         const float* c_prev = s > 0 ? states + ((size_t)(s - 1) * 2 + 1) * M * H : nullptr;
         const bool last = s == S - 1;
         const int next_phase = (s + 1) < S_enc ? TB2_PHASE_ENCODER : TB2_PHASE_DECODER;
         const float* Whh_next = next_phase == TB2_PHASE_ENCODER ? w->encoder_weight_hh : w->decoder_weight_hh;
+        if (rollout && (rc = rollout_fold(l, b.ro, s, S_enc, g->d_observed, st))) return rc;
         {
             KernelTimer kt("bwd_cell_head", st);
             rc = launch_cell_head(H, R, st,
                 active_rows, b.masked + (size_t)s * R, b.GP + (size_t)s * R * G4, c_prev,
                 last ? nullptr : b.DG + (size_t)(s + 1) * R * G4, Whh_next, nullptr, b.pass[cur ^ 1], b.pass[cur], b.dc,
-                d_normals + (size_t)s * M * 5, m->Wn, m->bn, b.DG + (size_t)s * R * G4,
+                dnorm + (size_t)s * M * 5, m->Wn, m->bn, b.DG + (size_t)s * R * G4,
                 b.HS + (size_t)s * R * H, b.DN + (size_t)s * R * 8, R);
         }
         if (rc) return rc;
+        if (rollout && s >= S_enc) {
+            float* DXs = b.DXIN + (size_t)s * R * EP;
+            if ((rc = gemm_nn(b.DG + (size_t)s * R * G4, G4, w->decoder_weight_ih, EP, DXs, EP, R, EP, G4, nullptr, st)))
+                return rc;
+            if ((rc = rollout_inputs(m, l, b.ro, b.X + (size_t)s * R * K, DXs, pooled ? b.G + (size_t)s * R * CG : nullptr,
+                                     R, b.row_of, observed, obs_length, positions, states, s, ws, g->d_observed, st)))
+                return rc;
+        }
     }
-    // (D) + (E) input gradients of all steps and the parameter gradients: one reduction per tensor
-    if ((rc = lstm_weight_grads(m, w, g, b, R, S, S_enc, true, st))) return rc;
+    // (D) + (E) input gradients of all steps (the rollout's decoder steps have theirs) and the parameter gradients: one
+    // reduction per tensor
+    if ((rc = lstm_weight_grads(m, w, g, b, R, S, S_enc, rollout ? 1 << TB2_PHASE_ENCODER : kAllPhases, st))) return rc;
     if (pooled) {
         relu_mask_kernel<<<(unsigned)(((size_t)S * R * P + 255) / 256), 256, 0, st>>>(b.X, K, b.DXIN, EP, S * R, E, P);
         TB2_LAUNCH_CHECK();
@@ -1806,13 +1960,33 @@ int tb2_lstm_sequence_backward(const tb2_lstm* m, const tb2_layout* l, const tb2
         if ((rc = colsum(b.DXIN + E, EP, S * R, P, g->pool_embedding_bias0, nullptr, b.scratch, b.scratch_floats, st)))
             return rc;
     }
-    if (g->d_observed) {     // the active rows' inputs, and through the directional pairs their neighbours'
-        TB2_CHECK_CUDA(cudaMemsetAsync(b.row_of, 0xff, M * sizeof(int), st));
-        row_of_kernel<<<(R + 255) / 256, 256, 0, st>>>(active_rows, R, b.row_of);
-        TB2_LAUNCH_CHECK();
-        if ((rc = observed_grads(m, l, b, b.G, R, b.row_of, observed, states, S_enc, ws, g->d_observed, st))) return rc;
-    }
+    if (g->d_observed &&
+        (rc = observed_grads(m, l, b, b.G, R, b.row_of, observed, states, S_enc, ws, g->d_observed, st)))
+        return rc;
     return TB2_OK;
+}
+
+int tb2_lstm_sequence_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lstm_weights* w,
+                               const float* observed, int32_t obs_length, const float* truth, int32_t n_decode,
+                               const float* positions, const float* states, const float* d_normals,
+                               const int32_t* active_rows, int32_t num_active, const tb2_lstm_grads* g,
+                               void* workspace, size_t workspace_bytes, void* bwd_workspace,
+                               size_t bwd_workspace_bytes, const void* cache, size_t cache_bytes, void* stream) {
+    return sequence_backward(m, l, w, observed, obs_length, truth, n_decode, positions, states, d_normals, nullptr,
+                             active_rows, num_active, g, workspace, workspace_bytes, bwd_workspace, bwd_workspace_bytes,
+                             cache, cache_bytes, stream);
+}
+
+int tb2_lstm_rollout_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lstm_weights* w, const float* observed,
+                              int32_t obs_length, int32_t n_decode, const float* positions, const float* states,
+                              const float* d_normals, const float* d_positions, const int32_t* active_rows,
+                              int32_t num_active, const tb2_lstm_grads* g, void* workspace, size_t workspace_bytes,
+                              void* bwd_workspace, size_t bwd_workspace_bytes, const void* cache, size_t cache_bytes,
+                              void* stream) {
+    TB2_REQUIRE(g && g->d_observed && d_positions, "the rollout backward needs d_positions and grads->d_observed");
+    return sequence_backward(m, l, w, observed, obs_length, nullptr, n_decode, positions, states, d_normals, d_positions,
+                             active_rows, num_active, g, workspace, workspace_bytes, bwd_workspace, bwd_workspace_bytes,
+                             cache, cache_bytes, stream);
 }
 
 size_t tb2_lstm_step_backward_workspace_bytes(const tb2_lstm* m, const tb2_layout* l) {
@@ -1884,7 +2058,7 @@ int tb2_lstm_step_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
     }
     if (rc) return rc;
     // (D) + (E) dX_in = dgates . W_ih and the step's weight gradients; d h_in through W_hh
-    if ((rc = lstm_weight_grads(m, w, g, b, M, 1, enc ? 1 : 0, true, st))) return rc;
+    if ((rc = lstm_weight_grads(m, w, g, b, M, 1, enc ? 1 : 0, kAllPhases, st))) return rc;
     if ((rc = gemm_nn(b.DG, G4, enc ? w->encoder_weight_hh : w->decoder_weight_hh, H, b.DH, H, M, H, G4, nullptr, st)))
         return rc;
     if (g->d_obs1 || g->d_obs2) {     // d obs1 / d obs2 through the step's velocity input

@@ -1,6 +1,7 @@
 """Drop-in surface of trajnetbaselines.lstm (reference: trajnetbaselines/lstm/__init__.py)."""
 from .loss import PredictionLoss, L2Loss
 from .lstm import LSTM, LSTMPredictor, drop_distant
+from .training import differentiable_rollout
 from .gridbased_pooling import GridBasedPooling
 from .non_gridbased_pooling import HiddenStateMLPPooling, NearestNeighborMLP, AttentionMLPPooling, NearestNeighborLSTM, TrajectronPooling
 
