@@ -69,7 +69,9 @@ extern "C" {
 const char* tb2_last_error(void);
 /* 106: one step call (tb2_lstm_step_forward) and one step-range call (tb2_lstm_forward_steps) take the goal, external
  * module, sampling, training-cache and host-output arguments that separate entry points took before.
- * 107: tb2_lstm_rollout_backward, tb2_attack_objective and tb2_attack_step. */
+ * 107: tb2_lstm_rollout_backward, tb2_attack_objective and tb2_attack_step.
+ * 108: tb2_lstm_sequence_backward and tb2_lstm_rollout_backward skip the reduction of every NULL tb2_lstm_grads
+ *      parameter field (the social backward no longer requires its pool fields). */
 int tb2_version(void);
 /* Number of library kernel launches issued by this process so far (bench "gpu_launches"). */
 uint64_t tb2_launch_count(void);
@@ -332,7 +334,9 @@ int tb2_pool_inputs_padded_backward(const tb2_layout* layout, const float* d_h_p
  * lstm/trainer.py:229-269, through LSTM.forward).  Gradient accumulators are fp32 device
  * buffers in the reference's parameter layout (+=, caller zeroes them).  Zero the whole struct
  * before filling it (memset / `= {0}`): a NULL field is a gradient the call does not compute, and
- * fields appended by later versions then stay NULL.
+ * fields appended by later versions then stay NULL.  tb2_lstm_sequence_backward and tb2_lstm_rollout_backward skip the
+ * reduction of each NULL parameter field (version 108); any of them may be NULL.  d_observed does not depend on which
+ * parameter fields are set (bit for bit), and a field that is set gets the bits of the call with every field set.
  * ------------------------------------------------------------------------------------- */
 typedef struct tb2_lstm_grads {
     float* input_embedding_weight;   /* [E-2, 2] */
@@ -400,7 +404,8 @@ int tb2_lstm_sequence_backward(const tb2_lstm* model, const tb2_layout* layout, 
  *   d_normals_dev    [S, M, 5] gradient wrt rel_pred_scene alone (nothing added by the caller)
  *   d_positions_dev  [S + (obs_length == 2), M, 2] gradient wrt LSTM.forward's pred_scene (at obs_length 2 it begins
  *                    with observed[-1] itself)
- *   grads->d_observed  required; the parameter gradients include the fed-back terms.
+ *   grads->d_observed  required; the parameter gradients include the fed-back terms.  With every parameter field NULL
+ *                    this is the inputs-only call (the collision attack's backward): no parameter reduction runs.
  * active_rows: tracks with a non-zero d_normals or d_positions row; directional pooling couples the tracks of a scene
  * through the relative velocities, so there every track must be listed (social pooling runs on all rows anyway).
  * Workspace: tb2_lstm_backward_workspace_bytes.  Goal models: TB2_ERR_UNSUPPORTED. */

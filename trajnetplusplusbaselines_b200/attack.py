@@ -26,6 +26,11 @@ from .lstm.training import check_rollout
 
 COL_LIMIT = 0.2
 
+PGDResult = collections.namedtuple('PGDResult', 'observed delta d_clean d_best clean positions')
+PGDResult.__doc__ = """All on the device.  observed [T_obs, M, 2] float32: the input with best_delta added to each scene's primary rows;
+delta [T_obs, B, 2] float32: the best iterate's perturbation of each primary; d_clean / d_best [B] float64: D of the
+clean and of the best iterate (+inf: no pair); clean / positions [F, M, 2] float32: the clean and the best iterate's
+free-running positions (differentiable_rollout's)."""
 AttackResult = collections.namedtuple('AttackResult', 'delta predictions clean_predictions d_clean d_attacked')
 AttackResult.__doc__ = """delta [n, obs_length, 2] float64: the primary's perturbation per observed frame (world frame);
 predictions / clean_predictions: per scene {0: [primary [pred_length, 2], neighbours [pred_length, N - 1, 2]]} as
@@ -38,26 +43,23 @@ def _rotate(v, angle):
     return np.stack([v[..., 0] * ct - v[..., 1] * st, v[..., 0] * st + v[..., 1] * ct], axis=-1)
 
 
-def _attack_chunk(model, xys, eps, steps, obs_length, pred_length, normalize_scene):
+def pgd_collision(model, observed, batch_split, pred_length, eps, steps, pad_to_batch_max):
+    """The attack's projected gradient descent on one batch: `observed` [T_obs, M, 2] float32 on the model's device,
+    batch_split [B + 1] (host), `steps` >= 1 iterations of step alpha = 2.5 eps / steps, each scene's primary moved
+    inside a per-frame L2 ball of radius eps.  pad_to_batch_max as in differentiable_rollout (True: the trainer's layout,
+    False: every scene on its own).  The backward runs with parameters=False (d observed alone); the model's mode and
+    its parameters' requires_grad are left as they are, and no random numbers are drawn.  Returns a PGDResult."""
     from .lstm.training import differentiable_rollout
     lib = _lib.load()
-    device = model._device()
-    split = np.zeros(len(xys) + 1, dtype=np.int64)
-    split[1:] = np.cumsum([xy.shape[1] for xy in xys])
-    B, M = len(xys), int(split[-1])
-    if normalize_scene:
-        # the frame is fixed by the clean observation: the attack runs in it, delta is rotated back at the end
-        from .lstm.scene_ops import preprocess_scenes
-        observed, _, _, rotation, center = preprocess_scenes([xy[:obs_length] for xy in xys], device=device,
-                                                             normalize_scene=True, obs_length=obs_length)[:5]
-    else:
-        observed = torch.Tensor(np.concatenate([xy[:obs_length] for xy in xys], axis=1)).to(device)
-    observed = observed.contiguous()
-    layout = model._layouts.get(torch.from_numpy(split), pad_to_batch_max=False, device=device)
+    device = observed.device
+    split = torch.as_tensor(batch_split, dtype=torch.int64).cpu()
+    B = int(split.numel()) - 1
+    layout = model._layouts.get(split, pad_to_batch_max=pad_to_batch_max, device=device)
     f32 = dict(dtype=torch.float32, device=device)
     f64 = dict(dtype=torch.float64, device=device)
-    delta = torch.zeros((obs_length, B, 2), **f32)
-    best_delta = torch.zeros((obs_length, B, 2), **f32)
+    T_obs = int(observed.shape[0])
+    delta = torch.zeros((T_obs, B, 2), **f32)
+    best_delta = torch.zeros((T_obs, B, 2), **f32)
     best_D = torch.full((B,), float('inf'), **f64)
     D = torch.empty((B,), **f64)
     observed_adv = observed.clone()
@@ -67,8 +69,8 @@ def _attack_chunk(model, xys, eps, steps, obs_length, pred_length, normalize_sce
         move = it < steps
         obs_in = observed_adv.clone().requires_grad_(move)
         with torch.enable_grad():
-            _, positions = differentiable_rollout(model, obs_in, torch.from_numpy(split), pred_length,
-                                                  pad_to_batch_max=False)
+            _, positions = differentiable_rollout(model, obs_in, split, pred_length, pad_to_batch_max=pad_to_batch_max,
+                                                  parameters=False)
         positions = positions.contiguous()
         F = int(positions.shape[0])
         dpos = torch.empty_like(positions)
@@ -79,9 +81,29 @@ def _attack_chunk(model, xys, eps, steps, obs_length, pred_length, normalize_sce
         if it == 0:           # iterate 0 also stays the best of a scene whose D is +inf on every iterate
             clean, d_clean, best_pos = positions.detach().clone(), D.clone(), positions.detach().clone()
         with torch.cuda.device(device):
-            _lib.check(lib.tb2_attack_step(layout.handle, _ptr(d_obs), _ptr(observed), obs_length, _ptr(delta), _ptr(D), F,
+            _lib.check(lib.tb2_attack_step(layout.handle, _ptr(d_obs), _ptr(observed), T_obs, _ptr(delta), _ptr(D), F,
                                            _ptr(positions), _ptr(best_D), _ptr(best_delta), _ptr(best_pos),
                                            _ptr(observed_adv), float(eps), float(alpha), int(move), st))
+    attacked = observed.clone()
+    primaries = split[:-1]
+    attacked[:, primaries] = observed[:, primaries] + best_delta
+    return PGDResult(attacked, best_delta, d_clean, best_D, clean, best_pos)
+
+
+def _attack_chunk(model, xys, eps, steps, obs_length, pred_length, normalize_scene):
+    device = model._device()
+    split = np.zeros(len(xys) + 1, dtype=np.int64)
+    split[1:] = np.cumsum([xy.shape[1] for xy in xys])
+    B = len(xys)
+    if normalize_scene:
+        # the frame is fixed by the clean observation: the attack runs in it, delta is rotated back at the end
+        from .lstm.scene_ops import preprocess_scenes
+        observed, _, _, rotation, center = preprocess_scenes([xy[:obs_length] for xy in xys], device=device,
+                                                             normalize_scene=True, obs_length=obs_length)[:5]
+    else:
+        observed = torch.Tensor(np.concatenate([xy[:obs_length] for xy in xys], axis=1)).to(device)
+    res = pgd_collision(model, observed.contiguous(), split, pred_length, eps, steps, pad_to_batch_max=False)
+    best_pos, clean, best_delta = res.positions, res.clean, res.delta
     if normalize_scene:
         from .lstm.scene_ops import inverse_scenes
         out, out_clean = inverse_scenes(best_pos, split, rotation, center), inverse_scenes(clean, split, rotation, center)
@@ -93,8 +115,8 @@ def _attack_chunk(model, xys, eps, steps, obs_length, pred_length, normalize_sce
     def per_scene(arr):
         return [{0: [np.array(arr[-pred_length:, split[i]]), np.array(arr[-pred_length:, split[i] + 1:split[i + 1]])]}
                 for i in range(B)]
-    return (delta_w.transpose(1, 0, 2), per_scene(out), per_scene(out_clean), d_clean.cpu().numpy(),
-            best_D.cpu().numpy())
+    return (delta_w.transpose(1, 0, 2), per_scene(out), per_scene(out_clean), res.d_clean.cpu().numpy(),
+            res.d_best.cpu().numpy())
 
 
 def collision_attack(model, xys, eps=0.1, steps=20, obs_length=9, pred_length=12, normalize_scene=False, chunk=1024):

@@ -410,7 +410,7 @@ __global__ void reduce_partials_kernel(const float* __restrict__ part, int Z, in
     float s = 0.f;
     for (int z = 0; z < Z; ++z) s += part[(size_t)z * N * Kc + idx];
     const size_t n = idx / Kc, k = idx - n * Kc;
-    C[n * ldc + k] += s;
+    if (C) C[n * ldc + k] += s;
     if (C2) C2[n * ldc + k] += s;
 }
 
@@ -479,11 +479,11 @@ __global__ void __launch_bounds__(256) bwd_embed_kernel(const float* __restrict_
         }
         __syncthreads();
     }
-    if (t == 0) {
+    if (t == 0 && dWe) {
         dWe[2 * k] += red[0][0];
         dWe[2 * k + 1] += red[1][0];
-        dbe[k] += red[2][0];
     }
+    if (t == 0 && dbe) dbe[k] += red[2][0];
 }
 
 
@@ -1187,10 +1187,11 @@ static int gemm_nn(const float* A, int lda, const float* B, int ldb, float* C, i
 }
 
 // C[n][k] += sum_r A[r][n] B[r][k]; rows are split over CTAs when the output has few tiles
-// (partials in `scratch`, summed in a fixed order: run-to-run deterministic)
+// (partials in `scratch`, summed in a fixed order: run-to-run deterministic).  C = NULL: a gradient the caller did not
+// ask for (tb2_lstm_grads), nothing runs.
 static int gemm_tn(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int R, int N, int Kc,
                    float* scratch, size_t scratch_floats, cudaStream_t st) {
-    if (R <= 0) return TB2_OK;
+    if (R <= 0 || !C) return TB2_OK;
     // row-major C (N x Kc) += A^T . B  <=>  column-major C^T (Kc x N) += B-view (Kc x R) . (A-view (N x R))^T
     if (cublas_gemm(CUBLAS_OP_N, CUBLAS_OP_T, Kc, N, R, B, ldb, A, lda, 1.f, C, ldc, "bwd_gemm_tn_cublas", st)) return TB2_OK;
     const int vec = (lda % 4 == 0 && ldb % 4 == 0 && aligned16(A) && aligned16(B)) ? 1 : 0;
@@ -1216,9 +1217,10 @@ static int gemm_tn(const float* A, int lda, const float* B, int ldb, float* C, i
     return TB2_OK;
 }
 
+// out (and out2, when set) += the column sums of A; either may be NULL, nothing runs when both are
 static int colsum(const float* A, int lda, int R, int N, float* out, float* out2, float* scratch,
                   size_t scratch_floats, cudaStream_t st) {
-    if (R <= 0) return TB2_OK;
+    if (R <= 0 || (!out && !out2)) return TB2_OK;
     int Z = (R + 63) / 64;
     if (Z > 64) Z = 64;
     while (Z > 1 && (size_t)Z * N > scratch_floats) --Z;
@@ -1421,7 +1423,7 @@ constexpr int kAllPhases = (1 << TB2_PHASE_ENCODER) | (1 << TB2_PHASE_DECODER);
 // LSTM, Hidden2Normal and InputEmbedding weight gradients: one reduction over all S * rows (step, row) records per
 // tensor.  dxin_phases (bit 1 << phase): those cells first compute dX_in = dgates . W_ih of all their steps (the social
 // backward, and the rollout backward's decoder, compute dX_in step by step inside the time loop instead, where the grid
-// MLP's backward or the position chain needs it).
+// MLP's backward or the position chain needs it).  A NULL field of g skips its reduction; dX_in is computed either way.
 static int lstm_weight_grads(const tb2_lstm* m, const tb2_lstm_weights* w, const tb2_lstm_grads* g, const RowRecords& b,
                              int rows, int S, int S_enc, int dxin_phases, cudaStream_t st) {
     const int K = m->K_gate, E = m->E, EP = E + m->P, H = m->H, G4 = 4 * H;
@@ -1451,9 +1453,11 @@ static int lstm_weight_grads(const tb2_lstm* m, const tb2_lstm_weights* w, const
     if ((rc = gemm_tn(b.DN, 8, b.HS, H, g->hidden2normal_weight, H, S * rows, 5, H, b.scratch, b.scratch_floats, st)))
         return rc;
     if ((rc = colsum(b.DN, 8, S * rows, 5, g->hidden2normal_bias, nullptr, b.scratch, b.scratch_floats, st))) return rc;
-    bwd_embed_kernel<<<E - 2, 256, 0, st>>>(b.X, K, b.DXIN, EP, b.VEL, S * rows, g->input_embedding_weight,
-                                            g->input_embedding_bias);
-    TB2_LAUNCH_CHECK();
+    if (g->input_embedding_weight || g->input_embedding_bias) {
+        bwd_embed_kernel<<<E - 2, 256, 0, st>>>(b.X, K, b.DXIN, EP, b.VEL, S * rows, g->input_embedding_weight,
+                                                g->input_embedding_bias);
+        TB2_LAUNCH_CHECK();
+    }
     return TB2_OK;
 }
 
@@ -1591,7 +1595,7 @@ static size_t carve_step_bwd(const tb2_lstm* m, const tb2_layout* l, void* base,
 
 template <int C>
 static int social_pair_kernels(const tb2_lstm* m, const tb2_layout* l, const SocBuffers& b, const float* lat,
-                               int nm1, int d1, cudaStream_t st) {
+                               int nm1, int d1, bool dw1, cudaStream_t st) {
     const bool mma = C == 16 && d1 % 32 == 0 && !m->tc_disabled;
     if (mma && b.Wt1_hi != nullptr && dgrid_mma_smem(d1) <= 200 * 1024) {
         static DynSmemConfig configured;
@@ -1605,6 +1609,7 @@ static int social_pair_kernels(const tb2_lstm* m, const tb2_layout* l, const Soc
             b.sorted, b.start, b.DH1, d1, m->Wt1, nm1, b.DGRID);
     }
     TB2_LAUNCH_CHECK();
+    if (!dw1) return TB2_OK;      // no pool.embedding.0.weight gradient asked for
     if (mma) {
         KernelTimer kt("social_dw1_mma", st);
         social_dw1_mma_kernel<<<dim3(m->cells, (d1 + 255) / 256), 256, 0, st>>>(
@@ -1652,13 +1657,12 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
     const bool two = m->n_mlp == 2;
     const size_t M = (size_t)Mi;
     const int nm1 = l->n_max > 1 ? l->n_max - 1 : 1;
-    TB2_REQUIRE(g->pool_embedding_weight0 && g->pool_embedding_bias0 && g->pool_encoding_weight &&
-                g->pool_encoding_bias && (!two || (g->pool_embedding_weight1 && g->pool_embedding_bias1)),
-                "social backward needs gradient buffers for pool.hidden_dim_encoding and pool.embedding");
+    // a NULL pool field skips its reduction, as in lstm_weight_grads; the d h / d observed chain never reads them
+    const bool dw1 = g->pool_embedding_weight0 != nullptr;
     SocBuffers b;
     carve_social(m, l, (size_t)S, bwd_workspace, &b);
     TB2_CHECK_CUDA(cudaMemsetAsync(b.dc, 0, M * H * sizeof(float), st));
-    TB2_CHECK_CUDA(cudaMemsetAsync(b.dWt1, 0, (size_t)cells * C * d1 * sizeof(float), st));
+    if (dw1) TB2_CHECK_CUDA(cudaMemsetAsync(b.dWt1, 0, (size_t)cells * C * d1 * sizeof(float), st));
     iota_kernel<<<(Mi + 255) / 256, 256, 0, st>>>(b.rows, Mi);
     TB2_LAUNCH_CHECK();
     int rc;
@@ -1793,10 +1797,10 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
         }
         TB2_LAUNCH_CHECK();
         switch (C) {
-            case 4: rc = social_pair_kernels<4>(m, l, b, lat, nm1, d1, st); break;
-            case 8: rc = social_pair_kernels<8>(m, l, b, lat, nm1, d1, st); break;
-            case 16: rc = social_pair_kernels<16>(m, l, b, lat, nm1, d1, st); break;
-            case 32: rc = social_pair_kernels<32>(m, l, b, lat, nm1, d1, st); break;
+            case 4: rc = social_pair_kernels<4>(m, l, b, lat, nm1, d1, dw1, st); break;
+            case 8: rc = social_pair_kernels<8>(m, l, b, lat, nm1, d1, dw1, st); break;
+            case 16: rc = social_pair_kernels<16>(m, l, b, lat, nm1, d1, dw1, st); break;
+            case 32: rc = social_pair_kernels<32>(m, l, b, lat, nm1, d1, dw1, st); break;
             default: set_error("social latent_dim must be 4, 8, 16 or 32"); return TB2_ERR_UNSUPPORTED;
         }
         if (rc) return rc;
@@ -1815,8 +1819,10 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
     }
     // (D) parameter gradients: one reduction over all (step, row) records per tensor
     if ((rc = lstm_weight_grads(m, w, g, b, Mi, S, S_enc, 0, st))) return rc;
-    untranspose_add_kernel<<<2048, 256, 0, st>>>(b.dWt1, g->pool_embedding_weight0, cells, C, d1);
-    TB2_LAUNCH_CHECK();
+    if (dw1) {
+        untranspose_add_kernel<<<2048, 256, 0, st>>>(b.dWt1, g->pool_embedding_weight0, cells, C, d1);
+        TB2_LAUNCH_CHECK();
+    }
     // lat_j = W_enc h_j + b_enc (gridbased_pooling.py:160-167): h of step s-1 is states[s-1]
     for (int s = 1; s < S; ++s) {
         const float* h_prev = states + ((size_t)(s - 1) * 2 + 0) * M * H;

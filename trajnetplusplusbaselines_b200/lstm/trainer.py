@@ -242,12 +242,18 @@ def check_trainable(model):
 class Trainer(object):
     """The reference's Trainer (lstm/trainer.py:28-311) over SceneStore scene sets: same constructor arguments, same
     `loop / train / val / train_batch / val_batch`.  train_batch / val_batch take the reference's arguments and do its
-    computation; they return the losses as device tensors (0-dim), which the loop reads back only where it logs."""
+    computation; they return the losses as device tensors (0-dim), which the loop reads back only where it logs.
+
+    adv_eps > 0 adds adversarial training against the collision attack (attack.pgd_collision): every training batch
+    first attacks its observation, each scene's primary moved inside a per-frame L2 ball of radius adv_eps (metres) by
+    adv_steps PGD iterations, then trains on (1 - adv_wt) * clean loss + adv_wt * attacked loss.  The attack draws no
+    random numbers, so the epoch plan is the one of a clean run.  adv_eps = 0 (the default) is the reference's
+    computation."""
 
     def __init__(self, model=None, criterion=None, optimizer=None, lr_scheduler=None,
                  device=None, batch_size=8, obs_length=9, pred_length=12, augment=True,
                  normalize_scene=False, save_every=1, start_length=0, obs_dropout=False,
-                 augment_noise=False, val_flag=True):
+                 augment_noise=False, val_flag=True, adv_eps=0.0, adv_steps=5, adv_wt=0.5):
         self.model = model if model is not None else LSTM()
         self.criterion = criterion if criterion is not None else PredictionLoss()
         self.optimizer = optimizer if optimizer is not None else \
@@ -274,6 +280,17 @@ class Trainer(object):
         self.obs_dropout = obs_dropout
 
         self.val_flag = val_flag
+        if not adv_eps >= 0:
+            raise ValueError("adv_eps must be >= 0, got %r" % (adv_eps,))
+        if adv_eps > 0:
+            if int(adv_steps) != adv_steps or adv_steps < 1:
+                raise ValueError("adv_steps must be an integer >= 1, got %r" % (adv_steps,))
+            if not 0 < adv_wt <= 1:
+                raise ValueError("adv_wt must be in (0, 1], got %r" % (adv_wt,))
+            from .training import check_rollout
+            check_rollout(self.model)         # NotImplementedError for the models the attack cannot differentiate
+        self.adv_eps, self.adv_steps, self.adv_wt = float(adv_eps), int(adv_steps), float(adv_wt)
+        self._col_counts = None           # [clean, attacked] scenes with D <= 0.2 m this epoch (adv_eps > 0), on the device
         self._start_lengths = None        # the epoch plan's obs_dropout draws, consumed by train_batch
         self._zeros = torch.zeros((0, 2), device=self.device)
 
@@ -324,6 +341,9 @@ class Trainer(object):
         n = len(scenes)
         losses = []
         self._start_lengths = iter(plan.start_lengths) if plan.start_lengths is not None else None
+        adv = self.adv_eps > 0
+        if adv:
+            self._col_counts = torch.zeros(2, dtype=torch.float64, device=self.device)
         try:
             for k, (batch_scene, batch_split) in enumerate(batches):
                 batch_start = time.time()
@@ -340,19 +360,31 @@ class Trainer(object):
                         'lr': self.get_lr(),
                         'loss': round(loss_value, 3),
                     })
+            col = self._col_counts
         finally:
             self._start_lengths = None
+            self._col_counts = None
 
         self.lr_scheduler.step()
         epoch_loss = 0.0
-        for value in (torch.stack(losses).cpu().tolist() if losses else []):
+        values = []
+        if adv:               # the collision counts come back with the losses, in one copy
+            values = torch.cat([torch.stack(losses).double(), col] if losses else [col]).cpu().tolist()
+            values, col = values[:-2], values[-2:]
+        elif losses:
+            values = torch.stack(losses).cpu().tolist()
+        for value in values:
             epoch_loss += value
-        self.log.info({
+        record = {
             'type': 'train-epoch',
             'epoch': epoch + 1,
             'loss': round(epoch_loss / (len(scenes)), 5),
             'time': round(time.time() - start_time, 1),
-        })
+        }
+        if adv:
+            record['col_clean'] = col[0] / len(scenes)
+            record['col_attacked'] = col[1] / len(scenes)
+        self.log.info(record)
 
     def val(self, scenes, goals, epoch):
         """Validation over the SceneStore `scenes` in store order (lstm/trainer.py:165-227)."""
@@ -394,14 +426,29 @@ class Trainer(object):
         prediction_truth = batch_scene[self.obs_length:self.seq_length - 1].clone()
         targets = batch_scene[self.obs_length:self.seq_length] - batch_scene[self.obs_length - 1:self.seq_length - 1]
 
-        rel_outputs, outputs = self.model(observed, batch_scene_goal, batch_split, prediction_truth)
+        def batch_loss(observed):
+            rel_outputs, outputs = self.model(observed, batch_scene_goal, batch_split, prediction_truth)
 
-        # For collision loss calculation
-        primary_prediction = batch_scene[-self.pred_length:].clone()
-        primary_prediction[:, batch_split[:-1]] = outputs[-self.pred_length:, batch_split[:-1]]
+            # For collision loss calculation
+            primary_prediction = batch_scene[-self.pred_length:].clone()
+            primary_prediction[:, batch_split[:-1]] = outputs[-self.pred_length:, batch_split[:-1]]
 
-        ## Loss wrt primary tracks of each scene only
-        loss = self.criterion(rel_outputs[-self.pred_length:], targets, batch_split, primary_prediction) * self.batch_size
+            ## Loss wrt primary tracks of each scene only
+            return self.criterion(rel_outputs[-self.pred_length:], targets, batch_split,
+                                  primary_prediction) * self.batch_size
+
+        if self.adv_eps > 0:
+            from ..attack import COL_LIMIT, pgd_collision
+            res = pgd_collision(self.model, observed, batch_split, self.pred_length, self.adv_eps, self.adv_steps,
+                                pad_to_batch_max=True)
+            if self._col_counts is not None:
+                self._col_counts += torch.stack([(res.d_clean <= COL_LIMIT).sum(), (res.d_best <= COL_LIMIT).sum()])
+            if self.adv_wt < 1:
+                loss = (1 - self.adv_wt) * batch_loss(observed) + self.adv_wt * batch_loss(res.observed)
+            else:             # adv_wt = 1: the clean forward is not run
+                loss = self.adv_wt * batch_loss(res.observed)
+        else:
+            loss = batch_loss(observed)
 
         self.optimizer.zero_grad()
         loss.backward()
@@ -564,6 +611,16 @@ def build_parser(epochs=25):
                                  help='collision loss weight')
     hyperparameters.add_argument('--col_distance', default=0.2, type=float,
                                  help='distance threshold post which collision occurs')
+
+    ## Adversarial training against the collision attack (python -m trajnetplusplusbaselines_b200.attack)
+    adversarial = parser.add_argument_group('adversarial training')
+    adversarial.add_argument('--adv_eps', default=0., type=float,
+                             help='radius (m) of the per-frame L2 ball the primary\'s observation is attacked in; '
+                                  '0 trains without the attack')
+    adversarial.add_argument('--adv_steps', default=5, type=int,
+                             help='PGD iterations of the attack per training batch')
+    adversarial.add_argument('--adv_wt', default=0.5, type=float,
+                             help='weight of the attacked loss, in (0, 1]; the clean loss gets 1 - adv_wt')
     return parser
 
 
@@ -603,6 +660,12 @@ def main(argv=None, epochs=25):
     args = parser.parse_args(argv)
     if args.disable_cuda:
         sys.exit("--disable-cuda: there is no CPU path, training runs on the GPU")
+    if not args.adv_eps >= 0:
+        sys.exit("--adv_eps must be >= 0 (got %g)" % args.adv_eps)
+    if args.adv_steps < 1:
+        sys.exit("--adv_steps must be >= 1 (got %d)" % args.adv_steps)
+    if not 0 < args.adv_wt <= 1:
+        sys.exit("--adv_wt must be in (0, 1] (got %g)" % args.adv_wt)
 
     ## Set seed for reproducibility
     torch.manual_seed(args.seed)
@@ -613,6 +676,9 @@ def main(argv=None, epochs=25):
     try:
         model = build_model(args)
         check_trainable(model)
+        if args.adv_eps > 0:
+            from .training import check_rollout
+            check_rollout(model)
     except (NotImplementedError, RuntimeError, ValueError) as e:
         sys.exit(str(e))
 
@@ -681,7 +747,8 @@ def main(argv=None, epochs=25):
                           criterion=criterion, batch_size=args.batch_size, obs_length=args.obs_length,
                           pred_length=args.pred_length, augment=args.augment, normalize_scene=args.normalize_scene,
                           save_every=args.save_every, start_length=args.start_length, obs_dropout=args.obs_dropout,
-                          augment_noise=args.augment_noise, val_flag=val_flag)
+                          augment_noise=args.augment_noise, val_flag=val_flag, adv_eps=args.adv_eps,
+                          adv_steps=args.adv_steps, adv_wt=args.adv_wt)
         trainer.loop(train_scenes, val_scenes, train_goals, val_goals, args.output, epochs=args.epochs,
                      start_epoch=start_epoch)
     finally:

@@ -74,10 +74,11 @@ def _save_forward(ctx, model, observed, params, forward_out):
 
 
 def _run_backward(ctx, active, d_obs, launch):
-    """One backward call over the rows `active` (int32 on the device): zeroed parameter gradients and d_obs (or None) go
-    into the gradient struct, `launch(lib, handle, weights, grads, workspace, bytes, bwd_workspace, bytes, positions of
-    the steps, cache bytes, device)` issues the call.  Returns autograd's tuple for the forward's arguments (model,
-    observed, three more, *params)."""
+    """One backward call over the rows `active` (int32 on the device): zeroed gradients of the parameters autograd asks
+    for (ctx.needs_input_grad) and d_obs (or None) go into the gradient struct, every other field stays NULL and the call
+    skips its reduction; `launch(lib, handle, weights, grads, workspace, bytes, bwd_workspace, bytes, positions of the
+    steps, cache bytes, device)` issues the call.  Returns autograd's tuple for the forward's arguments (model, observed,
+    three more, *params)."""
     model, layout = ctx.model, ctx.layout
     (positions,) = ctx.saved_tensors
     handle = model._engine()
@@ -85,7 +86,8 @@ def _run_backward(ctx, active, d_obs, launch):
     lib = _lib.load()
     S = ctx.num_steps
     R = int(active.numel())
-    targets = _grad_targets(model)
+    wanted = {id(p) for p, need in zip(ctx.params, ctx.needs_input_grad[5:]) if need}
+    targets = {k: p for k, p in _grad_targets(model).items() if id(p) in wanted}
     grads = {k: torch.zeros_like(p, dtype=torch.float32, device=device).contiguous() for k, p in targets.items()}
     if R > 0:
         g = _lib.LstmGrads()
@@ -109,7 +111,7 @@ def _run_backward(ctx, active, d_obs, launch):
     out = []
     for p in ctx.params:
         gr = by_param.get(id(p))
-        out.append(gr.to(p.dtype) if (gr is not None and p.requires_grad) else None)
+        out.append(gr.to(p.dtype) if gr is not None else None)
     d_in = None
     if d_obs is not None and ctx.needs_input_grad[1]:
         device_in, dtype_in = ctx.observed_meta
@@ -220,7 +222,7 @@ def check_rollout(model):
     _grad_targets(model)              # refuses the non-grid modules
 
 
-def differentiable_rollout(model, observed, batch_split, n_predict, pad_to_batch_max=True):
+def differentiable_rollout(model, observed, batch_split, n_predict, pad_to_batch_max=True, parameters=True):
     """(normals, positions) of the free-running forecast model(observed, None, batch_split, n_predict=n_predict), bit for
     bit, differentiable with nothing detached: unlike LSTM.forward's graph (the reference's, whose decoder inputs are
     detached), the gradient follows every fed-back position into the decoder's velocity inputs, the directional grid's
@@ -228,7 +230,8 @@ def differentiable_rollout(model, observed, batch_split, n_predict, pad_to_batch
     trainable.  pad_to_batch_max=False: every scene as if it were called on its own (LSTMPredictor.predict_batch_xy's
     layout).  Vanilla, occupancy, directional and social models; NotImplementedError (check_rollout) for goal models,
     the non-grid and user-defined interaction modules, S-GAN and VAE, before anything runs.  The backward makes no host
-    synchronisation."""
+    synchronisation.  parameters=False: the parameters are not inputs of the graph, so the backward computes d observed
+    alone (the inputs-only call), even for a model whose parameters are trainable, and leaves every `.grad` alone."""
     check_rollout(model)
-    params = tuple(model.parameters())
+    params = tuple(model.parameters()) if parameters else ()
     return _RolloutFn.apply(model, observed, batch_split, n_predict, pad_to_batch_max, *params)
