@@ -71,7 +71,8 @@ const char* tb2_last_error(void);
  * module, sampling, training-cache and host-output arguments that separate entry points took before.
  * 107: tb2_lstm_rollout_backward, tb2_attack_objective and tb2_attack_step.
  * 108: tb2_lstm_sequence_backward and tb2_lstm_rollout_backward skip the reduction of every NULL tb2_lstm_grads
- *      parameter field (the social backward no longer requires its pool fields). */
+ *      parameter field (the social backward no longer requires its pool fields).
+ * 109: tb2_lstm_relevance_workspace_bytes and tb2_lstm_relevance. */
 int tb2_version(void);
 /* Number of library kernel launches issued by this process so far (bench "gpu_launches"). */
 uint64_t tb2_launch_count(void);
@@ -416,6 +417,29 @@ int tb2_lstm_rollout_backward(const tb2_lstm* model, const tb2_layout* layout, c
                               const tb2_lstm_grads* grads, void* workspace_dev, size_t workspace_bytes,
                               void* bwd_workspace_dev, size_t bwd_workspace_bytes, const void* cache_dev,
                               size_t cache_bytes, void* stream);
+
+/* Layer-wise relevance (LRP) of a free-running forecast: for every scene b and prediction t (0 .. n_decode), how much
+ * the primary's predicted mean velocity at step s_t = obs_length - 2 + t relies on the primary's own velocity input and
+ * on each neighbour, at every step.  The explained scalar is y = |mu| of that step (0 when mu is 0 or not finite, or the
+ * primary is absent there).  Rules, with z' = z + eps sign(z): the eps-rule for hidden2normal (d = mu / |mu| fixed), the
+ * gate operand's g block and the embeddings' Linear layers; signal-take-all for the LSTM cell (the i, f, o gates get
+ * nothing); a grid cell's relevance goes to the neighbour that won it (last writer), a social cell's stops at the
+ * winner's latent.  Only the primaries are explained; y - sum(relevance) is what the biases and eps absorbed.
+ *   observed_dev, positions_dev, states_dev  as for tb2_lstm_rollout_backward: the forward of
+ *                    tb2_lstm_forward_steps over the S = obs_length - 1 + n_decode steps, no teacher forcing
+ *   relevance_out_dev [n_decode + 1, S, M]  the own column at each scene's primary, neighbour columns elsewhere
+ *   explained_out_dev [n_decode + 1, B]     y
+ * Vanilla, occupancy / directional (one_layer, constant 0, pool_to_input, widths <= 1024) and social (one_layer /
+ * two_layer, constant 0, pool_to_input, widths <= 1024) models; TB2_ERR_UNSUPPORTED names any other configuration
+ * (goal models, the non-grid and external modules, other grid embeddings).  Workspace:
+ * tb2_lstm_relevance_workspace_bytes (0 for an unsupported model), 256-byte aligned.  No host synchronisation; the
+ * result is bit-identical from run to run, and with per-scene padding (tb2_layout_set_padding 0) to per-scene calls. */
+size_t tb2_lstm_relevance_workspace_bytes(const tb2_lstm* model, const tb2_layout* layout, int32_t n_predict,
+                                          int32_t obs_length);
+int tb2_lstm_relevance(const tb2_lstm* model, const tb2_layout* layout, const tb2_lstm_weights* weights,
+                       const float* observed_dev, int32_t obs_length, int32_t n_decode, const float* positions_dev,
+                       const float* states_dev, float eps, float* relevance_out_dev, float* explained_out_dev,
+                       void* workspace_dev, size_t workspace_bytes, void* stream);
 
 /* Backward of one tb2_lstm_step_forward step of a TB2_POOL_EXTERNAL model, from the step's inputs: the gate
  * pre-activations are recomputed (one GEMM), then

@@ -309,6 +309,14 @@ int launch_nn_mlp_pool(const tb2_lstm* m, const tb2_layout* l, const float* obs1
 // C = act(A . B + bias), B [K, N] row-major, on the fp32 FFMA kernel (never cuBLAS); act = ReLU when relu != 0
 int launch_gemm_ffma(const float* A, int lda, const float* B, int ldb, float* C, int ldc, int M, int N, int K,
                      const float* bias, int relu, const char* name, cudaStream_t st);
+// The training backward's records on `rows` tracks (train.cu): bwd_gather_kernel's X = [emb | pooled | h_prev], grid rows
+// G (winners: the step's pool_prepare tables, null without a grid), velocity inputs and absence flags; and the gate
+// pre-activations GP [S][rows][4H] of all steps (with bias) on the FFMA kernel, each row's bits independent of `rows`
+int launch_bwd_gather(const tb2_lstm* m, const int* rows, int R, const float* obs1, const float* obs2,
+                      const float* h_prev, const Workspace* winners, const float* pooled_src, int nm1, float* X, float* G,
+                      float* vel, int* masked, cudaStream_t st);
+int launch_gate_preactivations(const tb2_lstm* m, const float* X, float* GP, int rows, int S, int S_enc,
+                               cudaStream_t st);
 bool dense_tc_supported(int K, int N);
 int launch_dense_tc(const void* a_hi, const void* a_lo, const void* w_hi, const void* w_lo, const float* bias,
                     float* Y, void* Y_hi, void* Y_lo, int M, int K, int N, int relu, cudaStream_t st);

@@ -1400,8 +1400,10 @@ static size_t carve_social(const tb2_lstm* m, const tb2_layout* l, size_t S, voi
 // (B) gate pre-activations of all steps: one GEMM per cell (encoder / decoder weights).  wgmma (the social backward,
 // when its row GEMMs run on the tensor cores): the 3-pass wgmma kernel on the bf16 splits of X and [W_ih | W_hh]
 // there; otherwise gemm_nn.
+// row_exact: the FFMA kernel whatever the size (launch_gemm_ffma, never cuBLAS), so every row's bits are independent of
+// how many rows the call has (the relevance pass).
 static int gate_preactivations(const tb2_lstm* m, const RowRecords& b, int rows, int S, int S_enc,
-                               const SocBuffers* wgmma, cudaStream_t st) {
+                               const SocBuffers* wgmma, cudaStream_t st, bool row_exact = false) {
     const int K = m->K_gate, G4 = 4 * m->H;
     for (int phase = 0; phase < 2; ++phase) {
         const int s0 = phase == TB2_PHASE_ENCODER ? 0 : S_enc;
@@ -1412,9 +1414,33 @@ static int gate_preactivations(const tb2_lstm* m, const RowRecords& b, int rows,
         const int rc = wgmma ? launch_dense_tc(wgmma->X_hi + x0, wgmma->X_lo + x0, wgmma->Wcat_hi[phase],
                                                wgmma->Wcat_lo[phase], m->bg[phase], GP, nullptr, nullptr, ns * rows, K,
                                                G4, 0, st)
-                             : gemm_nn(b.X + x0, K, m->WgT[phase], G4, GP, G4, ns * rows, G4, K, m->bg[phase], st);
+                     : row_exact ? launch_gemm_ffma(b.X + x0, K, m->WgT[phase], G4, GP, G4, ns * rows, G4, K, m->bg[phase], 0,
+                                                    "bwd_gemm", st)
+                                 : gemm_nn(b.X + x0, K, m->WgT[phase], G4, GP, G4, ns * rows, G4, K, m->bg[phase], st);
         if (rc) return rc;
     }
+    return TB2_OK;
+}
+
+int launch_gate_preactivations(const tb2_lstm* m, const float* X, float* GP, int rows, int S, int S_enc,
+                               cudaStream_t st) {
+    RowRecords r{};
+    r.X = const_cast<float*>(X);
+    r.GP = GP;
+    return gate_preactivations(m, r, rows, S, S_enc, nullptr, st, true);
+}
+
+int launch_bwd_gather(const tb2_lstm* m, const int* rows, int R, const float* obs1, const float* obs2,
+                      const float* h_prev, const Workspace* winners, const float* pooled_src, int nm1, float* X, float* G,
+                      float* vel, int* masked, cudaStream_t st) {
+    {
+        KernelTimer kt("bwd_gather", st);
+        bwd_gather_kernel<<<R, 256, 0, st>>>(rows, R, (const float2*)obs1, (const float2*)obs2, m->We, m->be, h_prev,
+                                             winners ? winners->win_count : nullptr, winners ? winners->win_ent : nullptr,
+                                             winners ? winners->win_val : nullptr, m->Wt1, m->base1, nm1, m->C, m->cells,
+                                             pooled_src, X, G, vel, masked, m->E, m->P, m->K_gate, m->H);
+    }
+    TB2_LAUNCH_CHECK();
     return TB2_OK;
 }
 
