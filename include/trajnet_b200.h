@@ -72,7 +72,8 @@ const char* tb2_last_error(void);
  * 107: tb2_lstm_rollout_backward, tb2_attack_objective and tb2_attack_step.
  * 108: tb2_lstm_sequence_backward and tb2_lstm_rollout_backward skip the reduction of every NULL tb2_lstm_grads
  *      parameter field (the social backward no longer requires its pool fields).
- * 109: tb2_lstm_relevance_workspace_bytes and tb2_lstm_relevance. */
+ * 109: tb2_lstm_relevance_workspace_bytes and tb2_lstm_relevance.
+ * 110: tb2_shapley_expand and tb2_shapley_values. */
 int tb2_version(void);
 /* Number of library kernel launches issued by this process so far (bench "gpu_launches"). */
 uint64_t tb2_launch_count(void);
@@ -440,6 +441,33 @@ int tb2_lstm_relevance(const tb2_lstm* model, const tb2_layout* layout, const tb
                        const float* observed_dev, int32_t obs_length, int32_t n_decode, const float* positions_dev,
                        const float* states_dev, float eps, float* relevance_out_dev, float* explained_out_dev,
                        void* workspace_dev, size_t workspace_bytes, void* stream);
+
+/* Shapley attribution of the primary's forecast error to its nearest neighbours (lstm/shapley.py), one launch each per
+ * chunk of scenes, no atomics.  A scene b of N_b rows (primary first) has K_b <= 12 players, the K_b nearest neighbours
+ * of the primary at the last observed frame (squared distance in float64 of the float32 positions, a non-finite one
+ * counts as +inf, ties go to the lower row), and 2^K_b instances, one per coalition mask (bit r = the player of rank r):
+ * the scene with the players outside the coalition deleted, the other rows in their original order.  instance_first
+ * [B + 1] gives each scene's first instance (instance_first[b + 1] - instance_first[b] = 2^K_b), instance_split [I + 1]
+ * the instances' rows, as the caller's batch_split of the instance batch (rows of instance i: N_b - K_b + popcount(mask)).
+ * tb2_shapley_expand -- expanded_out [obs_length, out_tracks, 2] = every instance's rows of observed [obs_length,
+ *   num_tracks, 2] (scene_off [B + 1]: the scenes' rows there); player_rows_out [B, 12] = each scene's player rows, by
+ *   rank, relative to the scene's first row (-1 past K_b); coalition_out [I] = each instance's mask.  max_scene >= every
+ *   N_b, at most 6144.
+ * tb2_shapley_values -- from positions [num_frames, num_tracks, 2] (the instance batch's forecast; its last pred_length
+ *   frames are scored) and truth [B, pred_length, 2] (double, the primaries' ground truth): per instance v = (ADE, FDE)
+ *   of its primary, tb2_score_scenes' arithmetic; with frame [B, 4] (cx, cy, cos, sin; NULL: none) the prediction is
+ *   first taken to the world frame as tb2_scenes_inverse does.  phi_{ade,fde}_out [B, 12] (double, NaN past K_b):
+ *   phi_j = sum over S subset of the players without j, in ascending mask order, of |S|! (K - |S| - 1)! / K! (v(S + j) -
+ *   v(S)); v_out [4, B] = v_ADE(all), v_FDE(all), v_ADE(none), v_FDE(none); values_out [I, 2] (optional) = v.
+ *   max_players >= every K_b (it sizes the shared-memory value table). */
+int tb2_shapley_expand(const float* observed_dev, int32_t obs_length, int32_t num_tracks, const int32_t* scene_off_dev,
+                       const int32_t* instance_first_dev, const int32_t* instance_split_dev, int32_t num_scenes,
+                       int32_t num_instances, int32_t max_scene, int32_t out_tracks, float* expanded_out_dev,
+                       int32_t* player_rows_out_dev, int32_t* coalition_out_dev, void* stream);
+int tb2_shapley_values(const float* positions_dev, int32_t num_frames, int32_t num_tracks, int32_t pred_length,
+                       const int32_t* instance_first_dev, const int32_t* instance_split_dev, int32_t num_scenes,
+                       int32_t max_players, const double* truth_dev, const double* frame_dev, double* phi_ade_out_dev,
+                       double* phi_fde_out_dev, double* v_out_dev, double* values_out_dev, void* stream);
 
 /* Backward of one tb2_lstm_step_forward step of a TB2_POOL_EXTERNAL model, from the step's inputs: the gate
  * pre-activations are recomputed (one GEMM), then

@@ -157,6 +157,9 @@ PROTOTYPES = {
     "tb2_lstm_relevance_workspace_bytes": (_sz, [_vp, _vp, _i32, _i32]),
     "tb2_lstm_relevance": (ctypes.c_int, [_vp, _vp, ctypes.POINTER(LstmWeights), _vp, _i32, _i32, _vp, _vp, ctypes.c_float,
                                           _vp, _vp, _vp, _sz, _vp]),
+    "tb2_shapley_expand": (ctypes.c_int, [_vp, _i32, _i32, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
+    "tb2_shapley_values": (ctypes.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp,
+                                          _vp]),
     "tb2_attack_objective": (ctypes.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp]),
     "tb2_attack_step": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp,
                                        ctypes.c_float, ctypes.c_float, _i32, _vp]),

@@ -24,10 +24,11 @@ NVCC_FLAGS = [
 
 
 # classical.cu is compared operation-by-operation with the CPU restatement (oracle/), metrics.cu and attack.cu decide
-# collisions at a distance threshold like numpy does, kalman.cu runs one EM / smoother code on the host (no FMA on baseline x86-64) and
-# on the device with bit-identical results: no FMA contraction
+# collisions at a distance threshold like numpy does, shapley.cu scores forecasts with metrics.cu's arithmetic and sums
+# Shapley values as the float64 restatement does, kalman.cu runs one EM / smoother code on the host (no FMA on baseline
+# x86-64) and on the device with bit-identical results: no FMA contraction
 PER_FILE_FLAGS = {"classical.cu": ["-fmad=false"], "metrics.cu": ["-fmad=false"], "attack.cu": ["-fmad=false"],
-                  "kalman.cu": ["-fmad=false"]}
+                  "kalman.cu": ["-fmad=false"], "shapley.cu": ["-fmad=false"]}
 
 
 def _nvcc():

@@ -73,6 +73,15 @@ __device__ __forceinline__ void mma_bf16_16816(float (&d)[4], const uint32_t (&a
         : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
+// rotate like einsum('ptc,ci->pti', xy, [[ct, st], [-st, ct]]): out0 = x ct + y (-st), out1 = x st + y ct, with
+// explicitly unfused products and sums (scene_ops.cu's arithmetic contract), so every file gets the same bits
+__device__ __forceinline__ double2 rotate_rn(double2 v, double ct, double st) {
+    double2 o;
+    o.x = __dadd_rn(__dmul_rn(v.x, ct), __dmul_rn(v.y, -st));
+    o.y = __dadd_rn(__dmul_rn(v.x, st), __dmul_rn(v.y, ct));
+    return o;
+}
+
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st,
                               Args&&... args) {

@@ -11,6 +11,7 @@
 #include <math.h>
 
 #include "common.cuh"
+#include "metrics.cuh"
 
 namespace tb2 {
 namespace {
@@ -146,19 +147,10 @@ __global__ void __launch_bounds__(32 * kScoreMaxWarps, 1) score_scenes_kernel(in
             continue;
         }
         for (int m = lane; m < K; m += 32) {
-            double sum = NAN, last = NAN;
-            if (m < Ks) {
-                sum = 0.0;
-                for (int t = 0; t < T; ++t) {
-                    const double2 p = modes[(size_t)m * T + t];
-                    const double dx = p.x - gt[t].x, dy = p.y - gt[t].y;
-                    last = sqrt(dx * dx + dy * dy);
-                    sum += last;
-                }
-                sum /= T;
-            }
-            ade[(size_t)s * K + m] = sum;
-            fde[(size_t)s * K + m] = last;
+            double a = NAN, f = NAN;
+            if (m < Ks) ade_fde([&](int t) { return modes[(size_t)m * T + t]; }, gt, T, a, f);
+            ade[(size_t)s * K + m] = a;
+            fde[(size_t)s * K + m] = f;
         }
         const int g0 = gt_off[s], g1 = gt_off[s + 1], p0 = pr_off[s], p1 = pr_off[s + 1];
         bool hit = false;

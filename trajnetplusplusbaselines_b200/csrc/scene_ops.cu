@@ -53,14 +53,6 @@ struct SceneTransformParams {
     int T, M, M_out;
 };
 
-// rotate like einsum('ptc,ci->pti', xy, [[ct, st], [-st, ct]]): out0 = x ct + y (-st), out1 = x st + y ct
-__device__ __forceinline__ double2 rotate_rn(double2 v, double ct, double st) {
-    double2 o;
-    o.x = __dadd_rn(__dmul_rn(v.x, ct), __dmul_rn(v.y, -st));
-    o.y = __dadd_rn(__dmul_rn(v.x, st), __dmul_rn(v.y, ct));
-    return o;
-}
-
 // The same rotation with einsum's accumulation: its sum of products starts from +0.0, so an exact -0.0 (both products
 // -0.0, e.g. the centred primary at the last observation) comes out as +0.0; every other value is rotate_rn's.
 __device__ __forceinline__ double2 einsum_rotate_rn(double2 v, double ct, double st) {
