@@ -73,7 +73,8 @@ const char* tb2_last_error(void);
  * 108: tb2_lstm_sequence_backward and tb2_lstm_rollout_backward skip the reduction of every NULL tb2_lstm_grads
  *      parameter field (the social backward no longer requires its pool fields).
  * 109: tb2_lstm_relevance_workspace_bytes and tb2_lstm_relevance.
- * 110: tb2_shapley_expand and tb2_shapley_values. */
+ * 110: tb2_shapley_expand and tb2_shapley_values.
+ * 111: tb2_shapley_sample_expand and tb2_shapley_sample_values. */
 int tb2_version(void);
 /* Number of library kernel launches issued by this process so far (bench "gpu_launches"). */
 uint64_t tb2_launch_count(void);
@@ -468,6 +469,35 @@ int tb2_shapley_values(const float* positions_dev, int32_t num_frames, int32_t n
                        const int32_t* instance_first_dev, const int32_t* instance_split_dev, int32_t num_scenes,
                        int32_t max_players, const double* truth_dev, const double* frame_dev, double* phi_ade_out_dev,
                        double* phi_fde_out_dev, double* v_out_dev, double* values_out_dev, void* stream);
+
+/* Sampled Shapley values of any number of players (lstm/shapley.py sampled_shapley), one call each per chunk of
+ * scenes, no atomics.  The players of scene b are its K_b nearest neighbours, ranked as for tb2_shapley_expand (K_b <=
+ * N_b - 1 and <= max_players, at most 6143).  permutations [B, pairs, max_players] holds per scene `pairs` permutations
+ * of its ranks 0..K_b - 1 (entries past K_b unread); permutation p of the scene (P = 2 pairs) is row p / 2, reversed
+ * when p is odd.  The scene's instances, each the scene with the players outside a coalition deleted (the other rows
+ * in their original order): 0 = no player, 1 = every player (K_b >= 1), then for p = 0..P-1 and k = 1..K_b-1 the first
+ * k players of permutation p, at 2 + p (K_b - 1) + k - 1: 1 instance for K_b = 0, 2 + P (K_b - 1) otherwise.
+ * instance_first [B + 1] gives each scene's first instance (K_b follows from its count), instance_split [I + 1] the
+ * instances' rows as the caller's batch_split of the instance batch.
+ * tb2_shapley_sample_expand -- player_rows_out [B, max_players] = each scene's player rows by rank (-1 past K_b);
+ *   expanded_out [obs_length, out_tracks, 2] = every instance's rows of observed [obs_length, num_tracks, 2]
+ *   (scene_off [B + 1]: the scenes' rows there).  max_scene >= every N_b, at most 6144.
+ * tb2_shapley_sample_values -- values_out [I, 2] = (ADE, FDE) of each instance's primary as tb2_shapley_values scores
+ *   it (truth, frame alike); then per scene and player j, with m_p(j) = v(first k + 1) - v(first k) of permutation p
+ *   where j is its k-th, a_q = (m_2q(j) + m_2q+1(j)) * 0.5, phi = (sum over ascending q of a_q) / pairs and se =
+ *   sqrt((sum over ascending q of (a_q - phi)^2) / (pairs (pairs - 1))): phi_{ade,fde}_out and se_{ade,fde}_out
+ *   [B, max_players] (double, NaN past K_b); v_out [4, B] = v_ADE(all), v_FDE(all), v_ADE(none), v_FDE(none). */
+int tb2_shapley_sample_expand(const float* observed_dev, int32_t obs_length, int32_t num_tracks,
+                              const int32_t* scene_off_dev, const int32_t* instance_first_dev,
+                              const int32_t* instance_split_dev, const int32_t* permutations_dev, int32_t num_scenes,
+                              int32_t num_instances, int32_t pairs, int32_t max_players, int32_t max_scene,
+                              int32_t out_tracks, float* expanded_out_dev, int32_t* player_rows_out_dev, void* stream);
+int tb2_shapley_sample_values(const float* positions_dev, int32_t num_frames, int32_t num_tracks, int32_t pred_length,
+                              const int32_t* instance_first_dev, const int32_t* instance_split_dev,
+                              const int32_t* permutations_dev, int32_t num_scenes, int32_t num_instances, int32_t pairs,
+                              int32_t max_players, const double* truth_dev, const double* frame_dev,
+                              double* values_out_dev, double* phi_ade_out_dev, double* phi_fde_out_dev,
+                              double* se_ade_out_dev, double* se_fde_out_dev, double* v_out_dev, void* stream);
 
 /* Backward of one tb2_lstm_step_forward step of a TB2_POOL_EXTERNAL model, from the step's inputs: the gate
  * pre-activations are recomputed (one GEMM), then

@@ -160,6 +160,10 @@ PROTOTYPES = {
     "tb2_shapley_expand": (ctypes.c_int, [_vp, _i32, _i32, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp, _vp, _vp]),
     "tb2_shapley_values": (ctypes.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp, _vp,
                                           _vp]),
+    "tb2_shapley_sample_expand": (ctypes.c_int, [_vp, _i32, _i32, _vp, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _i32, _i32,
+                                                 _vp, _vp, _vp]),
+    "tb2_shapley_sample_values": (ctypes.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp,
+                                                 _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
     "tb2_attack_objective": (ctypes.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp]),
     "tb2_attack_step": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp,
                                        ctypes.c_float, ctypes.c_float, _i32, _vp]),

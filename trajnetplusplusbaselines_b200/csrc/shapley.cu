@@ -9,6 +9,11 @@
 // into a shared-memory table of the scene's 2^K values, then sums each player's weighted marginals in ascending
 // coalition order.  One CTA per scene, no atomics: the results are bit-identical from run to run.  Compiled with
 // -fmad=false (build.py), so the values are the evaluator's bits and the sums the float64 restatement's.
+//
+// The sampled estimator (any K): tb2_shapley_sample_expand selects each scene's players once (one CTA per scene), then
+// writes the instances of the permutation prefixes (one CTA per instance); tb2_shapley_sample_values scores every
+// instance into global memory (one thread per instance), then reduces each player's antithetic-pair marginals in
+// ascending pair order (one CTA per scene, no atomics).
 #include <math.h>
 
 #include "common.cuh"
@@ -34,18 +39,11 @@ __device__ __forceinline__ int scene_of(const int32_t* __restrict__ instance_fir
     return lo;
 }
 
-__global__ void __launch_bounds__(kExpandThreads) shapley_expand_kernel(
-        const float2* __restrict__ observed, int obs_length, int num_tracks, const int32_t* __restrict__ scene_off,
-        const int32_t* __restrict__ instance_first, const int32_t* __restrict__ instance_split, int B, int out_tracks,
-        float2* __restrict__ expanded, int32_t* __restrict__ player_rows, int32_t* __restrict__ coalition) {
-    extern __shared__ double s_dist[];                  // [N] squared distance to the primary, +inf where not finite
-    __shared__ int s_player[kMaxPlayers];               // row of the player of each rank
-    const int i = blockIdx.x;
-    const int b = scene_of(instance_first, B, i);
-    const int K = 31 - __clz(instance_first[b + 1] - instance_first[b]);
-    const int mask = i - instance_first[b];
-    const int row0 = scene_off[b], N = scene_off[b + 1] - row0;
-    const float2* last = observed + (size_t)(obs_length - 1) * num_tracks + row0;
+// The scene's K players, by rank, into player[0, K): the K nearest neighbours of the primary at the last observed frame
+// last [N] (primary first), squared distance in float64, +inf where not finite, ties to the lower row.  s_dist [N] is
+// shared scratch; player may be shared or global.  The caller synchronises before reading player.
+__device__ __forceinline__ void select_players(const float2* __restrict__ last, int N, int K, double* s_dist,
+                                               int32_t* player) {
     const float2 p0 = last[0];
     for (int j = 1 + threadIdx.x; j < N; j += blockDim.x) {
         const float2 p = last[j];
@@ -59,24 +57,219 @@ __global__ void __launch_bounds__(kExpandThreads) shapley_expand_kernel(
         const double d = s_dist[j];
         int rank = 0;
         for (int r = 1; r < N && rank < K; ++r) rank += (s_dist[r] < d || (s_dist[r] == d && r < j)) ? 1 : 0;
-        if (rank < K) s_player[rank] = j;
+        if (rank < K) player[rank] = j;
     }
+}
+
+// s_dest [N]: on entry 1 for a kept row and 0 for a deleted one; on return the kept row's position in the instance
+// (its rank among the kept rows), -1 for a deleted one.  s_part [blockDim.x] is scratch.  Then every kept row of the
+// scene's observation goes to its position in the instance at out0.
+__device__ __forceinline__ void copy_kept_rows(const float2* __restrict__ observed, int obs_length, int num_tracks,
+                                               int row0, int N, int* s_dest, int* s_part,
+                                               float2* __restrict__ expanded, int out_tracks, int out0) {
+    const int per = (N + blockDim.x - 1) / blockDim.x;
+    const int j0 = min(N, (int)threadIdx.x * per), j1 = min(N, j0 + per);
+    int kept = 0;
+    for (int j = j0; j < j1; ++j) kept += s_dest[j];
+    s_part[threadIdx.x] = kept;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        int acc = 0;
+        for (int t = 0; t < (int)blockDim.x; ++t) {
+            const int c = s_part[t];
+            s_part[t] = acc;
+            acc += c;
+        }
+    }
+    __syncthreads();
+    int pos = s_part[threadIdx.x];
+    for (int j = j0; j < j1; ++j) s_dest[j] = s_dest[j] ? pos++ : -1;
+    __syncthreads();
+    for (int idx = threadIdx.x; idx < obs_length * N; idx += blockDim.x) {
+        const int t = idx / N, j = idx - t * N;
+        const int d = s_dest[j];
+        if (d >= 0) expanded[(size_t)t * out_tracks + out0 + d] = observed[(size_t)t * num_tracks + row0 + j];
+    }
+}
+
+__global__ void __launch_bounds__(kExpandThreads) shapley_expand_kernel(
+        const float2* __restrict__ observed, int obs_length, int num_tracks, const int32_t* __restrict__ scene_off,
+        const int32_t* __restrict__ instance_first, const int32_t* __restrict__ instance_split, int B, int out_tracks,
+        float2* __restrict__ expanded, int32_t* __restrict__ player_rows, int32_t* __restrict__ coalition) {
+    extern __shared__ double s_dist[];                  // [N] squared distance to the primary, then the rows' positions
+    __shared__ int s_player[kMaxPlayers];               // row of the player of each rank
+    __shared__ int s_part[kExpandThreads];
+    const int i = blockIdx.x;
+    const int b = scene_of(instance_first, B, i);
+    const int K = 31 - __clz(instance_first[b + 1] - instance_first[b]);
+    const int mask = i - instance_first[b];
+    const int row0 = scene_off[b], N = scene_off[b + 1] - row0;
+    select_players(observed + (size_t)(obs_length - 1) * num_tracks + row0, N, K, s_dist, s_player);
     __syncthreads();
     if (mask == 0 && threadIdx.x < kMaxPlayers) player_rows[b * kMaxPlayers + threadIdx.x] = threadIdx.x < K ? s_player[threadIdx.x] : -1;
     if (threadIdx.x == 0) coalition[i] = mask;
-    // row j goes to j - (number of deleted players below j); a deleted player is a rank r < K with bit r of mask clear
-    const int out0 = instance_split[i];
-    for (int idx = threadIdx.x; idx < obs_length * N; idx += blockDim.x) {
-        const int t = idx / N, j = idx - t * N;
-        int shift = 0;
-        bool kept = true;
-        for (int r = 0; r < K; ++r) {
-            if ((mask >> r) & 1) continue;
-            const int pr = s_player[r];
-            shift += pr < j ? 1 : 0;
-            kept = kept && pr != j;
+    // the distances are done with: their storage holds the rows' flags, then positions
+    int* s_dest = reinterpret_cast<int*>(s_dist);
+    for (int j = threadIdx.x; j < N; j += blockDim.x) s_dest[j] = 1;
+    __syncthreads();
+    // a deleted player is a rank r < K with bit r of mask clear
+    if (threadIdx.x < K && !((mask >> threadIdx.x) & 1)) s_dest[s_player[threadIdx.x]] = 0;
+    __syncthreads();
+    copy_kept_rows(observed, obs_length, num_tracks, row0, N, s_dest, s_part, expanded, out_tracks, instance_split[i]);
+}
+
+// Instances of a scene with K players under the sampled estimator: 1 for K = 0, else 2 + P (K - 1)
+__device__ __forceinline__ int sampled_players(int instances, int P) {
+    return instances == 1 ? 0 : (instances - 2) / P + 1;
+}
+
+// Local instance of the first k players of permutation p: 0 the empty coalition, 1 the full one, then P runs of K - 1
+__device__ __forceinline__ int sampled_instance(int p, int k, int K) {
+    return k == 0 ? 0 : k == K ? 1 : 2 + p * (K - 1) + k - 1;
+}
+
+__global__ void __launch_bounds__(kExpandThreads) shapley_sample_players_kernel(
+        const float2* __restrict__ observed, int obs_length, int num_tracks, const int32_t* __restrict__ scene_off,
+        const int32_t* __restrict__ instance_first, int P, int max_players, int32_t* __restrict__ player_rows) {
+    extern __shared__ double s_dist[];                  // [N]
+    const int b = blockIdx.x;
+    const int K = sampled_players(instance_first[b + 1] - instance_first[b], P);
+    const int row0 = scene_off[b], N = scene_off[b + 1] - row0;
+    int32_t* rows = player_rows + (size_t)b * max_players;
+    select_players(observed + (size_t)(obs_length - 1) * num_tracks + row0, N, K, s_dist, rows);
+    for (int r = K + threadIdx.x; r < max_players; r += blockDim.x) rows[r] = -1;
+}
+
+__global__ void __launch_bounds__(kExpandThreads) shapley_sample_expand_kernel(
+        const float2* __restrict__ observed, int obs_length, int num_tracks, const int32_t* __restrict__ scene_off,
+        const int32_t* __restrict__ instance_first, const int32_t* __restrict__ instance_split,
+        const int32_t* __restrict__ perms, int B, int pairs, int max_players, const int32_t* __restrict__ player_rows,
+        int out_tracks, float2* __restrict__ expanded) {
+    extern __shared__ int s_dest[];                     // [N] the rows' flags, then positions
+    __shared__ int s_part[kExpandThreads];
+    const int i = blockIdx.x;
+    const int b = scene_of(instance_first, B, i);
+    const int P = 2 * pairs;
+    const int K = sampled_players(instance_first[b + 1] - instance_first[b], P);
+    const int m = i - instance_first[b];
+    const int row0 = scene_off[b], N = scene_off[b + 1] - row0;
+    const int32_t* prow = player_rows + (size_t)b * max_players;
+    for (int j = threadIdx.x; j < N; j += blockDim.x) s_dest[j] = 1;
+    __syncthreads();
+    if (m == 0) {
+        for (int r = threadIdx.x; r < K; r += blockDim.x) s_dest[prow[r]] = 0;
+    } else if (m >= 2) {
+        // permutation p (pair p / 2's drawn one for even p, reversed for odd p) keeps its first k ranks
+        const int p = (m - 2) / (K - 1), k = m - 2 - p * (K - 1) + 1;
+        const int32_t* pi = perms + ((size_t)b * pairs + (p >> 1)) * max_players;
+        for (int r = k + threadIdx.x; r < K; r += blockDim.x) s_dest[prow[(p & 1) ? pi[K - 1 - r] : pi[r]]] = 0;
+    }
+    __syncthreads();
+    copy_kept_rows(observed, obs_length, num_tracks, row0, N, s_dest, s_part, expanded, out_tracks, instance_split[i]);
+}
+
+// The frame of scene b ([cx, cy, cos, sin] of frame [B, 4]); the identity without one
+struct SceneFrame {
+    double cx = 0.0, cy = 0.0, ct = 1.0, st = 0.0;
+    bool on = false;
+    __device__ __forceinline__ SceneFrame(const double* __restrict__ frame, int b) {
+        if (frame) {
+            cx = frame[b * 4 + 0];
+            cy = frame[b * 4 + 1];
+            ct = frame[b * 4 + 2];
+            st = frame[b * 4 + 3];
+            on = true;
         }
-        if (kept) expanded[(size_t)t * out_tracks + out0 + j - shift] = observed[(size_t)t * num_tracks + row0 + j];
+    }
+};
+
+// (ADE, FDE) of the primary at row of positions against gt [T], in the world frame as tb2_scenes_inverse computes it
+// (inverse_scenes): rotate, then add the centre
+__device__ __forceinline__ void score_primary(const float2* __restrict__ positions, int num_frames, int num_tracks,
+                                              int T, int row, const double2* __restrict__ gt, const SceneFrame& fr,
+                                              double& a, double& f) {
+    const float2* p = positions + (size_t)(num_frames - T) * num_tracks + row;
+    ade_fde([&](int t) {
+        const float2 q = p[(size_t)t * num_tracks];
+        double2 v = make_double2((double)q.x, (double)q.y);
+        if (fr.on) {
+            v = rotate_rn(v, fr.ct, fr.st);
+            v.x = __dadd_rn(v.x, fr.cx);
+            v.y = __dadd_rn(v.y, fr.cy);
+        }
+        return v;
+    }, gt, T, a, f);
+}
+
+__global__ void __launch_bounds__(kValuesThreads) shapley_sample_score_kernel(
+        const float2* __restrict__ positions, int num_frames, int num_tracks, int T,
+        const int32_t* __restrict__ instance_first, const int32_t* __restrict__ instance_split,
+        const double2* __restrict__ truth, const double* __restrict__ frame, int B, int I, double* __restrict__ values) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= I) return;
+    const int b = scene_of(instance_first, B, i);
+    double a, f;
+    score_primary(positions, num_frames, num_tracks, T, instance_split[i], truth + (size_t)b * T, SceneFrame(frame, b),
+                  a, f);
+    values[(size_t)i * 2 + 0] = a;
+    values[(size_t)i * 2 + 1] = f;
+}
+
+// Thread (metric, j) of scene b's CTA: per pair q, a_q = (m + m') * 0.5 with m, m' j's marginals v(first k + 1) -
+// v(first k) in the pair's drawn permutation and in its reverse; phi = (sum over ascending q of a_q) / Q, se =
+// sqrt((sum over ascending q of (a_q - phi)^2) / (Q (Q - 1))).  phi and se are accumulated in place.
+__global__ void __launch_bounds__(kValuesThreads) shapley_sample_reduce_kernel(
+        const double* __restrict__ values, const int32_t* __restrict__ instance_first, const int32_t* __restrict__ perms,
+        int B, int pairs, int max_players, double* __restrict__ phi_ade, double* __restrict__ phi_fde,
+        double* __restrict__ se_ade, double* __restrict__ se_fde, double* __restrict__ v_out) {
+    extern __shared__ int s_inv[];                      // [K] the position of each rank in the pair's permutation
+    const int b = blockIdx.x;
+    const int first = instance_first[b];
+    const int P = 2 * pairs;
+    const int K = sampled_players(instance_first[b + 1] - first, P);
+    const double* v = values + (size_t)first * 2;
+    const double Q = (double)pairs;
+    for (int pass = 0; pass < 2; ++pass) {
+        for (int q = 0; q < pairs; ++q) {
+            const int32_t* pi = perms + ((size_t)b * pairs + q) * max_players;
+            __syncthreads();
+            for (int k = threadIdx.x; k < K; k += blockDim.x) s_inv[pi[k]] = k;
+            __syncthreads();
+            for (int task = threadIdx.x; task < 2 * K; task += blockDim.x) {
+                const int metric = task >= K, j = task - metric * K;
+                const int k = s_inv[j], kr = K - 1 - k;
+                const double m0 = v[sampled_instance(2 * q, k + 1, K) * 2 + metric] -
+                                  v[sampled_instance(2 * q, k, K) * 2 + metric];
+                const double m1 = v[sampled_instance(2 * q + 1, kr + 1, K) * 2 + metric] -
+                                  v[sampled_instance(2 * q + 1, kr, K) * 2 + metric];
+                const double a = (m0 + m1) * 0.5;
+                double* phi = (metric ? phi_fde : phi_ade) + (size_t)b * max_players + j;
+                if (pass == 0) {
+                    *phi = (q ? *phi : 0.0) + a;
+                } else {
+                    double* se = (metric ? se_fde : se_ade) + (size_t)b * max_players + j;
+                    const double d = a - *phi;
+                    *se = (q ? *se : 0.0) + d * d;
+                }
+            }
+        }
+        for (int task = threadIdx.x; task < 2 * K; task += blockDim.x) {
+            const int metric = task >= K, j = task - metric * K;
+            const size_t o = (size_t)b * max_players + j;
+            if (pass == 0) (metric ? phi_fde : phi_ade)[o] /= Q;
+            else (metric ? se_fde : se_ade)[o] = sqrt((metric ? se_fde : se_ade)[o] / (Q * (Q - 1.0)));
+        }
+    }
+    for (int j = K + threadIdx.x; j < max_players; j += blockDim.x) {
+        const size_t o = (size_t)b * max_players + j;
+        phi_ade[o] = phi_fde[o] = se_ade[o] = se_fde[o] = NAN;
+    }
+    if (threadIdx.x == 0) {
+        const int full = K ? 1 : 0;
+        v_out[0 * B + b] = v[full * 2 + 0];
+        v_out[1 * B + b] = v[full * 2 + 1];
+        v_out[2 * B + b] = v[0];
+        v_out[3 * B + b] = v[1];
     }
 }
 
@@ -93,28 +286,10 @@ __global__ void __launch_bounds__(kValuesThreads) shapley_values_kernel(
     double* v_ade = s_v;
     double* v_fde = s_v + n;
     const double2* gt = truth + (size_t)b * T;
-    double cx = 0.0, cy = 0.0, ct = 1.0, st = 0.0;
-    if (frame) {
-        cx = frame[b * 4 + 0];
-        cy = frame[b * 4 + 1];
-        ct = frame[b * 4 + 2];
-        st = frame[b * 4 + 3];
-    }
+    const SceneFrame fr(frame, b);
     for (int m = threadIdx.x; m < n; m += blockDim.x) {
-        const int row = instance_split[first + m];      // the instance's primary
-        const float2* p = positions + (size_t)(num_frames - T) * num_tracks + row;
         double a, f;
-        // the world frame as tb2_scenes_inverse computes it (inverse_scenes): rotate, then add the centre
-        ade_fde([&](int t) {
-            const float2 q = p[(size_t)t * num_tracks];
-            double2 v = make_double2((double)q.x, (double)q.y);
-            if (frame) {
-                v = rotate_rn(v, ct, st);
-                v.x = __dadd_rn(v.x, cx);
-                v.y = __dadd_rn(v.y, cy);
-            }
-            return v;
-        }, gt, T, a, f);
+        score_primary(positions, num_frames, num_tracks, T, instance_split[first + m], gt, fr, a, f);  // its primary
         v_ade[m] = a;
         v_fde[m] = f;
         if (values_out) {
@@ -209,6 +384,80 @@ extern "C" int tb2_shapley_values(const float* positions_dev, int32_t num_frames
             (const float2*)positions_dev, num_frames, num_tracks, pred_length, instance_first_dev, instance_split_dev,
             (const double2*)truth_dev, frame_dev, num_scenes, phi_ade_out_dev, phi_fde_out_dev, v_out_dev,
             values_out_dev);
+    }
+    TB2_LAUNCH_CHECK();
+    return TB2_OK;
+}
+
+extern "C" int tb2_shapley_sample_expand(const float* observed_dev, int32_t obs_length, int32_t num_tracks,
+                                         const int32_t* scene_off_dev, const int32_t* instance_first_dev,
+                                         const int32_t* instance_split_dev, const int32_t* permutations_dev,
+                                         int32_t num_scenes, int32_t num_instances, int32_t pairs, int32_t max_players,
+                                         int32_t max_scene, int32_t out_tracks, float* expanded_out_dev,
+                                         int32_t* player_rows_out_dev, void* stream) {
+    TB2_REQUIRE(num_scenes >= 0 && num_instances >= num_scenes && num_tracks >= 0 && out_tracks >= 0,
+                "negative size, or fewer instances than scenes");
+    TB2_REQUIRE(obs_length >= 1, "obs_length must be >= 1");
+    TB2_REQUIRE(pairs >= 2, "pairs must be >= 2 (at least 4 permutations)");
+    TB2_REQUIRE(max_players >= 1 && max_players < kMaxSceneRows, "max_players must be in 1..6143");
+    if (num_scenes == 0) return TB2_OK;
+    TB2_REQUIRE(max_scene >= 1 && max_scene <= kMaxSceneRows, "max_scene must be in 1..6144");
+    TB2_REQUIRE(observed_dev && scene_off_dev && instance_first_dev && instance_split_dev && permutations_dev &&
+                    expanded_out_dev && player_rows_out_dev,
+                "null argument");
+    TB2_REQUIRE(((uintptr_t)observed_dev & 7) == 0 && ((uintptr_t)expanded_out_dev & 7) == 0,
+                "position arrays must be 8-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    {
+        KernelTimer kt("shapley_sample_players", st);
+        shapley_sample_players_kernel<<<num_scenes, kExpandThreads, (size_t)max_scene * sizeof(double), st>>>(
+            (const float2*)observed_dev, obs_length, num_tracks, scene_off_dev, instance_first_dev, 2 * pairs,
+            max_players, player_rows_out_dev);
+    }
+    TB2_LAUNCH_CHECK();
+    {
+        KernelTimer kt("shapley_sample_expand", st);
+        shapley_sample_expand_kernel<<<num_instances, kExpandThreads, (size_t)max_scene * sizeof(int), st>>>(
+            (const float2*)observed_dev, obs_length, num_tracks, scene_off_dev, instance_first_dev, instance_split_dev,
+            permutations_dev, num_scenes, pairs, max_players, player_rows_out_dev, out_tracks,
+            (float2*)expanded_out_dev);
+    }
+    TB2_LAUNCH_CHECK();
+    return TB2_OK;
+}
+
+extern "C" int tb2_shapley_sample_values(const float* positions_dev, int32_t num_frames, int32_t num_tracks,
+                                         int32_t pred_length, const int32_t* instance_first_dev,
+                                         const int32_t* instance_split_dev, const int32_t* permutations_dev,
+                                         int32_t num_scenes, int32_t num_instances, int32_t pairs, int32_t max_players,
+                                         const double* truth_dev, const double* frame_dev, double* values_out_dev,
+                                         double* phi_ade_out_dev, double* phi_fde_out_dev, double* se_ade_out_dev,
+                                         double* se_fde_out_dev, double* v_out_dev, void* stream) {
+    TB2_REQUIRE(num_scenes >= 0 && num_instances >= num_scenes && num_tracks >= 0,
+                "negative size, or fewer instances than scenes");
+    TB2_REQUIRE(pred_length >= 1 && pred_length <= num_frames, "pred_length must be in 1..num_frames");
+    TB2_REQUIRE(pairs >= 2, "pairs must be >= 2 (at least 4 permutations)");
+    TB2_REQUIRE(max_players >= 1 && max_players < kMaxSceneRows, "max_players must be in 1..6143");
+    if (num_scenes == 0) return TB2_OK;
+    TB2_REQUIRE(positions_dev && instance_first_dev && instance_split_dev && permutations_dev && truth_dev &&
+                    values_out_dev && phi_ade_out_dev && phi_fde_out_dev && se_ade_out_dev && se_fde_out_dev &&
+                    v_out_dev,
+                "null argument");
+    TB2_REQUIRE(((uintptr_t)positions_dev & 7) == 0 && ((uintptr_t)truth_dev & 15) == 0,
+                "positions must be 8-byte and truth 16-byte aligned");
+    cudaStream_t st = (cudaStream_t)stream;
+    {
+        KernelTimer kt("shapley_sample_score", st);
+        shapley_sample_score_kernel<<<(num_instances + kValuesThreads - 1) / kValuesThreads, kValuesThreads, 0, st>>>(
+            (const float2*)positions_dev, num_frames, num_tracks, pred_length, instance_first_dev, instance_split_dev,
+            (const double2*)truth_dev, frame_dev, num_scenes, num_instances, values_out_dev);
+    }
+    TB2_LAUNCH_CHECK();
+    {
+        KernelTimer kt("shapley_sample_reduce", st);
+        shapley_sample_reduce_kernel<<<num_scenes, kValuesThreads, (size_t)max_players * sizeof(int), st>>>(
+            values_out_dev, instance_first_dev, permutations_dev, num_scenes, pairs, max_players, phi_ade_out_dev,
+            phi_fde_out_dev, se_ade_out_dev, se_fde_out_dev, v_out_dev);
     }
     TB2_LAUNCH_CHECK();
     return TB2_OK;

@@ -2,7 +2,7 @@
 from .loss import PredictionLoss, L2Loss
 from .lstm import LSTM, LSTMPredictor, drop_distant
 from .training import differentiable_rollout
-from .shapley import Shapley, shapley, shapley_scenes
+from .shapley import SampledShapley, Shapley, sampled_shapley, sampled_shapley_scenes, shapley, shapley_scenes
 from .gridbased_pooling import GridBasedPooling
 from .non_gridbased_pooling import HiddenStateMLPPooling, NearestNeighborMLP, AttentionMLPPooling, NearestNeighborLSTM, TrajectronPooling
 
