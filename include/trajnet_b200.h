@@ -74,7 +74,8 @@ const char* tb2_last_error(void);
  *      parameter field (the social backward no longer requires its pool fields).
  * 109: tb2_lstm_relevance_workspace_bytes and tb2_lstm_relevance.
  * 110: tb2_shapley_expand and tb2_shapley_values.
- * 111: tb2_shapley_sample_expand and tb2_shapley_sample_values. */
+ * 111: tb2_shapley_sample_expand and tb2_shapley_sample_values.
+ * 112: tb2_lstm_sequence_backward_dh; tb2_snce_num_params, tb2_snce_forward and tb2_snce_backward. */
 int tb2_version(void);
 /* Number of library kernel launches issued by this process so far (bench "gpu_launches"). */
 uint64_t tb2_launch_count(void);
@@ -396,6 +397,22 @@ int tb2_lstm_sequence_backward(const tb2_lstm* model, const tb2_layout* layout, 
                                const tb2_lstm_grads* grads, void* workspace_dev, size_t workspace_bytes,
                                void* bwd_workspace_dev, size_t bwd_workspace_bytes, const void* cache_dev,
                                size_t cache_bytes, void* stream);
+
+/* tb2_lstm_sequence_backward with an upstream gradient on the hidden states (version 112):
+ *   d_hidden_dev     [S, M, H] gradient wrt each step's output h, the states_dev[s][0] the forward kept; NULL is
+ *                    tb2_lstm_sequence_backward itself.  It joins the gradient that reaches h from the later steps and
+ *                    the head before the absent-track branch, so an absent track's d h passes through its carried
+ *                    state like the head's.
+ * Other than social pooling, the backward runs on active_rows only: a row not listed there ignores its d_hidden, so
+ * the caller lists every row with a non-zero d_normals or d_hidden row. */
+int tb2_lstm_sequence_backward_dh(const tb2_lstm* model, const tb2_layout* layout, const tb2_lstm_weights* weights,
+                                  const float* observed_dev, int32_t obs_length, const float* truth_dev,
+                                  int32_t n_decode, const float* positions_dev, const float* states_dev,
+                                  const float* d_normals_dev, const float* d_hidden_dev,
+                                  const int32_t* active_rows_dev, int32_t num_active, const tb2_lstm_grads* grads,
+                                  void* workspace_dev, size_t workspace_bytes, void* bwd_workspace_dev,
+                                  size_t bwd_workspace_bytes, const void* cache_dev, size_t cache_bytes,
+                                  void* stream);
 
 /* Backward of a free-running forward (tb2_lstm_forward_steps with truth = NULL and a training cache for social pooling)
  * on the graph where nothing is detached (version 107): the decoder's fed-back positions carry gradient.  Decoder step
@@ -767,6 +784,36 @@ int tb2_kalman_predict_device(const double* obs_dev, const int64_t* track_offset
                               double* pred_out_dev, double* q_out_dev, double* r_out_dev,
                               double* last_state_out_dev, void* workspace_dev, size_t workspace_bytes,
                               void* stream);
+
+/* -------------------------------------------------------------------------------------
+ * Social-NCE contrastive term (version 112; lstm/contrast.py, DESIGN.md §1 A24).  Per scene b of `layout` (primary
+ * p = its first row), horizon step d = 1 .. horizon and frame f = obs_frame + d, with x0 = scene[obs_frame, p]:
+ *   positive  scene[f, p] - x0 + sigma eps[b, d - 1, 0]
+ *   negatives scene[f, j] - x0 + rho (cos k pi/4, sin k pi/4) + sigma eps[b, d - 1, 1 + 8 (j - p - 1) + k] for every
+ *             j of the scene after p with a finite scene[f, j], k = 0 .. 7
+ * keys = normalize(W2 relu(W1 [x, y, d] + b1) + b2), query = normalize(V2 relu(V1 h_p + c1) + c2) (normalize:
+ * v / max(|v|, 1e-12)) and, for a pair whose positive is finite, term = logsumexp(q . keys / temperature) -
+ * q . key_positive / temperature.
+ *   scene_dev   [num_frames, M, 2];  hidden_dev [M, hidden_dim] (the query is row p)
+ *   params_dev  [tb2_snce_num_params] packed as W1 [D, 3], b1 [D], W2 [E, D], b2 [E], V1 [D, H], c1 [D], V2 [E, D],
+ *               c2 [E] (D = mlp_dim in {16, 32, 64}, E = head_dim in {4, 8, 16}, H = hidden_dim <= 1024)
+ *   eps_dev     [B, horizon, 1 + 8 (max_scene - 1), 2] standard normals
+ * tb2_snce_forward writes terms_out [B, horizon] (0 for a pair that is not finite), valid_out [B, horizon] (1 / 0),
+ * and the per-scene gradients of sum_d term: d_hidden_part_out [B, H] (wrt h_p) and d_params_part_out
+ * [B, num_params].  Samples are streamed, so a scene of any size the layout holds is taken.
+ * tb2_snce_backward: with scale = d_loss[0] / max(count[0], 1) (count: the number of finite pairs, the sum of
+ * valid_out), d_params_out = scale * the partials summed over ascending scenes, and row p of d_hidden_out [M, H] =
+ * scale * d_hidden_part[b] (the other rows are not written).
+ * Neither uses atomics, and a scene's outputs do not depend on the other scenes of the batch (bit for bit). */
+int32_t tb2_snce_num_params(int32_t hidden_dim, int32_t mlp_dim, int32_t head_dim);
+int tb2_snce_forward(const tb2_layout* layout, const float* scene_dev, int32_t num_frames, int32_t obs_frame,
+                     int32_t horizon, const float* hidden_dev, int32_t hidden_dim, const float* params_dev,
+                     int32_t mlp_dim, int32_t head_dim, float temperature, float rho, float sigma, const float* eps_dev,
+                     float* terms_out, float* valid_out, float* d_hidden_part_out, float* d_params_part_out,
+                     void* stream);
+int tb2_snce_backward(const tb2_layout* layout, const float* d_loss_dev, const float* count_dev, int32_t hidden_dim,
+                      int32_t num_params, const float* d_hidden_part_dev, const float* d_params_part_dev,
+                      float* d_hidden_out, float* d_params_out, void* stream);
 
 #ifdef __cplusplus
 }

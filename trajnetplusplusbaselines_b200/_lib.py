@@ -151,6 +151,9 @@ PROTOTYPES = {
     "tb2_lstm_sequence_backward": (ctypes.c_int, [_vp, _vp, ctypes.POINTER(LstmWeights), _vp, _i32, _vp, _i32,
                                                   _vp, _vp, _vp, _vp, _i32, ctypes.POINTER(LstmGrads),
                                                   _vp, _sz, _vp, _sz, _vp, _sz, _vp]),
+    "tb2_lstm_sequence_backward_dh": (ctypes.c_int, [_vp, _vp, ctypes.POINTER(LstmWeights), _vp, _i32, _vp, _i32,
+                                                     _vp, _vp, _vp, _vp, _vp, _i32, ctypes.POINTER(LstmGrads),
+                                                     _vp, _sz, _vp, _sz, _vp, _sz, _vp]),
     "tb2_lstm_rollout_backward": (ctypes.c_int, [_vp, _vp, ctypes.POINTER(LstmWeights), _vp, _i32, _i32, _vp, _vp, _vp,
                                                  _vp, _vp, _i32, ctypes.POINTER(LstmGrads), _vp, _sz, _vp, _sz, _vp, _sz,
                                                  _vp]),
@@ -164,6 +167,10 @@ PROTOTYPES = {
                                                  _vp, _vp, _vp]),
     "tb2_shapley_sample_values": (ctypes.c_int, [_vp, _i32, _i32, _i32, _vp, _vp, _vp, _i32, _i32, _i32, _i32, _vp, _vp,
                                                  _vp, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "tb2_snce_num_params": (_i32, [_i32, _i32, _i32]),
+    "tb2_snce_forward": (ctypes.c_int, [_vp, _vp, _i32, _i32, _i32, _vp, _i32, _vp, _i32, _i32, ctypes.c_float,
+                                        ctypes.c_float, ctypes.c_float, _vp, _vp, _vp, _vp, _vp, _vp]),
+    "tb2_snce_backward": (ctypes.c_int, [_vp, _vp, _vp, _i32, _i32, _vp, _vp, _vp, _vp, _vp]),
     "tb2_attack_objective": (ctypes.c_int, [_vp, _vp, _i32, _i32, _vp, _vp, _vp]),
     "tb2_attack_step": (ctypes.c_int, [_vp, _vp, _vp, _i32, _vp, _vp, _i32, _vp, _vp, _vp, _vp, _vp,
                                        ctypes.c_float, ctypes.c_float, _i32, _vp]),

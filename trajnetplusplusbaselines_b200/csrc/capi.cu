@@ -182,7 +182,7 @@ using namespace tb2;
 extern "C" {
 
 const char* tb2_last_error(void) { return g_error.c_str(); }
-int tb2_version(void) { return 111; }
+int tb2_version(void) { return 112; }
 uint64_t tb2_launch_count(void) { return g_launch_count.load(); }
 
 int tb2_profile_begin(void) {

@@ -119,6 +119,8 @@ __global__ void __launch_bounds__(256) bwd_gather_kernel(
 //        incoming dh = dg_next[r] . Whh_next (recurrent part of the LATER step's gate gradient,
 //        W_hh in torch layout [4H, H]) + pass_prev[r] (what by-passed the cell there); both null
 //        at the last step.  dc [R,H] in place; upstream dnormal [M,5] (row-indexed by track)
+//        dh_ext [M,H] (row-indexed by track, null = none): an upstream gradient wrt this step's output h, added to the
+//        incoming dh before the masked-row branch, so an absent track's passes through its carried state
 //   out: dgates [R,4H], dc (gradient wrt c_prev), hs [R,H] (h of this step), dn_raw [R,8],
 //        pass_cur [R,H] (masked rows: dh goes straight through, lstm.py:158-166)
 template <int H>
@@ -128,7 +130,8 @@ __global__ void __launch_bounds__(4 * H) bwd_cell_head_kernel(
     const float* __restrict__ dh_rec, const float* __restrict__ pass_prev, float* __restrict__ pass_cur,
     float* __restrict__ dc,
     const float* __restrict__ dnormal, const float* __restrict__ Wn, const float* __restrict__ bn,
-    float* __restrict__ dgates, float* __restrict__ hs, float* __restrict__ dn_raw, int R) {
+    float* __restrict__ dgates, float* __restrict__ hs, float* __restrict__ dn_raw, const float* __restrict__ dh_ext,
+    int R) {
     constexpr int kPow2 = H <= 32 ? 32 : H <= 64 ? 64 : H <= 128 ? 128 : 256;     // tree width of the head sums
     __shared__ float red[5][H];
     __shared__ float dn_s[5];
@@ -158,6 +161,7 @@ __global__ void __launch_bounds__(4 * H) bwd_cell_head_kernel(
         dh_in = (part_s[0][u] + part_s[1][u]) + (part_s[2][u] + part_s[3][u]) + pass_prev[(size_t)r * H + u];
     }
     if (quarter != 0) return;       // the cell / head math below is one thread per unit (warps 0 .. H/32 - 1)
+    if (dh_ext) dh_in += dh_ext[(size_t)m * H + u];
     if (masked[r]) {   // absent track: state passes through, no parameter gradient
 #pragma unroll
         for (int g = 0; g < 4; ++g) dg[g * H + u] = 0.f;
@@ -1674,8 +1678,8 @@ static int social_step_records(const tb2_lstm* m, const tb2_layout* l, const Soc
 static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lstm_weights* w,
                            const float* observed, int obs_length, const float* truth, int n_decode,
                            const float* positions, const float* states, const float* d_normals,
-                           const float* d_positions, const tb2_lstm_grads* g, Workspace& ws, void* bwd_workspace,
-                           const TrainCache& cache, cudaStream_t st) {
+                           const float* d_positions, const float* d_hidden, const tb2_lstm_grads* g, Workspace& ws,
+                           void* bwd_workspace, const TrainCache& cache, cudaStream_t st) {
     const int S = obs_length - 1 + n_decode, S_enc = obs_length - 1;
     const int Mi = l->M, K = m->K_gate, E = m->E, P = m->P, EP = E + P, C = m->C, cells = m->cells;
     const int H = m->H, G4 = 4 * H;
@@ -1774,7 +1778,7 @@ static int social_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
                 b.rows, b.masked + (size_t)s * M, b.GP + (size_t)s * M * G4, c_prev, nullptr, Whh_next, dh_rec,
                 b.pass[cur ^ 1], b.pass[cur], b.dc,
                 dnorm + (size_t)s * M * 5, m->Wn, m->bn, DGs, b.HS + (size_t)s * M * H,
-                b.DN + (size_t)s * M * 8, Mi);
+                b.DN + (size_t)s * M * 8, d_hidden ? d_hidden + (size_t)s * M * H : nullptr, Mi);
         }
         if (rc) return rc;
         if (tcg) {
@@ -1877,11 +1881,12 @@ size_t tb2_lstm_backward_workspace_bytes(const tb2_lstm* m, const tb2_layout* l,
                      (size_t)l->M, nullptr, nullptr);
 }
 
-// tb2_lstm_sequence_backward (d_positions = NULL) and tb2_lstm_rollout_backward
+// tb2_lstm_sequence_backward (d_positions = d_hidden = NULL), tb2_lstm_sequence_backward_dh (d_positions = NULL) and
+// tb2_lstm_rollout_backward (d_hidden = NULL)
 static int sequence_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lstm_weights* w, const float* observed,
                              int32_t obs_length, const float* truth, int32_t n_decode, const float* positions,
                              const float* states, const float* d_normals, const float* d_positions,
-                             const int32_t* active_rows, int32_t num_active, const tb2_lstm_grads* g, void* workspace,
+                             const float* d_hidden, const int32_t* active_rows, int32_t num_active, const tb2_lstm_grads* g, void* workspace,
                              size_t workspace_bytes, void* bwd_workspace, size_t bwd_workspace_bytes, const void* cache,
                              size_t cache_bytes, void* stream) {
     TB2_REQUIRE(m && l && w && g, "null handle");
@@ -1917,7 +1922,7 @@ static int sequence_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_l
     carve_workspace(m, l, workspace, &ws);
     if (social)      // every track of a scene receives gradient: all rows, active_rows is ignored
         return social_backward(m, l, w, observed, obs_length, truth, n_decode, positions, states, d_normals, d_positions,
-                               g, ws, bwd_workspace, tc, st);
+                               d_hidden, g, ws, bwd_workspace, tc, st);
     const int R = num_active, K = m->K_gate, E = m->E, P = m->P, EP = E + P, H = m->H, G4 = 4 * H;
     const size_t M = (size_t)l->M;
     BwdBuffers b;
@@ -1968,7 +1973,7 @@ static int sequence_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_l
                 active_rows, b.masked + (size_t)s * R, b.GP + (size_t)s * R * G4, c_prev,
                 last ? nullptr : b.DG + (size_t)(s + 1) * R * G4, Whh_next, nullptr, b.pass[cur ^ 1], b.pass[cur], b.dc,
                 dnorm + (size_t)s * M * 5, m->Wn, m->bn, b.DG + (size_t)s * R * G4,
-                b.HS + (size_t)s * R * H, b.DN + (size_t)s * R * 8, R);
+                b.HS + (size_t)s * R * H, b.DN + (size_t)s * R * 8, d_hidden ? d_hidden + (size_t)s * M * H : nullptr, R);
         }
         if (rc) return rc;
         if (rollout && s >= S_enc) {
@@ -2005,8 +2010,19 @@ int tb2_lstm_sequence_backward(const tb2_lstm* m, const tb2_layout* l, const tb2
                                void* workspace, size_t workspace_bytes, void* bwd_workspace,
                                size_t bwd_workspace_bytes, const void* cache, size_t cache_bytes, void* stream) {
     return sequence_backward(m, l, w, observed, obs_length, truth, n_decode, positions, states, d_normals, nullptr,
-                             active_rows, num_active, g, workspace, workspace_bytes, bwd_workspace, bwd_workspace_bytes,
-                             cache, cache_bytes, stream);
+                             nullptr, active_rows, num_active, g, workspace, workspace_bytes, bwd_workspace,
+                             bwd_workspace_bytes, cache, cache_bytes, stream);
+}
+
+int tb2_lstm_sequence_backward_dh(const tb2_lstm* m, const tb2_layout* l, const tb2_lstm_weights* w,
+                                  const float* observed, int32_t obs_length, const float* truth, int32_t n_decode,
+                                  const float* positions, const float* states, const float* d_normals,
+                                  const float* d_hidden, const int32_t* active_rows, int32_t num_active,
+                                  const tb2_lstm_grads* g, void* workspace, size_t workspace_bytes, void* bwd_workspace,
+                                  size_t bwd_workspace_bytes, const void* cache, size_t cache_bytes, void* stream) {
+    return sequence_backward(m, l, w, observed, obs_length, truth, n_decode, positions, states, d_normals, nullptr,
+                             d_hidden, active_rows, num_active, g, workspace, workspace_bytes, bwd_workspace,
+                             bwd_workspace_bytes, cache, cache_bytes, stream);
 }
 
 int tb2_lstm_rollout_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lstm_weights* w, const float* observed,
@@ -2017,8 +2033,8 @@ int tb2_lstm_rollout_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_
                               void* stream) {
     TB2_REQUIRE(g && g->d_observed && d_positions, "the rollout backward needs d_positions and grads->d_observed");
     return sequence_backward(m, l, w, observed, obs_length, nullptr, n_decode, positions, states, d_normals, d_positions,
-                             active_rows, num_active, g, workspace, workspace_bytes, bwd_workspace, bwd_workspace_bytes,
-                             cache, cache_bytes, stream);
+                             nullptr, active_rows, num_active, g, workspace, workspace_bytes, bwd_workspace,
+                             bwd_workspace_bytes, cache, cache_bytes, stream);
 }
 
 size_t tb2_lstm_step_backward_workspace_bytes(const tb2_lstm* m, const tb2_layout* l) {
@@ -2086,7 +2102,7 @@ int tb2_lstm_step_backward(const tb2_lstm* m, const tb2_layout* l, const tb2_lst
     {
         KernelTimer kt("bwd_cell_head", st);
         rc = launch_cell_head(H, M, st, b.rows, b.masked, b.GP, c_in, nullptr, nullptr, d_h_out, b.pass[1], b.pass[0],
-                              d_c_in, d_normal, m->Wn, m->bn, b.DG, b.HS, b.DN, M);
+                              d_c_in, d_normal, m->Wn, m->bn, b.DG, b.HS, b.DN, nullptr, M);
     }
     if (rc) return rc;
     // (D) + (E) dX_in = dgates . W_ih and the step's weight gradients; d h_in through W_hh

@@ -248,22 +248,54 @@ class Trainer(object):
     first attacks its observation, each scene's primary moved inside a per-frame L2 ball of radius adv_eps (metres) by
     adv_steps PGD iterations, then trains on (1 - adv_wt) * clean loss + adv_wt * attacked loss.  The attack draws no
     random numbers, so the epoch plan is the one of a clean run.  adv_eps = 0 (the default) is the reference's
-    computation."""
+    computation.
+
+    contrast_weight > 0 adds the Social-NCE term (lstm/contrast.py): every training batch trains on
+    criterion * batch_size + contrast_weight * L_nce, the query being each primary's hidden state after the step that
+    consumed the last observed frame.  `contrast` is the SocialNCE module (default: SocialNCE(model.hidden_dim), built
+    after the model); its parameters join the optimizer.  The term draws its noise from torch's generator on the
+    device, so the epoch plan is the one of a clean run; the epoch records gain `loss_nce`, the mean L_nce over the
+    epoch's batches.  contrast_weight = 0 (the default) builds and draws nothing."""
 
     def __init__(self, model=None, criterion=None, optimizer=None, lr_scheduler=None,
                  device=None, batch_size=8, obs_length=9, pred_length=12, augment=True,
                  normalize_scene=False, save_every=1, start_length=0, obs_dropout=False,
-                 augment_noise=False, val_flag=True, adv_eps=0.0, adv_steps=5, adv_wt=0.5):
+                 augment_noise=False, val_flag=True, adv_eps=0.0, adv_steps=5, adv_wt=0.5,
+                 contrast_weight=0.0, contrast=None):
         self.model = model if model is not None else LSTM()
+        if not contrast_weight >= 0:
+            raise ValueError("contrast_weight must be >= 0, got %r" % (contrast_weight,))
+        self.contrast_weight = float(contrast_weight)
+        self.contrast = None
+        if self.contrast_weight > 0:
+            if adv_eps > 0:
+                raise ValueError("Social-NCE (contrast_weight > 0) together with adversarial training (adv_eps > 0) "
+                                 "is not built")
+            from .contrast import SocialNCE, check_contrast
+            check_contrast(self.model)
+            self.contrast = contrast if contrast is not None else SocialNCE(self.model.hidden_dim)
+            if self.contrast.hidden_dim != self.model.hidden_dim:
+                raise ValueError("the SocialNCE module is built for hidden_dim %d, the model has %d"
+                                 % (self.contrast.hidden_dim, self.model.hidden_dim))
+            if not 1 <= self.contrast.horizon <= pred_length:
+                raise ValueError("the Social-NCE horizon must be in [1, pred_length = %d], got %d"
+                                 % (pred_length, self.contrast.horizon))
         self.criterion = criterion if criterion is not None else PredictionLoss()
         self.optimizer = optimizer if optimizer is not None else \
             torch.optim.Adam(self.model.parameters(), lr=1e-3, weight_decay=1e-4)
+        if self.contrast is not None:
+            known = {id(p) for group in self.optimizer.param_groups for p in group['params']}
+            heads = [p for p in self.contrast.parameters() if id(p) not in known]
+            if heads:
+                self.optimizer.add_param_group({'params': heads})
         self.lr_scheduler = lr_scheduler if lr_scheduler is not None else \
             torch.optim.lr_scheduler.StepLR(self.optimizer, 15)
 
         self.device = device if device is not None else torch.device('cuda')
         self.model = self.model.to(self.device)
         self.criterion = self.criterion.to(self.device)
+        if self.contrast is not None:
+            self.contrast = self.contrast.to(self.device)
         self.log = logging.getLogger(self.__class__.__name__)
         self.save_every = save_every
 
@@ -292,6 +324,7 @@ class Trainer(object):
         self.adv_eps, self.adv_steps, self.adv_wt = float(adv_eps), int(adv_steps), float(adv_wt)
         self._col_counts = None           # [clean, attacked] scenes with D <= 0.2 m this epoch (adv_eps > 0), on the device
         self._start_lengths = None        # the epoch plan's obs_dropout draws, consumed by train_batch
+        self._nce_losses = None           # this epoch's L_nce per batch (contrast_weight > 0), on the device
         self._zeros = torch.zeros((0, 2), device=self.device)
 
     def _goals(self, num_tracks):
@@ -300,20 +333,25 @@ class Trainer(object):
             self._zeros = torch.zeros((max(num_tracks, 2 * self._zeros.shape[0]), 2), device=self.device)
         return self._zeros[:num_tracks]
 
+    def _state(self, epoch):
+        """The .state file's dict; the Social-NCE heads (which the .pkl predictor does not hold) under 'contrast'."""
+        state = {'epoch': epoch, 'state_dict': self.model.state_dict(),
+                 'optimizer': self.optimizer.state_dict(),
+                 'scheduler': self.lr_scheduler.state_dict()}
+        if self.contrast is not None:
+            state['contrast'] = self.contrast.state_dict()
+        return state
+
     def loop(self, train_scenes, val_scenes, train_goals, val_goals, out, epochs=35, start_epoch=0):
         for epoch in range(start_epoch, epochs):
             if epoch % self.save_every == 0:
-                state = {'epoch': epoch, 'state_dict': self.model.state_dict(),
-                         'optimizer': self.optimizer.state_dict(),
-                         'scheduler': self.lr_scheduler.state_dict()}
+                state = self._state(epoch)
                 LSTMPredictor(self.model).save(state, out + '.epoch{}'.format(epoch))
             self.train(train_scenes, train_goals, epoch)
             if self.val_flag:
                 self.val(val_scenes, val_goals, epoch)
 
-        state = {'epoch': epoch + 1, 'state_dict': self.model.state_dict(),
-                 'optimizer': self.optimizer.state_dict(),
-                 'scheduler': self.lr_scheduler.state_dict()}
+        state = self._state(epoch + 1)
         LSTMPredictor(self.model).save(state, out + '.epoch{}'.format(epoch + 1))
         LSTMPredictor(self.model).save(state, out)
 
@@ -342,8 +380,11 @@ class Trainer(object):
         losses = []
         self._start_lengths = iter(plan.start_lengths) if plan.start_lengths is not None else None
         adv = self.adv_eps > 0
+        nce = self.contrast is not None
         if adv:
             self._col_counts = torch.zeros(2, dtype=torch.float64, device=self.device)
+        if nce:
+            self._nce_losses = []
         try:
             for k, (batch_scene, batch_split) in enumerate(batches):
                 batch_start = time.time()
@@ -361,16 +402,21 @@ class Trainer(object):
                         'loss': round(loss_value, 3),
                     })
             col = self._col_counts
+            nce_losses = self._nce_losses
         finally:
             self._start_lengths = None
             self._col_counts = None
+            self._nce_losses = None
 
         self.lr_scheduler.step()
         epoch_loss = 0.0
-        values = []
+        values, nce_values = [], []
         if adv:               # the collision counts come back with the losses, in one copy
             values = torch.cat([torch.stack(losses).double(), col] if losses else [col]).cpu().tolist()
             values, col = values[:-2], values[-2:]
+        elif nce:             # the L_nce values come back with the losses, in one copy
+            values = torch.stack(losses + nce_losses).cpu().tolist() if losses else []
+            values, nce_values = values[:len(losses)], values[len(losses):]
         elif losses:
             values = torch.stack(losses).cpu().tolist()
         for value in values:
@@ -384,6 +430,8 @@ class Trainer(object):
         if adv:
             record['col_clean'] = col[0] / len(scenes)
             record['col_attacked'] = col[1] / len(scenes)
+        if nce:
+            record['loss_nce'] = round(sum(nce_values) / max(len(nce_values), 1), 5)
         self.log.info(record)
 
     def val(self, scenes, goals, epoch):
@@ -428,7 +476,9 @@ class Trainer(object):
 
         def batch_loss(observed):
             rel_outputs, outputs = self.model(observed, batch_scene_goal, batch_split, prediction_truth)
+            return task_loss(rel_outputs, outputs)
 
+        def task_loss(rel_outputs, outputs):
             # For collision loss calculation
             primary_prediction = batch_scene[-self.pred_length:].clone()
             primary_prediction[:, batch_split[:-1]] = outputs[-self.pred_length:, batch_split[:-1]]
@@ -447,6 +497,16 @@ class Trainer(object):
                 loss = (1 - self.adv_wt) * batch_loss(observed) + self.adv_wt * batch_loss(res.observed)
             else:             # adv_wt = 1: the clean forward is not run
                 loss = self.adv_wt * batch_loss(res.observed)
+        elif self.contrast is not None:
+            from .training import sequence_with_hidden
+            rel_outputs, outputs, hidden = sequence_with_hidden(self.model, observed, batch_split, prediction_truth,
+                                                                None)
+            # the query: h of the step whose input was the last observed frame (observed starts at start_length)
+            l_nce = self.contrast(batch_scene, hidden[observed.shape[0] - 2], batch_split, self.obs_length,
+                                  layouts=self.model._layouts)
+            loss = task_loss(rel_outputs, outputs) + self.contrast_weight * l_nce
+            if self._nce_losses is not None:
+                self._nce_losses.append(l_nce.detach())
         else:
             loss = batch_loss(observed)
 
@@ -621,6 +681,15 @@ def build_parser(epochs=25):
                              help='PGD iterations of the attack per training batch')
     adversarial.add_argument('--adv_wt', default=0.5, type=float,
                              help='weight of the attacked loss, in (0, 1]; the clean loss gets 1 - adv_wt')
+
+    ## Social-NCE contrastive term (lstm/contrast.py)
+    contrast = parser.add_argument_group('social-nce')
+    contrast.add_argument('--contrast_weight', default=0., type=float,
+                          help='weight of the Social-NCE term added to the training loss; 0 trains without it')
+    contrast.add_argument('--contrast_horizon', default=4, type=int,
+                          help='future steps whose positions make the Social-NCE samples, in [1, pred_length]')
+    contrast.add_argument('--contrast_temperature', default=0.1, type=float,
+                          help='temperature of the Social-NCE softmax, > 0')
     return parser
 
 
@@ -666,6 +735,16 @@ def main(argv=None, epochs=25):
         sys.exit("--adv_steps must be >= 1 (got %d)" % args.adv_steps)
     if not 0 < args.adv_wt <= 1:
         sys.exit("--adv_wt must be in (0, 1] (got %g)" % args.adv_wt)
+    if not args.contrast_weight >= 0:
+        sys.exit("--contrast_weight must be >= 0 (got %g)" % args.contrast_weight)
+    if args.contrast_weight > 0:          # the term's other flags matter only when it is on
+        if not 1 <= args.contrast_horizon <= args.pred_length:
+            sys.exit("--contrast_horizon must be in [1, pred_length = %d] (got %d)"
+                     % (args.pred_length, args.contrast_horizon))
+        if not args.contrast_temperature > 0:
+            sys.exit("--contrast_temperature must be > 0 (got %g)" % args.contrast_temperature)
+        if args.adv_eps > 0:
+            sys.exit("--contrast_weight > 0 together with --adv_eps > 0 is not built")
 
     ## Set seed for reproducibility
     torch.manual_seed(args.seed)
@@ -679,6 +758,12 @@ def main(argv=None, epochs=25):
         if args.adv_eps > 0:
             from .training import check_rollout
             check_rollout(model)
+        contrast = None
+        if args.contrast_weight > 0:      # after the model: its initialisation draws what a run without the term draws
+            from .contrast import SocialNCE, check_contrast
+            check_contrast(model)
+            contrast = SocialNCE(model.hidden_dim, horizon=args.contrast_horizon,
+                                 temperature=args.contrast_temperature)
     except (NotImplementedError, RuntimeError, ValueError) as e:
         sys.exit(str(e))
 
@@ -723,6 +808,9 @@ def main(argv=None, epochs=25):
 
         model = model.to(args.device)
         optimizer = torch.optim.Adam(model.parameters(), lr=args.lr, weight_decay=1e-4)
+        if contrast is not None:          # the heads' group, before the scheduler records each group's lr
+            contrast = contrast.to(args.device)
+            optimizer.add_param_group({'params': list(contrast.parameters())})
         lr_scheduler = None
         if args.step_size is not None:
             lr_scheduler = torch.optim.lr_scheduler.StepLR(optimizer, args.step_size)
@@ -736,7 +824,14 @@ def main(argv=None, epochs=25):
             print("Loading Model Dict")
             with open(args.load_state, 'rb') as f:
                 checkpoint = torch.load(f, map_location=args.device)
+            # a full state's optimizer has one parameter group more with the Social-NCE heads: resume like with like
+            if args.load_full_state and contrast is not None and 'contrast' not in checkpoint:
+                sys.exit("%s holds no Social-NCE heads: it was not trained with --contrast_weight > 0" % args.load_state)
+            if args.load_full_state and contrast is None and 'contrast' in checkpoint:
+                sys.exit("%s holds Social-NCE heads: resume it with --contrast_weight > 0" % args.load_state)
             model.load_state_dict(checkpoint['state_dict'], strict=args.load_state_strict)
+            if args.load_full_state and contrast is not None:
+                contrast.load_state_dict(checkpoint['contrast'])
             if args.load_full_state:
                 print("Loading Optimizer Dict")
                 optimizer.load_state_dict(checkpoint['optimizer'])
@@ -748,7 +843,8 @@ def main(argv=None, epochs=25):
                           pred_length=args.pred_length, augment=args.augment, normalize_scene=args.normalize_scene,
                           save_every=args.save_every, start_length=args.start_length, obs_dropout=args.obs_dropout,
                           augment_noise=args.augment_noise, val_flag=val_flag, adv_eps=args.adv_eps,
-                          adv_steps=args.adv_steps, adv_wt=args.adv_wt)
+                          adv_steps=args.adv_steps, adv_wt=args.adv_wt, contrast_weight=args.contrast_weight,
+                          contrast=contrast)
         trainer.loop(train_scenes, val_scenes, train_goals, val_goals, args.output, epochs=args.epochs,
                      start_epoch=start_epoch)
     finally:

@@ -10,6 +10,9 @@ When `observed` requires grad, the same backward also returns d observed: throug
 velocity inputs, the directional grid's relative velocities and the hidden states social pooling
 reads, plus pred = obs2 + mu of the encoder steps.  The decoder's inputs are detached, as in the
 reference (its deep copy of observed[-1] and prediction_truth, and the fed-back positions).
+
+`sequence_with_hidden` is the same forward with every step's hidden state as a third output, for losses on h (the
+Social-NCE query, lstm/contrast.py): its backward is tb2_lstm_sequence_backward_dh.
 """
 import ctypes
 
@@ -130,28 +133,12 @@ class _SequenceFn(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, d_normals, d_positions):
-        device = ctx.model._engine().device
-        S = ctx.num_steps
-        M = ctx.layout.num_tracks
-        obs_length = int(ctx.obs.shape[0])
-        dn = torch.zeros((S, M, 5), dtype=torch.float32, device=device)
-        if d_normals is not None:
-            dn += torch.nan_to_num(d_normals.to(device=device, dtype=torch.float32))
-        d_obs = None
-        if ctx.needs_input_grad[1]:
-            d_obs = torch.zeros((obs_length, M, 2), dtype=torch.float32, device=device)
-        if d_positions is not None:       # pred = obs2 + mu (lstm.py:232,255)
-            dp_all = torch.nan_to_num(d_positions.to(device=device, dtype=torch.float32))
-            dp = dp_all[-S:]
-            dn[:, :, :2] += dp
-            if d_obs is not None:         # obs2 of the encoder steps is observed[s + 1]; the decoder's are detached
-                if dp_all.shape[0] > S:   # obs_length 2: positions[0] is observed[-1] itself (lstm.py:222-223)
-                    d_obs[-1] += dp_all[0]
-                d_obs[1:obs_length] += dp[:obs_length - 1]
-        dn = dn.contiguous()
+        dn, d_obs = _sequence_upstream(ctx, d_normals, d_positions)
+        obs_length, S = int(ctx.obs.shape[0]), ctx.num_steps
+        device = dn.device
         social = ctx.model.pool is not None and getattr(ctx.model.pool, 'type_', None) == 'social'
         if social:      # the hidden-state scatter couples all tracks of a scene: every row is active
-            active = torch.arange(M, dtype=torch.int32, device=device)
+            active = torch.arange(dn.shape[1], dtype=torch.int32, device=device)
         else:
             active = (dn != 0).any(dim=2).any(dim=0).nonzero().flatten().to(torch.int32).contiguous()
 
@@ -163,12 +150,88 @@ class _SequenceFn(torch.autograd.Function):
         return _run_backward(ctx, active, d_obs, launch)
 
 
+def _sequence_upstream(ctx, d_normals, d_positions):
+    """The teacher-forced sequence's upstream gradients as its backward takes them: dn [S, M, 5] (d positions added to
+    the mu columns, pred = obs2 + mu) and d observed [obs_length, M, 2] (None unless `observed` requires grad)."""
+    device = ctx.model._engine().device
+    S = ctx.num_steps
+    M = ctx.layout.num_tracks
+    obs_length = int(ctx.obs.shape[0])
+    dn = torch.zeros((S, M, 5), dtype=torch.float32, device=device)
+    if d_normals is not None:
+        dn += torch.nan_to_num(d_normals.to(device=device, dtype=torch.float32))
+    d_obs = None
+    if ctx.needs_input_grad[1]:
+        d_obs = torch.zeros((obs_length, M, 2), dtype=torch.float32, device=device)
+    if d_positions is not None:       # pred = obs2 + mu (lstm.py:232,255)
+        dp_all = torch.nan_to_num(d_positions.to(device=device, dtype=torch.float32))
+        dp = dp_all[-S:]
+        dn[:, :, :2] += dp
+        if d_obs is not None:         # obs2 of the encoder steps is observed[s + 1]; the decoder's are detached
+            if dp_all.shape[0] > S:   # obs_length 2: positions[0] is observed[-1] itself (lstm.py:222-223)
+                d_obs[-1] += dp_all[0]
+            d_obs[1:obs_length] += dp[:obs_length - 1]
+    return dn.contiguous(), d_obs
+
+
 def sequence_with_grad(model, observed, batch_split, prediction_truth, n_predict):
     _refuse_goals(model)
     if torch.is_tensor(observed) and observed.requires_grad:
         _grad_targets(model)          # refuses the modules without a backward before anything runs
     params = tuple(model.parameters())
     return _SequenceFn.apply(model, observed, batch_split, prediction_truth, n_predict, *params)
+
+
+class _HiddenSequenceFn(torch.autograd.Function):
+    """_SequenceFn with every step's hidden state as a third output; its gradient enters tb2_lstm_sequence_backward_dh."""
+
+    @staticmethod
+    def forward(ctx, model, observed, batch_split, prediction_truth, n_predict, *params):
+        out = model._forward_nograd(observed, batch_split, prediction_truth, n_predict, want_states=True,
+                                    force_repack=True)
+        normals, positions = _save_forward(ctx, model, observed, params, out)
+        return normals, positions, out[2][:, 0].clone()
+
+    @staticmethod
+    def backward(ctx, d_normals, d_positions, d_hidden):
+        dn, d_obs = _sequence_upstream(ctx, d_normals, d_positions)
+        obs_length, S = int(ctx.obs.shape[0]), ctx.num_steps
+        device = dn.device
+        dh = None
+        if d_hidden is not None:
+            dh = torch.nan_to_num(d_hidden.to(device=device, dtype=torch.float32)).contiguous()
+        social = ctx.model.pool is not None and getattr(ctx.model.pool, 'type_', None) == 'social'
+        if social:      # the hidden-state scatter couples all tracks of a scene: every row is active
+            active = torch.arange(dn.shape[1], dtype=torch.int32, device=device)
+        else:
+            live = (dn != 0).any(dim=2).any(dim=0)
+            if dh is not None:
+                live |= (dh != 0).any(dim=2).any(dim=0)
+            active = live.nonzero().flatten().to(torch.int32).contiguous()
+
+        def launch(lib, handle, w, g, ws, need, bws, bneed, pos_steps, cache_bytes, device):
+            return lib.tb2_lstm_sequence_backward_dh(
+                handle.handle, ctx.layout.handle, ctypes.byref(w), _ptr(ctx.obs), obs_length, _ptr(ctx.truth),
+                S - (obs_length - 1), _ptr(pos_steps), _ptr(ctx.states), _ptr(dn), _ptr(dh), _ptr(active),
+                int(active.numel()), ctypes.byref(g), _ptr(ws), need, _ptr(bws), bneed, _ptr(ctx.cache), cache_bytes,
+                _stream(device))
+        return _run_backward(ctx, active, d_obs, launch)
+
+
+def sequence_with_hidden(model, observed, batch_split, prediction_truth, n_predict):
+    """(rel_outputs, outputs, hidden) of the training forward: the first two are model(observed, goals, batch_split,
+    prediction_truth / n_predict)'s, bit for bit, and hidden [S, M, H] is each step's output h (step s has consumed
+    observed[s + 1]; an absent track carries its state).  A loss on hidden differentiates through the recurrence, and
+    for social pooling through the hidden-state scatter into the neighbours, to every parameter and, when `observed`
+    requires grad, to observed.  Models: those sequence_with_grad trains, external interaction modules excepted."""
+    from .external import is_external
+    _refuse_goals(model)
+    if is_external(model.pool):
+        raise NotImplementedError("sequence_with_hidden of a user-defined interaction module (%s) is not built"
+                                  % type(model.pool).__name__)
+    _grad_targets(model)              # refuses the modules without a backward before anything runs
+    params = tuple(model.parameters())
+    return _HiddenSequenceFn.apply(model, observed, batch_split, prediction_truth, n_predict, *params)
 
 
 class _RolloutFn(torch.autograd.Function):
