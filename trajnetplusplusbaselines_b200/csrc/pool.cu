@@ -1191,7 +1191,8 @@ int launch_pool_mlp(const tb2_lstm* m, const tb2_layout* l, Workspace* ws, float
         gsel = 1;
         smem = l1_smem_bytes(l->group_cap[gsel], m->C, social, m->cells, nm1);
     }
-    TB2_REQUIRE(smem <= 227 * 1024, "scene group does not fit in shared memory (scene too large)");
+    // smem is what the FFMA sparse_layer1 kernel needs and is checked at its launch: pool_rows sizes its rows per CTA
+    // to its own shared memory and sparse_layer1_mma checks its own
     L1Params p;
     p.group_off = l->group_off[gsel];
     p.scene_off = l->scene_off;
@@ -1245,7 +1246,8 @@ int launch_pool_mlp(const tb2_lstm* m, const tb2_layout* l, Workspace* ws, float
         }
         TB2_LAUNCH_CHECK();
         rc = TB2_OK;
-    } else
+    } else {
+    TB2_REQUIRE(smem <= 227 * 1024, "scene group does not fit in shared memory (scene too large)");
     switch (m->cfg.pool_type) {
         case TB2_POOL_OCCUPANCY: rc = launch_l1_t<1, false>(p, l->num_groups[gsel], smem, st); break;
         case TB2_POOL_DIRECTIONAL: rc = launch_l1_t<2, false>(p, l->num_groups[gsel], smem, st); break;
@@ -1257,6 +1259,7 @@ int launch_pool_mlp(const tb2_lstm* m, const tb2_layout* l, Workspace* ws, float
             else { set_error("social latent_dim must be 4, 8, 16 or 32"); return TB2_ERR_UNSUPPORTED; }
             break;
         default: set_error("bad pool type"); return TB2_ERR_INVALID;
+    }
     }
     if (rc != TB2_OK) return rc;
     const float* x = l1_out;
